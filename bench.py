@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py — headline benchmark of the erasure-coding + CRC engine (contract: task brief ④).
+"""bench.py — headline benchmark of the erasure-coding + CRC engine.
 
   python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference]
   (N > 1: launched by torchrun, one rank per GPU; no data-path collective — chunks are independent,
@@ -7,13 +7,16 @@
 
 Workload (BASELINE.json configs[2], the configuration the metric is quoted on): ec(8,2) parity encode +
 CRC32 of every 64 KiB data and parity block over 64 MiB chunks.  The 4096-chunk batch (256 GiB) does not
-fit one B200, so a *step* is one pass of the hot path over one HBM-resident tile of --tile-chunks chunks
+fit one H100 (80 GB), so a *step* is one pass of the hot path over one HBM-resident tile of --tile-chunks chunks
 per GPU (default 512 = 32 GiB in, 8 GiB parity out); 8 steps on 1 GPU == the 4096-chunk batch.
 
 One JSON line on stdout (rank 0).  `value` = chunk-data GiB/s with inputs resident in HBM; `e2e` = the
 same metric through the host-buffer C-ABI call (pinned host memory, H2D + kernel + D2H inside the timed
 region); `roofline` = algorithmic bytes / measured duration against the measured HBM peak;
-`cpu_baseline` = the reference CPU implementation timed on this box's host cores on a bounded sample.
+`cpu_baseline` = the reference CPU implementation timed on this machine's host cores on a bounded sample.
+
+--dump-outputs DIR writes what the timed path returned in its last step (see dump_outputs) for output-for-output comparisons of
+two builds: the inputs are seeded, so the same arguments give the same inputs on every run.
 """
 import argparse
 import json
@@ -52,8 +55,8 @@ class stdout_to_stderr:
 def parse_args():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
-    ap.add_argument("--steps", type=int, default=8)
-    ap.add_argument("--warmup", type=int, default=3)
+    ap.add_argument("--steps", type=int, default=8, help="timed steps of every leg: the headline, each extra[] configuration and the e2e legs")
+    ap.add_argument("--warmup", type=int, default=3, help="untimed steps before each timed loop (at least 3 are run so every shape is warm)")
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--goal", default="ec(8,2)")
     ap.add_argument("--tile-chunks", type=int, default=512)
@@ -64,6 +67,7 @@ def parse_args():
     ap.add_argument("--cpu-chunks", type=int, default=0, help="chunks in the CPU baseline sample (0 = auto)")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-e2e", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="after the timed steps, write the last step's outputs as DIR/<name>.npy")
     return ap.parse_args()
 
 
@@ -459,6 +463,21 @@ class Extras:
         del outs, ocrc, dparts, dcrc
 
 
+DUMP_PARITY_SAMPLES = 1 << 22
+
+
+def dump_outputs(torch, out_dir, d_par, d_crc):
+    """The encode's outputs after the last timed step: every block CRC of the tile (crc.npy, float64 holds a uint32 exactly) and a
+    fixed, seeded sample of DUMP_PARITY_SAMPLES parity bytes (parity_sample.npy, float32; all parity would be 8 GiB) at the
+    positions parity_sample_index.npy (float64): 55 MB in all at the default tile."""
+    os.makedirs(out_dir, exist_ok=True)
+    idx = np.sort(np.random.default_rng(2024).integers(0, d_par.numel(), size=DUMP_PARITY_SAMPLES))
+    sample = d_par[torch.from_numpy(idx).to(d_par.device)].cpu().numpy()
+    np.save(os.path.join(out_dir, "parity_sample.npy"), sample.astype(np.float32))
+    np.save(os.path.join(out_dir, "parity_sample_index.npy"), idx.astype(np.float64))
+    np.save(os.path.join(out_dir, "crc.npy"), d_crc.cpu().numpy().view(np.uint32).astype(np.float64))
+
+
 def copy_roofline(torch, dev, in_bytes, out_bytes, dist, reps=3):
     """e2e ceiling of this host/GPU pair: pinned H2D of `in_bytes` and D2H of `out_bytes` issued together on two streams (what the
     3-slot pipeline overlaps), all ranks at once.  Returns seconds (max over ranks) for one such exchange."""
@@ -675,18 +694,20 @@ def main():
             assert (d_crc[c * crc_stride: (c + 1) * crc_stride].cpu().numpy().view(np.uint32) == c_ref).all(), f"headline CRCs differ from the reference (chunk {c})"
             headline_checked += 1
     crc_host = d_crc[:crc_stride].cpu().numpy().view(np.uint32)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(torch, args.dump_outputs, d_par, d_crc)
 
     peaks_path = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(peaks_path):
         peak, peak_src = float(json.load(open(peaks_path))["hbm_gbs"]), "MEASURED_PEAKS.json hbm_gbs (of measured)"
     else:
-        peak, peak_src = 6650.0, "B200_PROFILING.md fallback 6.65 TB/s (of fallback)"
+        peak, peak_src = 3350.0, "H100 SXM data-sheet HBM3 bandwidth 3.35 TB/s (not measured)"
 
     # ---- the other BASELINE configurations, same run, same buffers
     extra, extra_launches = [], 0
     if not args.no_extra and not probing:
         del d_par, d_crc
-        ex = Extras(torch, L, eng, dev, stream, d_data, T * CHUNK, peak, world, dist, rank, steps=5, warmup=3)
+        ex = Extras(torch, L, eng, dev, stream, d_data, T * CHUNK, peak, world, dist, rank, steps=args.steps, warmup=3)
         ex.encode("ec(3,2)", CHUNK, "BASELINE.json configs[1]: ec(3,2) encode + CRC, 64 MiB chunks", max_chunks=512)
         ex.recover("ec(8,2)", (1, 4), "BASELINE.json configs[3]: ec(8,2) degraded read, data parts 1 and 4 lost", n=128)
         ex.convert("ec(8,2)", (1, 4), "ec(3,2)", "SURVEY.md 8(f1): slice conversion for replication, ec(8,2) with data parts 1 and 4 lost -> ec(3,2)", n=64)
@@ -700,6 +721,10 @@ def main():
         except Exception as exc:  # noqa: BLE001
             ex.out.append({"name": "recover ec(5,3) parts [0, 1, 4] lost (verify + rebuild + image)", "error": f"{type(exc).__name__}: {exc}"[:300]})
         extra, extra_launches = ex.out, ex.launches
+        del ex
+        # the extras' freed buffers stay in torch's cache; the host-buffer calls below allocate their device staging through
+        # cudaMalloc, which on an 80 GB device fails unless that memory is returned
+        torch.cuda.empty_cache()
 
     # ---- end-to-end through the host-buffer C-ABI call (pinned memory, copies inside the timed region)
     e2e = None
@@ -755,13 +780,13 @@ def main():
                 rc = lib.lzgpu_encode_chunks(eng.h, C.byref(goal.c), Ep, CHUNK, pg_in.ctypes.data_as(C.c_void_p), CHUNK,
                                              pg_par.ctypes.data_as(C.c_void_p), par_stride, pg_crc.ctypes.data_as(C.c_void_p), crc_stride)
                 assert rc == 0, L._lib.last_error()
-            dtp = timed(pg_step, 2)
-            e2e["pageable_value"] = world * Ep * 2 * CHUNK / GIB / dtp
+            dtp = timed(pg_step, args.steps)
+            e2e["pageable_value"] = world * Ep * args.steps * CHUNK / GIB / dtp
             rc = lib.lzgpu_host_register(eng.h, pg_in.ctypes.data_as(C.c_void_p), pg_in.nbytes)
             rc |= lib.lzgpu_host_register(eng.h, pg_par.ctypes.data_as(C.c_void_p), pg_par.nbytes)
             if rc == 0:
-                dtr = timed(pg_step, 2)
-                e2e["registered_value"] = world * Ep * 2 * CHUNK / GIB / dtr
+                dtr = timed(pg_step, args.steps)
+                e2e["registered_value"] = world * Ep * args.steps * CHUNK / GIB / dtr
                 lib.lzgpu_host_unregister(eng.h, pg_in.ctypes.data_as(C.c_void_p))
                 lib.lzgpu_host_unregister(eng.h, pg_par.ctypes.data_as(C.c_void_p))
             e2e["pageable_note"] = f"{Ep} chunks per call from plain (pageable) numpy buffers, then the same buffers after lzgpu_host_register"
@@ -799,13 +824,13 @@ def main():
             rc = lib.lzgpu_recover_chunks(eng.h, C.byref(g82.c), Er, nb, a_parts, ps, a_crc, want.ctypes.data_as(C.c_void_p), a_out,
                                           img_h.data_ptr(), CHUNK, bad)
             assert rc == 0, L._lib.last_error()
-        dtr = timed(rec_step, max(2, args.steps // 2))
+        dtr = timed(rec_step, args.steps)
         for i in lost:
             assert torch.equal(out_h[i], dparts[i].cpu()), "e2e recover: rebuilt part differs"
         assert torch.equal(img_h, d_data[: Er * CHUNK].cpu()), "e2e recover: chunk image differs"
         rec_in, rec_out = Er * k * (ps + 4 * pb), Er * (len(lost) * ps + CHUNK)
         t_copy_r = copy_roofline(torch, dev, rec_in, rec_out, dist)
-        rec_value = world * Er * max(2, args.steps // 2) * CHUNK / GIB / dtr
+        rec_value = world * Er * args.steps * CHUNK / GIB / dtr
         rec_peak = world * Er * CHUNK / GIB / t_copy_r
         e2e["recover"] = {"value": rec_value, "unit": "GiB/s of chunk data", "config": f"{g82} degraded read, parts {list(lost)} lost, stored CRCs verified, "
                           f"rebuilt parts + chunk image returned; {Er} chunks per call", "h2d_bytes_per_step": rec_in, "d2h_bytes_per_step": rec_out,
@@ -824,15 +849,7 @@ def main():
     alg = algorithmic_bytes_per_chunk(k, m) * T
     kernel_ms = float(np.mean(step_ms))
     achieved = alg / (kernel_ms / 1e3) / 1e9
-    traffic, traffic_src = None, None
-    tp = os.path.join(ROOT, "profiles", "roofline_traffic.json")
-    if os.path.exists(tp):
-        try:
-            tj = json.load(open(tp))
-            traffic = tj.get("dram_bytes_per_chunk") * T if tj.get("dram_bytes_per_chunk") else None
-            traffic_src = "per-chunk DRAM bytes of the committed ncu --set full capture (profiles/roofline_traffic.json) x chunks per launch; NOT measured in this run"
-        except Exception:
-            traffic = None
+    traffic, traffic_src = None, "DRAM traffic not measured (no hardware counters in this run)"
     roofline = {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak, "traffic": traffic,
                 "traffic_source": traffic_src, "peak_source": peak_src, "algorithmic_bytes_per_launch": alg,
                 "kernel": "fused encode+CRC step" if launches_per_step <= 1.01 else f"{launches_per_step:.0f} kernels per step (generic route); duration = whole step",
@@ -858,7 +875,7 @@ def main():
         "dtype": "u8", "data": "synthetic",
         "config": {"workload": f"{goal} encode + per-64KiB-block CRC32, 64 MiB chunks (BASELINE.json configs[2])",
                    "chunks_per_step_per_gpu": T, "resident_bytes_per_gpu": T * (CHUNK + par_stride + 4 * crc_stride),
-                   "l2_policy": "inputs (32 GiB/step) far larger than the 126 MB L2; no flush needed",
+                   "l2_policy": "inputs (32 GiB/step) far larger than the 50 MB L2; no flush needed",
                    "parallelism": f"static round-robin of chunk tiles over {world} GPU(s), no collective",
                    "parity_check": f"{headline_checked} chunks of the timed tile (rank 0) bit-exact vs {checker_name}: parity parts and every block CRC"},
         "e2e": e2e, "gpu_launches": int(launches), "clocks": clocks, "roofline": roofline, "cpu_baseline": cpu_baseline,

@@ -1,9 +1,9 @@
 /*
- * lzgpu.h — C ABI of the B200-native erasure-coding + checksum engine (liblzgpu.so).
+ * lzgpu.h — C ABI of the H100-native erasure-coding + checksum engine (liblzgpu.so).
  *
  * This is the drop-in boundary for ONE hot path of lizardfs/lizardfs: xorN / ec(k,m) parity
  * encode, degraded-read recover and per-64 KiB-block CRC32 (SURVEY.md §8).  Plain pointers and
- * sizes only; no CUDA or torch types.  All arithmetic runs in hand-written sm_100a CUDA kernels;
+ * sizes only; no CUDA or torch types.  All arithmetic runs in hand-written sm_90a CUDA kernels;
  * there is NO CPU fallback: if no CUDA device / kernel image is usable every call fails loudly
  * (status < 0, or abort() with a message for the void reference signatures).
  *

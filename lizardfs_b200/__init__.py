@@ -1,9 +1,9 @@
-"""lizardfs_b200 — B200-native erasure-coding + CRC32 engine behind LizardFS's
+"""lizardfs_b200 — H100-native erasure-coding + CRC32 engine behind LizardFS's
 Goal / slice_traits / ReedSolomon / blockXor / mycrc32 interfaces.
 
 The package is a thin host-side mirror (ctypes) over liblzgpu.so, the C-ABI library whose
-kernels are hand-written CUDA for sm_100a.  No CPU fallback exists: importing the package
-without the built library, or creating an Engine without a B200, fails loudly.
+kernels are hand-written CUDA for sm_90a.  No CPU fallback exists: importing the package
+without the built library, or creating an Engine without an H100 (sm_90), fails loudly.
 """
 from . import _lib  # noqa: F401
 from ._lib import BLOCK_SIZE, BLOCKS_IN_CHUNK, CHUNK_SIZE  # noqa: F401

@@ -6,7 +6,7 @@
 // reference that does not define LIZARDFS_HAVE_ISA_L_ERASURE_CODE_H therefore references the mangled names
 // (_Z16gf_gen_rs_matrixPhii, _Z14ec_encode_dataiiiPhPS_S0_, ...).  This translation unit defines those, forwarding to the C
 // symbols through their lzgpu_isal_* aliases — it must not see the extern "C" declarations of the same names, which is why it
-// is a file of its own and does not include lzgpu.h.  Tested by tests/cpp test_link_substitution_cxx (the reference's
+// is a file of its own and does not include lzgpu.h.  Tested by oracle/_ref/test_link_substitution_cxx (the reference's
 // reed_solomon_unittest.cc compiled against galois_field.h).
 #include <cstdint>
 

@@ -29,7 +29,6 @@
 //     CRC    one row per thread: R*4 data rows (verified against the stored CRC when the row was read from a part, emitted as the
 //            destination data part's CRC either way), E*T*4 source parity rows (verified only), G*(M-1)*4 staged destination
 //            parity rows; the CRC of destination parity row 0 comes from linearity as in the encoder.
-// Measured history of this structure: profiles/probe_r2.md section 12.
 #pragma once
 #include "fused_kernel.cuh"
 
@@ -38,8 +37,8 @@ namespace lzd {
 // kConvertThreads (256) and kConvertNPST (4 staging stages) live in fused_plan.h next to convert_plan()
 
 // mbar_wait for warps that mostly find the phase incomplete (the rebuild warps run ahead of the TMA loads): sleep between the polls so
-// that the loop does not take issue slots from the worker warps of the same scheduler (ncu, run 12: the polling loops were 22 % of all
-// executed instructions)
+// that the loop does not take issue slots from the worker warps of the same scheduler (without the sleep the polling loops were a
+// large share of all executed instructions)
 __device__ __forceinline__ void mbar_wait_relaxed(uint32_t addr, uint32_t parity) {
 	uint32_t done;
 	for (;;) {
@@ -111,7 +110,7 @@ fused_convert_kernel(const __grid_constant__ TmapArray tmaps, const __grid_const
 	// Warp roles.  WORKER warps (the first n_wk) own the CRC streams and the GF items; with lost parts the remaining warps are
 	// REBUILD warps and do nothing else: they run ahead of the workers by as many stages as are loaded, so the workers find the
 	// lost rows in place (`rfull`) when a stage's turn comes.  (Measured, runs 9 / 10: with the rebuild in front of — or inside — warps
-	// that also carry GF items every step waited for it, profiles/probe_r2.md section 11.)
+	// that also carry GF items every step waited for it.)
 	const uint32_t n_rows = DROWS + SPROWS + PROWS;
 	const uint32_t n_wk = E ? (n_rows + 31) / 32 : NT / 32;        // the host guarantees n_wk < NT / 32 when E > 0
 	const uint32_t n_wk_threads = n_wk * 32;

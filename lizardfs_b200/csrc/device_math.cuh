@@ -35,7 +35,7 @@ __device__ __forceinline__ uint32_t gf_x2(uint32_t v) {
 	return ((v ^ hi) << 1) ^ __umulhi(hi, 0x3A000000u);
 #else
 	// diagnostics: (v - hi) * 2 = v*2 + hi*(-2), the byte-lane shift as two IMADs too.  Measured slower where gf_x2 is used
-	// (rows 2, 3): ec(8,4) 0.386 -> 0.355 of peak — the IMAD count then matches the LOP3 count and the FMA pipe binds.
+	// (rows 2, 3 of ec(8,4)) — the IMAD count then matches the LOP3 count and the FMA pipe binds.
 	uint32_t dbl;
 	asm("{\n\t.reg .u32 t;\n\tmul.lo.u32 t, %1, 2;\n\tmad.lo.u32 %0, %2, 0xFFFFFFFE, t;\n\t}" : "=r"(dbl) : "r"(v), "r"(hi));
 	return dbl ^ __umulhi(hi, 0x3A000000u);
@@ -64,8 +64,7 @@ __device__ __forceinline__ uint32_t gf_x2_add(uint32_t v, uint32_t d) {
 #ifndef LZ_CHAINED_DOUBLINGS
 #ifndef LZ_X4_FUSED
 // x4 as two chained doublings: 4 ALU + 6 FMA-pipe ops per word instead of the 5 + 4 of the one-step form below — one ALU op less
-// where the ALU pipe binds and the FMA pipe idles (round 2, same box: ec(5,3) 0.765 -> 0.792, ec(6,3) 0.762 -> 0.793 of the HBM
-// peak; ec(8,4) unchanged).  -DLZ_X4_FUSED selects the one-step form.
+// where the ALU pipe binds and the FMA pipe idles (measured faster for ec(5,3) and ec(6,3), ec(8,4) unchanged).  -DLZ_X4_FUSED selects the one-step form.
 __device__ __forceinline__ uint32_t gf_x4_add(uint32_t v, uint32_t d) { return gf_x2_add(gf_x2_add(v, 0u), d); }
 #else
 __device__ __forceinline__ uint32_t gf_x4_add(uint32_t v, uint32_t d) {

@@ -145,8 +145,8 @@ extern "C" int lzgpu_ctx_create(int device, lzgpu_ctx **out) {
 	DeviceGuard g(device);
 	cudaDeviceProp prop;
 	CUDA_TRY(cudaGetDeviceProperties(&prop, device));
-	if (prop.major != 10) {
-		lz_set_error("device %d is sm_%d%d; this library only carries sm_100a code", device, prop.major, prop.minor);
+	if (prop.major != 9 || prop.minor != 0) {
+		lz_set_error("device %d is sm_%d%d; this library only carries sm_90a code", device, prop.major, prop.minor);
 		return LZGPU_ERR_NO_DEVICE;
 	}
 	auto *ctx = new lzgpu_ctx();

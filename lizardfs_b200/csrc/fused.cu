@@ -54,7 +54,7 @@ struct FusedState {
 	int bs_max_stages = LZ_BS_MAX_STAGES;  // LZGPU_BS_STAGES: deepest data stage ring of the bit-sliced kernels
 	int bs_smem_cap = 200 * 1024;          // LZGPU_BS_SMEM_KB: their shared memory budget (one CTA per SM)
 	int bitslice = LZ_BITSLICE_DEFAULT;  // LZGPU_BITSLICE: Vandermonde parity rows on bit planes (W = 8 items, bitslice.cuh) — bit 0: four rows, bit 1: three rows with k >= 7, bit 2: three rows with any k; 0 = packed-byte Horner
-	int promo = 3;  // CU_TENSOR_MAP_L2_PROMOTION_L2_256B: +12% streaming bandwidth over 128B/none (profiles/probe_r1.md)
+	int promo = 3;  // CU_TENSOR_MAP_L2_PROMOTION_L2_256B: measured faster streaming than 128B/none
 };
 
 // x^n mod P for a possibly negative n (x has multiplicative order dividing 2^32 - 1)
@@ -325,7 +325,7 @@ static int set_all_bs_attrs() {
 
 // Fold window per shape: the 128-word window (3 LOP3 per word, one CTA per SM) pays off where the kernel is ALU bound
 // (many parity rows); the 64-word window (two CTAs per SM) is the default.  LZGPU_FOLD=64|128 forces one.
-// (measured in round 1, profiles/probe_r1.md: the 128-word window is slower for every goal — the kernels are bound by
+// (measured: the 128-word window is slower for every goal — the kernels are bound by
 // per-warp latency, not ALU throughput, and halving the resident warps costs more than the saved LOP3s — so it is only
 // compiled with -DLZ_ENABLE_FOLD128 for experiments)
 static int choose_fold(const FusedState *fs, int M, bool generic) {
@@ -480,8 +480,7 @@ static int fused_run(lzgpu_ctx *ctx, int M, bool generic, const uint8_t *coef_ro
 	LZ_FOLDED(3, 5, 8)    // ec(5,3)
 	LZ_FOLDED(3, 6, 8)    // ec(6,3)
 	LZ_FOLDED(4, 8, 8)    // ec(8,4) on one 16-warp CTA per SM
-	// more goals folded in round 2 (run 21: the runtime-k instantiation costs 25-40 %: ec(8,3) 0.455 -> 0.570, ec(6,4) 0.370 -> 0.495,
-	// ec(4,4) 0.388 -> 0.548 of the HBM peak)
+	// more goals folded (the runtime-k instantiation measured markedly slower for ec(8,3), ec(6,4), ec(4,4))
 	LZ_FOLDED(3, 8, 6)    // ec(8,3)
 	LZ_FOLDED(1, 4, 16)   // xor4 / ec(4,1)
 	LZ_FOLDED(2, 5, 10)   // ec(5,2)
@@ -670,26 +669,21 @@ int lz_fused_recover(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, 
 			p.erased_idx[e++] = static_cast<uint8_t>(j);
 		}
 	if (e == 0 || e != n_par) return LZGPU_NOT_HANDLED;
-	// Measured (profiles/sweep_r2.md, run 8): with general coefficients the rebuild is bound by the bit-plane multiplies, not by HBM, and
+	// Measured: with general coefficients the rebuild is bound by the bit-plane multiplies, not by HBM, and
 	// the grid-stride gf_dot_kernel (full occupancy, no stage barriers) does e >= 2 rows faster than this kernel's 16 warps per SM
-	// even though it needs separate CRC and image passes: ec(8,6) three lost 2.7 ms against 6.2 ms per 64 chunks.  One lost part
-	// (ec(8,6): 2.45 ms against 3.98 with verification and image), and two lost parts when the call verifies and wants the image
-	// (ec(4,5) 4.39 against 4.87, ec(21,4) 5.05 against 5.38), stay here.
+	// even though it needs separate CRC and image passes.  One lost part, and two lost parts when the call verifies and wants the
+	// image, measured faster here and stay here.
 	if (direct && !direct_forced && !(e == 1 || (e == 2 && d_part_crc && d_chunk_out))) return LZGPU_NOT_HANDLED;
 	// every requested missing part must be a data part
 	for (int i = K; i < N; ++i)
 		if (want[i] && !d_parts[i] && d_out && d_out[i]) return LZGPU_NOT_HANDLED;
 	// geometry: even G (1024-byte aligned slot regions), K*G*4 rows <= 256
-	// Two CTAs per SM with a 3-stage ring, or one CTA with 6 stages?  Measured on the same box (64 MiB chunks, fraction of
-	// the HBM copy peak, two / one):  ec(3,2) 2 lost 0.48 / 0.42 (+image 0.64 / 0.58),  xor3 1 lost 0.93 / 0.70 (+image
-	// 0.73 / 0.77),  ec(8,2) 2 lost 0.66 / 0.70 (+image 0.72 / 0.78),  ec(8,2) 1 lost 0.94 / 0.99.  So: the runtime-k
-	// shapes, except the single-erasure case that also writes the image.  LZGPU_RECOVER_TWO=0|1 forces either.
+	// Two CTAs per SM with a 3-stage ring, or one CTA with 6 stages?  Measured with 64 MiB chunks: two CTAs win for the runtime-k
+	// shapes, except the single-erasure case that also writes the image; the k = 8 instantiation keeps one.  LZGPU_RECOVER_TWO=0|1 forces either.
 	const bool two_auto = K != 8 && (e == 2 || (e == 1 && !d_chunk_out));
 	const bool two = e <= 2 && (fs->recover_two < 0 ? two_auto : fs->recover_two != 0);
-	// Measured (profiles/sweep_r2.md, fraction of the HBM peak, recover only / verify + image): the 16-warp CTA wins for the
-	// runtime-k shapes with two or more erased parts — ec(3,2) two lost 0.69 / 0.69 against 0.52 / 0.67 on two 9-warp CTAs, ec(5,3)
-	// three lost 0.29 / 0.42 against 0.23 / 0.32 and two lost 0.59 / 0.74 against 0.46 / 0.65 on one — while the k = 8 instantiation
-	// keeps one 9-warp CTA with six stages (two lost: 0.81 with verification and image against 0.70).  LZGPU_RECOVER_GEO=0|1|2 forces one.
+	// Measured (recover only and verify + image): the 16-warp CTA wins for the runtime-k shapes with two or more erased parts, against
+	// two 9-warp CTAs and against one, while the k = 8 instantiation keeps one 9-warp CTA with six stages.  LZGPU_RECOVER_GEO=0|1|2 forces one.
 	int geo = fs->recover_geo >= 0 ? fs->recover_geo : (K != 8 && e >= 2) ? 2 : (two ? 1 : 0);
 	if (direct) geo = 2;
 	if (geo == 1 && e > 2) geo = 0;
@@ -699,10 +693,9 @@ int lz_fused_recover(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, 
 	bool bs3 = !direct && e == 3 && fs->bs_recover && p.par_row[0] == 0 && p.par_row[1] == 1 && p.par_row[2] == 2;
 	uint32_t G = 0, n_stages = 0;
 	if (bs3) {
-		// Run 33 (fraction of the HBM peak, at most four / at most eight GF warps): rebuild only — no stream warps, G = 16, eight GF warps —
-		// ec(5,3) 0.440 / 0.682, ec(6,3) 0.388 / 0.628, ec(8,3) 0.452 / 0.648; with verification and image ec(5,3) 0.589 / 0.722 (seven GF
-		// warps), ec(6,3) 0.570 / 0.640 (six), but ec(8,3) 0.689 / 0.658 (five: one scheduler gets two of them).  So: the largest G, unless
-		// it only buys a fifth GF warp.
+		// Measured with at most four against at most eight GF warps: more GF warps win for rebuild only (no stream warps, G = 16, eight
+		// GF warps) and with verification and image for ec(5,3) (seven) and ec(6,3) (six), but ec(8,3) loses with five (one scheduler
+		// gets two of them).  So: the largest G, unless it only buys a fifth GF warp.
 		bool any_crc = false;
 		for (int a = 0; a < K; ++a) any_crc |= d_part_crc && d_part_crc[used[a]];
 		uint32_t g4 = 0;
@@ -872,7 +865,7 @@ int lz_fused_recover(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, 
 	}
 	if (direct) {
 		// item width: 16-byte items leave most of the 16 warps without work when k is large (G small)
-		// run 8: the 8 / 16-byte items win on every shape (ec(32,4) four lost: 12.0 ms against 38.0 per 64 chunks); 4-byte items stay for A/B
+		// the 8 / 16-byte items measured faster on every shape; 4-byte items stay for A/B
 		const bool wide = fs->direct_wide >= 0 ? fs->direct_wide != 0 : true;
 		switch (e) {
 			case 1: return launch_direct<1>(ctx, maps, p, smem, st, wide);
@@ -882,13 +875,13 @@ int lz_fused_recover(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, 
 		}
 	}
 	// ec(3,2) / ec(5,3) on the 16-warp geometry: compile-time k (the walk over the columns unrolls, parameter loads become immediates).
-	// Measured (run 18): ec(3,2) two lost, rebuild only 0.689 -> 0.827 of the HBM peak; with verification and image 0.692 -> 0.703.
+	// Measured faster than the runtime-k kernel for ec(3,2), most of all for rebuild only.
 	if (K == 3 && geo == 2 && fs->recover_k3) {
 		if (e == 1 && row0) return launch_recover_geo2<1, 3, 0, -1>(ctx, maps, p, smem, st);
 		if (e == 2 && row01) return launch_recover_geo2<2, 3, 0, 1>(ctx, maps, p, smem, st);
 	}
-	// ec(5,3) (run 19): two lost, rebuild only 0.585 -> 0.682 but with verification and image 0.749 -> 0.717 (the unrolled walk costs the CRC
-	// role registers), so that combination keeps the runtime-k kernel; three lost 0.329 -> 0.373 and 0.471 -> 0.519
+	// ec(5,3): two lost, faster for rebuild only but slower with verification and image (the unrolled walk costs the CRC role
+	// registers), so that combination keeps the runtime-k kernel; three lost faster either way
 	if (K == 5 && geo == 2 && fs->recover_k3) {
 		if (e == 2 && row01 && !(*verifying && d_chunk_out)) return launch_recover_geo2<2, 5, 0, 1>(ctx, maps, p, smem, st);
 		if (e == 3 && row01) return launch_recover_geo2<3, 5, 0, 1>(ctx, maps, p, smem, st);

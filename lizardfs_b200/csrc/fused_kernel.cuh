@@ -55,8 +55,8 @@ namespace lzd {
 
 // Diagnostics build (-DLZ_ALL_LANES_ARRIVE): every lane arrives on the parity-ring mbarriers instead of one elected
 // lane after __syncwarp().  compute-sanitizer racecheck does not model the cumulativity of __syncwarp + elected arrive
-// and reports the ring's STS/LDS pairs as hazards; with all lanes arriving the same protocol is reported clean
-// (profiles/sanitizer_r1.md).  The production build elects one lane (fewer barrier operations).
+// and reports the ring's STS/LDS pairs as hazards; with all lanes arriving the same protocol is reported clean.
+// The production build elects one lane (fewer barrier operations).
 #ifdef LZ_ALL_LANES_ARRIVE
 #define LZ_RING_ARRIVERS 32u
 #define LZ_RING_LANE(lane) true
@@ -290,7 +290,7 @@ __device__ __forceinline__ uint32_t fold_finish(uint32_t (&win)[FW], const uint3
 //   + 0    s_blk[2][64]       block linear CRCs of the current / previous unit (row-0 parity CRC)
 //   + 520  full[NST], empty[NST], pfull[NPST], pempty[NPST]   (8 bytes each)
 // Register budget: __launch_bounds__(288, 2) makes ptxas target 96 registers (2 CTAs/SM), (288, 1) -> 168.
-// (An explicit __maxnreg__(96) instead of the launch bounds produced a 5 % slower kernel on the same box: ptxas
+// (An explicit __maxnreg__(96) instead of the launch bounds produced a slower kernel: ptxas
 // schedules differently when it does not know the block size.)
 template <int M, bool GENERIC, int KT, int GT, int FW, bool STRIPED = false, bool SPLIT = false, int W = fused_item_words(M, GENERIC)>
 __global__ void __launch_bounds__(fused_threads(M, GENERIC, W == 8), fused_ctas_per_sm(M, GENERIC, FW, W == 8))
@@ -884,7 +884,7 @@ fused_recover_kernel(const __grid_constant__ TmapArray tmaps, const __grid_const
 							for (int w = 0; w < W; ++w) acc[r][w] ^= pv[w];
 						}
 						if (E == 2 && R0 == 0 && R1 == 1 && KT != 8) {
-							// (not the k = 8 instantiation: there the two bit-plane multiplies measured 5 % faster)
+							// (not the k = 8 instantiation: there the two bit-plane multiplies measured faster)
 							// RAID-6 elimination: S0 = d0 ^ d1, S1 = 2^x0 d0 ^ 2^x1 d1  =>  (2^x0 ^ 2^x1) d1 = S1 ^ 2^x0 S0, d0 = S0 ^ d1:
 							// ONE general multiply per word (w[1] = planes of (2^x0 ^ 2^x1)^-1) and x0 doublings (x0 is the smaller
 							// index; more than four doublings cost more than the bit-plane multiply by 2^x0, w[0]).

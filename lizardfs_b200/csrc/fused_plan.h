@@ -23,13 +23,14 @@ constexpr int kMaxParityRows = 128;
 constexpr int kSmemCap = 113 * 1024;                   // dynamic shared memory per CTA with two CTAs per SM
 
 // Three or four parity rows keep 12-16 Horner accumulators live next to the 64-word CRC window: at 96 registers the kernel
-// spills into its inner loop (ncu: long-scoreboard stalls on the local loads, profiles/ec84_r1_ncu_summary.md).  Those
+// spills into its inner loop (ncu: long-scoreboard stalls on the local loads).  Those
 // shapes run with 8 warps instead of 9, which lets two CTAs per SM have 128 registers per thread.
-// CTA shape per instantiation (parity rows M, Vandermonde or generic coefficients) — measured, profiles/sweep_r2.md:
-//   M <= 2            two 8-warp CTAs per SM (ec(8,2): G = 7, 252 of 256 threads carry a stream; +3.5 % over the 9-warp CTA whose
+// CTA shape per instantiation (parity rows M, Vandermonde or generic coefficients), each the faster one in A/B measurements on the
+// previous target (same per-SM shared memory, registers and schedulers as the H100; not re-swept on the H100):
+//   M <= 2            two 8-warp CTAs per SM (ec(8,2): G = 7, 252 of 256 threads carry a stream; faster than the 9-warp CTA whose
 //                     ninth warp — parity CRC only — unbalances the four schedulers)
 //   M == 3            two 8-warp CTAs per SM, 128 registers (12 Horner accumulators next to the 64-word CRC window spill at 96)
-//   M == 4            ONE 16-warp CTA per SM (ec(8,4): G = 8, every scheduler gets two item warps and three row warps; +11 % over
+//   M == 4            ONE 16-warp CTA per SM (ec(8,4): G = 8, every scheduler gets two item warps and three row warps; faster than
 //                     two 8-warp CTAs whose five item warps load the schedulers 2:1:1:1), deeper stage ring instead
 //   generic (Cauchy)  two 9-warp CTAs; item width chosen per launch (fused_generic_item_words)
 // Every value can be overridden at build time (-DLZ_T2=..., experiment builds next to the production library).
@@ -49,13 +50,13 @@ constexpr int kSmemCap = 113 * 1024;                   // dynamic shared memory 
 #define LZ_W3 4
 #endif
 #ifndef LZ_W4
-#define LZ_W4 2           // ec(8,4): 512 eight-byte items fill the 16 warps (0.43 -> 0.52 of the HBM peak, profiles/sweep_r2.md)
+#define LZ_W4 2           // ec(8,4): 512 eight-byte items fill the 16 warps (measured faster than 16-byte items)
 #endif
-// Bit-sliced GF role (bitslice.cuh; round 2, runs 26-28: ec(8,4) 0.52 -> 0.79, ec(6,4) 0.50 -> 0.71, ec(10,4) 0.42 -> 0.60, ec(8,3)
-// 0.57 -> 0.82, ec(31,3) 0.08 -> 0.23 of the HBM peak): three or four Vandermonde rows on ONE 16-warp CTA per SM whose last
+// Bit-sliced GF role (bitslice.cuh; measured faster than packed-word Horner for every four-row goal and for three rows on wide
+// stripes): three or four Vandermonde rows on ONE 16-warp CTA per SM whose last
 // ceil(16 G / 32) <= 4 warps only do the GF items (32-byte items on bit planes); the warps before them own the CRC streams.
-// LZGPU_BITSLICE / LZ_BITSLICE_DEFAULT: bit 0 = four parity rows, bit 1 = three parity rows with k >= 7 (narrower stripes measured
-// 3-5 % slower than the two 8-warp CTAs of the packed-byte route: ec(5,3) 0.750 / 0.731, ec(6,3) 0.784 / 0.746, ec(4,3) 0.778 / 0.770),
+// LZGPU_BITSLICE / LZ_BITSLICE_DEFAULT: bit 0 = four parity rows, bit 1 = three parity rows with k >= 7 (narrower stripes — ec(4,3),
+// ec(5,3), ec(6,3) — measured slightly slower than the two 8-warp CTAs of the packed-byte route),
 // bit 2 = three parity rows with any k (A/B).
 #ifndef LZ_BITSLICE_DEFAULT
 #define LZ_BITSLICE_DEFAULT 3
@@ -69,9 +70,9 @@ LZ_HD constexpr int fused_threads(int m, bool generic, bool bs = false) { return
 // (generic coefficients: chosen per launch by fused_generic_item_words — both widths are instantiated)
 LZ_HD constexpr int fused_item_words(int m, bool generic) { return generic ? 4 : m == 3 ? LZ_W3 : m == 4 ? LZ_W4 : 4; }
 // Generic (Cauchy) coefficients: 16-byte items when a step has at least three warps of them (the fixed cost per item — addresses,
-// narrow loads and stores — dominates otherwise: ec(8,6) 0.07 -> 0.12, ec(16,8) 0.04 -> 0.06 of the HBM peak with 16-byte items),
+// narrow loads and stores — dominates otherwise: 16-byte items measured faster for ec(8,6) and ec(16,8)),
 // 4-byte items when k > 20 leaves only two stripes per unit (ec(21,4): 64 sixteen-byte items would put every multiply on two warps;
-// 0.068 -> 0.076)
+// 4-byte items measured faster)
 LZ_HD constexpr int fused_generic_item_words(uint32_t G) { return 32 * G >= 96 ? 4 : 1; }
 // CTAs per SM: two, except for the 128-word fold window and for CTAs of more than nine warps (16 warps x 128 registers fill the
 // register file on their own; their stage ring is deeper instead)
@@ -99,17 +100,17 @@ inline size_t fused_smem_bytes(uint32_t rows, uint32_t prows, int fw, int m, boo
 // The bit-sliced kernels take their stage count at run time: as many stages as fit (their G is capped at 8 by the 128 GF threads,
 // so narrow stripes leave shared memory for a deeper ring — more bytes in flight per SM)
 #ifndef LZ_BS_MAX_STAGES
-#define LZ_BS_MAX_STAGES 4   // (run 28: 4 / 6 / 8 stages, 200 / 224 KB — within 1 % of each other for every goal; LZGPU_BS_STAGES, LZGPU_BS_SMEM_KB)
+#define LZ_BS_MAX_STAGES 4   // (4 / 6 / 8 stages, 200 / 224 KB measured alike for every goal; LZGPU_BS_STAGES, LZGPU_BS_SMEM_KB)
 #endif
 
 // Largest stripe group G such that data + parity-CRC rows fit the consumer threads, the data rows fit
 // one TMA box (<= 256 rows, a multiple of 8 for the 1024-byte stage alignment) and the stages fit shared memory.
 #ifndef LZ_GCAP
 #define LZ_GCAP 1         // on the one-CTA shapes never plan more GF items per step than the CTA has threads (ec(4,4): G = 16 would
-#endif                    // give every thread two items and leave half the warps without a stream: 0.35 -> 0.38 with G = 8)
+#endif                    // give every thread two items and leave half the warps without a stream; G = 8 measured faster)
 // (bit-sliced: 16 items of 32 bytes per stripe and step on the last ceil(16 g / 32) warps — at most bs_max_gf_warps of them —, the
-// streams on the warps before them.  Run 33: the encoders are ALU bound, a fifth or sixth GF warp only unbalances the four
-// schedulers — ec(4,4) G = 10 / five GF warps 0.66 against G = 8 / four 0.77, ec(6,4) 0.60 against 0.71 — so four is the default;
+// streams on the warps before them.  The encoders are ALU bound: a fifth or sixth GF warp only unbalances the four
+// schedulers — measured slower for ec(4,4) and ec(6,4) — so four is the default;
 // LZGPU_BS_GFW raises it for A/B runs.)
 #ifndef LZ_BS_MAX_GF_WARPS
 #define LZ_BS_MAX_GF_WARPS 4
@@ -140,8 +141,8 @@ struct FusedPlan {
 	bool bs = false;  // bit-sliced geometry (16 warps, four of them GF warps)
 };
 
-// striped_policy: -1 automatic (striped when per-chunk units would leave more than 12 % of their stripe slots empty — measured,
-// profiles/sweep_r1.md: G boxes per step instead of one cost 2-10 % at 64 MiB and win up to 2.4x at 1-4 MiB), 0 never, 1 always
+// striped_policy: -1 automatic (striped when per-chunk units would leave more than 12 % of their stripe slots empty — measured:
+// G boxes per step instead of one cost a few per cent at 64 MiB and win by a wide margin at 1-4 MiB), 0 never, 1 always
 inline FusedPlan fused_plan(int M, bool generic, uint32_t K, uint32_t n_chunks, uint32_t nb, size_t chunk_stride, int smem_cap, int fw,
                             int striped_policy, bool bs = false, int bs_max_stages = LZ_BS_MAX_STAGES, int bs_max_gf_warps = LZ_BS_MAX_GF_WARPS) {
 	FusedPlan pl;

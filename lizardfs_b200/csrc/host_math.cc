@@ -487,6 +487,6 @@ int lzgpu_plan_convert(const lzgpu_goal *src, const lzgpu_goal *dst, const uint8
 	return LZGPU_OK;
 }
 
-const char *lzgpu_version(void) { return "lizardfs_b200 0.1 (sm_100a)"; }
+const char *lzgpu_version(void) { return "lizardfs_b200 0.1 (sm_90a)"; }
 
 }  // extern "C"

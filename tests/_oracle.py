@@ -1,7 +1,10 @@
 """ctypes bindings for the CPU oracle (oracle/liboracle.so) and, when present, the real
 reference build (oracle/_ref/liblzref.so).  TEST INFRASTRUCTURE ONLY — nothing under
 lizardfs_b200/ imports this module."""
+import atexit
 import ctypes as C
+import hashlib
+import json
 import os
 import subprocess
 
@@ -163,13 +166,64 @@ def load_oracle():
 
 
 def load_ref():
+    """the reference compiled by oracle/Makefile (where its sources are present), or None"""
     path = os.path.join(ORACLE_DIR, "_ref", "liblzref.so")
     if not os.path.exists(path):
-        if os.path.isdir("/root/reference/src/common"):
-            build_oracle()
-        if not os.path.exists(path):
-            return None
+        return None
     return Lib(C.CDLL(path), "ref_")
+
+
+# ---- the reference's answers, recorded ------------------------------------------------------------
+# Tests that compare with the compiled reference compare digests of the answers.  Where oracle/_ref is built the reference is
+# called; elsewhere the digest recorded from it in REF_DIGESTS is used, so every comparison holds on a machine that cannot build
+# the reference.  LZ_RECORD_REF_DIGESTS=1 (with oracle/_ref built) rewrites REF_DIGESTS from the calls the tests make.
+REF_DIGESTS = os.path.join(ROOT, "tests", "golden", "reference_digests.json")
+_ref_lib = []
+_recorded = {}
+_table = {}
+
+
+def digest(*values):
+    """sha256 over the bytes of arrays / ints (ints as int64, None as a marker): equal digests = equal answers"""
+    h = hashlib.sha256()
+    for v in values:
+        if v is None:
+            h.update(b"none")
+        elif isinstance(v, (int, np.integer)):
+            h.update(np.int64(v).tobytes())
+        else:
+            h.update(np.ascontiguousarray(v).tobytes())
+    return h.hexdigest()
+
+
+def _write_recorded():
+    old = {}
+    if os.path.exists(REF_DIGESTS):
+        with open(REF_DIGESTS) as f:
+            old = json.load(f)
+    old.update(_recorded)
+    with open(REF_DIGESTS, "w") as f:
+        json.dump(dict(sorted(old.items())), f, indent=0)
+        f.write("\n")
+
+
+def ref_digest(tag, call):
+    """digest() of the tuple `call(ref)` returns, for the compiled reference; `tag` names the call uniquely"""
+    if not _ref_lib:
+        _ref_lib.append(load_ref())
+        if _ref_lib[0] is not None and os.environ.get("LZ_RECORD_REF_DIGESTS"):
+            atexit.register(_write_recorded)
+    ref = _ref_lib[0]
+    if ref is not None:
+        d = digest(*call(ref))
+        if os.environ.get("LZ_RECORD_REF_DIGESTS"):
+            _recorded[tag] = d
+        return d
+    if not _table:
+        with open(REF_DIGESTS) as f:
+            _table.update(json.load(f))
+    assert tag in _table, f"{tag}: no recorded answer of the reference in {REF_DIGESTS}"
+    return _table[tag]
 
 
 def fill_chunk(oracle, nbytes, seed, chunk_index=0):

@@ -9,9 +9,9 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on an H100 with -m gpu)")
     # the suites load the in-tree liblzgpu.so (host maths and ABI tests need it even without a GPU): build it if a fresh
-    # checkout has not run __graft_entry__.build() yet (nvcc cross-compiles for sm_100a without a device)
+    # checkout has not run __graft_entry__.build() yet (nvcc cross-compiles for sm_90a without a device)
     if not os.path.exists(os.path.join(ROOT, "lizardfs_b200", "liblzgpu.so")):
         import subprocess
         subprocess.run(["make", "-s", "-C", os.path.join(ROOT, "lizardfs_b200", "csrc"), "-j8"], check=False)

@@ -1,6 +1,6 @@
 // gtest.h — a few dozen lines standing in for <gtest/gtest.h> (googletest is not in this image) so that the REFERENCE'S OWN
 // unit-test sources (src/common/*_unittest.cc, compiled where they lie under /root/reference) build unmodified against
-// liblzgpu.so: tests/cpp/Makefile target test_link_substitution.  Only what those files use: TEST, EXPECT_/ASSERT_ EQ, NE,
+// liblzgpu.so: oracle/Makefile target _ref/test_link_substitution.  Only what those files use: TEST, EXPECT_/ASSERT_ EQ, NE,
 // TRUE, FALSE, GE, NO_THROW with optional `<< message`.  main() is in tests/cpp/link_substitution_main.cc.
 #pragma once
 #include <functional>

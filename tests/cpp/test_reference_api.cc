@@ -2,7 +2,7 @@
 // reference-named interfaces: ReedSolomon<32,32> (include/lzgpu_reed_solomon.hpp), mycrc32 /
 // mycrc32_combine / blockXor with C++ linkage (lizardfs_b200/csrc/compat_cxx.cc) and the ISA-L names.
 // Mirrors src/common/reed_solomon_unittest.cc:136-199, crc_unittest.cc:27-63, block_xor_unittest.cc:24-35.
-// Exit code 0 = all passed.  Needs a B200 (run by tests/test_gpu_cpp.py).
+// Exit code 0 = all passed.  Needs an H100 (run by tests/test_gpu_cpp.py).
 #include <cstdint>
 #include <cstdio>
 #include <cstdlib>

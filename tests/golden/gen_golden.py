@@ -1,5 +1,7 @@
 """Generate tests/golden/vectors.json from the UNMODIFIED reference (oracle/_ref/liblzref.so,
-built by oracle/Makefile from /root/reference sources).  Run in the build container:
+built by oracle/Makefile from the reference sources), and tests/golden/reference_digests.json: the
+digests of the reference's answers to the calls the tests make (tests/_oracle.py ref_digest).  Run
+where oracle/_ref is built:
 
     python tests/golden/gen_golden.py
 
@@ -86,6 +88,31 @@ def main():
     with open(os.path.join(os.path.dirname(__file__), "vectors.json"), "w") as f:
         json.dump(out, f, indent=1)
     print("wrote vectors.json with", len(out["cases"]), "cases")
+    record_reference_digests()
+
+
+def record_reference_digests():
+    """run the tests that compare with the reference with LZ_RECORD_REF_DIGESTS=1; the GPU one through a stand-in engine (the
+    oracle's conversion), since only the reference's side of it is recorded"""
+    import subprocess
+    if os.path.exists(O.REF_DIGESTS):
+        os.remove(O.REF_DIGESTS)
+    env = dict(os.environ, LZ_RECORD_REF_DIGESTS="1")
+    subprocess.run([sys.executable, "-m", "pytest", "-q", "-p", "no:cacheprovider", "tests/test_oracle.py", "tests/test_oracle_plans.py"],
+                   cwd=ROOT, env=env, check=True)
+    os.environ["LZ_RECORD_REF_DIGESTS"] = "1"
+    from tests import test_gpu_replication as R
+    oracle = O.load_oracle()
+
+    class OracleEngine:
+        def convert_chunks(self, src, dst, nb, parts, want):
+            sk = (src.kind, src.k, src.m)
+            avail = [None if p is None else p[0] for p in parts]
+            rc, out, ocrc, _ = O.convert_chunk(oracle, sk, avail, None, (dst.kind, dst.k, dst.m), want, nb)
+            assert rc == 0
+            return [o[None, :] for o in out], [c[None, :] for c in ocrc]
+    R.test_convert_chunks_vs_reference_planner(OracleEngine(), oracle)
+    print("recorded", len(O._recorded), "answers of the reference (plus those of the pytest run) in", O.REF_DIGESTS)
 
 
 if __name__ == "__main__":

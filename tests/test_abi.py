@@ -37,11 +37,11 @@ def test_reference_cxx_names_exported():
         assert mangled in out
 
 
-def test_library_has_only_sm100a_code_and_no_oracle_dependency():
+def test_library_has_only_sm90a_code_and_no_oracle_dependency():
     out = subprocess.run(["cuobjdump", "--list-elf", _lib.LIB_PATH], capture_output=True, text=True)
     if out.returncode == 0 and out.stdout.strip():
         archs = set(re.findall(r"sm_(\d+a?)", out.stdout))
-        assert archs == {"100a"}, archs
+        assert archs == {"90a"}, archs
     ldd = subprocess.run(["ldd", _lib.LIB_PATH], capture_output=True, text=True).stdout
     assert "oracle" not in ldd and "lzref" not in ldd
 

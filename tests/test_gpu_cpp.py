@@ -54,7 +54,7 @@ def test_read_plan_mirror_cpp():
     built and pre-executed by the reference's own ChunkReadPlanner (oracle/_ref) — must reproduce the reference's
     post-processed buffer byte for byte (tests/cpp/test_read_plan.cc)."""
     if not os.path.exists(READ_PLAN):
-        pytest.skip("oracle/_ref/liblzref.so was not built (no /root/reference), so the reference planners are unavailable")
+        pytest.skip("oracle/_ref/liblzref.so was not built (no reference sources), so the reference planners are unavailable")
     r = subprocess.run([READ_PLAN], capture_output=True, text=True, timeout=600)
     assert r.returncode == 0, r.stdout + r.stderr
     assert "all tests passed" in r.stdout
@@ -68,7 +68,7 @@ def _run_cpu_build(name, needs_ref=False):
         subprocess.run(["make", "-s", "-C", os.path.join(ROOT, "tests", "cpp")], check=True)
     if not os.path.exists(exe):
         assert needs_ref, f"{name} was not built"
-        pytest.skip("oracle/_ref/liblzref.so was not built (no /root/reference), so the reference planners are unavailable")
+        pytest.skip("oracle/_ref/liblzref.so was not built (no reference sources), so the reference planners are unavailable")
     r = subprocess.run([exe], capture_output=True, text=True, timeout=600)
     assert r.returncode == 0, r.stdout + r.stderr
     assert "all tests passed" in r.stdout
@@ -84,15 +84,16 @@ def test_read_plan_mirror_host_logic_on_cpu():
     _run_cpu_build("test_read_plan_cpu", needs_ref=True)
 
 
-LINK_SUB = os.path.join(ROOT, "tests", "cpp", "build", "test_link_substitution")
-LINK_SUB_CXX = os.path.join(ROOT, "tests", "cpp", "build", "test_link_substitution_cxx")
+# made by oracle/Makefile with oracle/_ref/liblzref.so (the reference's unit-test sources are compiled where they lie)
+LINK_SUB = os.path.join(ROOT, "oracle", "_ref", "test_link_substitution")
+LINK_SUB_CXX = os.path.join(ROOT, "oracle", "_ref", "test_link_substitution_cxx")
 
 
 def _need_link_sub(exe):
     if not os.path.exists(exe):
-        subprocess.run(["make", "-s", "-C", os.path.join(ROOT, "tests", "cpp")], check=False)
+        subprocess.run(["make", "-s", "-C", os.path.join(ROOT, "oracle")], check=False)
     if not os.path.exists(exe):
-        pytest.skip("built only where /root/reference exists (the reference's unit-test sources are compiled in place)")
+        pytest.skip("oracle/_ref was built without the reference sources, so the reference's unit tests are unavailable")
 
 
 @pytest.mark.parametrize("exe", [LINK_SUB, LINK_SUB_CXX], ids=["isal_names", "cxx_names"])

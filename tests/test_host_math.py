@@ -257,7 +257,7 @@ def test_convert_plan_decisions():
         avail = [0 if i in lost else 1 for i in range(s.k + s.m)]
         return L.Engine.plan_convert(s, d, avail, want if want is not None else [1] * (d.k + d.m)), s, d
 
-    # the measured case (profiles/probe_r2.md section 12): lcm(8, 3) = 24 blocks per unit, 152 rows on five warps, three rebuild warps
+    # the measured case: lcm(8, 3) = 24 blocks per unit, 152 rows on five warps, three rebuild warps
     p, s, d = plan("ec(8,2)", (1, 4), "ec(3,2)")
     assert (p["one_pass"], p["lost_data_parts"], p["stripes_per_unit"], p["source_stripes_per_unit"], p["worker_warps"], p["rebuild_warps"]) == (1, 2, 8, 3, 5, 3)
     assert p["stages"] == 4 and p["smem_bytes"] <= 113 * 1024

@@ -160,18 +160,16 @@ def test_survey_known_answers(oracle):
 
 
 # ---- oracle vs the real reference on random inputs ----------------------------------------------
-def test_oracle_equals_reference_random(oracle, ref):
-    if ref is None:
-        pytest.skip("oracle/_ref/liblzref.so not present")
+def test_oracle_equals_reference_random(oracle):
+    """against the compiled reference, or its answers recorded in tests/golden/reference_digests.json"""
     rng = np.random.default_rng(1234)
-    for _ in range(12):
+    for t in range(12):
         k = int(rng.integers(2, 12))
         m = int(rng.integers(1, 6))
         nb = int(rng.integers(1, 3 * k + 2))
         chunk = rng.integers(0, 256, size=nb * BLOCK, dtype=np.uint8)
         p1, c1 = oracle.encode_chunk(1, k, m, chunk)
-        p2, c2 = ref.encode_chunk(1, k, m, chunk)
-        assert (p1 == p2).all() and (c1 == c2).all()
+        assert O.digest(p1, c1) == O.ref_digest(f"random/{t}/encode", lambda ref: ref.encode_chunk(1, k, m, chunk))
         # degraded read with a random erasure pattern
         parts, pb = O.split_parts(chunk, k)
         allp = parts + [p for p in p1]
@@ -179,15 +177,19 @@ def test_oracle_equals_reference_random(oracle, ref):
         avail = [None if i in lost else allp[i] for i in range(k + m)]
         want = [1 if i in lost else 0 for i in range(k + m)]
         rc1, o1, _ = oracle.recover_chunk(1, k, m, avail, None, want, pb)
-        rc2, o2, _ = ref.recover_chunk(1, k, m, avail, None, want, pb)
-        assert rc1 == rc2 == 0
+        assert rc1 == 0
         for i in lost:
-            assert (o1[i] == allp[i]).all() and (o2[i] == allp[i]).all()
+            assert (o1[i] == allp[i]).all()
+
+        def ref_recover(ref):
+            rc2, o2, _ = ref.recover_chunk(1, k, m, avail, None, want, pb)
+            return [rc2] + [o2[i] for i in lost]
+        assert O.digest(rc1, *[o1[i] for i in lost]) == O.ref_digest(f"random/{t}/recover", ref_recover)
     for n in [1, 5, 4096, 65536, 65537]:
         buf = rng.integers(0, 256, size=n, dtype=np.uint8)
-        assert oracle.crc32(0x1234, buf) == ref.crc32(0x1234, buf)
-        assert oracle.crc32_combine(17, 99, n) == ref.crc32_combine(17, 99, n)
-        assert oracle.crc32_zeroblock(0xabc, n) == ref.crc32_zeroblock(0xabc, n)
+        ours = (oracle.crc32(0x1234, buf), oracle.crc32_combine(17, 99, n), oracle.crc32_zeroblock(0xabc, n))
+        assert O.digest(*ours) == O.ref_digest(f"random/crc/{n}", lambda ref: (ref.crc32(0x1234, buf), ref.crc32_combine(17, 99, n),
+                                                                                ref.crc32_zeroblock(0xabc, n)))
 
 
 def test_recover_detects_crc_mismatch(oracle):
@@ -206,15 +208,14 @@ def test_recover_detects_crc_mismatch(oracle):
     assert rc == 0 and (out[0] == allp[0]).all()
 
 
-def test_write_data_prefix_matches_reference(oracle, ref):
+def test_write_data_prefix_matches_reference(oracle):
     # the bytes printed by the reference's serializePrefix (cltocs.h:118-123) for a known packet
     got = O.write_data_prefix(oracle, 0x1122334455667788, 7, 3, 0, 65536, 0xAABBCCDD)
     assert got.tobytes().hex() == "000004bc0001001e0000000011223344556677880000000700030000000000010000aabbccdd"
     for args, want in GOLD["write_data_prefix"]:
         assert O.write_data_prefix(oracle, *args).tobytes().hex() == want
-    if ref is not None:
-        rng = np.random.default_rng(8)
-        for _ in range(20):
-            args = (int(rng.integers(0, 2**63)), int(rng.integers(0, 2**32)), int(rng.integers(0, 1024)), int(rng.integers(0, 65536)),
-                    int(rng.integers(1, 65537)), int(rng.integers(0, 2**32)))
-            assert (O.write_data_prefix(oracle, *args) == O.write_data_prefix(ref, *args)).all()
+    rng = np.random.default_rng(8)
+    for t in range(20):
+        args = (int(rng.integers(0, 2**63)), int(rng.integers(0, 2**32)), int(rng.integers(0, 1024)), int(rng.integers(0, 65536)),
+                int(rng.integers(1, 65537)), int(rng.integers(0, 2**32)))
+        assert O.digest(O.write_data_prefix(oracle, *args)) == O.ref_digest(f"write_data_prefix/{t}", lambda ref: (O.write_data_prefix(ref, *args),))

@@ -1,6 +1,6 @@
 // warpmap.cu — diagnostics: which hardware warp slot (%warpid) each warp of each co-resident CTA gets, for the CTA shapes the
 // fused kernels use.  The sub-partition (scheduler) of a warp is %warpid % 4 on this architecture; the table tells whether two
-// co-resident CTAs put their warp w on the same scheduler.   nvcc -arch=sm_100a -o warpmap warpmap.cu && ./warpmap
+// co-resident CTAs put their warp w on the same scheduler.   nvcc -arch=sm_90a -o warpmap warpmap.cu && ./warpmap
 #include <cstdio>
 #include <cstdlib>
 #include <cuda_runtime.h>

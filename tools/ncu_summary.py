@@ -1,6 +1,6 @@
 #!/usr/bin/env python
-"""ncu_summary.py REPORT.ncu-rep "title" "command" > profiles/xxx.md — the metrics the roofline discussion needs, from one
-`ncu --set full` capture (read with `ncu -i ... --page raw --csv`; works on the CPU box)."""
+"""ncu_summary.py REPORT.ncu-rep "title" "command" > summary.md — the metrics the roofline discussion needs, from one
+`ncu --set full` capture (read with `ncu -i ... --page raw --csv`; works on a machine without a GPU)."""
 import csv
 import subprocess
 import sys
@@ -11,7 +11,7 @@ rows = list(csv.reader(raw.splitlines()))
 hdr, units = rows[0], rows[1]
 print(f"# ncu --set full summary: {title}\n")
 if cmd:
-    print(f"Command (under gpurun, 1 GPU): `{cmd}`\n")
+    print(f"Command (1 GPU): `{cmd}`\n")
 print("Profiler timings are cold-cache / serialised; bench values are never taken under ncu.\n")
 KEYS = ["gpu__time_duration.sum", "dram__bytes_read.sum", "dram__bytes_write.sum", "dram__bytes.sum.per_second",
         "gpu__dram_throughput.avg.pct_of_peak_sustained_elapsed", "lts__t_sector_hit_rate.pct",

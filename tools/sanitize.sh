@@ -1,4 +1,4 @@
-# compute-sanitizer passes over a small encode + recover + scrub through the C ABI (run under gpurun).
+# compute-sanitizer passes over a small encode + recover + scrub through the C ABI (run on a GPU machine).
 # Full reports land in gpurun_out/sanitize_<tool>.log.
 mkdir -p gpurun_out
 cat > /tmp/san_case.py <<'PY'

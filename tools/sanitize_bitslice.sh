@@ -1,4 +1,4 @@
-# compute-sanitizer memcheck over the bit-sliced three- / four-parity-row encoders only (run under gpurun; the long case list is tools/sanitize.sh).
+# compute-sanitizer memcheck over the bit-sliced three- / four-parity-row encoders only (on a GPU machine; the long case list is tools/sanitize.sh).
 mkdir -p gpurun_out
 cat > /tmp/san_bs.py <<'PY'
 import os, sys
