@@ -156,6 +156,12 @@ typedef struct lzgpu_stats {
 } lzgpu_stats;
 void lzgpu_get_stats(lzgpu_ctx *ctx, lzgpu_stats *out);
 void lzgpu_reset_stats(lzgpu_ctx *ctx);
+/* Diagnostics: the grid (CTAs) and the work units of the context's most recent launch of a persistent streaming kernel (fused
+ * encode / CRC, degraded read, slice conversion; each CTA takes units blockIdx.x, + gridDim.x, ...).  Both 0 before the first one.
+ * Host-side bookkeeping of the launch, not a device query; with concurrent calls on one context "most recent" is whichever
+ * launched last.  LZGPU_GRID_CAP=n in the environment when the context is created caps every such grid at n CTAs (testing:
+ * every CTA then walks several units). */
+int lzgpu_debug_last_launch(lzgpu_ctx *ctx, uint32_t *grid, uint32_t *units);
 
 /* ---------------------------------------------------------------------------------------------
  * Device pool: several GPUs behind ONE process (the mount runs ten write workers in one process, src/mount/lizard_client.h:77,

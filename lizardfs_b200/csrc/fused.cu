@@ -55,7 +55,19 @@ struct FusedState {
 	int bs_smem_cap = 200 * 1024;          // LZGPU_BS_SMEM_KB: their shared memory budget (one CTA per SM)
 	int bitslice = LZ_BITSLICE_DEFAULT;  // LZGPU_BITSLICE: Vandermonde parity rows on bit planes (W = 8 items, bitslice.cuh) — bit 0: four rows, bit 1: three rows with k >= 7, bit 2: three rows with any k; 0 = packed-byte Horner
 	int promo = 3;  // CU_TENSOR_MAP_L2_PROMOTION_L2_256B: measured faster streaming than 128B/none
+	uint32_t grid_cap = 0;  // LZGPU_GRID_CAP (testing): at most this many CTAs per persistent launch, so that every CTA walks several units; 0 = no cap
+	std::atomic<uint64_t> last_launch{0};  // grid << 32 | total_units of the latest persistent launch (lzgpu_debug_last_launch)
 };
+
+// CTAs of a persistent launch (each CTA starts at unit blockIdx.x and steps by gridDim.x): one per unit, at most `per_sm` per SM,
+// and at most LZGPU_GRID_CAP when that is set
+static int persistent_grid(lzgpu_ctx *ctx, uint64_t total_units, int per_sm) {
+	FusedState *fs = ctx->fused;
+	uint64_t grid = std::min<uint64_t>(total_units, static_cast<uint64_t>(ctx->sm_count) * per_sm);
+	if (fs->grid_cap) grid = std::min<uint64_t>(grid, fs->grid_cap);
+	fs->last_launch.store(grid << 32 | total_units);
+	return static_cast<int>(grid);
+}
 
 // x^n mod P for a possibly negative n (x has multiplicative order dividing 2^32 - 1)
 static uint32_t crc_xpow_bits_signed(long long n) {
@@ -167,6 +179,7 @@ int lz_fused_init(lzgpu_ctx *ctx) {
 	if (const char *e = std::getenv("LZGPU_BS_RECOVER_GFW")) fs->bs_recover_gf_warps = std::max(1, std::min(16, std::atoi(e)));
 	if (const char *e = std::getenv("LZGPU_BS_STAGES")) fs->bs_max_stages = std::max(2, std::min(16, std::atoi(e)));
 	if (const char *e = std::getenv("LZGPU_BS_SMEM_KB")) fs->bs_smem_cap = std::max(64, std::min(226, std::atoi(e))) * 1024;
+	if (const char *e = std::getenv("LZGPU_GRID_CAP")) fs->grid_cap = static_cast<uint32_t>(std::max(0, std::atoi(e)));
 	void *fn = nullptr;
 	cudaDriverEntryPointQueryResult qres;
 	cudaError_t e = cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &qres);
@@ -262,6 +275,14 @@ void lz_fused_destroy(lzgpu_ctx *ctx) {
 	ctx->fused = nullptr;
 }
 
+extern "C" int lzgpu_debug_last_launch(lzgpu_ctx *ctx, uint32_t *grid, uint32_t *units) {
+	if (!ctx || !ctx->fused || !grid || !units) return LZGPU_ERR_ARG;
+	const uint64_t v = ctx->fused->last_launch.load();
+	*grid = static_cast<uint32_t>(v >> 32);
+	*units = static_cast<uint32_t>(v);
+	return LZGPU_OK;
+}
+
 static int make_tensor_map(FusedState *fs, CUtensorMap *map, const void *base, uint64_t rows_per_chunk, uint64_t n_chunks,
                            uint64_t chunk_stride, uint32_t box_rows) {
 	const cuuint64_t dims[3] = {static_cast<cuuint64_t>(kRowBytes), rows_per_chunk, n_chunks};
@@ -282,8 +303,7 @@ static int make_tensor_map(FusedState *fs, CUtensorMap *map, const void *base, u
 
 template <int M, bool GENERIC, int KT = 0, int GT = 0, int FW = 64, bool STRIPED = false, bool SPLIT = false>
 static int launch(lzgpu_ctx *ctx, const CUtensorMap &map, const FusedParams &p, size_t smem, cudaStream_t st) {
-	const int per_sm = fused_ctas_per_sm(M, GENERIC, FW);
-	const int grid = static_cast<int>(std::min<uint64_t>(p.total_units, static_cast<uint64_t>(ctx->sm_count) * per_sm));
+	const int grid = persistent_grid(ctx, p.total_units, fused_ctas_per_sm(M, GENERIC, FW));
 	if (GENERIC && fused_generic_item_words(p.G) == 1)
 		fused_stream_kernel<M, GENERIC, KT, GT, FW, STRIPED, SPLIT, GENERIC ? 1 : fused_item_words(M, GENERIC)><<<grid, fused_threads(M, GENERIC), smem, st>>>(map, p);
 	else
@@ -302,7 +322,7 @@ static int set_bs_attr() {
 }
 template <int M, int KT = 0, int GT = 0, bool STRIPED = false>
 static int launch_bs(lzgpu_ctx *ctx, const CUtensorMap &map, const FusedParams &p, size_t smem, cudaStream_t st) {
-	const int grid = static_cast<int>(std::min<uint64_t>(p.total_units, static_cast<uint64_t>(ctx->sm_count)));
+	const int grid = persistent_grid(ctx, p.total_units, 1);
 	fused_stream_kernel<M, false, KT, GT, 64, STRIPED, false, 8><<<grid, kBsThreads, smem, st>>>(map, p);
 	CUDA_TRY(cudaGetLastError());
 	ctx->stats.kernel_launches++;
@@ -591,7 +611,7 @@ int lz_fused_crc(lzgpu_ctx *ctx, const void *base, unsigned long long n_blocks, 
 // DIRECT form of the degraded read (any generator; the Cauchy codes): 16-warp CTA, runtime k, 16- or 4-byte items
 template <int E>
 static int launch_direct(lzgpu_ctx *ctx, const TmapArray &maps, const RecoverParams &p, size_t smem, cudaStream_t st, bool wide) {
-	const int grid = static_cast<int>(std::min<uint64_t>(p.total_units, static_cast<uint64_t>(ctx->sm_count)));
+	const int grid = persistent_grid(ctx, p.total_units, 1);
 	if (wide) fused_recover_kernel<E, 0, kRecoverDirect, -1, 64, 2, kDirectWide<E>><<<grid, recover_threads(2), smem, st>>>(maps, p);
 	else fused_recover_kernel<E, 0, kRecoverDirect, -1, 64, 2, 1><<<grid, recover_threads(2), smem, st>>>(maps, p);
 	CUDA_TRY(cudaGetLastError());
@@ -602,7 +622,7 @@ static int launch_direct(lzgpu_ctx *ctx, const TmapArray &maps, const RecoverPar
 // the 16-warp geometry alone (instantiations with a compile-time k other than 8: ec(3,2), the BASELINE configs[1] goal)
 template <int E, int KT, int R0, int R1>
 static int launch_recover_geo2(lzgpu_ctx *ctx, const TmapArray &maps, const RecoverParams &p, size_t smem, cudaStream_t st) {
-	const int gridb = static_cast<int>(std::min<uint64_t>(p.total_units, static_cast<uint64_t>(ctx->sm_count)));
+	const int gridb = persistent_grid(ctx, p.total_units, 1);
 	fused_recover_kernel<E, KT, R0, R1, 64, 2><<<gridb, recover_threads(2), smem, st>>>(maps, p);
 	CUDA_TRY(cudaGetLastError());
 	ctx->stats.kernel_launches++;
@@ -612,20 +632,20 @@ static int launch_recover_geo2(lzgpu_ctx *ctx, const TmapArray &maps, const Reco
 template <int E, int KT, int R0 = -1, int R1 = -1>
 static int launch_recover(lzgpu_ctx *ctx, const TmapArray &maps, const RecoverParams &p, size_t smem, cudaStream_t st, int geo) {
 	if (geo == 2) {
-		const int gridb = static_cast<int>(std::min<uint64_t>(p.total_units, static_cast<uint64_t>(ctx->sm_count)));
+		const int gridb = persistent_grid(ctx, p.total_units, 1);
 		fused_recover_kernel<E, KT, R0, R1, 64, 2><<<gridb, recover_threads(2), smem, st>>>(maps, p);
 		CUDA_TRY(cudaGetLastError());
 		ctx->stats.kernel_launches++;
 		return LZGPU_OK;
 	}
 	if (geo == 1 && E <= 2) {
-		const int grid2 = static_cast<int>(std::min<uint64_t>(p.total_units, static_cast<uint64_t>(ctx->sm_count) * 2));
+		const int grid2 = persistent_grid(ctx, p.total_units, 2);
 		fused_recover_kernel<(E <= 2 ? E : 1), KT, R0, R1, 64, 1><<<grid2, kFusedThreads, smem, st>>>(maps, p);
 		CUDA_TRY(cudaGetLastError());
 		ctx->stats.kernel_launches++;
 		return LZGPU_OK;
 	}
-	const int grid = static_cast<int>(std::min<uint64_t>(p.total_units, static_cast<uint64_t>(ctx->sm_count)));
+	const int grid = persistent_grid(ctx, p.total_units, 1);
 #ifdef LZ_ENABLE_FOLD128
 	if (ctx->fused->fold == 128) fused_recover_kernel<E, KT, R0, R1, 128><<<grid, kFusedThreads, smem, st>>>(maps, p);
 	else
@@ -855,7 +875,7 @@ int lz_fused_recover(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, 
 		bs_mask_set(mk.m[3], delta);
 		bs_mask_set(mk.m[4], A);
 		bs_mask_set(mk.m[5], lz::gf_mul_host(A, A));
-		const int grid = static_cast<int>(std::min<uint64_t>(p.total_units, static_cast<uint64_t>(ctx->sm_count)));
+		const int grid = persistent_grid(ctx, p.total_units, 1);
 		if (K == 5) bs_recover3_kernel<5><<<grid, kBsRecoverThreads, smem, st>>>(maps, p, mk);
 		else if (K == 8) bs_recover3_kernel<8><<<grid, kBsRecoverThreads, smem, st>>>(maps, p, mk);
 		else bs_recover3_kernel<0><<<grid, kBsRecoverThreads, smem, st>>>(maps, p, mk);
@@ -913,7 +933,7 @@ int lz_fused_recover(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, 
 // ---------------------------------------------------------------------------------------------------
 template <int M, int E>
 static int launch_convert(lzgpu_ctx *ctx, const TmapArray &maps, const ConvertParams &p, size_t smem, cudaStream_t st) {
-	const int grid = static_cast<int>(std::min<uint64_t>(p.total_units, static_cast<uint64_t>(ctx->sm_count) * 2));
+	const int grid = persistent_grid(ctx, p.total_units, 2);
 	if (M <= 2 && p.Kd == 3) fused_convert_kernel<(M <= 2 ? M : 1), E, 3><<<grid, kConvertThreads, smem, st>>>(maps, p);   // xor3 / ec(3,2) destinations
 	else fused_convert_kernel<M, E><<<grid, kConvertThreads, smem, st>>>(maps, p);
 	CUDA_TRY(cudaGetLastError());

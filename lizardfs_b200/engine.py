@@ -400,6 +400,13 @@ class Engine:
         self.lib.lzgpu_get_stats(self.h, C.byref(s))
         return {f[0]: getattr(s, f[0]) for f in LzStats._fields_}
 
+    def last_launch(self):
+        """(grid, units) of this context's most recent persistent kernel launch: CTAs launched and work units they shared
+        (lzgpu_debug_last_launch; (0, 0) before the first)"""
+        grid, units = C.c_uint32(), C.c_uint32()
+        _check(self.lib.lzgpu_debug_last_launch(self.h, C.byref(grid), C.byref(units)), "debug_last_launch")
+        return grid.value, units.value
+
     def sync(self):
         """waits for the device; in deferred-verification mode also collects the verdicts of the *_dev calls issued since the last
         sync and raises ChunkCrcError for the first mismatch"""
