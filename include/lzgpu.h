@@ -250,6 +250,9 @@ int lzgpu_recover_chunks_dev(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_
                              void *d_chunk_out, size_t chunk_out_stride,
                              int64_t *bad /* host, optional: chunk, part, block of the first mismatch */,
                              void *stream);
+/* Alignment (lzgpu_recover_chunks_dev, lzgpu_split_chunks_dev, lzgpu_convert_chunks_dev): every non-NULL part, output and image
+ * pointer must be 16-byte aligned and every non-NULL CRC array 4-byte aligned; strides are multiples of 16.  Otherwise the call
+ * returns LZGPU_ERR_ARG before anything is enqueued. */
 
 /* Wire-format producer (SURVEY.md §8 f3): LIZ_CLTOCS_WRITE_DATA packet prefixes (src/protocol/cltocs.h:116-137) for
  * every block of every part of the encoded chunks, built on the GPU straight from the CRC array of
@@ -273,6 +276,7 @@ int lzgpu_split_chunks(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks
                        const uint8_t *data, size_t chunk_stride, uint8_t *const *parts, size_t part_stride);
 int lzgpu_split_chunks_dev(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, uint32_t nb,
                            const void *d_data, size_t chunk_stride, void *const *d_parts, size_t part_stride, void *stream);
+                           /* d_data, d_parts[j]: 16-byte aligned (see lzgpu_recover_chunks_dev) */
 
 /* Replication / slice-type conversion (SURVEY.md §8 f1): rebuild parts of slice type `dst` from the available parts of
  * slice type `src`, one call for a batch of chunks.  Replaces, per part, SliceRecoveryPlanner's three methods
@@ -300,6 +304,7 @@ int lzgpu_convert_chunks_dev(lzgpu_ctx *ctx, const lzgpu_goal *src, const lzgpu_
                              const void *const *d_parts, size_t part_stride, const void *const *d_part_crc,
                              const uint8_t *want, void *const *d_out, size_t out_stride, void *const *d_out_crc,
                              int64_t *bad /* host; as in lzgpu_recover_chunks_dev */, void *stream);
+                             /* d_parts, d_out: 16-byte aligned; d_part_crc, d_out_crc: 4-byte aligned (see lzgpu_recover_chunks_dev) */
 
 /* CRC of n_blocks consecutive blocks of block_len bytes (block_len <= 65536, any value >= 1).
  * crc_out[i] = mycrc32(0, data + i*block_stride, block_len). */
@@ -401,7 +406,8 @@ void lzgpu_isal_ec_init_tables(int k, int rows, unsigned char *a, unsigned char 
 void lzgpu_isal_ec_encode_data(int len, int srcs, int dests, unsigned char *v, unsigned char **src, unsigned char **dest);
 
 /* Synthetic data generator used by bench / tests (device side): fills chunks with the splitmix64
- * counter stream documented in DESIGN.md §6 (same bytes as oracle lzo_fill_chunk). */
+ * counter stream documented in DESIGN.md §6 (same bytes as oracle lzo_fill_chunk).  d_data 8-byte aligned, chunk_len and
+ * chunk_stride multiples of 8 (LZGPU_ERR_ARG otherwise); the bytes between chunk_len and chunk_stride are not written. */
 int lzgpu_fill_chunks_dev(lzgpu_ctx *ctx, void *d_data, uint32_t n_chunks, size_t chunk_len,
                           size_t chunk_stride, uint64_t seed, uint64_t first_chunk_index, void *stream);
 

@@ -452,6 +452,19 @@ static int check_goal(const lzgpu_goal *g) {
 	return LZGPU_OK;
 }
 
+// Per-part pointer arrays of the recover / convert / split calls: every non-NULL buffer must be 16-byte aligned (the kernels load
+// and store up to 16 bytes at a time, and a misaligned base makes the fused route's tensor maps fail), every non-NULL CRC array
+// 4-byte aligned.  Checked before anything is enqueued.
+static int check_part_ptrs(const char *call, const char *what, const void *const *p, int n, uintptr_t align) {
+	if (!p) return LZGPU_OK;
+	for (int i = 0; i < n; ++i)
+		if (reinterpret_cast<uintptr_t>(p[i]) & (align - 1)) {
+			lz_set_error("%s: %s[%d] is not %u-byte aligned", call, what, i, static_cast<unsigned>(align));
+			return LZGPU_ERR_ARG;
+		}
+	return LZGPU_OK;
+}
+
 // parity coefficient rows of a goal: xorN is ec(N,1) (row of ones == plain XOR, chunk_writer.cc:373-381)
 static void goal_parity_rows(const lzgpu_goal *g, uint8_t *rows /* m*k */) {
 	uint8_t gen[LZGPU_MAX_PARTS * LZGPU_MAX_DATA];
@@ -644,6 +657,11 @@ static int recover_enqueue(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_ch
 		lz_set_error("recover: chunk_out_stride must cover nb blocks and be a multiple of 16");
 		return LZGPU_ERR_ARG;
 	}
+	int rc;
+	if ((rc = check_part_ptrs("recover", "parts", d_parts, n, 16)) || (rc = check_part_ptrs("recover", "out", d_out, n, 16)) ||
+	    (rc = check_part_ptrs("recover", "part_crc", d_part_crc, n, 4)))
+		return rc;
+	if (reinterpret_cast<uintptr_t>(d_chunk_out) & 15) { lz_set_error("recover: chunk_out is not 16-byte aligned"); return LZGPU_ERR_ARG; }
 
 	// ECReadPlan::recoverParts (ec_read_plan.h:126-133): the first k available parts are the inputs,
 	// everything else counts as erased.
@@ -661,7 +679,6 @@ static int recover_enqueue(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_ch
 		}
 	}
 	if (used < k) { lz_set_error("recover: only %d of %d required parts available", used, k); return LZGPU_ERR_TOO_FEW_PARTS; }
-	int rc;
 	if (any_crc) {
 		if ((rc = lz_status_acquire(ctx, &tk->slot))) return rc;
 		CUDA_TRY(cudaMemsetAsync(tk->slot.d, 0xff, sizeof(unsigned long long) * LZGPU_MAX_PARTS, st));
@@ -1053,6 +1070,10 @@ static int convert_enqueue(lzgpu_ctx *ctx, const lzgpu_goal *src, const lzgpu_go
 		lz_set_error("convert: strides too small or not multiples of 16");
 		return LZGPU_ERR_ARG;
 	}
+	const int ns = src->k + src->m;
+	if ((rc = check_part_ptrs("convert", "parts", d_parts, ns, 16)) || (rc = check_part_ptrs("convert", "out", d_out, nd, 16)) ||
+	    (rc = check_part_ptrs("convert", "part_crc", d_part_crc, ns, 4)) || (rc = check_part_ptrs("convert", "out_crc", d_out_crc, nd, 4)))
+		return rc;
 	for (int i = 0; i < nd; ++i)
 		if (want[i] && !d_out[i]) { lz_set_error("convert: wanted part %d has no output buffer", i); return LZGPU_ERR_ARG; }
 	TmpBuf t_image(ctx, st), t_par(ctx, st), t_crc(ctx, st), t_vcrc(ctx, st);
@@ -1406,6 +1427,8 @@ extern "C" int lzgpu_split_chunks_dev(lzgpu_ctx *ctx, const lzgpu_goal *goal, ui
 		lz_set_error("split: bad strides");
 		return LZGPU_ERR_ARG;
 	}
+	if (reinterpret_cast<uintptr_t>(d_data) & 15) { lz_set_error("split: data is not 16-byte aligned"); return LZGPU_ERR_ARG; }
+	if ((rc = check_part_ptrs("split", "parts", d_parts, static_cast<int>(k), 16))) return rc;
 	if (n_chunks == 0) return LZGPU_OK;
 	DeviceGuard g(ctx->device);
 	cudaStream_t st = stream ? static_cast<cudaStream_t>(stream) : ctx->stream;
@@ -1876,7 +1899,7 @@ extern "C" void lzgpu_recompute_crc_if_block_empty(const uint8_t *block, uint32_
 // ------------------------------------------------------------------------------------------------
 extern "C" int lzgpu_fill_chunks_dev(lzgpu_ctx *ctx, void *d_data, uint32_t n_chunks, size_t chunk_len, size_t chunk_stride, uint64_t seed,
                                       uint64_t first_chunk_index, void *stream) {
-	if (!ctx || !d_data || (chunk_len & 7) || (chunk_stride & 7)) return LZGPU_ERR_ARG;
+	if (!ctx || !d_data || (chunk_len & 7) || (chunk_stride & 7) || (reinterpret_cast<uintptr_t>(d_data) & 7)) return LZGPU_ERR_ARG;
 	DeviceGuard g(ctx->device);
 	cudaStream_t st = stream ? static_cast<cudaStream_t>(stream) : ctx->stream;
 	const unsigned long long wpc = chunk_len / 8, total = wpc * n_chunks;

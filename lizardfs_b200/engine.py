@@ -508,6 +508,11 @@ class Engine:
                "write_data_prefixes")
         return out
 
+    def write_data_prefixes_dev(self, goal, n_chunks, nb, d_crc, crc_stride, d_chunk_ids, d_out, write_id_base=0, stream=None):
+        """device-pointer form of write_data_prefixes: crc_stride in uint32 elements, d_out receives n_chunks*(k+m)*pb prefixes"""
+        _check(self.lib.lzgpu_write_data_prefixes_dev(self.h, C.byref(goal.c), n_chunks, nb, d_crc, crc_stride, d_chunk_ids, write_id_base,
+                                                      d_out, stream), "write_data_prefixes_dev")
+
     # ---- slice conversion ---------------------------------------------------------------------
     def split_chunks(self, goal, data, nb=None):
         """chunk order [n, nb*64K] -> list of k part-major data parts [n, pb*64K] (BlockConverter,
@@ -578,8 +583,12 @@ class Engine:
         do = (C.c_void_p * nd)(*[p if p else None for p in d_out])
         doc = (C.c_void_p * nd)(*[p if p else None for p in d_out_crc]) if d_out_crc is not None else None
         w = np.asarray(want, dtype=np.uint8)
-        _check(self.lib.lzgpu_convert_chunks_dev(self.h, C.byref(src.c), C.byref(dst.c), n_chunks, nb, dp, part_stride, dc, _p(w), do, out_stride,
-                                                 doc, None, stream), "convert_chunks_dev")
+        bad = (C.c_int64 * 3)(-1, -1, -1)
+        rc = self.lib.lzgpu_convert_chunks_dev(self.h, C.byref(src.c), C.byref(dst.c), n_chunks, nb, dp, part_stride, dc, _p(w), do, out_stride,
+                                               doc, bad, stream)
+        if rc == _lib.ERR_CRC:
+            raise ChunkCrcError(rc, "convert_chunks_dev", (bad[0], bad[1], bad[2]))
+        _check(rc, "convert_chunks_dev")
 
     # ---- CRC ---------------------------------------------------------------------------------
     def crc_blocks(self, data, block_len=BLOCK_SIZE, block_stride=None):
@@ -654,6 +663,12 @@ class Engine:
         if rc not in (_lib.OK, _lib.ERR_CRC, _lib.ERR_DAMAGED, _lib.ERR_ARG) or (rc == _lib.ERR_ARG and all(arr[i].status == 0 for i in range(n))):
             _check(rc, "write_blocks")
         return [arr[i].status for i in range(n)]
+
+    def write_blocks_dev(self, d_blocks, d_stored_crc, d_payload, d_writes, n_writes, sparse_rule=True, stream=None):
+        """device-pointer form of write_blocks: d_writes holds n_writes lzgpu_block_write records (_lib.LzBlockWrite) whose status
+        fields the kernel fills in; asynchronous, the per-request statuses are valid once the stream has passed the call"""
+        _check(self.lib.lzgpu_write_blocks_dev(self.h, d_blocks, d_stored_crc, d_payload, d_writes, n_writes, int(sparse_rule), stream),
+               "write_blocks_dev")
 
     # ---- device helpers ----------------------------------------------------------------------
     def fill_chunks_dev(self, d_data, n_chunks, chunk_len, chunk_stride, seed, first_chunk=0, stream=None):
