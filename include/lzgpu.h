@@ -162,6 +162,8 @@ void lzgpu_reset_stats(lzgpu_ctx *ctx);
  * launched last.  LZGPU_GRID_CAP=n in the environment when the context is created caps every such grid at n CTAs (testing:
  * every CTA then walks several units). */
 int lzgpu_debug_last_launch(lzgpu_ctx *ctx, uint32_t *grid, uint32_t *units);
+/* Diagnostics: verification result slots of the context — how many exist and how many a call holds right now (0 when no call runs). */
+int lzgpu_debug_status_slots(lzgpu_ctx *ctx, uint32_t *allocated, uint32_t *in_use);
 
 /* ---------------------------------------------------------------------------------------------
  * Device pool: several GPUs behind ONE process (the mount runs ten write workers in one process, src/mount/lizard_client.h:77,

@@ -71,6 +71,7 @@ SIGNATURES = {
     "lzgpu_get_stats": (None, [_vp, C.POINTER(LzStats)]),
     "lzgpu_reset_stats": (None, [_vp]),
     "lzgpu_debug_last_launch": (_int, [_vp, C.POINTER(_u32), C.POINTER(_u32)]),
+    "lzgpu_debug_status_slots": (_int, [_vp, C.POINTER(_u32), C.POINTER(_u32)]),
     "lzgpu_encode_chunks": (_int, [_vp, _goalp, _u32, _u32, _vp, _sz, _vp, _sz, _vp, _sz]),
     "lzgpu_encode_chunks_dev": (_int, [_vp, _goalp, _u32, _u32, _vp, _sz, _vp, _sz, _vp, _sz, _vp]),
     "lzgpu_recover_chunks": (_int, [_vp, _goalp, _u32, _u32, _vp, _sz, _vp, _vp, _vp, _vp, _sz, _vp]),

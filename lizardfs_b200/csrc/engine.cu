@@ -165,6 +165,8 @@ extern "C" void lzgpu_ctx_destroy(lzgpu_ctx *ctx) {
 	if (!ctx) return;
 	DeviceGuard g(ctx->device);
 	cudaDeviceSynchronize();
+	for (VerifyTicket &tk : ctx->pending) tk.take(nullptr);  // uncollected deferred verdicts: the device is idle, only the slots go back
+	ctx->pending.clear();
 	lz_fused_destroy(ctx);
 	for (auto &b : ctx->scratch) if (b.ptr) cudaFree(b.ptr);
 	if (ctx->d_crc_tables) cudaFree(ctx->d_crc_tables);
@@ -302,7 +304,7 @@ int TmpBuf::alloc(size_t bytes) {
 	return LZGPU_OK;
 }
 
-int lz_status_acquire(lzgpu_ctx *ctx, StatusSlot *out) {
+static int lz_status_acquire(lzgpu_ctx *ctx, StatusSlot *out) {
 	std::lock_guard<std::mutex> lk(ctx->slot_mu);
 	if (ctx->status_free.empty()) {
 		StatusSlot sl;
@@ -317,10 +319,90 @@ int lz_status_acquire(lzgpu_ctx *ctx, StatusSlot *out) {
 	return LZGPU_OK;
 }
 
-void lz_status_release(lzgpu_ctx *ctx, const StatusSlot &s) {
-	if (s.index < 0) return;
+static void lz_status_release(lzgpu_ctx *ctx, const StatusSlot &s) {
 	std::lock_guard<std::mutex> lk(ctx->slot_mu);
 	ctx->status_free.push_back(s.index);
+}
+
+extern "C" int lzgpu_debug_status_slots(lzgpu_ctx *ctx, uint32_t *allocated, uint32_t *in_use) {
+	if (!ctx || !allocated || !in_use) return LZGPU_ERR_ARG;
+	std::lock_guard<std::mutex> lk(ctx->slot_mu);
+	*allocated = static_cast<uint32_t>(ctx->status_all.size());
+	*in_use = static_cast<uint32_t>(ctx->status_all.size() - ctx->status_free.size());
+	return LZGPU_OK;
+}
+
+VerifyTicket &VerifyTicket::operator=(VerifyTicket &&o) noexcept {
+	if (this != &o) {
+		drop();
+		ctx_ = o.ctx_; st_ = o.st_; slot_ = o.slot_; fused_ = o.fused_; n_words_ = o.n_words_; blocks_ = o.blocks_;
+		o.slot_ = StatusSlot();
+	}
+	return *this;
+}
+
+int VerifyTicket::arm(lzgpu_ctx *ctx, cudaStream_t st) {
+	if (!armed()) {
+		int rc = lz_status_acquire(ctx, &slot_);
+		if (rc) return rc;
+		ctx_ = ctx;
+	}
+	st_ = st;
+	CUDA_TRY(cudaMemsetAsync(slot_.d, 0xff, sizeof(unsigned long long) * LZGPU_MAX_PARTS, st));
+	return LZGPU_OK;
+}
+
+int VerifyTicket::publish(bool fused, int n_words, uint32_t blocks) {
+	fused_ = fused;
+	n_words_ = n_words;
+	blocks_ = blocks;
+	CUDA_TRY(cudaMemcpyAsync(slot_.h, slot_.d, sizeof(unsigned long long) * n_words, cudaMemcpyDeviceToHost, st_));
+	return LZGPU_OK;
+}
+
+int VerifyTicket::take(int64_t *bad) {
+	if (!armed()) return LZGPU_OK;
+	long long best_chunk = -1, best_part = -1, best_block = -1;
+	if (fused_) {
+		const unsigned long long v = slot_.h[0];
+		if (v != ~0ull) {
+			best_chunk = static_cast<long long>(v / (64ull * 1024ull));
+			best_part = static_cast<long long>((v / 1024ull) % 64ull);
+			best_block = static_cast<long long>(v % 1024ull);
+		}
+	} else {
+		for (int i = 0; i < n_words_; ++i) {
+			const unsigned long long v = slot_.h[i];
+			if (v == ~0ull) continue;
+			const long long c = static_cast<long long>(v / blocks_), b = static_cast<long long>(v % blocks_);
+			if (best_chunk < 0 || c < best_chunk || (c == best_chunk && i < best_part)) { best_chunk = c; best_part = i; best_block = b; }
+		}
+	}
+	lz_status_release(ctx_, slot_);
+	slot_ = StatusSlot();
+	if (best_chunk < 0) return LZGPU_OK;
+	if (bad) { bad[0] = best_chunk; bad[1] = best_part; bad[2] = best_block; }
+	lz_set_error("CRC mismatch: chunk %lld part %lld block %lld", best_chunk, best_part, best_block);
+	return LZGPU_ERR_CRC;
+}
+
+int VerifyTicket::wait_take(int64_t *bad) {
+	if (!armed()) return LZGPU_OK;
+	cudaError_t e = cudaStreamSynchronize(st_);
+	if (e != cudaSuccess) {
+		cudaGetLastError();
+		lz_set_error("CUDA error %s while waiting for the verification result", cudaGetErrorName(e));
+		return LZGPU_ERR_CUDA;  // the slot goes back when the owner is destroyed
+	}
+	return take(bad);
+}
+
+void VerifyTicket::drop() {
+	if (!armed()) return;
+	cudaStreamSynchronize(st_);  // the memset, the compare kernels and the copy of the words must be done with the slot
+	cudaGetLastError();
+	lz_status_release(ctx_, slot_);
+	slot_ = StatusSlot();
 }
 
 // staging buffers of the host-pointer entry points, grown on demand and kept (slot = purpose; callers hold ctx->mu)
@@ -344,6 +426,44 @@ int lz_scratch(lzgpu_ctx *ctx, int slot, size_t bytes, void **out) {
 	}
 	*out = b.ptr;
 	return LZGPU_OK;
+}
+
+// The tile pipeline of the host-pointer entry points: tile t of `tile` items (chunks or blocks) runs on slot t % n_slots, with
+// that slot's stream and the caller's staging buffers for it, so the H2D copies of one tile overlap the kernels of the previous
+// and the D2H copies of the one before.  stage(slot, first, count, stream, owner) enqueues one tile and arms `owner` when the
+// tile verifies stored CRCs.  Stream order alone keeps a slot's staging buffers safe to re-use; a slot whose tile armed a
+// verification is waited for and its verdict taken before the slot is re-used, and at the end every slot is retired oldest
+// first, so the first CRC mismatch of the batch is the one reported (bad[0]: the chunk's index in the whole batch).  Every
+// stream that was used is idle when the call returns, after an error too.
+template <class Stage>
+static int run_tiles(lzgpu_ctx *ctx, size_t n_items, size_t tile, int n_slots, int64_t *bad, Stage &&stage) {
+	VerifyTicket tk[kHostSlots];
+	size_t first[kHostSlots] = {};
+	auto retire = [&](int s) {
+		int64_t local[3];
+		const int rc = tk[s].wait_take(local);
+		if (rc == LZGPU_ERR_CRC && bad) { bad[0] = local[0] + static_cast<int64_t>(first[s]); bad[1] = local[1]; bad[2] = local[2]; }
+		return rc;
+	};
+	int rc = LZGPU_OK;
+	size_t t = 0;
+	for (size_t i0 = 0; i0 < n_items && !rc; i0 += tile, ++t) {
+		const int s = static_cast<int>(t % n_slots);
+		if ((rc = retire(s))) break;
+		first[s] = i0;
+		rc = stage(s, i0, std::min(tile, n_items - i0), ctx->slot_stream[s], &tk[s]);
+	}
+	const int used = static_cast<int>(std::min<size_t>(t, n_slots));
+	for (int i = 0; i < used && !rc; ++i) rc = retire(static_cast<int>((t + i) % used));
+	for (int s = 0; s < used; ++s) {
+		const cudaError_t e = cudaStreamSynchronize(ctx->slot_stream[s]);
+		if (e != cudaSuccess && !rc) {
+			lz_set_error("CUDA error %s in the host pipeline", cudaGetErrorName(e));
+			rc = LZGPU_ERR_CUDA;
+		}
+	}
+	cudaGetLastError();
+	return rc;
 }
 
 static int grid_for(const lzgpu_ctx *ctx, unsigned long long work_items, int threads, int ctas_per_sm) {
@@ -579,8 +699,6 @@ extern "C" int lzgpu_encode_chunks(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint3
 	pin.add(data, static_cast<size_t>(n_chunks - 1) * chunk_stride + chunk_len);
 	pin.add(parity, static_cast<size_t>(n_chunks - 1) * parity_stride + par_bytes);
 	pin.add(crc, (static_cast<size_t>(n_chunks - 1) * crc_stride + n_crc) * 4);
-	// slot pipeline: tile t uses slot t % kHostSlots with its own stream, so the H2D of one tile overlaps the
-	// kernel of the previous and the D2H of the one before (both copy engines + compute busy).
 	const size_t d_chunk_stride = static_cast<size_t>(nb) * B;
 	const size_t d_crc_stride = (n_crc + 3) & ~size_t(3);
 	const uint32_t tile = std::max<uint32_t>(1, std::min<uint32_t>(n_chunks, kHostTileBytes / LZGPU_CHUNK_SIZE));
@@ -590,61 +708,48 @@ extern "C" int lzgpu_encode_chunks(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint3
 		if ((rc = lz_scratch(ctx, kScratchPar0 + s, tile * par_bytes, &d_par[s]))) return rc;
 		if ((rc = lz_scratch(ctx, kScratchCrc0 + s, tile * d_crc_stride * 4, &d_c[s]))) return rc;
 	}
-	for (uint32_t c0 = 0, t = 0; c0 < n_chunks; c0 += tile, ++t) {
-		const uint32_t n = std::min(tile, n_chunks - c0);
-		const int s = t % kHostSlots;
-		cudaStream_t st = ctx->slot_stream[s];
-		CUDA_TRY(cudaMemcpy2DAsync(d_in[s], d_chunk_stride, data + static_cast<size_t>(c0) * chunk_stride, chunk_stride, chunk_len, n,
-		                           cudaMemcpyHostToDevice, st));
-		rc = lzgpu_encode_chunks_dev(ctx, goal, n, chunk_len, d_in[s], d_chunk_stride, d_par[s], par_bytes, d_c[s], d_crc_stride, st);
+	return run_tiles(ctx, n_chunks, tile, kHostSlots, nullptr, [&](int s, size_t c0, size_t n, cudaStream_t st, VerifyTicket *) -> int {
+		CUDA_TRY(cudaMemcpy2DAsync(d_in[s], d_chunk_stride, data + c0 * chunk_stride, chunk_stride, chunk_len, n, cudaMemcpyHostToDevice, st));
+		int rc = lzgpu_encode_chunks_dev(ctx, goal, static_cast<uint32_t>(n), chunk_len, d_in[s], d_chunk_stride, d_par[s], par_bytes, d_c[s],
+		                                 d_crc_stride, st);
 		if (rc) return rc;
-		CUDA_TRY(cudaMemcpy2DAsync(parity + static_cast<size_t>(c0) * parity_stride, parity_stride, d_par[s], par_bytes, par_bytes, n,
-		                           cudaMemcpyDeviceToHost, st));
-		CUDA_TRY(cudaMemcpy2DAsync(crc + static_cast<size_t>(c0) * crc_stride, crc_stride * 4, d_c[s], d_crc_stride * 4, n_crc * 4, n,
-		                           cudaMemcpyDeviceToHost, st));
+		CUDA_TRY(cudaMemcpy2DAsync(parity + c0 * parity_stride, parity_stride, d_par[s], par_bytes, par_bytes, n, cudaMemcpyDeviceToHost, st));
+		CUDA_TRY(cudaMemcpy2DAsync(crc + c0 * crc_stride, crc_stride * 4, d_c[s], d_crc_stride * 4, n_crc * 4, n, cudaMemcpyDeviceToHost, st));
 		ctx->stats.bytes_h2d += static_cast<uint64_t>(n) * chunk_len;
 		ctx->stats.bytes_d2h += static_cast<uint64_t>(n) * (par_bytes + n_crc * 4);
-	}
-	for (auto &ss : ctx->slot_stream) CUDA_TRY(cudaStreamSynchronize(ss));
-	return LZGPU_OK;
+		return LZGPU_OK;
+	});
 }
 
 // ------------------------------------------------------------------------------------------------
 // batched recover
 // ------------------------------------------------------------------------------------------------
-// after the stream of the call has been synchronised: LZGPU_OK or LZGPU_ERR_CRC (+ first bad chunk / part / block); returns the slot
-static int ticket_result(lzgpu_ctx *ctx, VerifyTicket *tk, int64_t *bad) {
-	if (!tk->active()) return LZGPU_OK;
-	long long best_chunk = -1, best_part = -1, best_block = -1;
-	if (tk->fused) {
-		const unsigned long long v = tk->slot.h[0];
-		if (v != ~0ull) {
-			best_chunk = static_cast<long long>(v / (64ull * 1024ull));
-			best_part = static_cast<long long>((v / 1024ull) % 64ull);
-			best_block = static_cast<long long>(v % 1024ull);
-		}
+static int crc_of_parts(lzgpu_ctx *ctx, const void *d_part, uint32_t n_chunks, uint32_t pb, size_t stride, void *d_out, cudaStream_t st) {
+	const unsigned long long nblk = static_cast<unsigned long long>(n_chunks) * pb;
+	int rc = lz_fused_crc(ctx, d_part, nblk, pb, stride, d_out, pb, st);
+	if (rc == LZGPU_NOT_HANDLED) rc = lz_crc_blocks(ctx, d_part, nblk, pb, stride, LZGPU_BLOCK_SIZE, LZGPU_BLOCK_SIZE, d_out, pb, st);
+	return rc;
+}
+
+// Checks the n_chunks x pb stored CRCs of one part against its blocks; the first mismatch (chunk*pb + block) lowers *d_word.
+// d_tmp holds the computed CRCs.  With CRCs disabled a stored CRC is valid iff it is the constant, and the blocks are not read.
+static int verify_part(lzgpu_ctx *ctx, const void *d_part, uint32_t n_chunks, uint32_t pb, size_t stride, const void *d_stored, void *d_tmp,
+                       unsigned long long *d_word, cudaStream_t st) {
+	const unsigned long long nblk = static_cast<unsigned long long>(n_chunks) * pb;
+	if (!lzgpu_crc_enabled()) {
+		crc_compare_const_kernel<<<grid_for(ctx, nblk, 256, 4), 256, 0, st>>>(static_cast<const uint32_t *>(d_stored), nblk, LZGPU_FAKE_CRC, 0, d_word);
 	} else {
-		for (int i = 0; i < tk->n_words; ++i) {
-			const unsigned long long v = tk->slot.h[i];
-			if (v == ~0ull) continue;
-			const long long c = static_cast<long long>(v / tk->blocks), b = static_cast<long long>(v % tk->blocks);
-			if (best_chunk < 0 || c < best_chunk || (c == best_chunk && i < best_part)) { best_chunk = c; best_part = i; best_block = b; }
-		}
+		int rc = crc_of_parts(ctx, d_part, n_chunks, pb, stride, d_tmp, st);
+		if (rc) return rc;
+		crc_compare_kernel<<<grid_for(ctx, nblk, 256, 4), 256, 0, st>>>(static_cast<const uint32_t *>(d_tmp), static_cast<const uint32_t *>(d_stored),
+		                                                              nblk, kCrcZeroBlock64K, 0, 0, d_word);
 	}
-	lz_status_release(ctx, tk->slot);
-	tk->slot.index = -1;
-	if (best_chunk < 0) return LZGPU_OK;
-	if (bad) { bad[0] = best_chunk; bad[1] = best_part; bad[2] = best_block; }
-	lz_set_error("CRC mismatch: chunk %lld part %lld block %lld", best_chunk, best_part, best_block);
-	return LZGPU_ERR_CRC;
+	CUDA_TRY(cudaGetLastError());
+	ctx->stats.kernel_launches++;
+	return LZGPU_OK;
 }
 
-static void ticket_drop(lzgpu_ctx *ctx, VerifyTicket *tk) {
-	if (tk->active()) lz_status_release(ctx, tk->slot);
-	tk->slot.index = -1;
-}
-
-// enqueue the whole degraded read on `st` without synchronising; *tk describes the pending verification (if any)
+// enqueue the whole degraded read on `st` without synchronising; *tk is armed when stored CRCs of the parts read are verified
 static int recover_enqueue(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, uint32_t nb, const void *const *d_parts, size_t part_stride,
                            const void *const *d_part_crc, const uint8_t *want, void *const *d_out, void *d_chunk_out, size_t chunk_out_stride,
                            cudaStream_t st, VerifyTicket *tk) {
@@ -679,57 +784,36 @@ static int recover_enqueue(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_ch
 		}
 	}
 	if (used < k) { lz_set_error("recover: only %d of %d required parts available", used, k); return LZGPU_ERR_TOO_FEW_PARTS; }
-	if (any_crc) {
-		if ((rc = lz_status_acquire(ctx, &tk->slot))) return rc;
-		CUDA_TRY(cudaMemsetAsync(tk->slot.d, 0xff, sizeof(unsigned long long) * LZGPU_MAX_PARTS, st));
-	}
+	if (any_crc && (rc = tk->arm(ctx, st))) return rc;
+	// every part that is read and has stored CRCs, one result word each
+	TmpBuf tmp_crc(ctx, st);
+	auto verify_inputs = [&]() -> int {
+		int r;
+		for (int i = 0; i < n; ++i)
+			if (!erased[i] && d_part_crc[i] &&
+			    (r = verify_part(ctx, d_parts[i], n_chunks, pb, part_stride, d_part_crc[i], tmp_crc.p, tk->word(i), st)))
+				return r;
+		return LZGPU_OK;
+	};
 	const void *const *crc_for_kernels = d_part_crc;
 	if (any_crc && !lzgpu_crc_enabled()) {
-		// CRC-disabled build mode: a stored CRC is valid iff it is the constant; the kernels then run without verification
-		const unsigned long long nblk = static_cast<unsigned long long>(n_chunks) * pb;
-		for (int i = 0; i < n; ++i) {
-			if (erased[i] || !d_part_crc[i]) continue;
-			crc_compare_const_kernel<<<grid_for(ctx, nblk, 256, 4), 256, 0, st>>>(static_cast<const uint32_t *>(d_part_crc[i]), nblk, LZGPU_FAKE_CRC, 0, tk->slot.d + i);
-			CUDA_TRY(cudaGetLastError());
-			ctx->stats.kernel_launches++;
-		}
+		// CRC-disabled build mode: the constant is checked here, before either route; the kernels then run without verification
+		if ((rc = verify_inputs())) return rc;
 		crc_for_kernels = nullptr;
 	}
 
 	// 0. fused route: verify + rebuild the erased data parts + chunk-order image in one pass over the inputs
-	{
-		bool fused_verifying = false;
-		rc = lz_fused_recover(ctx, goal, n_chunks, nb, d_parts, part_stride, crc_for_kernels, want, d_out, d_chunk_out, chunk_out_stride, st,
-		                      tk->slot.d, &fused_verifying);
-		if (rc != LZGPU_NOT_HANDLED) {
-			if (rc) { ticket_drop(ctx, tk); return rc; }
-			ctx->stats.chunks_recovered += n_chunks;
-			if (any_crc) {
-				tk->fused = crc_for_kernels != nullptr;
-				tk->n_words = tk->fused ? 1 : n;
-				tk->blocks = pb;
-				CUDA_TRY(cudaMemcpyAsync(tk->slot.h, tk->slot.d, sizeof(unsigned long long) * tk->n_words, cudaMemcpyDeviceToHost, st));
-			}
-			return LZGPU_OK;
-		}
+	rc = lz_fused_recover(ctx, goal, n_chunks, nb, d_parts, part_stride, crc_for_kernels, want, d_out, d_chunk_out, chunk_out_stride, st, tk->word(0));
+	if (rc != LZGPU_NOT_HANDLED) {
+		if (rc) return rc;
+		ctx->stats.chunks_recovered += n_chunks;
+		if (!any_crc) return LZGPU_OK;
+		return crc_for_kernels ? tk->publish_fused() : tk->publish_per_part(n, pb);
 	}
 
 	// 1. verify the stored CRC of every block of every part that is read
-	TmpBuf tmp_crc(ctx, st);
 	if (any_crc && crc_for_kernels) {
-		const unsigned long long nblk = static_cast<unsigned long long>(n_chunks) * pb;
-		if ((rc = tmp_crc.alloc(nblk * 4))) { ticket_drop(ctx, tk); return rc; }
-		for (int i = 0; i < n; ++i) {
-			if (erased[i] || !d_part_crc[i]) continue;
-			rc = lz_fused_crc(ctx, d_parts[i], nblk, pb, part_stride, tmp_crc.p, pb, st);
-			if (rc == LZGPU_NOT_HANDLED) rc = lz_crc_blocks(ctx, d_parts[i], nblk, pb, part_stride, B, B, tmp_crc.p, pb, st);
-			if (rc) { ticket_drop(ctx, tk); return rc; }
-			crc_compare_kernel<<<grid_for(ctx, nblk, 256, 4), 256, 0, st>>>(static_cast<const uint32_t *>(tmp_crc.p),
-			                                                              static_cast<const uint32_t *>(d_part_crc[i]), nblk,
-			                                                              kCrcZeroBlock64K, 0, 0, tk->slot.d + i);
-			CUDA_TRY(cudaGetLastError());
-			ctx->stats.kernel_launches++;
-		}
+		if ((rc = tmp_crc.alloc(static_cast<size_t>(n_chunks) * pb * 4)) || (rc = verify_inputs())) return rc;
 	}
 
 	// 2. rebuild the wanted parts
@@ -743,7 +827,7 @@ static int recover_enqueue(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_ch
 		if (!o) {
 			if (!(d_chunk_out && i < k)) continue;  // not requested anywhere
 			tmp_owned.emplace_back(new TmpBuf(ctx, st));
-			if ((rc = tmp_owned.back()->alloc(static_cast<size_t>(n_chunks) * part_stride))) { ticket_drop(ctx, tk); return rc; }
+			if ((rc = tmp_owned.back()->alloc(static_cast<size_t>(n_chunks) * part_stride))) return rc;
 			o = tmp_owned.back()->p;
 			tmp_parts[i] = o;
 		}
@@ -758,7 +842,6 @@ static int recover_enqueue(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_ch
 		int nrows = lz::rs_recovery_matrix(k, m, erased, wanted, rows, &singular);
 		if (nrows != static_cast<int>(dst.size())) {
 			lz_set_error(singular ? "recover: decode matrix is singular" : "recover: bad erasure pattern");
-			ticket_drop(ctx, tk);
 			return LZGPU_ERR_ARG;
 		}
 		DotDesc d{};
@@ -773,7 +856,7 @@ static int recover_enqueue(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_ch
 		d.dst_block_stride = B;
 		d.units_per_block = B / 16;
 		d.blocks_per_chunk = pb;
-		if ((rc = lz_gf_dot(ctx, d, rows, st))) { ticket_drop(ctx, tk); return rc; }
+		if ((rc = lz_gf_dot(ctx, d, rows, st))) return rc;
 	}
 
 	// 3. optional chunk-order image (BlockConverter, chunk_read_planner.h:36-70)
@@ -794,13 +877,7 @@ static int recover_enqueue(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_ch
 		ctx->stats.kernel_launches++;
 	}
 	ctx->stats.chunks_recovered += n_chunks;
-	if (any_crc) {
-		tk->fused = false;
-		tk->n_words = n;
-		tk->blocks = pb;
-		CUDA_TRY(cudaMemcpyAsync(tk->slot.h, tk->slot.d, sizeof(unsigned long long) * n, cudaMemcpyDeviceToHost, st));
-	}
-	return LZGPU_OK;
+	return any_crc ? tk->publish_per_part(n, pb) : LZGPU_OK;
 }
 
 static int recover_check_args(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t nb, const void *parts, const uint8_t *want) {
@@ -820,6 +897,17 @@ static uint64_t recover_alg_bytes(const lzgpu_goal *goal, uint32_t n_chunks, uin
 	return n_chunks * (goal->k * pb * B + (crcs ? 4ull * goal->k * pb : 0) + out_parts * pb * B + (image ? static_cast<uint64_t>(nb) * B : 0));
 }
 
+// The verdict of a *_dev call: collected by lzgpu_dev_sync in deferred mode, otherwise waited for and reported by the call itself
+// (with or without `bad`) whenever stored CRCs were verified.
+static int dev_verdict(lzgpu_ctx *ctx, VerifyTicket &&tk, int64_t *bad) {
+	if (tk.armed() && ctx->deferred_verify.load()) {
+		std::lock_guard<std::mutex> lk(ctx->pending_mu);
+		ctx->pending.push_back(std::move(tk));
+		return LZGPU_OK;
+	}
+	return tk.wait_take(bad);
+}
+
 extern "C" int lzgpu_recover_chunks_dev(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, uint32_t nb,
                                          const void *const *d_parts, size_t part_stride, const void *const *d_part_crc,
                                          const uint8_t *want, void *const *d_out, void *d_chunk_out, size_t chunk_out_stride,
@@ -836,55 +924,7 @@ extern "C" int lzgpu_recover_chunks_dev(lzgpu_ctx *ctx, const lzgpu_goal *goal, 
 		if ((rc = recover_enqueue(ctx, goal, n_chunks, nb, d_parts, part_stride, d_part_crc, want, d_out, d_chunk_out, chunk_out_stride, st, &tk)))
 			return rc;
 	}
-	if (!tk.active()) return LZGPU_OK;
-	if (ctx->deferred_verify.load()) {  // the verdict is collected by lzgpu_dev_sync
-		std::lock_guard<std::mutex> lk(ctx->pending_mu);
-		ctx->pending.push_back(tk);
-		return LZGPU_OK;
-	}
-	// stored CRCs were supplied: the call reports their verdict itself (with or without `bad`)
-	cudaError_t e = cudaStreamSynchronize(st);
-	if (e != cudaSuccess) {
-		ticket_drop(ctx, &tk);
-		cudaGetLastError();
-		lz_set_error("CUDA error %s while waiting for the verification result", cudaGetErrorName(e));
-		return LZGPU_ERR_CUDA;
-	}
-	return ticket_result(ctx, &tk, bad);
-}
-
-// Host-pointer pipelines: tile t runs on slot t % kHostSlots with its own stream and staging buffers, so the H2D copies of one
-// tile overlap the kernels of the previous and the D2H copies of the one before.  Tiles are retired in order (stream
-// synchronised, verification result read) before their slot is re-used, so the first CRC mismatch of the batch is the one reported.
-struct SlotState {
-	VerifyTicket tk;
-	uint32_t c0 = 0;
-	bool busy = false;
-};
-
-static int retire_slot(lzgpu_ctx *ctx, int s, SlotState *ss, int64_t *bad) {
-	if (!ss->busy) return LZGPU_OK;
-	ss->busy = false;
-	cudaError_t e = cudaStreamSynchronize(ctx->slot_stream[s]);
-	if (e != cudaSuccess) {
-		ticket_drop(ctx, &ss->tk);
-		cudaGetLastError();
-		lz_set_error("CUDA error %s in the host pipeline", cudaGetErrorName(e));
-		return LZGPU_ERR_CUDA;
-	}
-	int64_t local[3] = {-1, -1, -1};
-	int rc = ticket_result(ctx, &ss->tk, local);
-	if (rc == LZGPU_ERR_CRC && bad) { bad[0] = local[0] + ss->c0; bad[1] = local[1]; bad[2] = local[2]; }
-	return rc;
-}
-
-static void drain_slots(lzgpu_ctx *ctx, SlotState *ss) {
-	for (int s = 0; s < kHostSlots; ++s) {
-		cudaStreamSynchronize(ctx->slot_stream[s]);
-		ticket_drop(ctx, &ss[s].tk);
-		ss[s].busy = false;
-	}
-	cudaGetLastError();
+	return dev_verdict(ctx, std::move(tk), bad);
 }
 
 extern "C" int lzgpu_recover_chunks(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, uint32_t nb,
@@ -920,26 +960,19 @@ extern "C" int lzgpu_recover_chunks(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint
 		if ((rc = lz_scratch(ctx, kScratchCrc0 + s, dev_crc * n, &d_crc_all[s]))) return rc;
 		if (chunk_out && (rc = lz_scratch(ctx, kScratchPar0 + s, static_cast<size_t>(tile) * nb * B, &d_img[s]))) return rc;
 	}
-	SlotState ss[kHostSlots];
-	uint32_t t = 0;
-	for (uint32_t c0 = 0; c0 < n_chunks; c0 += tile, ++t) {
-		const uint32_t nc = std::min(tile, n_chunks - c0);
-		const int s = static_cast<int>(t % n_slots);
-		if ((rc = retire_slot(ctx, s, &ss[s], bad))) { drain_slots(ctx, ss); return rc; }
-		cudaStream_t st = ctx->slot_stream[s];
+	return run_tiles(ctx, n_chunks, tile, n_slots, bad, [&](int s, size_t c0, size_t nc, cudaStream_t st, VerifyTicket *tk) -> int {
 		std::vector<const void *> dp(n, nullptr), dc(n, nullptr);
 		std::vector<void *> dout(n, nullptr);
 		bool any_crc = false;
 		for (int i = 0; i < n; ++i) {
 			uint8_t *slot = static_cast<uint8_t *>(d_all[s]) + dev_part * i;
 			if (parts[i]) {
-				CUDA_TRY(cudaMemcpy2DAsync(slot, part_bytes, parts[i] + static_cast<size_t>(c0) * part_stride, part_stride, part_bytes, nc,
-				                           cudaMemcpyHostToDevice, st));
+				CUDA_TRY(cudaMemcpy2DAsync(slot, part_bytes, parts[i] + c0 * part_stride, part_stride, part_bytes, nc, cudaMemcpyHostToDevice, st));
 				ctx->stats.bytes_h2d += static_cast<uint64_t>(nc) * part_bytes;
 				dp[i] = slot;
 				if (part_crc && part_crc[i]) {
 					uint8_t *cs = static_cast<uint8_t *>(d_crc_all[s]) + dev_crc * i;
-					CUDA_TRY(cudaMemcpyAsync(cs, part_crc[i] + static_cast<size_t>(c0) * pb, static_cast<size_t>(nc) * pb * 4, cudaMemcpyHostToDevice, st));
+					CUDA_TRY(cudaMemcpyAsync(cs, part_crc[i] + c0 * pb, nc * pb * 4, cudaMemcpyHostToDevice, st));
 					dc[i] = cs;
 					any_crc = true;
 				}
@@ -947,33 +980,26 @@ extern "C" int lzgpu_recover_chunks(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint
 				dout[i] = slot;
 			}
 		}
-		ss[s].c0 = c0;
+		int rc;
 		{
-			BatchTimer timer(ctx, st, recover_alg_bytes(goal, nc, nb, dp.data(), want, chunk_out != nullptr, any_crc));
-			rc = recover_enqueue(ctx, goal, nc, nb, dp.data(), part_bytes, any_crc ? dc.data() : nullptr, want, dout.data(), d_img[s],
-			                     static_cast<size_t>(nb) * B, st, &ss[s].tk);
+			BatchTimer timer(ctx, st, recover_alg_bytes(goal, static_cast<uint32_t>(nc), nb, dp.data(), want, chunk_out != nullptr, any_crc));
+			rc = recover_enqueue(ctx, goal, static_cast<uint32_t>(nc), nb, dp.data(), part_bytes, any_crc ? dc.data() : nullptr, want, dout.data(),
+			                     d_img[s], static_cast<size_t>(nb) * B, st, tk);
 		}
-		if (rc) { drain_slots(ctx, ss); return rc; }
-		ss[s].busy = true;
+		if (rc) return rc;
 		for (int i = 0; i < n; ++i) {
 			if (dout[i] && out && out[i] && want[i] && !parts[i]) {
-				CUDA_TRY(cudaMemcpy2DAsync(out[i] + static_cast<size_t>(c0) * part_stride, part_stride, dout[i], part_bytes, part_bytes, nc,
-				                           cudaMemcpyDeviceToHost, st));
+				CUDA_TRY(cudaMemcpy2DAsync(out[i] + c0 * part_stride, part_stride, dout[i], part_bytes, part_bytes, nc, cudaMemcpyDeviceToHost, st));
 				ctx->stats.bytes_d2h += static_cast<uint64_t>(nc) * part_bytes;
 			}
 		}
 		if (chunk_out) {
-			CUDA_TRY(cudaMemcpy2DAsync(chunk_out + static_cast<size_t>(c0) * chunk_out_stride, chunk_out_stride, d_img[s], static_cast<size_t>(nb) * B,
+			CUDA_TRY(cudaMemcpy2DAsync(chunk_out + c0 * chunk_out_stride, chunk_out_stride, d_img[s], static_cast<size_t>(nb) * B,
 			                           static_cast<size_t>(nb) * B, nc, cudaMemcpyDeviceToHost, st));
 			ctx->stats.bytes_d2h += static_cast<uint64_t>(nc) * nb * B;
 		}
-	}
-	// retire what is still in flight, oldest tile first
-	for (uint32_t i = 0; i < static_cast<uint32_t>(n_slots); ++i) {
-		const int s = static_cast<int>((t + i) % n_slots);
-		if ((rc = retire_slot(ctx, s, &ss[s], bad))) { drain_slots(ctx, ss); return rc; }
-	}
-	return LZGPU_OK;
+		return LZGPU_OK;
+	});
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -982,13 +1008,6 @@ extern "C" int lzgpu_recover_chunks(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint
 static bool goal_is_std(const lzgpu_goal *g) { return g && g->kind == LZGPU_KIND_STD && g->k == 1 && g->m == 0; }
 static int check_goal_or_std(const lzgpu_goal *g) { return goal_is_std(g) ? LZGPU_OK : check_goal(g); }
 static bool same_goal(const lzgpu_goal *a, const lzgpu_goal *b) { return a->kind == b->kind && a->k == b->k && a->m == b->m; }
-
-static int crc_of_parts(lzgpu_ctx *ctx, const void *d_part, uint32_t n_chunks, uint32_t pb, size_t stride, void *d_out, cudaStream_t st) {
-	const unsigned long long nblk = static_cast<unsigned long long>(n_chunks) * pb;
-	int rc = lz_fused_crc(ctx, d_part, nblk, pb, stride, d_out, pb, st);
-	if (rc == LZGPU_NOT_HANDLED) rc = lz_crc_blocks(ctx, d_part, nblk, pb, stride, LZGPU_BLOCK_SIZE, LZGPU_BLOCK_SIZE, d_out, pb, st);
-	return rc;
-}
 
 static int convert_check_args(lzgpu_ctx *ctx, const lzgpu_goal *src, const lzgpu_goal *dst, uint32_t nb, const void *parts, const uint8_t *want,
                               const void *out) {
@@ -999,16 +1018,15 @@ static int convert_check_args(lzgpu_ctx *ctx, const lzgpu_goal *src, const lzgpu
 	return LZGPU_OK;
 }
 
-// everything enqueued on `st`, nothing synchronised; *tk = pending verification of the source parts (if any)
 // The one-pass route of a slice conversion.  Handled (lz_fused_convert): sources on a Vandermonde generator with at most two data
 // parts lost (their parity rows 0, 1 in use), destinations with up to three parity parts, at least one parity part wanted (data
 // parts alone are BlockConverter picks, served by the degraded read + split).  LZGPU_OK: every wanted part is enqueued, *t_crc
-// holds the destination slice's block CRCs in chunk order and *tk the pending verification; LZGPU_NOT_HANDLED: nothing was enqueued.
+// holds the destination slice's block CRCs in chunk order and *tk the pending verification; LZGPU_NOT_HANDLED: no part was written.
 static int try_fused_convert(lzgpu_ctx *ctx, const lzgpu_goal *src, const lzgpu_goal *dst, uint32_t n_chunks, uint32_t nb, const void *const *d_parts,
                              size_t part_stride, const void *const *d_part_crc, const uint8_t *want, void *const *d_out, size_t out_stride,
                              cudaStream_t st, VerifyTicket *tk, TmpBuf *t_crc, size_t *crc_stride_out) {
 	const int ks = src->k, kd = dst->k, nd = dst->k + dst->m;
-	const uint32_t pbs = (nb + ks - 1) / ks, pbd = (nb + kd - 1) / kd;
+	const uint32_t pbd = (nb + kd - 1) / kd;
 	bool any_crc = false, parity_wanted = false;
 	int used = 0;
 	for (int i = 0; i < ks + src->m && used < ks; ++i)
@@ -1019,8 +1037,7 @@ static int try_fused_convert(lzgpu_ctx *ctx, const lzgpu_goal *src, const lzgpu_
 	if (!parity_wanted) return LZGPU_NOT_HANDLED;
 	int rc;
 	{
-		// the route is decided by pure host logic BEFORE anything is acquired or enqueued (a status slot that was memset on this stream
-		// must not go back to the pool while that memset is pending)
+		// the route is decided by pure host logic before anything is enqueued
 		uint8_t avail[LZGPU_MAX_PARTS] = {0};
 		for (int i = 0; i < ks + src->m; ++i) avail[i] = d_parts[i] ? 1 : 0;
 		lzgpu_convert_plan plan;
@@ -1028,31 +1045,18 @@ static int try_fused_convert(lzgpu_ctx *ctx, const lzgpu_goal *src, const lzgpu_
 	}
 	const size_t crc_stride = (nb + static_cast<size_t>(dst->m) * pbd + 3) & ~size_t(3);
 	if ((rc = t_crc->alloc(n_chunks * crc_stride * 4))) return rc;
-	if (any_crc) {
-		if ((rc = lz_status_acquire(ctx, &tk->slot))) return rc;
-		if (cudaMemsetAsync(tk->slot.d, 0xff, sizeof(unsigned long long) * LZGPU_MAX_PARTS, st) != cudaSuccess) { ticket_drop(ctx, tk); return LZGPU_ERR_CUDA; }
-	}
+	if (any_crc && (rc = tk->arm(ctx, st))) return rc;
 	void *outs[LZGPU_MAX_PARTS] = {nullptr};
 	for (int i = 0; i < nd; ++i) outs[i] = want[i] ? d_out[i] : nullptr;
-	bool verifying = false;
 	rc = lz_fused_convert(ctx, src, dst, n_chunks, nb, d_parts, part_stride, any_crc ? d_part_crc : nullptr, outs, out_stride, t_crc->p, crc_stride, st,
-	                      any_crc ? tk->slot.d : nullptr, &verifying);
+	                      tk->word(0));
 	if (rc != LZGPU_OK) {
-		// (a launch-time refusal — misaligned part pointers, a tensor map the driver rejects: rare)  The slot's memset is already on the
-		// stream: let it finish before the slot can be handed to another call
-		if (any_crc) {
-			cudaStreamSynchronize(st);
-			ticket_drop(ctx, tk);
-		}
+		// (a launch-time refusal — misaligned part pointers, a tensor map the driver rejects: rare)  The two-pass route re-arms the
+		// slot it already holds
 		t_crc->release();
 		return rc;
 	}
-	if (any_crc) {
-		tk->fused = true;
-		tk->n_words = 1;
-		tk->blocks = pbs;
-		if (cudaMemcpyAsync(tk->slot.h, tk->slot.d, sizeof(unsigned long long), cudaMemcpyDeviceToHost, st) != cudaSuccess) { ticket_drop(ctx, tk); return LZGPU_ERR_CUDA; }
-	}
+	if (any_crc && (rc = tk->publish_fused())) return rc;
 	*crc_stride_out = crc_stride;
 	ctx->stats.chunks_recovered += n_chunks;
 	ctx->stats.chunks_encoded += n_chunks;
@@ -1109,23 +1113,9 @@ static int convert_enqueue(lzgpu_ctx *ctx, const lzgpu_goal *src, const lzgpu_go
 			image = static_cast<const uint8_t *>(d_parts[0]);
 			image_stride = part_stride;
 			if (d_part_crc && d_part_crc[0]) {
-				const unsigned long long nblk = static_cast<unsigned long long>(n_chunks) * nb;
-				if ((rc = t_vcrc.alloc(nblk * 4))) return rc;
-				if ((rc = lz_status_acquire(ctx, &tk->slot))) return rc;
-				CUDA_TRY(cudaMemsetAsync(tk->slot.d, 0xff, sizeof(unsigned long long) * LZGPU_MAX_PARTS, st));
-				if (!lzgpu_crc_enabled()) {
-					crc_compare_const_kernel<<<grid_for(ctx, nblk, 256, 4), 256, 0, st>>>(static_cast<const uint32_t *>(d_part_crc[0]), nblk, LZGPU_FAKE_CRC, 0, tk->slot.d);
-				} else {
-					if ((rc = crc_of_parts(ctx, image, n_chunks, nb, image_stride, t_vcrc.p, st))) { ticket_drop(ctx, tk); return rc; }
-					crc_compare_kernel<<<grid_for(ctx, nblk, 256, 4), 256, 0, st>>>(static_cast<const uint32_t *>(t_vcrc.p), static_cast<const uint32_t *>(d_part_crc[0]),
-					                                                              nblk, kCrcZeroBlock64K, 0, 0, tk->slot.d);
-				}
-				CUDA_TRY(cudaGetLastError());
-				ctx->stats.kernel_launches++;
-				tk->fused = false;
-				tk->n_words = 1;
-				tk->blocks = nb;
-				CUDA_TRY(cudaMemcpyAsync(tk->slot.h, tk->slot.d, sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
+				if ((rc = t_vcrc.alloc(static_cast<size_t>(n_chunks) * nb * 4)) || (rc = tk->arm(ctx, st)) ||
+				    (rc = verify_part(ctx, image, n_chunks, nb, image_stride, d_part_crc[0], t_vcrc.p, tk->word(0), st)) || (rc = tk->publish_per_part(1, nb)))
+					return rc;
 			}
 			if (direct_image && direct_image != image)
 				CUDA_TRY(cudaMemcpy2DAsync(direct_image, out_stride, image, image_stride, static_cast<size_t>(nb) * B, n_chunks, cudaMemcpyDeviceToDevice, st));
@@ -1168,7 +1158,7 @@ static int convert_enqueue(lzgpu_ctx *ctx, const lzgpu_goal *src, const lzgpu_go
 			bool fused_done = false;
 			if (parity_wanted && image_stride >= static_cast<size_t>(nb) * B) {
 				const size_t crc_stride = (nb + static_cast<size_t>(dst->m) * pbd + 3) & ~size_t(3);
-				if ((rc = t_crc.alloc(n_chunks * crc_stride * 4))) { ticket_drop(ctx, tk); return rc; }
+				if ((rc = t_crc.alloc(n_chunks * crc_stride * 4))) return rc;
 				void *outs[LZGPU_MAX_PARTS] = {nullptr};
 				for (int i = 0; i < nd; ++i) outs[i] = want[i] ? d_out[i] : nullptr;
 				rc = lz_fused_encode_split(ctx, dst, n_chunks, nb, image, image_stride, outs, out_stride, t_crc.p, crc_stride, st);
@@ -1178,16 +1168,15 @@ static int convert_enqueue(lzgpu_ctx *ctx, const lzgpu_goal *src, const lzgpu_go
 					encode_crc_stride = crc_stride;
 					ctx->stats.chunks_encoded += n_chunks;
 				} else if (rc != LZGPU_NOT_HANDLED) {
-					ticket_drop(ctx, tk);
 					return rc;
 				}
 			}
 			if (!fused_done) {
-				if (data_wanted && (rc = lzgpu_split_chunks_dev(ctx, dst, n_chunks, nb, image, image_stride, dp, out_stride, st))) { ticket_drop(ctx, tk); return rc; }
+				if (data_wanted && (rc = lzgpu_split_chunks_dev(ctx, dst, n_chunks, nb, image, image_stride, dp, out_stride, st))) return rc;
 				if (parity_wanted) {
 					const size_t par_stride = static_cast<size_t>(dst->m) * pbd * B, crc_stride = (nb + static_cast<size_t>(dst->m) * pbd + 3) & ~size_t(3);
-					if ((rc = t_par.alloc(n_chunks * par_stride)) || (!t_crc.p && (rc = t_crc.alloc(n_chunks * crc_stride * 4)))) { ticket_drop(ctx, tk); return rc; }
-					if ((rc = encode_enqueue(ctx, dst, n_chunks, nb * B, image, image_stride, t_par.p, par_stride, t_crc.p, crc_stride, st))) { ticket_drop(ctx, tk); return rc; }
+					if ((rc = t_par.alloc(n_chunks * par_stride)) || (!t_crc.p && (rc = t_crc.alloc(n_chunks * crc_stride * 4)))) return rc;
+					if ((rc = encode_enqueue(ctx, dst, n_chunks, nb * B, image, image_stride, t_par.p, par_stride, t_crc.p, crc_stride, st))) return rc;
 					d_encode_crc = t_crc.p;
 					encode_crc_stride = crc_stride;
 					for (int r = 0; r < dst->m; ++r)
@@ -1201,7 +1190,7 @@ static int convert_enqueue(lzgpu_ctx *ctx, const lzgpu_goal *src, const lzgpu_go
 	// ChunkReplicator::replicate computes mycrc32 of every rebuilt block (chunk_replicator.cc:186-192)
 	if (d_out_crc && !lzgpu_crc_enabled()) {
 		for (int i = 0; i < nd; ++i)
-			if (want[i] && d_out_crc[i] && (rc = fill_crc(ctx, d_out_crc[i], pbd, pbd, n_chunks, st))) { ticket_drop(ctx, tk); return rc; }
+			if (want[i] && d_out_crc[i] && (rc = fill_crc(ctx, d_out_crc[i], pbd, pbd, n_chunks, st))) return rc;
 	} else if (d_out_crc) {
 		if (d_encode_crc) {
 			// the encode pass that produced the parity already checksummed every data and parity block of the destination slice
@@ -1220,7 +1209,7 @@ static int convert_enqueue(lzgpu_ctx *ctx, const lzgpu_goal *src, const lzgpu_go
 			}
 		} else {
 			for (int i = 0; i < nd; ++i)
-				if (want[i] && d_out_crc[i] && (rc = crc_of_parts(ctx, d_out[i], n_chunks, pbd, out_stride, d_out_crc[i], st))) { ticket_drop(ctx, tk); return rc; }
+				if (want[i] && d_out_crc[i] && (rc = crc_of_parts(ctx, d_out[i], n_chunks, pbd, out_stride, d_out_crc[i], st))) return rc;
 		}
 	}
 	return LZGPU_OK;
@@ -1250,20 +1239,7 @@ extern "C" int lzgpu_convert_chunks_dev(lzgpu_ctx *ctx, const lzgpu_goal *src, c
 		BatchTimer timer(ctx, st, convert_alg_bytes(src, dst, n_chunks, nb, want, d_part_crc != nullptr));
 		if ((rc = convert_enqueue(ctx, src, dst, n_chunks, nb, d_parts, part_stride, d_part_crc, want, d_out, out_stride, d_out_crc, st, &tk))) return rc;
 	}
-	if (!tk.active()) return LZGPU_OK;
-	if (ctx->deferred_verify.load()) {
-		std::lock_guard<std::mutex> lk(ctx->pending_mu);
-		ctx->pending.push_back(tk);
-		return LZGPU_OK;
-	}
-	cudaError_t e = cudaStreamSynchronize(st);
-	if (e != cudaSuccess) {
-		ticket_drop(ctx, &tk);
-		cudaGetLastError();
-		lz_set_error("CUDA error %s while waiting for the verification result", cudaGetErrorName(e));
-		return LZGPU_ERR_CUDA;
-	}
-	return ticket_result(ctx, &tk, bad);
+	return dev_verdict(ctx, std::move(tk), bad);
 }
 
 extern "C" int lzgpu_convert_chunks(lzgpu_ctx *ctx, const lzgpu_goal *src, const lzgpu_goal *dst, uint32_t n_chunks, uint32_t nb,
@@ -1293,7 +1269,7 @@ extern "C" int lzgpu_convert_chunks(lzgpu_ctx *ctx, const lzgpu_goal *src, const
 		if (parts[i]) pin.add(parts[i], static_cast<size_t>(n_chunks - 1) * part_stride + sbytes);
 	for (int i = 0; i < nd; ++i)
 		if (want[i]) pin.add(out[i], static_cast<size_t>(n_chunks - 1) * out_stride + dbytes);
-	// three pipeline slots (see lzgpu_recover_chunks); a same-slice rebuild writes into buffers shaped like the inputs
+	// a same-slice rebuild writes into buffers shaped like the inputs
 	const size_t per_chunk = sbytes * std::max(n_in, 1) + dbytes * n_out;
 	const uint32_t tile = static_cast<uint32_t>(std::max<size_t>(1, std::min<size_t>(n_chunks, (2 * kHostTileBytes) / per_chunk)));
 	const int n_slots = n_chunks > tile ? kHostSlots : 1;
@@ -1304,13 +1280,7 @@ extern "C" int lzgpu_convert_chunks(lzgpu_ctx *ctx, const lzgpu_goal *src, const
 		if ((rc = lz_scratch(ctx, kScratchPar0 + s, tile * dbytes * n_out, &d_o[s]))) return rc;
 		if ((rc = lz_scratch(ctx, kScratchOutCrc0 + s, static_cast<size_t>(tile) * pbd * 4 * n_out, &d_co[s]))) return rc;
 	}
-	SlotState ss[kHostSlots];
-	uint32_t t = 0;
-	for (uint32_t c0 = 0; c0 < n_chunks; c0 += tile, ++t) {
-		const uint32_t nc = std::min(tile, n_chunks - c0);
-		const int s = static_cast<int>(t % n_slots);
-		if ((rc = retire_slot(ctx, s, &ss[s], bad))) { drain_slots(ctx, ss); return rc; }
-		cudaStream_t st = ctx->slot_stream[s];
+	return run_tiles(ctx, n_chunks, tile, n_slots, bad, [&](int s, size_t c0, size_t nc, cudaStream_t st, VerifyTicket *tk) -> int {
 		std::vector<const void *> dp(ns, nullptr), dc(ns, nullptr);
 		std::vector<void *> dout(nd, nullptr), dcrc(nd, nullptr);
 		bool any_crc = false;
@@ -1318,12 +1288,12 @@ extern "C" int lzgpu_convert_chunks(lzgpu_ctx *ctx, const lzgpu_goal *src, const
 		for (int i = 0; i < ns; ++i) {
 			if (!parts[i]) continue;
 			uint8_t *slot = static_cast<uint8_t *>(d_in[s]) + static_cast<size_t>(a) * tile * sbytes;
-			CUDA_TRY(cudaMemcpy2DAsync(slot, sbytes, parts[i] + static_cast<size_t>(c0) * part_stride, part_stride, sbytes, nc, cudaMemcpyHostToDevice, st));
+			CUDA_TRY(cudaMemcpy2DAsync(slot, sbytes, parts[i] + c0 * part_stride, part_stride, sbytes, nc, cudaMemcpyHostToDevice, st));
 			ctx->stats.bytes_h2d += static_cast<uint64_t>(nc) * sbytes;
 			dp[i] = slot;
 			if (part_crc && part_crc[i]) {
 				uint8_t *cs = static_cast<uint8_t *>(d_cin[s]) + static_cast<size_t>(a) * tile * pbs * 4;
-				CUDA_TRY(cudaMemcpyAsync(cs, part_crc[i] + static_cast<size_t>(c0) * pbs, static_cast<size_t>(nc) * pbs * 4, cudaMemcpyHostToDevice, st));
+				CUDA_TRY(cudaMemcpyAsync(cs, part_crc[i] + c0 * pbs, nc * pbs * 4, cudaMemcpyHostToDevice, st));
 				dc[i] = cs;
 				any_crc = true;
 			}
@@ -1336,27 +1306,21 @@ extern "C" int lzgpu_convert_chunks(lzgpu_ctx *ctx, const lzgpu_goal *src, const
 			if (out_crc && out_crc[i]) dcrc[i] = static_cast<uint8_t *>(d_co[s]) + static_cast<size_t>(a) * tile * pbd * 4;
 			++a;
 		}
-		ss[s].c0 = c0;
+		int rc;
 		{
-			BatchTimer timer(ctx, st, convert_alg_bytes(src, dst, nc, nb, want, any_crc));
-			rc = convert_enqueue(ctx, src, dst, nc, nb, dp.data(), sbytes, any_crc ? dc.data() : nullptr, want, dout.data(), dbytes,
-			                     out_crc ? dcrc.data() : nullptr, st, &ss[s].tk);
+			BatchTimer timer(ctx, st, convert_alg_bytes(src, dst, static_cast<uint32_t>(nc), nb, want, any_crc));
+			rc = convert_enqueue(ctx, src, dst, static_cast<uint32_t>(nc), nb, dp.data(), sbytes, any_crc ? dc.data() : nullptr, want, dout.data(), dbytes,
+			                     out_crc ? dcrc.data() : nullptr, st, tk);
 		}
-		if (rc) { drain_slots(ctx, ss); return rc; }
-		ss[s].busy = true;
+		if (rc) return rc;
 		for (int i = 0; i < nd; ++i) {
 			if (!want[i]) continue;
-			CUDA_TRY(cudaMemcpy2DAsync(out[i] + static_cast<size_t>(c0) * out_stride, out_stride, dout[i], dbytes, dbytes, nc, cudaMemcpyDeviceToHost, st));
+			CUDA_TRY(cudaMemcpy2DAsync(out[i] + c0 * out_stride, out_stride, dout[i], dbytes, dbytes, nc, cudaMemcpyDeviceToHost, st));
 			ctx->stats.bytes_d2h += static_cast<uint64_t>(nc) * dbytes;
-			if (dcrc[i])
-				CUDA_TRY(cudaMemcpyAsync(out_crc[i] + static_cast<size_t>(c0) * pbd, dcrc[i], static_cast<size_t>(nc) * pbd * 4, cudaMemcpyDeviceToHost, st));
+			if (dcrc[i]) CUDA_TRY(cudaMemcpyAsync(out_crc[i] + c0 * pbd, dcrc[i], nc * pbd * 4, cudaMemcpyDeviceToHost, st));
 		}
-	}
-	for (uint32_t i = 0; i < static_cast<uint32_t>(n_slots); ++i) {
-		const int s = static_cast<int>((t + i) % n_slots);
-		if ((rc = retire_slot(ctx, s, &ss[s], bad))) { drain_slots(ctx, ss); return rc; }
-	}
-	return LZGPU_OK;
+		return LZGPU_OK;
+	});
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -1509,20 +1473,15 @@ extern "C" int lzgpu_crc_blocks(lzgpu_ctx *ctx, const uint8_t *data, size_t n_bl
 		if ((rc = lz_scratch(ctx, kScratchIn0 + s, std::min(per_tile, n_blocks) * dstride, &d_in[s]))) return rc;
 		if ((rc = lz_scratch(ctx, kScratchCrc0 + s, std::min(per_tile, n_blocks) * 4, &d_c[s]))) return rc;
 	}
-	size_t t = 0;
-	for (size_t b0 = 0; b0 < n_blocks; b0 += per_tile, ++t) {
-		const size_t n = std::min(per_tile, n_blocks - b0);
-		const int s = t & 1;
-		cudaStream_t st = ctx->slot_stream[s];
+	return run_tiles(ctx, n_blocks, per_tile, 2, nullptr, [&](int s, size_t b0, size_t n, cudaStream_t st, VerifyTicket *) -> int {
 		CUDA_TRY(cudaMemcpy2DAsync(d_in[s], dstride, data + b0 * block_stride, block_stride, block_len, n, cudaMemcpyHostToDevice, st));
-		if ((rc = lzgpu_crc_blocks_dev(ctx, d_in[s], n, block_len, dstride, d_c[s], st))) return rc;
+		int rc = lzgpu_crc_blocks_dev(ctx, d_in[s], n, block_len, dstride, d_c[s], st);
+		if (rc) return rc;
 		CUDA_TRY(cudaMemcpyAsync(crc_out + b0, d_c[s], n * 4, cudaMemcpyDeviceToHost, st));
 		ctx->stats.bytes_h2d += n * block_len;
 		ctx->stats.bytes_d2h += n * 4;
-	}
-	CUDA_TRY(cudaStreamSynchronize(ctx->slot_stream[0]));
-	CUDA_TRY(cudaStreamSynchronize(ctx->slot_stream[1]));
-	return LZGPU_OK;
+		return LZGPU_OK;
+	});
 }
 
 static int verify_common(lzgpu_ctx *ctx, const uint8_t *h_data, size_t n_blocks, uint32_t block_len, size_t h_stride, size_t h_offset,
@@ -1541,12 +1500,7 @@ static int verify_common(lzgpu_ctx *ctx, const uint8_t *h_data, size_t n_blocks,
 	if ((rc = lz_scratch(ctx, kScratchIn0, tile_blocks * dstride, &d_in))) return rc;
 	if ((rc = lz_scratch(ctx, kScratchCrc0, tile_blocks * 4, &d_c))) return rc;
 	if ((rc = lz_scratch(ctx, kScratchCrc0 + 1, tile_blocks * 4, &d_s))) return rc;
-	StatusSlot slot;
-	if ((rc = lz_status_acquire(ctx, &slot))) return rc;
-	struct SlotReturn {
-		lzgpu_ctx *c; StatusSlot s;
-		~SlotReturn() { lz_status_release(c, s); }
-	} slot_return{ctx, slot};
+	VerifyTicket tk;  // one result word per tile: its first mismatching block, read back as block b of a single n-block "chunk"
 	for (size_t b0 = 0; b0 < n_blocks; b0 += tile_blocks) {
 		const size_t n = std::min(tile_blocks, n_blocks - b0);
 		// cudaMemcpyDefault: the source may be host memory or (unified addressing) a device buffer, e.g. chunk files read straight
@@ -1554,10 +1508,10 @@ static int verify_common(lzgpu_ctx *ctx, const uint8_t *h_data, size_t n_blocks,
 		CUDA_TRY(cudaMemcpy2DAsync(d_in, dstride, h_data + h_offset + b0 * h_stride, h_stride, block_len, n, cudaMemcpyDefault, st));
 		CUDA_TRY(cudaMemcpy2DAsync(d_s, 4, reinterpret_cast<const uint8_t *>(h_stored) + b0 * stored_stride_bytes, stored_stride_bytes, 4, n,
 		                           cudaMemcpyDefault, st));
-		CUDA_TRY(cudaMemsetAsync(slot.d, 0xff, sizeof(unsigned long long), st));
+		if ((rc = tk.arm(ctx, st))) return rc;
 		const int crc_off = lzgpu_crc_enabled() ? 0 : 1;
 		if (crc_off && !sparse_rule) {
-			crc_compare_const_kernel<<<grid_for(ctx, n, 256, 4), 256, 0, st>>>(static_cast<const uint32_t *>(d_s), n, LZGPU_FAKE_CRC, big_endian, slot.d);
+			crc_compare_const_kernel<<<grid_for(ctx, n, 256, 4), 256, 0, st>>>(static_cast<const uint32_t *>(d_s), n, LZGPU_FAKE_CRC, big_endian, tk.word(0));
 			CUDA_TRY(cudaGetLastError());
 			ctx->stats.kernel_launches++;
 		} else {
@@ -1567,7 +1521,7 @@ static int verify_common(lzgpu_ctx *ctx, const uint8_t *h_data, size_t n_blocks,
 			if (rc == LZGPU_NOT_HANDLED) rc = lz_crc_blocks(ctx, d_in, n, n, 0, dstride, block_len, d_c, 0, st);
 			if (rc) return rc;
 			crc_compare_kernel<<<grid_for(ctx, n, 256, 4), 256, 0, st>>>(static_cast<const uint32_t *>(d_c), static_cast<const uint32_t *>(d_s), n,
-			                                                            lz::crc_of_zeros(block_len), sparse_rule, big_endian, slot.d, crc_off);
+			                                                            lz::crc_of_zeros(block_len), sparse_rule, big_endian, tk.word(0), crc_off);
 			CUDA_TRY(cudaGetLastError());
 			ctx->stats.kernel_launches++;
 		}
@@ -1575,15 +1529,17 @@ static int verify_common(lzgpu_ctx *ctx, const uint8_t *h_data, size_t n_blocks,
 			// holes accepted on their CRC are re-read and must really be all zero (crc.cc:235-243)
 			const unsigned grid = static_cast<unsigned>(std::min<size_t>(n, static_cast<size_t>(ctx->sm_count) * 8));
 			sparse_confirm_kernel<<<grid, 256, 0, st>>>(static_cast<const uint8_t *>(d_in), dstride, block_len, static_cast<const uint32_t *>(d_c),
-			                                            static_cast<const uint32_t *>(d_s), n, lz::crc_of_zeros(block_len), slot.d);
+			                                            static_cast<const uint32_t *>(d_s), n, lz::crc_of_zeros(block_len), tk.word(0));
 			CUDA_TRY(cudaGetLastError());
 			ctx->stats.kernel_launches++;
 		}
-		CUDA_TRY(cudaMemcpyAsync(slot.h, slot.d, sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
-		CUDA_TRY(cudaStreamSynchronize(st));
+		int64_t at[3];
+		if ((rc = tk.publish_per_part(1, static_cast<uint32_t>(n)))) return rc;
+		rc = tk.wait_take(at);
+		if (rc && rc != LZGPU_ERR_CRC) return rc;
 		ctx->stats.bytes_h2d += n * (block_len + 4ull);
-		if (slot.h[0] != ~0ull) {
-			const unsigned long long bad = b0 + slot.h[0];
+		if (rc) {
+			const unsigned long long bad = b0 + static_cast<unsigned long long>(at[2]);
 			if (first_bad) *first_bad = static_cast<int64_t>(bad);
 			lz_set_error("CRC mismatch in block %llu", bad);
 			return LZGPU_ERR_CRC;
@@ -1982,7 +1938,7 @@ extern "C" int lzgpu_dev_sync(lzgpu_ctx *ctx) {
 	int rc = LZGPU_OK;
 	for (VerifyTicket &tk : ctx->pending) {
 		int64_t bad[3] = {-1, -1, -1};
-		const int r = ticket_result(ctx, &tk, bad);
+		const int r = tk.take(bad);
 		if (r != LZGPU_OK && rc == LZGPU_OK) {
 			rc = r;
 			ctx->last_bad[0] = bad[0]; ctx->last_bad[1] = bad[1]; ctx->last_bad[2] = bad[2];

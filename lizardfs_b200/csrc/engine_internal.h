@@ -6,6 +6,7 @@
 #include <cstddef>
 #include <cstdint>
 #include <mutex>
+#include <utility>
 #include <vector>
 
 #include "lzgpu.h"
@@ -56,15 +57,39 @@ struct StatusSlot {
 	int index = -1;
 };
 
-// What a verifying call leaves behind: the result words are copied to the slot's pinned mirror on the call's stream and
-// decoded once that stream has been synchronised (by the public *_dev wrapper, by the host pipelines when they retire a tile, or
-// by lzgpu_dev_sync in deferred mode).
-struct VerifyTicket {
-	StatusSlot slot;       // index < 0: nothing was verified
-	bool fused = false;    // fused route: one word (chunk*64 + part)*1024 + block; otherwise one word per part: chunk*blocks + block
-	int n_words = 0;
-	uint32_t blocks = 0;   // blocks per chunk of a verified part (generic encoding)
-	bool active() const { return slot.index >= 0; }
+// Owner of one verification in flight.  arm() takes a slot and sets its result words to ~0 on the call's stream; the kernels
+// lower them to the first mismatch; publish_*() records how the words are encoded and copies them to the slot's pinned mirror
+// on the same stream; take() decodes them once that stream has been synchronised (by the public *_dev call, by the host
+// pipeline when it retires a tile, or by lzgpu_dev_sync in deferred mode) and returns the slot.  An armed owner that is
+// destroyed without take() first waits for its stream, so a slot never goes back to the pool with work on it still queued.
+class VerifyTicket {
+public:
+	VerifyTicket() = default;
+	VerifyTicket(VerifyTicket &&o) noexcept { *this = std::move(o); }
+	VerifyTicket &operator=(VerifyTicket &&o) noexcept;
+	~VerifyTicket() { drop(); }
+	bool armed() const { return slot_.index >= 0; }
+	// takes a slot (the one already held, when armed) and enqueues the memset of its words to ~0 on `st`
+	int arm(lzgpu_ctx *ctx, cudaStream_t st);
+	unsigned long long *word(int i) const { return slot_.d + i; }  // device result word i (word(0) is nullptr when not armed)
+	// fused route: one word (chunk*64 + part)*1024 + block
+	int publish_fused() { return publish(true, 1, 0); }
+	// one word per part (word i: part i), each chunk*blocks + block
+	int publish_per_part(int n_words, uint32_t blocks) { return publish(false, n_words, blocks); }
+	// after the stream has been synchronised: LZGPU_OK or LZGPU_ERR_CRC (+ first bad chunk / part / block); returns the slot
+	int take(int64_t *bad);
+	// waits for the stream, then take(); LZGPU_OK at once when nothing is armed
+	int wait_take(int64_t *bad);
+
+private:
+	int publish(bool fused, int n_words, uint32_t blocks);
+	void drop();
+	lzgpu_ctx *ctx_ = nullptr;
+	cudaStream_t st_ = nullptr;
+	StatusSlot slot_;
+	bool fused_ = false;
+	int n_words_ = 0;
+	uint32_t blocks_ = 0;
 };
 
 // per-batch device timing (lzgpu_stats.batch_*): CUDA events recorded around the kernels of a batched call on its stream,
@@ -124,8 +149,6 @@ struct TmpBuf {
 	}
 };
 
-int lz_status_acquire(lzgpu_ctx *ctx, StatusSlot *out);
-void lz_status_release(lzgpu_ctx *ctx, const StatusSlot &s);
 // scope guard for the batch timer: records the start event now and the end event + bytes at scope exit
 struct BatchTimer {
 	lzgpu_ctx *ctx;
@@ -157,18 +180,18 @@ int lz_fused_encode(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, u
                     void *d_parity, size_t parity_stride, void *d_crc, size_t crc_stride, cudaStream_t st);
 int lz_fused_encode_split(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, uint32_t nb, const void *d_data, size_t chunk_stride,
                           void *const *d_out, size_t out_stride, void *d_crc, size_t crc_stride, cudaStream_t st);
-// Fused degraded read (verify + rebuild erased data parts + chunk-order image).  When any part is verified (*verifying),
+// Fused degraded read (verify + rebuild erased data parts + chunk-order image).  When any part is verified,
 // first-bad information is written to d_first_bad[0] encoded as (chunk*64 + part)*1024 + block (~0 = all good); the caller
 // owns that word (a StatusSlot) and must pass it whenever d_part_crc is given.
 int lz_fused_recover(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, uint32_t nb, const void *const *d_parts, size_t part_stride,
                      const void *const *d_part_crc, const uint8_t *want, void *const *d_out, void *d_chunk_out, size_t chunk_out_stride,
-                     cudaStream_t st, unsigned long long *d_first_bad, bool *verifying);
+                     cudaStream_t st, unsigned long long *d_first_bad);
 // Fused slice conversion (convert_kernel.cuh): k parts of the source slice -> every wanted part of the destination slice (d_out[i],
 // nullptr = not wanted) + the destination slice's block CRCs in chunk order (nb data blocks, then m x pbd parity blocks per chunk),
 // one pass; verification as in lz_fused_recover.  LZGPU_NOT_HANDLED = take the two-pass route.
 int lz_fused_convert(lzgpu_ctx *ctx, const lzgpu_goal *src, const lzgpu_goal *dst, uint32_t n_chunks, uint32_t nb, const void *const *d_parts,
                      size_t part_stride, const void *const *d_part_crc, void *const *d_out, size_t out_stride, void *d_crc, size_t crc_stride,
-                     cudaStream_t st, unsigned long long *d_first_bad, bool *verifying);
+                     cudaStream_t st, unsigned long long *d_first_bad);
 // CRC of 64 KiB blocks: block (c, b) at base + c*chunk_stride + b*65536, out[c*out_chunk_stride + b]
 int lz_fused_crc(lzgpu_ctx *ctx, const void *base, unsigned long long n_blocks, unsigned long long blocks_per_chunk,
                  unsigned long long chunk_stride, void *out, unsigned long long out_chunk_stride, cudaStream_t st);

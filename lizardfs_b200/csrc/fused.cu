@@ -658,9 +658,9 @@ static int launch_recover(lzgpu_ctx *ctx, const TmapArray &maps, const RecoverPa
 
 int lz_fused_recover(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, uint32_t nb, const void *const *d_parts, size_t part_stride,
                      const void *const *d_part_crc, const uint8_t *want, void *const *d_out, void *d_chunk_out, size_t chunk_out_stride,
-                     cudaStream_t st, unsigned long long *d_first_bad, bool *verifying) {
+                     cudaStream_t st, unsigned long long *d_first_bad) {
 	FusedState *fs = ctx->fused;
-	*verifying = false;
+	bool verifying = false;
 	if (!fs || fs->disabled) return LZGPU_NOT_HANDLED;
 	const int K = goal->k, M = goal->m, N = K + M;
 	const bool direct = lz::uses_cauchy(K, M);   // no Horner syndromes for a Cauchy generator: general rows over the k inputs
@@ -785,7 +785,7 @@ int lz_fused_recover(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, 
 	p.zconst = lz::crc_of_zeros(LZGPU_BLOCK_SIZE);
 	for (int a = 0; a < K; ++a) {
 		p.stored[a] = d_part_crc ? static_cast<const uint32_t *>(d_part_crc[used[a]]) : nullptr;
-		if (p.stored[a]) *verifying = true;
+		if (p.stored[a]) verifying = true;
 	}
 	// V[r][x] = (2^row_r)^(erased_x); W = V^-1
 	uint8_t V[16], W[16];
@@ -858,7 +858,7 @@ int lz_fused_recover(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, 
 		                              CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
 		if (r != CUDA_SUCCESS) return LZGPU_NOT_HANDLED;
 	}
-	if (*verifying && !d_first_bad) return LZGPU_NOT_HANDLED;  // (callers that pass stored CRCs always pass the result word, initialised to ~0)
+	if (verifying && !d_first_bad) return LZGPU_NOT_HANDLED;  // (callers that pass stored CRCs always pass the result word, initialised to ~0)
 	const size_t smem = static_cast<size_t>(n_stages) * K * G * 4 * kStepBytes + 16 * n_stages + 64;
 	const bool row0 = p.par_row[0] == 0, row01 = e >= 2 && consecutive;
 	if (bs3) {
@@ -903,13 +903,13 @@ int lz_fused_recover(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, 
 	// ec(5,3): two lost, faster for rebuild only but slower with verification and image (the unrolled walk costs the CRC role
 	// registers), so that combination keeps the runtime-k kernel; three lost faster either way
 	if (K == 5 && geo == 2 && fs->recover_k3) {
-		if (e == 2 && row01 && !(*verifying && d_chunk_out)) return launch_recover_geo2<2, 5, 0, 1>(ctx, maps, p, smem, st);
+		if (e == 2 && row01 && !(verifying && d_chunk_out)) return launch_recover_geo2<2, 5, 0, 1>(ctx, maps, p, smem, st);
 		if (e == 3 && row01) return launch_recover_geo2<3, 5, 0, 1>(ctx, maps, p, smem, st);
 	}
 	// ec(4,2), ec(6,2), ec(6,3): the same rule as for k = 5
-	if (K == 4 && geo == 2 && fs->recover_k3 && e == 2 && row01 && !(*verifying && d_chunk_out)) return launch_recover_geo2<2, 4, 0, 1>(ctx, maps, p, smem, st);
+	if (K == 4 && geo == 2 && fs->recover_k3 && e == 2 && row01 && !(verifying && d_chunk_out)) return launch_recover_geo2<2, 4, 0, 1>(ctx, maps, p, smem, st);
 	if (K == 6 && geo == 2 && fs->recover_k3) {
-		if (e == 2 && row01 && !(*verifying && d_chunk_out)) return launch_recover_geo2<2, 6, 0, 1>(ctx, maps, p, smem, st);
+		if (e == 2 && row01 && !(verifying && d_chunk_out)) return launch_recover_geo2<2, 6, 0, 1>(ctx, maps, p, smem, st);
 		if (e == 3 && row01) return launch_recover_geo2<3, 6, 0, 1>(ctx, maps, p, smem, st);
 	}
 	switch (e) {
@@ -946,9 +946,9 @@ static int launch_convert(lzgpu_ctx *ctx, const TmapArray &maps, const ConvertPa
 // CRCs in chunk order (d_crc: nb data blocks, then m x pbd parity blocks per chunk), one pass.  LZGPU_NOT_HANDLED = use the two-pass route.
 int lz_fused_convert(lzgpu_ctx *ctx, const lzgpu_goal *src, const lzgpu_goal *dst, uint32_t n_chunks, uint32_t nb, const void *const *d_parts,
                      size_t part_stride, const void *const *d_part_crc, void *const *d_out, size_t out_stride, void *d_crc, size_t crc_stride,
-                     cudaStream_t st, unsigned long long *d_first_bad, bool *verifying) {
+                     cudaStream_t st, unsigned long long *d_first_bad) {
 	FusedState *fs = ctx->fused;
-	*verifying = false;
+	bool verifying = false;
 	if (!fs || fs->disabled || fs->convert_off) return LZGPU_NOT_HANDLED;
 	const int Ks = src->k, Ms = src->m, Kd = dst->k, Md = dst->m;
 	if (src->kind == LZGPU_KIND_STD || dst->kind == LZGPU_KIND_STD) return LZGPU_NOT_HANDLED;
@@ -994,7 +994,7 @@ int lz_fused_convert(lzgpu_ctx *ctx, const lzgpu_goal *src, const lzgpu_goal *ds
 		p.loaded_slot[a] = static_cast<uint8_t>(slot);
 		p.part_id[slot] = static_cast<uint8_t>(idx);
 		p.stored[slot] = d_part_crc ? static_cast<const uint32_t *>(d_part_crc[idx]) : nullptr;
-		if (p.stored[slot]) *verifying = true;
+		if (p.stored[slot]) verifying = true;
 		const cuuint64_t dims[3] = {static_cast<cuuint64_t>(kRowBytes), static_cast<cuuint64_t>(pbs) * 4, n_chunks};
 		const cuuint64_t strides[2] = {static_cast<cuuint64_t>(kRowBytes), part_stride};
 		const cuuint32_t box[3] = {kStepBytes, T * 4, 1};
@@ -1011,7 +1011,7 @@ int lz_fused_convert(lzgpu_ctx *ctx, const lzgpu_goal *src, const lzgpu_goal *ds
 		p.bl_entry[bl] = static_cast<uint16_t>(row0 * kStepBytes + ((row0 & 4) ? 64 : 0));
 	}
 	for (uint32_t x = 0; x < e; ++x) p.part_id[Ks + x] = static_cast<uint8_t>(Ks + x);
-	if (*verifying && !d_first_bad) return LZGPU_NOT_HANDLED;
+	if (verifying && !d_first_bad) return LZGPU_NOT_HANDLED;
 	if (e == 2) {
 		uint8_t gx0 = 1, gx1 = 1;
 		for (int t = 0; t < p.erased_idx[0]; ++t) gx0 = lz::gf_mul_host(gx0, 2);

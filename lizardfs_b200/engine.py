@@ -407,6 +407,12 @@ class Engine:
         _check(self.lib.lzgpu_debug_last_launch(self.h, C.byref(grid), C.byref(units)), "debug_last_launch")
         return grid.value, units.value
 
+    def status_slots(self):
+        """(allocated, in_use) verification result slots of this context (lzgpu_debug_status_slots)"""
+        allocated, in_use = C.c_uint32(), C.c_uint32()
+        _check(self.lib.lzgpu_debug_status_slots(self.h, C.byref(allocated), C.byref(in_use)), "debug_status_slots")
+        return allocated.value, in_use.value
+
     def sync(self):
         """waits for the device; in deferred-verification mode also collects the verdicts of the *_dev calls issued since the last
         sync and raises ChunkCrcError for the first mismatch"""
