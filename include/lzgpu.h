@@ -162,6 +162,30 @@ void lzgpu_reset_stats(lzgpu_ctx *ctx);
  * launched last.  LZGPU_GRID_CAP=n in the environment when the context is created caps every such grid at n CTAs (testing:
  * every CTA then walks several units). */
 int lzgpu_debug_last_launch(lzgpu_ctx *ctx, uint32_t *grid, uint32_t *units);
+/* Diagnostics: the whole geometry of that same launch, taken with grid and units as one snapshot.  It shows what a context's
+ * LZGPU_BS_* / LZGPU_BITSLICE / LZGPU_RECOVER_* switches made of a call, which lzgpu_plan_encode (build defaults) does not.
+ * kernel: LZGPU_KERNEL_* below (LZGPU_KERNEL_NONE and all fields 0 before the first launch).  G: stripes per work unit (destination
+ * stripes for the conversion).  stages: depth of the data stage ring.  gf_warps: warps that do GF work only (the bit-sliced kernels'
+ * item warps, the conversion's rebuild warps); 0 where the GF items share warps with the CRC streams.  smem_bytes: dynamic shared
+ * memory per CTA. */
+enum {
+	LZGPU_KERNEL_NONE = 0,
+	LZGPU_KERNEL_ENCODE = 1,           /* fused_stream_kernel, packed-word GF items: encode, CRC-only and split (conversion) forms */
+	LZGPU_KERNEL_ENCODE_BITSLICE = 2,  /* fused_stream_kernel, bit-sliced GF warps (three or four Vandermonde parity rows) */
+	LZGPU_KERNEL_RECOVER_GEO0 = 3,     /* fused_recover_kernel: one 9-warp CTA per SM */
+	LZGPU_KERNEL_RECOVER_GEO1 = 4,     /* fused_recover_kernel: two 9-warp CTAs per SM */
+	LZGPU_KERNEL_RECOVER_GEO2 = 5,     /* fused_recover_kernel: one 16-warp CTA per SM */
+	LZGPU_KERNEL_RECOVER_DIRECT = 6,   /* fused_recover_kernel, DIRECT form (Cauchy generators) */
+	LZGPU_KERNEL_RECOVER_BS3 = 7,      /* bs_recover3_kernel: three lost data parts on bit planes */
+	LZGPU_KERNEL_CONVERT = 8           /* fused_convert_kernel: one-pass slice conversion */
+};
+typedef struct lzgpu_launch_geometry {
+	int kernel;
+	uint32_t grid, units, threads;
+	uint32_t G, stages, gf_warps;
+	uint32_t smem_bytes;
+} lzgpu_launch_geometry;
+int lzgpu_debug_last_geometry(lzgpu_ctx *ctx, lzgpu_launch_geometry *out);
 /* Diagnostics: verification result slots of the context — how many exist and how many a call holds right now (0 when no call runs). */
 int lzgpu_debug_status_slots(lzgpu_ctx *ctx, uint32_t *allocated, uint32_t *in_use);
 

@@ -39,6 +39,16 @@ class LzConvertPlan(C.Structure):
                 ("stages", C.c_uint32), ("worker_warps", C.c_uint32), ("rebuild_warps", C.c_uint32), ("smem_bytes", C.c_uint32)]
 
 
+class LzLaunchGeometry(C.Structure):
+    _fields_ = [("kernel", C.c_int), ("grid", C.c_uint32), ("units", C.c_uint32), ("threads", C.c_uint32), ("G", C.c_uint32),
+                ("stages", C.c_uint32), ("gf_warps", C.c_uint32), ("smem_bytes", C.c_uint32)]
+
+
+# lzgpu_launch_geometry.kernel
+KERNEL_NONE, KERNEL_ENCODE, KERNEL_ENCODE_BITSLICE, KERNEL_RECOVER_GEO0, KERNEL_RECOVER_GEO1, KERNEL_RECOVER_GEO2, \
+    KERNEL_RECOVER_DIRECT, KERNEL_RECOVER_BS3, KERNEL_CONVERT = range(9)
+
+
 class LzBlockWrite(C.Structure):
     _fields_ = [("block", C.c_uint32), ("offset", C.c_uint32), ("size", C.c_uint32), ("crc", C.c_uint32),
                 ("payload_off", C.c_uint64), ("exists", C.c_uint32), ("status", C.c_int32)]
@@ -71,6 +81,7 @@ SIGNATURES = {
     "lzgpu_get_stats": (None, [_vp, C.POINTER(LzStats)]),
     "lzgpu_reset_stats": (None, [_vp]),
     "lzgpu_debug_last_launch": (_int, [_vp, C.POINTER(_u32), C.POINTER(_u32)]),
+    "lzgpu_debug_last_geometry": (_int, [_vp, C.POINTER(LzLaunchGeometry)]),
     "lzgpu_debug_status_slots": (_int, [_vp, C.POINTER(_u32), C.POINTER(_u32)]),
     "lzgpu_encode_chunks": (_int, [_vp, _goalp, _u32, _u32, _vp, _sz, _vp, _sz, _vp, _sz]),
     "lzgpu_encode_chunks_dev": (_int, [_vp, _goalp, _u32, _u32, _vp, _sz, _vp, _sz, _vp, _sz, _vp]),

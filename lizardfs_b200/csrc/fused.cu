@@ -9,6 +9,7 @@
 #include <numeric>
 #include <cstdlib>
 #include <cstring>
+#include <mutex>
 
 #include "engine_internal.h"
 #include "fused_kernel.cuh"
@@ -56,16 +57,32 @@ struct FusedState {
 	int bitslice = LZ_BITSLICE_DEFAULT;  // LZGPU_BITSLICE: Vandermonde parity rows on bit planes (W = 8 items, bitslice.cuh) — bit 0: four rows, bit 1: three rows with k >= 7, bit 2: three rows with any k; 0 = packed-byte Horner
 	int promo = 3;  // CU_TENSOR_MAP_L2_PROMOTION_L2_256B: measured faster streaming than 128B/none
 	uint32_t grid_cap = 0;  // LZGPU_GRID_CAP (testing): at most this many CTAs per persistent launch, so that every CTA walks several units; 0 = no cap
-	std::atomic<uint64_t> last_launch{0};  // grid << 32 | total_units of the latest persistent launch (lzgpu_debug_last_launch)
+	std::mutex last_mu;                     // guards last_geo: grid, units and the rest are recorded and read as one snapshot
+	lzgpu_launch_geometry last_geo{};       // the latest persistent launch (lzgpu_debug_last_launch, lzgpu_debug_last_geometry)
 };
 
+// what a launch site knows of its kernel's geometry before the grid is chosen (persistent_grid adds grid and units)
+static lzgpu_launch_geometry launch_geo(int kernel, uint32_t threads, uint32_t G, uint32_t stages, uint32_t gf_warps, size_t smem) {
+	lzgpu_launch_geometry g{};
+	g.kernel = kernel;
+	g.threads = threads;
+	g.G = G;
+	g.stages = stages;
+	g.gf_warps = gf_warps;
+	g.smem_bytes = static_cast<uint32_t>(smem);
+	return g;
+}
+
 // CTAs of a persistent launch (each CTA starts at unit blockIdx.x and steps by gridDim.x): one per unit, at most `per_sm` per SM,
-// and at most LZGPU_GRID_CAP when that is set
-static int persistent_grid(lzgpu_ctx *ctx, uint64_t total_units, int per_sm) {
+// and at most LZGPU_GRID_CAP when that is set.  Records the launch (geo, completed with grid and units) as the context's latest.
+static int persistent_grid(lzgpu_ctx *ctx, uint64_t total_units, int per_sm, lzgpu_launch_geometry geo) {
 	FusedState *fs = ctx->fused;
 	uint64_t grid = std::min<uint64_t>(total_units, static_cast<uint64_t>(ctx->sm_count) * per_sm);
 	if (fs->grid_cap) grid = std::min<uint64_t>(grid, fs->grid_cap);
-	fs->last_launch.store(grid << 32 | total_units);
+	geo.grid = static_cast<uint32_t>(grid);
+	geo.units = static_cast<uint32_t>(total_units);
+	std::lock_guard<std::mutex> lock(fs->last_mu);
+	fs->last_geo = geo;
 	return static_cast<int>(grid);
 }
 
@@ -277,9 +294,16 @@ void lz_fused_destroy(lzgpu_ctx *ctx) {
 
 extern "C" int lzgpu_debug_last_launch(lzgpu_ctx *ctx, uint32_t *grid, uint32_t *units) {
 	if (!ctx || !ctx->fused || !grid || !units) return LZGPU_ERR_ARG;
-	const uint64_t v = ctx->fused->last_launch.load();
-	*grid = static_cast<uint32_t>(v >> 32);
-	*units = static_cast<uint32_t>(v);
+	std::lock_guard<std::mutex> lock(ctx->fused->last_mu);
+	*grid = ctx->fused->last_geo.grid;
+	*units = ctx->fused->last_geo.units;
+	return LZGPU_OK;
+}
+
+extern "C" int lzgpu_debug_last_geometry(lzgpu_ctx *ctx, lzgpu_launch_geometry *out) {
+	if (!ctx || !ctx->fused || !out) return LZGPU_ERR_ARG;
+	std::lock_guard<std::mutex> lock(ctx->fused->last_mu);
+	*out = ctx->fused->last_geo;
 	return LZGPU_OK;
 }
 
@@ -303,7 +327,8 @@ static int make_tensor_map(FusedState *fs, CUtensorMap *map, const void *base, u
 
 template <int M, bool GENERIC, int KT = 0, int GT = 0, int FW = 64, bool STRIPED = false, bool SPLIT = false>
 static int launch(lzgpu_ctx *ctx, const CUtensorMap &map, const FusedParams &p, size_t smem, cudaStream_t st) {
-	const int grid = persistent_grid(ctx, p.total_units, fused_ctas_per_sm(M, GENERIC, FW));
+	const int grid = persistent_grid(ctx, p.total_units, fused_ctas_per_sm(M, GENERIC, FW),
+	                                 launch_geo(LZGPU_KERNEL_ENCODE, fused_threads(M, GENERIC), p.G, fused_nst(FW, M, GENERIC), 0, smem));
 	if (GENERIC && fused_generic_item_words(p.G) == 1)
 		fused_stream_kernel<M, GENERIC, KT, GT, FW, STRIPED, SPLIT, GENERIC ? 1 : fused_item_words(M, GENERIC)><<<grid, fused_threads(M, GENERIC), smem, st>>>(map, p);
 	else
@@ -322,7 +347,7 @@ static int set_bs_attr() {
 }
 template <int M, int KT = 0, int GT = 0, bool STRIPED = false>
 static int launch_bs(lzgpu_ctx *ctx, const CUtensorMap &map, const FusedParams &p, size_t smem, cudaStream_t st) {
-	const int grid = persistent_grid(ctx, p.total_units, 1);
+	const int grid = persistent_grid(ctx, p.total_units, 1, launch_geo(LZGPU_KERNEL_ENCODE_BITSLICE, kBsThreads, p.G, p.n_stages, (16 * p.G + 31) / 32, smem));
 	fused_stream_kernel<M, false, KT, GT, 64, STRIPED, false, 8><<<grid, kBsThreads, smem, st>>>(map, p);
 	CUDA_TRY(cudaGetLastError());
 	ctx->stats.kernel_launches++;
@@ -611,7 +636,7 @@ int lz_fused_crc(lzgpu_ctx *ctx, const void *base, unsigned long long n_blocks, 
 // DIRECT form of the degraded read (any generator; the Cauchy codes): 16-warp CTA, runtime k, 16- or 4-byte items
 template <int E>
 static int launch_direct(lzgpu_ctx *ctx, const TmapArray &maps, const RecoverParams &p, size_t smem, cudaStream_t st, bool wide) {
-	const int grid = persistent_grid(ctx, p.total_units, 1);
+	const int grid = persistent_grid(ctx, p.total_units, 1, launch_geo(LZGPU_KERNEL_RECOVER_DIRECT, recover_threads(2), p.G, p.n_stages, 0, smem));
 	if (wide) fused_recover_kernel<E, 0, kRecoverDirect, -1, 64, 2, kDirectWide<E>><<<grid, recover_threads(2), smem, st>>>(maps, p);
 	else fused_recover_kernel<E, 0, kRecoverDirect, -1, 64, 2, 1><<<grid, recover_threads(2), smem, st>>>(maps, p);
 	CUDA_TRY(cudaGetLastError());
@@ -622,7 +647,7 @@ static int launch_direct(lzgpu_ctx *ctx, const TmapArray &maps, const RecoverPar
 // the 16-warp geometry alone (instantiations with a compile-time k other than 8: ec(3,2), the BASELINE configs[1] goal)
 template <int E, int KT, int R0, int R1>
 static int launch_recover_geo2(lzgpu_ctx *ctx, const TmapArray &maps, const RecoverParams &p, size_t smem, cudaStream_t st) {
-	const int gridb = persistent_grid(ctx, p.total_units, 1);
+	const int gridb = persistent_grid(ctx, p.total_units, 1, launch_geo(LZGPU_KERNEL_RECOVER_GEO2, recover_threads(2), p.G, p.n_stages, 0, smem));
 	fused_recover_kernel<E, KT, R0, R1, 64, 2><<<gridb, recover_threads(2), smem, st>>>(maps, p);
 	CUDA_TRY(cudaGetLastError());
 	ctx->stats.kernel_launches++;
@@ -632,20 +657,20 @@ static int launch_recover_geo2(lzgpu_ctx *ctx, const TmapArray &maps, const Reco
 template <int E, int KT, int R0 = -1, int R1 = -1>
 static int launch_recover(lzgpu_ctx *ctx, const TmapArray &maps, const RecoverParams &p, size_t smem, cudaStream_t st, int geo) {
 	if (geo == 2) {
-		const int gridb = persistent_grid(ctx, p.total_units, 1);
+		const int gridb = persistent_grid(ctx, p.total_units, 1, launch_geo(LZGPU_KERNEL_RECOVER_GEO2, recover_threads(2), p.G, p.n_stages, 0, smem));
 		fused_recover_kernel<E, KT, R0, R1, 64, 2><<<gridb, recover_threads(2), smem, st>>>(maps, p);
 		CUDA_TRY(cudaGetLastError());
 		ctx->stats.kernel_launches++;
 		return LZGPU_OK;
 	}
 	if (geo == 1 && E <= 2) {
-		const int grid2 = persistent_grid(ctx, p.total_units, 2);
+		const int grid2 = persistent_grid(ctx, p.total_units, 2, launch_geo(LZGPU_KERNEL_RECOVER_GEO1, kFusedThreads, p.G, recover_stages(1), 0, smem));
 		fused_recover_kernel<(E <= 2 ? E : 1), KT, R0, R1, 64, 1><<<grid2, kFusedThreads, smem, st>>>(maps, p);
 		CUDA_TRY(cudaGetLastError());
 		ctx->stats.kernel_launches++;
 		return LZGPU_OK;
 	}
-	const int grid = persistent_grid(ctx, p.total_units, 1);
+	const int grid = persistent_grid(ctx, p.total_units, 1, launch_geo(LZGPU_KERNEL_RECOVER_GEO0, kFusedThreads, p.G, recover_stages(0), 0, smem));
 #ifdef LZ_ENABLE_FOLD128
 	if (ctx->fused->fold == 128) fused_recover_kernel<E, KT, R0, R1, 128><<<grid, kFusedThreads, smem, st>>>(maps, p);
 	else
@@ -875,7 +900,7 @@ int lz_fused_recover(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, 
 		bs_mask_set(mk.m[3], delta);
 		bs_mask_set(mk.m[4], A);
 		bs_mask_set(mk.m[5], lz::gf_mul_host(A, A));
-		const int grid = persistent_grid(ctx, p.total_units, 1);
+		const int grid = persistent_grid(ctx, p.total_units, 1, launch_geo(LZGPU_KERNEL_RECOVER_BS3, kBsRecoverThreads, G, n_stages, (16 * G + 31) / 32, smem));
 		if (K == 5) bs_recover3_kernel<5><<<grid, kBsRecoverThreads, smem, st>>>(maps, p, mk);
 		else if (K == 8) bs_recover3_kernel<8><<<grid, kBsRecoverThreads, smem, st>>>(maps, p, mk);
 		else bs_recover3_kernel<0><<<grid, kBsRecoverThreads, smem, st>>>(maps, p, mk);
@@ -932,8 +957,8 @@ int lz_fused_recover(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, 
 // fused slice conversion (convert_kernel.cuh)
 // ---------------------------------------------------------------------------------------------------
 template <int M, int E>
-static int launch_convert(lzgpu_ctx *ctx, const TmapArray &maps, const ConvertParams &p, size_t smem, cudaStream_t st) {
-	const int grid = persistent_grid(ctx, p.total_units, 2);
+static int launch_convert(lzgpu_ctx *ctx, const TmapArray &maps, const ConvertParams &p, size_t smem, cudaStream_t st, uint32_t rebuild_warps) {
+	const int grid = persistent_grid(ctx, p.total_units, 2, launch_geo(LZGPU_KERNEL_CONVERT, kConvertThreads, p.G, p.n_stages, rebuild_warps, smem));
 	if (M <= 2 && p.Kd == 3) fused_convert_kernel<(M <= 2 ? M : 1), E, 3><<<grid, kConvertThreads, smem, st>>>(maps, p);   // xor3 / ec(3,2) destinations
 	else fused_convert_kernel<M, E><<<grid, kConvertThreads, smem, st>>>(maps, p);
 	CUDA_TRY(cudaGetLastError());
@@ -1020,9 +1045,11 @@ int lz_fused_convert(lzgpu_ctx *ctx, const lzgpu_goal *src, const lzgpu_goal *ds
 		coef_planes_set(p.w[1], lz::gf_inv_host(gx0 ^ gx1));
 	}
 	p.dbl0 = (e == 2 && p.erased_idx[0] <= 4) ? p.erased_idx[0] : 0xffu;
+	const uint32_t rebuild_warps = kConvertThreads / 32 - pl.n_workers;   // (0 without lost parts: every warp is a worker)
 #define LZ_CONVERT_CASE(MM) \
 	case MM: \
-		return e == 0 ? launch_convert<MM, 0>(ctx, maps, p, smem, st) : e == 1 ? launch_convert<MM, 1>(ctx, maps, p, smem, st) : launch_convert<MM, 2>(ctx, maps, p, smem, st);
+		return e == 0 ? launch_convert<MM, 0>(ctx, maps, p, smem, st, rebuild_warps) : e == 1 ? launch_convert<MM, 1>(ctx, maps, p, smem, st, rebuild_warps) \
+		              : launch_convert<MM, 2>(ctx, maps, p, smem, st, rebuild_warps);
 	switch (Md) {
 		LZ_CONVERT_CASE(1)
 		LZ_CONVERT_CASE(2)

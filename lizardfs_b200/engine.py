@@ -407,6 +407,13 @@ class Engine:
         _check(self.lib.lzgpu_debug_last_launch(self.h, C.byref(grid), C.byref(units)), "debug_last_launch")
         return grid.value, units.value
 
+    def last_geometry(self):
+        """geometry of the same launch as last_launch() (lzgpu_debug_last_geometry): a dict of kernel (_lib.KERNEL_*), grid, units,
+        threads, G (stripes per unit), stages, gf_warps and smem_bytes"""
+        g = _lib.LzLaunchGeometry()
+        _check(self.lib.lzgpu_debug_last_geometry(self.h, C.byref(g)), "debug_last_geometry")
+        return {f: getattr(g, f) for f, _ in _lib.LzLaunchGeometry._fields_}
+
     def status_slots(self):
         """(allocated, in_use) verification result slots of this context (lzgpu_debug_status_slots)"""
         allocated, in_use = C.c_uint32(), C.c_uint32()
