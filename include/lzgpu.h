@@ -177,7 +177,8 @@ enum {
 	LZGPU_KERNEL_RECOVER_GEO2 = 5,     /* fused_recover_kernel: one 16-warp CTA per SM */
 	LZGPU_KERNEL_RECOVER_DIRECT = 6,   /* fused_recover_kernel, DIRECT form (Cauchy generators) */
 	LZGPU_KERNEL_RECOVER_BS3 = 7,      /* bs_recover3_kernel: three lost data parts on bit planes */
-	LZGPU_KERNEL_CONVERT = 8           /* fused_convert_kernel: one-pass slice conversion */
+	LZGPU_KERNEL_CONVERT = 8,          /* fused_convert_kernel: one-pass slice conversion */
+	LZGPU_KERNEL_CHECK = 9             /* fused_check_kernel: stripe check (lzgpu_check_stripes), one 16-warp CTA per SM */
 };
 typedef struct lzgpu_launch_geometry {
 	int kernel;
@@ -279,6 +280,40 @@ int lzgpu_recover_chunks_dev(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_
 /* Alignment (lzgpu_recover_chunks_dev, lzgpu_split_chunks_dev, lzgpu_convert_chunks_dev): every non-NULL part, output and image
  * pointer must be 16-byte aligned and every non-NULL CRC array 4-byte aligned; strides are multiples of 16.  Otherwise the call
  * returns LZGPU_ERR_ARG before anything is enqueued. */
+
+/* Stripe check: do the k+m parts of every chunk still form a codeword?  Every stored CRC covers one part's own bytes, so parts that
+ * stopped agreeing (a write that reached some parts of a stripe only, a part restored from another version, a bit flip upstream of
+ * the CRC) pass every scrub, and a degraded read or conversion from them returns wrong bytes with LZGPU_OK.
+ *   parts, part_stride, part_crc, bad   as in lzgpu_recover_chunks (layout, zero padding of short parts, stored CRCs, bad[0..2],
+ *                                       alignment, the CRC-disabled mode).  Every data part is required; a NULL parity part is a row
+ *                                       that is not checked, and at least one parity part must be given (otherwise
+ *                                       LZGPU_ERR_TOO_FEW_PARTS, before anything is enqueued).  Every given part is verified against
+ *                                       its stored CRCs in the same pass.
+ *   verdict[c]  (n_chunks entries, written for every chunk whether or not a stored CRC failed):
+ *     first_bad_stripe  lowest stripe s (= part block s) whose syndromes S_r = p_r ^ sum_j g_rj d_j are not all zero; -1: none
+ *     bad_rows          bit r: parity row r is checked and its syndrome is non-zero somewhere in that stripe
+ *     suspect_part      the part (this API's numbering) whose corruption alone explains that stripe: at every byte with a non-zero
+ *                       syndrome vector, the vector is a multiple of the part's column of H = [parity rows of the generator | I]
+ *                       restricted to the checked rows; -1 when no single part or more than one does.  With one checked row (xorN, or
+ *                       one parity part given) it is always -1.  With two checked rows two corrupt parts can look like a third,
+ *                       single one — a property of the code, not of this check.  With three or more checked rows two corrupt parts
+ *                       never produce a suspect.  Rebuild the suspect with lzgpu_convert_chunks.
+ * lzgpu_check_stripes returns LZGPU_ERR_CRC when a stored CRC failed, else LZGPU_ERR_INCONSISTENT when any chunk has a bad stripe,
+ * else LZGPU_OK.  lzgpu_check_stripes_dev writes the verdicts to d_verdict (device memory, 4-byte aligned; nothing else is written)
+ * on `stream` and, like lzgpu_recover_chunks_dev, waits for the stream only to report a stored-CRC verdict (deferred mode moves that
+ * to lzgpu_dev_sync); it returns LZGPU_OK or LZGPU_ERR_CRC and the caller reads the verdicts once the stream has passed the call. */
+#define LZGPU_ERR_INCONSISTENT (-8) /* some stripe's parts do not form a codeword (lzgpu_check_stripes) */
+typedef struct lzgpu_stripe_verdict {
+	int32_t first_bad_stripe; /* lowest stripe s (= part block s) whose syndromes are not all zero; -1: every stripe is a codeword */
+	uint32_t bad_rows;        /* bit r: parity row r (checked, non-zero syndrome) in that stripe */
+	int32_t suspect_part;     /* the one part (this API's numbering) whose error explains every syndrome byte of that stripe, else -1 */
+} lzgpu_stripe_verdict;
+int lzgpu_check_stripes(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, uint32_t nb,
+                        const uint8_t *const *parts, size_t part_stride, const uint32_t *const *part_crc,
+                        lzgpu_stripe_verdict *verdict, int64_t *bad);
+int lzgpu_check_stripes_dev(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, uint32_t nb,
+                            const void *const *d_parts, size_t part_stride, const void *const *d_part_crc,
+                            void *d_verdict, int64_t *bad, void *stream);
 
 /* Wire-format producer (SURVEY.md §8 f3): LIZ_CLTOCS_WRITE_DATA packet prefixes (src/protocol/cltocs.h:116-137) for
  * every block of every part of the encoded chunks, built on the GPU straight from the CRC array of

@@ -11,7 +11,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("LZGPU_LIB") or os.path.join(_HERE, "liblzgpu.so")
 
 OK = 0
-ERR_ARG, ERR_CUDA, ERR_NOMEM, ERR_CRC, ERR_TOO_FEW_PARTS, ERR_NO_DEVICE, ERR_DAMAGED = -1, -2, -3, -4, -5, -6, -7
+ERR_ARG, ERR_CUDA, ERR_NOMEM, ERR_CRC, ERR_TOO_FEW_PARTS, ERR_NO_DEVICE, ERR_DAMAGED, ERR_INCONSISTENT = -1, -2, -3, -4, -5, -6, -7, -8
 BLOCK_SIZE = 65536
 BLOCKS_IN_CHUNK = 1024
 CHUNK_SIZE = BLOCK_SIZE * BLOCKS_IN_CHUNK
@@ -46,7 +46,11 @@ class LzLaunchGeometry(C.Structure):
 
 # lzgpu_launch_geometry.kernel
 KERNEL_NONE, KERNEL_ENCODE, KERNEL_ENCODE_BITSLICE, KERNEL_RECOVER_GEO0, KERNEL_RECOVER_GEO1, KERNEL_RECOVER_GEO2, \
-    KERNEL_RECOVER_DIRECT, KERNEL_RECOVER_BS3, KERNEL_CONVERT = range(9)
+    KERNEL_RECOVER_DIRECT, KERNEL_RECOVER_BS3, KERNEL_CONVERT, KERNEL_CHECK = range(10)
+
+
+class LzStripeVerdict(C.Structure):
+    _fields_ = [("first_bad_stripe", C.c_int32), ("bad_rows", C.c_uint32), ("suspect_part", C.c_int32)]
 
 
 class LzBlockWrite(C.Structure):
@@ -87,6 +91,8 @@ SIGNATURES = {
     "lzgpu_encode_chunks_dev": (_int, [_vp, _goalp, _u32, _u32, _vp, _sz, _vp, _sz, _vp, _sz, _vp]),
     "lzgpu_recover_chunks": (_int, [_vp, _goalp, _u32, _u32, _vp, _sz, _vp, _vp, _vp, _vp, _sz, _vp]),
     "lzgpu_recover_chunks_dev": (_int, [_vp, _goalp, _u32, _u32, _vp, _sz, _vp, _vp, _vp, _vp, _sz, _vp, _vp]),
+    "lzgpu_check_stripes": (_int, [_vp, _goalp, _u32, _u32, _vp, _sz, _vp, _vp, _vp]),
+    "lzgpu_check_stripes_dev": (_int, [_vp, _goalp, _u32, _u32, _vp, _sz, _vp, _vp, _vp, _vp]),
     "lzgpu_write_data_prefixes": (_int, [_vp, _goalp, _u32, _u32, _vp, _sz, _vp, _u32, _vp]),
     "lzgpu_write_data_prefixes_dev": (_int, [_vp, _goalp, _u32, _u32, _vp, _sz, _vp, _u32, _vp, _vp]),
     "lzgpu_split_chunks": (_int, [_vp, _goalp, _u32, _u32, _vp, _sz, _vp, _sz]),

@@ -434,15 +434,21 @@ int lz_scratch(lzgpu_ctx *ctx, int slot, size_t bytes, void **out) {
 // tile verifies stored CRCs.  Stream order alone keeps a slot's staging buffers safe to re-use; a slot whose tile armed a
 // verification is waited for and its verdict taken before the slot is re-used, and at the end every slot is retired oldest
 // first, so the first CRC mismatch of the batch is the one reported (bad[0]: the chunk's index in the whole batch).  Every
-// stream that was used is idle when the call returns, after an error too.
+// stream that was used is idle when the call returns, after an error too.  every_tile: a CRC mismatch does not stop the pipeline (the
+// caller's other results are still wanted); the first one is reported once every tile has run.
 template <class Stage>
-static int run_tiles(lzgpu_ctx *ctx, size_t n_items, size_t tile, int n_slots, int64_t *bad, Stage &&stage) {
+static int run_tiles(lzgpu_ctx *ctx, size_t n_items, size_t tile, int n_slots, int64_t *bad, Stage &&stage, bool every_tile = false) {
 	VerifyTicket tk[kHostSlots];
 	size_t first[kHostSlots] = {};
+	int crc_rc = LZGPU_OK;
 	auto retire = [&](int s) {
 		int64_t local[3];
 		const int rc = tk[s].wait_take(local);
-		if (rc == LZGPU_ERR_CRC && bad) { bad[0] = local[0] + static_cast<int64_t>(first[s]); bad[1] = local[1]; bad[2] = local[2]; }
+		if (rc == LZGPU_ERR_CRC && bad && !crc_rc) { bad[0] = local[0] + static_cast<int64_t>(first[s]); bad[1] = local[1]; bad[2] = local[2]; }
+		if (rc == LZGPU_ERR_CRC && every_tile) {
+			crc_rc = rc;
+			return LZGPU_OK;
+		}
 		return rc;
 	};
 	int rc = LZGPU_OK;
@@ -463,7 +469,7 @@ static int run_tiles(lzgpu_ctx *ctx, size_t n_items, size_t tile, int n_slots, i
 		}
 	}
 	cudaGetLastError();
-	return rc;
+	return rc ? rc : crc_rc;
 }
 
 static int grid_for(const lzgpu_ctx *ctx, unsigned long long work_items, int threads, int ctas_per_sm) {
@@ -475,6 +481,33 @@ static int grid_for(const lzgpu_ctx *ctx, unsigned long long work_items, int thr
 // ------------------------------------------------------------------------------------------------
 // device-level building blocks (all asynchronous on `st`)
 // ------------------------------------------------------------------------------------------------
+// the kernel arguments of dot-product pass r0 .. r0 + nd - 1; returns its dynamic shared memory
+static size_t dot_pass_args(const DotDesc &d, const uint8_t *coef, unsigned r0, unsigned nd, DotArgs &a) {
+	bool all_one = true;
+	for (unsigned j = 0; j < d.n_src; ++j) a.src[j] = d.src[j];
+	for (unsigned r = 0; r < nd; ++r) {
+		a.dst[r] = d.dst[r0 + r];
+		for (unsigned j = 0; j < d.n_src; ++j) {
+			const uint8_t c = coef[(r0 + r) * d.n_src + j];
+			all_one &= c == 1;
+			a.coef[r * d.n_src + j] = c;  // the coefficients travel in the kernel parameters; the kernel expands them to planes
+		}
+	}
+	a.total_units = d.total_units;
+	a.src_chunk_stride = d.src_chunk_stride;
+	a.src_block_stride = d.src_block_stride;
+	a.dst_chunk_stride = d.dst_chunk_stride;
+	a.dst_block_stride = d.dst_block_stride;
+	a.units_per_block = d.units_per_block;
+	a.blocks_per_chunk = d.blocks_per_chunk;
+	a.n_src = d.n_src;
+	a.n_dst = nd;
+	a.valid_k = d.valid_k;
+	a.valid_nb = d.valid_nb;
+	a.pure_xor = all_one ? 1u : 0u;
+	return sizeof(CoefPlanes) * nd * d.n_src;
+}
+
 // dst[r] = XOR_j coef[r][j] * src[j]  over the addressing described in DotDesc
 int lz_gf_dot(lzgpu_ctx *ctx, const DotDesc &d, const uint8_t *coef /* n_dst x n_src */, cudaStream_t st) {
 	if (d.n_src < 1 || d.n_src > kMaxSrc || d.n_dst < 1) return LZGPU_ERR_ARG;
@@ -482,36 +515,35 @@ int lz_gf_dot(lzgpu_ctx *ctx, const DotDesc &d, const uint8_t *coef /* n_dst x n
 	for (unsigned r0 = 0; r0 < d.n_dst; r0 += kDotDests) {
 		const unsigned nd = std::min<unsigned>(kDotDests, d.n_dst - r0);
 		DotArgs a{};
-		bool all_one = true;
-		for (unsigned j = 0; j < d.n_src; ++j) a.src[j] = d.src[j];
-		for (unsigned r = 0; r < nd; ++r) {
-			a.dst[r] = d.dst[r0 + r];
-			for (unsigned j = 0; j < d.n_src; ++j) {
-				const uint8_t c = coef[(r0 + r) * d.n_src + j];
-				all_one &= c == 1;
-				a.coef[r * d.n_src + j] = c;  // the coefficients travel in the kernel parameters; the kernel expands them to planes
-			}
-		}
-		a.total_units = d.total_units;
-		a.src_chunk_stride = d.src_chunk_stride;
-		a.src_block_stride = d.src_block_stride;
-		a.dst_chunk_stride = d.dst_chunk_stride;
-		a.dst_block_stride = d.dst_block_stride;
-		a.units_per_block = d.units_per_block;
-		a.blocks_per_chunk = d.blocks_per_chunk;
-		a.n_src = d.n_src;
-		a.n_dst = nd;
-		a.valid_k = d.valid_k;
-		a.valid_nb = d.valid_nb;
-		a.pure_xor = all_one ? 1u : 0u;
+		const size_t smem = dot_pass_args(d, coef, r0, nd, a);
 		const int threads = 256;
 		const int grid = grid_for(ctx, d.total_units, threads, 8);
-		const size_t smem = sizeof(CoefPlanes) * nd * d.n_src;
 		switch (nd) {
 			case 1: gf_dot_kernel<1><<<grid, threads, smem, st>>>(a); break;
 			case 2: gf_dot_kernel<2><<<grid, threads, smem, st>>>(a); break;
 			case 3: gf_dot_kernel<3><<<grid, threads, smem, st>>>(a); break;
 			default: gf_dot_kernel<4><<<grid, threads, smem, st>>>(a); break;
+		}
+		CUDA_TRY(cudaGetLastError());
+		ctx->stats.kernel_launches++;
+	}
+	return LZGPU_OK;
+}
+
+// the same dot products compared with the stored rows d.dst[r] (read only): a 16-byte unit of chunk c, block s that differs lowers
+// verdict[3c] to s (lzgpu_check_stripes, generic route; no parity-sized temporary)
+static int lz_gf_check(lzgpu_ctx *ctx, const DotDesc &d, const uint8_t *coef, int *verdict, cudaStream_t st) {
+	for (unsigned r0 = 0; r0 < d.n_dst; r0 += kDotDests) {
+		const unsigned nd = std::min<unsigned>(kDotDests, d.n_dst - r0);
+		DotArgs a{};
+		const size_t smem = dot_pass_args(d, coef, r0, nd, a);
+		const int threads = 256;
+		const int grid = grid_for(ctx, d.total_units, threads, 8);
+		switch (nd) {
+			case 1: gf_check_kernel<1><<<grid, threads, smem, st>>>(a, verdict); break;
+			case 2: gf_check_kernel<2><<<grid, threads, smem, st>>>(a, verdict); break;
+			case 3: gf_check_kernel<3><<<grid, threads, smem, st>>>(a, verdict); break;
+			default: gf_check_kernel<4><<<grid, threads, smem, st>>>(a, verdict); break;
 		}
 		CUDA_TRY(cudaGetLastError());
 		ctx->stats.kernel_launches++;
@@ -1000,6 +1032,193 @@ extern "C" int lzgpu_recover_chunks(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint
 		}
 		return LZGPU_OK;
 	});
+}
+
+// ------------------------------------------------------------------------------------------------
+// stripe check: do the parts of every stripe still form a codeword?
+// ------------------------------------------------------------------------------------------------
+// dev: device pointers, whose alignment the kernels need (the host variant stages into aligned buffers)
+static int check_args(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t nb, const void *const *parts, const void *const *part_crc,
+                      const void *verdict, bool dev) {
+	if (!ctx || !parts || !verdict) return LZGPU_ERR_ARG;
+	int rc = check_goal(goal);
+	if (rc) return rc;
+	if (nb == 0 || nb > LZGPU_BLOCKS_IN_CHUNK) { lz_set_error("nb out of range"); return LZGPU_ERR_ARG; }
+	const int k = goal->k, n = goal->k + goal->m;
+	bool any_parity = false;
+	for (int i = 0; i < n; ++i) {
+		if (i < k && !parts[i]) { lz_set_error("check_stripes: data part %d is missing; every data part is required", i); return LZGPU_ERR_TOO_FEW_PARTS; }
+		any_parity |= i >= k && parts[i];
+	}
+	if (!any_parity) { lz_set_error("check_stripes: no parity part given, nothing to check"); return LZGPU_ERR_TOO_FEW_PARTS; }
+	if (!dev) return LZGPU_OK;
+	if ((rc = check_part_ptrs("check_stripes", "parts", parts, n, 16)) || (rc = check_part_ptrs("check_stripes", "part_crc", part_crc, n, 4))) return rc;
+	if (reinterpret_cast<uintptr_t>(verdict) & 3) { lz_set_error("check_stripes: verdict is not 4-byte aligned"); return LZGPU_ERR_ARG; }
+	return LZGPU_OK;
+}
+
+// enqueue the whole check on `st` (arguments validated by check_args); *tk is armed when stored CRCs are verified
+static int check_enqueue(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, uint32_t nb, const void *const *d_parts, size_t part_stride,
+                         const void *const *d_part_crc, void *d_verdict, cudaStream_t st, VerifyTicket *tk) {
+	const int k = goal->k, m = goal->m, n = k + m;
+	const uint32_t B = LZGPU_BLOCK_SIZE;
+	const uint32_t pb = (nb + k - 1) / k;
+	if (part_stride < static_cast<size_t>(pb) * B || (part_stride & 15)) { lz_set_error("check_stripes: bad part_stride"); return LZGPU_ERR_ARG; }
+	bool any_crc = false;
+	for (int i = 0; i < n; ++i) any_crc |= d_parts[i] && d_part_crc && d_part_crc[i];
+	int rc;
+	if (any_crc && (rc = tk->arm(ctx, st))) return rc;
+	// first_bad_stripe of every chunk starts above any stripe; the check kernels lower it, locate_kernel writes the whole verdict
+	CUDA_TRY(cudaMemsetAsync(d_verdict, 0x7f, static_cast<size_t>(n_chunks) * sizeof(lzgpu_stripe_verdict), st));
+	TmpBuf tmp_crc(ctx, st);
+	auto verify_inputs = [&]() -> int {
+		int r;
+		for (int i = 0; i < n; ++i)
+			if (d_parts[i] && d_part_crc[i] &&
+			    (r = verify_part(ctx, d_parts[i], n_chunks, pb, part_stride, d_part_crc[i], tmp_crc.p, tk->word(i), st)))
+				return r;
+		return LZGPU_OK;
+	};
+	const void *const *crc_for_kernels = d_part_crc;
+	if (any_crc && !lzgpu_crc_enabled()) {
+		if ((rc = verify_inputs())) return rc;  // the constant, before either route, as in the degraded read
+		crc_for_kernels = nullptr;
+	}
+	uint8_t gen_rows[LZGPU_MAX_PARITY * LZGPU_MAX_DATA];
+	goal_parity_rows(goal, gen_rows);
+	LocateArgs la{};
+	for (int i = 0; i < n; ++i) la.part[i] = static_cast<const uint8_t *>(d_parts[i]);
+	for (int r = 0; r < m; ++r)
+		if (d_parts[k + r]) {
+			la.row[la.n_rows] = static_cast<uint8_t>(r);
+			std::memcpy(la.coef + 32 * la.n_rows, gen_rows + r * k, k);
+			++la.n_rows;
+		}
+
+	rc = lz_fused_check(ctx, goal, n_chunks, nb, d_parts, part_stride, crc_for_kernels, d_verdict, st, tk->word(0));
+	const bool fused = rc != LZGPU_NOT_HANDLED;
+	if (fused && rc) return rc;
+	if (!fused) {
+		// generic route: stored CRCs part by part, then the parity rows recomputed from the data parts and compared per 16-byte unit
+		if (any_crc && crc_for_kernels && ((rc = tmp_crc.alloc(static_cast<size_t>(n_chunks) * pb * 4)) || (rc = verify_inputs()))) return rc;
+		uint8_t rows[LZGPU_MAX_PARITY * LZGPU_MAX_DATA];
+		uint8_t *stored[LZGPU_MAX_PARITY];
+		for (uint32_t i = 0; i < la.n_rows; ++i) {
+			std::memcpy(rows + i * k, la.coef + 32 * i, k);
+			stored[i] = const_cast<uint8_t *>(la.part[k + la.row[i]]);
+		}
+		DotDesc d{};
+		for (int j = 0; j < k; ++j) d.src[j] = la.part[j];
+		d.dst = stored;
+		d.n_src = k;
+		d.n_dst = la.n_rows;
+		d.total_units = static_cast<unsigned long long>(n_chunks) * pb * (B / 16);
+		d.src_chunk_stride = d.dst_chunk_stride = part_stride;
+		d.src_block_stride = d.dst_block_stride = B;
+		d.units_per_block = B / 16;
+		d.blocks_per_chunk = pb;
+		if ((rc = lz_gf_check(ctx, d, rows, static_cast<int *>(d_verdict), st))) return rc;
+	}
+	la.verdict = static_cast<int *>(d_verdict);
+	la.part_stride = part_stride;
+	la.k = k;
+	la.pb = pb;
+	locate_kernel<<<n_chunks, 256, 0, st>>>(la);
+	CUDA_TRY(cudaGetLastError());
+	ctx->stats.kernel_launches++;
+	if (!any_crc) return LZGPU_OK;
+	return (fused && crc_for_kernels) ? tk->publish_fused() : tk->publish_per_part(n, pb);
+}
+
+static uint64_t check_alg_bytes(const lzgpu_goal *goal, uint32_t n_chunks, uint32_t nb, const void *const *parts, const void *const *part_crc) {
+	// read every given part and its stored CRCs, write one verdict per chunk
+	const uint64_t pb = (nb + goal->k - 1) / goal->k, B = LZGPU_BLOCK_SIZE;
+	uint64_t bytes = sizeof(lzgpu_stripe_verdict);
+	for (int i = 0; i < goal->k + goal->m; ++i)
+		if (parts[i]) bytes += pb * B + ((part_crc && part_crc[i]) ? 4 * pb : 0);
+	return n_chunks * bytes;
+}
+
+extern "C" int lzgpu_check_stripes_dev(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, uint32_t nb, const void *const *d_parts,
+                                       size_t part_stride, const void *const *d_part_crc, void *d_verdict, int64_t *bad, void *stream) {
+	NvtxScope nvtx_scope("lzgpu::check_stripes_dev");
+	int rc = check_args(ctx, goal, nb, d_parts, d_part_crc, d_verdict, true);
+	if (rc) return rc;
+	if (n_chunks == 0) return LZGPU_OK;
+	DeviceGuard g(ctx->device);
+	cudaStream_t st = stream ? static_cast<cudaStream_t>(stream) : ctx->stream;
+	VerifyTicket tk;
+	{
+		BatchTimer timer(ctx, st, check_alg_bytes(goal, n_chunks, nb, d_parts, d_part_crc));
+		if ((rc = check_enqueue(ctx, goal, n_chunks, nb, d_parts, part_stride, d_part_crc, d_verdict, st, &tk))) return rc;
+	}
+	return dev_verdict(ctx, std::move(tk), bad);
+}
+
+extern "C" int lzgpu_check_stripes(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, uint32_t nb, const uint8_t *const *parts,
+                                   size_t part_stride, const uint32_t *const *part_crc, lzgpu_stripe_verdict *verdict, int64_t *bad) {
+	NvtxScope nvtx_scope("lzgpu::check_stripes");
+	int rc = check_args(ctx, goal, nb, reinterpret_cast<const void *const *>(parts), nullptr, verdict, false);
+	if (rc) return rc;
+	if (n_chunks == 0) return LZGPU_OK;
+	const int k = goal->k, n = goal->k + goal->m;
+	const uint32_t B = LZGPU_BLOCK_SIZE;
+	const uint32_t pb = (nb + k - 1) / k;
+	const size_t part_bytes = static_cast<size_t>(pb) * B;
+	if (part_stride < part_bytes) { lz_set_error("check_stripes: part_stride too small"); return LZGPU_ERR_ARG; }
+	int n_given = 0;
+	for (int i = 0; i < n; ++i) n_given += parts[i] ? 1 : 0;
+	std::lock_guard<std::mutex> lk(ctx->mu);
+	DeviceGuard g(ctx->device);
+	AutoPin pin(ctx);
+	for (int i = 0; i < n; ++i)
+		if (parts[i]) pin.add(parts[i], static_cast<size_t>(n_chunks - 1) * part_stride + part_bytes);
+	pin.add(verdict, static_cast<size_t>(n_chunks) * sizeof(lzgpu_stripe_verdict));
+	// device layout of a tile: every given part dense (stride = part_bytes), all parts of a slot in one buffer
+	const uint32_t tile = static_cast<uint32_t>(std::max<size_t>(1, std::min<size_t>(n_chunks, (2 * kHostTileBytes) / (part_bytes * n_given))));
+	const size_t dev_part = static_cast<size_t>(tile) * part_bytes;
+	const size_t dev_crc = static_cast<size_t>(tile) * pb * 4;
+	void *d_all[kHostSlots], *d_crc_all[kHostSlots], *d_ver[kHostSlots];
+	const int n_slots = n_chunks > tile ? kHostSlots : 1;
+	for (int s = 0; s < n_slots; ++s) {
+		if ((rc = lz_scratch(ctx, kScratchIn0 + s, dev_part * n, &d_all[s]))) return rc;
+		if ((rc = lz_scratch(ctx, kScratchCrc0 + s, dev_crc * n, &d_crc_all[s]))) return rc;
+		if ((rc = lz_scratch(ctx, kScratchPar0 + s, static_cast<size_t>(tile) * sizeof(lzgpu_stripe_verdict), &d_ver[s]))) return rc;
+	}
+	// a stored-CRC mismatch does not stop the pipeline: every chunk gets its verdict
+	rc = run_tiles(ctx, n_chunks, tile, n_slots, bad, [&](int s, size_t c0, size_t nc, cudaStream_t st, VerifyTicket *tk) -> int {
+		std::vector<const void *> dp(n, nullptr), dc(n, nullptr);
+		bool any_crc = false;
+		for (int i = 0; i < n; ++i) {
+			if (!parts[i]) continue;
+			uint8_t *slot = static_cast<uint8_t *>(d_all[s]) + dev_part * i;
+			CUDA_TRY(cudaMemcpy2DAsync(slot, part_bytes, parts[i] + c0 * part_stride, part_stride, part_bytes, nc, cudaMemcpyHostToDevice, st));
+			ctx->stats.bytes_h2d += static_cast<uint64_t>(nc) * part_bytes;
+			dp[i] = slot;
+			if (part_crc && part_crc[i]) {
+				uint8_t *cs = static_cast<uint8_t *>(d_crc_all[s]) + dev_crc * i;
+				CUDA_TRY(cudaMemcpyAsync(cs, part_crc[i] + c0 * pb, nc * pb * 4, cudaMemcpyHostToDevice, st));
+				dc[i] = cs;
+				any_crc = true;
+			}
+		}
+		int rc;
+		{
+			BatchTimer timer(ctx, st, check_alg_bytes(goal, static_cast<uint32_t>(nc), nb, dp.data(), any_crc ? dc.data() : nullptr));
+			rc = check_enqueue(ctx, goal, static_cast<uint32_t>(nc), nb, dp.data(), part_bytes, any_crc ? dc.data() : nullptr, d_ver[s], st, tk);
+		}
+		if (rc) return rc;
+		CUDA_TRY(cudaMemcpyAsync(verdict + c0, d_ver[s], nc * sizeof(lzgpu_stripe_verdict), cudaMemcpyDeviceToHost, st));
+		ctx->stats.bytes_d2h += nc * sizeof(lzgpu_stripe_verdict);
+		return LZGPU_OK;
+	}, true);
+	if (rc) return rc;
+	for (uint32_t c = 0; c < n_chunks; ++c)
+		if (verdict[c].first_bad_stripe >= 0) {
+			lz_set_error("check_stripes: chunk %u stripe %d is not a codeword", c, verdict[c].first_bad_stripe);
+			return LZGPU_ERR_INCONSISTENT;
+		}
+	return LZGPU_OK;
 }
 
 // ------------------------------------------------------------------------------------------------

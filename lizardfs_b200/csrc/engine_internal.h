@@ -192,6 +192,10 @@ int lz_fused_recover(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, 
 int lz_fused_convert(lzgpu_ctx *ctx, const lzgpu_goal *src, const lzgpu_goal *dst, uint32_t n_chunks, uint32_t nb, const void *const *d_parts,
                      size_t part_stride, const void *const *d_part_crc, void *const *d_out, size_t out_stride, void *d_crc, size_t crc_stride,
                      cudaStream_t st, unsigned long long *d_first_bad);
+// Fused stripe check (check_kernel.cuh) of a Vandermonde / xorN goal: data parts d_parts[0..k-1] (all given), the non-NULL parity
+// parts are the checked rows.  Lowers d_verdict's first_bad_stripe words (3 ints per chunk); stored-CRC mismatches as in lz_fused_recover.
+int lz_fused_check(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, uint32_t nb, const void *const *d_parts, size_t part_stride,
+                   const void *const *d_part_crc, void *d_verdict, cudaStream_t st, unsigned long long *d_first_bad);
 // CRC of 64 KiB blocks: block (c, b) at base + c*chunk_stride + b*65536, out[c*out_chunk_stride + b]
 int lz_fused_crc(lzgpu_ctx *ctx, const void *base, unsigned long long n_blocks, unsigned long long blocks_per_chunk,
                  unsigned long long chunk_stride, void *out, unsigned long long out_chunk_stride, cudaStream_t st);

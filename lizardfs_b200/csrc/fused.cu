@@ -15,6 +15,7 @@
 #include "fused_kernel.cuh"
 #include "convert_kernel.cuh"
 #include "bs_recover_kernel.cuh"
+#include "check_kernel.cuh"
 #include "host_math.h"
 
 using namespace lzd;
@@ -171,6 +172,13 @@ static int set_all_recover_attrs() {
 	CUDA_TRY(cudaFuncSetAttribute(bs_recover3_kernel<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, kRecoverSmemCapBig));
 	// DIRECT (any generator; Cauchy codes): 16-warp geometry, 4-byte items
 	if ((rc = set_direct_attr<1>()) || (rc = set_direct_attr<2>()) || (rc = set_direct_attr<3>()) || (rc = set_direct_attr<4>())) return rc;
+	CUDA_TRY(cudaFuncSetAttribute(fused_check_kernel<1, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kRecoverSmemCapBig));
+	CUDA_TRY(cudaFuncSetAttribute(fused_check_kernel<2, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kRecoverSmemCapBig));
+	CUDA_TRY(cudaFuncSetAttribute(fused_check_kernel<3, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kRecoverSmemCapBig));
+	CUDA_TRY(cudaFuncSetAttribute(fused_check_kernel<4, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kRecoverSmemCapBig));
+	CUDA_TRY(cudaFuncSetAttribute(fused_check_kernel<1, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kRecoverSmemCapBig));
+	CUDA_TRY(cudaFuncSetAttribute(fused_check_kernel<2, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kRecoverSmemCapBig));
+	CUDA_TRY(cudaFuncSetAttribute(fused_check_kernel<3, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kRecoverSmemCapBig));
 	return LZGPU_OK;
 }
 
@@ -951,6 +959,88 @@ int lz_fused_recover(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, 
 			if (row01) return launch_recover<4, 0, 0, 1>(ctx, maps, p, smem, st, geo);
 			return launch_recover<4, 0>(ctx, maps, p, smem, st, geo);
 	}
+}
+
+// ---------------------------------------------------------------------------------------------------
+// fused stripe check (check_kernel.cuh)
+// ---------------------------------------------------------------------------------------------------
+int lz_fused_check(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, uint32_t nb, const void *const *d_parts, size_t part_stride,
+                   const void *const *d_part_crc, void *d_verdict, cudaStream_t st, unsigned long long *d_first_bad) {
+	FusedState *fs = ctx->fused;
+	if (!fs || fs->disabled) return LZGPU_NOT_HANDLED;
+	const int K = goal->k, M = goal->m;
+	if (lz::uses_cauchy(K, M) || (part_stride % 16)) return LZGPU_NOT_HANDLED;
+	CheckParams p{};
+	const void *slot_ptr[kCheckMaxSlots];
+	uint32_t R = 0;
+	bool consecutive = true, verifying = false;
+	for (int a = 0; a < K; ++a) {
+		slot_ptr[a] = d_parts[a];
+		p.part_id[a] = static_cast<uint8_t>(a);
+	}
+	for (int r = 0; r < M; ++r) {
+		if (!d_parts[K + r]) continue;
+		consecutive &= static_cast<int>(R) == r;
+		slot_ptr[K + R] = d_parts[K + r];
+		p.part_id[K + R] = static_cast<uint8_t>(K + r);
+		p.row[R++] = static_cast<uint8_t>(r);
+	}
+	const uint32_t NSLOT = K + R;
+	for (uint32_t a = 0; a < NSLOT; ++a) {
+		p.stored[a] = d_part_crc ? static_cast<const uint32_t *>(d_part_crc[p.part_id[a]]) : nullptr;
+		verifying |= p.stored[a] != nullptr;
+	}
+	if (verifying && !d_first_bad) return LZGPU_NOT_HANDLED;
+	// one 16-warp CTA per SM: the largest even G whose NSLOT*G*4 rows give every row a thread (one TMA box per part: G*4 <= 256 rows),
+	// with at least three stages in the shared-memory budget
+	uint32_t G = 0;
+	for (uint32_t g = 2; g <= 64; g += 2) {
+		const uint32_t rows = NSLOT * g * 4;
+		if (rows > static_cast<uint32_t>(kCheckThreads) || 3 * static_cast<size_t>(rows) * kStepBytes + 256 > static_cast<size_t>(kRecoverSmemCapBig)) break;
+		G = g;
+	}
+	if (G == 0) return LZGPU_NOT_HANDLED;
+	const uint32_t pb = (nb + K - 1) / K;
+	const uint32_t n_stages = static_cast<uint32_t>(std::min<size_t>(6, (kRecoverSmemCapBig - 256) / (static_cast<size_t>(NSLOT) * G * 4 * kStepBytes)));
+	p.tables = ctx->d_crc_tables;
+	p.first_bad = d_first_bad;
+	p.verdict = static_cast<int *>(d_verdict);
+	p.n_chunks = n_chunks;
+	p.pb = pb;
+	p.K = K;
+	p.G = G;
+	p.units_per_chunk = (pb + G - 1) / G;
+	const uint64_t total = static_cast<uint64_t>(p.units_per_chunk) * n_chunks;
+	if (total > 0x7fffffffull) return LZGPU_NOT_HANDLED;
+	p.total_units = static_cast<uint32_t>(total);
+	p.n_stages = n_stages;
+	std::memcpy(p.qmult, fs->qmult64, sizeof(p.qmult));
+	p.zconst = lz::crc_of_zeros(LZGPU_BLOCK_SIZE);
+	CheckTmaps maps;
+	for (uint32_t a = 0; a < NSLOT; ++a) {
+		const cuuint64_t dims[3] = {static_cast<cuuint64_t>(kRowBytes), static_cast<cuuint64_t>(pb) * 4, n_chunks};
+		const cuuint64_t strides[2] = {static_cast<cuuint64_t>(kRowBytes), part_stride};
+		const cuuint32_t box[3] = {kStepBytes, G * 4, 1};
+		const cuuint32_t estr[3] = {1, 1, 1};
+		CUresult r = fs->encode_tiled(&maps.m[a], CU_TENSOR_MAP_DATA_TYPE_UINT8, 3, const_cast<void *>(slot_ptr[a]), dims, strides, box, estr,
+		                              CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, static_cast<CUtensorMapL2promotion>(fs->promo),
+		                              CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+		if (r != CUDA_SUCCESS) return LZGPU_NOT_HANDLED;
+	}
+	const size_t smem = static_cast<size_t>(n_stages) * NSLOT * G * 4 * kStepBytes + 16 * n_stages + 64;
+	const int grid = persistent_grid(ctx, p.total_units, 1, launch_geo(LZGPU_KERNEL_CHECK, kCheckThreads, G, n_stages, 0, smem));
+	switch (consecutive ? R : R + 4) {
+		case 1: fused_check_kernel<1, true><<<grid, kCheckThreads, smem, st>>>(maps, p); break;
+		case 2: fused_check_kernel<2, true><<<grid, kCheckThreads, smem, st>>>(maps, p); break;
+		case 3: fused_check_kernel<3, true><<<grid, kCheckThreads, smem, st>>>(maps, p); break;
+		case 4: fused_check_kernel<4, true><<<grid, kCheckThreads, smem, st>>>(maps, p); break;
+		case 5: fused_check_kernel<1, false><<<grid, kCheckThreads, smem, st>>>(maps, p); break;
+		case 6: fused_check_kernel<2, false><<<grid, kCheckThreads, smem, st>>>(maps, p); break;
+		default: fused_check_kernel<3, false><<<grid, kCheckThreads, smem, st>>>(maps, p); break;
+	}
+	CUDA_TRY(cudaGetLastError());
+	ctx->stats.kernel_launches++;
+	return LZGPU_OK;
 }
 
 // ---------------------------------------------------------------------------------------------------

@@ -30,8 +30,10 @@ struct DotArgs {
 	unsigned int pure_xor;  // every coefficient is 1 (xorN goals / parity row 0): skip the multiply
 };
 
-template <int ND>
-__global__ void __launch_bounds__(256) gf_dot_kernel(const DotArgs a) {
+// CHECK = false: dst_r = the dot product.  CHECK = true (lzgpu_check_stripes): dst_r holds the stored parity and is only read; a
+// 16-byte unit that differs from the dot product lowers the first_bad_stripe word of its chunk's verdict (3 ints per chunk).
+template <int ND, bool CHECK>
+__device__ __forceinline__ void gf_dot_body(const DotArgs &a, int *verdict) {
 	extern __shared__ CoefPlanes s_coef[];  // [ND][n_src]
 	for (unsigned i = threadIdx.x; i < ND * a.n_src; i += blockDim.x) coef_planes_set(s_coef[i], a.coef[i]);
 	__syncthreads();
@@ -70,9 +72,109 @@ __global__ void __launch_bounds__(256) gf_dot_kernel(const DotArgs a) {
 			}
 		}
 		const unsigned long long dst_off = c * a.dst_chunk_stride + s * a.dst_block_stride + 16ull * o;
+		if constexpr (CHECK) {
+			uint32_t diff = 0;
 #pragma unroll
-		for (int d = 0; d < ND; ++d)
-			st_stream(reinterpret_cast<uint4 *>(a.dst[d] + dst_off), make_uint4(acc[d][0], acc[d][1], acc[d][2], acc[d][3]));
+			for (int d = 0; d < ND; ++d) {
+				const uint4 v = ld_stream(reinterpret_cast<const uint4 *>(a.dst[d] + dst_off));
+				diff |= (v.x ^ acc[d][0]) | (v.y ^ acc[d][1]) | (v.z ^ acc[d][2]) | (v.w ^ acc[d][3]);
+			}
+			int *w = verdict + 3ull * c;
+			if (diff && static_cast<int>(s) < *reinterpret_cast<volatile int *>(w)) atomicMin(w, static_cast<int>(s));
+		} else {
+#pragma unroll
+			for (int d = 0; d < ND; ++d)
+				st_stream(reinterpret_cast<uint4 *>(a.dst[d] + dst_off), make_uint4(acc[d][0], acc[d][1], acc[d][2], acc[d][3]));
+		}
+	}
+}
+
+template <int ND>
+__global__ void __launch_bounds__(256) gf_dot_kernel(const DotArgs a) { gf_dot_body<ND, false>(a, nullptr); }
+
+template <int ND>
+__global__ void __launch_bounds__(256) gf_check_kernel(const DotArgs a, int *verdict) { gf_dot_body<ND, true>(a, verdict); }
+
+// The verdict of each chunk of lzgpu_check_stripes once a check kernel has lowered its first_bad_stripe word (initialised to a value
+// above any stripe).  One CTA per chunk; a clean chunk is written {-1, 0, -1} at once.  Otherwise the CTA recomputes the syndromes of
+// that stripe byte by byte from its k data blocks and checked parity blocks, S_i = p_row[i] ^ sum_j coef[i][j] d_j, ORs the rows with
+// a non-zero syndrome into bad_rows, and keeps as suspects the parts whose column of H = [parity rows of the generator | I],
+// restricted to the checked rows, is a multiple of the syndrome vector at every non-zero byte; one suspect left (and two or more
+// rows checked) names it.
+struct LocateArgs {
+	const uint8_t *part[64];            // data parts 0..k-1, then parity part r at k + r; nullptr = not given (a parity row not checked)
+	int *verdict;                       // lzgpu_stripe_verdict[n_chunks] as 3 ints
+	unsigned long long part_stride;
+	uint32_t k, pb, n_rows;
+	uint8_t row[32];                    // parity row of checked row i
+	uint8_t coef[32 * 32];              // [i][j]: coefficient of data part j in checked row i
+};
+
+__device__ __forceinline__ uint32_t gf_mul_tab(uint32_t a, uint32_t b, const uint8_t *lg, const uint8_t *ex) {
+	return (a && b) ? ex[lg[a] + lg[b]] : 0u;
+}
+
+__global__ void __launch_bounds__(256) locate_kernel(const LocateArgs a) {
+	__shared__ uint8_t s_log[256], s_exp[512];
+	__shared__ uint8_t s_syn[32][256];  // syndromes of this thread's current byte, one column per thread
+	__shared__ unsigned long long s_cand;
+	__shared__ unsigned s_rows;
+	const unsigned tid = threadIdx.x;
+	int *v = a.verdict + 3ull * blockIdx.x;
+	const int s = v[0];
+	if (s < 0 || static_cast<uint32_t>(s) >= a.pb) {
+		if (tid == 0) { v[0] = -1; v[1] = 0; v[2] = -1; }
+		return;
+	}
+	if (tid == 0) {
+		uint32_t x = 1;
+		for (int i = 0; i < 255; ++i) {
+			s_exp[i] = s_exp[i + 255] = static_cast<uint8_t>(x);
+			s_log[x] = static_cast<uint8_t>(i);
+			x = (x << 1) ^ ((x & 0x80u) ? 0x11du : 0u);
+		}
+		s_log[0] = 0;
+		unsigned long long cand = (1ull << a.k) - 1ull;
+		for (uint32_t i = 0; i < a.n_rows; ++i) cand |= 1ull << (a.k + a.row[i]);
+		s_cand = cand;
+		s_rows = 0;
+	}
+	__syncthreads();
+	unsigned long long cand = s_cand;
+	unsigned rows = 0;
+	const unsigned long long off = blockIdx.x * a.part_stride + static_cast<unsigned long long>(s) * 65536ull;
+	for (unsigned b = tid; b < 65536u; b += blockDim.x) {
+		int first = -1;
+		for (uint32_t i = 0; i < a.n_rows; ++i) {
+			uint32_t syn = a.part[a.k + a.row[i]][off + b];
+			for (uint32_t j = 0; j < a.k; ++j) syn ^= gf_mul_tab(a.coef[i * 32 + j], a.part[j][off + b], s_log, s_exp);
+			s_syn[i][tid] = static_cast<uint8_t>(syn);
+			if (syn) {
+				rows |= 1u << a.row[i];
+				if (first < 0) first = static_cast<int>(i);
+			}
+		}
+		if (first < 0) continue;
+		for (unsigned long long left = cand; left; left &= left - 1) {
+			const uint32_t part = static_cast<uint32_t>(__ffsll(static_cast<long long>(left)) - 1);
+			bool fits = true;
+			if (part < a.k) {
+				// S = e * column: e from the first non-zero row, then every row must agree
+				const uint32_t e = s_exp[s_log[s_syn[first][tid]] + 255 - s_log[a.coef[first * 32 + part]]];
+				for (uint32_t i = 0; i < a.n_rows && fits; ++i) fits = s_syn[i][tid] == gf_mul_tab(e, a.coef[i * 32 + part], s_log, s_exp);
+			} else {
+				for (uint32_t i = 0; i < a.n_rows && fits; ++i) fits = a.k + a.row[i] == part || s_syn[i][tid] == 0;
+			}
+			if (!fits) cand &= ~(1ull << part);
+		}
+	}
+	atomicAnd(&s_cand, cand);
+	atomicOr(&s_rows, rows);
+	__syncthreads();
+	if (tid == 0) {
+		const unsigned long long c = s_cand;
+		v[1] = static_cast<int>(s_rows);
+		v[2] = (a.n_rows >= 2 && c && !(c & (c - 1))) ? __ffsll(static_cast<long long>(c)) - 1 : -1;
 	}
 }
 

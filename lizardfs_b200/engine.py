@@ -507,6 +507,46 @@ class Engine:
             raise ChunkCrcError(rc, "recover_chunks_dev", (bad[0], bad[1], bad[2]))
         _check(rc, "recover_chunks_dev")
 
+    # ---- stripe check ------------------------------------------------------------------------
+    VERDICT_DTYPE = np.dtype([("first_bad_stripe", np.int32), ("bad_rows", np.uint32), ("suspect_part", np.int32)])
+
+    def check_stripes(self, goal, nb, parts, part_crc=None):
+        """Do the parts of every stripe still form a codeword (lzgpu_check_stripes)?  parts: list of k+m arrays [n_chunks, pb*64K];
+        every data part is required, None for a parity part = that row is not checked.  part_crc: as in recover_chunks.
+        Returns the verdicts, a structured array [n_chunks] of VERDICT_DTYPE (first_bad_stripe, bad_rows, suspect_part; -1 = none),
+        whether or not any chunk is inconsistent; raises ChunkCrcError on a stored-CRC mismatch (its .verdict holds the verdicts,
+        which are written for every chunk all the same)."""
+        assert len(parts) == goal.k + goal.m
+        pb = (nb + goal.k - 1) // goal.k
+        parts = [None if p is None else _u8(p).reshape(-1, pb * BLOCK_SIZE) for p in parts]
+        n = next(p.shape[0] for p in parts if p is not None)
+        crcs = None
+        if part_crc is not None:
+            crcs = [None if c is None else np.ascontiguousarray(c, dtype=np.uint32) for c in part_crc]
+        verdict = np.empty(n, dtype=self.VERDICT_DTYPE)
+        bad = (C.c_int64 * 3)(-1, -1, -1)
+        rc = self.lib.lzgpu_check_stripes(self.h, C.byref(goal.c), n, nb, _ptr_array(parts), pb * BLOCK_SIZE,
+                                          _ptr_array(crcs) if crcs is not None else None, _p(verdict), bad)
+        if rc == _lib.ERR_CRC:
+            err = ChunkCrcError(rc, "check_stripes", (bad[0], bad[1], bad[2]))
+            err.verdict = verdict
+            raise err
+        if rc != _lib.ERR_INCONSISTENT:
+            _check(rc, "check_stripes")
+        return verdict
+
+    def check_stripes_dev(self, goal, n_chunks, nb, d_parts, part_stride, d_part_crc, d_verdict, stream=None):
+        """Device-pointer stripe check: the verdicts go to d_verdict (n_chunks x 12 bytes, device memory).  With d_part_crc the
+        call waits for its stream and raises ChunkCrcError on a mismatch; without it the call only enqueues."""
+        n_parts = goal.k + goal.m
+        dp = (C.c_void_p * n_parts)(*[p if p else None for p in d_parts])
+        dc = (C.c_void_p * n_parts)(*[p if p else None for p in d_part_crc]) if d_part_crc is not None else None
+        bad = (C.c_int64 * 3)(-1, -1, -1)
+        rc = self.lib.lzgpu_check_stripes_dev(self.h, C.byref(goal.c), n_chunks, nb, dp, part_stride, dc, d_verdict, bad, stream)
+        if rc == _lib.ERR_CRC:
+            raise ChunkCrcError(rc, "check_stripes_dev", (bad[0], bad[1], bad[2]))
+        _check(rc, "check_stripes_dev")
+
     # ---- wire format --------------------------------------------------------------------------
     def write_data_prefixes(self, goal, nb, crc, chunk_ids, write_id_base=0):
         """LIZ_CLTOCS_WRITE_DATA prefixes (cltocs.h:116-137) for every block of every part: uint8 [n, k+m, pb, 38]

@@ -1,0 +1,150 @@
+"""Throughput of the stripe check (lzgpu_check_stripes_dev) on resident 64 MiB chunks with stored CRCs.
+
+For each goal: full chunks are generated on the device (lzgpu_fill_chunks_dev), split into parts and encoded in a chunk-major layout
+(part i of chunk c at base + (c*(k+m) + i)*pb*64K), and every part block's CRC is stored per part.  The check is then timed with CUDA
+events around `--iters` back-to-back calls after `--warmup` calls (deferred verification, so no call waits for the host).  Reported:
+GiB/s of chunk data, and algorithmic bytes (every part read, its stored CRCs read, 12 bytes of verdict written) over time against the
+H100 SXM data-sheet HBM3 bandwidth of 3.35 TB/s.  The ec(8,2) degraded read of the same batch (data parts 1 and 4 rebuilt, the eight
+parts read verified) is timed in the same run as the streaming reference point.  On each goal's timed buffers one byte is then flipped
+(its block CRC restored) and the fused and the generic route must return identical verdicts naming it.
+
+    python tools/bench_check.py [--chunks 16] [--iters 20] [--warmup 3]      (one JSON line per measurement)
+"""
+import argparse
+import json
+import os
+import subprocess
+import sys
+
+import torch
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+import lizardfs_b200 as L  # noqa: E402
+from lizardfs_b200 import _lib  # noqa: E402
+
+BLOCK = 65536
+NB = 1024
+HBM_TBPS = 3.35
+GOALS = ["ec(8,2)", "ec(5,3)", "ec(8,4)", "xor3", "ec(10,5)"]
+
+
+def card():
+    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"], capture_output=True, text=True)
+    return {"device": torch.cuda.get_device_name(0), "nvidia_smi": q.stdout.strip().splitlines()[0] if q.returncode == 0 else None}
+
+
+class Resident:
+    """n full chunks of a goal on the device, chunk-major parts, per-part stored CRCs"""
+
+    def __init__(self, eng, text, n, seed=1):
+        self.goal = L.SliceType(text)
+        k, m = self.goal.k, self.goal.m
+        self.k, self.m, self.n = k, m, n
+        self.pb = (NB + k - 1) // k
+        self.part_bytes = self.pb * BLOCK
+        self.stride = (k + m) * self.part_bytes
+        data = torch.empty(n * NB * BLOCK, dtype=torch.uint8, device="cuda")
+        eng.fill_chunks_dev(data.data_ptr(), n, NB * BLOCK, NB * BLOCK, seed)
+        self.buf = torch.empty(n * self.stride, dtype=torch.uint8, device="cuda")
+        base = self.buf.data_ptr()
+        self.ptrs = [base + i * self.part_bytes for i in range(k + m)]
+        eng.split_chunks_dev(self.goal, n, NB, data.data_ptr(), NB * BLOCK, self.ptrs[:k], self.stride)
+        crc = torch.empty(n * (NB + m * self.pb), dtype=torch.int32, device="cuda")
+        eng.encode_chunks_dev(self.goal, n, NB * BLOCK, data.data_ptr(), NB * BLOCK, self.ptrs[k], self.stride, crc.data_ptr(), NB + m * self.pb)
+        del data, crc
+        self.crc = torch.empty((k + m, n, self.pb), dtype=torch.int32, device="cuda")
+        for i in range(k + m):
+            for c in range(n):
+                eng.crc_blocks_dev(self.ptrs[i] + c * self.stride, self.pb, self.crc[i, c].data_ptr())
+        self.crc_ptrs = [self.crc[i].data_ptr() for i in range(k + m)]
+        torch.cuda.synchronize()
+
+    def alg_bytes(self):
+        return self.n * ((self.k + self.m) * (self.part_bytes + 4 * self.pb) + 12)
+
+
+def timed(call, iters, warmup, stream):
+    for _ in range(warmup):
+        call()
+    torch.cuda.synchronize()
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    e0.record(stream)
+    for _ in range(iters):
+        call()
+    e1.record(stream)
+    e1.synchronize()
+    return e0.elapsed_time(e1) / 1e3 / iters
+
+
+def verdicts(eng, r, out):
+    eng.check_stripes_dev(r.goal, r.n, NB, r.ptrs, r.stride, r.crc_ptrs, out.data_ptr())
+    torch.cuda.synchronize()
+    return out.cpu().numpy().view(L.Engine.VERDICT_DTYPE).copy()
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--chunks", type=int, default=16)
+    ap.add_argument("--iters", type=int, default=20)
+    ap.add_argument("--warmup", type=int, default=3)
+    args = ap.parse_args()
+    info = card()
+    eng = L.Engine(0)
+    os.environ["LZGPU_DISABLE_FUSED"] = "1"
+    generic = L.Engine(0)
+    del os.environ["LZGPU_DISABLE_FUSED"]
+    stream = torch.cuda.Stream()        # the calls and the events share one stream
+    st = stream.cuda_stream
+    eng.set_deferred_verify(True)
+    for text in GOALS:
+        r = Resident(eng, text, args.chunks)
+        out = torch.empty(12 * r.n, dtype=torch.uint8, device="cuda")
+        t = timed(lambda: eng.check_stripes_dev(r.goal, r.n, NB, r.ptrs, r.stride, r.crc_ptrs, out.data_ptr(), stream=st),
+                  args.iters, args.warmup, stream)
+        eng.sync()
+        geo = eng.last_geometry()
+        route = "fused" if geo["kernel"] == _lib.KERNEL_CHECK else "generic"
+        clean = verdicts(eng, r, out)
+        assert (clean["first_bad_stripe"] == -1).all(), "a clean batch reported a bad stripe"
+        # one injected fault: chunk n/2, data part 3, stripe 5; its block CRC restored so only the check sees it
+        c, part, s = r.n // 2, 3, 5
+        off = c * r.stride + part * r.part_bytes + s * BLOCK + 1234
+        r.buf[off] ^= 0x5A
+        eng.crc_blocks_dev(r.ptrs[part] + c * r.stride + s * BLOCK, 1, r.crc[part, c, s:].data_ptr())
+        eng.sync()
+        v_fused, v_generic = verdicts(eng, r, out), verdicts(generic, r, out)
+        assert (v_fused == v_generic).all(), "fused and generic verdicts differ"
+        bad = [(i, tuple(int(x) for x in v_fused[i])) for i in range(r.n) if v_fused[i]["first_bad_stripe"] >= 0]
+        want_rows = (1 << r.m) - 1
+        assert bad == [(c, (s, want_rows, part if r.m >= 2 else -1))], bad
+        print(json.dumps({"what": "check_stripes_dev", "goal": text, "route": route, "chunks": r.n, "chunk_mib": NB * BLOCK >> 20,
+                          "ms_per_call": round(t * 1e3, 3), "chunk_gib_s": round(r.n * NB * BLOCK / t / 2**30, 1),
+                          "alg_tb_s": round(r.alg_bytes() / t / 1e12, 3), "of_hbm": round(r.alg_bytes() / t / 1e12 / HBM_TBPS, 3),
+                          "geometry": geo, "fault_verdict": bad[0][1], "routes_agree": True, **info}), flush=True)
+        if text == "ec(8,2)":
+            r.buf[off] ^= 0x5A   # restore the byte: the degraded read runs on valid parts
+            eng.crc_blocks_dev(r.ptrs[part] + c * r.stride + s * BLOCK, 1, r.crc[part, c, s:].data_ptr())
+            lost = (1, 4)
+            outs = {j: torch.empty(r.n * r.stride, dtype=torch.uint8, device="cuda") for j in lost}
+            parts = [0 if i in lost else p for i, p in enumerate(r.ptrs)]
+            crcs = [0 if i in lost else p for i, p in enumerate(r.crc_ptrs)]
+            want = [1 if i in lost else 0 for i in range(r.k + r.m)]
+            d_out = [outs[i].data_ptr() if i in lost else 0 for i in range(r.k + r.m)]
+            t_rec = timed(lambda: eng.recover_chunks_dev(r.goal, r.n, NB, parts, r.stride, crcs, want, d_out, stream=st), args.iters, args.warmup, stream)
+            eng.sync()
+            rec_bytes = r.n * (r.k * (r.part_bytes + 4 * r.pb) + 2 * r.part_bytes)
+            print(json.dumps({"what": "recover_chunks_dev (reference point)", "goal": text, "lost": list(lost), "chunks": r.n,
+                              "ms_per_call": round(t_rec * 1e3, 3), "chunk_gib_s": round(r.n * NB * BLOCK / t_rec / 2**30, 1),
+                              "alg_tb_s": round(rec_bytes / t_rec / 1e12, 3), "of_hbm": round(rec_bytes / t_rec / 1e12 / HBM_TBPS, 3),
+                              "geometry": eng.last_geometry(), **info}), flush=True)
+            del outs
+        del r, out
+        torch.cuda.empty_cache()
+    eng.set_deferred_verify(False)
+    generic.close()
+    eng.close()
+
+
+if __name__ == "__main__":
+    main()
