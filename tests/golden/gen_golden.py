@@ -101,6 +101,7 @@ def record_reference_digests():
     subprocess.run([sys.executable, "-m", "pytest", "-q", "-p", "no:cacheprovider", "tests/test_oracle.py", "tests/test_oracle_plans.py"],
                    cwd=ROOT, env=env, check=True)
     os.environ["LZ_RECORD_REF_DIGESTS"] = "1"
+    from tests import test_gpu_convert_geometry as CG
     from tests import test_gpu_replication as R
     oracle = O.load_oracle()
 
@@ -112,6 +113,7 @@ def record_reference_digests():
             assert rc == 0
             return [o[None, :] for o in out], [c[None, :] for c in ocrc]
     R.test_convert_chunks_vs_reference_planner(OracleEngine(), oracle)
+    CG.test_convert_geometry_vs_reference_planner(OracleEngine(), oracle)
     print("recorded", len(O._recorded), "answers of the reference (plus those of the pytest run) in", O.REF_DIGESTS)
 
 

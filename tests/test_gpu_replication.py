@@ -114,8 +114,9 @@ def test_convert_full_size_round_trip(eng, oracle):
 
 
 FUSED_CONVERSIONS = [
-    # source, lost parts, blocks, destination: every pair the one-pass kernel takes (Vandermonde source, <= 2 data parts lost with parity
-    # rows 0, 1 in use, destination with <= 3 parity parts), ragged block counts on both stripings, and two that must fall back
+    # source, lost parts, blocks, destination: a sample of the pairs the one-pass kernel takes (Vandermonde source, <= 2 data parts lost
+    # with parity rows 0, 1 in use, destination with <= 3 parity parts; every unit geometry of its planner is in
+    # test_gpu_convert_geometry.py), ragged block counts on both stripings, and two that must fall back
     ("ec(8,2)", (1, 4), 48, "ec(3,2)", True), ("ec(8,2)", (1, 4), 61, "ec(3,2)", True), ("ec(8,2)", (0,), 35, "ec(3,2)", True),
     ("ec(8,2)", (), 50, "ec(3,2)", True), ("ec(8,2)", (7, 8), 29, "ec(5,3)", False),        # parity row 1 alone in use: two passes
     ("ec(3,2)", (0, 2), 31, "ec(8,2)", True), ("ec(3,2)", (1,), 10, "xor3", True), ("xor3", (2,), 25, "ec(3,2)", True),
