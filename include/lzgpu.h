@@ -110,6 +110,59 @@ typedef struct lzgpu_convert_plan {
 } lzgpu_convert_plan;
 int lzgpu_plan_convert(const lzgpu_goal *src, const lzgpu_goal *dst, const uint8_t *available, const uint8_t *want, lzgpu_convert_plan *out);
 
+/* How lzgpu_recover_chunks* will serve a degraded read (pure host logic, no GPU needed): which fused kernel instantiation and
+ * geometry it launches, or why it takes the generic route (gf_dot_kernel + separate CRC and image passes).  available[i]: part i
+ * can be read; want[i]: part i is requested (a wanted parity part that is not available is assumed to come with an output buffer);
+ * verify: stored CRCs are given for the parts read; image: a chunk-order image is written.  switches: the values a context reads from
+ * LZGPU_RECOVER_GEO, LZGPU_RECOVER_TWO, LZGPU_RECOVER_K3, LZGPU_BS_RECOVER, LZGPU_BS_RECOVER_GFW and LZGPU_DIRECT_WIDE (-1 = automatic
+ * where the variable has that value); NULL = the build's defaults.  Returns LZGPU_ERR_TOO_FEW_PARTS when fewer than k parts are
+ * available.  A context with LZGPU_DISABLE_FUSED=1 always takes the generic route, and a call whose strides or block count the
+ * fused kernels cannot address does too; neither is part of the plan. */
+typedef struct lzgpu_recover_switches {
+	int recover_geo;          /* -1, or 0 / 1 / 2: the packed-word geometry (one 9-warp CTA, two 9-warp CTAs, one 16-warp CTA per SM) */
+	int recover_two;          /* -1, or 0 / 1: one or two 9-warp CTAs per SM for e <= 2 */
+	int recover_k3;           /* 1; 0: no compile-time k instantiations (k = 3..6) on the 16-warp geometry */
+	int bs_recover;           /* 1; 0: three lost data parts with parity rows 0, 1, 2 stay on fused_recover_kernel */
+	int bs_recover_gf_warps;  /* 8: most GF warps of bs_recover3_kernel (1..16) */
+	int direct_wide;          /* -1; 0: 4-byte items on the DIRECT form, 1: 8- / 16-byte items, -2: Cauchy goals take the generic route */
+} lzgpu_recover_switches;
+enum {   /* lzgpu_recover_plan.refusal */
+	LZGPU_RECOVER_FUSED = 0,                  /* not refused: one fused kernel */
+	LZGPU_RECOVER_REFUSED_DIRECT_OFF = 1,     /* Cauchy goal under LZGPU_DIRECT_WIDE=-2 */
+	LZGPU_RECOVER_REFUSED_TOO_FEW_PARTS = 2,  /* fewer than k parts available */
+	LZGPU_RECOVER_REFUSED_OVER_FOUR_LOST = 3, /* more than four data parts among the k inputs are lost */
+	LZGPU_RECOVER_REFUSED_NO_LOST_DATA = 4,   /* every data part is available: only parity parts could be wanted */
+	LZGPU_RECOVER_REFUSED_DIRECT_SLOWER = 5,  /* Cauchy goal, e >= 2, not both stored CRCs and an image (the generic route is faster) */
+	LZGPU_RECOVER_REFUSED_PARITY_WANTED = 6,  /* a wanted parity part is not available */
+	LZGPU_RECOVER_REFUSED_NO_GEOMETRY = 7     /* no stripe group fits */
+};
+enum {   /* lzgpu_recover_plan.rows: which parity rows the instantiation knows at compile time */
+	LZGPU_RECOVER_ROWS_GENERAL = 0,  /* read per call */
+	LZGPU_RECOVER_ROWS_FIRST_E = 1,  /* rows 0 .. e-1 (row 0 for e = 1) */
+	LZGPU_RECOVER_ROWS_DIRECT = 2    /* DIRECT form: general rows over the k inputs, no syndromes */
+};
+enum {   /* lzgpu_recover_plan.solve */
+	LZGPU_RECOVER_SOLVE_DIRECT = 0,        /* the rows of the inverted k x k system (Cauchy generators) */
+	LZGPU_RECOVER_SOLVE_RAID6 = 1,         /* two unknowns, rows 0 and 1: 2^x0 S0 by doublings or one multiply, then one multiply */
+	LZGPU_RECOVER_SOLVE_ELIM3 = 2,         /* three unknowns, rows 0, 1, 2: A S0, A^2 S0 by doublings or two multiplies, then four */
+	LZGPU_RECOVER_SOLVE_INVERSE = 3,       /* d = V^-1 S */
+	LZGPU_RECOVER_SOLVE_INVERSE_ROW0 = 4   /* the same with row 0 known at compile time: the last unknown is S0 ^ the others */
+};
+typedef struct lzgpu_recover_plan {
+	int fused;                  /* 1: one fused kernel; 0: the generic route, for the reason in refusal */
+	int refusal;                /* LZGPU_RECOVER_FUSED / LZGPU_RECOVER_REFUSED_* */
+	int kernel;                 /* LZGPU_KERNEL_RECOVER_* (fused only, as every field below) */
+	uint32_t lost_data_parts;   /* e: data parts among the first k available parts' positions that are not available */
+	uint32_t kt;                /* compile-time k of the instantiation; 0 = k read at run time */
+	int rows;                   /* LZGPU_RECOVER_ROWS_* */
+	uint32_t item_bytes;        /* bytes per GF item */
+	int solve;                  /* LZGPU_RECOVER_SOLVE_* */
+	int doublings;              /* RAID6 / ELIM3: x0 doublings for the products with S0; -1: the multiplies (and for the other forms) */
+	uint32_t G, stages, threads, gf_warps, smem_bytes;   /* as lzgpu_debug_last_geometry reports the launch */
+} lzgpu_recover_plan;
+int lzgpu_plan_recover(const lzgpu_goal *goal, const uint8_t *available, const uint8_t *want, int verify, int image,
+                       const lzgpu_recover_switches *switches, lzgpu_recover_plan *out);
+
 /* Diagnostics (pure host logic, no GPU needed): the host build of the bit-plane arithmetic the four-parity-row encoder runs per
  * item (csrc/bitslice.cuh).  data = k columns of 32 bytes (column j = 32 bytes of data part j, k <= 32); parity receives the
  * 4 x 32 bytes of the Vandermonde parity rows 0..3 (coefficient of column j in row r: (2^r)^j, galois_field_isal.cc:53-69). */

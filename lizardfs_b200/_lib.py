@@ -39,6 +39,27 @@ class LzConvertPlan(C.Structure):
                 ("stages", C.c_uint32), ("worker_warps", C.c_uint32), ("rebuild_warps", C.c_uint32), ("smem_bytes", C.c_uint32)]
 
 
+class LzRecoverSwitches(C.Structure):
+    _fields_ = [("recover_geo", C.c_int), ("recover_two", C.c_int), ("recover_k3", C.c_int), ("bs_recover", C.c_int),
+                ("bs_recover_gf_warps", C.c_int), ("direct_wide", C.c_int)]
+
+
+RECOVER_SWITCHES_DEFAULT = dict(recover_geo=-1, recover_two=-1, recover_k3=1, bs_recover=1, bs_recover_gf_warps=8, direct_wide=-1)
+
+
+class LzRecoverPlan(C.Structure):
+    _fields_ = [("fused", C.c_int), ("refusal", C.c_int), ("kernel", C.c_int), ("lost_data_parts", C.c_uint32), ("kt", C.c_uint32),
+                ("rows", C.c_int), ("item_bytes", C.c_uint32), ("solve", C.c_int), ("doublings", C.c_int), ("G", C.c_uint32),
+                ("stages", C.c_uint32), ("threads", C.c_uint32), ("gf_warps", C.c_uint32), ("smem_bytes", C.c_uint32)]
+
+
+# lzgpu_recover_plan.refusal, .rows, .solve
+RECOVER_FUSED, RECOVER_REFUSED_DIRECT_OFF, RECOVER_REFUSED_TOO_FEW_PARTS, RECOVER_REFUSED_OVER_FOUR_LOST, RECOVER_REFUSED_NO_LOST_DATA, \
+    RECOVER_REFUSED_DIRECT_SLOWER, RECOVER_REFUSED_PARITY_WANTED, RECOVER_REFUSED_NO_GEOMETRY = range(8)
+RECOVER_ROWS_GENERAL, RECOVER_ROWS_FIRST_E, RECOVER_ROWS_DIRECT = range(3)
+RECOVER_SOLVE_DIRECT, RECOVER_SOLVE_RAID6, RECOVER_SOLVE_ELIM3, RECOVER_SOLVE_INVERSE, RECOVER_SOLVE_INVERSE_ROW0 = range(5)
+
+
 class LzLaunchGeometry(C.Structure):
     _fields_ = [("kernel", C.c_int), ("grid", C.c_uint32), ("units", C.c_uint32), ("threads", C.c_uint32), ("G", C.c_uint32),
                 ("stages", C.c_uint32), ("gf_warps", C.c_uint32), ("smem_bytes", C.c_uint32)]
@@ -68,6 +89,7 @@ SIGNATURES = {
     "lzgpu_goal_valid": (_int, [_goalp]),
     "lzgpu_plan_encode": (_int, [_goalp, _u32, _u32, _sz, _int, _vp]),
     "lzgpu_plan_convert": (_int, [_goalp, _goalp, _vp, _vp, _vp]),
+    "lzgpu_plan_recover": (_int, [_goalp, _vp, _vp, _int, _int, C.POINTER(LzRecoverSwitches), C.POINTER(LzRecoverPlan)]),
     "lzgpu_debug_bitslice_rows": (_int, [_int, _vp, _vp]),
     "lzgpu_debug_bitslice_recover3": (_int, [_int, _vp, _vp, _int, _vp]),
     "lzgpu_goal_slice_type": (_int, [_goalp]),

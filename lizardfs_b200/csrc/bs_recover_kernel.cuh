@@ -21,7 +21,7 @@ struct BsRecoverMasks {
 	uint32_t m[6][64];   // alpha, beta, gamma, delta of the three-unknown elimination (fused_recover_kernel, E = 3); A = 2^a, A^2
 };
 
-constexpr int kBsRecoverThreads = 512;
+// (kBsRecoverThreads: fused_plan.h)
 
 template <int KT>
 __global__ void __launch_bounds__(kBsRecoverThreads, 1)

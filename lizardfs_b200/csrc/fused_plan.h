@@ -1,9 +1,13 @@
 // fused_plan.h — geometry of the fused encode kernel as pure functions (no CUDA calls): which unit mode a batch gets, how many
-// stripes a unit holds, how many units there are.  Shared by the launcher (fused.cu) and the diagnostics entry point
-// lzgpu_plan_encode (engine side), so the decisions are unit-tested on a machine without a GPU (tests/test_host_math.py).
+// stripes a unit holds, how many units there are; the same for the one-pass slice conversion (convert_plan) and the router of the
+// degraded read (recover_plan).  Shared by the launchers (fused.cu) and the diagnostics entry points lzgpu_plan_encode,
+// lzgpu_plan_convert and lzgpu_plan_recover (host_math.cc), so the decisions are unit-tested on a machine without a GPU
+// (tests/test_host_math.py, tests/test_gpu_convert_geometry.py, tests/test_gpu_recover_geometry.py).
 #pragma once
 #include <cstddef>
 #include <cstdint>
+
+#include "lzgpu.h"
 
 #ifndef __CUDACC__
 #define LZ_HD
@@ -256,6 +260,209 @@ inline ConvertPlan convert_plan(int Ks, int Ms, bool src_cauchy, int Kd, int Md,
 			pl.G = g; pl.T = t; pl.region_rows = rr; pl.n_stages = ns; pl.n_workers = n_wk;
 			pl.smem = ns * stage + 24 * ns + fixed;
 		}
+	}
+	return pl;
+}
+
+// ---------------------------------------------------------------------------------------------------
+// Fused degraded read (fused_recover_kernel, fused_kernel.cuh; bs_recover3_kernel, bs_recover_kernel.cuh): the router as a pure
+// function, shared by lz_fused_recover (which dispatches on its fields alone) and lzgpu_plan_recover.
+// ---------------------------------------------------------------------------------------------------
+constexpr int kRecoverSmemCap = 200 * 1024;     // GEO 0: one 9-warp CTA per SM, 6 stages
+constexpr int kRecoverSmemCap2 = 100 * 1024;    // GEO 1: two 9-warp CTAs per SM, 3 stages (E <= 2)
+constexpr int kRecoverSmemCapBig = 208 * 1024;  // GEO 2, DIRECT, bs_recover3: one 16-warp CTA per SM
+constexpr int kBsRecoverThreads = 512;
+LZ_HD constexpr int recover_stages(int geo) { return geo == 1 ? 3 : 6; }
+LZ_HD constexpr int recover_threads(int geo) { return geo == 2 ? 512 : kFusedThreads; }
+#ifndef LZ_RW3
+#define LZ_RW3 2   // words per GF item for three or four erased parts on the 16-warp geometry (narrower items = fewer live accumulators)
+#endif
+LZ_HD constexpr int recover_item_words(int e, int geo) { return (geo == 2 && e >= 3) ? LZ_RW3 : 4; }
+// wide items of the DIRECT degraded read: 16 bytes for one rebuilt part, 8 for more (e x 4 accumulators next to the CRC window spill at 128 registers)
+LZ_HD constexpr int direct_wide_words(int e) { return e >= 2 ? 2 : 4; }
+
+// the one-CTA 16-warp routes (GEO 2, DIRECT, bs_recover3): as many stages as fit 208 KiB, at most six
+inline uint32_t recover_big_stages(uint32_t K, uint32_t G) {
+	const size_t fit = (kRecoverSmemCapBig - 256) / (static_cast<size_t>(K) * G * 4 * kStepBytes);
+	return static_cast<uint32_t>(fit < 6 ? fit : 6);
+}
+
+#ifndef LZ_BS_RECOVER_DEFAULT
+#define LZ_BS_RECOVER_DEFAULT 1
+#endif
+// the context switches the router reads (lzgpu_recover_switches; the defaults are the build's)
+inline lzgpu_recover_switches recover_switches_default() {
+	lzgpu_recover_switches s;
+	s.recover_geo = -1;
+	s.recover_two = -1;
+	s.recover_k3 = 1;
+	s.bs_recover = LZ_BS_RECOVER_DEFAULT;
+	s.bs_recover_gf_warps = 8;
+	s.direct_wide = -1;
+	return s;
+}
+
+struct RecoverPlan {
+	lzgpu_recover_plan out{};         // what lzgpu_plan_recover reports (refusal, kernel, instantiation, geometry)
+	int used[LZGPU_MAX_DATA] = {0};   // slot a -> part index: the first k available parts (ec_read_plan.h:126-133)
+	uint8_t erased_idx[4] = {0};      // data index of lost part x, ascending
+	uint8_t par_slot[4] = {0}, par_row[4] = {0};  // parity parts in use: slot and generator row, ascending
+	int geo = 0;                      // packed-word geometry (0, 1, 2) of the fused_recover_kernel routes
+	bool wide = false;                // DIRECT: 8- / 16-byte items (else 4)
+};
+
+// available[i]: part i (data parts first) can be read.  want_missing_parity: a wanted parity part that is not available has an
+// output buffer (only lost data parts are rebuilt here).  verify: some part read has stored CRCs.  image: a chunk-order image is
+// written.
+inline RecoverPlan recover_plan(int K, int M, bool cauchy, const uint8_t *available, bool want_missing_parity, bool verify, bool image,
+                                const lzgpu_recover_switches &sw) {
+	RecoverPlan pl;
+	lzgpu_recover_plan &o = pl.out;
+	o.doublings = -1;
+	const bool direct = cauchy;   // no Horner syndromes for a Cauchy generator: general rows over the k inputs
+	if (direct && sw.direct_wide == -2) { o.refusal = LZGPU_RECOVER_REFUSED_DIRECT_OFF; return pl; }   // A/B against the generic route
+	const bool direct_forced = direct && sw.direct_wide >= 0;
+	int n_used = 0;
+	for (int i = 0; i < K + M && n_used < K; ++i)
+		if (available[i]) pl.used[n_used++] = i;
+	if (n_used < K) { o.refusal = LZGPU_RECOVER_REFUSED_TOO_FEW_PARTS; return pl; }
+	bool present[LZGPU_MAX_DATA] = {false};
+	uint32_t e = 0, n_par = 0;
+	for (int a = 0; a < K; ++a) {
+		const int idx = pl.used[a];
+		if (idx < K) present[idx] = true;
+		else if (n_par < 4) { pl.par_slot[n_par] = static_cast<uint8_t>(a); pl.par_row[n_par] = static_cast<uint8_t>(idx - K); ++n_par; }
+		else { o.refusal = LZGPU_RECOVER_REFUSED_OVER_FOUR_LOST; return pl; }
+	}
+	for (int j = 0; j < K; ++j)
+		if (!present[j]) {
+			if (e >= 4) { o.refusal = LZGPU_RECOVER_REFUSED_OVER_FOUR_LOST; return pl; }
+			pl.erased_idx[e++] = static_cast<uint8_t>(j);
+		}
+	o.lost_data_parts = e;
+	if (e == 0 || e != n_par) { o.refusal = LZGPU_RECOVER_REFUSED_NO_LOST_DATA; return pl; }
+	// Measured: with general coefficients the rebuild is bound by the bit-plane multiplies, not by HBM, and
+	// the grid-stride gf_dot_kernel (full occupancy, no stage barriers) does e >= 2 rows faster than this kernel's 16 warps per SM
+	// even though it needs separate CRC and image passes.  One lost part, and two lost parts when the call verifies and wants the
+	// image, measured faster here and stay here.
+	if (direct && !direct_forced && !(e == 1 || (e == 2 && verify && image))) { o.refusal = LZGPU_RECOVER_REFUSED_DIRECT_SLOWER; return pl; }
+	// every requested missing part must be a data part
+	if (want_missing_parity) { o.refusal = LZGPU_RECOVER_REFUSED_PARITY_WANTED; return pl; }
+	// geometry: even G (1024-byte aligned slot regions), K*G*4 rows <= 256
+	// Two CTAs per SM with a 3-stage ring, or one CTA with 6 stages?  Measured with 64 MiB chunks: two CTAs win for the runtime-k
+	// shapes, except the single-erasure case that also writes the image; the k = 8 instantiation keeps one.  LZGPU_RECOVER_TWO=0|1 forces either.
+	const bool two_auto = K != 8 && (e == 2 || (e == 1 && !image));
+	const bool two = e <= 2 && (sw.recover_two < 0 ? two_auto : sw.recover_two != 0);
+	// Measured (recover only and verify + image): the 16-warp CTA wins for the runtime-k shapes with two or more erased parts, against
+	// two 9-warp CTAs and against one, while the k = 8 instantiation keeps one 9-warp CTA with six stages.  LZGPU_RECOVER_GEO=0|1|2 forces one.
+	int geo = sw.recover_geo >= 0 ? sw.recover_geo : (K != 8 && e >= 2) ? 2 : (two ? 1 : 0);
+	if (direct) geo = 2;
+	if (geo == 1 && e > 2) geo = 0;
+	// three lost data parts with parity rows 0, 1, 2 in use: bit planes + dedicated GF warps (bs_recover_kernel.cuh) — geometry: G even,
+	// the 16 G items of a step on the last ceil(16 G / 32) warps, the k G 4 input rows on the warps before them when the call verifies
+	// stored CRCs (no stream warps otherwise), one TMA box per part (G 4 <= 256 rows), at least three stages
+	bool bs3 = !direct && e == 3 && sw.bs_recover && pl.par_row[0] == 0 && pl.par_row[1] == 1 && pl.par_row[2] == 2;
+	uint32_t G = 0, n_stages = 0;
+	const uint32_t UK = static_cast<uint32_t>(K);
+	if (bs3) {
+		// Measured with at most four against at most eight GF warps: more GF warps win for rebuild only (no stream warps, G = 16, eight
+		// GF warps) and with verification and image for ec(5,3) (seven) and ec(6,3) (six), but ec(8,3) loses with five (one scheduler
+		// gets two of them).  So: the largest G, unless it only buys a fifth GF warp.
+		uint32_t g4 = 0;
+		for (uint32_t g = 2; g <= 64; g += 2) {
+			const size_t stage = static_cast<size_t>(UK) * g * 4 * kStepBytes;
+			const uint32_t gf_warps = (16 * g + 31) / 32, stream_warps = verify ? (UK * g * 4 + 31) / 32 : 0;
+			if (gf_warps > static_cast<uint32_t>(sw.bs_recover_gf_warps) || gf_warps + stream_warps > kBsRecoverThreads / 32 || 3 * stage + 256 > static_cast<size_t>(kRecoverSmemCapBig)) break;
+			G = g;
+			if (gf_warps <= 4) g4 = g;
+		}
+		if (G && g4 && (16 * G + 31) / 32 == 5) G = g4;
+		if (G) n_stages = recover_big_stages(UK, G);
+		else bs3 = false;
+	}
+	if (bs3) {
+		// (geometry chosen above)
+	} else if (geo == 2) {
+		// one 16-warp CTA: the largest G whose K*G*4 input rows fit 512 threads (one TMA box per part: G*4 <= 256 rows) and whose
+		// 32*G items fill whole rounds of the CTA (G a multiple of 16) where K allows, with at least three stages in 208 KiB
+		uint32_t best = 0, best16 = 0;
+		for (uint32_t g = 2; g <= 64; g += 2) {
+			const uint32_t rows = UK * g * 4;
+			if (rows > 512 || 3 * static_cast<size_t>(rows) * kStepBytes + 256 > kRecoverSmemCapBig) break;
+			best = g;
+			if (g % 16 == 0) best16 = g;
+		}
+		G = best16 ? best16 : best;
+		if (G) n_stages = recover_big_stages(UK, G);
+	} else {
+		n_stages = static_cast<uint32_t>(recover_stages(geo));
+		const size_t smem_cap = geo == 1 ? kRecoverSmemCap2 : kRecoverSmemCap;
+		for (uint32_t g = 2; g <= 64; g += 2) {
+			const uint32_t rows = UK * g * 4;
+			if (rows > kMaxRows || static_cast<size_t>(n_stages) * rows * kStepBytes + 256 > smem_cap) break;
+			G = g;
+		}
+	}
+	if (G == 0) { o.refusal = LZGPU_RECOVER_REFUSED_NO_GEOMETRY; return pl; }
+	pl.geo = geo;
+	o.fused = 1;
+	o.G = G;
+	o.stages = n_stages;
+	o.smem_bytes = static_cast<uint32_t>(static_cast<size_t>(n_stages) * UK * G * 4 * kStepBytes + 16 * n_stages + 64);
+	bool consecutive = true;   // parity rows 0, 1, .., e-1 in use (the first e parity parts are the available ones — the common case)
+	for (uint32_t r = 0; r < e; ++r) consecutive &= pl.par_row[r] == r;
+	const bool row0 = pl.par_row[0] == 0, row01 = e >= 2 && consecutive;
+	const int x0 = pl.erased_idx[0];
+	if (bs3) {
+		o.kernel = LZGPU_KERNEL_RECOVER_BS3;
+		o.kt = (K == 5 || K == 8) ? static_cast<uint32_t>(K) : 0;
+		o.rows = LZGPU_RECOVER_ROWS_FIRST_E;
+		o.item_bytes = 32;
+		o.solve = LZGPU_RECOVER_SOLVE_ELIM3;
+		o.doublings = x0 <= 3 ? x0 : -1;
+		o.threads = kBsRecoverThreads;
+		o.gf_warps = (16 * G + 31) / 32;
+		return pl;
+	}
+	if (direct) {
+		// item width: 16-byte items leave most of the 16 warps without work when k is large (G small)
+		// the 8 / 16-byte items measured faster on every shape; 4-byte items stay for A/B
+		pl.wide = sw.direct_wide >= 0 ? sw.direct_wide != 0 : true;
+		o.kernel = LZGPU_KERNEL_RECOVER_DIRECT;
+		o.rows = LZGPU_RECOVER_ROWS_DIRECT;
+		o.item_bytes = 4 * (pl.wide ? direct_wide_words(static_cast<int>(e)) : 1);
+		o.solve = LZGPU_RECOVER_SOLVE_DIRECT;
+		o.threads = recover_threads(2);
+		return pl;
+	}
+	o.kernel = geo == 2 ? LZGPU_KERNEL_RECOVER_GEO2 : geo == 1 ? LZGPU_KERNEL_RECOVER_GEO1 : LZGPU_KERNEL_RECOVER_GEO0;
+	o.threads = static_cast<uint32_t>(recover_threads(geo));
+	o.item_bytes = 4 * recover_item_words(static_cast<int>(e), geo);
+	o.rows = e == 1 ? (row0 ? LZGPU_RECOVER_ROWS_FIRST_E : LZGPU_RECOVER_ROWS_GENERAL) : (row01 ? LZGPU_RECOVER_ROWS_FIRST_E : LZGPU_RECOVER_ROWS_GENERAL);
+	// compile-time k (the walk over the columns unrolls, parameter loads become immediates):
+	// ec(3,2) / ec(5,3) on the 16-warp geometry, measured faster than the runtime-k kernel for ec(3,2), most of all for rebuild only.
+	// ec(5,3): two lost, faster for rebuild only but slower with verification and image (the unrolled walk costs the CRC role
+	// registers), so that combination keeps the runtime-k kernel; three lost faster either way.  ec(4,2), ec(6,2), ec(6,3): the same
+	// rule as for k = 5.  k = 8 (G = 8 or the 16-warp geometry): one and two lost parts with rows 0 (0, 1) in use.
+	const bool k8 = K == 8 && (G == 8 || geo == 2);
+	const bool vi = verify && image;
+	if (geo == 2 && sw.recover_k3 && ((K == 3 && ((e == 1 && row0) || (e == 2 && row01))) || ((K == 4 || K == 5 || K == 6) && e == 2 && row01 && !vi) ||
+	                                  ((K == 5 || K == 6) && e == 3 && row01)))
+		o.kt = static_cast<uint32_t>(K);
+	else if (k8 && e <= 2 && o.rows == LZGPU_RECOVER_ROWS_FIRST_E)
+		o.kt = 8;
+	// the form of the solve (fused_recover_kernel): RAID-6 elimination for two unknowns with rows 0, 1 (not the k = 8 instantiation:
+	// there the two bit-plane multiplies measured faster), x0 doublings for 2^x0 S0 up to x0 = 4, else the multiply by w[0]; the
+	// three-unknown elimination with rows 0, 1, 2, x0 doublings up to x0 = 3, else the multiplies by w[4], w[5]; otherwise
+	// d = V^-1 S, where row 0 known at compile time makes the last unknown S0 ^ (the others)
+	if (e == 2 && row01 && o.kt != 8) {
+		o.solve = LZGPU_RECOVER_SOLVE_RAID6;
+		o.doublings = x0 <= 4 ? x0 : -1;
+	} else if (e == 3 && row01) {
+		o.solve = LZGPU_RECOVER_SOLVE_ELIM3;
+		o.doublings = x0 <= 3 ? x0 : -1;
+	} else {
+		o.solve = o.rows == LZGPU_RECOVER_ROWS_FIRST_E ? LZGPU_RECOVER_SOLVE_INVERSE_ROW0 : LZGPU_RECOVER_SOLVE_INVERSE;
 	}
 	return pl;
 }

@@ -487,6 +487,18 @@ int lzgpu_plan_convert(const lzgpu_goal *src, const lzgpu_goal *dst, const uint8
 	return LZGPU_OK;
 }
 
+int lzgpu_plan_recover(const lzgpu_goal *goal, const uint8_t *available, const uint8_t *want, int verify, int image,
+                       const lzgpu_recover_switches *switches, lzgpu_recover_plan *out) {
+	if (!out || !available || !want || !lzgpu_goal_valid(goal)) return LZGPU_ERR_ARG;
+	const int K = goal->k, M = goal->m;
+	bool want_missing_parity = false;
+	for (int i = K; i < K + M; ++i) want_missing_parity |= want[i] && !available[i];
+	const lzd::RecoverPlan pl = lzd::recover_plan(K, M, lz::uses_cauchy(K, M), available, want_missing_parity, verify != 0, image != 0,
+	                                              switches ? *switches : lzd::recover_switches_default());
+	*out = pl.out;
+	return pl.out.refusal == LZGPU_RECOVER_REFUSED_TOO_FEW_PARTS ? LZGPU_ERR_TOO_FEW_PARTS : LZGPU_OK;
+}
+
 const char *lzgpu_version(void) { return "lizardfs_b200 0.1 (sm_90a)"; }
 
 }  // extern "C"

@@ -605,6 +605,26 @@ class Engine:
         _check(_lib.load().lzgpu_plan_convert(C.byref(src.c), C.byref(dst.c), _p(a), _p(w), C.byref(out)), "plan_convert")
         return {f: getattr(out, f) for f, _ in _lib.LzConvertPlan._fields_}
 
+    @staticmethod
+    def plan_recover(goal, available, want, verify, image, switches=None):
+        """how recover_chunks* would serve the degraded read (pure host logic, csrc/fused_plan.h recover_plan; no GPU needed): dict
+        with fused, refusal (_lib.RECOVER_REFUSED_*), kernel (_lib.KERNEL_RECOVER_*), lost_data_parts, kt (compile-time k, 0 =
+        runtime), rows, item_bytes, solve, doublings, G, stages, threads, gf_warps, smem_bytes.  switches: a dict of
+        lzgpu_recover_switches fields that differ from the build's defaults (_lib.RECOVER_SWITCHES_DEFAULT), None = the defaults."""
+        out = _lib.LzRecoverPlan()
+        a = np.asarray(available, dtype=np.uint8)
+        w = np.asarray(want, dtype=np.uint8)
+        assert a.size == goal.k + goal.m and w.size == goal.k + goal.m
+        sw = None
+        if switches is not None:
+            unknown = set(switches) - set(_lib.RECOVER_SWITCHES_DEFAULT)
+            assert not unknown, unknown
+            sw = C.byref(_lib.LzRecoverSwitches(**{**_lib.RECOVER_SWITCHES_DEFAULT, **switches}))
+        rc = _lib.load().lzgpu_plan_recover(C.byref(goal.c), _p(a), _p(w), int(bool(verify)), int(bool(image)), sw, C.byref(out))
+        if rc != _lib.ERR_TOO_FEW_PARTS:
+            _check(rc, "plan_recover")
+        return {f: getattr(out, f) for f, _ in _lib.LzRecoverPlan._fields_}
+
     def convert_chunks(self, src, dst, nb, parts, want, part_crc=None, with_crc=True):
         """Rebuild the `want`ed parts of slice type `dst` from the available `parts` of slice type `src`
         (SliceRecoveryPlanner, slice_recovery_planner.h:87-204).  parts[i]: (n_chunks, pb_src*65536) uint8 or None.
