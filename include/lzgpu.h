@@ -350,7 +350,8 @@ int lzgpu_recover_chunks_dev(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_
  *                       restricted to the checked rows; -1 when no single part or more than one does.  With one checked row (xorN, or
  *                       one parity part given) it is always -1.  With two checked rows two corrupt parts can look like a third,
  *                       single one — a property of the code, not of this check.  With three or more checked rows two corrupt parts
- *                       never produce a suspect.  Rebuild the suspect with lzgpu_convert_chunks.
+ *                       never produce a suspect.  The verdict says nothing about the stripes after the first: before rebuilding a
+ *                       part, take lzgpu_check_stripe_map and follow its repair rule.
  * lzgpu_check_stripes returns LZGPU_ERR_CRC when a stored CRC failed, else LZGPU_ERR_INCONSISTENT when any chunk has a bad stripe,
  * else LZGPU_OK.  lzgpu_check_stripes_dev writes the verdicts to d_verdict (device memory, 4-byte aligned; nothing else is written)
  * on `stream` and, like lzgpu_recover_chunks_dev, waits for the stream only to report a stored-CRC verdict (deferred mode moves that
@@ -367,6 +368,33 @@ int lzgpu_check_stripes(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunk
 int lzgpu_check_stripes_dev(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, uint32_t nb,
                             const void *const *d_parts, size_t part_stride, const void *const *d_part_crc,
                             void *d_verdict, int64_t *bad, void *stream);
+
+/* Stripe map: the check of lzgpu_check_stripes, with a state for every stripe of every chunk instead of the first bad one.
+ *   goal, n_chunks, nb, parts, part_stride, part_crc, bad   exactly as in lzgpu_check_stripes (stored CRCs verified in the same pass,
+ *                                       bad[0..2], alignment, the CRC-disabled mode, deferred verification, LZGPU_ERR_TOO_FEW_PARTS).
+ *   map[c * pb + s]  (pb = ceil(nb / k), the indexing of part_crc; n_chunks * pb entries, every one written, also when a stored CRC
+ *                    failed; nothing outside them is written): the state of stripe s (= part block s) of chunk c.
+ * For each chunk, the lowest s with bad_rows != 0 and its entry equal the verdict lzgpu_check_stripes returns for the same input.
+ * Repair rule.  Rebuilding a whole part reads k other parts over every stripe, so a second fault in another stripe spreads into the
+ * rebuilt part (stripe 5 bad in part 2 and stripe 9 bad in part 6: rebuilding part 2 whole computes its block 9 from the corrupt block
+ * of part 6, and stripe 9 then has two bad parts).  So, per chunk:
+ *   - suspect_part == -1 in any bad stripe: the chunk goes to an operator (no single part explains that stripe);
+ *   - every bad stripe names the same part: that part may be rebuilt whole (lzgpu_convert_chunks or lzgpu_recover_chunks);
+ *   - otherwise rebuild stripe by stripe: for each bad stripe s, a one-stripe window of lzgpu_recover_chunks (every part pointer
+ *     offset by s * 65536, nb = the blocks of that stripe, min(k, nb - s k)) with the named part as the one wanted.
+ * lzgpu_check_stripe_map returns LZGPU_ERR_CRC when a stored CRC failed, else LZGPU_ERR_INCONSISTENT when any stripe is bad, else
+ * LZGPU_OK.  lzgpu_check_stripe_map_dev writes the map to d_map (device memory, 4-byte aligned) on `stream` and returns LZGPU_OK or
+ * LZGPU_ERR_CRC, as lzgpu_check_stripes_dev. */
+typedef struct lzgpu_stripe_state {
+	uint32_t bad_rows;      /* bit r: checked parity row r has a non-zero syndrome in this stripe; 0 = the stripe is a codeword */
+	int32_t suspect_part;   /* as lzgpu_stripe_verdict.suspect_part, for this stripe; -1 when bad_rows == 0 */
+} lzgpu_stripe_state;
+int lzgpu_check_stripe_map(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, uint32_t nb,
+                           const uint8_t *const *parts, size_t part_stride, const uint32_t *const *part_crc,
+                           lzgpu_stripe_state *map, int64_t *bad);
+int lzgpu_check_stripe_map_dev(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, uint32_t nb,
+                               const void *const *d_parts, size_t part_stride, const void *const *d_part_crc,
+                               void *d_map, int64_t *bad, void *stream);
 
 /* Wire-format producer (SURVEY.md §8 f3): LIZ_CLTOCS_WRITE_DATA packet prefixes (src/protocol/cltocs.h:116-137) for
  * every block of every part of the encoded chunks, built on the GPU straight from the CRC array of

@@ -74,6 +74,10 @@ class LzStripeVerdict(C.Structure):
     _fields_ = [("first_bad_stripe", C.c_int32), ("bad_rows", C.c_uint32), ("suspect_part", C.c_int32)]
 
 
+class LzStripeState(C.Structure):
+    _fields_ = [("bad_rows", C.c_uint32), ("suspect_part", C.c_int32)]
+
+
 class LzBlockWrite(C.Structure):
     _fields_ = [("block", C.c_uint32), ("offset", C.c_uint32), ("size", C.c_uint32), ("crc", C.c_uint32),
                 ("payload_off", C.c_uint64), ("exists", C.c_uint32), ("status", C.c_int32)]
@@ -115,6 +119,8 @@ SIGNATURES = {
     "lzgpu_recover_chunks_dev": (_int, [_vp, _goalp, _u32, _u32, _vp, _sz, _vp, _vp, _vp, _vp, _sz, _vp, _vp]),
     "lzgpu_check_stripes": (_int, [_vp, _goalp, _u32, _u32, _vp, _sz, _vp, _vp, _vp]),
     "lzgpu_check_stripes_dev": (_int, [_vp, _goalp, _u32, _u32, _vp, _sz, _vp, _vp, _vp, _vp]),
+    "lzgpu_check_stripe_map": (_int, [_vp, _goalp, _u32, _u32, _vp, _sz, _vp, _vp, _vp]),
+    "lzgpu_check_stripe_map_dev": (_int, [_vp, _goalp, _u32, _u32, _vp, _sz, _vp, _vp, _vp, _vp]),
     "lzgpu_write_data_prefixes": (_int, [_vp, _goalp, _u32, _u32, _vp, _sz, _vp, _u32, _vp]),
     "lzgpu_write_data_prefixes_dev": (_int, [_vp, _goalp, _u32, _u32, _vp, _sz, _vp, _u32, _vp, _vp]),
     "lzgpu_split_chunks": (_int, [_vp, _goalp, _u32, _u32, _vp, _sz, _vp, _sz]),

@@ -11,7 +11,8 @@
 //   CRC role  thread t owns row t of the stage (slot t / 4G): a 16 KiB stream folded with the sparse multiple of P, compared with
 //             the stored CRC of its block at the end of the unit; the first mismatch lowers first_bad.
 //   GF role   item (stripe g, quarter q, 16-byte column): Horner over the k data columns per checked row, XOR the stored parity
-//             column, OR-reduce.  A thread keeps the lowest non-zero stripe of its unit and lowers the chunk's verdict word once.
+//             column, OR-reduce.  A thread keeps the lowest non-zero stripe of its unit and lowers the chunk's verdict word once
+//             (fused_check_kernel), or keeps the non-zero rows of each stripe for the stripe map (fused_check_map_kernel).
 #pragma once
 #include "fused_kernel.cuh"
 
@@ -36,10 +37,15 @@ struct CheckParams {
 	uint8_t part_id[kCheckMaxSlots];         // slot -> part index (error reporting)
 };
 
-// R = checked parity rows; CONSEC: they are rows 0 .. R-1 (row r multiplies by 2^r in one step), else p.row[r] doublings
-template <int R, bool CONSEC>
-__global__ void __launch_bounds__(kCheckThreads, 1)
-fused_check_kernel(const __grid_constant__ CheckTmaps tmaps, const __grid_constant__ CheckParams p) {
+// R = checked parity rows; CONSEC: they are rows 0 .. R-1 (row r multiplies by 2^r in one step), else p.row[r] doublings.
+// MAP = false: the per-chunk verdict word (lzgpu_check_stripes).  MAP = true (lzgpu_check_stripe_map): every stripe's bad_rows goes to
+// map[2 (c pb + s)] and its suspect_part word is set to -1 (locate_map_kernel names the suspects of the bad ones).  The items of
+// stripe g are items 32g .. 32g + 31, i.e. the 32 lanes of one warp in the same pass of the item loop, and that warp owns the stripe
+// for the whole unit: each lane keeps its row bits in a nibble per pass (at most 2048 items, four passes), and at the end of the unit
+// the warp OR-reduces each nibble and lane 0 stores the stripe's entry.  Units partition the stripes, so the map needs no memset and
+// no atomics.
+template <int R, bool CONSEC, bool MAP>
+__device__ __forceinline__ void fused_check_body(const CheckTmaps &tmaps, const CheckParams &p, uint32_t *map) {
 	constexpr int W = 4;
 	constexpr uint32_t CPI = 32 / W;
 	extern __shared__ __align__(1024) uint8_t smem[];
@@ -92,6 +98,7 @@ fused_check_kernel(const __grid_constant__ CheckTmaps tmaps, const __grid_consta
 		const uint32_t next_unit = unit + gridDim.x;
 		const uint32_t next_c = next_unit / p.units_per_chunk, next_gi = next_unit % p.units_per_chunk;
 		uint32_t bad_stripe = 0xffffffffu;
+		uint32_t map_bits = 0;  // MAP: nibble i = the row bits of this thread's item in pass i of the item loop
 #pragma unroll
 		for (int i = 0; i < 64; ++i) win[i] = 0;
 
@@ -133,15 +140,28 @@ fused_check_kernel(const __grid_constant__ CheckTmaps tmaps, const __grid_consta
 								}
 							}
 						}
-						uint32_t any = 0;
+						if constexpr (MAP) {
+							uint32_t bits = 0;
 #pragma unroll
-						for (int r = 0; r < R; ++r) {
-							uint32_t pv[W];
-							lds_item<W>(a_item + (K + r) * region_bytes, pv);
+							for (int r = 0; r < R; ++r) {
+								uint32_t pv[W], d = 0;
+								lds_item<W>(a_item + (K + r) * region_bytes, pv);
 #pragma unroll
-							for (int w = 0; w < W; ++w) any |= acc[r][w] ^ pv[w];
+								for (int w = 0; w < W; ++w) d |= acc[r][w] ^ pv[w];
+								if (d) bits |= 1u << (CONSEC ? r : p.row[r]);  // parity rows are 0..3 (m <= 4 on this route)
+							}
+							map_bits |= bits << (4 * (item / kCheckThreads));
+						} else {
+							uint32_t any = 0;
+#pragma unroll
+							for (int r = 0; r < R; ++r) {
+								uint32_t pv[W];
+								lds_item<W>(a_item + (K + r) * region_bytes, pv);
+#pragma unroll
+								for (int w = 0; w < W; ++w) any |= acc[r][w] ^ pv[w];
+							}
+							if (any) bad_stripe = min(bad_stripe, stripe0 + g);  // rows past the last stripe are zero-filled: never non-zero
 						}
-						if (any) bad_stripe = min(bad_stripe, stripe0 + g);  // rows past the last stripe are zero-filled: never non-zero
 					}
 				}
 
@@ -157,7 +177,21 @@ fused_check_kernel(const __grid_constant__ CheckTmaps tmaps, const __grid_consta
 			}
 		}
 
-		if (bad_stripe != 0xffffffffu) atomicMin(p.verdict + 3ull * c, static_cast<int>(bad_stripe));
+		if constexpr (MAP) {
+			// every lane of a GF warp ran the same passes (n_items and the thread count are multiples of 32)
+			if (warp_has_items)
+				for (uint32_t item0 = cw * 32, i = 0; item0 < n_items; item0 += kCheckThreads, ++i) {
+					const uint32_t bits = __reduce_or_sync(0xffffffffu, (map_bits >> (4 * i)) & 15u);
+					const uint32_t s = stripe0 + item0 / 32;
+					if (lane == 0 && s < p.pb) {
+						uint32_t *e = map + 2ull * (static_cast<unsigned long long>(c) * p.pb + s);
+						e[0] = bits;
+						e[1] = 0xffffffffu;
+					}
+				}
+		} else {
+			if (bad_stripe != 0xffffffffu) atomicMin(p.verdict + 3ull * c, static_cast<int>(bad_stripe));
+		}
 		// unit epilogue: the block CRCs against the stored ones
 		uint32_t lin = 0;
 		if (verify) lin = crc_mulmod(fold_finish<64>(win, p.tables), p.qmult[rr & 3]);
@@ -171,6 +205,19 @@ fused_check_kernel(const __grid_constant__ CheckTmaps tmaps, const __grid_consta
 			}
 		}
 	}
+}
+
+template <int R, bool CONSEC>
+__global__ void __launch_bounds__(kCheckThreads, 1)
+fused_check_kernel(const __grid_constant__ CheckTmaps tmaps, const __grid_constant__ CheckParams p) {
+	fused_check_body<R, CONSEC, false>(tmaps, p, nullptr);
+}
+
+// lzgpu_check_stripe_map: map = lzgpu_stripe_state[n_chunks * pb] as two words per entry
+template <int R, bool CONSEC>
+__global__ void __launch_bounds__(kCheckThreads, 1)
+fused_check_map_kernel(const __grid_constant__ CheckTmaps tmaps, const __grid_constant__ CheckParams p, uint32_t *map) {
+	fused_check_body<R, CONSEC, true>(tmaps, p, map);
 }
 
 }  // namespace lzd

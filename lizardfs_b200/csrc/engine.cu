@@ -531,15 +531,26 @@ int lz_gf_dot(lzgpu_ctx *ctx, const DotDesc &d, const uint8_t *coef /* n_dst x n
 }
 
 // the same dot products compared with the stored rows d.dst[r] (read only): a 16-byte unit of chunk c, block s that differs lowers
-// verdict[3c] to s (lzgpu_check_stripes, generic route; no parity-sized temporary)
-static int lz_gf_check(lzgpu_ctx *ctx, const DotDesc &d, const uint8_t *coef, int *verdict, cudaStream_t st) {
+// verdict[3c] to s (lzgpu_check_stripes, generic route; no parity-sized temporary).  map_rows (lzgpu_check_stripe_map): verdict is the
+// stripe map, zeroed, and a differing dest r sets bit map_rows[r] in the bad_rows word of its block's entry.
+static int lz_gf_check(lzgpu_ctx *ctx, const DotDesc &d, const uint8_t *coef, int *verdict, cudaStream_t st, const uint8_t *map_rows = nullptr) {
 	for (unsigned r0 = 0; r0 < d.n_dst; r0 += kDotDests) {
 		const unsigned nd = std::min<unsigned>(kDotDests, d.n_dst - r0);
 		DotArgs a{};
 		const size_t smem = dot_pass_args(d, coef, r0, nd, a);
 		const int threads = 256;
 		const int grid = grid_for(ctx, d.total_units, threads, 8);
-		switch (nd) {
+		if (map_rows) {
+			uint32_t rows = 0;
+			for (unsigned r = 0; r < nd; ++r) rows |= static_cast<uint32_t>(map_rows[r0 + r]) << (8 * r);
+			uint32_t *map = reinterpret_cast<uint32_t *>(verdict);
+			switch (nd) {
+				case 1: gf_check_map_kernel<1><<<grid, threads, smem, st>>>(a, map, rows); break;
+				case 2: gf_check_map_kernel<2><<<grid, threads, smem, st>>>(a, map, rows); break;
+				case 3: gf_check_map_kernel<3><<<grid, threads, smem, st>>>(a, map, rows); break;
+				default: gf_check_map_kernel<4><<<grid, threads, smem, st>>>(a, map, rows); break;
+			}
+		} else switch (nd) {
 			case 1: gf_check_kernel<1><<<grid, threads, smem, st>>>(a, verdict); break;
 			case 2: gf_check_kernel<2><<<grid, threads, smem, st>>>(a, verdict); break;
 			case 3: gf_check_kernel<3><<<grid, threads, smem, st>>>(a, verdict); break;
@@ -1057,9 +1068,10 @@ static int check_args(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t nb, const
 	return LZGPU_OK;
 }
 
-// enqueue the whole check on `st` (arguments validated by check_args); *tk is armed when stored CRCs are verified
+// enqueue the whole check on `st` (arguments validated by check_args); *tk is armed when stored CRCs are verified.  map: d_verdict is
+// the stripe map (lzgpu_check_stripe_map) instead of the verdicts.
 static int check_enqueue(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, uint32_t nb, const void *const *d_parts, size_t part_stride,
-                         const void *const *d_part_crc, void *d_verdict, cudaStream_t st, VerifyTicket *tk) {
+                         const void *const *d_part_crc, void *d_verdict, cudaStream_t st, VerifyTicket *tk, bool map = false) {
 	const int k = goal->k, m = goal->m, n = k + m;
 	const uint32_t B = LZGPU_BLOCK_SIZE;
 	const uint32_t pb = (nb + k - 1) / k;
@@ -1068,8 +1080,10 @@ static int check_enqueue(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chun
 	for (int i = 0; i < n; ++i) any_crc |= d_parts[i] && d_part_crc && d_part_crc[i];
 	int rc;
 	if (any_crc && (rc = tk->arm(ctx, st))) return rc;
-	// first_bad_stripe of every chunk starts above any stripe; the check kernels lower it, locate_kernel writes the whole verdict
-	CUDA_TRY(cudaMemsetAsync(d_verdict, 0x7f, static_cast<size_t>(n_chunks) * sizeof(lzgpu_stripe_verdict), st));
+	// first_bad_stripe of every chunk starts above any stripe; the check kernels lower it, locate_kernel writes the whole verdict.  The
+	// fused map kernel writes every entry of the map; the generic route ORs into a zeroed one.
+	const size_t map_bytes = static_cast<size_t>(n_chunks) * pb * sizeof(lzgpu_stripe_state);
+	if (!map) CUDA_TRY(cudaMemsetAsync(d_verdict, 0x7f, static_cast<size_t>(n_chunks) * sizeof(lzgpu_stripe_verdict), st));
 	TmpBuf tmp_crc(ctx, st);
 	auto verify_inputs = [&]() -> int {
 		int r;
@@ -1095,7 +1109,7 @@ static int check_enqueue(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chun
 			++la.n_rows;
 		}
 
-	rc = lz_fused_check(ctx, goal, n_chunks, nb, d_parts, part_stride, crc_for_kernels, d_verdict, st, tk->word(0));
+	rc = lz_fused_check(ctx, goal, n_chunks, nb, d_parts, part_stride, crc_for_kernels, d_verdict, st, tk->word(0), map);
 	const bool fused = rc != LZGPU_NOT_HANDLED;
 	if (fused && rc) return rc;
 	if (!fused) {
@@ -1117,54 +1131,74 @@ static int check_enqueue(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chun
 		d.src_block_stride = d.dst_block_stride = B;
 		d.units_per_block = B / 16;
 		d.blocks_per_chunk = pb;
-		if ((rc = lz_gf_check(ctx, d, rows, static_cast<int *>(d_verdict), st))) return rc;
+		if (map) CUDA_TRY(cudaMemsetAsync(d_verdict, 0, map_bytes, st));
+		if ((rc = lz_gf_check(ctx, d, rows, static_cast<int *>(d_verdict), st, map ? la.row : nullptr))) return rc;
 	}
 	la.verdict = static_cast<int *>(d_verdict);
 	la.part_stride = part_stride;
 	la.k = k;
 	la.pb = pb;
-	locate_kernel<<<n_chunks, 256, 0, st>>>(la);
+	if (map) {
+		const unsigned long long entries = static_cast<unsigned long long>(n_chunks) * pb;
+		locate_map_kernel<<<grid_for(ctx, entries * 256, 256, 8), 256, 0, st>>>(la, entries);
+	} else {
+		locate_kernel<<<n_chunks, 256, 0, st>>>(la);
+	}
 	CUDA_TRY(cudaGetLastError());
 	ctx->stats.kernel_launches++;
 	if (!any_crc) return LZGPU_OK;
 	return (fused && crc_for_kernels) ? tk->publish_fused() : tk->publish_per_part(n, pb);
 }
 
-static uint64_t check_alg_bytes(const lzgpu_goal *goal, uint32_t n_chunks, uint32_t nb, const void *const *parts, const void *const *part_crc) {
-	// read every given part and its stored CRCs, write one verdict per chunk
+static uint64_t check_alg_bytes(const lzgpu_goal *goal, uint32_t n_chunks, uint32_t nb, const void *const *parts, const void *const *part_crc,
+                                bool map = false) {
+	// read every given part and its stored CRCs, write one verdict per chunk (the map: one state per stripe)
 	const uint64_t pb = (nb + goal->k - 1) / goal->k, B = LZGPU_BLOCK_SIZE;
-	uint64_t bytes = sizeof(lzgpu_stripe_verdict);
+	uint64_t bytes = map ? pb * sizeof(lzgpu_stripe_state) : sizeof(lzgpu_stripe_verdict);
 	for (int i = 0; i < goal->k + goal->m; ++i)
 		if (parts[i]) bytes += pb * B + ((part_crc && part_crc[i]) ? 4 * pb : 0);
 	return n_chunks * bytes;
 }
 
-extern "C" int lzgpu_check_stripes_dev(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, uint32_t nb, const void *const *d_parts,
-                                       size_t part_stride, const void *const *d_part_crc, void *d_verdict, int64_t *bad, void *stream) {
-	NvtxScope nvtx_scope("lzgpu::check_stripes_dev");
-	int rc = check_args(ctx, goal, nb, d_parts, d_part_crc, d_verdict, true);
+static int check_dev(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, uint32_t nb, const void *const *d_parts, size_t part_stride,
+                     const void *const *d_part_crc, void *d_out, int64_t *bad, void *stream, bool map) {
+	int rc = check_args(ctx, goal, nb, d_parts, d_part_crc, d_out, true);
 	if (rc) return rc;
 	if (n_chunks == 0) return LZGPU_OK;
 	DeviceGuard g(ctx->device);
 	cudaStream_t st = stream ? static_cast<cudaStream_t>(stream) : ctx->stream;
 	VerifyTicket tk;
 	{
-		BatchTimer timer(ctx, st, check_alg_bytes(goal, n_chunks, nb, d_parts, d_part_crc));
-		if ((rc = check_enqueue(ctx, goal, n_chunks, nb, d_parts, part_stride, d_part_crc, d_verdict, st, &tk))) return rc;
+		BatchTimer timer(ctx, st, check_alg_bytes(goal, n_chunks, nb, d_parts, d_part_crc, map));
+		if ((rc = check_enqueue(ctx, goal, n_chunks, nb, d_parts, part_stride, d_part_crc, d_out, st, &tk, map))) return rc;
 	}
 	return dev_verdict(ctx, std::move(tk), bad);
 }
 
-extern "C" int lzgpu_check_stripes(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, uint32_t nb, const uint8_t *const *parts,
-                                   size_t part_stride, const uint32_t *const *part_crc, lzgpu_stripe_verdict *verdict, int64_t *bad) {
-	NvtxScope nvtx_scope("lzgpu::check_stripes");
-	int rc = check_args(ctx, goal, nb, reinterpret_cast<const void *const *>(parts), nullptr, verdict, false);
+extern "C" int lzgpu_check_stripes_dev(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, uint32_t nb, const void *const *d_parts,
+                                       size_t part_stride, const void *const *d_part_crc, void *d_verdict, int64_t *bad, void *stream) {
+	NvtxScope nvtx_scope("lzgpu::check_stripes_dev");
+	return check_dev(ctx, goal, n_chunks, nb, d_parts, part_stride, d_part_crc, d_verdict, bad, stream, false);
+}
+
+extern "C" int lzgpu_check_stripe_map_dev(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, uint32_t nb, const void *const *d_parts,
+                                          size_t part_stride, const void *const *d_part_crc, void *d_map, int64_t *bad, void *stream) {
+	NvtxScope nvtx_scope("lzgpu::check_stripe_map_dev");
+	return check_dev(ctx, goal, n_chunks, nb, d_parts, part_stride, d_part_crc, d_map, bad, stream, true);
+}
+
+// the host-pointer calls: out = lzgpu_stripe_verdict[n_chunks], or (map) lzgpu_stripe_state[n_chunks * pb]
+static int check_host(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, uint32_t nb, const uint8_t *const *parts,
+                      size_t part_stride, const uint32_t *const *part_crc, void *out, int64_t *bad, bool map) {
+	int rc = check_args(ctx, goal, nb, reinterpret_cast<const void *const *>(parts), nullptr, out, false);
 	if (rc) return rc;
 	if (n_chunks == 0) return LZGPU_OK;
 	const int k = goal->k, n = goal->k + goal->m;
 	const uint32_t B = LZGPU_BLOCK_SIZE;
 	const uint32_t pb = (nb + k - 1) / k;
 	const size_t part_bytes = static_cast<size_t>(pb) * B;
+	const size_t out_per_chunk = map ? pb * sizeof(lzgpu_stripe_state) : sizeof(lzgpu_stripe_verdict);
+	uint8_t *const out_bytes = static_cast<uint8_t *>(out);
 	if (part_stride < part_bytes) { lz_set_error("check_stripes: part_stride too small"); return LZGPU_ERR_ARG; }
 	int n_given = 0;
 	for (int i = 0; i < n; ++i) n_given += parts[i] ? 1 : 0;
@@ -1173,7 +1207,7 @@ extern "C" int lzgpu_check_stripes(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint3
 	AutoPin pin(ctx);
 	for (int i = 0; i < n; ++i)
 		if (parts[i]) pin.add(parts[i], static_cast<size_t>(n_chunks - 1) * part_stride + part_bytes);
-	pin.add(verdict, static_cast<size_t>(n_chunks) * sizeof(lzgpu_stripe_verdict));
+	pin.add(out, static_cast<size_t>(n_chunks) * out_per_chunk);
 	// device layout of a tile: every given part dense (stride = part_bytes), all parts of a slot in one buffer
 	const uint32_t tile = static_cast<uint32_t>(std::max<size_t>(1, std::min<size_t>(n_chunks, (2 * kHostTileBytes) / (part_bytes * n_given))));
 	const size_t dev_part = static_cast<size_t>(tile) * part_bytes;
@@ -1183,9 +1217,9 @@ extern "C" int lzgpu_check_stripes(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint3
 	for (int s = 0; s < n_slots; ++s) {
 		if ((rc = lz_scratch(ctx, kScratchIn0 + s, dev_part * n, &d_all[s]))) return rc;
 		if ((rc = lz_scratch(ctx, kScratchCrc0 + s, dev_crc * n, &d_crc_all[s]))) return rc;
-		if ((rc = lz_scratch(ctx, kScratchPar0 + s, static_cast<size_t>(tile) * sizeof(lzgpu_stripe_verdict), &d_ver[s]))) return rc;
+		if ((rc = lz_scratch(ctx, kScratchPar0 + s, static_cast<size_t>(tile) * out_per_chunk, &d_ver[s]))) return rc;
 	}
-	// a stored-CRC mismatch does not stop the pipeline: every chunk gets its verdict
+	// a stored-CRC mismatch does not stop the pipeline: every chunk gets its verdict (its map)
 	rc = run_tiles(ctx, n_chunks, tile, n_slots, bad, [&](int s, size_t c0, size_t nc, cudaStream_t st, VerifyTicket *tk) -> int {
 		std::vector<const void *> dp(n, nullptr), dc(n, nullptr);
 		bool any_crc = false;
@@ -1204,21 +1238,43 @@ extern "C" int lzgpu_check_stripes(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint3
 		}
 		int rc;
 		{
-			BatchTimer timer(ctx, st, check_alg_bytes(goal, static_cast<uint32_t>(nc), nb, dp.data(), any_crc ? dc.data() : nullptr));
-			rc = check_enqueue(ctx, goal, static_cast<uint32_t>(nc), nb, dp.data(), part_bytes, any_crc ? dc.data() : nullptr, d_ver[s], st, tk);
+			BatchTimer timer(ctx, st, check_alg_bytes(goal, static_cast<uint32_t>(nc), nb, dp.data(), any_crc ? dc.data() : nullptr, map));
+			rc = check_enqueue(ctx, goal, static_cast<uint32_t>(nc), nb, dp.data(), part_bytes, any_crc ? dc.data() : nullptr, d_ver[s], st, tk, map);
 		}
 		if (rc) return rc;
-		CUDA_TRY(cudaMemcpyAsync(verdict + c0, d_ver[s], nc * sizeof(lzgpu_stripe_verdict), cudaMemcpyDeviceToHost, st));
-		ctx->stats.bytes_d2h += nc * sizeof(lzgpu_stripe_verdict);
+		CUDA_TRY(cudaMemcpyAsync(out_bytes + c0 * out_per_chunk, d_ver[s], nc * out_per_chunk, cudaMemcpyDeviceToHost, st));
+		ctx->stats.bytes_d2h += nc * out_per_chunk;
 		return LZGPU_OK;
 	}, true);
 	if (rc) return rc;
+	if (map) {
+		const lzgpu_stripe_state *e = static_cast<const lzgpu_stripe_state *>(out);
+		for (size_t i = 0; i < static_cast<size_t>(n_chunks) * pb; ++i)
+			if (e[i].bad_rows) {
+				lz_set_error("check_stripe_map: chunk %zu stripe %zu is not a codeword", i / pb, i % pb);
+				return LZGPU_ERR_INCONSISTENT;
+			}
+		return LZGPU_OK;
+	}
+	const lzgpu_stripe_verdict *verdict = static_cast<const lzgpu_stripe_verdict *>(out);
 	for (uint32_t c = 0; c < n_chunks; ++c)
 		if (verdict[c].first_bad_stripe >= 0) {
 			lz_set_error("check_stripes: chunk %u stripe %d is not a codeword", c, verdict[c].first_bad_stripe);
 			return LZGPU_ERR_INCONSISTENT;
 		}
 	return LZGPU_OK;
+}
+
+extern "C" int lzgpu_check_stripes(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, uint32_t nb, const uint8_t *const *parts,
+                                   size_t part_stride, const uint32_t *const *part_crc, lzgpu_stripe_verdict *verdict, int64_t *bad) {
+	NvtxScope nvtx_scope("lzgpu::check_stripes");
+	return check_host(ctx, goal, n_chunks, nb, parts, part_stride, part_crc, verdict, bad, false);
+}
+
+extern "C" int lzgpu_check_stripe_map(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, uint32_t nb, const uint8_t *const *parts,
+                                      size_t part_stride, const uint32_t *const *part_crc, lzgpu_stripe_state *map, int64_t *bad) {
+	NvtxScope nvtx_scope("lzgpu::check_stripe_map");
+	return check_host(ctx, goal, n_chunks, nb, parts, part_stride, part_crc, map, bad, true);
 }
 
 // ------------------------------------------------------------------------------------------------

@@ -168,6 +168,13 @@ static int set_all_recover_attrs() {
 	CUDA_TRY(cudaFuncSetAttribute(fused_check_kernel<1, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kRecoverSmemCapBig));
 	CUDA_TRY(cudaFuncSetAttribute(fused_check_kernel<2, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kRecoverSmemCapBig));
 	CUDA_TRY(cudaFuncSetAttribute(fused_check_kernel<3, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kRecoverSmemCapBig));
+	CUDA_TRY(cudaFuncSetAttribute(fused_check_map_kernel<1, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kRecoverSmemCapBig));
+	CUDA_TRY(cudaFuncSetAttribute(fused_check_map_kernel<2, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kRecoverSmemCapBig));
+	CUDA_TRY(cudaFuncSetAttribute(fused_check_map_kernel<3, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kRecoverSmemCapBig));
+	CUDA_TRY(cudaFuncSetAttribute(fused_check_map_kernel<4, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kRecoverSmemCapBig));
+	CUDA_TRY(cudaFuncSetAttribute(fused_check_map_kernel<1, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kRecoverSmemCapBig));
+	CUDA_TRY(cudaFuncSetAttribute(fused_check_map_kernel<2, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kRecoverSmemCapBig));
+	CUDA_TRY(cudaFuncSetAttribute(fused_check_map_kernel<3, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kRecoverSmemCapBig));
 	return LZGPU_OK;
 }
 
@@ -884,7 +891,7 @@ int lz_fused_recover(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, 
 // fused stripe check (check_kernel.cuh)
 // ---------------------------------------------------------------------------------------------------
 int lz_fused_check(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, uint32_t nb, const void *const *d_parts, size_t part_stride,
-                   const void *const *d_part_crc, void *d_verdict, cudaStream_t st, unsigned long long *d_first_bad) {
+                   const void *const *d_part_crc, void *d_verdict, cudaStream_t st, unsigned long long *d_first_bad, bool map) {
 	FusedState *fs = ctx->fused;
 	if (!fs || fs->disabled) return LZGPU_NOT_HANDLED;
 	const int K = goal->k, M = goal->m;
@@ -923,7 +930,7 @@ int lz_fused_check(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, ui
 	const uint32_t n_stages = static_cast<uint32_t>(std::min<size_t>(6, (kRecoverSmemCapBig - 256) / (static_cast<size_t>(NSLOT) * G * 4 * kStepBytes)));
 	p.tables = ctx->d_crc_tables;
 	p.first_bad = d_first_bad;
-	p.verdict = static_cast<int *>(d_verdict);
+	p.verdict = map ? nullptr : static_cast<int *>(d_verdict);
 	p.n_chunks = n_chunks;
 	p.pb = pb;
 	p.K = K;
@@ -948,7 +955,17 @@ int lz_fused_check(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, ui
 	}
 	const size_t smem = static_cast<size_t>(n_stages) * NSLOT * G * 4 * kStepBytes + 16 * n_stages + 64;
 	const int grid = persistent_grid(ctx, p.total_units, 1, launch_geo(LZGPU_KERNEL_CHECK, kCheckThreads, G, n_stages, 0, smem));
-	switch (consecutive ? R : R + 4) {
+	uint32_t *d_map = static_cast<uint32_t *>(d_verdict);
+	if (map) switch (consecutive ? R : R + 4) {
+		case 1: fused_check_map_kernel<1, true><<<grid, kCheckThreads, smem, st>>>(maps, p, d_map); break;
+		case 2: fused_check_map_kernel<2, true><<<grid, kCheckThreads, smem, st>>>(maps, p, d_map); break;
+		case 3: fused_check_map_kernel<3, true><<<grid, kCheckThreads, smem, st>>>(maps, p, d_map); break;
+		case 4: fused_check_map_kernel<4, true><<<grid, kCheckThreads, smem, st>>>(maps, p, d_map); break;
+		case 5: fused_check_map_kernel<1, false><<<grid, kCheckThreads, smem, st>>>(maps, p, d_map); break;
+		case 6: fused_check_map_kernel<2, false><<<grid, kCheckThreads, smem, st>>>(maps, p, d_map); break;
+		default: fused_check_map_kernel<3, false><<<grid, kCheckThreads, smem, st>>>(maps, p, d_map); break;
+	}
+	else switch (consecutive ? R : R + 4) {
 		case 1: fused_check_kernel<1, true><<<grid, kCheckThreads, smem, st>>>(maps, p); break;
 		case 2: fused_check_kernel<2, true><<<grid, kCheckThreads, smem, st>>>(maps, p); break;
 		case 3: fused_check_kernel<3, true><<<grid, kCheckThreads, smem, st>>>(maps, p); break;

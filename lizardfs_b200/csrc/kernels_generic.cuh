@@ -30,10 +30,15 @@ struct DotArgs {
 	unsigned int pure_xor;  // every coefficient is 1 (xorN goals / parity row 0): skip the multiply
 };
 
-// CHECK = false: dst_r = the dot product.  CHECK = true (lzgpu_check_stripes): dst_r holds the stored parity and is only read; a
-// 16-byte unit that differs from the dot product lowers the first_bad_stripe word of its chunk's verdict (3 ints per chunk).
-template <int ND, bool CHECK>
-__device__ __forceinline__ void gf_dot_body(const DotArgs &a, int *verdict) {
+// The epilogue of gf_dot_body.  kDotStore: dst_r = the dot product.  kDotCheck (lzgpu_check_stripes): dst_r holds the stored parity and
+// is only read; a 16-byte unit that differs from the dot product lowers the first_bad_stripe word of its chunk's verdict (3 ints per
+// chunk).  kDotMap (lzgpu_check_stripe_map): as kDotCheck, but each differing dest d sets bit map_rows[8d..8d+7] (its parity row) and
+// the bits are ORed into the bad_rows word of the unit's stripe, map[2 (c blocks_per_chunk + s)]: a warp's 32 units lie in one block
+// (units_per_block and the grid stride are multiples of 32), so the warp reduces first and lane 0 issues one atomicOr.
+enum DotEpilogue { kDotStore, kDotCheck, kDotMap };
+
+template <int ND, DotEpilogue E>
+__device__ __forceinline__ void gf_dot_body(const DotArgs &a, int *verdict, uint32_t map_rows = 0) {
 	extern __shared__ CoefPlanes s_coef[];  // [ND][n_src]
 	for (unsigned i = threadIdx.x; i < ND * a.n_src; i += blockDim.x) coef_planes_set(s_coef[i], a.coef[i]);
 	__syncthreads();
@@ -72,7 +77,16 @@ __device__ __forceinline__ void gf_dot_body(const DotArgs &a, int *verdict) {
 			}
 		}
 		const unsigned long long dst_off = c * a.dst_chunk_stride + s * a.dst_block_stride + 16ull * o;
-		if constexpr (CHECK) {
+		if constexpr (E == kDotMap) {
+			uint32_t bits = 0;
+#pragma unroll
+			for (int d = 0; d < ND; ++d) {
+				const uint4 v = ld_stream(reinterpret_cast<const uint4 *>(a.dst[d] + dst_off));
+				if ((v.x ^ acc[d][0]) | (v.y ^ acc[d][1]) | (v.z ^ acc[d][2]) | (v.w ^ acc[d][3])) bits |= 1u << ((map_rows >> (8 * d)) & 31u);
+			}
+			bits = __reduce_or_sync(0xffffffffu, bits);
+			if (bits && (threadIdx.x & 31) == 0) atomicOr(reinterpret_cast<unsigned *>(verdict) + 2ull * (c * a.blocks_per_chunk + s), bits);
+		} else if constexpr (E == kDotCheck) {
 			uint32_t diff = 0;
 #pragma unroll
 			for (int d = 0; d < ND; ++d) {
@@ -90,10 +104,15 @@ __device__ __forceinline__ void gf_dot_body(const DotArgs &a, int *verdict) {
 }
 
 template <int ND>
-__global__ void __launch_bounds__(256) gf_dot_kernel(const DotArgs a) { gf_dot_body<ND, false>(a, nullptr); }
+__global__ void __launch_bounds__(256) gf_dot_kernel(const DotArgs a) { gf_dot_body<ND, kDotStore>(a, nullptr); }
 
 template <int ND>
-__global__ void __launch_bounds__(256) gf_check_kernel(const DotArgs a, int *verdict) { gf_dot_body<ND, true>(a, verdict); }
+__global__ void __launch_bounds__(256) gf_check_kernel(const DotArgs a, int *verdict) { gf_dot_body<ND, kDotCheck>(a, verdict); }
+
+template <int ND>
+__global__ void __launch_bounds__(256) gf_check_map_kernel(const DotArgs a, uint32_t *map, uint32_t map_rows) {
+	gf_dot_body<ND, kDotMap>(a, reinterpret_cast<int *>(map), map_rows);
+}
 
 // The verdict of each chunk of lzgpu_check_stripes once a check kernel has lowered its first_bad_stripe word (initialised to a value
 // above any stripe).  One CTA per chunk; a clean chunk is written {-1, 0, -1} at once.  Otherwise the CTA recomputes the syndromes of
@@ -103,7 +122,7 @@ __global__ void __launch_bounds__(256) gf_check_kernel(const DotArgs a, int *ver
 // rows checked) names it.
 struct LocateArgs {
 	const uint8_t *part[64];            // data parts 0..k-1, then parity part r at k + r; nullptr = not given (a parity row not checked)
-	int *verdict;                       // lzgpu_stripe_verdict[n_chunks] as 3 ints
+	int *verdict;                       // lzgpu_stripe_verdict[n_chunks] as 3 ints (locate_map_kernel: the stripe map, 2 ints per entry)
 	unsigned long long part_stride;
 	uint32_t k, pb, n_rows;
 	uint8_t row[32];                    // parity row of checked row i
@@ -114,41 +133,46 @@ __device__ __forceinline__ uint32_t gf_mul_tab(uint32_t a, uint32_t b, const uin
 	return (a && b) ? ex[lg[a] + lg[b]] : 0u;
 }
 
-__global__ void __launch_bounds__(256) locate_kernel(const LocateArgs a) {
-	__shared__ uint8_t s_log[256], s_exp[512];
-	__shared__ uint8_t s_syn[32][256];  // syndromes of this thread's current byte, one column per thread
-	__shared__ unsigned long long s_cand;
-	__shared__ unsigned s_rows;
-	const unsigned tid = threadIdx.x;
-	int *v = a.verdict + 3ull * blockIdx.x;
-	const int s = v[0];
-	if (s < 0 || static_cast<uint32_t>(s) >= a.pb) {
-		if (tid == 0) { v[0] = -1; v[1] = 0; v[2] = -1; }
-		return;
-	}
-	if (tid == 0) {
+struct LocateSmem {
+	uint8_t log[256], exp[512];
+	uint8_t syn[32][256];  // syndromes of this thread's current byte, one column per thread
+	unsigned long long cand;
+	unsigned rows;
+};
+
+// GF(2^8) log / exp tables (thread 0; the caller's next barrier publishes them)
+__device__ __forceinline__ void locate_tables(LocateSmem &sm) {
+	if (threadIdx.x == 0) {
 		uint32_t x = 1;
 		for (int i = 0; i < 255; ++i) {
-			s_exp[i] = s_exp[i + 255] = static_cast<uint8_t>(x);
-			s_log[x] = static_cast<uint8_t>(i);
+			sm.exp[i] = sm.exp[i + 255] = static_cast<uint8_t>(x);
+			sm.log[x] = static_cast<uint8_t>(i);
 			x = (x << 1) ^ ((x & 0x80u) ? 0x11du : 0u);
 		}
-		s_log[0] = 0;
+		sm.log[0] = 0;
+	}
+}
+
+// Stripe s of chunk c, by the whole CTA (every thread calls it; the tables are built): the rows with a non-zero syndrome (*rows) and
+// the suspect part, or -1.  Ends with a barrier, so the CTA can go on to another stripe.
+__device__ __forceinline__ int locate_stripe(const LocateArgs &a, LocateSmem &sm, unsigned long long c, uint32_t s, unsigned *rows_out) {
+	const unsigned tid = threadIdx.x;
+	if (tid == 0) {
 		unsigned long long cand = (1ull << a.k) - 1ull;
 		for (uint32_t i = 0; i < a.n_rows; ++i) cand |= 1ull << (a.k + a.row[i]);
-		s_cand = cand;
-		s_rows = 0;
+		sm.cand = cand;
+		sm.rows = 0;
 	}
 	__syncthreads();
-	unsigned long long cand = s_cand;
+	unsigned long long cand = sm.cand;
 	unsigned rows = 0;
-	const unsigned long long off = blockIdx.x * a.part_stride + static_cast<unsigned long long>(s) * 65536ull;
+	const unsigned long long off = c * a.part_stride + static_cast<unsigned long long>(s) * 65536ull;
 	for (unsigned b = tid; b < 65536u; b += blockDim.x) {
 		int first = -1;
 		for (uint32_t i = 0; i < a.n_rows; ++i) {
 			uint32_t syn = a.part[a.k + a.row[i]][off + b];
-			for (uint32_t j = 0; j < a.k; ++j) syn ^= gf_mul_tab(a.coef[i * 32 + j], a.part[j][off + b], s_log, s_exp);
-			s_syn[i][tid] = static_cast<uint8_t>(syn);
+			for (uint32_t j = 0; j < a.k; ++j) syn ^= gf_mul_tab(a.coef[i * 32 + j], a.part[j][off + b], sm.log, sm.exp);
+			sm.syn[i][tid] = static_cast<uint8_t>(syn);
 			if (syn) {
 				rows |= 1u << a.row[i];
 				if (first < 0) first = static_cast<int>(i);
@@ -160,21 +184,55 @@ __global__ void __launch_bounds__(256) locate_kernel(const LocateArgs a) {
 			bool fits = true;
 			if (part < a.k) {
 				// S = e * column: e from the first non-zero row, then every row must agree
-				const uint32_t e = s_exp[s_log[s_syn[first][tid]] + 255 - s_log[a.coef[first * 32 + part]]];
-				for (uint32_t i = 0; i < a.n_rows && fits; ++i) fits = s_syn[i][tid] == gf_mul_tab(e, a.coef[i * 32 + part], s_log, s_exp);
+				const uint32_t e = sm.exp[sm.log[sm.syn[first][tid]] + 255 - sm.log[a.coef[first * 32 + part]]];
+				for (uint32_t i = 0; i < a.n_rows && fits; ++i) fits = sm.syn[i][tid] == gf_mul_tab(e, a.coef[i * 32 + part], sm.log, sm.exp);
 			} else {
-				for (uint32_t i = 0; i < a.n_rows && fits; ++i) fits = a.k + a.row[i] == part || s_syn[i][tid] == 0;
+				for (uint32_t i = 0; i < a.n_rows && fits; ++i) fits = a.k + a.row[i] == part || sm.syn[i][tid] == 0;
 			}
 			if (!fits) cand &= ~(1ull << part);
 		}
 	}
-	atomicAnd(&s_cand, cand);
-	atomicOr(&s_rows, rows);
+	atomicAnd(&sm.cand, cand);
+	atomicOr(&sm.rows, rows);
 	__syncthreads();
-	if (tid == 0) {
-		const unsigned long long c = s_cand;
-		v[1] = static_cast<int>(s_rows);
-		v[2] = (a.n_rows >= 2 && c && !(c & (c - 1))) ? __ffsll(static_cast<long long>(c)) - 1 : -1;
+	const unsigned long long left = sm.cand;
+	*rows_out = sm.rows;
+	__syncthreads();
+	return (a.n_rows >= 2 && left && !(left & (left - 1))) ? __ffsll(static_cast<long long>(left)) - 1 : -1;
+}
+
+__global__ void __launch_bounds__(256) locate_kernel(const LocateArgs a) {
+	__shared__ LocateSmem sm;
+	int *v = a.verdict + 3ull * blockIdx.x;
+	const int s = v[0];
+	if (s < 0 || static_cast<uint32_t>(s) >= a.pb) {
+		if (threadIdx.x == 0) { v[0] = -1; v[1] = 0; v[2] = -1; }
+		return;
+	}
+	locate_tables(sm);
+	unsigned rows;
+	const int suspect = locate_stripe(a, sm, blockIdx.x, static_cast<uint32_t>(s), &rows);
+	if (threadIdx.x == 0) {
+		v[1] = static_cast<int>(rows);
+		v[2] = suspect;
+	}
+}
+
+// lzgpu_check_stripe_map, after either route has written every entry's bad_rows (a.verdict = the map as two words per entry, n
+// entries): grid-stride over the entries, one CTA per bad stripe, which names its suspect; a clean entry's suspect_part is set to -1.
+// bad_rows stays as the check kernel wrote it.
+__global__ void __launch_bounds__(256) locate_map_kernel(const LocateArgs a, unsigned long long n) {
+	__shared__ LocateSmem sm;
+	locate_tables(sm);  // built by every CTA: deferring it to the first bad entry makes ptxas spill the locate loop
+	for (unsigned long long e = blockIdx.x; e < n; e += gridDim.x) {
+		int *v = a.verdict + 2ull * e;
+		if (v[0] == 0) {
+			if (threadIdx.x == 0) v[1] = -1;
+			continue;
+		}
+		unsigned rows;
+		const int suspect = locate_stripe(a, sm, e / a.pb, static_cast<uint32_t>(e % a.pb), &rows);
+		if (threadIdx.x == 0) v[1] = suspect;
 	}
 }
 

@@ -547,6 +547,44 @@ class Engine:
             raise ChunkCrcError(rc, "check_stripes_dev", (bad[0], bad[1], bad[2]))
         _check(rc, "check_stripes_dev")
 
+    STRIPE_STATE_DTYPE = np.dtype([("bad_rows", np.uint32), ("suspect_part", np.int32)])
+
+    def check_stripe_map(self, goal, nb, parts, part_crc=None):
+        """The state of every stripe of every chunk (lzgpu_check_stripe_map); parts and part_crc as in check_stripes.  Returns a
+        structured array [n_chunks, pb] of STRIPE_STATE_DTYPE (bad_rows, 0 = a codeword; suspect_part, -1 = none), whether or not
+        any stripe is bad; raises ChunkCrcError on a stored-CRC mismatch (its .map holds the map, written in full all the same).
+        For each chunk the lowest bad stripe and its entry equal check_stripes' verdict."""
+        assert len(parts) == goal.k + goal.m
+        pb = (nb + goal.k - 1) // goal.k
+        parts = [None if p is None else _u8(p).reshape(-1, pb * BLOCK_SIZE) for p in parts]
+        n = next(p.shape[0] for p in parts if p is not None)
+        crcs = None
+        if part_crc is not None:
+            crcs = [None if c is None else np.ascontiguousarray(c, dtype=np.uint32) for c in part_crc]
+        smap = np.empty((n, pb), dtype=self.STRIPE_STATE_DTYPE)
+        bad = (C.c_int64 * 3)(-1, -1, -1)
+        rc = self.lib.lzgpu_check_stripe_map(self.h, C.byref(goal.c), n, nb, _ptr_array(parts), pb * BLOCK_SIZE,
+                                             _ptr_array(crcs) if crcs is not None else None, _p(smap), bad)
+        if rc == _lib.ERR_CRC:
+            err = ChunkCrcError(rc, "check_stripe_map", (bad[0], bad[1], bad[2]))
+            err.map = smap
+            raise err
+        if rc != _lib.ERR_INCONSISTENT:
+            _check(rc, "check_stripe_map")
+        return smap
+
+    def check_stripe_map_dev(self, goal, n_chunks, nb, d_parts, part_stride, d_part_crc, d_map, stream=None):
+        """Device-pointer stripe map: n_chunks * pb entries of 8 bytes go to d_map (device memory).  With d_part_crc the call waits
+        for its stream and raises ChunkCrcError on a mismatch; without it the call only enqueues."""
+        n_parts = goal.k + goal.m
+        dp = (C.c_void_p * n_parts)(*[p if p else None for p in d_parts])
+        dc = (C.c_void_p * n_parts)(*[p if p else None for p in d_part_crc]) if d_part_crc is not None else None
+        bad = (C.c_int64 * 3)(-1, -1, -1)
+        rc = self.lib.lzgpu_check_stripe_map_dev(self.h, C.byref(goal.c), n_chunks, nb, dp, part_stride, dc, d_map, bad, stream)
+        if rc == _lib.ERR_CRC:
+            raise ChunkCrcError(rc, "check_stripe_map_dev", (bad[0], bad[1], bad[2]))
+        _check(rc, "check_stripe_map_dev")
+
     # ---- wire format --------------------------------------------------------------------------
     def write_data_prefixes(self, goal, nb, crc, chunk_ids, write_id_base=0):
         """LIZ_CLTOCS_WRITE_DATA prefixes (cltocs.h:116-137) for every block of every part: uint8 [n, k+m, pb, 38]

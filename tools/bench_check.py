@@ -8,6 +8,11 @@ H100 SXM data-sheet HBM3 bandwidth of 3.35 TB/s.  The ec(8,2) degraded read of t
 parts read verified) is timed in the same run as the streaming reference point.  On each goal's timed buffers one byte is then flipped
 (its block CRC restored) and the fused and the generic route must return identical verdicts naming it.
 
+The stripe map (lzgpu_check_stripe_map_dev) is timed next to the check on the same resident batch, alternating the two calls, in three
+cases: a clean batch, one bad stripe per chunk (data part 3, stripe 5), and every stripe of every chunk bad (one byte of data part 0
+per stripe).  Clean stripes cost the one pass; a bad one is re-read by a CTA of its own to name its suspect.  In every case the maps of
+both routes must be identical and each chunk's lowest bad stripe must equal both routes' verdicts.
+
     python tools/bench_check.py [--chunks 16] [--iters 20] [--warmup 3]      (one JSON line per measurement)
 """
 import argparse
@@ -83,6 +88,58 @@ def verdicts(eng, r, out):
     return out.cpu().numpy().view(L.Engine.VERDICT_DTYPE).copy()
 
 
+def stripe_map(eng, r, out):
+    eng.check_stripe_map_dev(r.goal, r.n, NB, r.ptrs, r.stride, r.crc_ptrs, out.data_ptr())
+    torch.cuda.synchronize()
+    return out.cpu().numpy().view(L.Engine.STRIPE_STATE_DTYPE).reshape(r.n, r.pb).copy()
+
+
+def flip(eng, r, part, stripes, offset):
+    """flip one byte of `part` in each of `stripes` of every chunk, and restore the stored CRCs of those blocks"""
+    idx = torch.tensor([c * r.stride + part * r.part_bytes + s * BLOCK + offset for c in range(r.n) for s in stripes], device="cuda")
+    r.buf[idx] ^= 0x5A
+    for c in range(r.n):
+        eng.crc_blocks_dev(r.ptrs[part] + c * r.stride, r.pb, r.crc[part, c].data_ptr())
+    torch.cuda.synchronize()
+
+
+def map_rows(eng, generic, r, text, args, stream, info):
+    """time the map next to the check in the three cases, and check it against both routes' verdicts"""
+    st = stream.cuda_stream
+    out_v = torch.empty(12 * r.n, dtype=torch.uint8, device="cuda")
+    out_m = torch.empty(8 * r.n * r.pb, dtype=torch.uint8, device="cuda")
+    cases = [("clean", None), ("one_bad_stripe_per_chunk", (3, [5], 777)), ("every_stripe_bad", (0, range(r.pb), 4242))]
+    for case, fault in cases:
+        if fault:
+            flip(eng, r, *fault)
+        t_check = t_map = 0.0
+        for _ in range(2):               # alternate the calls, twice: other work shares the card
+            t_check += timed(lambda: eng.check_stripes_dev(r.goal, r.n, NB, r.ptrs, r.stride, r.crc_ptrs, out_v.data_ptr(), stream=st),
+                             args.iters, args.warmup, stream) / 2
+            t_map += timed(lambda: eng.check_stripe_map_dev(r.goal, r.n, NB, r.ptrs, r.stride, r.crc_ptrs, out_m.data_ptr(), stream=st),
+                           args.iters, args.warmup, stream) / 2
+        eng.sync()
+        route = "fused" if eng.last_geometry()["kernel"] == _lib.KERNEL_CHECK else "generic"
+        m_fused, m_generic = stripe_map(eng, r, out_m), stripe_map(generic, r, out_m)
+        assert (m_fused == m_generic).all(), "fused and generic maps differ"
+        for e in (eng, generic):
+            v = verdicts(e, r, out_v)
+            for c in range(r.n):
+                bad = m_fused[c]["bad_rows"].nonzero()[0]
+                first = (int(bad[0]), int(m_fused[c, bad[0]]["bad_rows"]), int(m_fused[c, bad[0]]["suspect_part"])) if len(bad) else (-1, 0, -1)
+                assert first == tuple(int(x) for x in v[c]), (c, first, v[c])
+        n_bad = int((m_fused["bad_rows"] != 0).sum())
+        assert n_bad == {"clean": 0, "one_bad_stripe_per_chunk": r.n, "every_stripe_bad": r.n * r.pb}[case]
+        if r.m >= 2 and fault:
+            assert (m_fused["suspect_part"][m_fused["bad_rows"] != 0] == fault[0]).all()
+        print(json.dumps({"what": "check_stripe_map_dev", "goal": text, "case": case, "route": route, "chunks": r.n,
+                          "chunk_mib": NB * BLOCK >> 20, "bad_stripes": n_bad, "ms_per_call": round(t_map * 1e3, 3),
+                          "check_stripes_ms_per_call": round(t_check * 1e3, 3), "map_over_check": round(t_map / t_check, 3),
+                          "chunk_gib_s": round(r.n * NB * BLOCK / t_map / 2**30, 1), "routes_agree": True, **info}), flush=True)
+        if fault:
+            flip(eng, r, *fault)         # flipped back: the next case starts from a clean batch
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--chunks", type=int, default=16)
@@ -139,6 +196,11 @@ def main():
                               "alg_tb_s": round(rec_bytes / t_rec / 1e12, 3), "of_hbm": round(rec_bytes / t_rec / 1e12 / HBM_TBPS, 3),
                               "geometry": eng.last_geometry(), **info}), flush=True)
             del outs
+        if text != "ec(8,2)":   # the map cases start from a clean batch (the ec(8,2) branch restored the byte already)
+            r.buf[off] ^= 0x5A
+            eng.crc_blocks_dev(r.ptrs[part] + c * r.stride + s * BLOCK, 1, r.crc[part, c, s:].data_ptr())
+            torch.cuda.synchronize()
+        map_rows(eng, generic, r, text, args, stream, info)
         del r, out
         torch.cuda.empty_cache()
     eng.set_deferred_verify(False)
