@@ -382,6 +382,7 @@ int lzgpu_check_stripes_dev(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_c
  *   - every bad stripe names the same part: that part may be rebuilt whole (lzgpu_convert_chunks or lzgpu_recover_chunks);
  *   - otherwise rebuild stripe by stripe: for each bad stripe s, a one-stripe window of lzgpu_recover_chunks (every part pointer
  *     offset by s * 65536, nb = the blocks of that stripe, min(k, nb - s k)) with the named part as the one wanted.
+ * lzgpu_correct_stripes does the stripe-by-stripe form in one call: check, map, and every stripe with a suspect corrected in place.
  * lzgpu_check_stripe_map returns LZGPU_ERR_CRC when a stored CRC failed, else LZGPU_ERR_INCONSISTENT when any stripe is bad, else
  * LZGPU_OK.  lzgpu_check_stripe_map_dev writes the map to d_map (device memory, 4-byte aligned) on `stream` and returns LZGPU_OK or
  * LZGPU_ERR_CRC, as lzgpu_check_stripes_dev. */
@@ -395,6 +396,49 @@ int lzgpu_check_stripe_map(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_ch
 int lzgpu_check_stripe_map_dev(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, uint32_t nb,
                                const void *const *d_parts, size_t part_stride, const void *const *d_part_crc,
                                void *d_map, int64_t *bad, void *stream);
+
+/* Stripe correction: the stripe map of lzgpu_check_stripe_map, and every stripe that names a suspect part corrected on the device, in
+ * place, in one call.  The bad part is located by the code (error correction), not known in advance as in the erasure rebuild of
+ * lzgpu_recover_chunks / lzgpu_convert_chunks.
+ *   goal, n_chunks, nb, parts, part_stride, part_crc, bad   exactly as in lzgpu_check_stripe_map (layout and zero padding, every data
+ *                                       part required, NULL parity parts not checked, LZGPU_ERR_TOO_FEW_PARTS before anything is
+ *                                       enqueued, 16-byte / 4-byte alignment of the _dev pointers, deferred verification, the
+ *                                       CRC-disabled mode).
+ *   fix[c * pb + s]  (n_chunks * pb entries, every one written, also when a stored CRC failed): bad_rows and suspect_part equal what
+ *                    lzgpu_check_stripe_map returns for the same input before the call; status and crc say what was written.
+ * Rule.  Stripe s of chunk c is corrected only when bad_rows != 0, suspect_part >= 0, and no given block of that stripe other than
+ * the suspect's fails its stored CRC (by the comparison the check makes).  With two checked rows, two parts corrupted by bit rot can
+ * look like a third, single suspect; their failing CRCs block the write (LZGPU_FIX_CRC_CONFLICT).  A suspect block that fails its own
+ * CRC is corrected: the syndromes and the CRC point at the same block.  Two parts of a stripe made stale by one partial write keep
+ * valid CRCs, and with only two checked rows they can still look like a third part, which is then rewritten: a property of the code,
+ * as stated for the map.  An xorN goal (one checked row) never names a suspect, so nothing is ever corrected; that is not an error.
+ * The corrected block is, byte for byte, what lzgpu_recover_chunks rebuilds for suspect_part from a one-stripe window in which that
+ * part is unavailable: from the first k given parts other than the suspect, in ascending index (ECReadPlan::recoverParts).  With a
+ * single faulty part that is the original block.
+ * Only the corrected blocks (in parts, in place) and the fix entries are written; part_crc is not: the caller stores each entry's crc
+ * alongside its block.
+ * lzgpu_correct_stripes returns LZGPU_ERR_CRC when a stored CRC failed (bad[0..2] as the map sets them; the corrections the rule
+ * allowed are still made), else LZGPU_ERR_INCONSISTENT when a stripe is left LZGPU_FIX_UNEXPLAINED, else LZGPU_OK.
+ * lzgpu_correct_stripes_dev writes the fix entries to d_fix (device memory, 4-byte aligned) on `stream` and returns LZGPU_OK or
+ * LZGPU_ERR_CRC, as lzgpu_check_stripe_map_dev; the caller reads d_fix once the stream has passed the call. */
+enum {   /* lzgpu_stripe_fix.status */
+	LZGPU_FIX_CLEAN = 0,        /* the stripe is a codeword; nothing written */
+	LZGPU_FIX_CORRECTED = 1,    /* block `stripe` of part suspect_part was rewritten in place; crc = its new block CRC */
+	LZGPU_FIX_UNEXPLAINED = 2,  /* bad, and no single part explains it (suspect_part == -1); nothing written */
+	LZGPU_FIX_CRC_CONFLICT = 3  /* bad with a suspect, but a given block of the stripe other than the suspect's fails its stored CRC; nothing written */
+};
+typedef struct lzgpu_stripe_fix {
+	uint32_t bad_rows;      /* as lzgpu_stripe_state, before the correction */
+	int32_t suspect_part;   /* as lzgpu_stripe_state, before the correction */
+	int32_t status;         /* LZGPU_FIX_* */
+	uint32_t crc;           /* CORRECTED: mycrc32(0, corrected block, 65536) (LZGPU_FAKE_CRC with CRCs disabled); else 0 */
+} lzgpu_stripe_fix;
+int lzgpu_correct_stripes(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, uint32_t nb,
+                          uint8_t *const *parts, size_t part_stride, const uint32_t *const *part_crc,
+                          lzgpu_stripe_fix *fix, int64_t *bad);
+int lzgpu_correct_stripes_dev(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, uint32_t nb,
+                              void *const *d_parts, size_t part_stride, const void *const *d_part_crc,
+                              void *d_fix, int64_t *bad, void *stream);
 
 /* Wire-format producer (SURVEY.md §8 f3): LIZ_CLTOCS_WRITE_DATA packet prefixes (src/protocol/cltocs.h:116-137) for
  * every block of every part of the encoded chunks, built on the GPU straight from the CRC array of

@@ -78,6 +78,14 @@ class LzStripeState(C.Structure):
     _fields_ = [("bad_rows", C.c_uint32), ("suspect_part", C.c_int32)]
 
 
+class LzStripeFix(C.Structure):
+    _fields_ = [("bad_rows", C.c_uint32), ("suspect_part", C.c_int32), ("status", C.c_int32), ("crc", C.c_uint32)]
+
+
+# lzgpu_stripe_fix.status
+FIX_CLEAN, FIX_CORRECTED, FIX_UNEXPLAINED, FIX_CRC_CONFLICT = range(4)
+
+
 class LzBlockWrite(C.Structure):
     _fields_ = [("block", C.c_uint32), ("offset", C.c_uint32), ("size", C.c_uint32), ("crc", C.c_uint32),
                 ("payload_off", C.c_uint64), ("exists", C.c_uint32), ("status", C.c_int32)]
@@ -121,6 +129,8 @@ SIGNATURES = {
     "lzgpu_check_stripes_dev": (_int, [_vp, _goalp, _u32, _u32, _vp, _sz, _vp, _vp, _vp, _vp]),
     "lzgpu_check_stripe_map": (_int, [_vp, _goalp, _u32, _u32, _vp, _sz, _vp, _vp, _vp]),
     "lzgpu_check_stripe_map_dev": (_int, [_vp, _goalp, _u32, _u32, _vp, _sz, _vp, _vp, _vp, _vp]),
+    "lzgpu_correct_stripes": (_int, [_vp, _goalp, _u32, _u32, _vp, _sz, _vp, _vp, _vp]),
+    "lzgpu_correct_stripes_dev": (_int, [_vp, _goalp, _u32, _u32, _vp, _sz, _vp, _vp, _vp, _vp]),
     "lzgpu_write_data_prefixes": (_int, [_vp, _goalp, _u32, _u32, _vp, _sz, _vp, _u32, _vp]),
     "lzgpu_write_data_prefixes_dev": (_int, [_vp, _goalp, _u32, _u32, _vp, _sz, _vp, _u32, _vp, _vp]),
     "lzgpu_split_chunks": (_int, [_vp, _goalp, _u32, _u32, _vp, _sz, _vp, _sz]),

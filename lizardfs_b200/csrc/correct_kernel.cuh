@@ -1,0 +1,141 @@
+// correct_kernel.cuh — lzgpu_correct_stripes: every stripe of the stripe map that names a suspect part gets that part's block
+// rebuilt in place from k other blocks of the stripe, unless a given block other than the suspect's fails its stored CRC.
+//
+// One CTA (256 threads) per entry that has a suspect, grid-stride over the map; an entry without one only gets its status.  Thread t
+// owns bytes [256t, 256t + 256) of every block of the stripe.  Each given block other than the suspect's is read once (16-byte
+// loads): its CRC for the gate when it has a stored CRC, and its GF product with the suspect's coefficient when it is one of the k
+// inputs (the first k given parts other than the suspect, ascending: the parts ECReadPlan::recoverParts picks when the suspect is
+// unavailable).  The corrected bytes stay in registers until the gate has passed; then they are stored over the suspect's block and
+// their CRC goes into the fix entry.  A CTA owns its stripe's blocks alone and the check pass has finished by stream order, so the
+// in-place stores race with nothing.
+//
+// CRC of a block: thread t folds its 256 bytes with the slicing tables (crc_step_word), shifts the result by the bytes after its
+// segment, x^(8 * 256 (255 - t)) (a multiplier computed once per CTA), and the CTA XOR-reduces: lin(block) = XOR_t lin(seg_t) *
+// x^(8 * |bytes after seg_t|), one crc_mulmod per block and thread instead of the eight levels of cta_crc_tree.
+#pragma once
+#include "kernels_generic.cuh"
+#include "lzgpu.h"
+
+namespace lzd {
+
+struct CorrectArgs {
+	uint8_t *part[64];                 // part i of chunk 0; nullptr = not given
+	const uint32_t *crc[64];           // stored CRCs of part i, [chunk * pb + block]; nullptr = none
+	const uint32_t *map;               // the stripe map, two words per entry (bad_rows, suspect_part)
+	lzgpu_stripe_fix *fix;             // one entry per map entry
+	const uint32_t *tables;            // 4 * 256 slicing tables
+	unsigned long long part_stride, n_entries;
+	unsigned long long given;          // bit i: part i is given
+	unsigned long long xor_row;        // bit i: every coefficient of suspect i's row is 1
+	uint32_t n_parts, k, pb;
+	int crc_disabled;                  // lzgpu_set_crc_enabled(0): stored CRCs are compared with the constant, blocks are not CRCed
+	uint32_t pow2[32];                 // x^(8 * 2^i) mod P
+	uint8_t coef[64][32];              // [suspect][input]: the suspect's block = sum_i coef * input block i
+};
+
+// one block of the stripe, thread t's 256 bytes: CRC (VERIFY) and, as input, acc ^= coef * v (MODE 1: coef 1; MODE 2: any coef)
+template <bool VERIFY, int MODE>
+__device__ __forceinline__ uint32_t correct_read(const uint8_t *blk, uint32_t (&acc)[64], const CoefPlanes &cp, const uint32_t *tab) {
+	uint4 v[16];
+	const uint4 *p = reinterpret_cast<const uint4 *>(blk) + threadIdx.x * 16;
+#pragma unroll
+	for (int i = 0; i < 16; ++i) v[i] = __ldg(p + i);
+	uint32_t st = 0;
+#pragma unroll
+	for (int i = 0; i < 16; ++i) {
+		const uint32_t w[4] = {v[i].x, v[i].y, v[i].z, v[i].w};
+#pragma unroll
+		for (int j = 0; j < 4; ++j) {
+			if constexpr (VERIFY) st = crc_step_word(st, w[j], tab);
+			if constexpr (MODE == 1) acc[4 * i + j] ^= w[j];
+			if constexpr (MODE == 2) acc[4 * i + j] = gf_mac(acc[4 * i + j], w[j], cp);
+		}
+	}
+	return st;
+}
+
+// thread t's CRC state of its segment -> the block's linear CRC, XOR-reduced into s_out[warp] (the caller's barrier publishes it)
+__device__ __forceinline__ void correct_crc_part(uint32_t st, uint32_t shift, uint32_t *s_out) {
+	st = __reduce_xor_sync(0xffffffffu, crc_mulmod(st, shift));
+	if ((threadIdx.x & 31) == 0) s_out[threadIdx.x >> 5] = st;
+}
+
+__global__ void __launch_bounds__(256) correct_map_kernel(const CorrectArgs a) {
+	__shared__ uint32_t s_tab[1024];
+	__shared__ CoefPlanes s_coef[32];
+	__shared__ uint32_t s_lin[64][8];  // per part, per warp: the XOR of the warp's shifted segment CRCs
+	__shared__ uint32_t s_out[8];
+	const unsigned t = threadIdx.x;
+	bool ready = false;
+	uint32_t shift = 0;
+	for (unsigned long long e = blockIdx.x; e < a.n_entries; e += gridDim.x) {
+		const uint32_t bad_rows = a.map[2 * e];
+		const int suspect = static_cast<int>(a.map[2 * e + 1]);
+		if (bad_rows == 0 || suspect < 0) {
+			if (t == 0) a.fix[e] = lzgpu_stripe_fix{bad_rows, suspect, bad_rows ? LZGPU_FIX_UNEXPLAINED : LZGPU_FIX_CLEAN, 0u};
+			continue;
+		}
+		if (!ready) {  // first entry with a suspect: tables and this thread's shift
+			for (unsigned i = t; i < 1024; i += 256) s_tab[i] = a.tables[i];
+			shift = crc_xpow_bytes_dev(256u * (255u - t), a.pow2);
+			ready = true;
+		}
+		if (t < a.k) coef_planes_set(s_coef[t], a.coef[suspect][t]);
+		__syncthreads();
+		const unsigned long long off = (e / a.pb) * a.part_stride + (e % a.pb) * 65536ull;
+		const bool xor_row = (a.xor_row >> suspect) & 1ull;
+		uint32_t acc[64];
+#pragma unroll
+		for (int i = 0; i < 64; ++i) acc[i] = 0;
+		uint32_t used = 0;
+		for (uint32_t p = 0; p < a.n_parts; ++p) {
+			if (!((a.given >> p) & 1ull) || static_cast<int>(p) == suspect) continue;
+			const bool input = used < a.k;
+			const bool verify = a.crc[p] && !a.crc_disabled;
+			const uint8_t *blk = a.part[p] + off;
+			uint32_t st = 0;
+			if (input && xor_row) st = verify ? correct_read<true, 1>(blk, acc, s_coef[0], s_tab) : correct_read<false, 1>(blk, acc, s_coef[0], s_tab);
+			else if (input) st = verify ? correct_read<true, 2>(blk, acc, s_coef[used], s_tab) : correct_read<false, 2>(blk, acc, s_coef[used], s_tab);
+			else if (verify) st = correct_read<true, 0>(blk, acc, s_coef[0], s_tab);
+			if (verify) correct_crc_part(st, shift, s_lin[p]);
+			used += input ? 1u : 0u;
+		}
+		__syncthreads();
+		// the gate: thread p compares part p's stored CRC as the check does (the CRC-disabled mode: with the constant)
+		bool fail = false;
+		if (t < a.n_parts && ((a.given >> t) & 1ull) && static_cast<int>(t) != suspect && a.crc[t]) {
+			const uint32_t stored = a.crc[t][e];  // e = chunk * pb + block
+			if (a.crc_disabled) {
+				fail = stored != LZGPU_FAKE_CRC;
+			} else {
+				uint32_t lin = 0;
+#pragma unroll
+				for (int w = 0; w < 8; ++w) lin ^= s_lin[t][w];
+				fail = (lin ^ kCrcZeroBlock64K) != stored;
+			}
+		}
+		const bool conflict = __syncthreads_or(fail);
+		uint32_t crc = 0;
+		if (!conflict) {
+			uint4 *dst = reinterpret_cast<uint4 *>(a.part[suspect] + off) + t * 16;
+#pragma unroll
+			for (int i = 0; i < 16; ++i) dst[i] = make_uint4(acc[4 * i], acc[4 * i + 1], acc[4 * i + 2], acc[4 * i + 3]);
+			if (a.crc_disabled) {
+				crc = LZGPU_FAKE_CRC;
+			} else {
+				uint32_t st = 0;
+#pragma unroll
+				for (int i = 0; i < 64; ++i) st = crc_step_word(st, acc[i], s_tab);
+				correct_crc_part(st, shift, s_out);
+				__syncthreads();
+				crc = kCrcZeroBlock64K;
+#pragma unroll
+				for (int w = 0; w < 8; ++w) crc ^= s_out[w];
+			}
+		}
+		if (t == 0) a.fix[e] = lzgpu_stripe_fix{bad_rows, suspect, conflict ? LZGPU_FIX_CRC_CONFLICT : LZGPU_FIX_CORRECTED, crc};
+		__syncthreads();  // s_coef, s_lin and s_out are re-used by the next entry
+	}
+}
+
+}  // namespace lzd

@@ -17,6 +17,7 @@
 
 #include "engine_internal.h"
 #include "host_math.h"
+#include "correct_kernel.cuh"
 #include "kernels_generic.cuh"
 #include "lzgpu.h"
 
@@ -1275,6 +1276,193 @@ extern "C" int lzgpu_check_stripe_map(lzgpu_ctx *ctx, const lzgpu_goal *goal, ui
                                       size_t part_stride, const uint32_t *const *part_crc, lzgpu_stripe_state *map, int64_t *bad) {
 	NvtxScope nvtx_scope("lzgpu::check_stripe_map");
 	return check_host(ctx, goal, n_chunks, nb, parts, part_stride, part_crc, map, bad, true);
+}
+
+// ------------------------------------------------------------------------------------------------
+// stripe correction: the stripe map, then every stripe that names a suspect rebuilt in place (correct_kernel.cuh)
+// ------------------------------------------------------------------------------------------------
+static_assert(sizeof(lzgpu_stripe_fix) == 16 && sizeof(lzgpu_stripe_state) == 8, "fix and map entries as the kernels write them");
+
+// The coefficient rows of every part that can be named (given, with k other given parts) for the parts given in `given`: the
+// suspect's block from the first k given parts other than it, the inputs ECReadPlan::recoverParts picks when it is unavailable.
+static int correct_table(const lzgpu_goal *goal, unsigned long long given, CorrectArgs &a) {
+	const int k = goal->k, n = goal->k + goal->m;
+	a.given = given;
+	a.n_parts = n;
+	a.k = k;
+	for (int p = 0; p < n; ++p) {
+		if (!((given >> p) & 1ull)) continue;
+		uint8_t erased[LZGPU_MAX_PARTS] = {0}, wanted[LZGPU_MAX_PARTS] = {0}, row[LZGPU_MAX_DATA];
+		int used = 0;
+		for (int i = 0; i < n; ++i) {
+			if (!((given >> i) & 1ull) || i == p || used >= k) erased[i] = 1;
+			else ++used;
+		}
+		if (used < k) continue;  // never named: a suspect needs two checked rows, so k + 1 other given parts
+		wanted[p] = 1;
+		bool singular = false;
+		if (lz::rs_recovery_matrix(k, goal->m, erased, wanted, row, &singular) != 1) {
+			lz_set_error("correct_stripes: no recovery row for part %d%s", p, singular ? " (singular)" : "");
+			return LZGPU_ERR_ARG;
+		}
+		bool ones = true;
+		for (int j = 0; j < k; ++j) {
+			a.coef[p][j] = row[j];
+			ones &= row[j] == 1;
+		}
+		if (ones) a.xor_row |= 1ull << p;
+	}
+	return LZGPU_OK;
+}
+
+// correct_map_kernel over n_entries map entries (pb per chunk) on `st`; a carries the table (correct_table) and the part pointers
+static int correct_enqueue(lzgpu_ctx *ctx, CorrectArgs &a, unsigned long long n_entries, uint32_t pb, size_t part_stride, const void *d_map,
+                           void *d_fix, cudaStream_t st) {
+	a.map = static_cast<const uint32_t *>(d_map);
+	a.fix = static_cast<lzgpu_stripe_fix *>(d_fix);
+	a.tables = ctx->d_crc_tables;
+	a.part_stride = part_stride;
+	a.n_entries = n_entries;
+	a.pb = pb;
+	a.crc_disabled = lzgpu_crc_enabled() ? 0 : 1;
+	uint32_t x = 0x00800000u;  // x^8
+	for (int i = 0; i < 32; ++i) {
+		a.pow2[i] = x;
+		x = lz::crc_mulmod(x, x);
+	}
+	correct_map_kernel<<<grid_for(ctx, n_entries * 256, 256, 2), 256, 0, st>>>(a);
+	CUDA_TRY(cudaGetLastError());
+	ctx->stats.kernel_launches++;
+	return LZGPU_OK;
+}
+
+extern "C" int lzgpu_correct_stripes_dev(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, uint32_t nb, void *const *d_parts,
+                                         size_t part_stride, const void *const *d_part_crc, void *d_fix, int64_t *bad, void *stream) {
+	NvtxScope nvtx_scope("lzgpu::correct_stripes_dev");
+	int rc = check_args(ctx, goal, nb, d_parts, d_part_crc, d_fix, true);
+	if (rc) return rc;
+	if (n_chunks == 0) return LZGPU_OK;
+	const int n = goal->k + goal->m;
+	const uint32_t pb = (nb + goal->k - 1) / goal->k;
+	const unsigned long long entries = static_cast<unsigned long long>(n_chunks) * pb;
+	CorrectArgs a{};
+	unsigned long long given = 0;
+	for (int i = 0; i < n; ++i) {
+		a.part[i] = static_cast<uint8_t *>(d_parts[i]);
+		a.crc[i] = d_parts[i] && d_part_crc ? static_cast<const uint32_t *>(d_part_crc[i]) : nullptr;
+		given |= d_parts[i] ? 1ull << i : 0ull;
+	}
+	if ((rc = correct_table(goal, given, a))) return rc;  // before anything is enqueued: no host work between check and correction
+	DeviceGuard g(ctx->device);
+	cudaStream_t st = stream ? static_cast<cudaStream_t>(stream) : ctx->stream;
+	VerifyTicket tk;
+	{
+		// the map's bytes and one fix entry per stripe; the corrected blocks are not counted (the host does not know them here)
+		BatchTimer timer(ctx, st, check_alg_bytes(goal, n_chunks, nb, d_parts, d_part_crc, true) + entries * sizeof(lzgpu_stripe_fix));
+		TmpBuf map(ctx, st);  // the map kernels write 8-byte entries; correct_map_kernel copies them into the 16-byte fix entries
+		if ((rc = map.alloc(entries * sizeof(lzgpu_stripe_state)))) return rc;
+		if ((rc = check_enqueue(ctx, goal, n_chunks, nb, d_parts, part_stride, d_part_crc, map.p, st, &tk, true))) return rc;
+		if ((rc = correct_enqueue(ctx, a, entries, pb, part_stride, map.p, d_fix, st))) return rc;
+	}
+	return dev_verdict(ctx, std::move(tk), bad);
+}
+
+// The host-pointer correction, phase 2: the stripes `todo` (map indices with a suspect) gathered into one-stripe "chunks" (pb = 1:
+// the parts are zero-padded, so a short last stripe has the same syndromes), tile by tile, through correct_map_kernel with the map
+// entries the check found; the fix entries go to fix[], the corrected blocks back into the caller's parts.
+static int correct_host_stripes(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t pb, uint8_t *const *parts, size_t part_stride,
+                                const uint32_t *const *part_crc, const lzgpu_stripe_state *map, const std::vector<size_t> &todo,
+                                lzgpu_stripe_fix *fix) {
+	const int n = goal->k + goal->m;
+	const size_t B = LZGPU_BLOCK_SIZE;
+	unsigned long long given = 0;
+	int n_given = 0;
+	for (int i = 0; i < n; ++i)
+		if (parts[i]) {
+			given |= 1ull << i;
+			++n_given;
+		}
+	CorrectArgs a{};
+	int rc = correct_table(goal, given, a);
+	if (rc) return rc;
+	std::lock_guard<std::mutex> lk(ctx->mu);
+	DeviceGuard g(ctx->device);
+	const size_t tile = std::max<size_t>(1, std::min<size_t>(todo.size(), (2 * kHostTileBytes) / (B * n_given)));
+	void *d_in, *d_crc, *d_entries;
+	if ((rc = lz_scratch(ctx, kScratchIn0, tile * B * n, &d_in)) || (rc = lz_scratch(ctx, kScratchCrc0, tile * 4 * n, &d_crc)) ||
+	    (rc = lz_scratch(ctx, kScratchPar0, tile * (sizeof(lzgpu_stripe_state) + sizeof(lzgpu_stripe_fix)), &d_entries)))
+		return rc;
+	void *d_map = d_entries;
+	void *d_fix = static_cast<uint8_t *>(d_entries) + tile * sizeof(lzgpu_stripe_state);
+	for (int i = 0; i < n; ++i) {
+		a.part[i] = parts[i] ? static_cast<uint8_t *>(d_in) + tile * B * i : nullptr;
+		a.crc[i] = parts[i] && part_crc && part_crc[i] ? static_cast<const uint32_t *>(d_crc) + tile * i : nullptr;
+	}
+	std::vector<uint32_t> h_crc(tile * n);
+	std::vector<lzgpu_stripe_state> h_map(tile);
+	std::vector<lzgpu_stripe_fix> h_fix(tile);
+	cudaStream_t st = ctx->slot_stream[0];
+	for (size_t t0 = 0; t0 < todo.size(); t0 += tile) {
+		const size_t nt = std::min(tile, todo.size() - t0);
+		for (size_t j = 0; j < nt; ++j) {
+			const size_t e = todo[t0 + j], c = e / pb, s = e % pb;
+			for (int i = 0; i < n; ++i) {
+				if (!parts[i]) continue;
+				CUDA_TRY(cudaMemcpyAsync(a.part[i] + j * B, parts[i] + c * part_stride + s * B, B, cudaMemcpyHostToDevice, st));
+				if (a.crc[i]) h_crc[tile * i + j] = part_crc[i][e];
+			}
+			h_map[j] = map[e];
+		}
+		ctx->stats.bytes_h2d += nt * n_given * B;
+		CUDA_TRY(cudaMemcpyAsync(d_crc, h_crc.data(), tile * 4 * n, cudaMemcpyHostToDevice, st));
+		CUDA_TRY(cudaMemcpyAsync(d_map, h_map.data(), nt * sizeof(lzgpu_stripe_state), cudaMemcpyHostToDevice, st));
+		{
+			BatchTimer timer(ctx, st, nt * (n_given * B + sizeof(lzgpu_stripe_state) + sizeof(lzgpu_stripe_fix)));
+			if ((rc = correct_enqueue(ctx, a, nt, 1, B, d_map, d_fix, st))) return rc;
+		}
+		CUDA_TRY(cudaMemcpyAsync(h_fix.data(), d_fix, nt * sizeof(lzgpu_stripe_fix), cudaMemcpyDeviceToHost, st));
+		CUDA_TRY(cudaStreamSynchronize(st));
+		for (size_t j = 0; j < nt; ++j) {
+			const size_t e = todo[t0 + j], c = e / pb, s = e % pb;
+			fix[e] = h_fix[j];
+			if (h_fix[j].status != LZGPU_FIX_CORRECTED) continue;
+			const int p = h_fix[j].suspect_part;
+			CUDA_TRY(cudaMemcpyAsync(parts[p] + c * part_stride + s * B, a.part[p] + j * B, B, cudaMemcpyDeviceToHost, st));
+			ctx->stats.bytes_d2h += B;
+		}
+		CUDA_TRY(cudaStreamSynchronize(st));
+	}
+	return LZGPU_OK;
+}
+
+extern "C" int lzgpu_correct_stripes(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, uint32_t nb, uint8_t *const *parts,
+                                     size_t part_stride, const uint32_t *const *part_crc, lzgpu_stripe_fix *fix, int64_t *bad) {
+	NvtxScope nvtx_scope("lzgpu::correct_stripes");
+	if (!fix) return LZGPU_ERR_ARG;
+	// phase 1: the map of the whole batch through the check's tile pipeline (only the map comes back)
+	const uint32_t pb = goal && goal->k > 0 ? (nb + goal->k - 1) / goal->k : 0;
+	std::vector<lzgpu_stripe_state> map(std::max<size_t>(1, static_cast<size_t>(n_chunks) * pb));
+	const int check_rc = check_host(ctx, goal, n_chunks, nb, parts, part_stride, part_crc, map.data(), bad, true);
+	if (check_rc != LZGPU_OK && check_rc != LZGPU_ERR_CRC && check_rc != LZGPU_ERR_INCONSISTENT) return check_rc;
+	if (n_chunks == 0) return LZGPU_OK;
+	std::vector<size_t> todo;
+	for (size_t e = 0; e < static_cast<size_t>(n_chunks) * pb; ++e) {
+		const lzgpu_stripe_state &m = map[e];
+		fix[e] = lzgpu_stripe_fix{m.bad_rows, m.suspect_part, m.bad_rows ? LZGPU_FIX_UNEXPLAINED : LZGPU_FIX_CLEAN, 0u};
+		if (m.bad_rows && m.suspect_part >= 0) todo.push_back(e);
+	}
+	// phase 2: only the stripes with a suspect travel again
+	if (!todo.empty()) {
+		const int rc = correct_host_stripes(ctx, goal, pb, parts, part_stride, part_crc, map.data(), todo, fix);
+		if (rc) return rc;
+	}
+	if (check_rc == LZGPU_ERR_CRC) return check_rc;  // bad[0..2] and the message as the map set them
+	for (size_t e = 0; e < static_cast<size_t>(n_chunks) * pb; ++e)
+		if (fix[e].status == LZGPU_FIX_UNEXPLAINED) {
+			lz_set_error("correct_stripes: chunk %zu stripe %zu is not a codeword and no single part explains it", e / pb, e % pb);
+			return LZGPU_ERR_INCONSISTENT;
+		}
+	return LZGPU_OK;
 }
 
 // ------------------------------------------------------------------------------------------------

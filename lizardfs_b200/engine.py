@@ -585,6 +585,50 @@ class Engine:
             raise ChunkCrcError(rc, "check_stripe_map_dev", (bad[0], bad[1], bad[2]))
         _check(rc, "check_stripe_map_dev")
 
+    STRIPE_FIX_DTYPE = np.dtype([("bad_rows", np.uint32), ("suspect_part", np.int32), ("status", np.int32), ("crc", np.uint32)])
+
+    def correct_stripes(self, goal, nb, parts, part_crc=None):
+        """Check every stripe and correct in place each one that names a suspect part (lzgpu_correct_stripes).  parts and part_crc
+        as in check_stripe_map, but every given part must be a writeable C-contiguous uint8 array: a corrected block is written
+        into it.  part_crc is not changed: the new CRC of a corrected block is in its entry.  Returns a structured array [n_chunks,
+        pb] of STRIPE_FIX_DTYPE (bad_rows and suspect_part as the map had them before the call; status = _lib.FIX_*; crc of the
+        corrected block), whether or not a stripe is left bad; raises ChunkCrcError on a stored-CRC mismatch (its .fix holds the
+        entries, written in full all the same, and the corrections the rule allowed are made)."""
+        assert len(parts) == goal.k + goal.m
+        pb = (nb + goal.k - 1) // goal.k
+        for p in parts:
+            if p is not None and not (isinstance(p, np.ndarray) and p.dtype == np.uint8 and p.flags.c_contiguous and p.flags.writeable):
+                raise ValueError("correct_stripes corrects the parts in place: each must be a writeable C-contiguous uint8 array")
+        parts = [None if p is None else p.reshape(-1, pb * BLOCK_SIZE) for p in parts]
+        n = next(p.shape[0] for p in parts if p is not None)
+        crcs = None
+        if part_crc is not None:
+            crcs = [None if c is None else np.ascontiguousarray(c, dtype=np.uint32) for c in part_crc]
+        fix = np.empty((n, pb), dtype=self.STRIPE_FIX_DTYPE)
+        bad = (C.c_int64 * 3)(-1, -1, -1)
+        rc = self.lib.lzgpu_correct_stripes(self.h, C.byref(goal.c), n, nb, _ptr_array(parts), pb * BLOCK_SIZE,
+                                            _ptr_array(crcs) if crcs is not None else None, _p(fix), bad)
+        if rc == _lib.ERR_CRC:
+            err = ChunkCrcError(rc, "correct_stripes", (bad[0], bad[1], bad[2]))
+            err.fix = fix
+            raise err
+        if rc != _lib.ERR_INCONSISTENT:
+            _check(rc, "correct_stripes")
+        return fix
+
+    def correct_stripes_dev(self, goal, n_chunks, nb, d_parts, part_stride, d_part_crc, d_fix, stream=None):
+        """Device-pointer stripe correction: the corrected blocks are written into d_parts, n_chunks * pb entries of 16 bytes go to
+        d_fix (device memory).  With d_part_crc the call waits for its stream and raises ChunkCrcError on a mismatch; without it
+        the call only enqueues."""
+        n_parts = goal.k + goal.m
+        dp = (C.c_void_p * n_parts)(*[p if p else None for p in d_parts])
+        dc = (C.c_void_p * n_parts)(*[p if p else None for p in d_part_crc]) if d_part_crc is not None else None
+        bad = (C.c_int64 * 3)(-1, -1, -1)
+        rc = self.lib.lzgpu_correct_stripes_dev(self.h, C.byref(goal.c), n_chunks, nb, dp, part_stride, dc, d_fix, bad, stream)
+        if rc == _lib.ERR_CRC:
+            raise ChunkCrcError(rc, "correct_stripes_dev", (bad[0], bad[1], bad[2]))
+        _check(rc, "correct_stripes_dev")
+
     # ---- wire format --------------------------------------------------------------------------
     def write_data_prefixes(self, goal, nb, crc, chunk_ids, write_id_base=0):
         """LIZ_CLTOCS_WRITE_DATA prefixes (cltocs.h:116-137) for every block of every part: uint8 [n, k+m, pb, 38]

@@ -13,6 +13,12 @@ cases: a clean batch, one bad stripe per chunk (data part 3, stripe 5), and ever
 per stripe).  Clean stripes cost the one pass; a bad one is re-read by a CTA of its own to name its suspect.  In every case the maps of
 both routes must be identical and each chunk's lowest bad stripe must equal both routes' verdicts.
 
+The stripe correction (lzgpu_correct_stripes_dev) is timed against the map on the same resident batch in the same three cases, with
+CUDA events around each call only.  A correction repairs the batch, so before every timed call the faulty bytes are put back by device
+copies on the same stream, outside the timed region.  With one bad stripe per chunk the existing route is timed too: the map, the map
+back on the host, then one lzgpu_recover_chunks_dev call per bad stripe over a one-stripe window, writing the suspect's block in place.
+In every case the fix entries of both routes must be identical and the corrected bytes must be the original ones.
+
     python tools/bench_check.py [--chunks 16] [--iters 20] [--warmup 3]      (one JSON line per measurement)
 """
 import argparse
@@ -140,6 +146,102 @@ def map_rows(eng, generic, r, text, args, stream, info):
             flip(eng, r, *fault)         # flipped back: the next case starts from a clean batch
 
 
+def timed_each(call, restore, iters, warmup, stream):
+    """mean time of one call, CUDA events around the call only; restore() runs on `stream` before each call, outside the events"""
+    for _ in range(warmup):
+        restore()
+        call()
+    torch.cuda.synchronize()
+    evs = []
+    for _ in range(iters):
+        restore()
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record(stream)
+        call()
+        e1.record(stream)
+        evs.append((e0, e1))
+    torch.cuda.synchronize()
+    return sum(a.elapsed_time(b) for a, b in evs) / 1e3 / iters
+
+
+def window_repair(eng, r, out_m, stream):
+    """the route before lzgpu_correct_stripes: the map, back on the host, then a one-stripe recover_chunks_dev window per bad stripe"""
+    st = stream.cuda_stream
+    eng.check_stripe_map_dev(r.goal, r.n, NB, r.ptrs, r.stride, r.crc_ptrs, out_m.data_ptr(), stream=st)
+    with torch.cuda.stream(stream):
+        smap = out_m.cpu().numpy().view(L.Engine.STRIPE_STATE_DTYPE).reshape(r.n, r.pb)
+    n = r.k + r.m
+    for c, s in zip(*smap["bad_rows"].nonzero()):
+        p = int(smap[c, s]["suspect_part"])
+        if p < 0:
+            continue
+        off = int(c) * r.stride + int(s) * BLOCK
+        window = [0 if i == p else r.ptrs[i] + off for i in range(n)]
+        d_out = [r.ptrs[p] + off if i == p else 0 for i in range(n)]
+        eng.recover_chunks_dev(r.goal, 1, min(r.k, NB - int(s) * r.k), window, r.stride, None, [int(i == p) for i in range(n)], d_out,
+                               stream=st)
+
+
+def correct_rows(eng, generic, r, text, args, stream, info):
+    """time the correction against the map (and, with one bad stripe per chunk, against map + one-stripe windows); check both routes"""
+    st = stream.cuda_stream
+    out_m = torch.empty(8 * r.n * r.pb, dtype=torch.uint8, device="cuda")
+    out_f = torch.empty(16 * r.n * r.pb, dtype=torch.uint8, device="cuda")
+    cases = [("clean", None), ("one_bad_stripe_per_chunk", (3, [5], 777)), ("every_stripe_bad", (0, range(r.pb), 4242))]
+    for case, fault in cases:
+        idx = good = faulty = None
+        if fault:
+            part, stripes, offset = fault
+            idx = torch.tensor([c * r.stride + part * r.part_bytes + s * BLOCK + offset for c in range(r.n) for s in stripes], device="cuda")
+            good = r.buf[idx].clone()
+            flip(eng, r, *fault)         # the stored CRCs now match the faulty blocks: only the stripe check sees them
+            faulty = r.buf[idx].clone()
+
+        def restore():
+            if idx is not None:
+                with torch.cuda.stream(stream):
+                    r.buf[idx] = faulty
+
+        def correct():
+            eng.correct_stripes_dev(r.goal, r.n, NB, r.ptrs, r.stride, r.crc_ptrs, out_f.data_ptr(), stream=st)
+
+        def smap():
+            eng.check_stripe_map_dev(r.goal, r.n, NB, r.ptrs, r.stride, r.crc_ptrs, out_m.data_ptr(), stream=st)
+
+        t_corr = t_map = t_win = 0.0
+        for _ in range(2):               # alternate the calls, twice: other work shares the card
+            t_corr += timed_each(correct, restore, args.iters, args.warmup, stream) / 2
+            t_map += timed_each(smap, restore, args.iters, args.warmup, stream) / 2
+            if case == "one_bad_stripe_per_chunk":
+                t_win += timed_each(lambda: window_repair(eng, r, out_m, stream), restore, args.iters, args.warmup, stream) / 2
+        eng.sync()
+        fixes = []
+        for e in (eng, generic):
+            restore()
+            torch.cuda.synchronize()
+            e.correct_stripes_dev(r.goal, r.n, NB, r.ptrs, r.stride, r.crc_ptrs, out_f.data_ptr())
+            torch.cuda.synchronize()
+            fixes.append(out_f.cpu().numpy().view(L.Engine.STRIPE_FIX_DTYPE).reshape(r.n, r.pb).copy())
+            if idx is not None and r.m >= 2:
+                assert (r.buf[idx] == good).all(), "a corrected block differs from the original"
+        assert (fixes[0] == fixes[1]).all(), "fused and generic fix entries differ"
+        n_fixed = int((fixes[0]["status"] == _lib.FIX_CORRECTED).sum())
+        n_bad = int((fixes[0]["bad_rows"] != 0).sum())
+        assert n_bad == {"clean": 0, "one_bad_stripe_per_chunk": r.n, "every_stripe_bad": r.n * r.pb}[case]
+        assert n_fixed == (n_bad if r.m >= 2 else 0)
+        row = {"what": "correct_stripes_dev", "goal": text, "case": case, "chunks": r.n, "chunk_mib": NB * BLOCK >> 20, "bad_stripes": n_bad,
+               "corrected": n_fixed, "ms_per_call": round(t_corr * 1e3, 3), "check_stripe_map_ms_per_call": round(t_map * 1e3, 3),
+               "correct_over_map": round(t_corr / t_map, 3)}
+        if t_win:
+            row.update({"map_and_windows_ms": round(t_win * 1e3, 3), "correct_over_map_and_windows": round(t_corr / t_win, 3)})
+        print(json.dumps({**row, "routes_agree": True, **info}), flush=True)
+        if fault:                        # the original bytes and their CRCs: the next case starts from a clean batch
+            r.buf[idx] = good
+            for c in range(r.n):
+                eng.crc_blocks_dev(r.ptrs[fault[0]] + c * r.stride, r.pb, r.crc[fault[0], c].data_ptr())
+            torch.cuda.synchronize()
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--chunks", type=int, default=16)
@@ -201,6 +303,7 @@ def main():
             eng.crc_blocks_dev(r.ptrs[part] + c * r.stride + s * BLOCK, 1, r.crc[part, c, s:].data_ptr())
             torch.cuda.synchronize()
         map_rows(eng, generic, r, text, args, stream, info)
+        correct_rows(eng, generic, r, text, args, stream, info)
         del r, out
         torch.cuda.empty_cache()
     eng.set_deferred_verify(False)
