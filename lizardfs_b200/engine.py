@@ -59,7 +59,95 @@ def _ptr_array(arrs):
     out = (C.c_void_p * len(arrs))()
     for i, a in enumerate(arrs):
         out[i] = None if a is None else a.ctypes.data
+    out._arrays = arrs                  # the pointers stay valid as long as the array of them
     return out
+
+
+def _dev_ptrs(ptrs, n):
+    """C array of n device pointers (ints; 0 or None = absent), None for None"""
+    return None if ptrs is None else (C.c_void_p * n)(*[p if p else None for p in ptrs])
+
+
+def _host_parts(parts, part_crc, pb, in_place=False, crc_rows=False):
+    """The parts of a host-pointer batch call, each None or [n_chunks, pb * 64 KiB] uint8 (in_place: the call writes into them, so
+    each must already be a writeable C-contiguous uint8 array), and their stored CRCs (uint32, crc_rows: [n_chunks, pb] each).
+    Returns (parts, n_chunks, C array of the CRC pointers or None)."""
+    if in_place:
+        for p in parts:
+            if p is not None and not (isinstance(p, np.ndarray) and p.dtype == np.uint8 and p.flags.c_contiguous and p.flags.writeable):
+                raise ValueError("correct_stripes corrects the parts in place: each must be a writeable C-contiguous uint8 array")
+    parts = [None if p is None else (p if in_place else _u8(p)).reshape(-1, pb * BLOCK_SIZE) for p in parts]
+    n = next(p.shape[0] for p in parts if p is not None)
+    if part_crc is None:
+        return parts, n, None
+    crcs = [None if c is None else np.ascontiguousarray(c, dtype=np.uint32) for c in part_crc]
+    if crc_rows:
+        crcs = [None if c is None else c.reshape(n, pb) for c in crcs]
+    return parts, n, _ptr_array(crcs)
+
+
+def _check_crc(rc, where, bad, **result):
+    """Raises ChunkCrcError on a stored-CRC mismatch (.where = bad; `result`, e.g. verdict=..., attached to it) and LzGpuError on
+    any other failure.  A call that returns a `result` may also return ERR_INCONSISTENT: the result says where, it is no failure."""
+    if rc == _lib.ERR_CRC:
+        err = ChunkCrcError(rc, where, tuple(bad))
+        for name, value in result.items():
+            setattr(err, name, value)
+        raise err
+    if not (result and rc == _lib.ERR_INCONSISTENT):
+        _check(rc, where)
+
+
+def _name(fn):
+    return fn.__name__.removeprefix("lzgpu_")
+
+
+# the bodies of the batch calls that Engine and Pool share, `fn` the C function (the context or the pool as its first argument)
+def _encode_chunks(fn, h, goal, data, chunk_len, parity=None, crc=None):
+    data = _u8(data)
+    if data.ndim == 1:
+        data = data.reshape(1, -1)
+    n, stride = data.shape
+    if chunk_len is None:
+        chunk_len = stride
+    nb, pb = Engine.geometry(goal, chunk_len)
+    if parity is None:
+        parity = np.empty((n, goal.m, pb * BLOCK_SIZE), dtype=np.uint8)
+    if crc is None:
+        crc = np.empty((n, nb + goal.m * pb), dtype=np.uint32)
+    _check(fn(h, C.byref(goal.c), n, chunk_len, _p(data), stride, _p(parity), goal.m * pb * BLOCK_SIZE, _p(crc), nb + goal.m * pb), _name(fn))
+    return parity, crc
+
+
+def _recover_chunks(fn, h, goal, nb, parts, part_crc, want, chunk_image):
+    n_parts = goal.k + goal.m
+    assert len(parts) == n_parts
+    pb = (nb + goal.k - 1) // goal.k
+    parts, n, crcs = _host_parts(parts, part_crc, pb)
+    if want is None:
+        want = [1 if (parts[i] is None and i < goal.k) else 0 for i in range(n_parts)]
+    w = np.asarray(want, dtype=np.uint8)
+    out = [np.zeros((n, pb * BLOCK_SIZE), dtype=np.uint8) if (w[i] and parts[i] is None) else None for i in range(n_parts)]
+    img = np.zeros((n, nb * BLOCK_SIZE), dtype=np.uint8) if chunk_image else None
+    bad = (C.c_int64 * 3)(-1, -1, -1)
+    rc = fn(h, C.byref(goal.c), n, nb, _ptr_array(parts), pb * BLOCK_SIZE, crcs, _p(w), _ptr_array(out), _p(img), nb * BLOCK_SIZE, bad)
+    _check_crc(rc, _name(fn), bad)
+    return out, img
+
+
+def _convert_chunks(fn, h, src, dst, nb, parts, want, part_crc, with_crc):
+    ns, nd = src.k + src.m, dst.k + dst.m
+    pbs, pbd = -(-nb // src.k), -(-nb // dst.k)
+    arrs, n, crcs = _host_parts(parts, part_crc, pbs, crc_rows=True)
+    w = np.asarray(want, dtype=np.uint8)
+    assert len(arrs) == ns and w.size == nd
+    out = [np.zeros((n, pbd * BLOCK_SIZE), dtype=np.uint8) if w[i] else None for i in range(nd)]
+    ocrc = [np.zeros((n, pbd), dtype=np.uint32) if (w[i] and with_crc) else None for i in range(nd)]
+    bad = (C.c_int64 * 3)(-1, -1, -1)
+    rc = fn(h, C.byref(src.c), C.byref(dst.c), n, nb, _ptr_array(arrs), pbs * BLOCK_SIZE, crcs, _p(w), _ptr_array(out), pbd * BLOCK_SIZE,
+            _ptr_array(ocrc) if with_crc else None, bad)
+    _check_crc(rc, _name(fn), bad)
+    return out, ocrc
 
 
 # ------------------------------------------------------------------------------------------------
@@ -251,64 +339,14 @@ class Pool:
         return {f[0]: getattr(s, f[0]) for f in LzStats._fields_}
 
     def encode_chunks(self, goal, data, chunk_len=None, parity=None, crc=None):
-        data = _u8(data)
-        if data.ndim == 1:
-            data = data.reshape(1, -1)
-        n, stride = data.shape
-        if chunk_len is None:
-            chunk_len = stride
-        nb, pb = Engine.geometry(goal, chunk_len)
-        if parity is None:
-            parity = np.empty((n, goal.m, pb * BLOCK_SIZE), dtype=np.uint8)
-        if crc is None:
-            crc = np.empty((n, nb + goal.m * pb), dtype=np.uint32)
-        _check(self.lib.lzgpu_pool_encode_chunks(self.h, C.byref(goal.c), n, chunk_len, _p(data), stride, _p(parity),
-                                                 goal.m * pb * BLOCK_SIZE, _p(crc), nb + goal.m * pb), "pool_encode_chunks")
-        return parity, crc
+        return _encode_chunks(self.lib.lzgpu_pool_encode_chunks, self.h, goal, data, chunk_len, parity, crc)
 
     def recover_chunks(self, goal, nb, parts, part_crc=None, want=None, chunk_image=False):
-        n_parts = goal.k + goal.m
-        pb = (nb + goal.k - 1) // goal.k
-        parts = [None if p is None else _u8(p).reshape(-1, pb * BLOCK_SIZE) for p in parts]
-        n = next(p.shape[0] for p in parts if p is not None)
-        if want is None:
-            want = [1 if (parts[i] is None and i < goal.k) else 0 for i in range(n_parts)]
-        w = np.asarray(want, dtype=np.uint8)
-        out = [np.zeros((n, pb * BLOCK_SIZE), dtype=np.uint8) if (w[i] and parts[i] is None) else None for i in range(n_parts)]
-        crcs = None
-        if part_crc is not None:
-            crcs = [None if c is None else np.ascontiguousarray(c, dtype=np.uint32) for c in part_crc]
-        img = np.zeros((n, nb * BLOCK_SIZE), dtype=np.uint8) if chunk_image else None
-        bad = (C.c_int64 * 3)(-1, -1, -1)
-        rc = self.lib.lzgpu_pool_recover_chunks(self.h, C.byref(goal.c), n, nb, _ptr_array(parts), pb * BLOCK_SIZE,
-                                                _ptr_array(crcs) if crcs is not None else None, _p(w), _ptr_array(out),
-                                                _p(img), nb * BLOCK_SIZE, bad)
-        if rc == _lib.ERR_CRC:
-            raise ChunkCrcError(rc, "pool_recover_chunks", (bad[0], bad[1], bad[2]))
-        _check(rc, "pool_recover_chunks")
-        return out, img
+        return _recover_chunks(self.lib.lzgpu_pool_recover_chunks, self.h, goal, nb, parts, part_crc, want, chunk_image)
 
     def convert_chunks(self, src, dst, nb, parts, want, part_crc=None, with_crc=True):
         """Engine.convert_chunks over every device of the pool (lzgpu_pool_convert_chunks)"""
-        ns, nd = src.k + src.m, dst.k + dst.m
-        pbs, pbd = -(-nb // src.k), -(-nb // dst.k)
-        arrs = [None if p is None else _u8(p).reshape(-1, pbs * BLOCK_SIZE) for p in parts]
-        n = next(a.shape[0] for a in arrs if a is not None)
-        crcs = None
-        if part_crc is not None:
-            crcs = [None if c is None else np.ascontiguousarray(c, dtype=np.uint32).reshape(n, pbs) for c in part_crc]
-        w = np.asarray(want, dtype=np.uint8)
-        assert len(arrs) == ns and w.size == nd
-        out = [np.zeros((n, pbd * BLOCK_SIZE), dtype=np.uint8) if w[i] else None for i in range(nd)]
-        ocrc = [np.zeros((n, pbd), dtype=np.uint32) if (w[i] and with_crc) else None for i in range(nd)]
-        bad = (C.c_int64 * 3)(-1, -1, -1)
-        rc = self.lib.lzgpu_pool_convert_chunks(self.h, C.byref(src.c), C.byref(dst.c), n, nb, _ptr_array(arrs), pbs * BLOCK_SIZE,
-                                                _ptr_array(crcs) if crcs is not None else None, _p(w), _ptr_array(out), pbd * BLOCK_SIZE,
-                                                _ptr_array(ocrc) if with_crc else None, bad)
-        if rc == _lib.ERR_CRC:
-            raise ChunkCrcError(rc, "pool_convert_chunks", tuple(bad))
-        _check(rc, "pool_convert_chunks")
-        return out, ocrc
+        return _convert_chunks(self.lib.lzgpu_pool_convert_chunks, self.h, src, dst, nb, parts, want, part_crc, with_crc)
 
     def crc_blocks(self, data, block_len=BLOCK_SIZE):
         data = _u8(data).reshape(-1, block_len)
@@ -427,7 +465,7 @@ class Engine:
         if rc == _lib.ERR_CRC:
             bad = (C.c_int64 * 3)(-1, -1, -1)
             self.lib.lzgpu_last_bad(self.h, bad)
-            raise ChunkCrcError(rc, "dev_sync (deferred verification)", (bad[0], bad[1], bad[2]))
+            _check_crc(rc, "dev_sync (deferred verification)", bad)
         _check(rc, "dev_sync")
 
     def set_deferred_verify(self, enabled):
@@ -443,18 +481,7 @@ class Engine:
     # ---- encode ------------------------------------------------------------------------------
     def encode_chunks(self, goal, data, chunk_len=None):
         """data: uint8 array [n_chunks, stride] (chunk order). Returns (parity [n, m, pb*64K], crc [n, nb+m*pb])."""
-        data = _u8(data)
-        if data.ndim == 1:
-            data = data.reshape(1, -1)
-        n, stride = data.shape
-        if chunk_len is None:
-            chunk_len = stride
-        nb, pb = self.geometry(goal, chunk_len)
-        parity = np.empty((n, goal.m, pb * BLOCK_SIZE), dtype=np.uint8)
-        crc = np.empty((n, nb + goal.m * pb), dtype=np.uint32)
-        _check(self.lib.lzgpu_encode_chunks(self.h, C.byref(goal.c), n, chunk_len, _p(data), stride, _p(parity),
-                                            goal.m * pb * BLOCK_SIZE, _p(crc), nb + goal.m * pb), "encode_chunks")
-        return parity, crc
+        return _encode_chunks(self.lib.lzgpu_encode_chunks, self.h, goal, data, chunk_len)
 
     def encode_chunks_dev(self, goal, n_chunks, chunk_len, d_data, chunk_stride, d_parity, parity_stride, d_crc, crc_stride, stream=None):
         _check(self.lib.lzgpu_encode_chunks_dev(self.h, C.byref(goal.c), n_chunks, chunk_len, d_data, chunk_stride, d_parity,
@@ -466,27 +493,7 @@ class Engine:
         part_crc: optional list of arrays [n_chunks, pb] (uint32) or None per part.
         want: flags of requested parts (default: every unavailable data part).
         Returns (out_list, chunk_out or None); raises ChunkCrcError on a stored-CRC mismatch."""
-        n_parts = goal.k + goal.m
-        assert len(parts) == n_parts
-        pb = (nb + goal.k - 1) // goal.k
-        parts = [None if p is None else _u8(p).reshape(-1, pb * BLOCK_SIZE) for p in parts]
-        n = next(p.shape[0] for p in parts if p is not None)
-        if want is None:
-            want = [1 if (parts[i] is None and i < goal.k) else 0 for i in range(n_parts)]
-        w = np.asarray(want, dtype=np.uint8)
-        out = [np.zeros((n, pb * BLOCK_SIZE), dtype=np.uint8) if (w[i] and parts[i] is None) else None for i in range(n_parts)]
-        crcs = None
-        if part_crc is not None:
-            crcs = [None if c is None else np.ascontiguousarray(c, dtype=np.uint32) for c in part_crc]
-        img = np.zeros((n, nb * BLOCK_SIZE), dtype=np.uint8) if chunk_image else None
-        bad = (C.c_int64 * 3)(-1, -1, -1)
-        rc = self.lib.lzgpu_recover_chunks(self.h, C.byref(goal.c), n, nb, _ptr_array(parts), pb * BLOCK_SIZE,
-                                           _ptr_array(crcs) if crcs is not None else None, _p(w), _ptr_array(out),
-                                           _p(img), nb * BLOCK_SIZE, bad)
-        if rc == _lib.ERR_CRC:
-            raise ChunkCrcError(rc, "recover_chunks", (bad[0], bad[1], bad[2]))
-        _check(rc, "recover_chunks")
-        return out, img
+        return _recover_chunks(self.lib.lzgpu_recover_chunks, self.h, goal, nb, parts, part_crc, want, chunk_image)
 
     def recover_chunks_dev(self, goal, n_chunks, nb, d_parts, part_stride, d_part_crc, want, d_out, d_chunk_out=None,
                            chunk_out_stride=None, stream=None):
@@ -496,16 +503,32 @@ class Engine:
         if d_chunk_out and chunk_out_stride is None:
             raise ValueError("recover_chunks_dev: chunk_out_stride is required with d_chunk_out")
         chunk_out_stride = chunk_out_stride or 0
-        dp = (C.c_void_p * n_parts)(*[p if p else None for p in d_parts])
-        dc = (C.c_void_p * n_parts)(*[p if p else None for p in d_part_crc]) if d_part_crc is not None else None
-        do = (C.c_void_p * n_parts)(*[p if p else None for p in d_out])
         w = np.asarray(want, dtype=np.uint8)
         bad = (C.c_int64 * 3)(-1, -1, -1)
-        rc = self.lib.lzgpu_recover_chunks_dev(self.h, C.byref(goal.c), n_chunks, nb, dp, part_stride, dc, _p(w), do, d_chunk_out,
+        rc = self.lib.lzgpu_recover_chunks_dev(self.h, C.byref(goal.c), n_chunks, nb, _dev_ptrs(d_parts, n_parts), part_stride,
+                                               _dev_ptrs(d_part_crc, n_parts), _p(w), _dev_ptrs(d_out, n_parts), d_chunk_out,
                                                chunk_out_stride, bad, stream)
-        if rc == _lib.ERR_CRC:
-            raise ChunkCrcError(rc, "recover_chunks_dev", (bad[0], bad[1], bad[2]))
-        _check(rc, "recover_chunks_dev")
+        _check_crc(rc, "recover_chunks_dev", bad)
+
+    def _part_batch_dev(self, fn, goal, n_chunks, nb, d_parts, part_stride, d_part_crc, d_result, stream):
+        # the device-pointer check, map and correction: the same arguments, the result (verdicts, map or fix entries) on the device
+        n_parts = goal.k + goal.m
+        bad = (C.c_int64 * 3)(-1, -1, -1)
+        rc = fn(self.h, C.byref(goal.c), n_chunks, nb, _dev_ptrs(d_parts, n_parts), part_stride, _dev_ptrs(d_part_crc, n_parts), d_result,
+                bad, stream)
+        _check_crc(rc, _name(fn), bad)
+
+    def _part_batch(self, fn, goal, nb, parts, part_crc, result, attr, in_place=False):
+        # the host-pointer check, map and correction: result(n_chunks, pb) makes the array the call fills, which is returned, and
+        # attached to a ChunkCrcError as `attr`
+        assert len(parts) == goal.k + goal.m
+        pb = (nb + goal.k - 1) // goal.k
+        parts, n, crcs = _host_parts(parts, part_crc, pb, in_place=in_place)
+        out = result(n, pb)
+        bad = (C.c_int64 * 3)(-1, -1, -1)
+        rc = fn(self.h, C.byref(goal.c), n, nb, _ptr_array(parts), pb * BLOCK_SIZE, crcs, _p(out), bad)
+        _check_crc(rc, _name(fn), bad, **{attr: out})
+        return out
 
     # ---- stripe check ------------------------------------------------------------------------
     VERDICT_DTYPE = np.dtype([("first_bad_stripe", np.int32), ("bad_rows", np.uint32), ("suspect_part", np.int32)])
@@ -516,36 +539,13 @@ class Engine:
         Returns the verdicts, a structured array [n_chunks] of VERDICT_DTYPE (first_bad_stripe, bad_rows, suspect_part; -1 = none),
         whether or not any chunk is inconsistent; raises ChunkCrcError on a stored-CRC mismatch (its .verdict holds the verdicts,
         which are written for every chunk all the same)."""
-        assert len(parts) == goal.k + goal.m
-        pb = (nb + goal.k - 1) // goal.k
-        parts = [None if p is None else _u8(p).reshape(-1, pb * BLOCK_SIZE) for p in parts]
-        n = next(p.shape[0] for p in parts if p is not None)
-        crcs = None
-        if part_crc is not None:
-            crcs = [None if c is None else np.ascontiguousarray(c, dtype=np.uint32) for c in part_crc]
-        verdict = np.empty(n, dtype=self.VERDICT_DTYPE)
-        bad = (C.c_int64 * 3)(-1, -1, -1)
-        rc = self.lib.lzgpu_check_stripes(self.h, C.byref(goal.c), n, nb, _ptr_array(parts), pb * BLOCK_SIZE,
-                                          _ptr_array(crcs) if crcs is not None else None, _p(verdict), bad)
-        if rc == _lib.ERR_CRC:
-            err = ChunkCrcError(rc, "check_stripes", (bad[0], bad[1], bad[2]))
-            err.verdict = verdict
-            raise err
-        if rc != _lib.ERR_INCONSISTENT:
-            _check(rc, "check_stripes")
-        return verdict
+        return self._part_batch(self.lib.lzgpu_check_stripes, goal, nb, parts, part_crc,
+                                lambda n, pb: np.empty(n, dtype=self.VERDICT_DTYPE), "verdict")
 
     def check_stripes_dev(self, goal, n_chunks, nb, d_parts, part_stride, d_part_crc, d_verdict, stream=None):
         """Device-pointer stripe check: the verdicts go to d_verdict (n_chunks x 12 bytes, device memory).  With d_part_crc the
         call waits for its stream and raises ChunkCrcError on a mismatch; without it the call only enqueues."""
-        n_parts = goal.k + goal.m
-        dp = (C.c_void_p * n_parts)(*[p if p else None for p in d_parts])
-        dc = (C.c_void_p * n_parts)(*[p if p else None for p in d_part_crc]) if d_part_crc is not None else None
-        bad = (C.c_int64 * 3)(-1, -1, -1)
-        rc = self.lib.lzgpu_check_stripes_dev(self.h, C.byref(goal.c), n_chunks, nb, dp, part_stride, dc, d_verdict, bad, stream)
-        if rc == _lib.ERR_CRC:
-            raise ChunkCrcError(rc, "check_stripes_dev", (bad[0], bad[1], bad[2]))
-        _check(rc, "check_stripes_dev")
+        self._part_batch_dev(self.lib.lzgpu_check_stripes_dev, goal, n_chunks, nb, d_parts, part_stride, d_part_crc, d_verdict, stream)
 
     STRIPE_STATE_DTYPE = np.dtype([("bad_rows", np.uint32), ("suspect_part", np.int32)])
 
@@ -554,36 +554,13 @@ class Engine:
         structured array [n_chunks, pb] of STRIPE_STATE_DTYPE (bad_rows, 0 = a codeword; suspect_part, -1 = none), whether or not
         any stripe is bad; raises ChunkCrcError on a stored-CRC mismatch (its .map holds the map, written in full all the same).
         For each chunk the lowest bad stripe and its entry equal check_stripes' verdict."""
-        assert len(parts) == goal.k + goal.m
-        pb = (nb + goal.k - 1) // goal.k
-        parts = [None if p is None else _u8(p).reshape(-1, pb * BLOCK_SIZE) for p in parts]
-        n = next(p.shape[0] for p in parts if p is not None)
-        crcs = None
-        if part_crc is not None:
-            crcs = [None if c is None else np.ascontiguousarray(c, dtype=np.uint32) for c in part_crc]
-        smap = np.empty((n, pb), dtype=self.STRIPE_STATE_DTYPE)
-        bad = (C.c_int64 * 3)(-1, -1, -1)
-        rc = self.lib.lzgpu_check_stripe_map(self.h, C.byref(goal.c), n, nb, _ptr_array(parts), pb * BLOCK_SIZE,
-                                             _ptr_array(crcs) if crcs is not None else None, _p(smap), bad)
-        if rc == _lib.ERR_CRC:
-            err = ChunkCrcError(rc, "check_stripe_map", (bad[0], bad[1], bad[2]))
-            err.map = smap
-            raise err
-        if rc != _lib.ERR_INCONSISTENT:
-            _check(rc, "check_stripe_map")
-        return smap
+        return self._part_batch(self.lib.lzgpu_check_stripe_map, goal, nb, parts, part_crc,
+                                lambda n, pb: np.empty((n, pb), dtype=self.STRIPE_STATE_DTYPE), "map")
 
     def check_stripe_map_dev(self, goal, n_chunks, nb, d_parts, part_stride, d_part_crc, d_map, stream=None):
         """Device-pointer stripe map: n_chunks * pb entries of 8 bytes go to d_map (device memory).  With d_part_crc the call waits
         for its stream and raises ChunkCrcError on a mismatch; without it the call only enqueues."""
-        n_parts = goal.k + goal.m
-        dp = (C.c_void_p * n_parts)(*[p if p else None for p in d_parts])
-        dc = (C.c_void_p * n_parts)(*[p if p else None for p in d_part_crc]) if d_part_crc is not None else None
-        bad = (C.c_int64 * 3)(-1, -1, -1)
-        rc = self.lib.lzgpu_check_stripe_map_dev(self.h, C.byref(goal.c), n_chunks, nb, dp, part_stride, dc, d_map, bad, stream)
-        if rc == _lib.ERR_CRC:
-            raise ChunkCrcError(rc, "check_stripe_map_dev", (bad[0], bad[1], bad[2]))
-        _check(rc, "check_stripe_map_dev")
+        self._part_batch_dev(self.lib.lzgpu_check_stripe_map_dev, goal, n_chunks, nb, d_parts, part_stride, d_part_crc, d_map, stream)
 
     STRIPE_FIX_DTYPE = np.dtype([("bad_rows", np.uint32), ("suspect_part", np.int32), ("status", np.int32), ("crc", np.uint32)])
 
@@ -594,40 +571,14 @@ class Engine:
         pb] of STRIPE_FIX_DTYPE (bad_rows and suspect_part as the map had them before the call; status = _lib.FIX_*; crc of the
         corrected block), whether or not a stripe is left bad; raises ChunkCrcError on a stored-CRC mismatch (its .fix holds the
         entries, written in full all the same, and the corrections the rule allowed are made)."""
-        assert len(parts) == goal.k + goal.m
-        pb = (nb + goal.k - 1) // goal.k
-        for p in parts:
-            if p is not None and not (isinstance(p, np.ndarray) and p.dtype == np.uint8 and p.flags.c_contiguous and p.flags.writeable):
-                raise ValueError("correct_stripes corrects the parts in place: each must be a writeable C-contiguous uint8 array")
-        parts = [None if p is None else p.reshape(-1, pb * BLOCK_SIZE) for p in parts]
-        n = next(p.shape[0] for p in parts if p is not None)
-        crcs = None
-        if part_crc is not None:
-            crcs = [None if c is None else np.ascontiguousarray(c, dtype=np.uint32) for c in part_crc]
-        fix = np.empty((n, pb), dtype=self.STRIPE_FIX_DTYPE)
-        bad = (C.c_int64 * 3)(-1, -1, -1)
-        rc = self.lib.lzgpu_correct_stripes(self.h, C.byref(goal.c), n, nb, _ptr_array(parts), pb * BLOCK_SIZE,
-                                            _ptr_array(crcs) if crcs is not None else None, _p(fix), bad)
-        if rc == _lib.ERR_CRC:
-            err = ChunkCrcError(rc, "correct_stripes", (bad[0], bad[1], bad[2]))
-            err.fix = fix
-            raise err
-        if rc != _lib.ERR_INCONSISTENT:
-            _check(rc, "correct_stripes")
-        return fix
+        return self._part_batch(self.lib.lzgpu_correct_stripes, goal, nb, parts, part_crc,
+                                lambda n, pb: np.empty((n, pb), dtype=self.STRIPE_FIX_DTYPE), "fix", in_place=True)
 
     def correct_stripes_dev(self, goal, n_chunks, nb, d_parts, part_stride, d_part_crc, d_fix, stream=None):
         """Device-pointer stripe correction: the corrected blocks are written into d_parts, n_chunks * pb entries of 16 bytes go to
         d_fix (device memory).  With d_part_crc the call waits for its stream and raises ChunkCrcError on a mismatch; without it
         the call only enqueues."""
-        n_parts = goal.k + goal.m
-        dp = (C.c_void_p * n_parts)(*[p if p else None for p in d_parts])
-        dc = (C.c_void_p * n_parts)(*[p if p else None for p in d_part_crc]) if d_part_crc is not None else None
-        bad = (C.c_int64 * 3)(-1, -1, -1)
-        rc = self.lib.lzgpu_correct_stripes_dev(self.h, C.byref(goal.c), n_chunks, nb, dp, part_stride, dc, d_fix, bad, stream)
-        if rc == _lib.ERR_CRC:
-            raise ChunkCrcError(rc, "correct_stripes_dev", (bad[0], bad[1], bad[2]))
-        _check(rc, "correct_stripes_dev")
+        self._part_batch_dev(self.lib.lzgpu_correct_stripes_dev, goal, n_chunks, nb, d_parts, part_stride, d_part_crc, d_fix, stream)
 
     # ---- wire format --------------------------------------------------------------------------
     def write_data_prefixes(self, goal, nb, crc, chunk_ids, write_id_base=0):
@@ -664,8 +615,8 @@ class Engine:
         return parts
 
     def split_chunks_dev(self, goal, n_chunks, nb, d_data, chunk_stride, d_parts, part_stride, stream=None):
-        dp = (C.c_void_p * goal.k)(*[p if p else None for p in d_parts])
-        _check(self.lib.lzgpu_split_chunks_dev(self.h, C.byref(goal.c), n_chunks, nb, d_data, chunk_stride, dp, part_stride, stream), "split_chunks_dev")
+        _check(self.lib.lzgpu_split_chunks_dev(self.h, C.byref(goal.c), n_chunks, nb, d_data, chunk_stride, _dev_ptrs(d_parts, goal.k), part_stride,
+                                               stream), "split_chunks_dev")
 
     def plan_encode(self, goal, n_chunks, nb, chunk_stride=None, striped_policy=-1):
         """how encode_chunks_dev would lay the batch out (pure host logic, csrc/fused_plan.h): dict with fused, mode
@@ -711,39 +662,16 @@ class Engine:
         """Rebuild the `want`ed parts of slice type `dst` from the available `parts` of slice type `src`
         (SliceRecoveryPlanner, slice_recovery_planner.h:87-204).  parts[i]: (n_chunks, pb_src*65536) uint8 or None.
         Returns (out, out_crc): lists indexed by destination part (None where not wanted)."""
-        ns, nd = src.k + src.m, dst.k + dst.m
-        pbs, pbd = -(-nb // src.k), -(-nb // dst.k)
-        arrs = [None if p is None else _u8(p).reshape(-1, pbs * BLOCK_SIZE) for p in parts]
-        n = next(a.shape[0] for a in arrs if a is not None)
-        crcs = None
-        if part_crc is not None:
-            crcs = [None if c is None else np.ascontiguousarray(c, dtype=np.uint32).reshape(n, pbs) for c in part_crc]
-        w = np.asarray(want, dtype=np.uint8)
-        assert len(arrs) == ns and w.size == nd
-        out = [np.zeros((n, pbd * BLOCK_SIZE), dtype=np.uint8) if w[i] else None for i in range(nd)]
-        ocrc = [np.zeros((n, pbd), dtype=np.uint32) if (w[i] and with_crc) else None for i in range(nd)]
-        bad = (C.c_int64 * 3)(-1, -1, -1)
-        rc = self.lib.lzgpu_convert_chunks(self.h, C.byref(src.c), C.byref(dst.c), n, nb, _ptr_array(arrs), pbs * BLOCK_SIZE,
-                                           _ptr_array(crcs) if crcs is not None else None, _p(w), _ptr_array(out), pbd * BLOCK_SIZE,
-                                           _ptr_array(ocrc) if with_crc else None, bad)
-        if rc == _lib.ERR_CRC:
-            raise ChunkCrcError(rc, "convert_chunks", tuple(bad))
-        _check(rc, "convert_chunks")
-        return out, ocrc
+        return _convert_chunks(self.lib.lzgpu_convert_chunks, self.h, src, dst, nb, parts, want, part_crc, with_crc)
 
     def convert_chunks_dev(self, src, dst, n_chunks, nb, d_parts, part_stride, want, d_out, out_stride, d_part_crc=None, d_out_crc=None, stream=None):
         ns, nd = src.k + src.m, dst.k + dst.m
-        dp = (C.c_void_p * ns)(*[p if p else None for p in d_parts])
-        dc = (C.c_void_p * ns)(*[p if p else None for p in d_part_crc]) if d_part_crc is not None else None
-        do = (C.c_void_p * nd)(*[p if p else None for p in d_out])
-        doc = (C.c_void_p * nd)(*[p if p else None for p in d_out_crc]) if d_out_crc is not None else None
         w = np.asarray(want, dtype=np.uint8)
         bad = (C.c_int64 * 3)(-1, -1, -1)
-        rc = self.lib.lzgpu_convert_chunks_dev(self.h, C.byref(src.c), C.byref(dst.c), n_chunks, nb, dp, part_stride, dc, _p(w), do, out_stride,
-                                               doc, bad, stream)
-        if rc == _lib.ERR_CRC:
-            raise ChunkCrcError(rc, "convert_chunks_dev", (bad[0], bad[1], bad[2]))
-        _check(rc, "convert_chunks_dev")
+        rc = self.lib.lzgpu_convert_chunks_dev(self.h, C.byref(src.c), C.byref(dst.c), n_chunks, nb, _dev_ptrs(d_parts, ns), part_stride,
+                                               _dev_ptrs(d_part_crc, ns), _p(w), _dev_ptrs(d_out, nd), out_stride, _dev_ptrs(d_out_crc, nd),
+                                               bad, stream)
+        _check_crc(rc, "convert_chunks_dev", bad)
 
     # ---- CRC ---------------------------------------------------------------------------------
     def crc_blocks(self, data, block_len=BLOCK_SIZE, block_stride=None):
@@ -763,9 +691,7 @@ class Engine:
         stored = np.ascontiguousarray(stored_crc, dtype=np.uint32)
         bad = C.c_int64(-1)
         rc = self.lib.lzgpu_verify_blocks(self.h, _p(data), stored.size, block_len, block_len, _p(stored), int(sparse_rule), C.byref(bad))
-        if rc == _lib.ERR_CRC:
-            raise ChunkCrcError(rc, "verify_blocks", (bad.value,))
-        _check(rc, "verify_blocks")
+        _check_crc(rc, "verify_blocks", (bad.value,))
 
     def verify_interleaved(self, records):
         """records: on-disk layout, n x (4-byte big-endian CRC + 65536 data bytes) (chunk.h:40)."""
@@ -773,17 +699,13 @@ class Engine:
         n = records.size // (4 + BLOCK_SIZE)
         bad = C.c_int64(-1)
         rc = self.lib.lzgpu_verify_interleaved(self.h, _p(records), n, C.byref(bad))
-        if rc == _lib.ERR_CRC:
-            raise ChunkCrcError(rc, "verify_interleaved", (bad.value,))
-        _check(rc, "verify_interleaved")
+        _check_crc(rc, "verify_interleaved", (bad.value,))
 
     def verify_interleaved_ptr(self, ptr, n_blocks):
         """same, `ptr` = raw address of the records: host memory or a device buffer of this engine's device"""
         bad = C.c_int64(-1)
         rc = self.lib.lzgpu_verify_interleaved(self.h, ptr, n_blocks, C.byref(bad))
-        if rc == _lib.ERR_CRC:
-            raise ChunkCrcError(rc, "verify_interleaved", (bad.value,))
-        _check(rc, "verify_interleaved")
+        _check_crc(rc, "verify_interleaved", (bad.value,))
 
     def moosefs_header_size(self, data_parts=1):
         return int(self.lib.lzgpu_moosefs_header_size(data_parts))
@@ -793,9 +715,7 @@ class Engine:
         img = _u8(file_image).reshape(-1)
         bad = C.c_int64(-1)
         rc = self.lib.lzgpu_verify_moosefs(self.h, data_parts, _p(img), n_blocks, C.byref(bad))
-        if rc == _lib.ERR_CRC:
-            raise ChunkCrcError(rc, "verify_moosefs", (bad.value,))
-        _check(rc, "verify_moosefs")
+        _check_crc(rc, "verify_moosefs", (bad.value,))
 
     # ---- chunkserver block writes ----------------------------------------------------------------
     def write_blocks(self, blocks, stored_crc, writes, sparse_rule=True):
