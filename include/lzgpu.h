@@ -163,6 +163,25 @@ typedef struct lzgpu_recover_plan {
 int lzgpu_plan_recover(const lzgpu_goal *goal, const uint8_t *available, const uint8_t *want, int verify, int image,
                        const lzgpu_recover_switches *switches, lzgpu_recover_plan *out);
 
+/* How lzgpu_check_stripes / lzgpu_check_stripe_map / lzgpu_correct_stripes will check a batch (pure host logic, no GPU needed):
+ * the launch of fused_check_kernel (fused_check_map_kernel for the map), or the generic route.  given[i] (k+m flags): part i is
+ * given.  rows and consecutive describe the checked parity rows whatever the route; the fields after them only a fused plan.
+ * fused = 0: a Cauchy generator or no geometry fits (the generic route: parity rows recomputed in passes of four, then compared).
+ * Returns LZGPU_ERR_TOO_FEW_PARTS, as the calls do, when a data part or every parity part is missing.  A context with
+ * LZGPU_DISABLE_FUSED=1 always takes the generic route, and a call whose stride is not a multiple of 16 does too; neither is part
+ * of the plan. */
+typedef struct lzgpu_check_plan {
+	int fused;             /* 1: one fused_check_kernel launch; 0: the generic route */
+	uint32_t rows;         /* R: checked parity rows (given parity parts) */
+	int consecutive;       /* 1: they are rows 0 .. R-1 (the kernel's compile-time rows); 0: read per call */
+	uint32_t G;            /* stripes per work unit (fused only, as every field below) */
+	uint32_t stages;       /* depth of the stage ring */
+	uint32_t threads;      /* threads per CTA */
+	uint32_t item_passes;  /* passes of the CTA over the 32 G GF items of a step: ceil(32 G / threads) */
+	uint32_t smem_bytes;   /* dynamic shared memory per CTA */
+} lzgpu_check_plan;
+int lzgpu_plan_check(const lzgpu_goal *goal, const uint8_t *given, lzgpu_check_plan *out);
+
 /* Diagnostics (pure host logic, no GPU needed): the host build of the bit-plane arithmetic the four-parity-row encoder runs per
  * item (csrc/bitslice.cuh).  data = k columns of 32 bytes (column j = 32 bytes of data part j, k <= 32); parity receives the
  * 4 x 32 bytes of the Vandermonde parity rows 0..3 (coefficient of column j in row r: (2^r)^j, galois_field_isal.cc:53-69). */

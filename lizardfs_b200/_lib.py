@@ -60,6 +60,11 @@ RECOVER_ROWS_GENERAL, RECOVER_ROWS_FIRST_E, RECOVER_ROWS_DIRECT = range(3)
 RECOVER_SOLVE_DIRECT, RECOVER_SOLVE_RAID6, RECOVER_SOLVE_ELIM3, RECOVER_SOLVE_INVERSE, RECOVER_SOLVE_INVERSE_ROW0 = range(5)
 
 
+class LzCheckPlan(C.Structure):
+    _fields_ = [("fused", C.c_int), ("rows", C.c_uint32), ("consecutive", C.c_int), ("G", C.c_uint32), ("stages", C.c_uint32),
+                ("threads", C.c_uint32), ("item_passes", C.c_uint32), ("smem_bytes", C.c_uint32)]
+
+
 class LzLaunchGeometry(C.Structure):
     _fields_ = [("kernel", C.c_int), ("grid", C.c_uint32), ("units", C.c_uint32), ("threads", C.c_uint32), ("G", C.c_uint32),
                 ("stages", C.c_uint32), ("gf_warps", C.c_uint32), ("smem_bytes", C.c_uint32)]
@@ -102,6 +107,7 @@ SIGNATURES = {
     "lzgpu_plan_encode": (_int, [_goalp, _u32, _u32, _sz, _int, _vp]),
     "lzgpu_plan_convert": (_int, [_goalp, _goalp, _vp, _vp, _vp]),
     "lzgpu_plan_recover": (_int, [_goalp, _vp, _vp, _int, _int, C.POINTER(LzRecoverSwitches), C.POINTER(LzRecoverPlan)]),
+    "lzgpu_plan_check": (_int, [_goalp, _vp, C.POINTER(LzCheckPlan)]),
     "lzgpu_debug_bitslice_rows": (_int, [_int, _vp, _vp]),
     "lzgpu_debug_bitslice_recover3": (_int, [_int, _vp, _vp, _int, _vp]),
     "lzgpu_goal_slice_type": (_int, [_goalp]),

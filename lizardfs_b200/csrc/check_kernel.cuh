@@ -18,7 +18,7 @@
 
 namespace lzd {
 
-constexpr int kCheckThreads = 512;
+// (kCheckThreads and the geometry: check_plan, fused_plan.h)
 constexpr int kCheckMaxSlots = 36;  // k data parts + up to four parity rows (ec(32,3) is the widest Vandermonde goal)
 
 struct CheckTmaps {

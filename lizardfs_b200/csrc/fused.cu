@@ -895,39 +895,32 @@ int lz_fused_check(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, ui
 	FusedState *fs = ctx->fused;
 	if (!fs || fs->disabled) return LZGPU_NOT_HANDLED;
 	const int K = goal->k, M = goal->m;
-	if (lz::uses_cauchy(K, M) || (part_stride % 16)) return LZGPU_NOT_HANDLED;
+	if (part_stride % 16) return LZGPU_NOT_HANDLED;
+	// the geometry (check_plan, fused_plan.h): the checked parity rows, G and the stage ring
+	uint8_t given[LZGPU_MAX_PARTS];
+	for (int i = 0; i < K + M; ++i) given[i] = d_parts[i] ? 1 : 0;
+	const CheckPlan pl = check_plan(K, M, lz::uses_cauchy(K, M), given);
+	const lzgpu_check_plan &o = pl.out;
+	if (!o.fused) return LZGPU_NOT_HANDLED;
 	CheckParams p{};
 	const void *slot_ptr[kCheckMaxSlots];
-	uint32_t R = 0;
-	bool consecutive = true, verifying = false;
+	const uint32_t R = o.rows, G = o.G, n_stages = o.stages, NSLOT = K + R;
+	bool verifying = false;
 	for (int a = 0; a < K; ++a) {
 		slot_ptr[a] = d_parts[a];
 		p.part_id[a] = static_cast<uint8_t>(a);
 	}
-	for (int r = 0; r < M; ++r) {
-		if (!d_parts[K + r]) continue;
-		consecutive &= static_cast<int>(R) == r;
-		slot_ptr[K + R] = d_parts[K + r];
-		p.part_id[K + R] = static_cast<uint8_t>(K + r);
-		p.row[R++] = static_cast<uint8_t>(r);
+	for (uint32_t r = 0; r < R; ++r) {
+		slot_ptr[K + r] = d_parts[K + pl.row[r]];
+		p.part_id[K + r] = static_cast<uint8_t>(K + pl.row[r]);
+		p.row[r] = pl.row[r];
 	}
-	const uint32_t NSLOT = K + R;
 	for (uint32_t a = 0; a < NSLOT; ++a) {
 		p.stored[a] = d_part_crc ? static_cast<const uint32_t *>(d_part_crc[p.part_id[a]]) : nullptr;
 		verifying |= p.stored[a] != nullptr;
 	}
 	if (verifying && !d_first_bad) return LZGPU_NOT_HANDLED;
-	// one 16-warp CTA per SM: the largest even G whose NSLOT*G*4 rows give every row a thread (one TMA box per part: G*4 <= 256 rows),
-	// with at least three stages in the shared-memory budget
-	uint32_t G = 0;
-	for (uint32_t g = 2; g <= 64; g += 2) {
-		const uint32_t rows = NSLOT * g * 4;
-		if (rows > static_cast<uint32_t>(kCheckThreads) || 3 * static_cast<size_t>(rows) * kStepBytes + 256 > static_cast<size_t>(kRecoverSmemCapBig)) break;
-		G = g;
-	}
-	if (G == 0) return LZGPU_NOT_HANDLED;
 	const uint32_t pb = (nb + K - 1) / K;
-	const uint32_t n_stages = static_cast<uint32_t>(std::min<size_t>(6, (kRecoverSmemCapBig - 256) / (static_cast<size_t>(NSLOT) * G * 4 * kStepBytes)));
 	p.tables = ctx->d_crc_tables;
 	p.first_bad = d_first_bad;
 	p.verdict = map ? nullptr : static_cast<int *>(d_verdict);
@@ -953,9 +946,10 @@ int lz_fused_check(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, ui
 		                              CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
 		if (r != CUDA_SUCCESS) return LZGPU_NOT_HANDLED;
 	}
-	const size_t smem = static_cast<size_t>(n_stages) * NSLOT * G * 4 * kStepBytes + 16 * n_stages + 64;
-	const int grid = persistent_grid(ctx, p.total_units, 1, launch_geo(LZGPU_KERNEL_CHECK, kCheckThreads, G, n_stages, 0, smem));
+	const size_t smem = o.smem_bytes;
+	const int grid = persistent_grid(ctx, p.total_units, 1, launch_geo(LZGPU_KERNEL_CHECK, o.threads, G, n_stages, 0, smem));
 	uint32_t *d_map = static_cast<uint32_t *>(d_verdict);
+	const bool consecutive = o.consecutive != 0;
 	if (map) switch (consecutive ? R : R + 4) {
 		case 1: fused_check_map_kernel<1, true><<<grid, kCheckThreads, smem, st>>>(maps, p, d_map); break;
 		case 2: fused_check_map_kernel<2, true><<<grid, kCheckThreads, smem, st>>>(maps, p, d_map); break;

@@ -1,8 +1,9 @@
 // fused_plan.h — geometry of the fused encode kernel as pure functions (no CUDA calls): which unit mode a batch gets, how many
-// stripes a unit holds, how many units there are; the same for the one-pass slice conversion (convert_plan) and the router of the
-// degraded read (recover_plan).  Shared by the launchers (fused.cu) and the diagnostics entry points lzgpu_plan_encode,
-// lzgpu_plan_convert and lzgpu_plan_recover (host_math.cc), so the decisions are unit-tested on a machine without a GPU
-// (tests/test_host_math.py, tests/test_gpu_convert_geometry.py, tests/test_gpu_recover_geometry.py).
+// stripes a unit holds, how many units there are; the same for the one-pass slice conversion (convert_plan), the router of the
+// degraded read (recover_plan) and the stripe check (check_plan).  Shared by the launchers (fused.cu) and the diagnostics entry
+// points lzgpu_plan_encode, lzgpu_plan_convert, lzgpu_plan_recover and lzgpu_plan_check (host_math.cc), so the decisions are
+// unit-tested on a machine without a GPU (tests/test_host_math.py, tests/test_gpu_convert_geometry.py,
+// tests/test_gpu_recover_geometry.py, tests/test_gpu_check_geometry.py).
 #pragma once
 #include <cstddef>
 #include <cstdint>
@@ -464,6 +465,53 @@ inline RecoverPlan recover_plan(int K, int M, bool cauchy, const uint8_t *availa
 	} else {
 		o.solve = o.rows == LZGPU_RECOVER_ROWS_FIRST_E ? LZGPU_RECOVER_SOLVE_INVERSE_ROW0 : LZGPU_RECOVER_SOLVE_INVERSE;
 	}
+	return pl;
+}
+
+// ---------------------------------------------------------------------------------------------------
+// Fused stripe check (fused_check_kernel / fused_check_map_kernel, check_kernel.cuh): the geometry as a pure function, shared by
+// lz_fused_check (which launches exactly what it returns) and lzgpu_plan_check.
+// ---------------------------------------------------------------------------------------------------
+constexpr int kCheckThreads = 512;
+
+struct CheckPlan {
+	lzgpu_check_plan out{};      // what lzgpu_plan_check reports
+	uint8_t row[4] = {0};        // generator row of checked parity slot K + r (fused only)
+};
+
+// given[i]: part i is given (data parts first; every data part is, the caller checks that).  One 16-warp CTA per SM: the largest
+// even G whose NSLOT*G*4 rows give every row a thread (one TMA box per part: G*4 <= 256 rows), with at least three stages in the
+// shared-memory budget; then as many stages as fit, at most six.
+inline CheckPlan check_plan(int K, int M, bool cauchy, const uint8_t *given) {
+	CheckPlan pl;
+	lzgpu_check_plan &o = pl.out;
+	uint32_t R = 0;
+	bool consecutive = true;
+	for (int r = 0; r < M; ++r) {
+		if (!given[K + r]) continue;
+		consecutive &= static_cast<int>(R) == r;
+		if (R < 4) pl.row[R] = static_cast<uint8_t>(r);
+		++R;
+	}
+	o.rows = R;
+	o.consecutive = consecutive ? 1 : 0;
+	if (cauchy || R == 0 || R > 4) return pl;
+	const uint32_t NSLOT = static_cast<uint32_t>(K) + R;
+	uint32_t G = 0;
+	for (uint32_t g = 2; g <= 64; g += 2) {
+		const uint32_t rows = NSLOT * g * 4;
+		if (rows > static_cast<uint32_t>(kCheckThreads) || 3 * static_cast<size_t>(rows) * kStepBytes + 256 > static_cast<size_t>(kRecoverSmemCapBig)) break;
+		G = g;
+	}
+	if (G == 0) return pl;
+	const size_t fit = (kRecoverSmemCapBig - 256) / (static_cast<size_t>(NSLOT) * G * 4 * kStepBytes);
+	const uint32_t n_stages = static_cast<uint32_t>(fit < 6 ? fit : 6);
+	o.fused = 1;
+	o.G = G;
+	o.stages = n_stages;
+	o.threads = kCheckThreads;
+	o.item_passes = (32 * G + kCheckThreads - 1) / kCheckThreads;
+	o.smem_bytes = static_cast<uint32_t>(static_cast<size_t>(n_stages) * NSLOT * G * 4 * kStepBytes + 16 * n_stages + 64);
 	return pl;
 }
 

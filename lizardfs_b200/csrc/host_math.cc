@@ -499,6 +499,20 @@ int lzgpu_plan_recover(const lzgpu_goal *goal, const uint8_t *available, const u
 	return pl.out.refusal == LZGPU_RECOVER_REFUSED_TOO_FEW_PARTS ? LZGPU_ERR_TOO_FEW_PARTS : LZGPU_OK;
 }
 
+int lzgpu_plan_check(const lzgpu_goal *goal, const uint8_t *given, lzgpu_check_plan *out) {
+	if (!out || !given || !lzgpu_goal_valid(goal)) return LZGPU_ERR_ARG;
+	const int K = goal->k, M = goal->m;
+	*out = lzgpu_check_plan{};
+	bool any_parity = false;
+	for (int i = 0; i < K + M; ++i) {
+		if (i < K && !given[i]) return LZGPU_ERR_TOO_FEW_PARTS;
+		any_parity |= i >= K && given[i];
+	}
+	if (!any_parity) return LZGPU_ERR_TOO_FEW_PARTS;
+	*out = lzd::check_plan(K, M, lz::uses_cauchy(K, M), given).out;
+	return LZGPU_OK;
+}
+
 const char *lzgpu_version(void) { return "lizardfs_b200 0.1 (sm_90a)"; }
 
 }  // extern "C"

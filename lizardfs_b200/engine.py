@@ -658,6 +658,18 @@ class Engine:
             _check(rc, "plan_recover")
         return {f: getattr(out, f) for f, _ in _lib.LzRecoverPlan._fields_}
 
+    @staticmethod
+    def plan_check(goal, given):
+        """how check_stripes / check_stripe_map / correct_stripes would check the batch (pure host logic, csrc/fused_plan.h
+        check_plan; no GPU needed): dict with fused (0 = the generic route), rows (checked parity rows), consecutive (rows 0 .. R-1),
+        G, stages, threads, item_passes, smem_bytes.  given: k+m flags, part i given; a missing data part or no parity part raises
+        LzGpuError (ERR_TOO_FEW_PARTS), as the calls do."""
+        out = _lib.LzCheckPlan()
+        g = np.asarray(given, dtype=np.uint8)
+        assert g.size == goal.k + goal.m
+        _check(_lib.load().lzgpu_plan_check(C.byref(goal.c), _p(g), C.byref(out)), "plan_check")
+        return {f: getattr(out, f) for f, _ in _lib.LzCheckPlan._fields_}
+
     def convert_chunks(self, src, dst, nb, parts, want, part_crc=None, with_crc=True):
         """Rebuild the `want`ed parts of slice type `dst` from the available `parts` of slice type `src`
         (SliceRecoveryPlanner, slice_recovery_planner.h:87-204).  parts[i]: (n_chunks, pb_src*65536) uint8 or None.
