@@ -181,6 +181,12 @@ typedef struct lzgpu_check_plan {
 	uint32_t smem_bytes;   /* dynamic shared memory per CTA */
 } lzgpu_check_plan;
 int lzgpu_plan_check(const lzgpu_goal *goal, const uint8_t *given, lzgpu_check_plan *out);
+/* The same for lzgpu_check_stripe_map_degraded / lzgpu_correct_stripes_degraded: any part may be missing.  rows and consecutive
+ * describe every given parity part (the input rows and the spares); the fused route is fused_check_degraded_kernel when a data part
+ * is missing (at most three can be, with at most four given parity rows), with G and the stage ring counted over the given data parts.
+ * With every data part given the result is exactly lzgpu_plan_check's.  Returns LZGPU_ERR_TOO_FEW_PARTS when fewer than k + 1 parts
+ * are given, as the calls do. */
+int lzgpu_plan_check_degraded(const lzgpu_goal *goal, const uint8_t *given, lzgpu_check_plan *out);
 
 /* Diagnostics (pure host logic, no GPU needed): the host build of the bit-plane arithmetic the four-parity-row encoder runs per
  * item (csrc/bitslice.cuh).  data = k columns of 32 bytes (column j = 32 bytes of data part j, k <= 32); parity receives the
@@ -250,7 +256,8 @@ enum {
 	LZGPU_KERNEL_RECOVER_DIRECT = 6,   /* fused_recover_kernel, DIRECT form (Cauchy generators) */
 	LZGPU_KERNEL_RECOVER_BS3 = 7,      /* bs_recover3_kernel: three lost data parts on bit planes */
 	LZGPU_KERNEL_CONVERT = 8,          /* fused_convert_kernel: one-pass slice conversion */
-	LZGPU_KERNEL_CHECK = 9             /* fused_check_kernel: stripe check (lzgpu_check_stripes), one 16-warp CTA per SM */
+	LZGPU_KERNEL_CHECK = 9,            /* fused_check_kernel: stripe check (lzgpu_check_stripes), one 16-warp CTA per SM */
+	LZGPU_KERNEL_CHECK_DEGRADED = 10   /* fused_check_degraded_kernel: stripe map with lost data parts (lzgpu_check_stripe_map_degraded) */
 };
 typedef struct lzgpu_launch_geometry {
 	int kernel;
@@ -458,6 +465,38 @@ int lzgpu_correct_stripes(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chu
 int lzgpu_correct_stripes_dev(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, uint32_t nb,
                               void *const *d_parts, size_t part_stride, const void *const *d_part_crc,
                               void *d_fix, int64_t *bad, void *stream);
+
+/* Stripe map and correction of chunks that have lost parts, to run before the lost parts are rebuilt.  A rebuild
+ * (lzgpu_recover_chunks, lzgpu_convert_chunks) reads the first k available parts and nothing else; if one of them is stale (valid
+ * CRCs, wrong bytes), the rebuilt block is wrong too and gets a fresh CRC, and the stripe then has two bad parts that no check can
+ * name.  These calls use the given parts beyond the first k to find and correct such a part first (errors-and-erasures decoding).
+ *   goal, n_chunks, nb, parts, part_stride, part_crc, bad, map / fix   exactly as in lzgpu_check_stripe_map / lzgpu_correct_stripes
+ *                    (layout, stored CRCs of every given part verified in the same pass, bad[0..2], deferred mode, alignment, the
+ *                    CRC-disabled mode, return codes), except that any part may be NULL: at least k + 1 parts must be given
+ *                    (otherwise LZGPU_ERR_TOO_FEW_PARTS, before anything is enqueued).
+ * The inputs are the first k given parts in ascending index (ECReadPlan::recoverParts picks them); the other given parts, the
+ * spares, are always parity parts.  A stripe is consistent exactly when every spare block equals its re-encoding from the k inputs.
+ *   bad_rows      bit r: spare part k + r disagrees in that stripe (an input never gets a bit)
+ *   suspect_part  the single given part (this API's numbering) whose corruption alone explains every non-zero syndrome byte, by the
+ *                 column test of the map over the check matrix [M | I] of the punctured code, M = the spares' recovery rows over the
+ *                 inputs; -1 otherwise.  With one spare (ec(8,2) with a part lost) a bad stripe is detected, never blamed, as with
+ *                 xorN; with two spares the two-row caveat of the map applies.
+ * A corrected block is what a one-stripe lzgpu_recover_chunks window rebuilds for the suspect from the first k given parts other
+ * than it; the rule and the CRC gate are lzgpu_correct_stripes'.  A missing part is never written.  With every data part given,
+ * both calls return byte for byte what lzgpu_check_stripe_map / lzgpu_correct_stripes return.  The route: lzgpu_plan_check_degraded
+ * (lzgpu_debug_last_geometry reports LZGPU_KERNEL_CHECK_DEGRADED when a data part is missing on the fused route). */
+int lzgpu_check_stripe_map_degraded(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, uint32_t nb,
+                                    const uint8_t *const *parts, size_t part_stride, const uint32_t *const *part_crc,
+                                    lzgpu_stripe_state *map, int64_t *bad);
+int lzgpu_check_stripe_map_degraded_dev(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, uint32_t nb,
+                                        const void *const *d_parts, size_t part_stride, const void *const *d_part_crc,
+                                        void *d_map, int64_t *bad, void *stream);
+int lzgpu_correct_stripes_degraded(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, uint32_t nb,
+                                   uint8_t *const *parts, size_t part_stride, const uint32_t *const *part_crc,
+                                   lzgpu_stripe_fix *fix, int64_t *bad);
+int lzgpu_correct_stripes_degraded_dev(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, uint32_t nb,
+                                       void *const *d_parts, size_t part_stride, const void *const *d_part_crc,
+                                       void *d_fix, int64_t *bad, void *stream);
 
 /* Wire-format producer (SURVEY.md §8 f3): LIZ_CLTOCS_WRITE_DATA packet prefixes (src/protocol/cltocs.h:116-137) for
  * every block of every part of the encoded chunks, built on the GPU straight from the CRC array of

@@ -72,7 +72,7 @@ class LzLaunchGeometry(C.Structure):
 
 # lzgpu_launch_geometry.kernel
 KERNEL_NONE, KERNEL_ENCODE, KERNEL_ENCODE_BITSLICE, KERNEL_RECOVER_GEO0, KERNEL_RECOVER_GEO1, KERNEL_RECOVER_GEO2, \
-    KERNEL_RECOVER_DIRECT, KERNEL_RECOVER_BS3, KERNEL_CONVERT, KERNEL_CHECK = range(10)
+    KERNEL_RECOVER_DIRECT, KERNEL_RECOVER_BS3, KERNEL_CONVERT, KERNEL_CHECK, KERNEL_CHECK_DEGRADED = range(11)
 
 
 class LzStripeVerdict(C.Structure):
@@ -108,6 +108,7 @@ SIGNATURES = {
     "lzgpu_plan_convert": (_int, [_goalp, _goalp, _vp, _vp, _vp]),
     "lzgpu_plan_recover": (_int, [_goalp, _vp, _vp, _int, _int, C.POINTER(LzRecoverSwitches), C.POINTER(LzRecoverPlan)]),
     "lzgpu_plan_check": (_int, [_goalp, _vp, C.POINTER(LzCheckPlan)]),
+    "lzgpu_plan_check_degraded": (_int, [_goalp, _vp, C.POINTER(LzCheckPlan)]),
     "lzgpu_debug_bitslice_rows": (_int, [_int, _vp, _vp]),
     "lzgpu_debug_bitslice_recover3": (_int, [_int, _vp, _vp, _int, _vp]),
     "lzgpu_goal_slice_type": (_int, [_goalp]),
@@ -137,6 +138,10 @@ SIGNATURES = {
     "lzgpu_check_stripe_map_dev": (_int, [_vp, _goalp, _u32, _u32, _vp, _sz, _vp, _vp, _vp, _vp]),
     "lzgpu_correct_stripes": (_int, [_vp, _goalp, _u32, _u32, _vp, _sz, _vp, _vp, _vp]),
     "lzgpu_correct_stripes_dev": (_int, [_vp, _goalp, _u32, _u32, _vp, _sz, _vp, _vp, _vp, _vp]),
+    "lzgpu_check_stripe_map_degraded": (_int, [_vp, _goalp, _u32, _u32, _vp, _sz, _vp, _vp, _vp]),
+    "lzgpu_check_stripe_map_degraded_dev": (_int, [_vp, _goalp, _u32, _u32, _vp, _sz, _vp, _vp, _vp, _vp]),
+    "lzgpu_correct_stripes_degraded": (_int, [_vp, _goalp, _u32, _u32, _vp, _sz, _vp, _vp, _vp]),
+    "lzgpu_correct_stripes_degraded_dev": (_int, [_vp, _goalp, _u32, _u32, _vp, _sz, _vp, _vp, _vp, _vp]),
     "lzgpu_write_data_prefixes": (_int, [_vp, _goalp, _u32, _u32, _vp, _sz, _vp, _u32, _vp]),
     "lzgpu_write_data_prefixes_dev": (_int, [_vp, _goalp, _u32, _u32, _vp, _sz, _vp, _u32, _vp, _vp]),
     "lzgpu_split_chunks": (_int, [_vp, _goalp, _u32, _u32, _vp, _sz, _vp, _sz]),

@@ -13,6 +13,13 @@
 //   GF role   item (stripe g, quarter q, 16-byte column): Horner over the k data columns per checked row, XOR the stored parity
 //             column, OR-reduce.  A thread keeps the lowest non-zero stripe of its unit and lowers the chunk's verdict word once
 //             (fused_check_kernel), or keeps the non-zero rows of each stripe for the stripe map (fused_check_map_kernel).
+//
+// Lost data parts (lzgpu_check_stripe_map_degraded, fused_check_degraded_kernel): E data positions L have no slot.  The inputs are the
+// k - E given data parts and the first E given parity rows P_in, the spares the other given rows P_sp (ECReadPlan::recoverParts).
+// The Horner pass still runs over all k positions (a lost one contributes its multiply step only), so S_r = p_r ^ sum_{j not in L}
+// g_rj d_j for every given row, and the spare rows are checked by  T_i = S_sp_i ^ sum_x C_ix S_in_x  with C = G[P_sp, L] G[P_in, L]^-1
+// (the host reads C off the spares' recovery rows: the coefficients of the input parity parts).  T_i is spare block sp_i minus its
+// re-encoding from the k inputs, what the generic route compares; it costs (R - E) E gf_mac per packed word.
 #pragma once
 #include "fused_kernel.cuh"
 
@@ -37,20 +44,27 @@ struct CheckParams {
 	uint8_t part_id[kCheckMaxSlots];         // slot -> part index (error reporting)
 };
 
+// fused_check_degraded_kernel's own parameter (CheckParams keeps its layout: the existing kernels' parameter offsets do not move)
+struct CheckLost {
+	uint32_t mask;                           // bit j: data position j has no slot
+	CoefPlanes elim[4];                      // C[i][x] at elim[i * E + x]: spare row E + i, input row x
+};
+
 // R = checked parity rows; CONSEC: they are rows 0 .. R-1 (row r multiplies by 2^r in one step), else p.row[r] doublings.
 // MAP = false: the per-chunk verdict word (lzgpu_check_stripes).  MAP = true (lzgpu_check_stripe_map): every stripe's bad_rows goes to
 // map[2 (c pb + s)] and its suspect_part word is set to -1 (locate_map_kernel names the suspects of the bad ones).  The items of
 // stripe g are items 32g .. 32g + 31, i.e. the 32 lanes of one warp in the same pass of the item loop, and that warp owns the stripe
 // for the whole unit: each lane keeps its row bits in a nibble per pass (at most 2048 items, four passes), and at the end of the unit
 // the warp OR-reduces each nibble and lane 0 stores the stripe's entry.  Units partition the stripes, so the map needs no memset and
-// no atomics.
-template <int R, bool CONSEC, bool MAP>
-__device__ __forceinline__ void fused_check_body(const CheckTmaps &tmaps, const CheckParams &p, uint32_t *map) {
+// no atomics.  E lost data positions (MAP only): slots 0 .. K-E-1 hold the given data parts, slot K - E + r parity row r.
+template <int R, bool CONSEC, bool MAP, int E = 0>
+__device__ __forceinline__ void fused_check_body(const CheckTmaps &tmaps, const CheckParams &p, uint32_t *map, const CheckLost *lost = nullptr) {
+	static_assert(E == 0 || (MAP && E < R), "a lost data part needs a spare row, and only the map form has one");
 	constexpr int W = 4;
 	constexpr uint32_t CPI = 32 / W;
 	extern __shared__ __align__(1024) uint8_t smem[];
 	const uint32_t sbase = smem_u32(smem);
-	const uint32_t K = p.K, G = p.G, NSLOT = K + R, n_stages = p.n_stages;
+	const uint32_t K = p.K, G = p.G, NSLOT = K - E + R, n_stages = p.n_stages;
 	const uint32_t RG = G * 4;                       // rows per slot region
 	const uint32_t ROWS = NSLOT * RG;
 	const uint32_t region_bytes = RG * kStepBytes;   // multiple of 1024 (G even)
@@ -119,9 +133,17 @@ __device__ __forceinline__ void fused_check_body(const CheckTmaps &tmaps, const 
 						for (int r = 0; r < R; ++r)
 #pragma unroll
 							for (int w = 0; w < W; ++w) acc[r][w] = 0;
+						uint32_t slot_j = K - E;  // E > 0: the slot of the next given data position is slot_j - 1
 						for (int j = static_cast<int>(K) - 1; j >= 0; --j) {
 							uint32_t v[W];
-							lds_item<W>(a_item + j * region_bytes, v);
+							if constexpr (E == 0) {
+								lds_item<W>(a_item + j * region_bytes, v);
+							} else if ((lost->mask >> j) & 1u) {
+#pragma unroll
+								for (int w = 0; w < W; ++w) v[w] = 0;  // the multiply step alone
+							} else {
+								lds_item<W>(a_item + --slot_j * region_bytes, v);
+							}
 #pragma unroll
 							for (int r = 0; r < R; ++r) {
 								const int fixed = CONSEC ? r : -1;
@@ -140,7 +162,7 @@ __device__ __forceinline__ void fused_check_body(const CheckTmaps &tmaps, const 
 								}
 							}
 						}
-						if constexpr (MAP) {
+						if constexpr (MAP && E == 0) {
 							uint32_t bits = 0;
 #pragma unroll
 							for (int r = 0; r < R; ++r) {
@@ -150,6 +172,31 @@ __device__ __forceinline__ void fused_check_body(const CheckTmaps &tmaps, const 
 								for (int w = 0; w < W; ++w) d |= acc[r][w] ^ pv[w];
 								if (d) bits |= 1u << (CONSEC ? r : p.row[r]);  // parity rows are 0..3 (m <= 4 on this route)
 							}
+							map_bits |= bits << (4 * (item / kCheckThreads));
+						} else if constexpr (MAP) {
+							// acc[r] becomes S_r; only the spare rows E .. R-1 get a bit
+#pragma unroll
+							for (int r = 0; r < R; ++r) {
+								uint32_t pv[W];
+								lds_item<W>(a_item + (K - E + r) * region_bytes, pv);
+#pragma unroll
+								for (int w = 0; w < W; ++w) acc[r][w] ^= pv[w];
+							}
+							// word by word, and the funnel-shift form of every product: the (E, R) = (2, 4) instantiation spills otherwise
+							uint32_t d[R] = {};
+#pragma unroll
+							for (int w = 0; w < W; ++w)
+#pragma unroll
+								for (int i = E; i < R; ++i) {
+									uint32_t t = acc[i][w];
+#pragma unroll
+									for (int x = 0; x < E; ++x) t = gf_mac<8>(t, acc[x][w], lost->elim[(i - E) * E + x]);
+									d[i] |= t;
+								}
+							uint32_t bits = 0;
+#pragma unroll
+							for (int i = E; i < R; ++i)
+								if (d[i]) bits |= 1u << (CONSEC ? i : p.row[i]);
 							map_bits |= bits << (4 * (item / kCheckThreads));
 						} else {
 							uint32_t any = 0;
@@ -218,6 +265,14 @@ template <int R, bool CONSEC>
 __global__ void __launch_bounds__(kCheckThreads, 1)
 fused_check_map_kernel(const __grid_constant__ CheckTmaps tmaps, const __grid_constant__ CheckParams p, uint32_t *map) {
 	fused_check_body<R, CONSEC, true>(tmaps, p, map);
+}
+
+// lzgpu_check_stripe_map_degraded: the map with E lost data parts (1 <= E < R), bad_rows bits for the spare rows only
+template <int E, int R, bool CONSEC>
+__global__ void __launch_bounds__(kCheckThreads, 1)
+fused_check_degraded_kernel(const __grid_constant__ CheckTmaps tmaps, const __grid_constant__ CheckParams p, uint32_t *map,
+                            const __grid_constant__ CheckLost lost) {
+	fused_check_body<R, CONSEC, true, E>(tmaps, p, map, &lost);
 }
 
 }  // namespace lzd

@@ -1127,17 +1127,24 @@ extern "C" int lzgpu_recover_chunks(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint
 // ------------------------------------------------------------------------------------------------
 // stripe check: do the parts of every stripe still form a codeword?
 // ------------------------------------------------------------------------------------------------
-// dev: device pointers, whose alignment the kernels need (the host variant stages into aligned buffers)
+// dev: device pointers, whose alignment the kernels need (the host variant stages into aligned buffers).  degraded: any part may be
+// missing as long as k + 1 are given (the _degraded calls); otherwise every data part and one parity part are required.
 static int check_args(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t nb, const void *const *parts, const void *const *part_crc,
-                      const void *verdict, bool dev) {
+                      const void *verdict, bool dev, bool degraded = false) {
 	if (!parts || !verdict) return LZGPU_ERR_ARG;
 	int rc = check_batch(ctx, goal, nb);
 	if (rc) return rc;
 	const int k = goal->k, n = goal->k + goal->m;
+	int n_given = 0;
 	bool any_parity = false;
 	for (int i = 0; i < n; ++i) {
-		if (i < k && !parts[i]) { lz_set_error("check_stripes: data part %d is missing; every data part is required", i); return LZGPU_ERR_TOO_FEW_PARTS; }
+		if (i < k && !parts[i] && !degraded) { lz_set_error("check_stripes: data part %d is missing; every data part is required", i); return LZGPU_ERR_TOO_FEW_PARTS; }
 		any_parity |= i >= k && parts[i];
+		n_given += parts[i] ? 1 : 0;
+	}
+	if (degraded && n_given < k + 1) {
+		lz_set_error("check_stripes: %d parts given; a degraded check needs k + 1 = %d (one beyond the inputs)", n_given, k + 1);
+		return LZGPU_ERR_TOO_FEW_PARTS;
 	}
 	if (!any_parity) { lz_set_error("check_stripes: no parity part given, nothing to check"); return LZGPU_ERR_TOO_FEW_PARTS; }
 	if (!dev) return LZGPU_OK;
@@ -1154,6 +1161,44 @@ static int check_enqueue(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chun
 	const uint32_t B = LZGPU_BLOCK_SIZE;
 	const uint32_t pb = (nb + k - 1) / k;
 	if (part_stride < static_cast<size_t>(pb) * B || (part_stride & 15)) { lz_set_error("check_stripes: bad part_stride"); return LZGPU_ERR_ARG; }
+	// The inputs are the first k given parts (ECReadPlan::recoverParts), the spares the given parts after them: always parity parts.
+	// Each checked row is a spare against its recovery row over the inputs; with every data part given those are the data parts and
+	// the generator's parity rows.  la.part[0 .. k-1] are the inputs, la.part[k + r] spare parity part r.
+	LocateArgs la{};
+	InputParts inputs{};
+	uint8_t erased[LZGPU_MAX_PARTS] = {0}, spare[LZGPU_MAX_PARTS] = {0};
+	int used = 0;
+	for (int i = 0; i < n; ++i) {
+		la.part[i] = static_cast<const uint8_t *>(d_parts[i]);
+		if (!d_parts[i] || used >= k) erased[i] = 1;
+		else inputs.part[used++] = static_cast<uint8_t>(i);
+		spare[i] = erased[i] && d_parts[i];
+	}
+	const int lost = k - std::count_if(d_parts, d_parts + k, [](const void *p) { return p != nullptr; });
+	uint8_t rows[LZGPU_MAX_PARITY * LZGPU_MAX_DATA];
+	if (lost == 0) {
+		goal_parity_rows(goal, rows);
+	} else {
+		bool singular = false;
+		if (lz::rs_recovery_matrix(k, m, erased, spare, rows, &singular) < 1) {
+			lz_set_error(singular ? "check_stripes: decode matrix is singular" : "check_stripes: bad erasure pattern");
+			return LZGPU_ERR_ARG;
+		}
+		for (int j = 0; j < k; ++j) la.part[j] = static_cast<const uint8_t *>(d_parts[inputs.part[j]]);
+	}
+	for (int r = 0; r < m; ++r)
+		if (spare[k + r]) {
+			la.row[la.n_rows] = static_cast<uint8_t>(r);
+			std::memcpy(la.coef + 32 * la.n_rows, rows + (lost ? la.n_rows : r) * k, k);  // recovery rows come in ascending part order
+			++la.n_rows;
+		}
+	// the fused route's elimination C[i][x]: in spare i's recovery row, the coefficient of input parity part x (input k - lost + x);
+	// that route takes at most three lost data parts (check_plan)
+	uint8_t elim[LZGPU_MAX_PARITY * 3];
+	if (lost > 0 && lost <= 3)
+		for (uint32_t i = 0; i < la.n_rows; ++i)
+			for (int x = 0; x < lost; ++x) elim[i * lost + x] = la.coef[32 * i + k - lost + x];
+
 	InputCrcs crcs(ctx, st, tk, d_parts, d_part_crc, n, n, n_chunks, pb, part_stride);  // every given part is read
 	int rc = crcs.begin();
 	if (rc) return rc;
@@ -1161,18 +1206,9 @@ static int check_enqueue(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chun
 	// fused map kernel writes every entry of the map; the generic route ORs into a zeroed one.
 	const size_t map_bytes = static_cast<size_t>(n_chunks) * pb * sizeof(lzgpu_stripe_state);
 	if (!map) CUDA_TRY(cudaMemsetAsync(d_verdict, 0x7f, static_cast<size_t>(n_chunks) * sizeof(lzgpu_stripe_verdict), st));
-	uint8_t gen_rows[LZGPU_MAX_PARITY * LZGPU_MAX_DATA];
-	goal_parity_rows(goal, gen_rows);
-	LocateArgs la{};
-	for (int i = 0; i < n; ++i) la.part[i] = static_cast<const uint8_t *>(d_parts[i]);
-	for (int r = 0; r < m; ++r)
-		if (d_parts[k + r]) {
-			la.row[la.n_rows] = static_cast<uint8_t>(r);
-			std::memcpy(la.coef + 32 * la.n_rows, gen_rows + r * k, k);
-			++la.n_rows;
-		}
 
-	rc = lz_fused_check(ctx, goal, n_chunks, nb, d_parts, part_stride, crcs.for_kernels(), d_verdict, st, crcs.fused_word(), map);
+	rc = lz_fused_check(ctx, goal, n_chunks, nb, d_parts, part_stride, crcs.for_kernels(), d_verdict, st, crcs.fused_word(), map,
+	                    lost ? elim : nullptr);
 	const bool fused = rc != LZGPU_NOT_HANDLED;
 	if (fused && rc) return rc;
 	if (!fused) {
@@ -1203,7 +1239,8 @@ static int check_enqueue(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chun
 	la.pb = pb;
 	if (map) {
 		const unsigned long long entries = static_cast<unsigned long long>(n_chunks) * pb;
-		locate_map_kernel<<<grid_for(ctx, entries * 256, 256, 8), 256, 0, st>>>(la, entries);
+		if (lost) locate_map_degraded_kernel<<<grid_for(ctx, entries * 256, 256, 8), 256, 0, st>>>(la, entries, inputs);
+		else locate_map_kernel<<<grid_for(ctx, entries * 256, 256, 8), 256, 0, st>>>(la, entries);
 	} else {
 		locate_kernel<<<n_chunks, 256, 0, st>>>(la);
 	}
@@ -1223,8 +1260,8 @@ static uint64_t check_alg_bytes(const lzgpu_goal *goal, uint32_t n_chunks, uint3
 }
 
 static int check_dev(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, uint32_t nb, const void *const *d_parts, size_t part_stride,
-                     const void *const *d_part_crc, void *d_out, int64_t *bad, void *stream, bool map) {
-	int rc = check_args(ctx, goal, nb, d_parts, d_part_crc, d_out, true);
+                     const void *const *d_part_crc, void *d_out, int64_t *bad, void *stream, bool map, bool degraded = false) {
+	int rc = check_args(ctx, goal, nb, d_parts, d_part_crc, d_out, true, degraded);
 	if (rc || n_chunks == 0) return rc;
 	return dev_call(ctx, stream, check_alg_bytes(goal, n_chunks, nb, d_parts, d_part_crc, map), bad, [&](cudaStream_t st, VerifyTicket *tk) {
 		return check_enqueue(ctx, goal, n_chunks, nb, d_parts, part_stride, d_part_crc, d_out, st, tk, map);
@@ -1243,10 +1280,17 @@ extern "C" int lzgpu_check_stripe_map_dev(lzgpu_ctx *ctx, const lzgpu_goal *goal
 	return check_dev(ctx, goal, n_chunks, nb, d_parts, part_stride, d_part_crc, d_map, bad, stream, true);
 }
 
+extern "C" int lzgpu_check_stripe_map_degraded_dev(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, uint32_t nb,
+                                                   const void *const *d_parts, size_t part_stride, const void *const *d_part_crc, void *d_map,
+                                                   int64_t *bad, void *stream) {
+	NvtxScope nvtx_scope("lzgpu::check_stripe_map_degraded_dev");
+	return check_dev(ctx, goal, n_chunks, nb, d_parts, part_stride, d_part_crc, d_map, bad, stream, true, true);
+}
+
 // the host-pointer calls: out = lzgpu_stripe_verdict[n_chunks], or (map) lzgpu_stripe_state[n_chunks * pb]
 static int check_host(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, uint32_t nb, const uint8_t *const *parts,
-                      size_t part_stride, const uint32_t *const *part_crc, void *out, int64_t *bad, bool map) {
-	int rc = check_args(ctx, goal, nb, reinterpret_cast<const void *const *>(parts), nullptr, out, false);
+                      size_t part_stride, const uint32_t *const *part_crc, void *out, int64_t *bad, bool map, bool degraded = false) {
+	int rc = check_args(ctx, goal, nb, reinterpret_cast<const void *const *>(parts), nullptr, out, false, degraded);
 	if (rc) return rc;
 	if (n_chunks == 0) return LZGPU_OK;
 	const int k = goal->k, n = goal->k + goal->m;
@@ -1312,6 +1356,13 @@ extern "C" int lzgpu_check_stripe_map(lzgpu_ctx *ctx, const lzgpu_goal *goal, ui
 	return check_host(ctx, goal, n_chunks, nb, parts, part_stride, part_crc, map, bad, true);
 }
 
+extern "C" int lzgpu_check_stripe_map_degraded(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, uint32_t nb,
+                                               const uint8_t *const *parts, size_t part_stride, const uint32_t *const *part_crc,
+                                               lzgpu_stripe_state *map, int64_t *bad) {
+	NvtxScope nvtx_scope("lzgpu::check_stripe_map_degraded");
+	return check_host(ctx, goal, n_chunks, nb, parts, part_stride, part_crc, map, bad, true, true);
+}
+
 // ------------------------------------------------------------------------------------------------
 // stripe correction: the stripe map, then every stripe that names a suspect rebuilt in place (correct_kernel.cuh)
 // ------------------------------------------------------------------------------------------------
@@ -1370,10 +1421,9 @@ static int correct_enqueue(lzgpu_ctx *ctx, CorrectArgs &a, unsigned long long n_
 	return LZGPU_OK;
 }
 
-extern "C" int lzgpu_correct_stripes_dev(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, uint32_t nb, void *const *d_parts,
-                                         size_t part_stride, const void *const *d_part_crc, void *d_fix, int64_t *bad, void *stream) {
-	NvtxScope nvtx_scope("lzgpu::correct_stripes_dev");
-	int rc = check_args(ctx, goal, nb, d_parts, d_part_crc, d_fix, true);
+static int correct_dev(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, uint32_t nb, void *const *d_parts, size_t part_stride,
+                       const void *const *d_part_crc, void *d_fix, int64_t *bad, void *stream, bool degraded) {
+	int rc = check_args(ctx, goal, nb, d_parts, d_part_crc, d_fix, true, degraded);
 	if (rc) return rc;
 	if (n_chunks == 0) return LZGPU_OK;
 	const int n = goal->k + goal->m;
@@ -1397,6 +1447,18 @@ extern "C" int lzgpu_correct_stripes_dev(lzgpu_ctx *ctx, const lzgpu_goal *goal,
 			return rc;
 		return correct_enqueue(ctx, a, entries, pb, part_stride, map.p, d_fix, st);
 	});
+}
+
+extern "C" int lzgpu_correct_stripes_dev(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, uint32_t nb, void *const *d_parts,
+                                         size_t part_stride, const void *const *d_part_crc, void *d_fix, int64_t *bad, void *stream) {
+	NvtxScope nvtx_scope("lzgpu::correct_stripes_dev");
+	return correct_dev(ctx, goal, n_chunks, nb, d_parts, part_stride, d_part_crc, d_fix, bad, stream, false);
+}
+
+extern "C" int lzgpu_correct_stripes_degraded_dev(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, uint32_t nb, void *const *d_parts,
+                                                  size_t part_stride, const void *const *d_part_crc, void *d_fix, int64_t *bad, void *stream) {
+	NvtxScope nvtx_scope("lzgpu::correct_stripes_degraded_dev");
+	return correct_dev(ctx, goal, n_chunks, nb, d_parts, part_stride, d_part_crc, d_fix, bad, stream, true);
 }
 
 // The host-pointer correction, phase 2: the stripes `todo` (map indices with a suspect) gathered into one-stripe "chunks" (pb = 1:
@@ -1467,14 +1529,13 @@ static int correct_host_stripes(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t
 	return LZGPU_OK;
 }
 
-extern "C" int lzgpu_correct_stripes(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, uint32_t nb, uint8_t *const *parts,
-                                     size_t part_stride, const uint32_t *const *part_crc, lzgpu_stripe_fix *fix, int64_t *bad) {
-	NvtxScope nvtx_scope("lzgpu::correct_stripes");
+static int correct_host(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, uint32_t nb, uint8_t *const *parts, size_t part_stride,
+                        const uint32_t *const *part_crc, lzgpu_stripe_fix *fix, int64_t *bad, bool degraded) {
 	if (!fix) return LZGPU_ERR_ARG;
 	// phase 1: the map of the whole batch through the check's tile pipeline (only the map comes back)
 	const uint32_t pb = goal && goal->k > 0 ? (nb + goal->k - 1) / goal->k : 0;
 	std::vector<lzgpu_stripe_state> map(std::max<size_t>(1, static_cast<size_t>(n_chunks) * pb));
-	const int check_rc = check_host(ctx, goal, n_chunks, nb, parts, part_stride, part_crc, map.data(), bad, true);
+	const int check_rc = check_host(ctx, goal, n_chunks, nb, parts, part_stride, part_crc, map.data(), bad, true, degraded);
 	if (check_rc != LZGPU_OK && check_rc != LZGPU_ERR_CRC && check_rc != LZGPU_ERR_INCONSISTENT) return check_rc;
 	if (n_chunks == 0) return LZGPU_OK;
 	std::vector<size_t> todo;
@@ -1495,6 +1556,18 @@ extern "C" int lzgpu_correct_stripes(lzgpu_ctx *ctx, const lzgpu_goal *goal, uin
 			return LZGPU_ERR_INCONSISTENT;
 		}
 	return LZGPU_OK;
+}
+
+extern "C" int lzgpu_correct_stripes(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, uint32_t nb, uint8_t *const *parts,
+                                     size_t part_stride, const uint32_t *const *part_crc, lzgpu_stripe_fix *fix, int64_t *bad) {
+	NvtxScope nvtx_scope("lzgpu::correct_stripes");
+	return correct_host(ctx, goal, n_chunks, nb, parts, part_stride, part_crc, fix, bad, false);
+}
+
+extern "C" int lzgpu_correct_stripes_degraded(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, uint32_t nb, uint8_t *const *parts,
+                                              size_t part_stride, const uint32_t *const *part_crc, lzgpu_stripe_fix *fix, int64_t *bad) {
+	NvtxScope nvtx_scope("lzgpu::correct_stripes_degraded");
+	return correct_host(ctx, goal, n_chunks, nb, parts, part_stride, part_crc, fix, bad, true);
 }
 
 // ------------------------------------------------------------------------------------------------

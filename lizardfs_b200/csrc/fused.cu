@@ -175,6 +175,15 @@ static int set_all_recover_attrs() {
 	CUDA_TRY(cudaFuncSetAttribute(fused_check_map_kernel<1, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kRecoverSmemCapBig));
 	CUDA_TRY(cudaFuncSetAttribute(fused_check_map_kernel<2, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kRecoverSmemCapBig));
 	CUDA_TRY(cudaFuncSetAttribute(fused_check_map_kernel<3, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kRecoverSmemCapBig));
+	CUDA_TRY(cudaFuncSetAttribute(fused_check_degraded_kernel<1, 2, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kRecoverSmemCapBig));
+	CUDA_TRY(cudaFuncSetAttribute(fused_check_degraded_kernel<1, 3, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kRecoverSmemCapBig));
+	CUDA_TRY(cudaFuncSetAttribute(fused_check_degraded_kernel<1, 4, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kRecoverSmemCapBig));
+	CUDA_TRY(cudaFuncSetAttribute(fused_check_degraded_kernel<2, 3, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kRecoverSmemCapBig));
+	CUDA_TRY(cudaFuncSetAttribute(fused_check_degraded_kernel<2, 4, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kRecoverSmemCapBig));
+	CUDA_TRY(cudaFuncSetAttribute(fused_check_degraded_kernel<3, 4, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kRecoverSmemCapBig));
+	CUDA_TRY(cudaFuncSetAttribute(fused_check_degraded_kernel<1, 2, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kRecoverSmemCapBig));
+	CUDA_TRY(cudaFuncSetAttribute(fused_check_degraded_kernel<1, 3, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kRecoverSmemCapBig));
+	CUDA_TRY(cudaFuncSetAttribute(fused_check_degraded_kernel<2, 3, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kRecoverSmemCapBig));
 	return LZGPU_OK;
 }
 
@@ -891,7 +900,8 @@ int lz_fused_recover(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, 
 // fused stripe check (check_kernel.cuh)
 // ---------------------------------------------------------------------------------------------------
 int lz_fused_check(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, uint32_t nb, const void *const *d_parts, size_t part_stride,
-                   const void *const *d_part_crc, void *d_verdict, cudaStream_t st, unsigned long long *d_first_bad, bool map) {
+                   const void *const *d_part_crc, void *d_verdict, cudaStream_t st, unsigned long long *d_first_bad, bool map,
+                   const uint8_t *elim) {
 	FusedState *fs = ctx->fused;
 	if (!fs || fs->disabled) return LZGPU_NOT_HANDLED;
 	const int K = goal->k, M = goal->m;
@@ -903,18 +913,27 @@ int lz_fused_check(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, ui
 	const lzgpu_check_plan &o = pl.out;
 	if (!o.fused) return LZGPU_NOT_HANDLED;
 	CheckParams p{};
+	CheckLost lost{};
 	const void *slot_ptr[kCheckMaxSlots];
-	const uint32_t R = o.rows, G = o.G, n_stages = o.stages, NSLOT = K + R;
-	bool verifying = false;
+	// the given data parts in slots 0 .. D-1, then the parity rows; a lost data part has no slot
+	uint32_t D = 0;
 	for (int a = 0; a < K; ++a) {
-		slot_ptr[a] = d_parts[a];
-		p.part_id[a] = static_cast<uint8_t>(a);
+		if (!d_parts[a]) {
+			lost.mask |= 1u << a;
+			continue;
+		}
+		slot_ptr[D] = d_parts[a];
+		p.part_id[D++] = static_cast<uint8_t>(a);
 	}
+	const uint32_t R = o.rows, G = o.G, n_stages = o.stages, NSLOT = D + R, E = K - D;
+	if (E > 0 && (!map || !elim)) return LZGPU_ERR_ARG;  // (cannot happen: only the degraded map loses data parts)
+	bool verifying = false;
 	for (uint32_t r = 0; r < R; ++r) {
-		slot_ptr[K + r] = d_parts[K + pl.row[r]];
-		p.part_id[K + r] = static_cast<uint8_t>(K + pl.row[r]);
+		slot_ptr[D + r] = d_parts[K + pl.row[r]];
+		p.part_id[D + r] = static_cast<uint8_t>(K + pl.row[r]);
 		p.row[r] = pl.row[r];
 	}
+	for (uint32_t i = 0; E > 0 && i < (R - E) * E; ++i) coef_planes_set(lost.elim[i], elim[i]);
 	for (uint32_t a = 0; a < NSLOT; ++a) {
 		p.stored[a] = d_part_crc ? static_cast<const uint32_t *>(d_part_crc[p.part_id[a]]) : nullptr;
 		verifying |= p.stored[a] != nullptr;
@@ -947,10 +966,23 @@ int lz_fused_check(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, ui
 		if (r != CUDA_SUCCESS) return LZGPU_NOT_HANDLED;
 	}
 	const size_t smem = o.smem_bytes;
-	const int grid = persistent_grid(ctx, p.total_units, 1, launch_geo(LZGPU_KERNEL_CHECK, o.threads, G, n_stages, 0, smem));
+	const int grid = persistent_grid(ctx, p.total_units, 1, launch_geo(E > 0 ? LZGPU_KERNEL_CHECK_DEGRADED : LZGPU_KERNEL_CHECK, o.threads, G,
+	                                                                   n_stages, 0, smem));
 	uint32_t *d_map = static_cast<uint32_t *>(d_verdict);
 	const bool consecutive = o.consecutive != 0;
-	if (map) switch (consecutive ? R : R + 4) {
+	// E lost data parts, R given parity rows: E < R <= 4, and rows other than 0 .. R-1 only with m <= 4, so R <= 3 (m >= 5 is Cauchy)
+	if (E > 0) switch (10 * E + (consecutive ? R : R + 4)) {
+		case 12: fused_check_degraded_kernel<1, 2, true><<<grid, kCheckThreads, smem, st>>>(maps, p, d_map, lost); break;
+		case 13: fused_check_degraded_kernel<1, 3, true><<<grid, kCheckThreads, smem, st>>>(maps, p, d_map, lost); break;
+		case 14: fused_check_degraded_kernel<1, 4, true><<<grid, kCheckThreads, smem, st>>>(maps, p, d_map, lost); break;
+		case 23: fused_check_degraded_kernel<2, 3, true><<<grid, kCheckThreads, smem, st>>>(maps, p, d_map, lost); break;
+		case 24: fused_check_degraded_kernel<2, 4, true><<<grid, kCheckThreads, smem, st>>>(maps, p, d_map, lost); break;
+		case 34: fused_check_degraded_kernel<3, 4, true><<<grid, kCheckThreads, smem, st>>>(maps, p, d_map, lost); break;
+		case 16: fused_check_degraded_kernel<1, 2, false><<<grid, kCheckThreads, smem, st>>>(maps, p, d_map, lost); break;
+		case 17: fused_check_degraded_kernel<1, 3, false><<<grid, kCheckThreads, smem, st>>>(maps, p, d_map, lost); break;
+		default: fused_check_degraded_kernel<2, 3, false><<<grid, kCheckThreads, smem, st>>>(maps, p, d_map, lost); break;
+	}
+	else if (map) switch (consecutive ? R : R + 4) {
 		case 1: fused_check_map_kernel<1, true><<<grid, kCheckThreads, smem, st>>>(maps, p, d_map); break;
 		case 2: fused_check_map_kernel<2, true><<<grid, kCheckThreads, smem, st>>>(maps, p, d_map); break;
 		case 3: fused_check_map_kernel<3, true><<<grid, kCheckThreads, smem, st>>>(maps, p, d_map); break;

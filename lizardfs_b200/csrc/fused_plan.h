@@ -479,13 +479,15 @@ struct CheckPlan {
 	uint8_t row[4] = {0};        // generator row of checked parity slot K + r (fused only)
 };
 
-// given[i]: part i is given (data parts first; every data part is, the caller checks that).  One 16-warp CTA per SM: the largest
-// even G whose NSLOT*G*4 rows give every row a thread (one TMA box per part: G*4 <= 256 rows), with at least three stages in the
+// given[i]: part i is given (data parts first).  A missing data part has no slot (fused_check_degraded_kernel; the degraded calls
+// guarantee more given parity rows than lost data parts).  One 16-warp CTA per SM: the largest even G whose NSLOT*G*4 rows give
+// every row a thread (one TMA box per part: G*4 <= 256 rows), NSLOT = given data parts + R, with at least three stages in the
 // shared-memory budget; then as many stages as fit, at most six.
 inline CheckPlan check_plan(int K, int M, bool cauchy, const uint8_t *given) {
 	CheckPlan pl;
 	lzgpu_check_plan &o = pl.out;
-	uint32_t R = 0;
+	uint32_t D = 0, R = 0;
+	for (int j = 0; j < K; ++j) D += given[j] ? 1u : 0u;
 	bool consecutive = true;
 	for (int r = 0; r < M; ++r) {
 		if (!given[K + r]) continue;
@@ -495,8 +497,8 @@ inline CheckPlan check_plan(int K, int M, bool cauchy, const uint8_t *given) {
 	}
 	o.rows = R;
 	o.consecutive = consecutive ? 1 : 0;
-	if (cauchy || R == 0 || R > 4) return pl;
-	const uint32_t NSLOT = static_cast<uint32_t>(K) + R;
+	if (cauchy || R == 0 || R > 4 || D + R <= static_cast<uint32_t>(K)) return pl;
+	const uint32_t NSLOT = D + R;
 	uint32_t G = 0;
 	for (uint32_t g = 2; g <= 64; g += 2) {
 		const uint32_t rows = NSLOT * g * 4;

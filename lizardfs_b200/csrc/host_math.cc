@@ -513,6 +513,17 @@ int lzgpu_plan_check(const lzgpu_goal *goal, const uint8_t *given, lzgpu_check_p
 	return LZGPU_OK;
 }
 
+int lzgpu_plan_check_degraded(const lzgpu_goal *goal, const uint8_t *given, lzgpu_check_plan *out) {
+	if (!out || !given || !lzgpu_goal_valid(goal)) return LZGPU_ERR_ARG;
+	const int K = goal->k, M = goal->m;
+	*out = lzgpu_check_plan{};
+	int n_given = 0;
+	for (int i = 0; i < K + M; ++i) n_given += given[i] ? 1 : 0;
+	if (n_given < K + 1) return LZGPU_ERR_TOO_FEW_PARTS;
+	*out = lzd::check_plan(K, M, lz::uses_cauchy(K, M), given).out;
+	return LZGPU_OK;
+}
+
 const char *lzgpu_version(void) { return "lizardfs_b200 0.1 (sm_90a)"; }
 
 }  // extern "C"

@@ -220,8 +220,10 @@ __global__ void __launch_bounds__(256) locate_kernel(const LocateArgs a) {
 
 // lzgpu_check_stripe_map, after either route has written every entry's bad_rows (a.verdict = the map as two words per entry, n
 // entries): grid-stride over the entries, one CTA per bad stripe, which names its suspect; a clean entry's suspect_part is set to -1.
-// bad_rows stays as the check kernel wrote it.
-__global__ void __launch_bounds__(256) locate_map_kernel(const LocateArgs a, unsigned long long n) {
+// bad_rows stays as the check kernel wrote it.  REMAP (lzgpu_check_stripe_map_degraded): a.part[0 .. k-1] are the k inputs, not the
+// data parts, so a suspect j < k is reported as input_part[j]; a spare keeps its index.
+template <bool REMAP>
+__device__ __forceinline__ void locate_map_entries(const LocateArgs &a, unsigned long long n, const uint8_t *input_part) {
 	__shared__ LocateSmem sm;
 	locate_tables(sm);  // built by every CTA: deferring it to the first bad entry makes ptxas spill the locate loop
 	for (unsigned long long e = blockIdx.x; e < n; e += gridDim.x) {
@@ -232,8 +234,19 @@ __global__ void __launch_bounds__(256) locate_map_kernel(const LocateArgs a, uns
 		}
 		unsigned rows;
 		const int suspect = locate_stripe(a, sm, e / a.pb, static_cast<uint32_t>(e % a.pb), &rows);
-		if (threadIdx.x == 0) v[1] = suspect;
+		if (threadIdx.x == 0) v[1] = REMAP && suspect >= 0 && static_cast<uint32_t>(suspect) < a.k ? input_part[suspect] : suspect;
 	}
+}
+
+__global__ void __launch_bounds__(256) locate_map_kernel(const LocateArgs a, unsigned long long n) {
+	locate_map_entries<false>(a, n, nullptr);
+}
+
+struct InputParts {
+	uint8_t part[32];  // input j of the degraded map: part part[j]
+};
+__global__ void __launch_bounds__(256) locate_map_degraded_kernel(const LocateArgs a, unsigned long long n, const __grid_constant__ InputParts in) {
+	locate_map_entries<true>(a, n, in.part);
 }
 
 // CRC-disabled build mode (reference crc.cc:28-41): every emitted CRC is the constant, stored CRCs are compared with it

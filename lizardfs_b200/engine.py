@@ -580,6 +580,30 @@ class Engine:
         the call only enqueues."""
         self._part_batch_dev(self.lib.lzgpu_correct_stripes_dev, goal, n_chunks, nb, d_parts, part_stride, d_part_crc, d_fix, stream)
 
+    def check_stripe_map_degraded(self, goal, nb, parts, part_crc=None):
+        """The stripe map of chunks that have lost parts (lzgpu_check_stripe_map_degraded), to take before a lost part is rebuilt.
+        parts and part_crc as in check_stripe_map, but any part may be None as long as k + 1 are given: the first k given parts are
+        the inputs, the others (parity parts) are checked against their re-encoding from the inputs, and bad_rows bit r is spare part
+        k + r.  With every data part given the result is check_stripe_map's."""
+        return self._part_batch(self.lib.lzgpu_check_stripe_map_degraded, goal, nb, parts, part_crc,
+                                lambda n, pb: np.empty((n, pb), dtype=self.STRIPE_STATE_DTYPE), "map")
+
+    def check_stripe_map_degraded_dev(self, goal, n_chunks, nb, d_parts, part_stride, d_part_crc, d_map, stream=None):
+        """Device-pointer form of check_stripe_map_degraded, as check_stripe_map_dev"""
+        self._part_batch_dev(self.lib.lzgpu_check_stripe_map_degraded_dev, goal, n_chunks, nb, d_parts, part_stride, d_part_crc, d_map,
+                             stream)
+
+    def correct_stripes_degraded(self, goal, nb, parts, part_crc=None):
+        """correct_stripes on the map of check_stripe_map_degraded (lzgpu_correct_stripes_degraded): every stripe that names a
+        suspect has its block rewritten in place from the first k given parts other than it; a missing part is never written"""
+        return self._part_batch(self.lib.lzgpu_correct_stripes_degraded, goal, nb, parts, part_crc,
+                                lambda n, pb: np.empty((n, pb), dtype=self.STRIPE_FIX_DTYPE), "fix", in_place=True)
+
+    def correct_stripes_degraded_dev(self, goal, n_chunks, nb, d_parts, part_stride, d_part_crc, d_fix, stream=None):
+        """Device-pointer form of correct_stripes_degraded, as correct_stripes_dev"""
+        self._part_batch_dev(self.lib.lzgpu_correct_stripes_degraded_dev, goal, n_chunks, nb, d_parts, part_stride, d_part_crc, d_fix,
+                             stream)
+
     # ---- wire format --------------------------------------------------------------------------
     def write_data_prefixes(self, goal, nb, crc, chunk_ids, write_id_base=0):
         """LIZ_CLTOCS_WRITE_DATA prefixes (cltocs.h:116-137) for every block of every part: uint8 [n, k+m, pb, 38]
@@ -668,6 +692,16 @@ class Engine:
         g = np.asarray(given, dtype=np.uint8)
         assert g.size == goal.k + goal.m
         _check(_lib.load().lzgpu_plan_check(C.byref(goal.c), _p(g), C.byref(out)), "plan_check")
+        return {f: getattr(out, f) for f, _ in _lib.LzCheckPlan._fields_}
+
+    @staticmethod
+    def plan_check_degraded(goal, given):
+        """how check_stripe_map_degraded / correct_stripes_degraded would check the batch (lzgpu_plan_check_degraded): the dict of
+        plan_check; any part may be missing, fewer than k + 1 given parts raise LzGpuError (ERR_TOO_FEW_PARTS), as the calls do"""
+        out = _lib.LzCheckPlan()
+        g = np.asarray(given, dtype=np.uint8)
+        assert g.size == goal.k + goal.m
+        _check(_lib.load().lzgpu_plan_check_degraded(C.byref(goal.c), _p(g), C.byref(out)), "plan_check_degraded")
         return {f: getattr(out, f) for f, _ in _lib.LzCheckPlan._fields_}
 
     def convert_chunks(self, src, dst, nb, parts, want, part_crc=None, with_crc=True):

@@ -19,7 +19,13 @@ copies on the same stream, outside the timed region.  With one bad stripe per ch
 back on the host, then one lzgpu_recover_chunks_dev call per bad stripe over a one-stripe window, writing the suspect's block in place.
 In every case the fix entries of both routes must be identical and the corrected bytes must be the original ones.
 
-    python tools/bench_check.py [--chunks 16] [--iters 20] [--warmup 3]      (one JSON line per measurement)
+The degraded map (lzgpu_check_stripe_map_degraded_dev) runs on the same kind of batch with data parts missing: ec(8,2) without part 1
+(one spare), ec(5,3) without part 1, ec(8,3) without parts 1 and 4, ec(8,4) without part 1 and without parts 1 and 4.  Each row times
+it on the fused and the generic route and times the full-parts map of the same goal, alternating the three calls twice.  Algorithmic
+bytes are the given parts, their stored CRCs and the 8-byte map entries.  Both routes must return identical maps, clean and with one
+stale input block per chunk, which they must name when there are two spares or more.
+
+    python tools/bench_check.py [--chunks 16] [--iters 20] [--warmup 3] [--only degraded]      (one JSON line per measurement)
 """
 import argparse
 import json
@@ -242,11 +248,76 @@ def correct_rows(eng, generic, r, text, args, stream, info):
             torch.cuda.synchronize()
 
 
+DEGRADED = [("ec(8,2)", (1,)), ("ec(5,3)", (1,)), ("ec(8,3)", (1, 4)), ("ec(8,4)", (1,)), ("ec(8,4)", (1, 4))]
+
+
+def degraded_rows(eng, generic, args, stream, info):
+    """the degraded map on both routes and the full-parts map of the same goal, same resident batch"""
+    st = stream.cuda_stream
+    for text, lost in DEGRADED:
+        r = Resident(eng, text, args.chunks)
+        n = r.k + r.m
+        out = torch.empty(8 * r.n * r.pb, dtype=torch.uint8, device="cuda")
+        parts = [0 if i in lost else p for i, p in enumerate(r.ptrs)]
+        crcs = [0 if i in lost else p for i, p in enumerate(r.crc_ptrs)]
+
+        def degraded(e):
+            e.check_stripe_map_degraded_dev(r.goal, r.n, NB, parts, r.stride, crcs, out.data_ptr(), stream=st)
+
+        def full():
+            eng.check_stripe_map_dev(r.goal, r.n, NB, r.ptrs, r.stride, r.crc_ptrs, out.data_ptr(), stream=st)
+
+        t_fused = t_generic = t_full = 0.0
+        for _ in range(2):               # alternate the calls, twice: other work shares the card
+            t_fused += timed(lambda: degraded(eng), args.iters, args.warmup, stream) / 2
+            eng.sync()
+            geo = eng.last_geometry()
+            t_generic += timed(lambda: degraded(generic), args.iters, args.warmup, stream) / 2
+            generic.sync()
+            t_full += timed(full, args.iters, args.warmup, stream) / 2
+            eng.sync()
+        assert geo["kernel"] == _lib.KERNEL_CHECK_DEGRADED, geo
+        given = [i for i in range(n) if i not in lost]
+        spares = given[r.k:]
+        stale = 3                        # an input data part in every goal here
+        maps = []
+        for fault in (None, (stale, [5], 777)):
+            if fault:
+                flip(eng, r, *fault)
+            got = []
+            for e in (eng, generic):
+                degraded(e)
+                e.sync()
+                got.append(out.cpu().numpy().view(L.Engine.STRIPE_STATE_DTYPE).reshape(r.n, r.pb).copy())
+            assert (got[0] == got[1]).all(), "fused and generic degraded maps differ"
+            maps.append(got[0])
+            if fault:
+                flip(eng, r, *fault)
+        assert not maps[0]["bad_rows"].any()
+        bad = maps[1]["bad_rows"] != 0
+        assert bad.sum() == r.n and bad[:, 5].all()
+        assert (maps[1]["suspect_part"][:, 5] == (stale if len(spares) >= 2 else -1)).all()
+        deg_bytes = r.n * (len(given) * (r.part_bytes + 4 * r.pb) + 8 * r.pb)
+        full_bytes = r.n * (n * (r.part_bytes + 4 * r.pb) + 8 * r.pb)
+        rate = lambda b, t: round(b / t / 1e12, 3)
+        print(json.dumps({"what": "check_stripe_map_degraded_dev", "goal": text, "lost": list(lost), "spares": len(spares),
+                          "chunks": r.n, "chunk_mib": NB * BLOCK >> 20, "fused_ms": round(t_fused * 1e3, 3),
+                          "generic_ms": round(t_generic * 1e3, 3), "full_parts_map_ms": round(t_full * 1e3, 3),
+                          "fused_alg_tb_s": rate(deg_bytes, t_fused), "fused_of_hbm": round(deg_bytes / t_fused / 1e12 / HBM_TBPS, 3),
+                          "generic_alg_tb_s": rate(deg_bytes, t_generic), "generic_of_hbm": round(deg_bytes / t_generic / 1e12 / HBM_TBPS, 3),
+                          "full_parts_alg_tb_s": rate(full_bytes, t_full), "full_parts_of_hbm": round(full_bytes / t_full / 1e12 / HBM_TBPS, 3),
+                          "fused_chunk_gib_s": round(r.n * NB * BLOCK / t_fused / 2**30, 1), "geometry": geo, "routes_agree": True,
+                          **info}), flush=True)
+        del r, out
+        torch.cuda.empty_cache()
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--chunks", type=int, default=16)
     ap.add_argument("--iters", type=int, default=20)
     ap.add_argument("--warmup", type=int, default=3)
+    ap.add_argument("--only", choices=["degraded"], default=None, help="run only the degraded-map rows")
     args = ap.parse_args()
     info = card()
     eng = L.Engine(0)
@@ -256,7 +327,10 @@ def main():
     stream = torch.cuda.Stream()        # the calls and the events share one stream
     st = stream.cuda_stream
     eng.set_deferred_verify(True)
-    for text in GOALS:
+    generic.set_deferred_verify(True)
+    degraded_rows(eng, generic, args, stream, info)
+    generic.set_deferred_verify(False)
+    for text in (GOALS if args.only is None else []):
         r = Resident(eng, text, args.chunks)
         out = torch.empty(12 * r.n, dtype=torch.uint8, device="cuda")
         t = timed(lambda: eng.check_stripes_dev(r.goal, r.n, NB, r.ptrs, r.stride, r.crc_ptrs, out.data_ptr(), stream=st),
