@@ -197,6 +197,10 @@ int lzgpu_debug_bitslice_rows(int k, const uint8_t *data, uint8_t *parity);
  * the 3 x 32 rebuilt bytes.  Runs the host build of the kernel's plane arithmetic: syndromes by Horner steps, the elimination's
  * products as masked XORs (doublings for A S0, A^2 S0 when lost[0] <= 3 and use_doublings != 0, else two more masked products). */
 int lzgpu_debug_bitslice_recover3(int k, const int *lost, const uint8_t *cols, int use_doublings, uint8_t *out);
+/* The host build of the per-stripe row derivation of lzgpu_repair_stripes (csrc/repair_rows.h): for goal (k, m) and the k input parts
+ * inputs[0 .. k-1] (ascending), rows[w * k + j] = the coefficient of input j in the block of part wanted[w], w < n_wanted.  Returns
+ * n_wanted, or LZGPU_ERR_ARG for bad arguments or a singular submatrix. */
+int lzgpu_debug_repair_rows(int k, int m, const uint8_t *inputs, const uint8_t *wanted, int n_wanted, uint8_t *rows);
 
 /* ---------------------------------------------------------------------------------------------
  * Engine context: one per (process, device).  Owns streams, pinned staging and device scratch.
@@ -497,6 +501,51 @@ int lzgpu_correct_stripes_degraded(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint3
 int lzgpu_correct_stripes_degraded_dev(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, uint32_t nb,
                                        void *const *d_parts, size_t part_stride, const void *const *d_part_crc,
                                        void *d_fix, int64_t *bad, void *stream);
+
+/* Stripe repair: the correction of lzgpu_correct_stripes_degraded, plus the blocks that fail their stored CRCs (bit rot, a torn write,
+ * a bad sector) rebuilt in place as erasures: errors-and-erasures decoding with the stored CRCs as the erasure locator.  With m
+ * checked rows the code can name one unknown bad block, or rebuild up to m blocks whose places are known; the CRCs give those places.
+ * So an xorN goal, a chunk with one spare, and a stripe of ec(8,2) with two rotten blocks are repaired, which the correction cannot do,
+ * and a rotten block no longer means dropping and re-replicating its whole part.
+ *   goal, n_chunks, nb, parts, part_stride, part_crc   exactly as in lzgpu_correct_stripes_degraded (layout, zero padding, any part may
+ *                    be NULL, at least k + 1 given, the inputs are the first k given parts), except that every given part must have
+ *                    stored CRCs (part_crc[i] != NULL), and the call refuses to run while CRCs are disabled (there is no locator
+ *                    then), as lzgpu_write_blocks* do.  Both refusals return LZGPU_ERR_ARG before anything is enqueued.
+ *   fix[c * pb + s]  one entry for every stripe.
+ * Rule, per stripe, with F = the given blocks of the stripe that fail their stored CRCs (the comparison the check makes):
+ *   1. F empty: the entry (first four fields) and the bytes written are those of lzgpu_correct_stripes_degraded for the same input
+ *      (CLEAN / CORRECTED / UNEXPLAINED; with no failing CRC the correction's gate always passes).
+ *   2. bad_rows == 0, F not empty: LZGPU_FIX_CRC_ONLY, nothing written.  The stripe agrees with itself, so a stored CRC is wrong (or
+ *      every block of the stripe is): for the caller to decide.
+ *   3. bad_rows != 0 and |F| <= given - k: every block in F is rebuilt from the first k given parts outside F, in ascending index
+ *      (what a one-stripe lzgpu_recover_chunks window with the parts of F unavailable returns).  The rebuilt blocks are written only
+ *      if every one of them matches its stored CRC: LZGPU_FIX_REBUILT, and the stored CRCs stay valid, so no CRC is rewritten.
+ *      Otherwise nothing is written and the status is LZGPU_FIX_CRC_CONFLICT (an input that is stale but has a valid CRC makes the
+ *      rebuild wrong; so does an erasure pattern whose matrix is singular).
+ *   4. bad_rows != 0 and |F| > given - k: LZGPU_FIX_CRC_CONFLICT, nothing written.
+ * A limit: a stale block with a valid CRC among the given parts that are not inputs survives a REBUILT stripe (the rebuild does not
+ * read it).  A second call finds F empty and treats that stripe under rule 1.
+ * lzgpu_repair_stripes returns LZGPU_ERR_CRC when a block still fails its stored CRC after the call (an entry is CRC_ONLY or
+ * CRC_CONFLICT), else LZGPU_ERR_INCONSISTENT when a stripe is left UNEXPLAINED, else LZGPU_OK.
+ * lzgpu_repair_stripes_dev enqueues the whole repair on `stream` and returns LZGPU_OK (or an argument or CUDA error) without waiting
+ * for the stream, unlike the other _dev calls given stored CRCs: every CRC failure is reported in the entries, which the caller reads
+ * from d_fix (device memory, 8-byte aligned) once the stream has passed the call.  Deferred verification has no effect on it.
+ * Alignment otherwise as in lzgpu_correct_stripes_dev.  lzgpu_debug_last_geometry reports the check's launch. */
+enum {   /* lzgpu_stripe_repair.status, beside LZGPU_FIX_CLEAN .. LZGPU_FIX_CRC_CONFLICT */
+	LZGPU_FIX_REBUILT = 4,      /* every block in crc_failed was rebuilt in place and now matches its stored CRC */
+	LZGPU_FIX_CRC_ONLY = 5      /* the stripe is a codeword, but the blocks in crc_failed fail their stored CRCs; nothing written */
+};
+typedef struct lzgpu_stripe_repair {
+	uint32_t bad_rows;      /* as lzgpu_stripe_state, before the call */
+	int32_t suspect_part;   /* as lzgpu_stripe_state, before the call (the code's locator) */
+	int32_t status;         /* LZGPU_FIX_* */
+	uint32_t crc;           /* CORRECTED: the new CRC of suspect_part's block; else 0 */
+	uint64_t crc_failed;    /* bit p: the given block of part p in this stripe failed its stored CRC before the call */
+} lzgpu_stripe_repair;      /* 24 bytes, 8-byte aligned */
+int lzgpu_repair_stripes(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, uint32_t nb,
+                         uint8_t *const *parts, size_t part_stride, const uint32_t *const *part_crc, lzgpu_stripe_repair *fix);
+int lzgpu_repair_stripes_dev(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, uint32_t nb,
+                             void *const *d_parts, size_t part_stride, const void *const *d_part_crc, void *d_fix, void *stream);
 
 /* Wire-format producer (SURVEY.md §8 f3): LIZ_CLTOCS_WRITE_DATA packet prefixes (src/protocol/cltocs.h:116-137) for
  * every block of every part of the encoded chunks, built on the GPU straight from the CRC array of

@@ -87,8 +87,13 @@ class LzStripeFix(C.Structure):
     _fields_ = [("bad_rows", C.c_uint32), ("suspect_part", C.c_int32), ("status", C.c_int32), ("crc", C.c_uint32)]
 
 
-# lzgpu_stripe_fix.status
-FIX_CLEAN, FIX_CORRECTED, FIX_UNEXPLAINED, FIX_CRC_CONFLICT = range(4)
+# lzgpu_stripe_fix.status (lzgpu_stripe_repair.status: also REBUILT and CRC_ONLY)
+FIX_CLEAN, FIX_CORRECTED, FIX_UNEXPLAINED, FIX_CRC_CONFLICT, FIX_REBUILT, FIX_CRC_ONLY = range(6)
+
+
+class LzStripeRepair(C.Structure):
+    _fields_ = [("bad_rows", C.c_uint32), ("suspect_part", C.c_int32), ("status", C.c_int32), ("crc", C.c_uint32),
+                ("crc_failed", C.c_uint64)]
 
 
 class LzBlockWrite(C.Structure):
@@ -111,6 +116,7 @@ SIGNATURES = {
     "lzgpu_plan_check_degraded": (_int, [_goalp, _vp, C.POINTER(LzCheckPlan)]),
     "lzgpu_debug_bitslice_rows": (_int, [_int, _vp, _vp]),
     "lzgpu_debug_bitslice_recover3": (_int, [_int, _vp, _vp, _int, _vp]),
+    "lzgpu_debug_repair_rows": (_int, [_int, _int, _vp, _vp, _int, _vp]),
     "lzgpu_goal_slice_type": (_int, [_goalp]),
     "lzgpu_goal_from_slice_type": (_int, [_int, _goalp]),
     "lzgpu_ref_part_index": (_int, [_goalp, _int]),
@@ -142,6 +148,8 @@ SIGNATURES = {
     "lzgpu_check_stripe_map_degraded_dev": (_int, [_vp, _goalp, _u32, _u32, _vp, _sz, _vp, _vp, _vp, _vp]),
     "lzgpu_correct_stripes_degraded": (_int, [_vp, _goalp, _u32, _u32, _vp, _sz, _vp, _vp, _vp]),
     "lzgpu_correct_stripes_degraded_dev": (_int, [_vp, _goalp, _u32, _u32, _vp, _sz, _vp, _vp, _vp, _vp]),
+    "lzgpu_repair_stripes": (_int, [_vp, _goalp, _u32, _u32, _vp, _sz, _vp, _vp]),
+    "lzgpu_repair_stripes_dev": (_int, [_vp, _goalp, _u32, _u32, _vp, _sz, _vp, _vp, _vp]),
     "lzgpu_write_data_prefixes": (_int, [_vp, _goalp, _u32, _u32, _vp, _sz, _vp, _u32, _vp]),
     "lzgpu_write_data_prefixes_dev": (_int, [_vp, _goalp, _u32, _u32, _vp, _sz, _vp, _u32, _vp, _vp]),
     "lzgpu_split_chunks": (_int, [_vp, _goalp, _u32, _u32, _vp, _sz, _vp, _sz]),

@@ -57,8 +57,12 @@ struct CheckLost {
 // for the whole unit: each lane keeps its row bits in a nibble per pass (at most 2048 items, four passes), and at the end of the unit
 // the warp OR-reduces each nibble and lane 0 stores the stripe's entry.  Units partition the stripes, so the map needs no memset and
 // no atomics.  E lost data positions (MAP only): slots 0 .. K-E-1 hold the given data parts, slot K - E + r parity row r.
-template <int R, bool CONSEC, bool MAP, int E = 0>
-__device__ __forceinline__ void fused_check_body(const CheckTmaps &tmaps, const CheckParams &p, uint32_t *map, const CheckLost *lost = nullptr) {
+// FAILED (lzgpu_repair_stripes, MAP only): a block that fails its stored CRC also sets bit part in failed[c pb + s] (zeroed by the
+// caller), so that every failing block of every stripe is known, not only the first of the batch.
+template <int R, bool CONSEC, bool MAP, int E = 0, bool FAILED = false>
+__device__ __forceinline__ void fused_check_body(const CheckTmaps &tmaps, const CheckParams &p, uint32_t *map, const CheckLost *lost = nullptr,
+                                                 unsigned long long *failed = nullptr) {
+	static_assert(!FAILED || MAP, "the failing blocks are recorded by the map form");
 	static_assert(E == 0 || (MAP && E < R), "a lost data part needs a spare row, and only the map form has one");
 	constexpr int W = 4;
 	constexpr uint32_t CPI = 32 / W;
@@ -248,7 +252,10 @@ __device__ __forceinline__ void fused_check_body(const CheckTmaps &tmaps, const 
 			const uint32_t s = stripe0 + (rr >> 2);
 			if (s < p.pb) {
 				const uint32_t want = __ldg(p.stored[slot] + static_cast<unsigned long long>(c) * p.pb + s);
-				if ((lin ^ p.zconst) != want) atomicMin(p.first_bad, (static_cast<unsigned long long>(c) * 64ull + p.part_id[slot]) * 1024ull + s);
+				if ((lin ^ p.zconst) != want) {
+					atomicMin(p.first_bad, (static_cast<unsigned long long>(c) * 64ull + p.part_id[slot]) * 1024ull + s);
+					if constexpr (FAILED) atomicOr(failed + static_cast<unsigned long long>(c) * p.pb + s, 1ull << p.part_id[slot]);
+				}
 			}
 		}
 	}
@@ -273,6 +280,20 @@ __global__ void __launch_bounds__(kCheckThreads, 1)
 fused_check_degraded_kernel(const __grid_constant__ CheckTmaps tmaps, const __grid_constant__ CheckParams p, uint32_t *map,
                             const __grid_constant__ CheckLost lost) {
 	fused_check_body<R, CONSEC, true, E>(tmaps, p, map, &lost);
+}
+
+// lzgpu_repair_stripes: the map kernels that also record every block that fails its stored CRC (failed[c * pb + s], bit part)
+template <int R, bool CONSEC>
+__global__ void __launch_bounds__(kCheckThreads, 1)
+fused_check_repair_kernel(const __grid_constant__ CheckTmaps tmaps, const __grid_constant__ CheckParams p, uint32_t *map, unsigned long long *failed) {
+	fused_check_body<R, CONSEC, true, 0, true>(tmaps, p, map, nullptr, failed);
+}
+
+template <int E, int R, bool CONSEC>
+__global__ void __launch_bounds__(kCheckThreads, 1)
+fused_check_repair_degraded_kernel(const __grid_constant__ CheckTmaps tmaps, const __grid_constant__ CheckParams p, uint32_t *map,
+                                   const __grid_constant__ CheckLost lost, unsigned long long *failed) {
+	fused_check_body<R, CONSEC, true, E, true>(tmaps, p, map, &lost, failed);
 }
 
 }  // namespace lzd

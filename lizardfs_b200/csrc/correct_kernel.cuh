@@ -15,6 +15,7 @@
 #pragma once
 #include "kernels_generic.cuh"
 #include "lzgpu.h"
+#include "repair_rows.h"
 
 namespace lzd {
 
@@ -135,6 +136,147 @@ __global__ void __launch_bounds__(256) correct_map_kernel(const CorrectArgs a) {
 		}
 		if (t == 0) a.fix[e] = lzgpu_stripe_fix{bad_rows, suspect, conflict ? LZGPU_FIX_CRC_CONFLICT : LZGPU_FIX_CORRECTED, crc};
 		__syncthreads();  // s_coef, s_lin and s_out are re-used by the next entry
+	}
+}
+
+// lzgpu_repair_stripes: the map entry and F = failed[e] (bit p: the block of part p fails its stored CRC, set by the check pass) give
+// the set X of blocks to rebuild: {suspect} when F is empty (the correction's rule 1, without its gate: no block fails), F itself
+// when the stripe is bad and |F| <= given - k (rule 3).  Every other entry only gets its status.  The inputs are the first k given
+// parts outside X, ascending; the rows of X over them come from repair_rows (repair_rows.h) in shared memory.  One pass over the
+// inputs per block of X (correct_read into 64 registers, then the CTA's CRC of the result): rule 3 stores nothing until every rebuilt
+// block has matched its stored CRC, so the last block stays in registers and the others are computed again for the store (2|X| - 1
+// passes, the later ones from L2).
+struct RepairArgs {
+	uint8_t *part[64];                 // part i of chunk 0; nullptr = not given
+	const uint32_t *crc[64];           // stored CRCs of part i, [chunk * pb + block] (every given part has them)
+	const uint32_t *map;               // the stripe map, two words per entry (bad_rows, suspect_part)
+	const unsigned long long *failed;  // F per entry
+	lzgpu_stripe_repair *fix;          // one entry per map entry
+	const uint32_t *tables;            // 4 * 256 slicing tables
+	unsigned long long part_stride, n_entries;
+	unsigned long long given;          // bit i: part i is given
+	uint32_t n_parts, k, pb;
+	uint32_t pow2[32];                 // x^(8 * 2^i) mod P
+	uint8_t gen[32 * 32];              // parity row r of the generator at gen[32 r]
+};
+
+// one block of X: thread t's 256 bytes of sum_j rows[j] * input j into acc (all-one rows by XOR), and the block's CRC in every thread
+__device__ __forceinline__ uint32_t repair_block(const RepairArgs &a, unsigned long long off, const uint8_t *in, const uint8_t *row, uint32_t (&acc)[64],
+                                                 CoefPlanes *s_coef, const uint32_t *s_tab, uint32_t shift, uint32_t *s_out) {
+	const unsigned t = threadIdx.x;
+	bool ones = true;
+	for (uint32_t j = 0; j < a.k; ++j) ones &= row[j] == 1;
+	if (t < a.k) coef_planes_set(s_coef[t], row[t]);
+	__syncthreads();
+#pragma unroll
+	for (int i = 0; i < 64; ++i) acc[i] = 0;
+	for (uint32_t j = 0; j < a.k; ++j) {
+		const uint8_t *blk = a.part[in[j]] + off;
+		if (ones) correct_read<false, 1>(blk, acc, s_coef[0], s_tab);
+		else correct_read<false, 2>(blk, acc, s_coef[j], s_tab);
+	}
+	uint32_t st = 0;
+#pragma unroll
+	for (int i = 0; i < 64; ++i) st = crc_step_word(st, acc[i], s_tab);
+	correct_crc_part(st, shift, s_out);
+	__syncthreads();
+	uint32_t crc = kCrcZeroBlock64K;
+#pragma unroll
+	for (int w = 0; w < 8; ++w) crc ^= s_out[w];
+	__syncthreads();  // s_coef and s_out are re-used by the next block
+	return crc;
+}
+
+__device__ __forceinline__ void repair_store(uint8_t *blk, const uint32_t (&acc)[64]) {
+	uint4 *dst = reinterpret_cast<uint4 *>(blk) + threadIdx.x * 16;
+#pragma unroll
+	for (int i = 0; i < 16; ++i) dst[i] = make_uint4(acc[4 * i], acc[4 * i + 1], acc[4 * i + 2], acc[4 * i + 3]);
+}
+
+struct CtaSync {
+	__device__ void operator()() const { __syncthreads(); }
+};
+
+// The rule of one entry without its data (host and device): the status, and in *x the blocks to rebuild (0: the status is final).
+// spare = given parts - k.  REBUILT and CORRECTED are provisional until the rebuilt blocks exist (rule 3: until their CRCs match).
+LZ_HD inline int repair_rule(uint32_t bad_rows, int suspect, unsigned long long f, int spare, unsigned long long *x) {
+	*x = 0;
+	if (!f) {
+		if (!bad_rows) return LZGPU_FIX_CLEAN;
+		if (suspect < 0) return LZGPU_FIX_UNEXPLAINED;
+		*x = 1ull << suspect;
+		return LZGPU_FIX_CORRECTED;
+	}
+	if (!bad_rows) return LZGPU_FIX_CRC_ONLY;
+	int n = 0;
+	for (unsigned long long b = f; b; b &= b - 1) ++n;
+	if (n > spare) return LZGPU_FIX_CRC_CONFLICT;
+	*x = f;
+	return LZGPU_FIX_REBUILT;
+}
+
+__global__ void __launch_bounds__(256) repair_map_kernel(const RepairArgs a) {
+	__shared__ uint32_t s_tab[1024];
+	__shared__ CoefPlanes s_coef[32];
+	__shared__ GfTables s_gf;
+	__shared__ uint8_t s_mat[32][64];
+	__shared__ uint8_t s_rows[32 * 32];
+	__shared__ uint8_t s_in[32], s_want[64];
+	__shared__ uint32_t s_pivot, s_out[8];
+	const unsigned t = threadIdx.x;
+	const int spare = __popcll(a.given) - static_cast<int>(a.k);
+	bool ready = false;
+	uint32_t shift = 0;
+	for (unsigned long long e = blockIdx.x; e < a.n_entries; e += gridDim.x) {
+		const uint32_t bad_rows = a.map[2 * e];
+		const int suspect = static_cast<int>(a.map[2 * e + 1]);
+		const unsigned long long f = a.failed[e];
+		unsigned long long x;
+		int status = repair_rule(bad_rows, suspect, f, spare, &x);
+		if (!x) {
+			if (t == 0) a.fix[e] = lzgpu_stripe_repair{bad_rows, suspect, status, 0u, f};
+			continue;
+		}
+		if (!ready) {  // first entry with work: tables and this thread's shift
+			for (unsigned i = t; i < 1024; i += 256) s_tab[i] = a.tables[i];
+			if (t == 0) gf_tables_build(s_gf);
+			shift = crc_xpow_bytes_dev(256u * (255u - t), a.pow2);
+			ready = true;
+		}
+		if (t == 0) {
+			uint32_t ni = 0, nw = 0;
+			for (uint32_t p = 0; p < a.n_parts; ++p) {
+				if (!((a.given >> p) & 1ull)) continue;
+				if ((x >> p) & 1ull) s_want[nw++] = static_cast<uint8_t>(p);
+				else if (ni < a.k) s_in[ni++] = static_cast<uint8_t>(p);
+			}
+		}
+		__syncthreads();
+		const uint32_t nw = static_cast<uint32_t>(__popcll(x));
+		const unsigned long long off = (e / a.pb) * a.part_stride + (e % a.pb) * 65536ull;
+		uint32_t crc = 0;
+		if (!repair_rows(a.k, a.gen, s_in, s_want, nw, s_gf, s_mat, &s_pivot, s_rows, t, 256u, CtaSync())) {
+			status = f ? LZGPU_FIX_CRC_CONFLICT : LZGPU_FIX_UNEXPLAINED;  // a singular pattern: nothing rebuilt
+		} else {
+			uint32_t acc[64];
+			bool match = true;
+			for (uint32_t w = 0; w < nw && match; ++w) {
+				crc = repair_block(a, off, s_in, s_rows + 32 * w, acc, s_coef, s_tab, shift, s_out);
+				match = !f || crc == a.crc[s_want[w]][e];  // e = chunk * pb + block
+			}
+			if (!match) {
+				status = LZGPU_FIX_CRC_CONFLICT;
+			} else {
+				repair_store(a.part[s_want[nw - 1]] + off, acc);
+				for (uint32_t w = 0; w + 1 < nw; ++w) {
+					repair_block(a, off, s_in, s_rows + 32 * w, acc, s_coef, s_tab, shift, s_out);
+					repair_store(a.part[s_want[w]] + off, acc);
+				}
+			}
+			if (f) crc = 0;  // REBUILT: the blocks match the CRCs the caller already has
+		}
+		if (t == 0) a.fix[e] = lzgpu_stripe_repair{bad_rows, suspect, status, status == LZGPU_FIX_CORRECTED ? crc : 0u, f};
+		__syncthreads();  // s_in, s_want and s_rows are re-used by the next entry
 	}
 }
 

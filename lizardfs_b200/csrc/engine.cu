@@ -862,12 +862,15 @@ static int verify_part(lzgpu_ctx *ctx, const void *d_part, uint32_t n_chunks, ui
 // The stored CRCs of the parts one enqueue reads: the first n_read given parts of d_parts[0 .. n-1] (the reference checks each block
 // it receives, read_operation_executor.cc:257-269; a surplus part is never requested).  It decides whether they are verified, by which
 // route, and how the ticket's words are encoded.  In the CRC-disabled build mode a stored CRC is valid iff it is the constant: begin()
-// checks that before either route runs, and the kernels get no CRCs.
+// checks that before either route runs, and the kernels get no CRCs.  failed (lzgpu_repair_stripes, CRCs enabled): every failing block
+// sets the bit of its part in its word of failed[n_chunks * pb] (zeroed here), and nothing else reports a mismatch: the result words
+// are a stream-ordered temporary, no ticket is armed and nothing waits for the stream.
 class InputCrcs {
 public:
 	InputCrcs(lzgpu_ctx *ctx, cudaStream_t st, VerifyTicket *tk, const void *const *d_parts, const void *const *d_part_crc, int n, int n_read,
-	          uint32_t n_chunks, uint32_t pb, size_t stride)
-	    : ctx_(ctx), st_(st), tk_(tk), parts_(d_parts), crc_(d_part_crc), n_(n), n_chunks_(n_chunks), pb_(pb), stride_(stride), tmp_(ctx, st) {
+	          uint32_t n_chunks, uint32_t pb, size_t stride, unsigned long long *failed = nullptr)
+	    : ctx_(ctx), st_(st), tk_(tk), parts_(d_parts), crc_(d_part_crc), n_(n), n_chunks_(n_chunks), pb_(pb), stride_(stride), failed_(failed),
+	      tmp_(ctx, st), words_(ctx, st) {
 		for (int i = 0, used = 0; i < n && used < n_read; ++i)
 			if (d_parts[i]) {
 				++used;
@@ -877,13 +880,21 @@ public:
 	bool any() const { return read_ != 0; }
 	// arms the ticket when a part read has stored CRCs (in the CRC-disabled mode, also checks them)
 	int begin() {
+		if (failed_) {
+			int rc = words_.alloc(sizeof(unsigned long long) * n_);
+			if (rc) return rc;
+			CUDA_TRY(cudaMemsetAsync(words_.p, 0xff, sizeof(unsigned long long) * n_, st_));
+			CUDA_TRY(cudaMemsetAsync(failed_, 0, sizeof(unsigned long long) * n_chunks_ * pb_, st_));
+			return LZGPU_OK;
+		}
 		if (!any()) return LZGPU_OK;
 		int rc = tk_->arm(ctx_, st_);
 		return (rc || lzgpu_crc_enabled()) ? rc : verify_each();
 	}
 	// the fused route's CRC array (nullptr: nothing left to verify) and its result word
 	const void *const *for_kernels() const { return any() && lzgpu_crc_enabled() ? crc_ : nullptr; }
-	unsigned long long *fused_word() const { return tk_->word(0); }
+	unsigned long long *fused_word() const { return word(0); }
+	unsigned long long *failed() const { return failed_; }
 	// the generic route: every part read, part by part, before the kernels that read them
 	int verify() {
 		if (!for_kernels()) return LZGPU_OK;
@@ -892,15 +903,24 @@ public:
 	}
 	// fused: the fused route ran with for_kernels()
 	int publish(bool fused) {
-		if (!any()) return LZGPU_OK;
+		if (!any() || failed_) return LZGPU_OK;
 		return fused && for_kernels() ? tk_->publish_fused() : tk_->publish_per_part(n_, pb_);
 	}
 
 private:
+	unsigned long long *word(int i) const { return failed_ ? static_cast<unsigned long long *>(words_.p) + i : tk_->word(i); }
 	int verify_each() {
 		int rc;
-		for (int i = 0; i < n_; ++i)
-			if (((read_ >> i) & 1ull) && (rc = verify_part(ctx_, parts_[i], n_chunks_, pb_, stride_, crc_[i], tmp_.p, tk_->word(i), st_))) return rc;
+		const unsigned long long nblk = static_cast<unsigned long long>(n_chunks_) * pb_;
+		for (int i = 0; i < n_; ++i) {
+			if (!((read_ >> i) & 1ull)) continue;
+			if ((rc = verify_part(ctx_, parts_[i], n_chunks_, pb_, stride_, crc_[i], tmp_.p, word(i), st_))) return rc;
+			if (!failed_) continue;
+			crc_failed_kernel<<<grid_for(ctx_, nblk, 256, 4), 256, 0, st_>>>(static_cast<const uint32_t *>(tmp_.p), static_cast<const uint32_t *>(crc_[i]),
+			                                                               nblk, 1ull << i, failed_);
+			CUDA_TRY(cudaGetLastError());
+			ctx_->stats.kernel_launches++;
+		}
 		return LZGPU_OK;
 	}
 	lzgpu_ctx *ctx_;
@@ -911,8 +931,9 @@ private:
 	int n_;
 	uint32_t n_chunks_, pb_;
 	size_t stride_;
+	unsigned long long *failed_;
 	unsigned long long read_ = 0;
-	TmpBuf tmp_;
+	TmpBuf tmp_, words_;
 };
 
 // enqueue the whole degraded read on `st` without synchronising; *tk is armed when stored CRCs of the parts read are verified
@@ -1154,9 +1175,11 @@ static int check_args(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t nb, const
 }
 
 // enqueue the whole check on `st` (arguments validated by check_args); *tk is armed when stored CRCs are verified.  map: d_verdict is
-// the stripe map (lzgpu_check_stripe_map) instead of the verdicts.
+// the stripe map (lzgpu_check_stripe_map) instead of the verdicts.  d_failed (map only, lzgpu_repair_stripes): the failing blocks of
+// every stripe, one word per entry (InputCrcs), instead of the first mismatch on *tk.
 static int check_enqueue(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, uint32_t nb, const void *const *d_parts, size_t part_stride,
-                         const void *const *d_part_crc, void *d_verdict, cudaStream_t st, VerifyTicket *tk, bool map = false) {
+                         const void *const *d_part_crc, void *d_verdict, cudaStream_t st, VerifyTicket *tk, bool map = false,
+                         unsigned long long *d_failed = nullptr) {
 	const int k = goal->k, m = goal->m, n = k + m;
 	const uint32_t B = LZGPU_BLOCK_SIZE;
 	const uint32_t pb = (nb + k - 1) / k;
@@ -1199,7 +1222,7 @@ static int check_enqueue(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chun
 		for (uint32_t i = 0; i < la.n_rows; ++i)
 			for (int x = 0; x < lost; ++x) elim[i * lost + x] = la.coef[32 * i + k - lost + x];
 
-	InputCrcs crcs(ctx, st, tk, d_parts, d_part_crc, n, n, n_chunks, pb, part_stride);  // every given part is read
+	InputCrcs crcs(ctx, st, tk, d_parts, d_part_crc, n, n, n_chunks, pb, part_stride, d_failed);  // every given part is read
 	int rc = crcs.begin();
 	if (rc) return rc;
 	// first_bad_stripe of every chunk starts above any stripe; the check kernels lower it, locate_kernel writes the whole verdict.  The
@@ -1208,7 +1231,7 @@ static int check_enqueue(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chun
 	if (!map) CUDA_TRY(cudaMemsetAsync(d_verdict, 0x7f, static_cast<size_t>(n_chunks) * sizeof(lzgpu_stripe_verdict), st));
 
 	rc = lz_fused_check(ctx, goal, n_chunks, nb, d_parts, part_stride, crcs.for_kernels(), d_verdict, st, crcs.fused_word(), map,
-	                    lost ? elim : nullptr);
+	                    lost ? elim : nullptr, crcs.failed());
 	const bool fused = rc != LZGPU_NOT_HANDLED;
 	if (fused && rc) return rc;
 	if (!fused) {
@@ -1287,9 +1310,11 @@ extern "C" int lzgpu_check_stripe_map_degraded_dev(lzgpu_ctx *ctx, const lzgpu_g
 	return check_dev(ctx, goal, n_chunks, nb, d_parts, part_stride, d_part_crc, d_map, bad, stream, true, true);
 }
 
-// the host-pointer calls: out = lzgpu_stripe_verdict[n_chunks], or (map) lzgpu_stripe_state[n_chunks * pb]
+// the host-pointer calls: out = lzgpu_stripe_verdict[n_chunks], or (map) lzgpu_stripe_state[n_chunks * pb]; failed (map only,
+// lzgpu_repair_stripes): the failing blocks of every stripe, n_chunks * pb words, instead of the first mismatch
 static int check_host(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, uint32_t nb, const uint8_t *const *parts,
-                      size_t part_stride, const uint32_t *const *part_crc, void *out, int64_t *bad, bool map, bool degraded = false) {
+                      size_t part_stride, const uint32_t *const *part_crc, void *out, int64_t *bad, bool map, bool degraded = false,
+                      uint64_t *failed = nullptr) {
 	int rc = check_args(ctx, goal, nb, reinterpret_cast<const void *const *>(parts), nullptr, out, false, degraded);
 	if (rc) return rc;
 	if (n_chunks == 0) return LZGPU_OK;
@@ -1298,6 +1323,7 @@ static int check_host(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks,
 	const uint32_t pb = (nb + k - 1) / k;
 	const size_t part_bytes = static_cast<size_t>(pb) * B;
 	const size_t out_per_chunk = map ? pb * sizeof(lzgpu_stripe_state) : sizeof(lzgpu_stripe_verdict);
+	const size_t failed_per_chunk = failed ? pb * sizeof(uint64_t) : 0;
 	uint8_t *const out_bytes = static_cast<uint8_t *>(out);
 	if (part_stride < part_bytes) { lz_set_error("check_stripes: part_stride too small"); return LZGPU_ERR_ARG; }
 	GivenParts in(parts, part_crc, n, part_stride, pb);
@@ -1305,24 +1331,30 @@ static int check_host(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks,
 	DeviceGuard g(ctx->device);
 	AutoPin pin(ctx);
 	pin.add(out, static_cast<size_t>(n_chunks) * out_per_chunk);
+	if (failed) pin.add(failed, static_cast<size_t>(n_chunks) * failed_per_chunk);
 	const uint32_t tile = static_cast<uint32_t>(std::max<size_t>(1, std::min<size_t>(n_chunks, (2 * kHostTileBytes) / (part_bytes * in.n_given))));
 	void *d_ver[kHostSlots];
 	const int n_slots = n_chunks > tile ? kHostSlots : 1;
 	if ((rc = in.prepare(ctx, pin, n_chunks, tile, n_slots, in.n_given))) return rc;
 	for (int s = 0; s < n_slots; ++s)
-		if ((rc = lz_scratch(ctx, kScratchPar0 + s, static_cast<size_t>(tile) * out_per_chunk, &d_ver[s]))) return rc;
+		if ((rc = lz_scratch(ctx, kScratchPar0 + s, static_cast<size_t>(tile) * (out_per_chunk + failed_per_chunk), &d_ver[s]))) return rc;
 	// a stored-CRC mismatch does not stop the pipeline: every chunk gets its verdict (its map)
 	rc = run_tiles(ctx, n_chunks, tile, n_slots, bad, [&](int s, size_t c0, size_t nc, cudaStream_t st, VerifyTicket *tk) -> int {
 		GivenParts::Tile t;
 		int rc = in.stage(ctx, s, c0, nc, st, t);
 		if (rc) return rc;
+		unsigned long long *d_failed = failed ? reinterpret_cast<unsigned long long *>(static_cast<uint8_t *>(d_ver[s]) + tile * out_per_chunk) : nullptr;
 		{
 			BatchTimer timer(ctx, st, check_alg_bytes(goal, static_cast<uint32_t>(nc), nb, t.dp.data(), t.crcs(), map));
-			rc = check_enqueue(ctx, goal, static_cast<uint32_t>(nc), nb, t.dp.data(), part_bytes, t.crcs(), d_ver[s], st, tk, map);
+			rc = check_enqueue(ctx, goal, static_cast<uint32_t>(nc), nb, t.dp.data(), part_bytes, t.crcs(), d_ver[s], st, tk, map, d_failed);
 		}
 		if (rc) return rc;
 		CUDA_TRY(cudaMemcpyAsync(out_bytes + c0 * out_per_chunk, d_ver[s], nc * out_per_chunk, cudaMemcpyDeviceToHost, st));
 		ctx->stats.bytes_d2h += nc * out_per_chunk;
+		if (failed) {
+			CUDA_TRY(cudaMemcpyAsync(failed + c0 * pb, d_failed, nc * failed_per_chunk, cudaMemcpyDeviceToHost, st));
+			ctx->stats.bytes_d2h += nc * failed_per_chunk;
+		}
 		return LZGPU_OK;
 	}, true);
 	if (rc) return rc;
@@ -1568,6 +1600,196 @@ extern "C" int lzgpu_correct_stripes_degraded(lzgpu_ctx *ctx, const lzgpu_goal *
                                               size_t part_stride, const uint32_t *const *part_crc, lzgpu_stripe_fix *fix, int64_t *bad) {
 	NvtxScope nvtx_scope("lzgpu::correct_stripes_degraded");
 	return correct_host(ctx, goal, n_chunks, nb, parts, part_stride, part_crc, fix, bad, true);
+}
+
+// ------------------------------------------------------------------------------------------------
+// stripe repair: the degraded map with every block that fails its stored CRC, then the correction's rule or those blocks rebuilt as
+// erasures (repair_map_kernel, correct_kernel.cuh)
+// ------------------------------------------------------------------------------------------------
+static_assert(sizeof(lzgpu_stripe_repair) == 24 && alignof(lzgpu_stripe_repair) == 8, "repair entries as repair_map_kernel writes them");
+
+// the arguments of lzgpu_correct_stripes_degraded, and the repair's own refusals (before anything is enqueued)
+static int repair_args(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t nb, const void *const *parts, const void *const *part_crc, const void *fix,
+                       bool dev) {
+	int rc = check_args(ctx, goal, nb, parts, part_crc, fix, dev, true);
+	if (rc) return rc;
+	if (!lzgpu_crc_enabled()) { lz_set_error("repair_stripes: CRCs are disabled, so nothing locates the blocks to rebuild"); return LZGPU_ERR_ARG; }
+	for (int i = 0; i < goal->k + goal->m; ++i)
+		if (parts[i] && (!part_crc || !part_crc[i])) { lz_set_error("repair_stripes: part %d is given without stored CRCs", i); return LZGPU_ERR_ARG; }
+	if (dev && (reinterpret_cast<uintptr_t>(fix) & 7)) { lz_set_error("repair_stripes: fix is not 8-byte aligned"); return LZGPU_ERR_ARG; }
+	return LZGPU_OK;
+}
+
+// the goal's part of the kernel arguments: the given parts and the generator's parity rows
+static void repair_table(const lzgpu_goal *goal, unsigned long long given, RepairArgs &a) {
+	uint8_t rows[LZGPU_MAX_PARITY * LZGPU_MAX_DATA];
+	goal_parity_rows(goal, rows);
+	for (int r = 0; r < goal->m; ++r) std::memcpy(a.gen + 32 * r, rows + r * goal->k, goal->k);
+	a.given = given;
+	a.n_parts = goal->k + goal->m;
+	a.k = goal->k;
+}
+
+// repair_map_kernel over n_entries entries (pb per chunk) on `st`; a carries the table (repair_table) and the part and CRC pointers
+static int repair_enqueue(lzgpu_ctx *ctx, RepairArgs &a, unsigned long long n_entries, uint32_t pb, size_t part_stride, const void *d_map,
+                          const void *d_failed, void *d_fix, cudaStream_t st) {
+	a.map = static_cast<const uint32_t *>(d_map);
+	a.failed = static_cast<const unsigned long long *>(d_failed);
+	a.fix = static_cast<lzgpu_stripe_repair *>(d_fix);
+	a.tables = ctx->d_crc_tables;
+	a.part_stride = part_stride;
+	a.n_entries = n_entries;
+	a.pb = pb;
+	uint32_t x = 0x00800000u;  // x^8
+	for (int i = 0; i < 32; ++i) {
+		a.pow2[i] = x;
+		x = lz::crc_mulmod(x, x);
+	}
+	repair_map_kernel<<<grid_for(ctx, n_entries * 256, 256, 2), 256, 0, st>>>(a);
+	CUDA_TRY(cudaGetLastError());
+	ctx->stats.kernel_launches++;
+	return LZGPU_OK;
+}
+
+extern "C" int lzgpu_repair_stripes_dev(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, uint32_t nb, void *const *d_parts,
+                                        size_t part_stride, const void *const *d_part_crc, void *d_fix, void *stream) {
+	NvtxScope nvtx_scope("lzgpu::repair_stripes_dev");
+	int rc = repair_args(ctx, goal, nb, d_parts, d_part_crc, d_fix, true);
+	if (rc || n_chunks == 0) return rc;
+	const uint32_t pb = (nb + goal->k - 1) / goal->k;
+	const unsigned long long entries = static_cast<unsigned long long>(n_chunks) * pb;
+	RepairArgs a{};
+	unsigned long long given = 0;
+	for (int i = 0; i < goal->k + goal->m; ++i) {
+		a.part[i] = static_cast<uint8_t *>(d_parts[i]);
+		a.crc[i] = d_parts[i] ? static_cast<const uint32_t *>(d_part_crc[i]) : nullptr;
+		given |= d_parts[i] ? 1ull << i : 0ull;
+	}
+	repair_table(goal, given, a);
+	DeviceGuard g(ctx->device);
+	cudaStream_t st = stream ? static_cast<cudaStream_t>(stream) : ctx->stream;
+	// the map's bytes and one entry per stripe; the rebuilt blocks are not counted (the host does not know them here)
+	BatchTimer timer(ctx, st, check_alg_bytes(goal, n_chunks, nb, d_parts, d_part_crc, true) + entries * sizeof(lzgpu_stripe_repair));
+	TmpBuf map(ctx, st), failed(ctx, st);
+	if ((rc = map.alloc(entries * sizeof(lzgpu_stripe_state))) || (rc = failed.alloc(entries * sizeof(uint64_t))) ||
+	    (rc = check_enqueue(ctx, goal, n_chunks, nb, d_parts, part_stride, d_part_crc, map.p, st, nullptr, true,
+	                        static_cast<unsigned long long *>(failed.p))))
+		return rc;
+	return repair_enqueue(ctx, a, entries, pb, part_stride, map.p, failed.p, d_fix, st);
+}
+
+// The host-pointer repair, phase 2: the stripes `todo` (map indices with blocks to rebuild) gathered into one-stripe "chunks" as in
+// correct_host_stripes, tile by tile, through repair_map_kernel with the map entries and failing blocks the check found; the entries
+// go to fix[], the rewritten blocks back into the caller's parts.
+static int repair_host_stripes(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t pb, uint8_t *const *parts, size_t part_stride,
+                               const uint32_t *const *part_crc, const lzgpu_stripe_state *map, const uint64_t *failed,
+                               const std::vector<size_t> &todo, lzgpu_stripe_repair *fix) {
+	const int n = goal->k + goal->m;
+	const size_t B = LZGPU_BLOCK_SIZE;
+	unsigned long long given = 0;
+	int n_given = 0;
+	for (int i = 0; i < n; ++i)
+		if (parts[i]) {
+			given |= 1ull << i;
+			++n_given;
+		}
+	RepairArgs a{};
+	repair_table(goal, given, a);
+	std::lock_guard<std::mutex> lk(ctx->mu);
+	DeviceGuard g(ctx->device);
+	const size_t tile = std::max<size_t>(1, std::min<size_t>(todo.size(), (2 * kHostTileBytes) / (B * n_given)));
+	const size_t entry_bytes = sizeof(lzgpu_stripe_state) + sizeof(uint64_t) + sizeof(lzgpu_stripe_repair);
+	void *d_in, *d_crc, *d_entries;
+	int rc;
+	if ((rc = lz_scratch(ctx, kScratchIn0, tile * B * n, &d_in)) || (rc = lz_scratch(ctx, kScratchCrc0, tile * 4 * n, &d_crc)) ||
+	    (rc = lz_scratch(ctx, kScratchPar0, tile * entry_bytes, &d_entries)))
+		return rc;
+	void *d_failed = d_entries;  // 8-byte words first: every part of d_entries stays 8-byte aligned
+	void *d_fix = static_cast<uint8_t *>(d_entries) + tile * sizeof(uint64_t);
+	void *d_map = static_cast<uint8_t *>(d_fix) + tile * sizeof(lzgpu_stripe_repair);
+	for (int i = 0; i < n; ++i) {
+		a.part[i] = parts[i] ? static_cast<uint8_t *>(d_in) + tile * B * i : nullptr;
+		a.crc[i] = parts[i] ? static_cast<const uint32_t *>(d_crc) + tile * i : nullptr;
+	}
+	std::vector<uint32_t> h_crc(tile * n);
+	std::vector<lzgpu_stripe_state> h_map(tile);
+	std::vector<uint64_t> h_failed(tile);
+	std::vector<lzgpu_stripe_repair> h_fix(tile);
+	cudaStream_t st = ctx->slot_stream[0];
+	for (size_t t0 = 0; t0 < todo.size(); t0 += tile) {
+		const size_t nt = std::min(tile, todo.size() - t0);
+		for (size_t j = 0; j < nt; ++j) {
+			const size_t e = todo[t0 + j], c = e / pb, s = e % pb;
+			for (int i = 0; i < n; ++i) {
+				if (!parts[i]) continue;
+				CUDA_TRY(cudaMemcpyAsync(a.part[i] + j * B, parts[i] + c * part_stride + s * B, B, cudaMemcpyHostToDevice, st));
+				h_crc[tile * i + j] = part_crc[i][e];
+			}
+			h_map[j] = map[e];
+			h_failed[j] = failed[e];
+		}
+		ctx->stats.bytes_h2d += nt * n_given * B;
+		CUDA_TRY(cudaMemcpyAsync(d_crc, h_crc.data(), tile * 4 * n, cudaMemcpyHostToDevice, st));
+		CUDA_TRY(cudaMemcpyAsync(d_map, h_map.data(), nt * sizeof(lzgpu_stripe_state), cudaMemcpyHostToDevice, st));
+		CUDA_TRY(cudaMemcpyAsync(d_failed, h_failed.data(), nt * sizeof(uint64_t), cudaMemcpyHostToDevice, st));
+		{
+			BatchTimer timer(ctx, st, nt * (n_given * B + entry_bytes));
+			if ((rc = repair_enqueue(ctx, a, nt, 1, B, d_map, d_failed, d_fix, st))) return rc;
+		}
+		CUDA_TRY(cudaMemcpyAsync(h_fix.data(), d_fix, nt * sizeof(lzgpu_stripe_repair), cudaMemcpyDeviceToHost, st));
+		CUDA_TRY(cudaStreamSynchronize(st));
+		for (size_t j = 0; j < nt; ++j) {
+			const size_t e = todo[t0 + j], c = e / pb, s = e % pb;
+			fix[e] = h_fix[j];
+			unsigned long long written = 0;
+			if (h_fix[j].status == LZGPU_FIX_CORRECTED) written = 1ull << h_fix[j].suspect_part;
+			if (h_fix[j].status == LZGPU_FIX_REBUILT) written = h_fix[j].crc_failed;
+			for (; written; written &= written - 1) {
+				const int p = __builtin_ctzll(written);
+				CUDA_TRY(cudaMemcpyAsync(parts[p] + c * part_stride + s * B, a.part[p] + j * B, B, cudaMemcpyDeviceToHost, st));
+				ctx->stats.bytes_d2h += B;
+			}
+		}
+		CUDA_TRY(cudaStreamSynchronize(st));
+	}
+	return LZGPU_OK;
+}
+
+extern "C" int lzgpu_repair_stripes(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, uint32_t nb, uint8_t *const *parts,
+                                    size_t part_stride, const uint32_t *const *part_crc, lzgpu_stripe_repair *fix) {
+	NvtxScope nvtx_scope("lzgpu::repair_stripes");
+	int rc = repair_args(ctx, goal, nb, reinterpret_cast<const void *const *>(parts), reinterpret_cast<const void *const *>(part_crc), fix, false);
+	if (rc) return rc;
+	if (n_chunks == 0) return LZGPU_OK;
+	// phase 1: the map and the failing blocks of the whole batch through the check's tile pipeline
+	const uint32_t pb = (nb + goal->k - 1) / goal->k;
+	const size_t entries = static_cast<size_t>(n_chunks) * pb;
+	std::vector<lzgpu_stripe_state> map(entries);
+	std::vector<uint64_t> failed(entries);
+	rc = check_host(ctx, goal, n_chunks, nb, parts, part_stride, part_crc, map.data(), nullptr, true, true, failed.data());
+	if (rc != LZGPU_OK && rc != LZGPU_ERR_INCONSISTENT) return rc;
+	int spare = -goal->k;
+	for (int i = 0; i < goal->k + goal->m; ++i) spare += parts[i] ? 1 : 0;
+	std::vector<size_t> todo;
+	for (size_t e = 0; e < entries; ++e) {
+		unsigned long long x;
+		const int status = repair_rule(map[e].bad_rows, map[e].suspect_part, failed[e], spare, &x);
+		fix[e] = lzgpu_stripe_repair{map[e].bad_rows, map[e].suspect_part, status, 0u, failed[e]};
+		if (x) todo.push_back(e);
+	}
+	// phase 2: only the stripes with blocks to rebuild travel again
+	if (!todo.empty() && (rc = repair_host_stripes(ctx, goal, pb, parts, part_stride, part_crc, map.data(), failed.data(), todo, fix))) return rc;
+	for (size_t e = 0; e < entries; ++e)
+		if (fix[e].status == LZGPU_FIX_CRC_ONLY || fix[e].status == LZGPU_FIX_CRC_CONFLICT) {
+			lz_set_error("repair_stripes: chunk %zu stripe %zu: a block still fails its stored CRC (status %d)", e / pb, e % pb, fix[e].status);
+			return LZGPU_ERR_CRC;
+		}
+	for (size_t e = 0; e < entries; ++e)
+		if (fix[e].status == LZGPU_FIX_UNEXPLAINED) {
+			lz_set_error("repair_stripes: chunk %zu stripe %zu is not a codeword and no single part explains it", e / pb, e % pb);
+			return LZGPU_ERR_INCONSISTENT;
+		}
+	return LZGPU_OK;
 }
 
 // ------------------------------------------------------------------------------------------------

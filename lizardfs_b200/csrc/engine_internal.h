@@ -196,10 +196,11 @@ int lz_fused_convert(lzgpu_ctx *ctx, const lzgpu_goal *src, const lzgpu_goal *ds
 // parts are the checked rows.  Lowers d_verdict's first_bad_stripe words (3 ints per chunk); stored-CRC mismatches as in lz_fused_recover.
 // map: d_verdict is the stripe map instead (lzgpu_stripe_state[n_chunks * pb]); every entry gets its bad_rows and suspect_part = -1.
 // A NULL data part (map only, lzgpu_check_stripe_map_degraded): elim = C[i][x], (R - E) x E, spare row E + i against input row x of
-// the R given parity rows; bad_rows then has the bits of the spare rows only.
+// the R given parity rows; bad_rows then has the bits of the spare rows only.  d_failed (map only, lzgpu_repair_stripes): one zeroed
+// word per entry, in which every block that fails its stored CRC sets the bit of its part.
 int lz_fused_check(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, uint32_t nb, const void *const *d_parts, size_t part_stride,
                    const void *const *d_part_crc, void *d_verdict, cudaStream_t st, unsigned long long *d_first_bad, bool map,
-                   const uint8_t *elim);
+                   const uint8_t *elim, unsigned long long *d_failed = nullptr);
 // CRC of 64 KiB blocks: block (c, b) at base + c*chunk_stride + b*65536, out[c*out_chunk_stride + b]
 int lz_fused_crc(lzgpu_ctx *ctx, const void *base, unsigned long long n_blocks, unsigned long long blocks_per_chunk,
                  unsigned long long chunk_stride, void *out, unsigned long long out_chunk_stride, cudaStream_t st);

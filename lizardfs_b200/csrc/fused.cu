@@ -184,6 +184,22 @@ static int set_all_recover_attrs() {
 	CUDA_TRY(cudaFuncSetAttribute(fused_check_degraded_kernel<1, 2, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kRecoverSmemCapBig));
 	CUDA_TRY(cudaFuncSetAttribute(fused_check_degraded_kernel<1, 3, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kRecoverSmemCapBig));
 	CUDA_TRY(cudaFuncSetAttribute(fused_check_degraded_kernel<2, 3, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kRecoverSmemCapBig));
+	CUDA_TRY(cudaFuncSetAttribute(fused_check_repair_kernel<1, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kRecoverSmemCapBig));
+	CUDA_TRY(cudaFuncSetAttribute(fused_check_repair_kernel<2, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kRecoverSmemCapBig));
+	CUDA_TRY(cudaFuncSetAttribute(fused_check_repair_kernel<3, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kRecoverSmemCapBig));
+	CUDA_TRY(cudaFuncSetAttribute(fused_check_repair_kernel<4, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kRecoverSmemCapBig));
+	CUDA_TRY(cudaFuncSetAttribute(fused_check_repair_kernel<1, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kRecoverSmemCapBig));
+	CUDA_TRY(cudaFuncSetAttribute(fused_check_repair_kernel<2, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kRecoverSmemCapBig));
+	CUDA_TRY(cudaFuncSetAttribute(fused_check_repair_kernel<3, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kRecoverSmemCapBig));
+	CUDA_TRY(cudaFuncSetAttribute(fused_check_repair_degraded_kernel<1, 2, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kRecoverSmemCapBig));
+	CUDA_TRY(cudaFuncSetAttribute(fused_check_repair_degraded_kernel<1, 3, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kRecoverSmemCapBig));
+	CUDA_TRY(cudaFuncSetAttribute(fused_check_repair_degraded_kernel<1, 4, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kRecoverSmemCapBig));
+	CUDA_TRY(cudaFuncSetAttribute(fused_check_repair_degraded_kernel<2, 3, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kRecoverSmemCapBig));
+	CUDA_TRY(cudaFuncSetAttribute(fused_check_repair_degraded_kernel<2, 4, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kRecoverSmemCapBig));
+	CUDA_TRY(cudaFuncSetAttribute(fused_check_repair_degraded_kernel<3, 4, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kRecoverSmemCapBig));
+	CUDA_TRY(cudaFuncSetAttribute(fused_check_repair_degraded_kernel<1, 2, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kRecoverSmemCapBig));
+	CUDA_TRY(cudaFuncSetAttribute(fused_check_repair_degraded_kernel<1, 3, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kRecoverSmemCapBig));
+	CUDA_TRY(cudaFuncSetAttribute(fused_check_repair_degraded_kernel<2, 3, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kRecoverSmemCapBig));
 	return LZGPU_OK;
 }
 
@@ -901,8 +917,9 @@ int lz_fused_recover(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, 
 // ---------------------------------------------------------------------------------------------------
 int lz_fused_check(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, uint32_t nb, const void *const *d_parts, size_t part_stride,
                    const void *const *d_part_crc, void *d_verdict, cudaStream_t st, unsigned long long *d_first_bad, bool map,
-                   const uint8_t *elim) {
+                   const uint8_t *elim, unsigned long long *d_failed) {
 	FusedState *fs = ctx->fused;
+	if (d_failed && !map) return LZGPU_ERR_ARG;  // (cannot happen: only the repair asks for the failing blocks, through the map)
 	if (!fs || fs->disabled) return LZGPU_NOT_HANDLED;
 	const int K = goal->k, M = goal->m;
 	if (part_stride % 16) return LZGPU_NOT_HANDLED;
@@ -971,7 +988,27 @@ int lz_fused_check(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, ui
 	uint32_t *d_map = static_cast<uint32_t *>(d_verdict);
 	const bool consecutive = o.consecutive != 0;
 	// E lost data parts, R given parity rows: E < R <= 4, and rows other than 0 .. R-1 only with m <= 4, so R <= 3 (m >= 5 is Cauchy)
-	if (E > 0) switch (10 * E + (consecutive ? R : R + 4)) {
+	if (d_failed && E > 0) switch (10 * E + (consecutive ? R : R + 4)) {
+		case 12: fused_check_repair_degraded_kernel<1, 2, true><<<grid, kCheckThreads, smem, st>>>(maps, p, d_map, lost, d_failed); break;
+		case 13: fused_check_repair_degraded_kernel<1, 3, true><<<grid, kCheckThreads, smem, st>>>(maps, p, d_map, lost, d_failed); break;
+		case 14: fused_check_repair_degraded_kernel<1, 4, true><<<grid, kCheckThreads, smem, st>>>(maps, p, d_map, lost, d_failed); break;
+		case 23: fused_check_repair_degraded_kernel<2, 3, true><<<grid, kCheckThreads, smem, st>>>(maps, p, d_map, lost, d_failed); break;
+		case 24: fused_check_repair_degraded_kernel<2, 4, true><<<grid, kCheckThreads, smem, st>>>(maps, p, d_map, lost, d_failed); break;
+		case 34: fused_check_repair_degraded_kernel<3, 4, true><<<grid, kCheckThreads, smem, st>>>(maps, p, d_map, lost, d_failed); break;
+		case 16: fused_check_repair_degraded_kernel<1, 2, false><<<grid, kCheckThreads, smem, st>>>(maps, p, d_map, lost, d_failed); break;
+		case 17: fused_check_repair_degraded_kernel<1, 3, false><<<grid, kCheckThreads, smem, st>>>(maps, p, d_map, lost, d_failed); break;
+		default: fused_check_repair_degraded_kernel<2, 3, false><<<grid, kCheckThreads, smem, st>>>(maps, p, d_map, lost, d_failed); break;
+	}
+	else if (d_failed) switch (consecutive ? R : R + 4) {
+		case 1: fused_check_repair_kernel<1, true><<<grid, kCheckThreads, smem, st>>>(maps, p, d_map, d_failed); break;
+		case 2: fused_check_repair_kernel<2, true><<<grid, kCheckThreads, smem, st>>>(maps, p, d_map, d_failed); break;
+		case 3: fused_check_repair_kernel<3, true><<<grid, kCheckThreads, smem, st>>>(maps, p, d_map, d_failed); break;
+		case 4: fused_check_repair_kernel<4, true><<<grid, kCheckThreads, smem, st>>>(maps, p, d_map, d_failed); break;
+		case 5: fused_check_repair_kernel<1, false><<<grid, kCheckThreads, smem, st>>>(maps, p, d_map, d_failed); break;
+		case 6: fused_check_repair_kernel<2, false><<<grid, kCheckThreads, smem, st>>>(maps, p, d_map, d_failed); break;
+		default: fused_check_repair_kernel<3, false><<<grid, kCheckThreads, smem, st>>>(maps, p, d_map, d_failed); break;
+	}
+	else if (E > 0) switch (10 * E + (consecutive ? R : R + 4)) {
 		case 12: fused_check_degraded_kernel<1, 2, true><<<grid, kCheckThreads, smem, st>>>(maps, p, d_map, lost); break;
 		case 13: fused_check_degraded_kernel<1, 3, true><<<grid, kCheckThreads, smem, st>>>(maps, p, d_map, lost); break;
 		case 14: fused_check_degraded_kernel<1, 4, true><<<grid, kCheckThreads, smem, st>>>(maps, p, d_map, lost); break;

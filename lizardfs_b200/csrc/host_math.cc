@@ -7,6 +7,7 @@
 
 #include "bitslice.cuh"
 #include "fused_plan.h"
+#include "repair_rows.h"
 
 #include <cctype>
 #include <cstdio>
@@ -457,6 +458,28 @@ int lzgpu_debug_bitslice_recover3(int k, const int *lost, const uint8_t *cols, i
 		std::memcpy(out + 32 * x, d[x], 32);
 	}
 	return LZGPU_OK;
+}
+
+// Diagnostics: the host build of repair_map_kernel's row derivation (one thread, no barrier), on the generator the kernel is given.
+int lzgpu_debug_repair_rows(int k, int m, const uint8_t *inputs, const uint8_t *wanted, int n_wanted, uint8_t *rows) {
+	if (k < 1 || k > LZGPU_MAX_DATA || m < 1 || m > LZGPU_MAX_PARITY || !inputs || !wanted || !rows || n_wanted < 1 || n_wanted > m) return LZGPU_ERR_ARG;
+	uint64_t used = 0;
+	for (int i = 0; i < k; ++i) {
+		if (inputs[i] >= k + m || (i && inputs[i] <= inputs[i - 1])) return LZGPU_ERR_ARG;
+		used |= 1ull << inputs[i];
+	}
+	for (int w = 0; w < n_wanted; ++w)
+		if (wanted[w] >= k + m || ((used >> wanted[w]) & 1ull)) return LZGPU_ERR_ARG;
+	uint8_t full[LZGPU_MAX_PARTS * LZGPU_MAX_DATA], gen[32 * 32] = {0};
+	lz::rs_generator(k, m, full);
+	for (int r = 0; r < m; ++r) std::memcpy(gen + 32 * r, full + (k + r) * k, k);
+	lzd::GfTables tb;
+	lzd::gf_tables_build(tb);
+	uint8_t mat[32][64], out[32 * 32];
+	uint32_t pivot = 0;
+	if (!lzd::repair_rows(k, gen, inputs, wanted, n_wanted, tb, mat, &pivot, out, 0, 1, [] {})) return LZGPU_ERR_ARG;
+	for (int w = 0; w < n_wanted; ++w) std::memcpy(rows + w * k, out + 32 * w, k);
+	return n_wanted;
 }
 
 int lzgpu_plan_convert(const lzgpu_goal *src, const lzgpu_goal *dst, const uint8_t *available, const uint8_t *want, lzgpu_convert_plan *out) {

@@ -451,6 +451,15 @@ __global__ void __launch_bounds__(256) crc_compare_kernel(const uint32_t *comput
 	}
 }
 
+// lzgpu_repair_stripes, generic route: every block of one part whose computed CRC is not the stored one sets `bit` in its word of
+// failed (one word per block, chunk * pb + block, zeroed by the caller)
+__global__ void __launch_bounds__(256) crc_failed_kernel(const uint32_t *computed, const uint32_t *stored, unsigned long long n,
+                                                         unsigned long long bit, unsigned long long *failed) {
+	const unsigned long long stride = static_cast<unsigned long long>(gridDim.x) * blockDim.x;
+	for (unsigned long long i = static_cast<unsigned long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < n; i += stride)
+		if (computed[i] != stored[i]) atomicOr(failed + i, bit);
+}
+
 // Exact form of the sparse-block rule.  The reference accepts a stored CRC of 0 only when the block IS all zero
 // (crc.cc:235-243 compares the bytes), not merely when its CRC equals that of 64 KiB of zeros; crc_compare_kernel
 // accepts on the CRC, this pass re-reads only those accepted blocks (sparse chunk files: the holes) and rejects the

@@ -604,6 +604,31 @@ class Engine:
         self._part_batch_dev(self.lib.lzgpu_correct_stripes_degraded_dev, goal, n_chunks, nb, d_parts, part_stride, d_part_crc, d_fix,
                              stream)
 
+    STRIPE_REPAIR_DTYPE = np.dtype([("bad_rows", np.uint32), ("suspect_part", np.int32), ("status", np.int32), ("crc", np.uint32),
+                                    ("crc_failed", np.uint64)])
+
+    def repair_stripes(self, goal, nb, parts, part_crc):
+        """correct_stripes_degraded, plus every block that fails its stored CRC rebuilt in place as an erasure (lzgpu_repair_stripes).
+        parts as in correct_stripes_degraded; part_crc is required for every given part.  Returns a structured array [n_chunks, pb]
+        of STRIPE_REPAIR_DTYPE (crc_failed: bit p = the block of part p failed its stored CRC before the call; status = _lib.FIX_*,
+        REBUILT and CRC_ONLY included), whether or not a stripe is left bad; raises ChunkCrcError when a block still fails its stored
+        CRC after the call (its .fix holds the entries, and every repair the rule allowed is made)."""
+        assert len(parts) == goal.k + goal.m
+        pb = (nb + goal.k - 1) // goal.k
+        parts, n, crcs = _host_parts(parts, part_crc, pb, in_place=True)
+        out = np.empty((n, pb), dtype=self.STRIPE_REPAIR_DTYPE)
+        rc = self.lib.lzgpu_repair_stripes(self.h, C.byref(goal.c), n, nb, _ptr_array(parts), pb * BLOCK_SIZE, crcs, _p(out))
+        _check_crc(rc, "repair_stripes", (-1, -1, -1), fix=out)
+        return out
+
+    def repair_stripes_dev(self, goal, n_chunks, nb, d_parts, part_stride, d_part_crc, d_fix, stream=None):
+        """Device-pointer form of repair_stripes: the rewritten blocks go into d_parts, n_chunks * pb entries of 24 bytes to d_fix
+        (device memory, 8-byte aligned).  The call only enqueues, with or without failing CRCs: the entries report them."""
+        n_parts = goal.k + goal.m
+        rc = self.lib.lzgpu_repair_stripes_dev(self.h, C.byref(goal.c), n_chunks, nb, _dev_ptrs(d_parts, n_parts), part_stride,
+                                               _dev_ptrs(d_part_crc, n_parts), d_fix, stream)
+        _check(rc, "repair_stripes_dev")
+
     # ---- wire format --------------------------------------------------------------------------
     def write_data_prefixes(self, goal, nb, crc, chunk_ids, write_id_base=0):
         """LIZ_CLTOCS_WRITE_DATA prefixes (cltocs.h:116-137) for every block of every part: uint8 [n, k+m, pb, 38]

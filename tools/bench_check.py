@@ -25,7 +25,13 @@ it on the fused and the generic route and times the full-parts map of the same g
 bytes are the given parts, their stored CRCs and the 8-byte map entries.  Both routes must return identical maps, clean and with one
 stale input block per chunk, which they must name when there are two spares or more.
 
-    python tools/bench_check.py [--chunks 16] [--iters 20] [--warmup 3] [--only degraded]      (one JSON line per measurement)
+The stripe repair (lzgpu_repair_stripes_dev) runs on the same kind of batch for ec(8,2), ec(8,4) and xor3, in three cases, each
+timed as the correction is (the rotten bytes put back before every call, outside the events): a clean batch, against
+lzgpu_correct_stripes_dev; one rotten block (bytes changed, stored CRC kept) in each of the first k stripes of part 3 of every chunk,
+against today's alternative, dropping part 3 and rebuilding it whole with lzgpu_recover_chunks_dev; and m rotten blocks in every
+stripe, the worst case, alone.  Both routes must return identical entries, and the rebuilt bytes must be the original ones.
+
+    python tools/bench_check.py [--chunks 16] [--iters 20] [--warmup 3] [--only degraded|repair]      (one JSON line per measurement)
 """
 import argparse
 import json
@@ -248,6 +254,72 @@ def correct_rows(eng, generic, r, text, args, stream, info):
             torch.cuda.synchronize()
 
 
+def repair_rows(eng, generic, args, stream, info):
+    """time the repair against the correction (clean), a whole-part recover (one rotten block in k stripes of part 3 per chunk) and
+    alone (m rotten blocks in every stripe); check both routes and the rebuilt bytes"""
+    st = stream.cuda_stream
+    for text in ("ec(8,2)", "ec(8,4)", "xor3"):
+        r = Resident(eng, text, args.chunks)
+        n = r.k + r.m
+        out_f = torch.empty(24 * r.n * r.pb, dtype=torch.uint8, device="cuda")
+        rebuilt = torch.empty(r.n * r.stride, dtype=torch.uint8, device="cuda")
+        cases = [("clean", []), ("one_rotten_block_in_k_stripes", [(3 % n, s) for s in range(r.k)]),
+                 ("m_rotten_blocks_in_every_stripe", [(p, s) for s in range(r.pb) for p in range(r.m)])]
+        for case, blocks in cases:
+            idx = good = faulty = None
+            if blocks:                   # the stored CRCs stay the original ones: every rotten block fails its own
+                idx = torch.tensor([c * r.stride + p * r.part_bytes + s * BLOCK + 777 + 64 * p for c in range(r.n) for p, s in blocks],
+                                   device="cuda")
+                good = r.buf[idx].clone()
+                faulty = good ^ 0x5A
+
+            def restore():
+                if idx is not None:
+                    with torch.cuda.stream(stream):
+                        r.buf[idx] = faulty
+
+            def repair(e=eng):
+                e.repair_stripes_dev(r.goal, r.n, NB, r.ptrs, r.stride, r.crc_ptrs, out_f.data_ptr(), stream=st)
+
+            def correct():
+                eng.correct_stripes_dev(r.goal, r.n, NB, r.ptrs, r.stride, r.crc_ptrs, out_f.data_ptr(), stream=st)
+
+            def recover_part():          # today's alternative: drop part 3 and rebuild it whole from k others
+                lost = 3 % n
+                parts = [0 if i == lost else p for i, p in enumerate(r.ptrs)]
+                crcs = [0 if i == lost else p for i, p in enumerate(r.crc_ptrs)]
+                eng.recover_chunks_dev(r.goal, r.n, NB, parts, r.stride, crcs, [int(i == lost) for i in range(n)],
+                                       [rebuilt.data_ptr() if i == lost else 0 for i in range(n)], stream=st)
+
+            other = {"clean": ("correct_stripes_dev", correct), "one_rotten_block_in_k_stripes": ("recover_chunks_dev_whole_part", recover_part)}.get(case)
+            t_rep = t_other = 0.0
+            for _ in range(2):           # alternate the calls, twice: other work shares the card
+                t_rep += timed_each(repair, restore, args.iters, args.warmup, stream) / 2
+                if other:
+                    t_other += timed_each(other[1], restore, args.iters, args.warmup, stream) / 2
+            eng.sync()
+            fixes = []
+            for e in (eng, generic):
+                restore()
+                torch.cuda.synchronize()
+                repair(e)
+                torch.cuda.synchronize()
+                fixes.append(out_f.cpu().numpy().view(L.Engine.STRIPE_REPAIR_DTYPE).reshape(r.n, r.pb).copy())
+                if idx is not None:
+                    assert (r.buf[idx] == good).all(), "a rebuilt block differs from the original"
+            assert (fixes[0] == fixes[1]).all(), "fused and generic repair entries differ"
+            n_rebuilt = int((fixes[0]["status"] == _lib.FIX_REBUILT).sum())
+            assert n_rebuilt == r.n * len({s for _, s in blocks}), (case, n_rebuilt)
+            assert int((fixes[0]["status"] == _lib.FIX_CLEAN).sum()) == r.n * r.pb - n_rebuilt
+            row = {"what": "repair_stripes_dev", "goal": text, "case": case, "chunks": r.n, "chunk_mib": NB * BLOCK >> 20,
+                   "rotten_blocks": len(blocks) * r.n, "rebuilt_stripes": n_rebuilt, "ms_per_call": round(t_rep * 1e3, 3)}
+            if other:
+                row.update({f"{other[0]}_ms_per_call": round(t_other * 1e3, 3), f"repair_over_{other[0]}": round(t_rep / t_other, 3)})
+            print(json.dumps({**row, "routes_agree": True, **info}), flush=True)
+        del r, out_f, rebuilt
+        torch.cuda.empty_cache()
+
+
 DEGRADED = [("ec(8,2)", (1,)), ("ec(5,3)", (1,)), ("ec(8,3)", (1, 4)), ("ec(8,4)", (1,)), ("ec(8,4)", (1, 4))]
 
 
@@ -317,7 +389,7 @@ def main():
     ap.add_argument("--chunks", type=int, default=16)
     ap.add_argument("--iters", type=int, default=20)
     ap.add_argument("--warmup", type=int, default=3)
-    ap.add_argument("--only", choices=["degraded"], default=None, help="run only the degraded-map rows")
+    ap.add_argument("--only", choices=["degraded", "repair"], default=None, help="run only the degraded-map rows, or only the repair rows")
     args = ap.parse_args()
     info = card()
     eng = L.Engine(0)
@@ -328,7 +400,10 @@ def main():
     st = stream.cuda_stream
     eng.set_deferred_verify(True)
     generic.set_deferred_verify(True)
-    degraded_rows(eng, generic, args, stream, info)
+    if args.only in (None, "degraded"):
+        degraded_rows(eng, generic, args, stream, info)
+    if args.only in (None, "repair"):
+        repair_rows(eng, generic, args, stream, info)
     generic.set_deferred_verify(False)
     for text in (GOALS if args.only is None else []):
         r = Resident(eng, text, args.chunks)
