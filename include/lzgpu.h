@@ -201,6 +201,12 @@ int lzgpu_debug_bitslice_recover3(int k, const int *lost, const uint8_t *cols, i
  * inputs[0 .. k-1] (ascending), rows[w * k + j] = the coefficient of input j in the block of part wanted[w], w < n_wanted.  Returns
  * n_wanted, or LZGPU_ERR_ARG for bad arguments or a singular submatrix. */
 int lzgpu_debug_repair_rows(int k, int m, const uint8_t *inputs, const uint8_t *wanted, int n_wanted, uint8_t *rows);
+/* The host build of the error locator of lzgpu_decode_stripes (csrc/decode_locate.h): given[i] and failed[i] (k + m flags) name the
+ * given parts and those among them that fail their CRCs (F); blocks[i] holds len bytes of part i's block (ignored when not given).
+ * Returns |E| (0 when the code punctured by F is a codeword; *located = E, bit p = part p), LZGPU_ERR_INCONSISTENT when no unique E of
+ * at most two given parts outside F with 2 |E| + |F| <= given - k explains every byte, or LZGPU_ERR_ARG for bad arguments. */
+int lzgpu_debug_locate_errors(int k, int m, const uint8_t *given, const uint8_t *failed, const uint8_t *const *blocks, uint32_t len,
+                              uint64_t *located);
 
 /* ---------------------------------------------------------------------------------------------
  * Engine context: one per (process, device).  Owns streams, pinned staging and device scratch.
@@ -380,7 +386,7 @@ int lzgpu_recover_chunks_dev(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_
  *                       restricted to the checked rows; -1 when no single part or more than one does.  With one checked row (xorN, or
  *                       one parity part given) it is always -1.  With two checked rows two corrupt parts can look like a third,
  *                       single one — a property of the code, not of this check.  With three or more checked rows two corrupt parts
- *                       never produce a suspect.  The verdict says nothing about the stripes after the first: before rebuilding a
+ *                       never produce a suspect (lzgpu_decode_stripes locates them with four or more).  The verdict says nothing about the stripes after the first: before rebuilding a
  *                       part, take lzgpu_check_stripe_map and follow its repair rule.
  * lzgpu_check_stripes returns LZGPU_ERR_CRC when a stored CRC failed, else LZGPU_ERR_INCONSISTENT when any chunk has a bad stripe,
  * else LZGPU_OK.  lzgpu_check_stripes_dev writes the verdicts to d_verdict (device memory, 4-byte aligned; nothing else is written)
@@ -545,6 +551,48 @@ typedef struct lzgpu_stripe_repair {
 int lzgpu_repair_stripes(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, uint32_t nb,
                          uint8_t *const *parts, size_t part_stride, const uint32_t *const *part_crc, lzgpu_stripe_repair *fix);
 int lzgpu_repair_stripes_dev(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, uint32_t nb,
+                             void *const *d_parts, size_t part_stride, const void *const *d_part_crc, void *d_fix, void *stream);
+
+/* Stripe decode: lzgpu_repair_stripes, then errors-and-erasures decoding up to the code's radius where the repair gives up.  With
+ * s = given - k spare rows and the |F| blocks that fail their stored CRCs as erasures, the code can still locate e unknown bad blocks
+ * (valid CRC, wrong bytes: a stale part after a partial write or a restore from an older version) whenever 2 e + |F| <= s.  So two
+ * stale parts of an ec(8,4) stripe, or one stale part beside a rotten block of ec(8,3), are corrected in place where the repair
+ * leaves the stripe UNEXPLAINED or CRC_CONFLICT.
+ *   goal, n_chunks, nb, parts, part_stride, part_crc   exactly as in lzgpu_repair_stripes (any part may be NULL, at least k + 1 given,
+ *                    stored CRCs required for every given part, refused while CRCs are disabled: LZGPU_ERR_ARG before anything is
+ *                    enqueued), and the return codes are the repair's (LZGPU_ERR_CRC, else LZGPU_ERR_INCONSISTENT, else LZGPU_OK).
+ *   fix[c * pb + s]  one entry for every stripe; its first 24 bytes are an lzgpu_stripe_repair.
+ * Rule, per stripe, with F and s as above:
+ *   1. When lzgpu_repair_stripes ends the stripe CLEAN, CORRECTED, REBUILT or CRC_ONLY, the first 24 bytes of the entry and the bytes
+ *      written are the repair's, and located = 0.
+ *   2. When it ends the stripe UNEXPLAINED or CRC_CONFLICT, the code punctured by F is decoded: its inputs are the first k given parts
+ *      outside F, the other given parts outside F its s - |F| spares.  The call looks for the smallest e, 1 <= e <= 2 with
+ *      2 e + |F| <= s, for which exactly one set E of e given parts outside F explains the punctured syndromes at every byte (they lie
+ *      in the span of E's columns of [M | I], M = the spares' recovery rows over the inputs).  If there is one, F and E are rebuilt
+ *      from the first k given parts outside F and E, ascending, and written only if every block of F then matches its stored CRC:
+ *      LZGPU_FIX_DECODED, crc = 0, located = E, located_crc = E's new CRCs (part_crc is not written; the caller stores them).
+ *      Otherwise the repair's entry stands and nothing is written.  With F empty the map has already tried e = 1, so only e = 2
+ *      (s >= 4) is new there.
+ * Limits:
+ *   - More bad blocks than the radius allows can look like fewer, as two bad parts can look like one with two checked rows.  With F
+ *     empty no CRC confirms a DECODED stripe: the result is the code's nearest codeword.
+ *   - As in the repair, a stale spare that is not an input survives a REBUILT stripe (rule 1 keeps the repair's result); a second call
+ *     finds F empty and corrects it.
+ * lzgpu_decode_stripes_dev enqueues the whole call on `stream` and never waits for it, deferred mode or not, as
+ * lzgpu_repair_stripes_dev; d_fix must be 8-byte aligned. */
+enum { LZGPU_FIX_DECODED = 6 };  /* lzgpu_stripe_decode.status, beside LZGPU_FIX_CLEAN .. LZGPU_FIX_CRC_ONLY */
+typedef struct lzgpu_stripe_decode {
+	uint32_t bad_rows;        /* as lzgpu_stripe_repair */
+	int32_t suspect_part;     /* as lzgpu_stripe_repair */
+	int32_t status;           /* LZGPU_FIX_* */
+	uint32_t crc;             /* as lzgpu_stripe_repair (0 when DECODED) */
+	uint64_t crc_failed;      /* as lzgpu_stripe_repair */
+	uint64_t located;         /* DECODED: bit p = the block of part p that the code located (valid CRC, wrong bytes) and rewrote */
+	uint32_t located_crc[2];  /* DECODED: mycrc32 of the rewritten located blocks, ascending part; else 0 */
+} lzgpu_stripe_decode;        /* 40 bytes, 8-byte aligned; the first 24 bytes are an lzgpu_stripe_repair */
+int lzgpu_decode_stripes(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, uint32_t nb,
+                         uint8_t *const *parts, size_t part_stride, const uint32_t *const *part_crc, lzgpu_stripe_decode *fix);
+int lzgpu_decode_stripes_dev(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, uint32_t nb,
                              void *const *d_parts, size_t part_stride, const void *const *d_part_crc, void *d_fix, void *stream);
 
 /* Wire-format producer (SURVEY.md §8 f3): LIZ_CLTOCS_WRITE_DATA packet prefixes (src/protocol/cltocs.h:116-137) for

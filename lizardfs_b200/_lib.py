@@ -87,13 +87,18 @@ class LzStripeFix(C.Structure):
     _fields_ = [("bad_rows", C.c_uint32), ("suspect_part", C.c_int32), ("status", C.c_int32), ("crc", C.c_uint32)]
 
 
-# lzgpu_stripe_fix.status (lzgpu_stripe_repair.status: also REBUILT and CRC_ONLY)
-FIX_CLEAN, FIX_CORRECTED, FIX_UNEXPLAINED, FIX_CRC_CONFLICT, FIX_REBUILT, FIX_CRC_ONLY = range(6)
+# lzgpu_stripe_fix.status (lzgpu_stripe_repair.status: also REBUILT and CRC_ONLY; lzgpu_stripe_decode.status: also DECODED)
+FIX_CLEAN, FIX_CORRECTED, FIX_UNEXPLAINED, FIX_CRC_CONFLICT, FIX_REBUILT, FIX_CRC_ONLY, FIX_DECODED = range(7)
 
 
 class LzStripeRepair(C.Structure):
     _fields_ = [("bad_rows", C.c_uint32), ("suspect_part", C.c_int32), ("status", C.c_int32), ("crc", C.c_uint32),
                 ("crc_failed", C.c_uint64)]
+
+
+class LzStripeDecode(C.Structure):
+    _fields_ = [("bad_rows", C.c_uint32), ("suspect_part", C.c_int32), ("status", C.c_int32), ("crc", C.c_uint32),
+                ("crc_failed", C.c_uint64), ("located", C.c_uint64), ("located_crc", C.c_uint32 * 2)]
 
 
 class LzBlockWrite(C.Structure):
@@ -117,6 +122,7 @@ SIGNATURES = {
     "lzgpu_debug_bitslice_rows": (_int, [_int, _vp, _vp]),
     "lzgpu_debug_bitslice_recover3": (_int, [_int, _vp, _vp, _int, _vp]),
     "lzgpu_debug_repair_rows": (_int, [_int, _int, _vp, _vp, _int, _vp]),
+    "lzgpu_debug_locate_errors": (_int, [_int, _int, _vp, _vp, _vp, _u32, _vp]),
     "lzgpu_goal_slice_type": (_int, [_goalp]),
     "lzgpu_goal_from_slice_type": (_int, [_int, _goalp]),
     "lzgpu_ref_part_index": (_int, [_goalp, _int]),
@@ -150,6 +156,8 @@ SIGNATURES = {
     "lzgpu_correct_stripes_degraded_dev": (_int, [_vp, _goalp, _u32, _u32, _vp, _sz, _vp, _vp, _vp, _vp]),
     "lzgpu_repair_stripes": (_int, [_vp, _goalp, _u32, _u32, _vp, _sz, _vp, _vp]),
     "lzgpu_repair_stripes_dev": (_int, [_vp, _goalp, _u32, _u32, _vp, _sz, _vp, _vp, _vp]),
+    "lzgpu_decode_stripes": (_int, [_vp, _goalp, _u32, _u32, _vp, _sz, _vp, _vp]),
+    "lzgpu_decode_stripes_dev": (_int, [_vp, _goalp, _u32, _u32, _vp, _sz, _vp, _vp, _vp]),
     "lzgpu_write_data_prefixes": (_int, [_vp, _goalp, _u32, _u32, _vp, _sz, _vp, _u32, _vp]),
     "lzgpu_write_data_prefixes_dev": (_int, [_vp, _goalp, _u32, _u32, _vp, _sz, _vp, _u32, _vp, _vp]),
     "lzgpu_split_chunks": (_int, [_vp, _goalp, _u32, _u32, _vp, _sz, _vp, _sz]),

@@ -16,6 +16,7 @@
 #include "kernels_generic.cuh"
 #include "lzgpu.h"
 #include "repair_rows.h"
+#include "decode_locate.h"
 
 namespace lzd {
 
@@ -277,6 +278,111 @@ __global__ void __launch_bounds__(256) repair_map_kernel(const RepairArgs a) {
 		}
 		if (t == 0) a.fix[e] = lzgpu_stripe_repair{bad_rows, suspect, status, status == LZGPU_FIX_CORRECTED ? crc : 0u, f};
 		__syncthreads();  // s_in, s_want and s_rows are re-used by the next entry
+	}
+}
+
+// lzgpu_decode_stripes: after repair_map_kernel has written every entry into a temporary, the entries it left UNEXPLAINED or
+// CRC_CONFLICT are decoded up to the code's radius (decode_locate.h): with F = crc_failed and s = given - k, the code punctured by F
+// (inputs: the first k given parts outside F; spares: the other given parts outside F) locates E, |E| <= 2 with 2 |E| + |F| <= s.
+// Then X = F | E is rebuilt from the first k given parts outside X as repair_map_kernel rebuilds F, storing nothing until every block
+// of F has matched its stored CRC.  Every other entry is copied with located = 0.
+struct DecodeArgs {
+	RepairArgs r;                     // the parts, CRCs, tables and generator of the repair (map, failed and fix unused)
+	const lzgpu_stripe_repair *rep;   // the repair's entries
+	lzgpu_stripe_decode *fix;         // one entry per repair entry
+};
+
+// Host and device: an entry of the repair that rule 2 of the decode can still serve (spare = given parts - k)
+LZ_HD inline bool decode_eligible(int status, unsigned long long f, int spare) {
+	int n = 0;
+	for (unsigned long long b = f; b; b &= b - 1) ++n;
+	if (status == LZGPU_FIX_UNEXPLAINED) return !f && spare >= 4;
+	return status == LZGPU_FIX_CRC_CONFLICT && f && n + 2 <= spare;
+}
+
+__global__ void __launch_bounds__(256) decode_map_kernel(const DecodeArgs d) {
+	const RepairArgs &a = d.r;
+	__shared__ uint32_t s_tab[1024];
+	__shared__ CoefPlanes s_coef[32];
+	__shared__ GfTables s_gf;
+	__shared__ uint8_t s_mat[32][64];
+	__shared__ uint8_t s_rows[32 * 32];
+	__shared__ uint8_t s_pt[64], s_in[32], s_want[64];
+	__shared__ const uint8_t *s_blk[64];
+	__shared__ LocateScratch s_loc;
+	__shared__ uint32_t s_pivot, s_out[8];
+	const unsigned t = threadIdx.x;
+	const int spare = __popcll(a.given) - static_cast<int>(a.k);
+	bool ready = false;
+	uint32_t shift = 0;
+	for (unsigned long long e = blockIdx.x; e < a.n_entries; e += gridDim.x) {
+		const lzgpu_stripe_repair r = d.rep[e];
+		const unsigned long long f = r.crc_failed;
+		if (!decode_eligible(r.status, f, spare)) {
+			if (t == 0) d.fix[e] = lzgpu_stripe_decode{r.bad_rows, r.suspect_part, r.status, r.crc, f, 0ull, {0u, 0u}};
+			continue;
+		}
+		if (!ready) {  // first entry with work: tables and this thread's shift
+			for (unsigned i = t; i < 1024; i += 256) s_tab[i] = a.tables[i];
+			if (t == 0) gf_tables_build(s_gf);
+			shift = crc_xpow_bytes_dev(256u * (255u - t), a.pow2);
+			ready = true;
+		}
+		const unsigned long long off = (e / a.pb) * a.part_stride + (e % a.pb) * 65536ull;
+		const unsigned long long kept = a.given & ~f;
+		const uint32_t sp = static_cast<uint32_t>(__popcll(kept)) - a.k;
+		if (t == 0) {  // the punctured code's columns: inputs, then spares
+			uint32_t n = 0;
+			for (uint32_t p = 0; p < a.n_parts; ++p)
+				if ((kept >> p) & 1ull) {
+					s_blk[n] = a.part[p] + off;
+					s_pt[n++] = static_cast<uint8_t>(p);
+				}
+		}
+		__syncthreads();
+		int status = r.status;
+		unsigned long long located = 0;
+		uint32_t lcrc[2] = {0u, 0u};
+		unsigned long long cols = 0;
+		if (repair_rows(a.k, a.gen, s_pt, s_pt + a.k, sp, s_gf, s_mat, &s_pivot, s_rows, t, 256u, CtaSync()) &&
+		    locate_errors(a.k, sp, s_rows, s_blk, 65536u, s_gf, s_loc, t, 256u, CtaSync(), &cols) > 0) {
+			for (unsigned long long b = cols; b; b &= b - 1) located |= 1ull << s_pt[__ffsll(static_cast<long long>(b)) - 1];
+			const unsigned long long x = f | located;
+			__syncthreads();  // every thread has read s_pt
+			if (t == 0) {
+				uint32_t ni = 0, nw = 0;
+				for (uint32_t p = 0; p < a.n_parts; ++p) {
+					if (!((a.given >> p) & 1ull)) continue;
+					if ((x >> p) & 1ull) s_want[nw++] = static_cast<uint8_t>(p);
+					else if (ni < a.k) s_in[ni++] = static_cast<uint8_t>(p);
+				}
+			}
+			__syncthreads();
+			const uint32_t nw = static_cast<uint32_t>(__popcll(x));
+			if (repair_rows(a.k, a.gen, s_in, s_want, nw, s_gf, s_mat, &s_pivot, s_rows, t, 256u, CtaSync())) {
+				uint32_t acc[64];
+				bool match = true;
+				uint32_t nl = 0;
+				for (uint32_t w = 0; w < nw && match; ++w) {
+					const uint32_t crc = repair_block(a, off, s_in, s_rows + 32 * w, acc, s_coef, s_tab, shift, s_out);
+					if ((f >> s_want[w]) & 1ull) match = crc == a.crc[s_want[w]][e];  // e = chunk * pb + block
+					else if (nl++) lcrc[1] = crc;
+					else lcrc[0] = crc;
+				}
+				if (match) {
+					repair_store(a.part[s_want[nw - 1]] + off, acc);
+					for (uint32_t w = 0; w + 1 < nw; ++w) {
+						repair_block(a, off, s_in, s_rows + 32 * w, acc, s_coef, s_tab, shift, s_out);
+						repair_store(a.part[s_want[w]] + off, acc);
+					}
+					status = LZGPU_FIX_DECODED;
+				}
+			}
+		}
+		if (status != LZGPU_FIX_DECODED) located = 0, lcrc[0] = lcrc[1] = 0;
+		if (t == 0)
+			d.fix[e] = lzgpu_stripe_decode{r.bad_rows, r.suspect_part, status, status == LZGPU_FIX_DECODED ? 0u : r.crc, f, located, {lcrc[0], lcrc[1]}};
+		__syncthreads();  // s_pt, s_blk, s_in, s_want, s_rows and s_loc are re-used by the next entry
 	}
 }
 

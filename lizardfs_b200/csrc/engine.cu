@@ -1604,19 +1604,22 @@ extern "C" int lzgpu_correct_stripes_degraded(lzgpu_ctx *ctx, const lzgpu_goal *
 
 // ------------------------------------------------------------------------------------------------
 // stripe repair: the degraded map with every block that fails its stored CRC, then the correction's rule or those blocks rebuilt as
-// erasures (repair_map_kernel, correct_kernel.cuh)
+// erasures (repair_map_kernel, correct_kernel.cuh); stripe decode: the repair, then up to two located blocks beside the erasures
+// where it gives up (decode_map_kernel)
 // ------------------------------------------------------------------------------------------------
 static_assert(sizeof(lzgpu_stripe_repair) == 24 && alignof(lzgpu_stripe_repair) == 8, "repair entries as repair_map_kernel writes them");
+static_assert(sizeof(lzgpu_stripe_decode) == 40 && alignof(lzgpu_stripe_decode) == 8 && offsetof(lzgpu_stripe_decode, located) == 24,
+              "decode entries as decode_map_kernel writes them");
 
-// the arguments of lzgpu_correct_stripes_degraded, and the repair's own refusals (before anything is enqueued)
+// the arguments of lzgpu_correct_stripes_degraded, and the repair's own refusals (before anything is enqueued); name: the call's
 static int repair_args(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t nb, const void *const *parts, const void *const *part_crc, const void *fix,
-                       bool dev) {
+                       bool dev, const char *name) {
 	int rc = check_args(ctx, goal, nb, parts, part_crc, fix, dev, true);
 	if (rc) return rc;
-	if (!lzgpu_crc_enabled()) { lz_set_error("repair_stripes: CRCs are disabled, so nothing locates the blocks to rebuild"); return LZGPU_ERR_ARG; }
+	if (!lzgpu_crc_enabled()) { lz_set_error("%s: CRCs are disabled, so nothing locates the blocks to rebuild", name); return LZGPU_ERR_ARG; }
 	for (int i = 0; i < goal->k + goal->m; ++i)
-		if (parts[i] && (!part_crc || !part_crc[i])) { lz_set_error("repair_stripes: part %d is given without stored CRCs", i); return LZGPU_ERR_ARG; }
-	if (dev && (reinterpret_cast<uintptr_t>(fix) & 7)) { lz_set_error("repair_stripes: fix is not 8-byte aligned"); return LZGPU_ERR_ARG; }
+		if (parts[i] && (!part_crc || !part_crc[i])) { lz_set_error("%s: part %d is given without stored CRCs", name, i); return LZGPU_ERR_ARG; }
+	if (dev && (reinterpret_cast<uintptr_t>(fix) & 7)) { lz_set_error("%s: fix is not 8-byte aligned", name); return LZGPU_ERR_ARG; }
 	return LZGPU_OK;
 }
 
@@ -1632,10 +1635,10 @@ static void repair_table(const lzgpu_goal *goal, unsigned long long given, Repai
 
 // repair_map_kernel over n_entries entries (pb per chunk) on `st`; a carries the table (repair_table) and the part and CRC pointers
 static int repair_enqueue(lzgpu_ctx *ctx, RepairArgs &a, unsigned long long n_entries, uint32_t pb, size_t part_stride, const void *d_map,
-                          const void *d_failed, void *d_fix, cudaStream_t st) {
+                          const void *d_failed, lzgpu_stripe_repair *d_fix, cudaStream_t st) {
 	a.map = static_cast<const uint32_t *>(d_map);
 	a.failed = static_cast<const unsigned long long *>(d_failed);
-	a.fix = static_cast<lzgpu_stripe_repair *>(d_fix);
+	a.fix = d_fix;
 	a.tables = ctx->d_crc_tables;
 	a.part_stride = part_stride;
 	a.n_entries = n_entries;
@@ -1651,10 +1654,36 @@ static int repair_enqueue(lzgpu_ctx *ctx, RepairArgs &a, unsigned long long n_en
 	return LZGPU_OK;
 }
 
-extern "C" int lzgpu_repair_stripes_dev(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, uint32_t nb, void *const *d_parts,
-                                        size_t part_stride, const void *const *d_part_crc, void *d_fix, void *stream) {
-	NvtxScope nvtx_scope("lzgpu::repair_stripes_dev");
-	int rc = repair_args(ctx, goal, nb, d_parts, d_part_crc, d_fix, true);
+// lzgpu_decode_stripes: the repair into a stream-ordered temporary of repair entries, then decode_map_kernel over them
+static int repair_enqueue(lzgpu_ctx *ctx, RepairArgs &a, unsigned long long n_entries, uint32_t pb, size_t part_stride, const void *d_map,
+                          const void *d_failed, lzgpu_stripe_decode *d_fix, cudaStream_t st) {
+	TmpBuf rep(ctx, st);
+	int rc;
+	if ((rc = rep.alloc(n_entries * sizeof(lzgpu_stripe_repair))) ||
+	    (rc = repair_enqueue(ctx, a, n_entries, pb, part_stride, d_map, d_failed, static_cast<lzgpu_stripe_repair *>(rep.p), st)))
+		return rc;
+	const DecodeArgs d{a, static_cast<const lzgpu_stripe_repair *>(rep.p), d_fix};
+	decode_map_kernel<<<grid_for(ctx, n_entries * 256, 256, 2), 256, 0, st>>>(d);
+	CUDA_TRY(cudaGetLastError());
+	ctx->stats.kernel_launches++;
+	return LZGPU_OK;
+}
+
+// the blocks an entry says were written in place
+static unsigned long long fix_written(const lzgpu_stripe_repair &f) {
+	if (f.status == LZGPU_FIX_CORRECTED) return 1ull << f.suspect_part;
+	return f.status == LZGPU_FIX_REBUILT ? f.crc_failed : 0ull;
+}
+static unsigned long long fix_written(const lzgpu_stripe_decode &f) {
+	if (f.status == LZGPU_FIX_CORRECTED) return 1ull << f.suspect_part;
+	return f.status == LZGPU_FIX_REBUILT || f.status == LZGPU_FIX_DECODED ? f.crc_failed | f.located : 0ull;
+}
+
+// the repair's and the decode's _dev call (Fix: the entry kind, which picks the kernels)
+template <class Fix>
+static int repair_dev(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, uint32_t nb, void *const *d_parts, size_t part_stride,
+                      const void *const *d_part_crc, void *d_fix, void *stream, const char *name) {
+	int rc = repair_args(ctx, goal, nb, d_parts, d_part_crc, d_fix, true, name);
 	if (rc || n_chunks == 0) return rc;
 	const uint32_t pb = (nb + goal->k - 1) / goal->k;
 	const unsigned long long entries = static_cast<unsigned long long>(n_chunks) * pb;
@@ -1669,21 +1698,34 @@ extern "C" int lzgpu_repair_stripes_dev(lzgpu_ctx *ctx, const lzgpu_goal *goal, 
 	DeviceGuard g(ctx->device);
 	cudaStream_t st = stream ? static_cast<cudaStream_t>(stream) : ctx->stream;
 	// the map's bytes and one entry per stripe; the rebuilt blocks are not counted (the host does not know them here)
-	BatchTimer timer(ctx, st, check_alg_bytes(goal, n_chunks, nb, d_parts, d_part_crc, true) + entries * sizeof(lzgpu_stripe_repair));
+	BatchTimer timer(ctx, st, check_alg_bytes(goal, n_chunks, nb, d_parts, d_part_crc, true) + entries * sizeof(Fix));
 	TmpBuf map(ctx, st), failed(ctx, st);
 	if ((rc = map.alloc(entries * sizeof(lzgpu_stripe_state))) || (rc = failed.alloc(entries * sizeof(uint64_t))) ||
 	    (rc = check_enqueue(ctx, goal, n_chunks, nb, d_parts, part_stride, d_part_crc, map.p, st, nullptr, true,
 	                        static_cast<unsigned long long *>(failed.p))))
 		return rc;
-	return repair_enqueue(ctx, a, entries, pb, part_stride, map.p, failed.p, d_fix, st);
+	return repair_enqueue(ctx, a, entries, pb, part_stride, map.p, failed.p, static_cast<Fix *>(d_fix), st);
 }
 
-// The host-pointer repair, phase 2: the stripes `todo` (map indices with blocks to rebuild) gathered into one-stripe "chunks" as in
-// correct_host_stripes, tile by tile, through repair_map_kernel with the map entries and failing blocks the check found; the entries
-// go to fix[], the rewritten blocks back into the caller's parts.
+extern "C" int lzgpu_repair_stripes_dev(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, uint32_t nb, void *const *d_parts,
+                                        size_t part_stride, const void *const *d_part_crc, void *d_fix, void *stream) {
+	NvtxScope nvtx_scope("lzgpu::repair_stripes_dev");
+	return repair_dev<lzgpu_stripe_repair>(ctx, goal, n_chunks, nb, d_parts, part_stride, d_part_crc, d_fix, stream, "repair_stripes");
+}
+
+extern "C" int lzgpu_decode_stripes_dev(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, uint32_t nb, void *const *d_parts,
+                                        size_t part_stride, const void *const *d_part_crc, void *d_fix, void *stream) {
+	NvtxScope nvtx_scope("lzgpu::decode_stripes_dev");
+	return repair_dev<lzgpu_stripe_decode>(ctx, goal, n_chunks, nb, d_parts, part_stride, d_part_crc, d_fix, stream, "decode_stripes");
+}
+
+// The host-pointer repair and decode, phase 2: the stripes `todo` (map indices with work) gathered into one-stripe "chunks" as in
+// correct_host_stripes, tile by tile, through the kernels of the entry kind with the map entries and failing blocks the check found;
+// the entries go to fix[], the rewritten blocks back into the caller's parts.
+template <class Fix>
 static int repair_host_stripes(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t pb, uint8_t *const *parts, size_t part_stride,
                                const uint32_t *const *part_crc, const lzgpu_stripe_state *map, const uint64_t *failed,
-                               const std::vector<size_t> &todo, lzgpu_stripe_repair *fix) {
+                               const std::vector<size_t> &todo, Fix *fix) {
 	const int n = goal->k + goal->m;
 	const size_t B = LZGPU_BLOCK_SIZE;
 	unsigned long long given = 0;
@@ -1698,7 +1740,7 @@ static int repair_host_stripes(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t 
 	std::lock_guard<std::mutex> lk(ctx->mu);
 	DeviceGuard g(ctx->device);
 	const size_t tile = std::max<size_t>(1, std::min<size_t>(todo.size(), (2 * kHostTileBytes) / (B * n_given)));
-	const size_t entry_bytes = sizeof(lzgpu_stripe_state) + sizeof(uint64_t) + sizeof(lzgpu_stripe_repair);
+	const size_t entry_bytes = sizeof(lzgpu_stripe_state) + sizeof(uint64_t) + sizeof(Fix);
 	void *d_in, *d_crc, *d_entries;
 	int rc;
 	if ((rc = lz_scratch(ctx, kScratchIn0, tile * B * n, &d_in)) || (rc = lz_scratch(ctx, kScratchCrc0, tile * 4 * n, &d_crc)) ||
@@ -1706,7 +1748,7 @@ static int repair_host_stripes(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t 
 		return rc;
 	void *d_failed = d_entries;  // 8-byte words first: every part of d_entries stays 8-byte aligned
 	void *d_fix = static_cast<uint8_t *>(d_entries) + tile * sizeof(uint64_t);
-	void *d_map = static_cast<uint8_t *>(d_fix) + tile * sizeof(lzgpu_stripe_repair);
+	void *d_map = static_cast<uint8_t *>(d_fix) + tile * sizeof(Fix);
 	for (int i = 0; i < n; ++i) {
 		a.part[i] = parts[i] ? static_cast<uint8_t *>(d_in) + tile * B * i : nullptr;
 		a.crc[i] = parts[i] ? static_cast<const uint32_t *>(d_crc) + tile * i : nullptr;
@@ -1714,7 +1756,7 @@ static int repair_host_stripes(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t 
 	std::vector<uint32_t> h_crc(tile * n);
 	std::vector<lzgpu_stripe_state> h_map(tile);
 	std::vector<uint64_t> h_failed(tile);
-	std::vector<lzgpu_stripe_repair> h_fix(tile);
+	std::vector<Fix> h_fix(tile);
 	cudaStream_t st = ctx->slot_stream[0];
 	for (size_t t0 = 0; t0 < todo.size(); t0 += tile) {
 		const size_t nt = std::min(tile, todo.size() - t0);
@@ -1734,17 +1776,14 @@ static int repair_host_stripes(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t 
 		CUDA_TRY(cudaMemcpyAsync(d_failed, h_failed.data(), nt * sizeof(uint64_t), cudaMemcpyHostToDevice, st));
 		{
 			BatchTimer timer(ctx, st, nt * (n_given * B + entry_bytes));
-			if ((rc = repair_enqueue(ctx, a, nt, 1, B, d_map, d_failed, d_fix, st))) return rc;
+			if ((rc = repair_enqueue(ctx, a, nt, 1, B, d_map, d_failed, static_cast<Fix *>(d_fix), st))) return rc;
 		}
-		CUDA_TRY(cudaMemcpyAsync(h_fix.data(), d_fix, nt * sizeof(lzgpu_stripe_repair), cudaMemcpyDeviceToHost, st));
+		CUDA_TRY(cudaMemcpyAsync(h_fix.data(), d_fix, nt * sizeof(Fix), cudaMemcpyDeviceToHost, st));
 		CUDA_TRY(cudaStreamSynchronize(st));
 		for (size_t j = 0; j < nt; ++j) {
 			const size_t e = todo[t0 + j], c = e / pb, s = e % pb;
 			fix[e] = h_fix[j];
-			unsigned long long written = 0;
-			if (h_fix[j].status == LZGPU_FIX_CORRECTED) written = 1ull << h_fix[j].suspect_part;
-			if (h_fix[j].status == LZGPU_FIX_REBUILT) written = h_fix[j].crc_failed;
-			for (; written; written &= written - 1) {
+			for (unsigned long long written = fix_written(h_fix[j]); written; written &= written - 1) {
 				const int p = __builtin_ctzll(written);
 				CUDA_TRY(cudaMemcpyAsync(parts[p] + c * part_stride + s * B, a.part[p] + j * B, B, cudaMemcpyDeviceToHost, st));
 				ctx->stats.bytes_d2h += B;
@@ -1755,10 +1794,12 @@ static int repair_host_stripes(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t 
 	return LZGPU_OK;
 }
 
-extern "C" int lzgpu_repair_stripes(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, uint32_t nb, uint8_t *const *parts,
-                                    size_t part_stride, const uint32_t *const *part_crc, lzgpu_stripe_repair *fix) {
-	NvtxScope nvtx_scope("lzgpu::repair_stripes");
-	int rc = repair_args(ctx, goal, nb, reinterpret_cast<const void *const *>(parts), reinterpret_cast<const void *const *>(part_crc), fix, false);
+// the repair's and the decode's host-pointer call: phase 1 maps the whole batch, phase 2 stages the stripes with work (the repair's
+// blocks to rebuild, and for the decode the entries its rule 2 can still serve)
+template <class Fix>
+static int repair_host(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, uint32_t nb, uint8_t *const *parts, size_t part_stride,
+                       const uint32_t *const *part_crc, Fix *fix, bool decode, const char *name) {
+	int rc = repair_args(ctx, goal, nb, reinterpret_cast<const void *const *>(parts), reinterpret_cast<const void *const *>(part_crc), fix, false, name);
 	if (rc) return rc;
 	if (n_chunks == 0) return LZGPU_OK;
 	// phase 1: the map and the failing blocks of the whole batch through the check's tile pipeline
@@ -1774,22 +1815,39 @@ extern "C" int lzgpu_repair_stripes(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint
 	for (size_t e = 0; e < entries; ++e) {
 		unsigned long long x;
 		const int status = repair_rule(map[e].bad_rows, map[e].suspect_part, failed[e], spare, &x);
-		fix[e] = lzgpu_stripe_repair{map[e].bad_rows, map[e].suspect_part, status, 0u, failed[e]};
-		if (x) todo.push_back(e);
+		fix[e] = Fix{};
+		fix[e].bad_rows = map[e].bad_rows;
+		fix[e].suspect_part = map[e].suspect_part;
+		fix[e].status = status;
+		fix[e].crc_failed = failed[e];
+		if (x || (decode && decode_eligible(status, failed[e], spare))) todo.push_back(e);
 	}
-	// phase 2: only the stripes with blocks to rebuild travel again
+	// phase 2: only the stripes with work travel again
 	if (!todo.empty() && (rc = repair_host_stripes(ctx, goal, pb, parts, part_stride, part_crc, map.data(), failed.data(), todo, fix))) return rc;
 	for (size_t e = 0; e < entries; ++e)
 		if (fix[e].status == LZGPU_FIX_CRC_ONLY || fix[e].status == LZGPU_FIX_CRC_CONFLICT) {
-			lz_set_error("repair_stripes: chunk %zu stripe %zu: a block still fails its stored CRC (status %d)", e / pb, e % pb, fix[e].status);
+			lz_set_error("%s: chunk %zu stripe %zu: a block still fails its stored CRC (status %d)", name, e / pb, e % pb, fix[e].status);
 			return LZGPU_ERR_CRC;
 		}
 	for (size_t e = 0; e < entries; ++e)
 		if (fix[e].status == LZGPU_FIX_UNEXPLAINED) {
-			lz_set_error("repair_stripes: chunk %zu stripe %zu is not a codeword and no single part explains it", e / pb, e % pb);
+			lz_set_error("%s: chunk %zu stripe %zu is not a codeword and %s", name, e / pb, e % pb,
+			             decode ? "no set of parts within the code's radius explains it" : "no single part explains it");
 			return LZGPU_ERR_INCONSISTENT;
 		}
 	return LZGPU_OK;
+}
+
+extern "C" int lzgpu_repair_stripes(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, uint32_t nb, uint8_t *const *parts,
+                                    size_t part_stride, const uint32_t *const *part_crc, lzgpu_stripe_repair *fix) {
+	NvtxScope nvtx_scope("lzgpu::repair_stripes");
+	return repair_host(ctx, goal, n_chunks, nb, parts, part_stride, part_crc, fix, false, "repair_stripes");
+}
+
+extern "C" int lzgpu_decode_stripes(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, uint32_t nb, uint8_t *const *parts,
+                                    size_t part_stride, const uint32_t *const *part_crc, lzgpu_stripe_decode *fix) {
+	NvtxScope nvtx_scope("lzgpu::decode_stripes");
+	return repair_host(ctx, goal, n_chunks, nb, parts, part_stride, part_crc, fix, true, "decode_stripes");
 }
 
 // ------------------------------------------------------------------------------------------------

@@ -8,6 +8,7 @@
 #include "bitslice.cuh"
 #include "fused_plan.h"
 #include "repair_rows.h"
+#include "decode_locate.h"
 
 #include <cctype>
 #include <cstdio>
@@ -480,6 +481,40 @@ int lzgpu_debug_repair_rows(int k, int m, const uint8_t *inputs, const uint8_t *
 	if (!lzd::repair_rows(k, gen, inputs, wanted, n_wanted, tb, mat, &pivot, out, 0, 1, [] {})) return LZGPU_ERR_ARG;
 	for (int w = 0; w < n_wanted; ++w) std::memcpy(rows + w * k, out + 32 * w, k);
 	return n_wanted;
+}
+
+// Diagnostics: the host build of decode_map_kernel's locator (one thread, no barrier): the punctured code's rows, then locate_errors.
+int lzgpu_debug_locate_errors(int k, int m, const uint8_t *given, const uint8_t *failed, const uint8_t *const *blocks, uint32_t len,
+                              uint64_t *located) {
+	if (k < 1 || k > LZGPU_MAX_DATA || m < 1 || m > LZGPU_MAX_PARITY || !given || !failed || !blocks || !located || len < 1) return LZGPU_ERR_ARG;
+	uint8_t pt[LZGPU_MAX_PARTS];
+	const uint8_t *blk[LZGPU_MAX_PARTS];
+	uint32_t n = 0;
+	for (int i = 0; i < k + m; ++i) {
+		if (failed[i] && !given[i]) return LZGPU_ERR_ARG;
+		if (!given[i] || failed[i]) continue;
+		if (!blocks[i]) return LZGPU_ERR_ARG;
+		blk[n] = blocks[i];
+		pt[n++] = static_cast<uint8_t>(i);
+	}
+	if (n < static_cast<uint32_t>(k)) return LZGPU_ERR_ARG;
+	uint8_t full[LZGPU_MAX_PARTS * LZGPU_MAX_DATA], gen[32 * 32] = {0};
+	lz::rs_generator(k, m, full);
+	for (int r = 0; r < m; ++r) std::memcpy(gen + 32 * r, full + (k + r) * k, k);
+	lzd::GfTables tb;
+	lzd::gf_tables_build(tb);
+	static thread_local lzd::LocateScratch sc;
+	uint8_t mat[32][64], rows[32 * 32];
+	uint32_t pivot = 0;
+	const uint32_t s = n - k;
+	if (s && !lzd::repair_rows(k, gen, pt, pt + k, s, tb, mat, &pivot, rows, 0, 1, [] {})) return LZGPU_ERR_ARG;
+	unsigned long long cols = 0;
+	const int e = lzd::locate_errors(k, s, rows, blk, len, tb, sc, 0, 1, [] {}, &cols);
+	if (e < 0) return LZGPU_ERR_INCONSISTENT;
+	*located = 0;
+	for (uint32_t q = 0; q < n; ++q)
+		if ((cols >> q) & 1ull) *located |= 1ull << pt[q];
+	return e;
 }
 
 int lzgpu_plan_convert(const lzgpu_goal *src, const lzgpu_goal *dst, const uint8_t *available, const uint8_t *want, lzgpu_convert_plan *out) {

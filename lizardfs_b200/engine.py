@@ -629,6 +629,31 @@ class Engine:
                                                _dev_ptrs(d_part_crc, n_parts), d_fix, stream)
         _check(rc, "repair_stripes_dev")
 
+    STRIPE_DECODE_DTYPE = np.dtype([("bad_rows", np.uint32), ("suspect_part", np.int32), ("status", np.int32), ("crc", np.uint32),
+                                    ("crc_failed", np.uint64), ("located", np.uint64), ("located_crc", np.uint32, (2,))])
+
+    def decode_stripes(self, goal, nb, parts, part_crc):
+        """repair_stripes, then errors-and-erasures decoding up to the code's radius where the repair gives up (lzgpu_decode_stripes):
+        up to two located blocks (valid CRC, wrong bytes) per stripe beside the failing ones.  Arguments as in repair_stripes.
+        Returns a structured array [n_chunks, pb] of STRIPE_DECODE_DTYPE (the first five fields as repair_stripes returns them unless
+        status == _lib.FIX_DECODED; located: bit p = part p's block was located and rewritten; located_crc: their new CRCs,
+        ascending part); raises ChunkCrcError when a block still fails its stored CRC after the call (its .fix holds the entries)."""
+        assert len(parts) == goal.k + goal.m
+        pb = (nb + goal.k - 1) // goal.k
+        parts, n, crcs = _host_parts(parts, part_crc, pb, in_place=True)
+        out = np.empty((n, pb), dtype=self.STRIPE_DECODE_DTYPE)
+        rc = self.lib.lzgpu_decode_stripes(self.h, C.byref(goal.c), n, nb, _ptr_array(parts), pb * BLOCK_SIZE, crcs, _p(out))
+        _check_crc(rc, "decode_stripes", (-1, -1, -1), fix=out)
+        return out
+
+    def decode_stripes_dev(self, goal, n_chunks, nb, d_parts, part_stride, d_part_crc, d_fix, stream=None):
+        """Device-pointer form of decode_stripes: the rewritten blocks go into d_parts, n_chunks * pb entries of 40 bytes to d_fix
+        (device memory, 8-byte aligned).  The call only enqueues, as repair_stripes_dev."""
+        n_parts = goal.k + goal.m
+        rc = self.lib.lzgpu_decode_stripes_dev(self.h, C.byref(goal.c), n_chunks, nb, _dev_ptrs(d_parts, n_parts), part_stride,
+                                               _dev_ptrs(d_part_crc, n_parts), d_fix, stream)
+        _check(rc, "decode_stripes_dev")
+
     # ---- wire format --------------------------------------------------------------------------
     def write_data_prefixes(self, goal, nb, crc, chunk_ids, write_id_base=0):
         """LIZ_CLTOCS_WRITE_DATA prefixes (cltocs.h:116-137) for every block of every part: uint8 [n, k+m, pb, 38]

@@ -31,7 +31,13 @@ lzgpu_correct_stripes_dev; one rotten block (bytes changed, stored CRC kept) in 
 against today's alternative, dropping part 3 and rebuilding it whole with lzgpu_recover_chunks_dev; and m rotten blocks in every
 stripe, the worst case, alone.  Both routes must return identical entries, and the rebuilt bytes must be the original ones.
 
-    python tools/bench_check.py [--chunks 16] [--iters 20] [--warmup 3] [--only degraded|repair]      (one JSON line per measurement)
+The stripe decode (lzgpu_decode_stripes_dev) is timed against the repair and the map on the same batch, alternated, as the repair is:
+clean for ec(8,3), ec(8,4) and ec(10,5); two stale parts (bytes changed, stored CRCs recomputed) in each of the first k stripes of
+every chunk (ec(8,4)); one stale and one rotten block there (ec(8,3)); two stale parts in every stripe (ec(8,4)).  The repair leaves
+those stripes unfixed.  The cost per decoded stripe, (decode - repair) / decoded stripes, is reported next to the map's locate cost,
+(map - clean map) / bad stripes.  Both routes must return identical entries, and the rewritten bytes must be the original ones.
+
+    python tools/bench_check.py [--chunks 16] [--iters 20] [--warmup 3] [--only degraded|repair|decode]      (one JSON line per measurement)
 """
 import argparse
 import json
@@ -320,6 +326,93 @@ def repair_rows(eng, generic, args, stream, info):
         torch.cuda.empty_cache()
 
 
+def decode_rows(eng, generic, args, stream, info):
+    """time the decode against the repair on the same batch: clean, two stale parts in each of the first k stripes (ec(8,4)), one
+    stale and one rotten block there (ec(8,3)), two stale parts in every stripe (ec(8,4)); next to it the map, clean and on the same
+    batch, for the locate cost per bad stripe; check both routes and the rewritten bytes"""
+    st = stream.cuda_stream
+    cases = [("ec(8,3)", "clean", [], []), ("ec(8,4)", "clean", [], []), ("ec(10,5)", "clean", [], []),
+             ("ec(8,4)", "two_stale_in_k_stripes", [(p, s) for s in range(8) for p in (1, 9)], []),
+             ("ec(8,3)", "stale_and_rotten_in_k_stripes", [(5, s) for s in range(8)], [(3, s) for s in range(8)]),
+             ("ec(8,4)", "two_stale_in_every_stripe", [(p, s) for s in range(128) for p in (1, 9)], [])]
+    r, resident, clean_map = None, None, {}
+    for text, case, stale, rotten in cases:
+        if resident != text:
+            del r
+            torch.cuda.empty_cache()
+            r, resident = Resident(eng, text, args.chunks), text
+        out_f = torch.empty(40 * r.n * r.pb, dtype=torch.uint8, device="cuda")
+        out_r = torch.empty(24 * r.n * r.pb, dtype=torch.uint8, device="cuda")
+        out_m = torch.empty(8 * r.n * r.pb, dtype=torch.uint8, device="cuda")
+        blocks = stale + rotten
+        idx = good = faulty = None
+        if blocks:                       # stale blocks get their CRCs recomputed, rotten ones keep the original
+            idx = torch.tensor([c * r.stride + p * r.part_bytes + s * BLOCK + 777 + 64 * p for c in range(r.n) for p, s in blocks],
+                               device="cuda")
+            good = r.buf[idx].clone()
+            faulty = good ^ 0x5A
+            r.buf[idx] = faulty
+            for p in {p for p, _ in stale}:
+                for c in range(r.n):
+                    eng.crc_blocks_dev(r.ptrs[p] + c * r.stride, r.pb, r.crc[p, c].data_ptr())
+            torch.cuda.synchronize()
+
+        def restore():
+            if idx is not None:
+                with torch.cuda.stream(stream):
+                    r.buf[idx] = faulty
+
+        def decode(e=eng):
+            e.decode_stripes_dev(r.goal, r.n, NB, r.ptrs, r.stride, r.crc_ptrs, out_f.data_ptr(), stream=st)
+
+        def repair():
+            eng.repair_stripes_dev(r.goal, r.n, NB, r.ptrs, r.stride, r.crc_ptrs, out_r.data_ptr(), stream=st)
+
+        def smap():
+            eng.check_stripe_map_dev(r.goal, r.n, NB, r.ptrs, r.stride, r.crc_ptrs, out_m.data_ptr(), stream=st)
+
+        t_dec = t_rep = t_map = 0.0
+        for _ in range(2):               # alternate the calls, twice: other work shares the card
+            t_dec += timed_each(decode, restore, args.iters, args.warmup, stream) / 2
+            t_rep += timed_each(repair, restore, args.iters, args.warmup, stream) / 2
+            t_map += timed_each(smap, restore, args.iters, args.warmup, stream) / 2
+        try:
+            eng.sync()
+        except L.ChunkCrcError:          # the map's deferred verdict on the rotten blocks
+            assert rotten
+        fixes = []
+        for e in (eng, generic):
+            restore()
+            torch.cuda.synchronize()
+            decode(e)
+            torch.cuda.synchronize()
+            fixes.append(out_f.cpu().numpy().view(L.Engine.STRIPE_DECODE_DTYPE).reshape(r.n, r.pb).copy())
+            if idx is not None:
+                assert (r.buf[idx] == good).all(), "a decoded block differs from the original"
+        assert fixes[0].tobytes() == fixes[1].tobytes(), "fused and generic decode entries differ"
+        n_dec = int((fixes[0]["status"] == _lib.FIX_DECODED).sum())
+        assert n_dec == r.n * len({s for _, s in blocks}), (case, n_dec)
+        assert int((fixes[0]["status"] == _lib.FIX_CLEAN).sum()) == r.n * r.pb - n_dec
+        row = {"what": "decode_stripes_dev", "goal": text, "case": case, "chunks": r.n, "chunk_mib": NB * BLOCK >> 20,
+               "decoded_stripes": n_dec, "ms_per_call": round(t_dec * 1e3, 3), "repair_stripes_dev_ms_per_call": round(t_rep * 1e3, 3),
+               "decode_over_repair": round(t_dec / t_rep, 3), "check_stripe_map_dev_ms_per_call": round(t_map * 1e3, 3)}
+        if case == "clean":
+            clean_map[text] = t_map
+        else:
+            row.update({"decode_us_per_decoded_stripe": round((t_dec - t_rep) / n_dec * 1e6, 2),
+                        "map_locate_us_per_bad_stripe": round((t_map - clean_map[text]) / n_dec * 1e6, 2)})
+        print(json.dumps({**row, "routes_agree": True, **info}), flush=True)
+        if idx is not None:              # the original bytes and CRCs: the next case starts from a clean batch
+            r.buf[idx] = good
+            for p in {p for p, _ in stale}:
+                for c in range(r.n):
+                    eng.crc_blocks_dev(r.ptrs[p] + c * r.stride, r.pb, r.crc[p, c].data_ptr())
+            torch.cuda.synchronize()
+        del out_f, out_r, out_m
+    del r
+    torch.cuda.empty_cache()
+
+
 DEGRADED = [("ec(8,2)", (1,)), ("ec(5,3)", (1,)), ("ec(8,3)", (1, 4)), ("ec(8,4)", (1,)), ("ec(8,4)", (1, 4))]
 
 
@@ -389,7 +482,8 @@ def main():
     ap.add_argument("--chunks", type=int, default=16)
     ap.add_argument("--iters", type=int, default=20)
     ap.add_argument("--warmup", type=int, default=3)
-    ap.add_argument("--only", choices=["degraded", "repair"], default=None, help="run only the degraded-map rows, or only the repair rows")
+    ap.add_argument("--only", choices=["degraded", "repair", "decode"], default=None,
+                    help="run only the degraded-map rows, the repair rows or the decode rows")
     args = ap.parse_args()
     info = card()
     eng = L.Engine(0)
@@ -404,6 +498,8 @@ def main():
         degraded_rows(eng, generic, args, stream, info)
     if args.only in (None, "repair"):
         repair_rows(eng, generic, args, stream, info)
+    if args.only in (None, "decode"):
+        decode_rows(eng, generic, args, stream, info)
     generic.set_deferred_verify(False)
     for text in (GOALS if args.only is None else []):
         r = Resident(eng, text, args.chunks)
