@@ -62,6 +62,37 @@ __device__ __forceinline__ void correct_crc_part(uint32_t st, uint32_t shift, ui
 	if ((threadIdx.x & 31) == 0) s_out[threadIdx.x >> 5] = st;
 }
 
+// the CRC of the 64 KiB block whose thread-t bytes are acc, in every thread (one barrier publishes s_out)
+__device__ __forceinline__ uint32_t block_crc(const uint32_t (&acc)[64], const uint32_t *s_tab, uint32_t shift, uint32_t *s_out) {
+	uint32_t st = 0;
+#pragma unroll
+	for (int i = 0; i < 64; ++i) st = crc_step_word(st, acc[i], s_tab);
+	correct_crc_part(st, shift, s_out);
+	__syncthreads();
+	uint32_t crc = kCrcZeroBlock64K;
+#pragma unroll
+	for (int w = 0; w < 8; ++w) crc ^= s_out[w];
+	return crc;
+}
+
+// thread t's 256 bytes of acc over its part of the block
+__device__ __forceinline__ void block_store(uint8_t *blk, const uint32_t (&acc)[64]) {
+	uint4 *dst = reinterpret_cast<uint4 *>(blk) + threadIdx.x * 16;
+#pragma unroll
+	for (int i = 0; i < 16; ++i) dst[i] = make_uint4(acc[4 * i], acc[4 * i + 1], acc[4 * i + 2], acc[4 * i + 3]);
+}
+
+// the per-CTA setup, on the first entry with work: the slicing tables, this thread's shift and (s_gf given) the GF tables
+__device__ __forceinline__ void cta_setup(bool &ready, uint32_t &shift, uint32_t *s_tab, GfTables *s_gf, const uint32_t *tables,
+                                          const uint32_t *pow2) {
+	if (ready) return;
+	const unsigned t = threadIdx.x;
+	for (unsigned i = t; i < 1024; i += 256) s_tab[i] = tables[i];
+	if (s_gf && t == 0) gf_tables_build(*s_gf);
+	shift = crc_xpow_bytes_dev(256u * (255u - t), pow2);
+	ready = true;
+}
+
 __global__ void __launch_bounds__(256) correct_map_kernel(const CorrectArgs a) {
 	__shared__ uint32_t s_tab[1024];
 	__shared__ CoefPlanes s_coef[32];
@@ -77,11 +108,7 @@ __global__ void __launch_bounds__(256) correct_map_kernel(const CorrectArgs a) {
 			if (t == 0) a.fix[e] = lzgpu_stripe_fix{bad_rows, suspect, bad_rows ? LZGPU_FIX_UNEXPLAINED : LZGPU_FIX_CLEAN, 0u};
 			continue;
 		}
-		if (!ready) {  // first entry with a suspect: tables and this thread's shift
-			for (unsigned i = t; i < 1024; i += 256) s_tab[i] = a.tables[i];
-			shift = crc_xpow_bytes_dev(256u * (255u - t), a.pow2);
-			ready = true;
-		}
+		cta_setup(ready, shift, s_tab, nullptr, a.tables, a.pow2);
 		if (t < a.k) coef_planes_set(s_coef[t], a.coef[suspect][t]);
 		__syncthreads();
 		const unsigned long long off = (e / a.pb) * a.part_stride + (e % a.pb) * 65536ull;
@@ -119,21 +146,8 @@ __global__ void __launch_bounds__(256) correct_map_kernel(const CorrectArgs a) {
 		const bool conflict = __syncthreads_or(fail);
 		uint32_t crc = 0;
 		if (!conflict) {
-			uint4 *dst = reinterpret_cast<uint4 *>(a.part[suspect] + off) + t * 16;
-#pragma unroll
-			for (int i = 0; i < 16; ++i) dst[i] = make_uint4(acc[4 * i], acc[4 * i + 1], acc[4 * i + 2], acc[4 * i + 3]);
-			if (a.crc_disabled) {
-				crc = LZGPU_FAKE_CRC;
-			} else {
-				uint32_t st = 0;
-#pragma unroll
-				for (int i = 0; i < 64; ++i) st = crc_step_word(st, acc[i], s_tab);
-				correct_crc_part(st, shift, s_out);
-				__syncthreads();
-				crc = kCrcZeroBlock64K;
-#pragma unroll
-				for (int w = 0; w < 8; ++w) crc ^= s_out[w];
-			}
+			block_store(a.part[suspect] + off, acc);
+			crc = a.crc_disabled ? LZGPU_FAKE_CRC : block_crc(acc, s_tab, shift, s_out);
 		}
 		if (t == 0) a.fix[e] = lzgpu_stripe_fix{bad_rows, suspect, conflict ? LZGPU_FIX_CRC_CONFLICT : LZGPU_FIX_CORRECTED, crc};
 		__syncthreads();  // s_coef, s_lin and s_out are re-used by the next entry
@@ -176,22 +190,9 @@ __device__ __forceinline__ uint32_t repair_block(const RepairArgs &a, unsigned l
 		if (ones) correct_read<false, 1>(blk, acc, s_coef[0], s_tab);
 		else correct_read<false, 2>(blk, acc, s_coef[j], s_tab);
 	}
-	uint32_t st = 0;
-#pragma unroll
-	for (int i = 0; i < 64; ++i) st = crc_step_word(st, acc[i], s_tab);
-	correct_crc_part(st, shift, s_out);
-	__syncthreads();
-	uint32_t crc = kCrcZeroBlock64K;
-#pragma unroll
-	for (int w = 0; w < 8; ++w) crc ^= s_out[w];
+	const uint32_t crc = block_crc(acc, s_tab, shift, s_out);
 	__syncthreads();  // s_coef and s_out are re-used by the next block
 	return crc;
-}
-
-__device__ __forceinline__ void repair_store(uint8_t *blk, const uint32_t (&acc)[64]) {
-	uint4 *dst = reinterpret_cast<uint4 *>(blk) + threadIdx.x * 16;
-#pragma unroll
-	for (int i = 0; i < 16; ++i) dst[i] = make_uint4(acc[4 * i], acc[4 * i + 1], acc[4 * i + 2], acc[4 * i + 3]);
 }
 
 struct CtaSync {
@@ -216,14 +217,20 @@ LZ_HD inline int repair_rule(uint32_t bad_rows, int suspect, unsigned long long 
 	return LZGPU_FIX_REBUILT;
 }
 
+// the shared arrays of a rebuild (repair_rows' matrix and pivot, the inputs, the targets, their rows, the coefficient planes of one
+// row and the CTA's CRC partials)
+struct RebuildShared {
+	CoefPlanes coef[32];
+	uint8_t mat[32][64];
+	uint8_t rows[32 * 32];
+	uint8_t in[32], want[64];
+	uint32_t pivot, out[8];
+};
+
 __global__ void __launch_bounds__(256) repair_map_kernel(const RepairArgs a) {
 	__shared__ uint32_t s_tab[1024];
-	__shared__ CoefPlanes s_coef[32];
 	__shared__ GfTables s_gf;
-	__shared__ uint8_t s_mat[32][64];
-	__shared__ uint8_t s_rows[32 * 32];
-	__shared__ uint8_t s_in[32], s_want[64];
-	__shared__ uint32_t s_pivot, s_out[8];
+	__shared__ RebuildShared s;
 	const unsigned t = threadIdx.x;
 	const int spare = __popcll(a.given) - static_cast<int>(a.k);
 	bool ready = false;
@@ -238,46 +245,41 @@ __global__ void __launch_bounds__(256) repair_map_kernel(const RepairArgs a) {
 			if (t == 0) a.fix[e] = lzgpu_stripe_repair{bad_rows, suspect, status, 0u, f};
 			continue;
 		}
-		if (!ready) {  // first entry with work: tables and this thread's shift
-			for (unsigned i = t; i < 1024; i += 256) s_tab[i] = a.tables[i];
-			if (t == 0) gf_tables_build(s_gf);
-			shift = crc_xpow_bytes_dev(256u * (255u - t), a.pow2);
-			ready = true;
-		}
+		cta_setup(ready, shift, s_tab, &s_gf, a.tables, a.pow2);
 		if (t == 0) {
 			uint32_t ni = 0, nw = 0;
 			for (uint32_t p = 0; p < a.n_parts; ++p) {
 				if (!((a.given >> p) & 1ull)) continue;
-				if ((x >> p) & 1ull) s_want[nw++] = static_cast<uint8_t>(p);
-				else if (ni < a.k) s_in[ni++] = static_cast<uint8_t>(p);
+				if ((x >> p) & 1ull) s.want[nw++] = static_cast<uint8_t>(p);
+				else if (ni < a.k) s.in[ni++] = static_cast<uint8_t>(p);
 			}
 		}
 		__syncthreads();
 		const uint32_t nw = static_cast<uint32_t>(__popcll(x));
 		const unsigned long long off = (e / a.pb) * a.part_stride + (e % a.pb) * 65536ull;
 		uint32_t crc = 0;
-		if (!repair_rows(a.k, a.gen, s_in, s_want, nw, s_gf, s_mat, &s_pivot, s_rows, t, 256u, CtaSync())) {
+		if (!repair_rows(a.k, a.gen, s.in, s.want, nw, s_gf, s.mat, &s.pivot, s.rows, t, 256u, CtaSync())) {
 			status = f ? LZGPU_FIX_CRC_CONFLICT : LZGPU_FIX_UNEXPLAINED;  // a singular pattern: nothing rebuilt
 		} else {
 			uint32_t acc[64];
 			bool match = true;
 			for (uint32_t w = 0; w < nw && match; ++w) {
-				crc = repair_block(a, off, s_in, s_rows + 32 * w, acc, s_coef, s_tab, shift, s_out);
-				match = !f || crc == a.crc[s_want[w]][e];  // e = chunk * pb + block
+				crc = repair_block(a, off, s.in, s.rows + 32 * w, acc, s.coef, s_tab, shift, s.out);
+				match = !f || crc == a.crc[s.want[w]][e];  // e = chunk * pb + block
 			}
 			if (!match) {
 				status = LZGPU_FIX_CRC_CONFLICT;
 			} else {
-				repair_store(a.part[s_want[nw - 1]] + off, acc);
+				block_store(a.part[s.want[nw - 1]] + off, acc);
 				for (uint32_t w = 0; w + 1 < nw; ++w) {
-					repair_block(a, off, s_in, s_rows + 32 * w, acc, s_coef, s_tab, shift, s_out);
-					repair_store(a.part[s_want[w]] + off, acc);
+					repair_block(a, off, s.in, s.rows + 32 * w, acc, s.coef, s_tab, shift, s.out);
+					block_store(a.part[s.want[w]] + off, acc);
 				}
 			}
 			if (f) crc = 0;  // REBUILT: the blocks match the CRCs the caller already has
 		}
 		if (t == 0) a.fix[e] = lzgpu_stripe_repair{bad_rows, suspect, status, status == LZGPU_FIX_CORRECTED ? crc : 0u, f};
-		__syncthreads();  // s_in, s_want and s_rows are re-used by the next entry
+		__syncthreads();  // s.in, s.want and s.rows are re-used by the next entry
 	}
 }
 
@@ -303,14 +305,11 @@ LZ_HD inline bool decode_eligible(int status, unsigned long long f, int spare) {
 __global__ void __launch_bounds__(256) decode_map_kernel(const DecodeArgs d) {
 	const RepairArgs &a = d.r;
 	__shared__ uint32_t s_tab[1024];
-	__shared__ CoefPlanes s_coef[32];
 	__shared__ GfTables s_gf;
-	__shared__ uint8_t s_mat[32][64];
-	__shared__ uint8_t s_rows[32 * 32];
-	__shared__ uint8_t s_pt[64], s_in[32], s_want[64];
+	__shared__ RebuildShared s;
+	__shared__ uint8_t s_pt[64];
 	__shared__ const uint8_t *s_blk[64];
 	__shared__ LocateScratch s_loc;
-	__shared__ uint32_t s_pivot, s_out[8];
 	const unsigned t = threadIdx.x;
 	const int spare = __popcll(a.given) - static_cast<int>(a.k);
 	bool ready = false;
@@ -322,12 +321,7 @@ __global__ void __launch_bounds__(256) decode_map_kernel(const DecodeArgs d) {
 			if (t == 0) d.fix[e] = lzgpu_stripe_decode{r.bad_rows, r.suspect_part, r.status, r.crc, f, 0ull, {0u, 0u}};
 			continue;
 		}
-		if (!ready) {  // first entry with work: tables and this thread's shift
-			for (unsigned i = t; i < 1024; i += 256) s_tab[i] = a.tables[i];
-			if (t == 0) gf_tables_build(s_gf);
-			shift = crc_xpow_bytes_dev(256u * (255u - t), a.pow2);
-			ready = true;
-		}
+		cta_setup(ready, shift, s_tab, &s_gf, a.tables, a.pow2);
 		const unsigned long long off = (e / a.pb) * a.part_stride + (e % a.pb) * 65536ull;
 		const unsigned long long kept = a.given & ~f;
 		const uint32_t sp = static_cast<uint32_t>(__popcll(kept)) - a.k;
@@ -344,36 +338,37 @@ __global__ void __launch_bounds__(256) decode_map_kernel(const DecodeArgs d) {
 		unsigned long long located = 0;
 		uint32_t lcrc[2] = {0u, 0u};
 		unsigned long long cols = 0;
-		if (repair_rows(a.k, a.gen, s_pt, s_pt + a.k, sp, s_gf, s_mat, &s_pivot, s_rows, t, 256u, CtaSync()) &&
-		    locate_errors(a.k, sp, s_rows, s_blk, 65536u, s_gf, s_loc, t, 256u, CtaSync(), &cols) > 0) {
+		if (repair_rows(a.k, a.gen, s_pt, s_pt + a.k, sp, s_gf, s.mat, &s.pivot, s.rows, t, 256u, CtaSync()) &&
+		    locate_errors(a.k, sp, s.rows, s_blk, 65536u, s_gf, s_loc, t, 256u, CtaSync(), &cols) > 0) {
 			for (unsigned long long b = cols; b; b &= b - 1) located |= 1ull << s_pt[__ffsll(static_cast<long long>(b)) - 1];
-			const unsigned long long x = f | located;
 			__syncthreads();  // every thread has read s_pt
+			// X = F | E, F gated; E's CRCs go into the entry
+			const unsigned long long x = f | located;
 			if (t == 0) {
 				uint32_t ni = 0, nw = 0;
 				for (uint32_t p = 0; p < a.n_parts; ++p) {
 					if (!((a.given >> p) & 1ull)) continue;
-					if ((x >> p) & 1ull) s_want[nw++] = static_cast<uint8_t>(p);
-					else if (ni < a.k) s_in[ni++] = static_cast<uint8_t>(p);
+					if ((x >> p) & 1ull) s.want[nw++] = static_cast<uint8_t>(p);
+					else if (ni < a.k) s.in[ni++] = static_cast<uint8_t>(p);
 				}
 			}
 			__syncthreads();
 			const uint32_t nw = static_cast<uint32_t>(__popcll(x));
-			if (repair_rows(a.k, a.gen, s_in, s_want, nw, s_gf, s_mat, &s_pivot, s_rows, t, 256u, CtaSync())) {
+			if (repair_rows(a.k, a.gen, s.in, s.want, nw, s_gf, s.mat, &s.pivot, s.rows, t, 256u, CtaSync())) {
 				uint32_t acc[64];
 				bool match = true;
 				uint32_t nl = 0;
 				for (uint32_t w = 0; w < nw && match; ++w) {
-					const uint32_t crc = repair_block(a, off, s_in, s_rows + 32 * w, acc, s_coef, s_tab, shift, s_out);
-					if ((f >> s_want[w]) & 1ull) match = crc == a.crc[s_want[w]][e];  // e = chunk * pb + block
+					const uint32_t crc = repair_block(a, off, s.in, s.rows + 32 * w, acc, s.coef, s_tab, shift, s.out);
+					if ((f >> s.want[w]) & 1ull) match = crc == a.crc[s.want[w]][e];  // e = chunk * pb + block
 					else if (nl++) lcrc[1] = crc;
 					else lcrc[0] = crc;
 				}
 				if (match) {
-					repair_store(a.part[s_want[nw - 1]] + off, acc);
+					block_store(a.part[s.want[nw - 1]] + off, acc);
 					for (uint32_t w = 0; w + 1 < nw; ++w) {
-						repair_block(a, off, s_in, s_rows + 32 * w, acc, s_coef, s_tab, shift, s_out);
-						repair_store(a.part[s_want[w]] + off, acc);
+						repair_block(a, off, s.in, s.rows + 32 * w, acc, s.coef, s_tab, shift, s.out);
+						block_store(a.part[s.want[w]] + off, acc);
 					}
 					status = LZGPU_FIX_DECODED;
 				}
@@ -382,7 +377,7 @@ __global__ void __launch_bounds__(256) decode_map_kernel(const DecodeArgs d) {
 		if (status != LZGPU_FIX_DECODED) located = 0, lcrc[0] = lcrc[1] = 0;
 		if (t == 0)
 			d.fix[e] = lzgpu_stripe_decode{r.bad_rows, r.suspect_part, status, status == LZGPU_FIX_DECODED ? 0u : r.crc, f, located, {lcrc[0], lcrc[1]}};
-		__syncthreads();  // s_pt, s_blk, s_in, s_want, s_rows and s_loc are re-used by the next entry
+		__syncthreads();  // s_pt, s_blk, s.in, s.want, s.rows and s_loc are re-used by the next entry
 	}
 }
 

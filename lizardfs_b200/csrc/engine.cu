@@ -1400,9 +1400,32 @@ extern "C" int lzgpu_check_stripe_map_degraded(lzgpu_ctx *ctx, const lzgpu_goal 
 // ------------------------------------------------------------------------------------------------
 static_assert(sizeof(lzgpu_stripe_fix) == 16 && sizeof(lzgpu_stripe_state) == 8, "fix and map entries as the kernels write them");
 
+// part i and its stored CRCs into a.part[i] / a.crc[i] (nullptr: not given, no CRCs); returns the given mask, and its size in *n_given
+template <class Args>
+static unsigned long long fix_parts(Args &a, int n, void *const *parts, const void *const *part_crc, int *n_given = nullptr) {
+	unsigned long long given = 0;
+	for (int i = 0; i < n; ++i) {
+		a.part[i] = static_cast<uint8_t *>(parts[i]);
+		a.crc[i] = parts[i] && part_crc ? static_cast<const uint32_t *>(part_crc[i]) : nullptr;
+		given |= parts[i] ? 1ull << i : 0ull;
+	}
+	if (n_given) *n_given = __builtin_popcountll(given);
+	return given;
+}
+
+// the tail of the correction's and the repair's kernel arguments
+template <class Args>
+static void fix_tail(lzgpu_ctx *ctx, Args &a, unsigned long long n_entries, uint32_t pb, size_t part_stride) {
+	a.tables = ctx->d_crc_tables;
+	a.part_stride = part_stride;
+	a.n_entries = n_entries;
+	a.pb = pb;
+	lz::crc_xpow2_table(a.pow2);
+}
+
 // The coefficient rows of every part that can be named (given, with k other given parts) for the parts given in `given`: the
 // suspect's block from the first k given parts other than it, the inputs ECReadPlan::recoverParts picks when it is unavailable.
-static int correct_table(const lzgpu_goal *goal, unsigned long long given, CorrectArgs &a) {
+static int fix_table(const lzgpu_goal *goal, unsigned long long given, CorrectArgs &a) {
 	const int k = goal->k, n = goal->k + goal->m;
 	a.given = given;
 	a.n_parts = n;
@@ -1432,174 +1455,18 @@ static int correct_table(const lzgpu_goal *goal, unsigned long long given, Corre
 	return LZGPU_OK;
 }
 
-// correct_map_kernel over n_entries map entries (pb per chunk) on `st`; a carries the table (correct_table) and the part pointers
-static int correct_enqueue(lzgpu_ctx *ctx, CorrectArgs &a, unsigned long long n_entries, uint32_t pb, size_t part_stride, const void *d_map,
-                           void *d_fix, cudaStream_t st) {
+// correct_map_kernel over n_entries map entries (pb per chunk) on `st`; a carries the table (fix_table) and the part pointers.  The
+// correction takes no F words (d_failed: unused).
+static int fix_enqueue(lzgpu_ctx *ctx, CorrectArgs &a, unsigned long long n_entries, uint32_t pb, size_t part_stride, const void *d_map,
+                       const void *d_failed, lzgpu_stripe_fix *d_fix, cudaStream_t st) {
 	a.map = static_cast<const uint32_t *>(d_map);
-	a.fix = static_cast<lzgpu_stripe_fix *>(d_fix);
-	a.tables = ctx->d_crc_tables;
-	a.part_stride = part_stride;
-	a.n_entries = n_entries;
-	a.pb = pb;
+	a.fix = d_fix;
 	a.crc_disabled = lzgpu_crc_enabled() ? 0 : 1;
-	uint32_t x = 0x00800000u;  // x^8
-	for (int i = 0; i < 32; ++i) {
-		a.pow2[i] = x;
-		x = lz::crc_mulmod(x, x);
-	}
+	fix_tail(ctx, a, n_entries, pb, part_stride);
 	correct_map_kernel<<<grid_for(ctx, n_entries * 256, 256, 2), 256, 0, st>>>(a);
 	CUDA_TRY(cudaGetLastError());
 	ctx->stats.kernel_launches++;
 	return LZGPU_OK;
-}
-
-static int correct_dev(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, uint32_t nb, void *const *d_parts, size_t part_stride,
-                       const void *const *d_part_crc, void *d_fix, int64_t *bad, void *stream, bool degraded) {
-	int rc = check_args(ctx, goal, nb, d_parts, d_part_crc, d_fix, true, degraded);
-	if (rc) return rc;
-	if (n_chunks == 0) return LZGPU_OK;
-	const int n = goal->k + goal->m;
-	const uint32_t pb = (nb + goal->k - 1) / goal->k;
-	const unsigned long long entries = static_cast<unsigned long long>(n_chunks) * pb;
-	CorrectArgs a{};
-	unsigned long long given = 0;
-	for (int i = 0; i < n; ++i) {
-		a.part[i] = static_cast<uint8_t *>(d_parts[i]);
-		a.crc[i] = d_parts[i] && d_part_crc ? static_cast<const uint32_t *>(d_part_crc[i]) : nullptr;
-		given |= d_parts[i] ? 1ull << i : 0ull;
-	}
-	if ((rc = correct_table(goal, given, a))) return rc;  // before anything is enqueued: no host work between check and correction
-	// the map's bytes and one fix entry per stripe; the corrected blocks are not counted (the host does not know them here)
-	const uint64_t alg_bytes = check_alg_bytes(goal, n_chunks, nb, d_parts, d_part_crc, true) + entries * sizeof(lzgpu_stripe_fix);
-	return dev_call(ctx, stream, alg_bytes, bad, [&](cudaStream_t st, VerifyTicket *tk) {
-		TmpBuf map(ctx, st);  // the map kernels write 8-byte entries; correct_map_kernel copies them into the 16-byte fix entries
-		int rc;
-		if ((rc = map.alloc(entries * sizeof(lzgpu_stripe_state))) ||
-		    (rc = check_enqueue(ctx, goal, n_chunks, nb, d_parts, part_stride, d_part_crc, map.p, st, tk, true)))
-			return rc;
-		return correct_enqueue(ctx, a, entries, pb, part_stride, map.p, d_fix, st);
-	});
-}
-
-extern "C" int lzgpu_correct_stripes_dev(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, uint32_t nb, void *const *d_parts,
-                                         size_t part_stride, const void *const *d_part_crc, void *d_fix, int64_t *bad, void *stream) {
-	NvtxScope nvtx_scope("lzgpu::correct_stripes_dev");
-	return correct_dev(ctx, goal, n_chunks, nb, d_parts, part_stride, d_part_crc, d_fix, bad, stream, false);
-}
-
-extern "C" int lzgpu_correct_stripes_degraded_dev(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, uint32_t nb, void *const *d_parts,
-                                                  size_t part_stride, const void *const *d_part_crc, void *d_fix, int64_t *bad, void *stream) {
-	NvtxScope nvtx_scope("lzgpu::correct_stripes_degraded_dev");
-	return correct_dev(ctx, goal, n_chunks, nb, d_parts, part_stride, d_part_crc, d_fix, bad, stream, true);
-}
-
-// The host-pointer correction, phase 2: the stripes `todo` (map indices with a suspect) gathered into one-stripe "chunks" (pb = 1:
-// the parts are zero-padded, so a short last stripe has the same syndromes), tile by tile, through correct_map_kernel with the map
-// entries the check found; the fix entries go to fix[], the corrected blocks back into the caller's parts.
-static int correct_host_stripes(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t pb, uint8_t *const *parts, size_t part_stride,
-                                const uint32_t *const *part_crc, const lzgpu_stripe_state *map, const std::vector<size_t> &todo,
-                                lzgpu_stripe_fix *fix) {
-	const int n = goal->k + goal->m;
-	const size_t B = LZGPU_BLOCK_SIZE;
-	unsigned long long given = 0;
-	int n_given = 0;
-	for (int i = 0; i < n; ++i)
-		if (parts[i]) {
-			given |= 1ull << i;
-			++n_given;
-		}
-	CorrectArgs a{};
-	int rc = correct_table(goal, given, a);
-	if (rc) return rc;
-	std::lock_guard<std::mutex> lk(ctx->mu);
-	DeviceGuard g(ctx->device);
-	const size_t tile = std::max<size_t>(1, std::min<size_t>(todo.size(), (2 * kHostTileBytes) / (B * n_given)));
-	void *d_in, *d_crc, *d_entries;
-	if ((rc = lz_scratch(ctx, kScratchIn0, tile * B * n, &d_in)) || (rc = lz_scratch(ctx, kScratchCrc0, tile * 4 * n, &d_crc)) ||
-	    (rc = lz_scratch(ctx, kScratchPar0, tile * (sizeof(lzgpu_stripe_state) + sizeof(lzgpu_stripe_fix)), &d_entries)))
-		return rc;
-	void *d_map = d_entries;
-	void *d_fix = static_cast<uint8_t *>(d_entries) + tile * sizeof(lzgpu_stripe_state);
-	for (int i = 0; i < n; ++i) {
-		a.part[i] = parts[i] ? static_cast<uint8_t *>(d_in) + tile * B * i : nullptr;
-		a.crc[i] = parts[i] && part_crc && part_crc[i] ? static_cast<const uint32_t *>(d_crc) + tile * i : nullptr;
-	}
-	std::vector<uint32_t> h_crc(tile * n);
-	std::vector<lzgpu_stripe_state> h_map(tile);
-	std::vector<lzgpu_stripe_fix> h_fix(tile);
-	cudaStream_t st = ctx->slot_stream[0];
-	for (size_t t0 = 0; t0 < todo.size(); t0 += tile) {
-		const size_t nt = std::min(tile, todo.size() - t0);
-		for (size_t j = 0; j < nt; ++j) {
-			const size_t e = todo[t0 + j], c = e / pb, s = e % pb;
-			for (int i = 0; i < n; ++i) {
-				if (!parts[i]) continue;
-				CUDA_TRY(cudaMemcpyAsync(a.part[i] + j * B, parts[i] + c * part_stride + s * B, B, cudaMemcpyHostToDevice, st));
-				if (a.crc[i]) h_crc[tile * i + j] = part_crc[i][e];
-			}
-			h_map[j] = map[e];
-		}
-		ctx->stats.bytes_h2d += nt * n_given * B;
-		CUDA_TRY(cudaMemcpyAsync(d_crc, h_crc.data(), tile * 4 * n, cudaMemcpyHostToDevice, st));
-		CUDA_TRY(cudaMemcpyAsync(d_map, h_map.data(), nt * sizeof(lzgpu_stripe_state), cudaMemcpyHostToDevice, st));
-		{
-			BatchTimer timer(ctx, st, nt * (n_given * B + sizeof(lzgpu_stripe_state) + sizeof(lzgpu_stripe_fix)));
-			if ((rc = correct_enqueue(ctx, a, nt, 1, B, d_map, d_fix, st))) return rc;
-		}
-		CUDA_TRY(cudaMemcpyAsync(h_fix.data(), d_fix, nt * sizeof(lzgpu_stripe_fix), cudaMemcpyDeviceToHost, st));
-		CUDA_TRY(cudaStreamSynchronize(st));
-		for (size_t j = 0; j < nt; ++j) {
-			const size_t e = todo[t0 + j], c = e / pb, s = e % pb;
-			fix[e] = h_fix[j];
-			if (h_fix[j].status != LZGPU_FIX_CORRECTED) continue;
-			const int p = h_fix[j].suspect_part;
-			CUDA_TRY(cudaMemcpyAsync(parts[p] + c * part_stride + s * B, a.part[p] + j * B, B, cudaMemcpyDeviceToHost, st));
-			ctx->stats.bytes_d2h += B;
-		}
-		CUDA_TRY(cudaStreamSynchronize(st));
-	}
-	return LZGPU_OK;
-}
-
-static int correct_host(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, uint32_t nb, uint8_t *const *parts, size_t part_stride,
-                        const uint32_t *const *part_crc, lzgpu_stripe_fix *fix, int64_t *bad, bool degraded) {
-	if (!fix) return LZGPU_ERR_ARG;
-	// phase 1: the map of the whole batch through the check's tile pipeline (only the map comes back)
-	const uint32_t pb = goal && goal->k > 0 ? (nb + goal->k - 1) / goal->k : 0;
-	std::vector<lzgpu_stripe_state> map(std::max<size_t>(1, static_cast<size_t>(n_chunks) * pb));
-	const int check_rc = check_host(ctx, goal, n_chunks, nb, parts, part_stride, part_crc, map.data(), bad, true, degraded);
-	if (check_rc != LZGPU_OK && check_rc != LZGPU_ERR_CRC && check_rc != LZGPU_ERR_INCONSISTENT) return check_rc;
-	if (n_chunks == 0) return LZGPU_OK;
-	std::vector<size_t> todo;
-	for (size_t e = 0; e < static_cast<size_t>(n_chunks) * pb; ++e) {
-		const lzgpu_stripe_state &m = map[e];
-		fix[e] = lzgpu_stripe_fix{m.bad_rows, m.suspect_part, m.bad_rows ? LZGPU_FIX_UNEXPLAINED : LZGPU_FIX_CLEAN, 0u};
-		if (m.bad_rows && m.suspect_part >= 0) todo.push_back(e);
-	}
-	// phase 2: only the stripes with a suspect travel again
-	if (!todo.empty()) {
-		const int rc = correct_host_stripes(ctx, goal, pb, parts, part_stride, part_crc, map.data(), todo, fix);
-		if (rc) return rc;
-	}
-	if (check_rc == LZGPU_ERR_CRC) return check_rc;  // bad[0..2] and the message as the map set them
-	for (size_t e = 0; e < static_cast<size_t>(n_chunks) * pb; ++e)
-		if (fix[e].status == LZGPU_FIX_UNEXPLAINED) {
-			lz_set_error("correct_stripes: chunk %zu stripe %zu is not a codeword and no single part explains it", e / pb, e % pb);
-			return LZGPU_ERR_INCONSISTENT;
-		}
-	return LZGPU_OK;
-}
-
-extern "C" int lzgpu_correct_stripes(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, uint32_t nb, uint8_t *const *parts,
-                                     size_t part_stride, const uint32_t *const *part_crc, lzgpu_stripe_fix *fix, int64_t *bad) {
-	NvtxScope nvtx_scope("lzgpu::correct_stripes");
-	return correct_host(ctx, goal, n_chunks, nb, parts, part_stride, part_crc, fix, bad, false);
-}
-
-extern "C" int lzgpu_correct_stripes_degraded(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, uint32_t nb, uint8_t *const *parts,
-                                              size_t part_stride, const uint32_t *const *part_crc, lzgpu_stripe_fix *fix, int64_t *bad) {
-	NvtxScope nvtx_scope("lzgpu::correct_stripes_degraded");
-	return correct_host(ctx, goal, n_chunks, nb, parts, part_stride, part_crc, fix, bad, true);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -1624,30 +1491,23 @@ static int repair_args(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t nb, cons
 }
 
 // the goal's part of the kernel arguments: the given parts and the generator's parity rows
-static void repair_table(const lzgpu_goal *goal, unsigned long long given, RepairArgs &a) {
+static int fix_table(const lzgpu_goal *goal, unsigned long long given, RepairArgs &a) {
 	uint8_t rows[LZGPU_MAX_PARITY * LZGPU_MAX_DATA];
 	goal_parity_rows(goal, rows);
 	for (int r = 0; r < goal->m; ++r) std::memcpy(a.gen + 32 * r, rows + r * goal->k, goal->k);
 	a.given = given;
 	a.n_parts = goal->k + goal->m;
 	a.k = goal->k;
+	return LZGPU_OK;
 }
 
-// repair_map_kernel over n_entries entries (pb per chunk) on `st`; a carries the table (repair_table) and the part and CRC pointers
-static int repair_enqueue(lzgpu_ctx *ctx, RepairArgs &a, unsigned long long n_entries, uint32_t pb, size_t part_stride, const void *d_map,
-                          const void *d_failed, lzgpu_stripe_repair *d_fix, cudaStream_t st) {
+// repair_map_kernel over n_entries entries (pb per chunk) on `st`; a carries the table (fix_table) and the part and CRC pointers
+static int fix_enqueue(lzgpu_ctx *ctx, RepairArgs &a, unsigned long long n_entries, uint32_t pb, size_t part_stride, const void *d_map,
+                       const void *d_failed, lzgpu_stripe_repair *d_fix, cudaStream_t st) {
 	a.map = static_cast<const uint32_t *>(d_map);
 	a.failed = static_cast<const unsigned long long *>(d_failed);
 	a.fix = d_fix;
-	a.tables = ctx->d_crc_tables;
-	a.part_stride = part_stride;
-	a.n_entries = n_entries;
-	a.pb = pb;
-	uint32_t x = 0x00800000u;  // x^8
-	for (int i = 0; i < 32; ++i) {
-		a.pow2[i] = x;
-		x = lz::crc_mulmod(x, x);
-	}
+	fix_tail(ctx, a, n_entries, pb, part_stride);
 	repair_map_kernel<<<grid_for(ctx, n_entries * 256, 256, 2), 256, 0, st>>>(a);
 	CUDA_TRY(cudaGetLastError());
 	ctx->stats.kernel_launches++;
@@ -1655,12 +1515,12 @@ static int repair_enqueue(lzgpu_ctx *ctx, RepairArgs &a, unsigned long long n_en
 }
 
 // lzgpu_decode_stripes: the repair into a stream-ordered temporary of repair entries, then decode_map_kernel over them
-static int repair_enqueue(lzgpu_ctx *ctx, RepairArgs &a, unsigned long long n_entries, uint32_t pb, size_t part_stride, const void *d_map,
-                          const void *d_failed, lzgpu_stripe_decode *d_fix, cudaStream_t st) {
+static int fix_enqueue(lzgpu_ctx *ctx, RepairArgs &a, unsigned long long n_entries, uint32_t pb, size_t part_stride, const void *d_map,
+                       const void *d_failed, lzgpu_stripe_decode *d_fix, cudaStream_t st) {
 	TmpBuf rep(ctx, st);
 	int rc;
 	if ((rc = rep.alloc(n_entries * sizeof(lzgpu_stripe_repair))) ||
-	    (rc = repair_enqueue(ctx, a, n_entries, pb, part_stride, d_map, d_failed, static_cast<lzgpu_stripe_repair *>(rep.p), st)))
+	    (rc = fix_enqueue(ctx, a, n_entries, pb, part_stride, d_map, d_failed, static_cast<lzgpu_stripe_repair *>(rep.p), st)))
 		return rc;
 	const DecodeArgs d{a, static_cast<const lzgpu_stripe_repair *>(rep.p), d_fix};
 	decode_map_kernel<<<grid_for(ctx, n_entries * 256, 256, 2), 256, 0, st>>>(d);
@@ -1670,6 +1530,7 @@ static int repair_enqueue(lzgpu_ctx *ctx, RepairArgs &a, unsigned long long n_en
 }
 
 // the blocks an entry says were written in place
+static unsigned long long fix_written(const lzgpu_stripe_fix &f) { return f.status == LZGPU_FIX_CORRECTED ? 1ull << f.suspect_part : 0ull; }
 static unsigned long long fix_written(const lzgpu_stripe_repair &f) {
 	if (f.status == LZGPU_FIX_CORRECTED) return 1ull << f.suspect_part;
 	return f.status == LZGPU_FIX_REBUILT ? f.crc_failed : 0ull;
@@ -1679,83 +1540,99 @@ static unsigned long long fix_written(const lzgpu_stripe_decode &f) {
 	return f.status == LZGPU_FIX_REBUILT || f.status == LZGPU_FIX_DECODED ? f.crc_failed | f.located : 0ull;
 }
 
-// the repair's and the decode's _dev call (Fix: the entry kind, which picks the kernels)
+// The entry kind picks the kernel arguments, and whether the check's F words (the blocks that fail their stored CRCs) go with the map
 template <class Fix>
-static int repair_dev(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, uint32_t nb, void *const *d_parts, size_t part_stride,
-                      const void *const *d_part_crc, void *d_fix, void *stream, const char *name) {
-	int rc = repair_args(ctx, goal, nb, d_parts, d_part_crc, d_fix, true, name);
-	if (rc || n_chunks == 0) return rc;
+using FixArgs = std::conditional_t<std::is_same_v<Fix, lzgpu_stripe_fix>, CorrectArgs, RepairArgs>;
+template <class Fix>
+constexpr bool kFixFailed = !std::is_same_v<Fix, lzgpu_stripe_fix>;
+
+// the _dev call of the correction, the repair and the decode, after its argument check.  The repair's and the decode's check collects
+// F words, so it never arms the ticket and the call never waits.
+template <class Fix>
+static int fix_dev(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, uint32_t nb, void *const *d_parts, size_t part_stride,
+                   const void *const *d_part_crc, void *d_fix, int64_t *bad, void *stream) {
 	const uint32_t pb = (nb + goal->k - 1) / goal->k;
 	const unsigned long long entries = static_cast<unsigned long long>(n_chunks) * pb;
-	RepairArgs a{};
-	unsigned long long given = 0;
-	for (int i = 0; i < goal->k + goal->m; ++i) {
-		a.part[i] = static_cast<uint8_t *>(d_parts[i]);
-		a.crc[i] = d_parts[i] ? static_cast<const uint32_t *>(d_part_crc[i]) : nullptr;
-		given |= d_parts[i] ? 1ull << i : 0ull;
-	}
-	repair_table(goal, given, a);
-	DeviceGuard g(ctx->device);
-	cudaStream_t st = stream ? static_cast<cudaStream_t>(stream) : ctx->stream;
-	// the map's bytes and one entry per stripe; the rebuilt blocks are not counted (the host does not know them here)
-	BatchTimer timer(ctx, st, check_alg_bytes(goal, n_chunks, nb, d_parts, d_part_crc, true) + entries * sizeof(Fix));
-	TmpBuf map(ctx, st), failed(ctx, st);
-	if ((rc = map.alloc(entries * sizeof(lzgpu_stripe_state))) || (rc = failed.alloc(entries * sizeof(uint64_t))) ||
-	    (rc = check_enqueue(ctx, goal, n_chunks, nb, d_parts, part_stride, d_part_crc, map.p, st, nullptr, true,
-	                        static_cast<unsigned long long *>(failed.p))))
-		return rc;
-	return repair_enqueue(ctx, a, entries, pb, part_stride, map.p, failed.p, static_cast<Fix *>(d_fix), st);
+	FixArgs<Fix> a{};
+	int rc = fix_table(goal, fix_parts(a, goal->k + goal->m, d_parts, d_part_crc), a);
+	if (rc) return rc;  // before anything is enqueued: no host work between check and correction
+	// the map's bytes and one entry per stripe; the rewritten blocks are not counted (the host does not know them here)
+	const uint64_t alg_bytes = check_alg_bytes(goal, n_chunks, nb, d_parts, d_part_crc, true) + entries * sizeof(Fix);
+	return dev_call(ctx, stream, alg_bytes, bad, [&](cudaStream_t st, VerifyTicket *tk) {
+		TmpBuf map(ctx, st), failed(ctx, st);  // the map kernels write 8-byte entries; the stripe kernels copy them into the fix entries
+		int rc;
+		if ((rc = map.alloc(entries * sizeof(lzgpu_stripe_state))) || (kFixFailed<Fix> && (rc = failed.alloc(entries * sizeof(uint64_t)))) ||
+		    (rc = check_enqueue(ctx, goal, n_chunks, nb, d_parts, part_stride, d_part_crc, map.p, st, tk, true,
+		                        static_cast<unsigned long long *>(failed.p))))
+			return rc;
+		return fix_enqueue(ctx, a, entries, pb, part_stride, map.p, failed.p, static_cast<Fix *>(d_fix), st);
+	});
+}
+
+extern "C" int lzgpu_correct_stripes_dev(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, uint32_t nb, void *const *d_parts,
+                                         size_t part_stride, const void *const *d_part_crc, void *d_fix, int64_t *bad, void *stream) {
+	NvtxScope nvtx_scope("lzgpu::correct_stripes_dev");
+	const int rc = check_args(ctx, goal, nb, d_parts, d_part_crc, d_fix, true);
+	if (rc || n_chunks == 0) return rc;
+	return fix_dev<lzgpu_stripe_fix>(ctx, goal, n_chunks, nb, d_parts, part_stride, d_part_crc, d_fix, bad, stream);
+}
+
+extern "C" int lzgpu_correct_stripes_degraded_dev(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, uint32_t nb, void *const *d_parts,
+                                                  size_t part_stride, const void *const *d_part_crc, void *d_fix, int64_t *bad, void *stream) {
+	NvtxScope nvtx_scope("lzgpu::correct_stripes_degraded_dev");
+	const int rc = check_args(ctx, goal, nb, d_parts, d_part_crc, d_fix, true, true);
+	if (rc || n_chunks == 0) return rc;
+	return fix_dev<lzgpu_stripe_fix>(ctx, goal, n_chunks, nb, d_parts, part_stride, d_part_crc, d_fix, bad, stream);
 }
 
 extern "C" int lzgpu_repair_stripes_dev(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, uint32_t nb, void *const *d_parts,
                                         size_t part_stride, const void *const *d_part_crc, void *d_fix, void *stream) {
 	NvtxScope nvtx_scope("lzgpu::repair_stripes_dev");
-	return repair_dev<lzgpu_stripe_repair>(ctx, goal, n_chunks, nb, d_parts, part_stride, d_part_crc, d_fix, stream, "repair_stripes");
+	const int rc = repair_args(ctx, goal, nb, d_parts, d_part_crc, d_fix, true, "repair_stripes");
+	if (rc || n_chunks == 0) return rc;
+	return fix_dev<lzgpu_stripe_repair>(ctx, goal, n_chunks, nb, d_parts, part_stride, d_part_crc, d_fix, nullptr, stream);
 }
 
 extern "C" int lzgpu_decode_stripes_dev(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, uint32_t nb, void *const *d_parts,
                                         size_t part_stride, const void *const *d_part_crc, void *d_fix, void *stream) {
 	NvtxScope nvtx_scope("lzgpu::decode_stripes_dev");
-	return repair_dev<lzgpu_stripe_decode>(ctx, goal, n_chunks, nb, d_parts, part_stride, d_part_crc, d_fix, stream, "decode_stripes");
+	const int rc = repair_args(ctx, goal, nb, d_parts, d_part_crc, d_fix, true, "decode_stripes");
+	if (rc || n_chunks == 0) return rc;
+	return fix_dev<lzgpu_stripe_decode>(ctx, goal, n_chunks, nb, d_parts, part_stride, d_part_crc, d_fix, nullptr, stream);
 }
 
-// The host-pointer repair and decode, phase 2: the stripes `todo` (map indices with work) gathered into one-stripe "chunks" as in
-// correct_host_stripes, tile by tile, through the kernels of the entry kind with the map entries and failing blocks the check found;
-// the entries go to fix[], the rewritten blocks back into the caller's parts.
+// The host-pointer calls, phase 2: the stripes `todo` (map indices with work) gathered into one-stripe "chunks" (pb = 1: the parts
+// are zero-padded, so a short last stripe has the same syndromes), tile by tile, through the kernels of the entry kind with the map
+// entries (and F words) the check found; the entries go to fix[], the rewritten blocks back into the caller's parts.
 template <class Fix>
-static int repair_host_stripes(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t pb, uint8_t *const *parts, size_t part_stride,
-                               const uint32_t *const *part_crc, const lzgpu_stripe_state *map, const uint64_t *failed,
-                               const std::vector<size_t> &todo, Fix *fix) {
+static int fix_host_stripes(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t pb, uint8_t *const *parts, size_t part_stride,
+                            const uint32_t *const *part_crc, const lzgpu_stripe_state *map, const uint64_t *failed,
+                            const std::vector<size_t> &todo, Fix *fix) {
 	const int n = goal->k + goal->m;
 	const size_t B = LZGPU_BLOCK_SIZE;
-	unsigned long long given = 0;
-	int n_given = 0;
-	for (int i = 0; i < n; ++i)
-		if (parts[i]) {
-			given |= 1ull << i;
-			++n_given;
-		}
-	RepairArgs a{};
-	repair_table(goal, given, a);
+	FixArgs<Fix> a{};
+	int n_given;
+	int rc = fix_table(goal, fix_parts(a, n, reinterpret_cast<void *const *>(parts), reinterpret_cast<const void *const *>(part_crc), &n_given), a);
+	if (rc) return rc;
 	std::lock_guard<std::mutex> lk(ctx->mu);
 	DeviceGuard g(ctx->device);
 	const size_t tile = std::max<size_t>(1, std::min<size_t>(todo.size(), (2 * kHostTileBytes) / (B * n_given)));
-	const size_t entry_bytes = sizeof(lzgpu_stripe_state) + sizeof(uint64_t) + sizeof(Fix);
+	const size_t f_bytes = kFixFailed<Fix> ? sizeof(uint64_t) : 0;
+	const size_t entry_bytes = sizeof(lzgpu_stripe_state) + f_bytes + sizeof(Fix);
 	void *d_in, *d_crc, *d_entries;
-	int rc;
 	if ((rc = lz_scratch(ctx, kScratchIn0, tile * B * n, &d_in)) || (rc = lz_scratch(ctx, kScratchCrc0, tile * 4 * n, &d_crc)) ||
 	    (rc = lz_scratch(ctx, kScratchPar0, tile * entry_bytes, &d_entries)))
 		return rc;
 	void *d_failed = d_entries;  // 8-byte words first: every part of d_entries stays 8-byte aligned
-	void *d_fix = static_cast<uint8_t *>(d_entries) + tile * sizeof(uint64_t);
+	void *d_fix = static_cast<uint8_t *>(d_entries) + tile * f_bytes;
 	void *d_map = static_cast<uint8_t *>(d_fix) + tile * sizeof(Fix);
-	for (int i = 0; i < n; ++i) {
-		a.part[i] = parts[i] ? static_cast<uint8_t *>(d_in) + tile * B * i : nullptr;
-		a.crc[i] = parts[i] ? static_cast<const uint32_t *>(d_crc) + tile * i : nullptr;
+	for (int i = 0; i < n; ++i) {  // the staged copies: stripe j of part i at d_in + (tile i + j) B, its stored CRC at d_crc[tile i + j]
+		if (a.part[i]) a.part[i] = static_cast<uint8_t *>(d_in) + tile * B * i;
+		if (a.crc[i]) a.crc[i] = static_cast<const uint32_t *>(d_crc) + tile * i;
 	}
 	std::vector<uint32_t> h_crc(tile * n);
 	std::vector<lzgpu_stripe_state> h_map(tile);
-	std::vector<uint64_t> h_failed(tile);
+	std::vector<uint64_t> h_failed(kFixFailed<Fix> ? tile : 0);
 	std::vector<Fix> h_fix(tile);
 	cudaStream_t st = ctx->slot_stream[0];
 	for (size_t t0 = 0; t0 < todo.size(); t0 += tile) {
@@ -1765,18 +1642,18 @@ static int repair_host_stripes(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t 
 			for (int i = 0; i < n; ++i) {
 				if (!parts[i]) continue;
 				CUDA_TRY(cudaMemcpyAsync(a.part[i] + j * B, parts[i] + c * part_stride + s * B, B, cudaMemcpyHostToDevice, st));
-				h_crc[tile * i + j] = part_crc[i][e];
+				if (a.crc[i]) h_crc[tile * i + j] = part_crc[i][e];
 			}
 			h_map[j] = map[e];
-			h_failed[j] = failed[e];
+			if (kFixFailed<Fix>) h_failed[j] = failed[e];
 		}
 		ctx->stats.bytes_h2d += nt * n_given * B;
 		CUDA_TRY(cudaMemcpyAsync(d_crc, h_crc.data(), tile * 4 * n, cudaMemcpyHostToDevice, st));
 		CUDA_TRY(cudaMemcpyAsync(d_map, h_map.data(), nt * sizeof(lzgpu_stripe_state), cudaMemcpyHostToDevice, st));
-		CUDA_TRY(cudaMemcpyAsync(d_failed, h_failed.data(), nt * sizeof(uint64_t), cudaMemcpyHostToDevice, st));
+		if (kFixFailed<Fix>) CUDA_TRY(cudaMemcpyAsync(d_failed, h_failed.data(), nt * sizeof(uint64_t), cudaMemcpyHostToDevice, st));
 		{
 			BatchTimer timer(ctx, st, nt * (n_given * B + entry_bytes));
-			if ((rc = repair_enqueue(ctx, a, nt, 1, B, d_map, d_failed, static_cast<Fix *>(d_fix), st))) return rc;
+			if ((rc = fix_enqueue(ctx, a, nt, 1, B, d_map, d_failed, static_cast<Fix *>(d_fix), st))) return rc;
 		}
 		CUDA_TRY(cudaMemcpyAsync(h_fix.data(), d_fix, nt * sizeof(Fix), cudaMemcpyDeviceToHost, st));
 		CUDA_TRY(cudaStreamSynchronize(st));
@@ -1794,60 +1671,104 @@ static int repair_host_stripes(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t 
 	return LZGPU_OK;
 }
 
-// the repair's and the decode's host-pointer call: phase 1 maps the whole batch, phase 2 stages the stripes with work (the repair's
-// blocks to rebuild, and for the decode the entries its rule 2 can still serve)
+// The host-pointer calls: phase 1 maps the whole batch through the check's tile pipeline (with the F words for the repair and the
+// decode), every entry gets repair_rule's status (F = 0 for the correction), and phase 2 stages the stripes with work (for the
+// decode also the entries its rule 2 can still serve).  Returns the check's LZGPU_OK, LZGPU_ERR_CRC or LZGPU_ERR_INCONSISTENT, or
+// the first other error.
 template <class Fix>
-static int repair_host(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, uint32_t nb, uint8_t *const *parts, size_t part_stride,
-                       const uint32_t *const *part_crc, Fix *fix, bool decode, const char *name) {
-	int rc = repair_args(ctx, goal, nb, reinterpret_cast<const void *const *>(parts), reinterpret_cast<const void *const *>(part_crc), fix, false, name);
-	if (rc) return rc;
-	if (n_chunks == 0) return LZGPU_OK;
-	// phase 1: the map and the failing blocks of the whole batch through the check's tile pipeline
-	const uint32_t pb = (nb + goal->k - 1) / goal->k;
+static int fix_host(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, uint32_t nb, uint8_t *const *parts, size_t part_stride,
+                    const uint32_t *const *part_crc, Fix *fix, int64_t *bad, bool degraded) {
+	const uint32_t pb = goal && goal->k > 0 ? (nb + goal->k - 1) / goal->k : 0;
 	const size_t entries = static_cast<size_t>(n_chunks) * pb;
-	std::vector<lzgpu_stripe_state> map(entries);
-	std::vector<uint64_t> failed(entries);
-	rc = check_host(ctx, goal, n_chunks, nb, parts, part_stride, part_crc, map.data(), nullptr, true, true, failed.data());
-	if (rc != LZGPU_OK && rc != LZGPU_ERR_INCONSISTENT) return rc;
+	std::vector<lzgpu_stripe_state> map(std::max<size_t>(1, entries));
+	std::vector<uint64_t> failed(kFixFailed<Fix> ? entries : 0);
+	const int check_rc = check_host(ctx, goal, n_chunks, nb, parts, part_stride, part_crc, map.data(), bad, true, degraded,
+	                                kFixFailed<Fix> ? failed.data() : nullptr);
+	if (check_rc != LZGPU_OK && check_rc != LZGPU_ERR_CRC && check_rc != LZGPU_ERR_INCONSISTENT) return check_rc;
+	if (n_chunks == 0) return LZGPU_OK;
 	int spare = -goal->k;
 	for (int i = 0; i < goal->k + goal->m; ++i) spare += parts[i] ? 1 : 0;
 	std::vector<size_t> todo;
 	for (size_t e = 0; e < entries; ++e) {
+		const uint64_t f = kFixFailed<Fix> ? failed[e] : 0;
 		unsigned long long x;
-		const int status = repair_rule(map[e].bad_rows, map[e].suspect_part, failed[e], spare, &x);
+		const int status = repair_rule(map[e].bad_rows, map[e].suspect_part, f, spare, &x);
 		fix[e] = Fix{};
 		fix[e].bad_rows = map[e].bad_rows;
 		fix[e].suspect_part = map[e].suspect_part;
 		fix[e].status = status;
-		fix[e].crc_failed = failed[e];
-		if (x || (decode && decode_eligible(status, failed[e], spare))) todo.push_back(e);
+		if constexpr (kFixFailed<Fix>) fix[e].crc_failed = f;
+		if (x || (std::is_same_v<Fix, lzgpu_stripe_decode> && decode_eligible(status, f, spare))) todo.push_back(e);
 	}
 	// phase 2: only the stripes with work travel again
-	if (!todo.empty() && (rc = repair_host_stripes(ctx, goal, pb, parts, part_stride, part_crc, map.data(), failed.data(), todo, fix))) return rc;
-	for (size_t e = 0; e < entries; ++e)
-		if (fix[e].status == LZGPU_FIX_CRC_ONLY || fix[e].status == LZGPU_FIX_CRC_CONFLICT) {
-			lz_set_error("%s: chunk %zu stripe %zu: a block still fails its stored CRC (status %d)", name, e / pb, e % pb, fix[e].status);
-			return LZGPU_ERR_CRC;
-		}
+	int rc;
+	if (!todo.empty() && (rc = fix_host_stripes(ctx, goal, pb, parts, part_stride, part_crc, map.data(), failed.data(), todo, fix))) return rc;
+	return check_rc;
+}
+
+// LZGPU_ERR_INCONSISTENT with the first stripe left UNEXPLAINED ("<name>: chunk c stripe s is not a codeword and <why>"), else LZGPU_OK
+template <class Fix>
+static int fix_unexplained(const Fix *fix, size_t entries, uint32_t pb, const char *name, const char *why) {
 	for (size_t e = 0; e < entries; ++e)
 		if (fix[e].status == LZGPU_FIX_UNEXPLAINED) {
-			lz_set_error("%s: chunk %zu stripe %zu is not a codeword and %s", name, e / pb, e % pb,
-			             decode ? "no set of parts within the code's radius explains it" : "no single part explains it");
+			lz_set_error("%s: chunk %zu stripe %zu is not a codeword and %s", name, e / pb, e % pb, why);
 			return LZGPU_ERR_INCONSISTENT;
 		}
 	return LZGPU_OK;
 }
 
+static int correct_host(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, uint32_t nb, uint8_t *const *parts, size_t part_stride,
+                        const uint32_t *const *part_crc, lzgpu_stripe_fix *fix, int64_t *bad, bool degraded) {
+	if (!fix) return LZGPU_ERR_ARG;
+	const int rc = fix_host(ctx, goal, n_chunks, nb, parts, part_stride, part_crc, fix, bad, degraded);
+	if (rc != LZGPU_OK && rc != LZGPU_ERR_INCONSISTENT) return rc;  // LZGPU_ERR_CRC: bad[0..2] and the message as the map set them
+	if (n_chunks == 0) return LZGPU_OK;
+	return fix_unexplained(fix, static_cast<size_t>(n_chunks) * ((nb + goal->k - 1) / goal->k), (nb + goal->k - 1) / goal->k,
+	                       "correct_stripes", "no single part explains it");
+}
+
+extern "C" int lzgpu_correct_stripes(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, uint32_t nb, uint8_t *const *parts,
+                                     size_t part_stride, const uint32_t *const *part_crc, lzgpu_stripe_fix *fix, int64_t *bad) {
+	NvtxScope nvtx_scope("lzgpu::correct_stripes");
+	return correct_host(ctx, goal, n_chunks, nb, parts, part_stride, part_crc, fix, bad, false);
+}
+
+extern "C" int lzgpu_correct_stripes_degraded(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, uint32_t nb, uint8_t *const *parts,
+                                              size_t part_stride, const uint32_t *const *part_crc, lzgpu_stripe_fix *fix, int64_t *bad) {
+	NvtxScope nvtx_scope("lzgpu::correct_stripes_degraded");
+	return correct_host(ctx, goal, n_chunks, nb, parts, part_stride, part_crc, fix, bad, true);
+}
+
+// the repair's and the decode's host-pointer call: their refusals, then LZGPU_ERR_CRC for a block that still fails its stored CRC
+template <class Fix>
+static int repair_host(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, uint32_t nb, uint8_t *const *parts, size_t part_stride,
+                       const uint32_t *const *part_crc, Fix *fix, const char *name, const char *why) {
+	int rc = repair_args(ctx, goal, nb, reinterpret_cast<const void *const *>(parts), reinterpret_cast<const void *const *>(part_crc), fix, false, name);
+	if (rc) return rc;
+	if (n_chunks == 0) return LZGPU_OK;
+	rc = fix_host(ctx, goal, n_chunks, nb, parts, part_stride, part_crc, fix, nullptr, true);
+	if (rc != LZGPU_OK && rc != LZGPU_ERR_INCONSISTENT) return rc;
+	const uint32_t pb = (nb + goal->k - 1) / goal->k;
+	const size_t entries = static_cast<size_t>(n_chunks) * pb;
+	for (size_t e = 0; e < entries; ++e)
+		if (fix[e].status == LZGPU_FIX_CRC_ONLY || fix[e].status == LZGPU_FIX_CRC_CONFLICT) {
+			lz_set_error("%s: chunk %zu stripe %zu: a block still fails its stored CRC (status %d)", name, e / pb, e % pb, fix[e].status);
+			return LZGPU_ERR_CRC;
+		}
+	return fix_unexplained(fix, entries, pb, name, why);
+}
+
 extern "C" int lzgpu_repair_stripes(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, uint32_t nb, uint8_t *const *parts,
                                     size_t part_stride, const uint32_t *const *part_crc, lzgpu_stripe_repair *fix) {
 	NvtxScope nvtx_scope("lzgpu::repair_stripes");
-	return repair_host(ctx, goal, n_chunks, nb, parts, part_stride, part_crc, fix, false, "repair_stripes");
+	return repair_host(ctx, goal, n_chunks, nb, parts, part_stride, part_crc, fix, "repair_stripes", "no single part explains it");
 }
 
 extern "C" int lzgpu_decode_stripes(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, uint32_t nb, uint8_t *const *parts,
                                     size_t part_stride, const uint32_t *const *part_crc, lzgpu_stripe_decode *fix) {
 	NvtxScope nvtx_scope("lzgpu::decode_stripes");
-	return repair_host(ctx, goal, n_chunks, nb, parts, part_stride, part_crc, fix, true, "decode_stripes");
+	return repair_host(ctx, goal, n_chunks, nb, parts, part_stride, part_crc, fix, "decode_stripes",
+	                   "no set of parts within the code's radius explains it");
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -2410,11 +2331,7 @@ extern "C" int lzgpu_write_blocks_dev(lzgpu_ctx *ctx, void *d_blocks, void *d_st
 	a.payload = static_cast<const uint8_t *>(d_payload);
 	a.writes = static_cast<BlockWrite *>(d_writes);
 	a.tables = ctx->d_crc_tables;
-	uint32_t p = 0x00800000u;  // x^8
-	for (int i = 0; i < 32; ++i) {
-		a.pow2[i] = p;
-		p = lz::crc_mulmod(p, p);
-	}
+	lz::crc_xpow2_table(a.pow2);
 	a.n_writes = n_writes;
 	a.sparse_rule = sparse_rule;
 	const unsigned grid = std::min<unsigned>(n_writes, static_cast<unsigned>(ctx->sm_count) * 8);

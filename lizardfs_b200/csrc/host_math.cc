@@ -121,6 +121,14 @@ uint32_t crc_xpow_bytes(uint64_t nbytes) {
 	return acc;
 }
 
+void crc_xpow2_table(uint32_t pow2[32]) {
+	uint32_t x = 0x00800000u;  // x^8
+	for (int i = 0; i < 32; ++i) {
+		pow2[i] = x;
+		x = crc_mulmod(x, x);
+	}
+}
+
 // CRC(A||B) = CRC(A)*x^(8|B|) xor CRC(B)  (crcutil gf_util.h:92-105 "Concatenate")
 uint32_t crc_combine(uint32_t crc1, uint32_t crc2, uint64_t len2) {
 	return crc_mulmod(crc1, crc_xpow_bytes(len2)) ^ crc2;

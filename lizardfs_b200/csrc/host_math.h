@@ -25,6 +25,7 @@ int rs_recovery_matrix(int k, int m, const uint8_t *erased, const uint8_t *wante
 constexpr uint32_t kCrcPolyReflected = 0xEDB88320u;
 uint32_t crc_mulmod(uint32_t a, uint32_t b);
 uint32_t crc_xpow_bytes(uint64_t nbytes);            // x^(8*nbytes) mod P
+void crc_xpow2_table(uint32_t pow2[32]);             // pow2[i] = x^(8 * 2^i) mod P
 uint32_t crc_of_zeros(uint64_t nbytes);              // mycrc32(0, zeros, nbytes)
 uint32_t crc_combine(uint32_t crc1, uint32_t crc2, uint64_t len2);
 void crc_make_tables(uint32_t tab[4][256]);          // slicing-by-4 tables for x^32..x^56 steps

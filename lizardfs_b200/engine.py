@@ -530,6 +530,24 @@ class Engine:
         _check_crc(rc, _name(fn), bad, **{attr: out})
         return out
 
+    def _stripe_fix_dev(self, fn, goal, n_chunks, nb, d_parts, part_stride, d_part_crc, d_fix, stream):
+        # the device-pointer repair and decode: the check's arguments without `bad`, as the call only enqueues
+        n_parts = goal.k + goal.m
+        rc = fn(self.h, C.byref(goal.c), n_chunks, nb, _dev_ptrs(d_parts, n_parts), part_stride, _dev_ptrs(d_part_crc, n_parts), d_fix,
+                stream)
+        _check(rc, _name(fn))
+
+    def _stripe_fix(self, fn, goal, nb, parts, part_crc, dtype):
+        # the host-pointer repair and decode: the parts are rewritten in place, the entries of `dtype` [n_chunks, pb] are returned
+        # and attached to a ChunkCrcError as .fix
+        assert len(parts) == goal.k + goal.m
+        pb = (nb + goal.k - 1) // goal.k
+        parts, n, crcs = _host_parts(parts, part_crc, pb, in_place=True)
+        out = np.empty((n, pb), dtype=dtype)
+        rc = fn(self.h, C.byref(goal.c), n, nb, _ptr_array(parts), pb * BLOCK_SIZE, crcs, _p(out))
+        _check_crc(rc, _name(fn), (-1, -1, -1), fix=out)
+        return out
+
     # ---- stripe check ------------------------------------------------------------------------
     VERDICT_DTYPE = np.dtype([("first_bad_stripe", np.int32), ("bad_rows", np.uint32), ("suspect_part", np.int32)])
 
@@ -613,21 +631,12 @@ class Engine:
         of STRIPE_REPAIR_DTYPE (crc_failed: bit p = the block of part p failed its stored CRC before the call; status = _lib.FIX_*,
         REBUILT and CRC_ONLY included), whether or not a stripe is left bad; raises ChunkCrcError when a block still fails its stored
         CRC after the call (its .fix holds the entries, and every repair the rule allowed is made)."""
-        assert len(parts) == goal.k + goal.m
-        pb = (nb + goal.k - 1) // goal.k
-        parts, n, crcs = _host_parts(parts, part_crc, pb, in_place=True)
-        out = np.empty((n, pb), dtype=self.STRIPE_REPAIR_DTYPE)
-        rc = self.lib.lzgpu_repair_stripes(self.h, C.byref(goal.c), n, nb, _ptr_array(parts), pb * BLOCK_SIZE, crcs, _p(out))
-        _check_crc(rc, "repair_stripes", (-1, -1, -1), fix=out)
-        return out
+        return self._stripe_fix(self.lib.lzgpu_repair_stripes, goal, nb, parts, part_crc, self.STRIPE_REPAIR_DTYPE)
 
     def repair_stripes_dev(self, goal, n_chunks, nb, d_parts, part_stride, d_part_crc, d_fix, stream=None):
         """Device-pointer form of repair_stripes: the rewritten blocks go into d_parts, n_chunks * pb entries of 24 bytes to d_fix
         (device memory, 8-byte aligned).  The call only enqueues, with or without failing CRCs: the entries report them."""
-        n_parts = goal.k + goal.m
-        rc = self.lib.lzgpu_repair_stripes_dev(self.h, C.byref(goal.c), n_chunks, nb, _dev_ptrs(d_parts, n_parts), part_stride,
-                                               _dev_ptrs(d_part_crc, n_parts), d_fix, stream)
-        _check(rc, "repair_stripes_dev")
+        self._stripe_fix_dev(self.lib.lzgpu_repair_stripes_dev, goal, n_chunks, nb, d_parts, part_stride, d_part_crc, d_fix, stream)
 
     STRIPE_DECODE_DTYPE = np.dtype([("bad_rows", np.uint32), ("suspect_part", np.int32), ("status", np.int32), ("crc", np.uint32),
                                     ("crc_failed", np.uint64), ("located", np.uint64), ("located_crc", np.uint32, (2,))])
@@ -638,21 +647,12 @@ class Engine:
         Returns a structured array [n_chunks, pb] of STRIPE_DECODE_DTYPE (the first five fields as repair_stripes returns them unless
         status == _lib.FIX_DECODED; located: bit p = part p's block was located and rewritten; located_crc: their new CRCs,
         ascending part); raises ChunkCrcError when a block still fails its stored CRC after the call (its .fix holds the entries)."""
-        assert len(parts) == goal.k + goal.m
-        pb = (nb + goal.k - 1) // goal.k
-        parts, n, crcs = _host_parts(parts, part_crc, pb, in_place=True)
-        out = np.empty((n, pb), dtype=self.STRIPE_DECODE_DTYPE)
-        rc = self.lib.lzgpu_decode_stripes(self.h, C.byref(goal.c), n, nb, _ptr_array(parts), pb * BLOCK_SIZE, crcs, _p(out))
-        _check_crc(rc, "decode_stripes", (-1, -1, -1), fix=out)
-        return out
+        return self._stripe_fix(self.lib.lzgpu_decode_stripes, goal, nb, parts, part_crc, self.STRIPE_DECODE_DTYPE)
 
     def decode_stripes_dev(self, goal, n_chunks, nb, d_parts, part_stride, d_part_crc, d_fix, stream=None):
         """Device-pointer form of decode_stripes: the rewritten blocks go into d_parts, n_chunks * pb entries of 40 bytes to d_fix
         (device memory, 8-byte aligned).  The call only enqueues, as repair_stripes_dev."""
-        n_parts = goal.k + goal.m
-        rc = self.lib.lzgpu_decode_stripes_dev(self.h, C.byref(goal.c), n_chunks, nb, _dev_ptrs(d_parts, n_parts), part_stride,
-                                               _dev_ptrs(d_part_crc, n_parts), d_fix, stream)
-        _check(rc, "decode_stripes_dev")
+        self._stripe_fix_dev(self.lib.lzgpu_decode_stripes_dev, goal, n_chunks, nb, d_parts, part_stride, d_part_crc, d_fix, stream)
 
     # ---- wire format --------------------------------------------------------------------------
     def write_data_prefixes(self, goal, nb, crc, chunk_ids, write_id_base=0):
