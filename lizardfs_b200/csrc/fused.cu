@@ -24,15 +24,10 @@ typedef CUresult (*EncodeTiledFn)(CUtensorMap *, CUtensorMapDataType, cuuint32_t
                                   const cuuint32_t *, const cuuint32_t *, CUtensorMapInterleave, CUtensorMapSwizzle,
                                   CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
 
-// two CTAs per SM: 228 KiB per SM minus 1 KiB reserved per CTA
-constexpr int kSmemCap128 = 226 * 1024;       // FW = 128 variant: one CTA per SM
-// (the degraded read's shared-memory caps: fused_plan.h, next to recover_plan())
-
 struct FusedState {
 	EncodeTiledFn encode_tiled = nullptr;
-	uint32_t qmult64[4], qmult128[4];
+	uint32_t qmult[4];
 	int max_smem = 0;
-	int fold = 0;  // LZGPU_FOLD: 0 = per-goal default, 64 / 128 = force
 	bool disabled = false;
 	uint32_t probe = 0;
 	uint32_t *d_sm_ctr = nullptr;
@@ -91,119 +86,238 @@ static uint32_t crc_xpow_bits_signed(long long n) {
 	return acc;
 }
 
-template <int M, bool GENERIC, int KT = 0, int GT = 0, int FW = 64, bool STRIPED = false, bool SPLIT = false, int W = fused_item_words(M, GENERIC)>
-static int set_smem_attr(int bytes) {
-	if (FW == 64) bytes = std::max(bytes, fused_smem_cap(M, GENERIC, FW));  // one-CTA-per-SM shapes use a deeper ring
-	CUDA_TRY(cudaFuncSetAttribute(fused_stream_kernel<M, GENERIC, KT, GT, FW, STRIPED, SPLIT, W>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
-	if constexpr (GENERIC && W == 4) return set_smem_attr<M, GENERIC, KT, GT, FW, STRIPED, SPLIT, 1>(bytes);  // the narrow-item twin
+static uint8_t gf_pow2(int n) {
+	uint8_t v = 1;
+	for (int i = 0; i < n; ++i) v = lz::gf_mul_host(v, 2);
+	return v;
+}
+
+// RAID-6 solve of lost data parts x0, x1 from parity rows 0 and 1 (fused_recover_kernel, fused_convert_kernel): w[0] = planes of
+// 2^x0, w[1] = planes of (2^x0 ^ 2^x1)^-1
+static void set_raid6_pair(CoefPlanes *w, int x0, int x1) {
+	const uint8_t g0 = gf_pow2(x0);
+	coef_planes_set(w[0], g0);
+	coef_planes_set(w[1], lz::gf_inv_host(g0 ^ gf_pow2(x1)));
+}
+
+// the three-unknown elimination with parity rows 0, 1, 2 (the fused_recover_kernel comment; bs_recover3_kernel): alpha, beta, gamma,
+// delta, then 2^x0 and 4^x0.  p, q, p^q are non-zero because 2 has order 255 and the positions differ by less than 32.
+static void elim3_constants(int x0, int x1, int x2, uint8_t c[6]) {
+	const uint8_t A = gf_pow2(x0), pp = A ^ gf_pow2(x1), qq = A ^ gf_pow2(x2);
+	c[0] = lz::gf_inv_host(lz::gf_mul_host(qq, pp ^ qq));
+	c[1] = lz::gf_mul_host(pp, c[0]);
+	c[2] = lz::gf_inv_host(pp);
+	c[3] = lz::gf_mul_host(qq, c[2]);
+	c[4] = A;
+	c[5] = lz::gf_mul_host(A, A);
+}
+
+// One persistent launch: geo.threads threads and geo.smem_bytes bytes of shared memory per CTA, the grid from persistent_grid
+template <class... P, class... A>
+static int launch(lzgpu_ctx *ctx, void (*kernel)(P...), const lzgpu_launch_geometry &geo, int per_sm, uint64_t units, cudaStream_t st,
+                  const A &...args) {
+	const int grid = persistent_grid(ctx, units, per_sm, geo);
+	kernel<<<grid, geo.threads, geo.smem_bytes, st>>>(args...);
+	CUDA_TRY(cudaGetLastError());
+	ctx->stats.kernel_launches++;
 	return LZGPU_OK;
 }
 
-template <int E, int KT, int R0 = -1, int R1 = -1>
-static int set_recover_attr() {
-	CUDA_TRY(cudaFuncSetAttribute(fused_recover_kernel<E, KT, R0, R1, 64>, cudaFuncAttributeMaxDynamicSharedMemorySize, kRecoverSmemCap));
-	if constexpr (E <= 2) CUDA_TRY(cudaFuncSetAttribute(fused_recover_kernel<E, KT, R0, R1, 64, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, kRecoverSmemCap2));
-	CUDA_TRY(cudaFuncSetAttribute(fused_recover_kernel<E, KT, R0, R1, 64, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, kRecoverSmemCapBig));
-#ifdef LZ_ENABLE_FOLD128
-	CUDA_TRY(cudaFuncSetAttribute(fused_recover_kernel<E, KT, R0, R1, 128>, cudaFuncAttributeMaxDynamicSharedMemorySize, kRecoverSmemCap));
-#endif
+template <class F>
+static int set_smem(F *kernel, int bytes) {
+	CUDA_TRY(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
 	return LZGPU_OK;
 }
 
-template <int E>
-static int set_direct_attr() {
-	CUDA_TRY(cudaFuncSetAttribute(fused_recover_kernel<E, 0, kRecoverDirect, -1, 64, 2, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, kRecoverSmemCapBig));
-	CUDA_TRY(cudaFuncSetAttribute(fused_recover_kernel<E, 0, kRecoverDirect, -1, 64, 2, direct_wide_words(E)>, cudaFuncAttributeMaxDynamicSharedMemorySize, kRecoverSmemCapBig));
-	return LZGPU_OK;
+// ---------------------------------------------------------------------------------------------------
+// Every kernel instantiation, one table per family.  lz_fused_init sets the shared-memory limit of each entry; the launch sites
+// take the entry their plan names.  A kernel missing here is neither compiled nor launched.
+// ---------------------------------------------------------------------------------------------------
+// Encoders (fused_stream_kernel): packed-word items, or bit-sliced ones (bs: W = 8, one 16-warp CTA per SM, the last
+// ceil(16 G / 32) warps take the 16 G items of a step, the warps before them the G (K + M - 1) * 4 streams; the plan made with
+// bs = true guarantees both fit).  k = g = 0: runtime k and G.
+using EncodeKernel = void (*)(CUtensorMap, FusedParams);
+struct EncodeKernelEntry {
+	int m;
+	bool generic, striped, split, bs;
+	uint32_t k, g;
+	EncodeKernel fn;
+	EncodeKernel narrow;  // generic coefficients: the 4-byte-item twin (fused_generic_item_words)
+};
+template <int M, bool GENERIC, int KT = 0, int GT = 0, bool STRIPED = false, bool SPLIT = false>
+static EncodeKernelEntry encoder() {
+	EncodeKernelEntry k{M, GENERIC, STRIPED, SPLIT, false, KT, GT, fused_stream_kernel<M, GENERIC, KT, GT, 64, STRIPED, SPLIT>, nullptr};
+	if constexpr (GENERIC) k.narrow = fused_stream_kernel<M, GENERIC, KT, GT, 64, STRIPED, SPLIT, 1>;
+	return k;
 }
+template <int M, int KT = 0, int GT = 0, bool STRIPED = false>
+static EncodeKernelEntry bitsliced() {
+	return {M, false, STRIPED, false, true, KT, GT, fused_stream_kernel<M, false, KT, GT, 64, STRIPED, false, 8>, nullptr};
+}
+static const EncodeKernelEntry kEncoders[] = {
+	// runtime k and G: the CRC pass alone (M = 0), Vandermonde and generic (Cauchy) coefficients, the conversion form, striped units
+	encoder<0, false>(), encoder<1, false>(), encoder<2, false>(), encoder<3, false>(), encoder<4, false>(),
+	encoder<1, true>(), encoder<2, true>(), encoder<3, true>(), encoder<4, true>(),
+	encoder<1, false, 0, 0, false, true>(), encoder<2, false, 0, 0, false, true>(), encoder<3, false, 0, 0, false, true>(),
+	encoder<4, false, 0, 0, false, true>(), encoder<4, true, 0, 0, false, true>(),
+	encoder<1, false, 0, 0, true>(), encoder<2, false, 0, 0, true>(), encoder<3, false, 0, 0, true>(), encoder<4, false, 0, 0, true>(),
+	encoder<4, true, 0, 0, true>(),
+	// constant-folded (M, K, G) for the common goals (K, G from pick_group)
+	encoder<2, false, 8, 7>(),    // ec(8,2)
+	encoder<1, false, 2, 32>(),   // xor2
+	encoder<1, false, 3, 20>(),   // xor3
+	encoder<2, false, 3, 16>(),   // ec(3,2)
+	encoder<2, false, 4, 12>(),   // ec(4,2)
+	encoder<2, false, 6, 9>(),    // ec(6,2)
+	encoder<3, false, 5, 8>(),    // ec(5,3)
+	encoder<3, false, 6, 8>(),    // ec(6,3)
+	encoder<4, false, 8, 8>(),    // ec(8,4) on one 16-warp CTA per SM
+	// more goals folded (the runtime-k instantiation measured markedly slower for ec(8,3), ec(6,4), ec(4,4))
+	encoder<3, false, 8, 6>(),    // ec(8,3)
+	encoder<1, false, 4, 16>(),   // xor4 / ec(4,1)
+	encoder<2, false, 5, 10>(),   // ec(5,2)
+	encoder<2, false, 10, 5>(),   // ec(10,2)
+	encoder<3, false, 4, 8>(),    // ec(4,3)
+	encoder<4, false, 10, 6>(),   // ec(10,4)
+	encoder<4, false, 12, 5>(),   // ec(12,4)
+	encoder<4, false, 6, 8>(),    // ec(6,4)
+	encoder<4, false, 4, 8>(),    // ec(4,4)
+	encoder<2, false, 8, 7, true>(), encoder<1, false, 2, 32, true>(), encoder<1, false, 3, 20, true>(), encoder<2, false, 3, 16, true>(),
+	encoder<3, false, 5, 8, true>(), encoder<4, false, 8, 8, true>(),
+	// bit-sliced: runtime k and G, then the constant-folded (M, K, G), G from pick_group(.., bs = true)
+	bitsliced<3>(), bitsliced<4>(), bitsliced<3, 0, 0, true>(), bitsliced<4, 0, 0, true>(),
+	bitsliced<4, 8, 8>(), bitsliced<4, 10, 6>(), bitsliced<4, 12, 5>(), bitsliced<4, 6, 8>(), bitsliced<4, 4, 8>(),
+	bitsliced<3, 8, 8>(), bitsliced<3, 9, 6>(), bitsliced<3, 10, 6>(), bitsliced<3, 12, 5>(), bitsliced<4, 8, 8, true>(),
+};
 
-template <int M>
-static int set_convert_attr() {
-	CUDA_TRY(cudaFuncSetAttribute(fused_convert_kernel<M, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemCap));
-	CUDA_TRY(cudaFuncSetAttribute(fused_convert_kernel<M, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemCap));
-	CUDA_TRY(cudaFuncSetAttribute(fused_convert_kernel<M, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemCap));
-	if (M <= 2) {
-		constexpr int MM = M <= 2 ? M : 1;
-		CUDA_TRY(cudaFuncSetAttribute(fused_convert_kernel<MM, 0, 3>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemCap));
-		CUDA_TRY(cudaFuncSetAttribute(fused_convert_kernel<MM, 1, 3>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemCap));
-		CUDA_TRY(cudaFuncSetAttribute(fused_convert_kernel<MM, 2, 3>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemCap));
+// the folded entry of (M, K, G) where there is one, else the runtime-k one; nullptr: the fused path does not take the shape
+static const EncodeKernelEntry *find_encoder(int M, bool generic, uint32_t K, uint32_t G, bool striped, bool split, bool bs) {
+	const EncodeKernelEntry *runtime_k = nullptr;
+	for (const EncodeKernelEntry &k : kEncoders) {
+		if (k.m != M || k.generic != generic || k.striped != striped || k.split != split || k.bs != bs) continue;
+		if (k.k == K && k.g == G) return &k;
+		if (k.k == 0) runtime_k = &k;
 	}
-	return LZGPU_OK;
-}
-static int set_all_convert_attrs() {
-	int rc;
-	if ((rc = set_convert_attr<1>()) || (rc = set_convert_attr<2>()) || (rc = set_convert_attr<3>())) return rc;
-	return LZGPU_OK;
+	return runtime_k;
 }
 
-// function attributes are per device: done once per context
-static int set_all_recover_attrs() {
-	int rc;
-	if ((rc = set_recover_attr<1, 8, 0>())) return rc;
-	if ((rc = set_recover_attr<1, 0, 0>())) return rc;
-	if ((rc = set_recover_attr<1, 0>())) return rc;
-	if ((rc = set_recover_attr<2, 8, 0, 1>())) return rc;
-	if ((rc = set_recover_attr<2, 0, 0, 1>())) return rc;
-	if ((rc = set_recover_attr<2, 0>())) return rc;
-	if ((rc = set_recover_attr<3, 0, 0, 1>())) return rc;
-	if ((rc = set_recover_attr<3, 0>())) return rc;
-	if ((rc = set_recover_attr<4, 0, 0, 1>())) return rc;
-	if ((rc = set_recover_attr<4, 0>())) return rc;
-	CUDA_TRY(cudaFuncSetAttribute(fused_recover_kernel<1, 3, 0, -1, 64, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, kRecoverSmemCapBig));
-	CUDA_TRY(cudaFuncSetAttribute(fused_recover_kernel<2, 3, 0, 1, 64, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, kRecoverSmemCapBig));
-	CUDA_TRY(cudaFuncSetAttribute(fused_recover_kernel<2, 5, 0, 1, 64, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, kRecoverSmemCapBig));
-	CUDA_TRY(cudaFuncSetAttribute(fused_recover_kernel<3, 5, 0, 1, 64, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, kRecoverSmemCapBig));
-	CUDA_TRY(cudaFuncSetAttribute(fused_recover_kernel<2, 4, 0, 1, 64, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, kRecoverSmemCapBig));
-	CUDA_TRY(cudaFuncSetAttribute(fused_recover_kernel<2, 6, 0, 1, 64, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, kRecoverSmemCapBig));
-	CUDA_TRY(cudaFuncSetAttribute(fused_recover_kernel<3, 6, 0, 1, 64, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, kRecoverSmemCapBig));
-	CUDA_TRY(cudaFuncSetAttribute(bs_recover3_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, kRecoverSmemCapBig));
-	CUDA_TRY(cudaFuncSetAttribute(bs_recover3_kernel<5>, cudaFuncAttributeMaxDynamicSharedMemorySize, kRecoverSmemCapBig));
-	CUDA_TRY(cudaFuncSetAttribute(bs_recover3_kernel<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, kRecoverSmemCapBig));
-	// DIRECT (any generator; Cauchy codes): 16-warp geometry, 4-byte items
-	if ((rc = set_direct_attr<1>()) || (rc = set_direct_attr<2>()) || (rc = set_direct_attr<3>()) || (rc = set_direct_attr<4>())) return rc;
-	CUDA_TRY(cudaFuncSetAttribute(fused_check_kernel<1, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kRecoverSmemCapBig));
-	CUDA_TRY(cudaFuncSetAttribute(fused_check_kernel<2, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kRecoverSmemCapBig));
-	CUDA_TRY(cudaFuncSetAttribute(fused_check_kernel<3, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kRecoverSmemCapBig));
-	CUDA_TRY(cudaFuncSetAttribute(fused_check_kernel<4, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kRecoverSmemCapBig));
-	CUDA_TRY(cudaFuncSetAttribute(fused_check_kernel<1, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kRecoverSmemCapBig));
-	CUDA_TRY(cudaFuncSetAttribute(fused_check_kernel<2, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kRecoverSmemCapBig));
-	CUDA_TRY(cudaFuncSetAttribute(fused_check_kernel<3, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kRecoverSmemCapBig));
-	CUDA_TRY(cudaFuncSetAttribute(fused_check_map_kernel<1, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kRecoverSmemCapBig));
-	CUDA_TRY(cudaFuncSetAttribute(fused_check_map_kernel<2, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kRecoverSmemCapBig));
-	CUDA_TRY(cudaFuncSetAttribute(fused_check_map_kernel<3, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kRecoverSmemCapBig));
-	CUDA_TRY(cudaFuncSetAttribute(fused_check_map_kernel<4, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kRecoverSmemCapBig));
-	CUDA_TRY(cudaFuncSetAttribute(fused_check_map_kernel<1, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kRecoverSmemCapBig));
-	CUDA_TRY(cudaFuncSetAttribute(fused_check_map_kernel<2, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kRecoverSmemCapBig));
-	CUDA_TRY(cudaFuncSetAttribute(fused_check_map_kernel<3, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kRecoverSmemCapBig));
-	CUDA_TRY(cudaFuncSetAttribute(fused_check_degraded_kernel<1, 2, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kRecoverSmemCapBig));
-	CUDA_TRY(cudaFuncSetAttribute(fused_check_degraded_kernel<1, 3, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kRecoverSmemCapBig));
-	CUDA_TRY(cudaFuncSetAttribute(fused_check_degraded_kernel<1, 4, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kRecoverSmemCapBig));
-	CUDA_TRY(cudaFuncSetAttribute(fused_check_degraded_kernel<2, 3, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kRecoverSmemCapBig));
-	CUDA_TRY(cudaFuncSetAttribute(fused_check_degraded_kernel<2, 4, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kRecoverSmemCapBig));
-	CUDA_TRY(cudaFuncSetAttribute(fused_check_degraded_kernel<3, 4, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kRecoverSmemCapBig));
-	CUDA_TRY(cudaFuncSetAttribute(fused_check_degraded_kernel<1, 2, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kRecoverSmemCapBig));
-	CUDA_TRY(cudaFuncSetAttribute(fused_check_degraded_kernel<1, 3, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kRecoverSmemCapBig));
-	CUDA_TRY(cudaFuncSetAttribute(fused_check_degraded_kernel<2, 3, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kRecoverSmemCapBig));
-	CUDA_TRY(cudaFuncSetAttribute(fused_check_repair_kernel<1, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kRecoverSmemCapBig));
-	CUDA_TRY(cudaFuncSetAttribute(fused_check_repair_kernel<2, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kRecoverSmemCapBig));
-	CUDA_TRY(cudaFuncSetAttribute(fused_check_repair_kernel<3, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kRecoverSmemCapBig));
-	CUDA_TRY(cudaFuncSetAttribute(fused_check_repair_kernel<4, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kRecoverSmemCapBig));
-	CUDA_TRY(cudaFuncSetAttribute(fused_check_repair_kernel<1, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kRecoverSmemCapBig));
-	CUDA_TRY(cudaFuncSetAttribute(fused_check_repair_kernel<2, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kRecoverSmemCapBig));
-	CUDA_TRY(cudaFuncSetAttribute(fused_check_repair_kernel<3, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kRecoverSmemCapBig));
-	CUDA_TRY(cudaFuncSetAttribute(fused_check_repair_degraded_kernel<1, 2, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kRecoverSmemCapBig));
-	CUDA_TRY(cudaFuncSetAttribute(fused_check_repair_degraded_kernel<1, 3, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kRecoverSmemCapBig));
-	CUDA_TRY(cudaFuncSetAttribute(fused_check_repair_degraded_kernel<1, 4, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kRecoverSmemCapBig));
-	CUDA_TRY(cudaFuncSetAttribute(fused_check_repair_degraded_kernel<2, 3, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kRecoverSmemCapBig));
-	CUDA_TRY(cudaFuncSetAttribute(fused_check_repair_degraded_kernel<2, 4, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kRecoverSmemCapBig));
-	CUDA_TRY(cudaFuncSetAttribute(fused_check_repair_degraded_kernel<3, 4, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kRecoverSmemCapBig));
-	CUDA_TRY(cudaFuncSetAttribute(fused_check_repair_degraded_kernel<1, 2, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kRecoverSmemCapBig));
-	CUDA_TRY(cudaFuncSetAttribute(fused_check_repair_degraded_kernel<1, 3, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kRecoverSmemCapBig));
-	CUDA_TRY(cudaFuncSetAttribute(fused_check_repair_degraded_kernel<2, 3, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kRecoverSmemCapBig));
-	return LZGPU_OK;
+// Degraded read (fused_recover_kernel), keyed by the plan's kernel, lost data parts, compile-time k (0: runtime) and parity rows:
+// 0 .. e-1 (first_e: R0 = 0, R1 = 1) or any.  DIRECT (any generator; the Cauchy codes): 16-warp geometry, 4-byte or wide items.
+using RecoverKernel = void (*)(TmapArray, RecoverParams);
+struct RecoverKernelEntry {
+	int kernel;  // LZGPU_KERNEL_RECOVER_GEO0 / _GEO1 / _GEO2 / _DIRECT
+	uint32_t e, kt;
+	bool first_e, wide;
+	RecoverKernel fn;
+};
+template <int GEO, int E, int KT, int R0 = -1, int R1 = -1>
+static RecoverKernelEntry recoverer() {
+	constexpr int kernel = GEO == 2 ? LZGPU_KERNEL_RECOVER_GEO2 : GEO == 1 ? LZGPU_KERNEL_RECOVER_GEO1 : LZGPU_KERNEL_RECOVER_GEO0;
+	return {kernel, E, KT, R0 == 0, false, fused_recover_kernel<E, KT, R0, R1, 64, GEO>};
+}
+template <int E, bool WIDE>
+static RecoverKernelEntry direct() {
+	return {LZGPU_KERNEL_RECOVER_DIRECT, E, 0, false, WIDE, fused_recover_kernel<E, 0, kRecoverDirect, -1, 64, 2, WIDE ? direct_wide_words(E) : 1>};
+}
+static const RecoverKernelEntry kRecoverers[] = {
+	// every geometry (two 9-warp CTAs per SM only for e <= 2); k = 8 with rows 0 .. e-1 for e <= 2
+	recoverer<0, 1, 8, 0>(), recoverer<1, 1, 8, 0>(), recoverer<2, 1, 8, 0>(),
+	recoverer<0, 1, 0, 0>(), recoverer<1, 1, 0, 0>(), recoverer<2, 1, 0, 0>(),
+	recoverer<0, 1, 0>(), recoverer<1, 1, 0>(), recoverer<2, 1, 0>(),
+	recoverer<0, 2, 8, 0, 1>(), recoverer<1, 2, 8, 0, 1>(), recoverer<2, 2, 8, 0, 1>(),
+	recoverer<0, 2, 0, 0, 1>(), recoverer<1, 2, 0, 0, 1>(), recoverer<2, 2, 0, 0, 1>(),
+	recoverer<0, 2, 0>(), recoverer<1, 2, 0>(), recoverer<2, 2, 0>(),
+	recoverer<0, 3, 0, 0, 1>(), recoverer<2, 3, 0, 0, 1>(), recoverer<0, 3, 0>(), recoverer<2, 3, 0>(),
+	recoverer<0, 4, 0, 0, 1>(), recoverer<2, 4, 0, 0, 1>(), recoverer<0, 4, 0>(), recoverer<2, 4, 0>(),
+	// a compile-time k other than 8 (ec(3,2), the BASELINE configs[1] goal; ec(4,2), ec(5,3), ec(6,2), ec(6,3)): the 16-warp geometry
+	// only, rows 0 .. e-1
+	recoverer<2, 1, 3, 0>(), recoverer<2, 2, 3, 0, 1>(), recoverer<2, 2, 4, 0, 1>(), recoverer<2, 2, 5, 0, 1>(),
+	recoverer<2, 3, 5, 0, 1>(), recoverer<2, 2, 6, 0, 1>(), recoverer<2, 3, 6, 0, 1>(),
+	direct<1, false>(), direct<2, false>(), direct<3, false>(), direct<4, false>(),
+	direct<1, true>(), direct<2, true>(), direct<3, true>(), direct<4, true>(),
+};
+static int recover_smem_cap(int kernel) {
+	return kernel == LZGPU_KERNEL_RECOVER_GEO0 ? kRecoverSmemCap : kernel == LZGPU_KERNEL_RECOVER_GEO1 ? kRecoverSmemCap2 : kRecoverSmemCapBig;
 }
 
-static int set_all_bs_attrs();
+// three lost data parts on bit planes (bs_recover3_kernel), keyed by the compile-time k (0: runtime)
+using BsRecoverKernel = void (*)(TmapArray, RecoverParams, BsRecoverMasks);
+static const struct {
+	uint32_t kt;
+	BsRecoverKernel fn;
+} kBsRecoverers[] = {{0, bs_recover3_kernel<0>}, {5, bs_recover3_kernel<5>}, {8, bs_recover3_kernel<8>}};
+
+// Stripe checks (check_kernel.cuh), keyed by the checked parity rows R, whether they are rows 0 .. R-1, and for the degraded forms
+// the lost data parts E.  check_plan gives E < R <= 4, and rows other than 0 .. R-1 only with m <= 4, so R <= 3 (m >= 5 is Cauchy).
+using CheckKernel = void (*)(CheckTmaps, CheckParams);
+using CheckMapKernel = void (*)(CheckTmaps, CheckParams, uint32_t *);
+using CheckRepairKernel = void (*)(CheckTmaps, CheckParams, uint32_t *, unsigned long long *);
+using CheckDegradedKernel = void (*)(CheckTmaps, CheckParams, uint32_t *, CheckLost);
+using CheckRepairDegradedKernel = void (*)(CheckTmaps, CheckParams, uint32_t *, CheckLost, unsigned long long *);
+struct CheckKernels {
+	uint32_t r;
+	bool consecutive;
+	CheckKernel check;
+	CheckMapKernel map;
+	CheckRepairKernel repair;
+};
+struct CheckDegradedKernels {
+	uint32_t e, r;
+	bool consecutive;
+	CheckDegradedKernel map;
+	CheckRepairDegradedKernel repair;
+};
+template <int R, bool C>
+static CheckKernels checkers() {
+	return {R, C, fused_check_kernel<R, C>, fused_check_map_kernel<R, C>, fused_check_repair_kernel<R, C>};
+}
+template <int E, int R, bool C>
+static CheckDegradedKernels degraded_checkers() {
+	return {E, R, C, fused_check_degraded_kernel<E, R, C>, fused_check_repair_degraded_kernel<E, R, C>};
+}
+static const CheckKernels kCheckers[] = {checkers<1, true>(),  checkers<2, true>(),  checkers<3, true>(), checkers<4, true>(),
+                                         checkers<1, false>(), checkers<2, false>(), checkers<3, false>()};
+static const CheckDegradedKernels kDegradedCheckers[] = {
+	degraded_checkers<1, 2, true>(),  degraded_checkers<1, 3, true>(),  degraded_checkers<1, 4, true>(),
+	degraded_checkers<2, 3, true>(),  degraded_checkers<2, 4, true>(),  degraded_checkers<3, 4, true>(),
+	degraded_checkers<1, 2, false>(), degraded_checkers<1, 3, false>(), degraded_checkers<2, 3, false>()};
+
+// Slice conversion (fused_convert_kernel), keyed by the destination's parity parts, the lost source data parts and a compile-time
+// destination k (0: runtime; 3 for the xor3 / ec(3,2) destinations)
+using ConvertKernel = void (*)(TmapArray, ConvertParams);
+static const struct {
+	int m;
+	uint32_t e;
+	int kd;
+	ConvertKernel fn;
+} kConverters[] = {
+	{1, 0, 0, fused_convert_kernel<1, 0>}, {1, 1, 0, fused_convert_kernel<1, 1>}, {1, 2, 0, fused_convert_kernel<1, 2>},
+	{2, 0, 0, fused_convert_kernel<2, 0>}, {2, 1, 0, fused_convert_kernel<2, 1>}, {2, 2, 0, fused_convert_kernel<2, 2>},
+	{3, 0, 0, fused_convert_kernel<3, 0>}, {3, 1, 0, fused_convert_kernel<3, 1>}, {3, 2, 0, fused_convert_kernel<3, 2>},
+	{1, 0, 3, fused_convert_kernel<1, 0, 3>}, {1, 1, 3, fused_convert_kernel<1, 1, 3>}, {1, 2, 3, fused_convert_kernel<1, 2, 3>},
+	{2, 0, 3, fused_convert_kernel<2, 0, 3>}, {2, 1, 3, fused_convert_kernel<2, 1, 3>}, {2, 2, 3, fused_convert_kernel<2, 2, 3>},
+};
+
+// function attributes are per device: set once per context
+static int set_all_smem_attrs(const FusedState *fs) {
+	int rc;
+	const int smem = std::min(fs->max_smem, kSmemCap);
+	for (const EncodeKernelEntry &k : kEncoders) {
+		const int bytes = k.bs ? 226 * 1024 : std::max(smem, fused_smem_cap(k.m, k.generic, 64));  // one-CTA-per-SM shapes use a deeper ring
+		if ((rc = set_smem(k.fn, bytes)) || (k.narrow && (rc = set_smem(k.narrow, bytes)))) return rc;
+	}
+	for (const RecoverKernelEntry &k : kRecoverers)
+		if ((rc = set_smem(k.fn, recover_smem_cap(k.kernel)))) return rc;
+	for (const auto &k : kBsRecoverers)
+		if ((rc = set_smem(k.fn, kRecoverSmemCapBig))) return rc;
+	for (const CheckKernels &k : kCheckers)
+		if ((rc = set_smem(k.check, kRecoverSmemCapBig)) || (rc = set_smem(k.map, kRecoverSmemCapBig)) || (rc = set_smem(k.repair, kRecoverSmemCapBig))) return rc;
+	for (const CheckDegradedKernels &k : kDegradedCheckers)
+		if ((rc = set_smem(k.map, kRecoverSmemCapBig)) || (rc = set_smem(k.repair, kRecoverSmemCapBig))) return rc;
+	for (const auto &k : kConverters)
+		if ((rc = set_smem(k.fn, kSmemCap))) return rc;
+	return LZGPU_OK;
+}
 
 int lz_fused_init(lzgpu_ctx *ctx) {
 	auto *fs = new FusedState();
@@ -235,84 +349,11 @@ int lz_fused_init(lzgpu_ctx *ctx) {
 		return LZGPU_ERR_CUDA;
 	}
 	fs->encode_tiled = reinterpret_cast<EncodeTiledFn>(fn);
-	for (int q = 0; q < 4; ++q) {
-		fs->qmult64[q] = crc_xpow_bits_signed(32ll * (4096ll * (3 - q) - FoldSpec<64>::deg));
-		fs->qmult128[q] = crc_xpow_bits_signed(32ll * (4096ll * (3 - q) - FoldSpec<128>::deg));
-	}
-	if (const char *e = std::getenv("LZGPU_FOLD")) fs->fold = std::atoi(e);
+	for (int q = 0; q < 4; ++q) fs->qmult[q] = crc_xpow_bits_signed(32ll * (4096ll * (3 - q) - FoldSpec<64>::deg));
 	CUDA_TRY(cudaDeviceGetAttribute(&fs->max_smem, cudaDevAttrMaxSharedMemoryPerBlockOptin, ctx->device));
 	CUDA_TRY(cudaMalloc(&fs->d_sm_ctr, 256 * sizeof(uint32_t)));
 	CUDA_TRY(cudaMemset(fs->d_sm_ctr, 0, 256 * sizeof(uint32_t)));
-	const int smem = std::min(fs->max_smem, kSmemCap);
-	int rc;
-	if ((rc = set_smem_attr<0, false>(smem))) return rc;
-	if ((rc = set_smem_attr<1, false>(smem))) return rc;
-	if ((rc = set_smem_attr<2, false>(smem))) return rc;
-	if ((rc = set_smem_attr<3, false>(smem))) return rc;
-	if ((rc = set_smem_attr<4, false>(smem))) return rc;
-	if ((rc = set_smem_attr<4, true>(smem))) return rc;
-	if ((rc = set_smem_attr<1, true>(smem))) return rc;
-	if ((rc = set_smem_attr<2, true>(smem))) return rc;
-	if ((rc = set_smem_attr<3, true>(smem))) return rc;
-	if ((rc = set_smem_attr<1, false, 0, 0, 64, false, true>(smem))) return rc;
-	if ((rc = set_smem_attr<2, false, 0, 0, 64, false, true>(smem))) return rc;
-	if ((rc = set_smem_attr<3, false, 0, 0, 64, false, true>(smem))) return rc;
-	if ((rc = set_smem_attr<4, false, 0, 0, 64, false, true>(smem))) return rc;
-	if ((rc = set_smem_attr<4, true, 0, 0, 64, false, true>(smem))) return rc;
-	if ((rc = set_smem_attr<1, false, 0, 0, 64, true>(smem))) return rc;
-	if ((rc = set_smem_attr<2, false, 0, 0, 64, true>(smem))) return rc;
-	if ((rc = set_smem_attr<3, false, 0, 0, 64, true>(smem))) return rc;
-	if ((rc = set_smem_attr<4, false, 0, 0, 64, true>(smem))) return rc;
-	if ((rc = set_smem_attr<4, true, 0, 0, 64, true>(smem))) return rc;
-	if ((rc = set_smem_attr<2, false, 8, 7, 64, true>(smem))) return rc;
-	if ((rc = set_smem_attr<1, false, 2, 32, 64, true>(smem))) return rc;
-	if ((rc = set_smem_attr<1, false, 3, 20, 64, true>(smem))) return rc;
-	if ((rc = set_smem_attr<2, false, 3, 16, 64, true>(smem))) return rc;
-	if ((rc = set_smem_attr<3, false, 5, 8, 64, true>(smem))) return rc;
-	if ((rc = set_smem_attr<4, false, 8, 8, 64, true>(smem))) return rc;
-	if ((rc = set_smem_attr<2, false, 8, 7>(smem))) return rc;
-	if ((rc = set_smem_attr<1, false, 2, 32>(smem))) return rc;
-	if ((rc = set_smem_attr<1, false, 3, 20>(smem))) return rc;
-	if ((rc = set_smem_attr<2, false, 3, 16>(smem))) return rc;
-	if ((rc = set_smem_attr<2, false, 4, 12>(smem))) return rc;
-	if ((rc = set_smem_attr<2, false, 6, 9>(smem))) return rc;
-	if ((rc = set_smem_attr<3, false, 5, 8>(smem))) return rc;
-	if ((rc = set_smem_attr<3, false, 6, 8>(smem))) return rc;
-	if ((rc = set_smem_attr<4, false, 8, 8>(smem))) return rc;
-	if ((rc = set_smem_attr<3, false, 8, 6>(smem))) return rc;
-	if ((rc = set_smem_attr<1, false, 4, 16>(smem))) return rc;
-	if ((rc = set_smem_attr<2, false, 5, 10>(smem))) return rc;
-	if ((rc = set_smem_attr<2, false, 10, 5>(smem))) return rc;
-	if ((rc = set_smem_attr<3, false, 4, 8>(smem))) return rc;
-	if ((rc = set_smem_attr<4, false, 10, 6>(smem))) return rc;
-	if ((rc = set_smem_attr<4, false, 12, 5>(smem))) return rc;
-	if ((rc = set_smem_attr<4, false, 6, 8>(smem))) return rc;
-	if ((rc = set_smem_attr<4, false, 4, 8>(smem))) return rc;
-#if LZ_T2 == 288
-	if ((rc = set_smem_attr<2, false, 8, 8>(smem))) return rc;
-#endif
-#if LZ_T4 != 512
-	if ((rc = set_smem_attr<4, false, 8, 5>(smem))) return rc;
-#endif
-#if LZ_T3 == 512
-	if ((rc = set_smem_attr<3, false, 5, 12>(smem))) return rc;
-	if ((rc = set_smem_attr<3, false, 6, 10>(smem))) return rc;
-#endif
-#ifdef LZ_ENABLE_FOLD128
-	const int smem128 = std::min(fs->max_smem, kSmemCap128);
-	if ((rc = set_smem_attr<0, false, 0, 0, 128>(smem128))) return rc;
-	if ((rc = set_smem_attr<1, false, 0, 0, 128>(smem128))) return rc;
-	if ((rc = set_smem_attr<2, false, 0, 0, 128>(smem128))) return rc;
-	if ((rc = set_smem_attr<3, false, 0, 0, 128>(smem128))) return rc;
-	if ((rc = set_smem_attr<4, false, 0, 0, 128>(smem128))) return rc;
-	if ((rc = set_smem_attr<2, false, 8, 8, 128>(smem128))) return rc;
-	if ((rc = set_smem_attr<4, false, 8, 5, 128>(smem128))) return rc;
-	if ((rc = set_smem_attr<3, false, 5, 8, 128>(smem128))) return rc;
-#endif
-	if ((rc = set_all_bs_attrs())) return rc;
-	if ((rc = set_all_recover_attrs())) return rc;
-	if ((rc = set_all_convert_attrs())) return rc;
-	return LZGPU_OK;
+	return set_all_smem_attrs(fs);
 }
 
 void lz_fused_destroy(lzgpu_ctx *ctx) {
@@ -336,81 +377,15 @@ extern "C" int lzgpu_debug_last_geometry(lzgpu_ctx *ctx, lzgpu_launch_geometry *
 	return LZGPU_OK;
 }
 
-static int make_tensor_map(FusedState *fs, CUtensorMap *map, const void *base, uint64_t rows_per_chunk, uint64_t n_chunks,
-                           uint64_t chunk_stride, uint32_t box_rows) {
+// rows_per_chunk rows of kRowBytes per chunk, chunk c at base + c * chunk_stride (0: contiguous), boxes of box_rows rows
+static CUresult make_tensor_map(const FusedState *fs, CUtensorMap *map, const void *base, uint64_t rows_per_chunk, uint64_t n_chunks,
+                                uint64_t chunk_stride, uint32_t box_rows) {
 	const cuuint64_t dims[3] = {static_cast<cuuint64_t>(kRowBytes), rows_per_chunk, n_chunks};
 	const cuuint64_t strides[2] = {static_cast<cuuint64_t>(kRowBytes), chunk_stride ? chunk_stride : rows_per_chunk * kRowBytes};
 	const cuuint32_t box[3] = {kStepBytes, box_rows, 1};
 	const cuuint32_t estr[3] = {1, 1, 1};
-	CUresult r = fs->encode_tiled(map, CU_TENSOR_MAP_DATA_TYPE_UINT8, 3, const_cast<void *>(base), dims, strides, box, estr,
-	                              CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, static_cast<CUtensorMapL2promotion>(fs->promo),
-	                              CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-	if (r != CUDA_SUCCESS) {
-		lz_set_error("cuTensorMapEncodeTiled failed with CUresult %d (rows/chunk %llu, chunks %llu, stride %llu, box rows %u)",
-		             static_cast<int>(r), static_cast<unsigned long long>(rows_per_chunk), static_cast<unsigned long long>(n_chunks),
-		             static_cast<unsigned long long>(chunk_stride), box_rows);
-		return LZGPU_ERR_CUDA;
-	}
-	return LZGPU_OK;
-}
-
-template <int M, bool GENERIC, int KT = 0, int GT = 0, int FW = 64, bool STRIPED = false, bool SPLIT = false>
-static int launch(lzgpu_ctx *ctx, const CUtensorMap &map, const FusedParams &p, size_t smem, cudaStream_t st) {
-	const int grid = persistent_grid(ctx, p.total_units, fused_ctas_per_sm(M, GENERIC, FW),
-	                                 launch_geo(LZGPU_KERNEL_ENCODE, fused_threads(M, GENERIC), p.G, fused_nst(FW, M, GENERIC), 0, smem));
-	if (GENERIC && fused_generic_item_words(p.G) == 1)
-		fused_stream_kernel<M, GENERIC, KT, GT, FW, STRIPED, SPLIT, GENERIC ? 1 : fused_item_words(M, GENERIC)><<<grid, fused_threads(M, GENERIC), smem, st>>>(map, p);
-	else
-		fused_stream_kernel<M, GENERIC, KT, GT, FW, STRIPED, SPLIT><<<grid, fused_threads(M, GENERIC), smem, st>>>(map, p);
-	CUDA_TRY(cudaGetLastError());
-	ctx->stats.kernel_launches++;
-	return LZGPU_OK;
-}
-
-// bit-sliced instantiations (W = 8: one 16-warp CTA per SM, the last ceil(16 G / 32) warps take the 16 G items of a step, the warps before them the
-// G (K + M - 1) * 4 streams; the plan made with bs = true guarantees both fit)
-template <int M, int KT = 0, int GT = 0, bool STRIPED = false>
-static int set_bs_attr() {
-	CUDA_TRY(cudaFuncSetAttribute(fused_stream_kernel<M, false, KT, GT, 64, STRIPED, false, 8>, cudaFuncAttributeMaxDynamicSharedMemorySize, 226 * 1024));
-	return LZGPU_OK;
-}
-template <int M, int KT = 0, int GT = 0, bool STRIPED = false>
-static int launch_bs(lzgpu_ctx *ctx, const CUtensorMap &map, const FusedParams &p, size_t smem, cudaStream_t st) {
-	const int grid = persistent_grid(ctx, p.total_units, 1, launch_geo(LZGPU_KERNEL_ENCODE_BITSLICE, kBsThreads, p.G, p.n_stages, (16 * p.G + 31) / 32, smem));
-	fused_stream_kernel<M, false, KT, GT, 64, STRIPED, false, 8><<<grid, kBsThreads, smem, st>>>(map, p);
-	CUDA_TRY(cudaGetLastError());
-	ctx->stats.kernel_launches++;
-	return LZGPU_OK;
-}
-// the constant-folded (M, K, G) of the bit-sliced route: G from pick_group(.., bs = true)
-#define LZ_BS_FOLDED_LIST(X) X(4, 8, 8) X(4, 10, 6) X(4, 12, 5) X(4, 6, 8) X(4, 4, 8) X(3, 8, 8) X(3, 9, 6) X(3, 10, 6) X(3, 12, 5)
-#define LZ_BS_FOLDED_STRIPED_LIST(X) X(4, 8, 8)
-static int set_all_bs_attrs() {
-	int rc;
-#define LZ_X(MM, KK, GG) if ((rc = set_bs_attr<MM, KK, GG>())) return rc;
-	LZ_BS_FOLDED_LIST(LZ_X)
-#undef LZ_X
-#define LZ_X(MM, KK, GG) if ((rc = set_bs_attr<MM, KK, GG, true>())) return rc;
-	LZ_BS_FOLDED_STRIPED_LIST(LZ_X)
-#undef LZ_X
-	if ((rc = set_bs_attr<3>()) || (rc = set_bs_attr<4>()) || (rc = set_bs_attr<3, 0, 0, true>()) || (rc = set_bs_attr<4, 0, 0, true>())) return rc;
-	return LZGPU_OK;
-}
-
-// Fold window per shape: the 128-word window (3 LOP3 per word, one CTA per SM) pays off where the kernel is ALU bound
-// (many parity rows); the 64-word window (two CTAs per SM) is the default.  LZGPU_FOLD=64|128 forces one.
-// (measured: the 128-word window is slower for every goal — the kernels are bound by
-// per-warp latency, not ALU throughput, and halving the resident warps costs more than the saved LOP3s — so it is only
-// compiled with -DLZ_ENABLE_FOLD128 for experiments)
-static int choose_fold(const FusedState *fs, int M, bool generic) {
-	(void)M;
-#ifdef LZ_ENABLE_FOLD128
-	if (fs->fold == 128 && !generic) return 128;
-#else
-	(void)fs;
-	(void)generic;
-#endif
-	return 64;
+	return fs->encode_tiled(map, CU_TENSOR_MAP_DATA_TYPE_UINT8, 3, const_cast<void *>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+	                        CU_TENSOR_MAP_SWIZZLE_128B, static_cast<CUtensorMapL2promotion>(fs->promo), CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
 }
 
 // split_out != nullptr: the conversion form — K + M destination part buffers (nullptr = part not wanted), data parts stored by the
@@ -420,15 +395,13 @@ static int fused_run(lzgpu_ctx *ctx, int M, bool generic, const uint8_t *coef_ro
                      cudaStream_t st, void *const *split_out = nullptr, size_t split_stride = 0, uint32_t crc_row_base = 0, bool skip_data_crc = false,
                      int striped_policy = -2 /* -2: the context's setting */) {
 	FusedState *fs = ctx->fused;
-	const uint32_t PC = M == 0 ? 0 : (generic ? M : M - 1);
-	const int fw = choose_fold(fs, M, generic);
 	// unit geometry: per-chunk, flat or striped units, stripes per unit (fused_plan.h; unit-tested without a GPU); the bit-sliced
 	// geometry first where it is switched on, the packed-byte one if a shape does not fit it
 	const int spol = split_out ? 0 : (striped_policy == -2 ? fs->striped : striped_policy);
 	FusedPlan pl;
-	if (!split_out && fw == 64 && fused_bitslice(M, generic, fs->bitslice, K))
-		pl = fused_plan(M, generic, K, n_chunks, nb, chunk_stride, std::min(fs->max_smem, fs->bs_smem_cap), fw, spol, true, fs->bs_max_stages, fs->bs_max_gf_warps);
-	if (!pl.ok) pl = fused_plan(M, generic, K, n_chunks, nb, chunk_stride, std::min(fs->max_smem, fw == 64 ? fused_smem_cap(M, generic, fw) : kSmemCap128), fw, spol);
+	if (!split_out && fused_bitslice(M, generic, fs->bitslice, K))
+		pl = fused_plan(M, generic, K, n_chunks, nb, chunk_stride, std::min(fs->max_smem, fs->bs_smem_cap), 64, spol, true, fs->bs_max_stages, fs->bs_max_gf_warps);
+	if (!pl.ok) pl = fused_plan(M, generic, K, n_chunks, nb, chunk_stride, std::min(fs->max_smem, fused_smem_cap(M, generic, 64)), 64, spol);
 	if (!pl.ok || (reinterpret_cast<uintptr_t>(d_data) % 16)) return LZGPU_NOT_HANDLED;
 	const uint32_t G = pl.G;
 	const bool flat = pl.mode == 1u, striped = pl.mode == 2u;
@@ -448,7 +421,7 @@ static int fused_run(lzgpu_ctx *ctx, int M, bool generic, const uint8_t *coef_ro
 	p.flat_magic = (1ull << 40) / p.pb + 1;
 	p.units_per_chunk = pl.units_per_chunk;
 	p.total_units = pl.total_units;
-	std::memcpy(p.qmult, fw == 64 ? fs->qmult64 : fs->qmult128, sizeof(p.qmult));
+	std::memcpy(p.qmult, fs->qmult, sizeof(p.qmult));
 	p.zconst = lz::crc_of_zeros(LZGPU_BLOCK_SIZE);
 	p.probe = fs->probe;
 	p.evict_first = static_cast<uint32_t>(fs->evict_first);
@@ -460,129 +433,29 @@ static int fused_run(lzgpu_ctx *ctx, int M, bool generic, const uint8_t *coef_ro
 				coef_planes_set(p.coef[r * 32 + j], coef_rows[r * K + j]);
 			}
 	}
+	// flat: the batch is one run of stripes; striped: one box per stripe
+	const uint64_t map_rows = flat ? static_cast<uint64_t>(n_chunks) * nb * 4 : static_cast<uint64_t>(nb) * 4, map_chunks = flat ? 1 : n_chunks;
+	const uint64_t map_stride = flat ? 0 : chunk_stride;
+	const uint32_t box_rows = striped ? K * 4 : G * K * 4;
 	CUtensorMap map;
-	const uint32_t rows = G * K * 4;
-	int rc = flat ? make_tensor_map(fs, &map, d_data, static_cast<uint64_t>(n_chunks) * nb * 4, 1, 0, rows)
-	              : make_tensor_map(fs, &map, d_data, static_cast<uint64_t>(nb) * 4, n_chunks, chunk_stride, striped ? K * 4 : rows);
-	if (rc) return rc;
-	const size_t smem = pl.smem;
-	(void)PC;
+	const CUresult r = make_tensor_map(fs, &map, d_data, map_rows, map_chunks, map_stride, box_rows);
+	if (r != CUDA_SUCCESS) {
+		lz_set_error("cuTensorMapEncodeTiled failed with CUresult %d (rows/chunk %llu, chunks %llu, stride %llu, box rows %u)", static_cast<int>(r),
+		             static_cast<unsigned long long>(map_rows), static_cast<unsigned long long>(map_chunks), static_cast<unsigned long long>(map_stride), box_rows);
+		return LZGPU_ERR_CUDA;
+	}
 	if (split_out) {
 		if (striped || (split_stride % 16)) return LZGPU_NOT_HANDLED;
 		for (uint32_t j = 0; j < K; ++j) p.data_out[j] = static_cast<uint8_t *>(split_out[j]);
 		for (int r = 0; r < M; ++r) p.par_out[r] = static_cast<uint8_t *>(split_out[K + r]);
 		p.part_out_stride = split_stride;
-		if (generic) {
-			if (M != 4) return LZGPU_NOT_HANDLED;
-			return launch<4, true, 0, 0, 64, false, true>(ctx, map, p, smem, st);
-		}
-		switch (M) {
-			case 1: return launch<1, false, 0, 0, 64, false, true>(ctx, map, p, smem, st);
-			case 2: return launch<2, false, 0, 0, 64, false, true>(ctx, map, p, smem, st);
-			case 3: return launch<3, false, 0, 0, 64, false, true>(ctx, map, p, smem, st);
-			case 4: return launch<4, false, 0, 0, 64, false, true>(ctx, map, p, smem, st);
-		}
-		return LZGPU_NOT_HANDLED;
 	}
-	if (pl.bs) {
-		if (striped) {
-#define LZ_X(MM, KK, GG) if (M == MM && K == KK && G == GG) return launch_bs<MM, KK, GG, true>(ctx, map, p, smem, st);
-			LZ_BS_FOLDED_STRIPED_LIST(LZ_X)
-#undef LZ_X
-			return M == 3 ? launch_bs<3, 0, 0, true>(ctx, map, p, smem, st) : launch_bs<4, 0, 0, true>(ctx, map, p, smem, st);
-		}
-#define LZ_X(MM, KK, GG) if (M == MM && K == KK && G == GG) return launch_bs<MM, KK, GG>(ctx, map, p, smem, st);
-		LZ_BS_FOLDED_LIST(LZ_X)
-#undef LZ_X
-		return M == 3 ? launch_bs<3>(ctx, map, p, smem, st) : launch_bs<4>(ctx, map, p, smem, st);
-	}
-	if (striped) {
-		if (generic) {
-			if (M != 4) return LZGPU_NOT_HANDLED;
-			return launch<4, true, 0, 0, 64, true>(ctx, map, p, smem, st);
-		}
-#define LZ_FOLDED_STRIPED(MM, KK, GG) \
-	if (M == MM && K == KK && G == GG) return launch<MM, false, KK, GG, 64, true>(ctx, map, p, smem, st);
-		LZ_FOLDED_STRIPED(2, 8, 7)
-		LZ_FOLDED_STRIPED(1, 2, 32)
-		LZ_FOLDED_STRIPED(1, 3, 20)
-		LZ_FOLDED_STRIPED(2, 3, 16)
-		LZ_FOLDED_STRIPED(3, 5, 8)
-		LZ_FOLDED_STRIPED(4, 8, 8)
-#undef LZ_FOLDED_STRIPED
-		switch (M) {
-			case 1: return launch<1, false, 0, 0, 64, true>(ctx, map, p, smem, st);
-			case 2: return launch<2, false, 0, 0, 64, true>(ctx, map, p, smem, st);
-			case 3: return launch<3, false, 0, 0, 64, true>(ctx, map, p, smem, st);
-			case 4: return launch<4, false, 0, 0, 64, true>(ctx, map, p, smem, st);
-		}
-		return LZGPU_NOT_HANDLED;
-	}
-	if (generic) {
-		switch (M) {
-			case 1: return launch<1, true>(ctx, map, p, smem, st);
-			case 2: return launch<2, true>(ctx, map, p, smem, st);
-			case 3: return launch<3, true>(ctx, map, p, smem, st);
-			case 4: return launch<4, true>(ctx, map, p, smem, st);
-		}
-		return LZGPU_NOT_HANDLED;
-	}
-#ifdef LZ_ENABLE_FOLD128
-	if (fw == 128) {
-		if (M == 2 && K == 8 && G == 8) return launch<2, false, 8, 8, 128>(ctx, map, p, smem, st);
-		if (M == 4 && K == 8 && G == 5) return launch<4, false, 8, 5, 128>(ctx, map, p, smem, st);
-		if (M == 3 && K == 5 && G == 8) return launch<3, false, 5, 8, 128>(ctx, map, p, smem, st);
-		switch (M) {
-			case 0: return launch<0, false, 0, 0, 128>(ctx, map, p, smem, st);
-			case 1: return launch<1, false, 0, 0, 128>(ctx, map, p, smem, st);
-			case 2: return launch<2, false, 0, 0, 128>(ctx, map, p, smem, st);
-			case 3: return launch<3, false, 0, 0, 128>(ctx, map, p, smem, st);
-			case 4: return launch<4, false, 0, 0, 128>(ctx, map, p, smem, st);
-		}
-		return LZGPU_NOT_HANDLED;
-	}
-#endif
-	// constant-folded instantiations for the common goals (k, G from pick_group), runtime k/G otherwise
-#define LZ_FOLDED(MM, KK, GG) \
-	if (M == MM && K == KK && G == GG) return launch<MM, false, KK, GG>(ctx, map, p, smem, st);
-	LZ_FOLDED(2, 8, 7)    // ec(8,2)
-	LZ_FOLDED(1, 2, 32)   // xor2
-	LZ_FOLDED(1, 3, 20)   // xor3
-	LZ_FOLDED(2, 3, 16)   // ec(3,2)
-	LZ_FOLDED(2, 4, 12)   // ec(4,2)
-	LZ_FOLDED(2, 6, 9)    // ec(6,2)
-	LZ_FOLDED(3, 5, 8)    // ec(5,3)
-	LZ_FOLDED(3, 6, 8)    // ec(6,3)
-	LZ_FOLDED(4, 8, 8)    // ec(8,4) on one 16-warp CTA per SM
-	// more goals folded (the runtime-k instantiation measured markedly slower for ec(8,3), ec(6,4), ec(4,4))
-	LZ_FOLDED(3, 8, 6)    // ec(8,3)
-	LZ_FOLDED(1, 4, 16)   // xor4 / ec(4,1)
-	LZ_FOLDED(2, 5, 10)   // ec(5,2)
-	LZ_FOLDED(2, 10, 5)   // ec(10,2)
-	LZ_FOLDED(3, 4, 8)    // ec(4,3)
-	LZ_FOLDED(4, 10, 6)   // ec(10,4)
-	LZ_FOLDED(4, 12, 5)   // ec(12,4)
-	LZ_FOLDED(4, 6, 8)    // ec(6,4)
-	LZ_FOLDED(4, 4, 8)    // ec(4,4)
-#if LZ_T2 == 288
-	LZ_FOLDED(2, 8, 8)    // experiment builds with the nine-warp CTA of round 1
-#endif
-#if LZ_T4 != 512
-	LZ_FOLDED(4, 8, 5)
-#endif
-#if LZ_T3 == 512
-	LZ_FOLDED(3, 5, 12)
-	LZ_FOLDED(3, 6, 10)
-#endif
-#undef LZ_FOLDED
-	switch (M) {
-		case 0: return launch<0, false>(ctx, map, p, smem, st);
-		case 1: return launch<1, false>(ctx, map, p, smem, st);
-		case 2: return launch<2, false>(ctx, map, p, smem, st);
-		case 3: return launch<3, false>(ctx, map, p, smem, st);
-		case 4: return launch<4, false>(ctx, map, p, smem, st);
-	}
-	return LZGPU_NOT_HANDLED;
+	const EncodeKernelEntry *k = find_encoder(M, generic, K, G, striped, split_out != nullptr, pl.bs);
+	if (!k) return LZGPU_NOT_HANDLED;
+	const lzgpu_launch_geometry geo = launch_geo(pl.bs ? LZGPU_KERNEL_ENCODE_BITSLICE : LZGPU_KERNEL_ENCODE, pl.threads, G, pl.n_stages,
+	                                             pl.bs ? (16 * G + 31) / 32 : 0, pl.smem);
+	const EncodeKernel fn = k->narrow && fused_generic_item_words(G) == 1 ? k->narrow : k->fn;
+	return launch(ctx, fn, geo, fused_ctas_per_sm(M, generic, 64, pl.bs), p.total_units, st, map, p);
 }
 
 int lz_fused_encode(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, uint32_t nb, const void *d_data, size_t chunk_stride,
@@ -662,69 +535,6 @@ int lz_fused_crc(lzgpu_ctx *ctx, const void *base, unsigned long long n_blocks, 
 // ---------------------------------------------------------------------------------------------------
 // fused degraded read
 // ---------------------------------------------------------------------------------------------------
-// DIRECT form of the degraded read (any generator; the Cauchy codes): 16-warp CTA, runtime k, 16- or 4-byte items
-template <int E>
-static int launch_direct(lzgpu_ctx *ctx, const TmapArray &maps, const RecoverParams &p, size_t smem, cudaStream_t st, bool wide) {
-	const int grid = persistent_grid(ctx, p.total_units, 1, launch_geo(LZGPU_KERNEL_RECOVER_DIRECT, recover_threads(2), p.G, p.n_stages, 0, smem));
-	if (wide) fused_recover_kernel<E, 0, kRecoverDirect, -1, 64, 2, direct_wide_words(E)><<<grid, recover_threads(2), smem, st>>>(maps, p);
-	else fused_recover_kernel<E, 0, kRecoverDirect, -1, 64, 2, 1><<<grid, recover_threads(2), smem, st>>>(maps, p);
-	CUDA_TRY(cudaGetLastError());
-	ctx->stats.kernel_launches++;
-	return LZGPU_OK;
-}
-
-// the 16-warp geometry alone (instantiations with a compile-time k other than 8: ec(3,2), the BASELINE configs[1] goal)
-template <int E, int KT, int R0, int R1>
-static int launch_recover_geo2(lzgpu_ctx *ctx, const TmapArray &maps, const RecoverParams &p, size_t smem, cudaStream_t st) {
-	const int gridb = persistent_grid(ctx, p.total_units, 1, launch_geo(LZGPU_KERNEL_RECOVER_GEO2, recover_threads(2), p.G, p.n_stages, 0, smem));
-	fused_recover_kernel<E, KT, R0, R1, 64, 2><<<gridb, recover_threads(2), smem, st>>>(maps, p);
-	CUDA_TRY(cudaGetLastError());
-	ctx->stats.kernel_launches++;
-	return LZGPU_OK;
-}
-
-template <int E, int KT, int R0 = -1, int R1 = -1>
-static int launch_recover(lzgpu_ctx *ctx, const TmapArray &maps, const RecoverParams &p, size_t smem, cudaStream_t st, int geo) {
-	if (geo == 2) {
-		const int gridb = persistent_grid(ctx, p.total_units, 1, launch_geo(LZGPU_KERNEL_RECOVER_GEO2, recover_threads(2), p.G, p.n_stages, 0, smem));
-		fused_recover_kernel<E, KT, R0, R1, 64, 2><<<gridb, recover_threads(2), smem, st>>>(maps, p);
-		CUDA_TRY(cudaGetLastError());
-		ctx->stats.kernel_launches++;
-		return LZGPU_OK;
-	}
-	if (geo == 1 && E <= 2) {
-		const int grid2 = persistent_grid(ctx, p.total_units, 2, launch_geo(LZGPU_KERNEL_RECOVER_GEO1, kFusedThreads, p.G, recover_stages(1), 0, smem));
-		fused_recover_kernel<(E <= 2 ? E : 1), KT, R0, R1, 64, 1><<<grid2, kFusedThreads, smem, st>>>(maps, p);
-		CUDA_TRY(cudaGetLastError());
-		ctx->stats.kernel_launches++;
-		return LZGPU_OK;
-	}
-	const int grid = persistent_grid(ctx, p.total_units, 1, launch_geo(LZGPU_KERNEL_RECOVER_GEO0, kFusedThreads, p.G, recover_stages(0), 0, smem));
-#ifdef LZ_ENABLE_FOLD128
-	if (ctx->fused->fold == 128) fused_recover_kernel<E, KT, R0, R1, 128><<<grid, kFusedThreads, smem, st>>>(maps, p);
-	else
-#endif
-		fused_recover_kernel<E, KT, R0, R1, 64><<<grid, kFusedThreads, smem, st>>>(maps, p);
-	CUDA_TRY(cudaGetLastError());
-	ctx->stats.kernel_launches++;
-	return LZGPU_OK;
-}
-
-// instantiations with a compile-time k other than 8 (ec(3,2), the BASELINE configs[1] goal; ec(4,2), ec(5,3), ec(6,2), ec(6,3)) exist
-// on the 16-warp geometry only; the plan names them with kt, e and rows 0 .. e-1
-static int launch_recover_kt(lzgpu_ctx *ctx, const TmapArray &maps, const RecoverParams &p, size_t smem, cudaStream_t st, const lzgpu_recover_plan &o) {
-	switch (o.kt * 8 + o.lost_data_parts) {
-		case 3 * 8 + 1: return launch_recover_geo2<1, 3, 0, -1>(ctx, maps, p, smem, st);
-		case 3 * 8 + 2: return launch_recover_geo2<2, 3, 0, 1>(ctx, maps, p, smem, st);
-		case 4 * 8 + 2: return launch_recover_geo2<2, 4, 0, 1>(ctx, maps, p, smem, st);
-		case 5 * 8 + 2: return launch_recover_geo2<2, 5, 0, 1>(ctx, maps, p, smem, st);
-		case 5 * 8 + 3: return launch_recover_geo2<3, 5, 0, 1>(ctx, maps, p, smem, st);
-		case 6 * 8 + 2: return launch_recover_geo2<2, 6, 0, 1>(ctx, maps, p, smem, st);
-		case 6 * 8 + 3: return launch_recover_geo2<3, 6, 0, 1>(ctx, maps, p, smem, st);
-		default: lz_set_error("recover: no instantiation for k = %u, e = %u", o.kt, o.lost_data_parts); return LZGPU_ERR_ARG;
-	}
-}
-
 int lz_fused_recover(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, uint32_t nb, const void *const *d_parts, size_t part_stride,
                      const void *const *d_part_crc, const uint8_t *want, void *const *d_out, void *d_chunk_out, size_t chunk_out_stride,
                      cudaStream_t st, unsigned long long *d_first_bad) {
@@ -745,8 +555,7 @@ int lz_fused_recover(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, 
 	const RecoverPlan pl = recover_plan(K, M, direct, available, want_missing_parity, verifying, d_chunk_out != nullptr, fs->recover);
 	const lzgpu_recover_plan &o = pl.out;
 	if (!o.fused) return LZGPU_NOT_HANDLED;
-	const uint32_t e = o.lost_data_parts, G = o.G, n_stages = o.stages;
-	const int geo = pl.geo;
+	const uint32_t e = o.lost_data_parts, G = o.G;
 	RecoverParams p{};
 	std::memset(p.slot_of_data, 0xff, sizeof(p.slot_of_data));
 	for (int a = 0; a < K; ++a) {
@@ -761,11 +570,10 @@ int lz_fused_recover(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, 
 		p.par_row[x] = pl.par_row[x];
 	}
 	const uint32_t pb = (nb + K - 1) / K;
-	for (uint32_t x = 0; x < e; ++x) {
+	for (uint32_t x = 0; x < e; ++x) {   // a part nothing is requested for is still solved (cheap), not stored
 		const int j = p.erased_idx[x];
 		void *dst = d_out ? d_out[j] : nullptr;
 		p.out[x] = (want[j] || d_chunk_out) ? static_cast<uint8_t *>(dst) : nullptr;
-		if (!p.out[x] && !d_chunk_out) {}  // nothing requested for this part: still solved (cheap), not stored
 	}
 	p.image = static_cast<uint8_t *>(d_chunk_out);
 	p.out_stride = part_stride;
@@ -782,19 +590,14 @@ int lz_fused_recover(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, 
 	if (total > 0x7fffffffull) return LZGPU_NOT_HANDLED;
 	p.total_units = static_cast<uint32_t>(total);
 	p.e = e;
-	p.n_stages = n_stages;
-#ifdef LZ_ENABLE_FOLD128
-	std::memcpy(p.qmult, fs->fold == 128 ? fs->qmult128 : fs->qmult64, sizeof(p.qmult));
-#else
-	std::memcpy(p.qmult, fs->qmult64, sizeof(p.qmult));
-#endif
+	p.n_stages = o.stages;
+	std::memcpy(p.qmult, fs->qmult, sizeof(p.qmult));
 	p.zconst = lz::crc_of_zeros(LZGPU_BLOCK_SIZE);
 	for (int a = 0; a < K; ++a) p.stored[a] = d_part_crc ? static_cast<const uint32_t *>(d_part_crc[pl.used[a]]) : nullptr;
 	// V[r][x] = (2^row_r)^(erased_x); W = V^-1
 	uint8_t V[16], W[16];
 	for (uint32_t r = 0; r < e; ++r) {
-		uint8_t gen = 1;
-		for (int t = 0; t < p.par_row[r]; ++t) gen = lz::gf_mul_host(gen, 2);
+		const uint8_t gen = gf_pow2(p.par_row[r]);
 		for (uint32_t x = 0; x < e; ++x) {
 			uint8_t v = 1;
 			for (int t = 0; t < p.erased_idx[x]; ++t) v = lz::gf_mul_host(v, gen);
@@ -819,14 +622,10 @@ int lz_fused_recover(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, 
 			coef_planes_set(p.w[x * 4 + r], W[x * e + r]);
 		}
 	p.raid6_dbl = 0xffu;
-	const bool k8 = K == 8 && (G == 8 || geo == 2);
+	const bool k8 = K == 8 && (G == 8 || pl.geo == 2);
 	if (e == 2 && p.par_row[0] == 0 && p.par_row[1] == 1 && !k8) {
-		// RAID-6 shape on a runtime-k instantiation: w[0] = planes of 2^x0, w[1] = planes of (2^x0 ^ 2^x1)^-1 (see the kernel)
-		uint8_t gx0 = 1, gx1 = 1;
-		for (int t = 0; t < p.erased_idx[0]; ++t) gx0 = lz::gf_mul_host(gx0, 2);
-		for (int t = 0; t < p.erased_idx[1]; ++t) gx1 = lz::gf_mul_host(gx1, 2);
-		coef_planes_set(p.w[0], gx0);
-		coef_planes_set(p.w[1], lz::gf_inv_host(gx0 ^ gx1));
+		// RAID-6 shape on a runtime-k instantiation (see the kernel)
+		set_raid6_pair(p.w, p.erased_idx[0], p.erased_idx[1]);
 		if (o.solve == LZGPU_RECOVER_SOLVE_RAID6 && o.doublings >= 0) p.raid6_dbl = static_cast<uint32_t>(o.doublings);
 	}
 	// "rows 0, 1, .., e-1 in use" (the first e parity parts are the available ones — the common case): instantiations that
@@ -834,82 +633,34 @@ int lz_fused_recover(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, 
 	bool consecutive = true;
 	for (uint32_t r = 0; r < e; ++r) consecutive &= p.par_row[r] == r;
 	p.elim3_dbl = 0xffu;
+	uint8_t elim3[6] = {0};
 	if (e == 3 && consecutive) {
-		// three unknowns, parity rows 0, 1, 2: the elimination of the kernel comment (w[0..3] = alpha, beta, gamma, delta; w[4], w[5]
-		// = 2^a, 4^a when a > 3).  p, q, p^q are non-zero because 2 has order 255 and the positions differ by less than 32.
-		auto pw2 = [](int t) { uint8_t v = 1; for (int i = 0; i < t; ++i) v = lz::gf_mul_host(v, 2); return v; };
-		const uint8_t A = pw2(p.erased_idx[0]), B = pw2(p.erased_idx[1]), C = pw2(p.erased_idx[2]);
-		const uint8_t pp = A ^ B, qq = A ^ C;
-		const uint8_t alpha = lz::gf_inv_host(lz::gf_mul_host(qq, pp ^ qq)), beta = lz::gf_mul_host(pp, alpha);
-		const uint8_t gamma = lz::gf_inv_host(pp), delta = lz::gf_mul_host(qq, gamma);
-		coef_planes_set(p.w[0], alpha);
-		coef_planes_set(p.w[1], beta);
-		coef_planes_set(p.w[2], gamma);
-		coef_planes_set(p.w[3], delta);
-		coef_planes_set(p.w[4], A);
-		coef_planes_set(p.w[5], lz::gf_mul_host(A, A));
+		// three unknowns, parity rows 0, 1, 2: w[0..3] = alpha, beta, gamma, delta; w[4], w[5] = 2^a, 4^a when a > 3
+		elim3_constants(p.erased_idx[0], p.erased_idx[1], p.erased_idx[2], elim3);
+		for (int i = 0; i < 6; ++i) coef_planes_set(p.w[i], elim3[i]);
 		if (o.solve == LZGPU_RECOVER_SOLVE_ELIM3 && o.doublings >= 0) p.elim3_dbl = static_cast<uint32_t>(o.doublings);
 	}
 	TmapArray maps;
-	for (int a = 0; a < K; ++a) {
-		const cuuint64_t dims[3] = {static_cast<cuuint64_t>(kRowBytes), static_cast<cuuint64_t>(pb) * 4, n_chunks};
-		const cuuint64_t strides[2] = {static_cast<cuuint64_t>(kRowBytes), part_stride};
-		const cuuint32_t box[3] = {kStepBytes, G * 4, 1};
-		const cuuint32_t estr[3] = {1, 1, 1};
-		CUresult r = fs->encode_tiled(&maps.m[a], CU_TENSOR_MAP_DATA_TYPE_UINT8, 3, const_cast<void *>(d_parts[pl.used[a]]), dims, strides, box, estr,
-		                              CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, static_cast<CUtensorMapL2promotion>(fs->promo),
-		                              CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-		if (r != CUDA_SUCCESS) return LZGPU_NOT_HANDLED;
-	}
+	for (int a = 0; a < K; ++a)
+		if (make_tensor_map(fs, &maps.m[a], d_parts[pl.used[a]], static_cast<uint64_t>(pb) * 4, n_chunks, part_stride, G * 4) != CUDA_SUCCESS)
+			return LZGPU_NOT_HANDLED;
 	if (verifying && !d_first_bad) return LZGPU_NOT_HANDLED;  // (callers that pass stored CRCs always pass the result word, initialised to ~0)
-	const size_t smem = o.smem_bytes;
 	// what the plan names is what launches
+	const lzgpu_launch_geometry geo = launch_geo(o.kernel, o.threads, G, o.stages, o.gf_warps, o.smem_bytes);
 	if (o.kernel == LZGPU_KERNEL_RECOVER_BS3) {
-		// the six constants of the elimination (computed above for the packed-word kernel) as 8 x 8 bit matrices of all-ones / zero words
+		// the six constants of the elimination (set above for the packed-word kernel) as 8 x 8 bit matrices of all-ones / zero words
 		BsRecoverMasks mk;
-		auto pw2 = [](int t) { uint8_t v = 1; for (int i = 0; i < t; ++i) v = lz::gf_mul_host(v, 2); return v; };
-		const uint8_t A = pw2(p.erased_idx[0]), B = pw2(p.erased_idx[1]), C = pw2(p.erased_idx[2]);
-		const uint8_t pp = A ^ B, qq = A ^ C;
-		const uint8_t alpha = lz::gf_inv_host(lz::gf_mul_host(qq, pp ^ qq)), beta = lz::gf_mul_host(pp, alpha);
-		const uint8_t gamma = lz::gf_inv_host(pp), delta = lz::gf_mul_host(qq, gamma);
-		bs_mask_set(mk.m[0], alpha);
-		bs_mask_set(mk.m[1], beta);
-		bs_mask_set(mk.m[2], gamma);
-		bs_mask_set(mk.m[3], delta);
-		bs_mask_set(mk.m[4], A);
-		bs_mask_set(mk.m[5], lz::gf_mul_host(A, A));
-		const int grid = persistent_grid(ctx, p.total_units, 1, launch_geo(LZGPU_KERNEL_RECOVER_BS3, o.threads, G, n_stages, o.gf_warps, smem));
-		if (o.kt == 5) bs_recover3_kernel<5><<<grid, kBsRecoverThreads, smem, st>>>(maps, p, mk);
-		else if (o.kt == 8) bs_recover3_kernel<8><<<grid, kBsRecoverThreads, smem, st>>>(maps, p, mk);
-		else bs_recover3_kernel<0><<<grid, kBsRecoverThreads, smem, st>>>(maps, p, mk);
-		CUDA_TRY(cudaGetLastError());
-		ctx->stats.kernel_launches++;
-		return LZGPU_OK;
+		for (int i = 0; i < 6; ++i) bs_mask_set(mk.m[i], elim3[i]);
+		for (const auto &k : kBsRecoverers)
+			if (k.kt == o.kt) return launch(ctx, k.fn, geo, 1, p.total_units, st, maps, p, mk);
+	} else {
+		const bool first_e = o.rows == LZGPU_RECOVER_ROWS_FIRST_E;
+		for (const RecoverKernelEntry &k : kRecoverers)
+			if (k.kernel == o.kernel && k.e == e && k.kt == o.kt && k.first_e == first_e && k.wide == pl.wide)
+				return launch(ctx, k.fn, geo, o.kernel == LZGPU_KERNEL_RECOVER_GEO1 ? 2 : 1, p.total_units, st, maps, p);
 	}
-	if (o.kernel == LZGPU_KERNEL_RECOVER_DIRECT) {
-		switch (e) {
-			case 1: return launch_direct<1>(ctx, maps, p, smem, st, pl.wide);
-			case 2: return launch_direct<2>(ctx, maps, p, smem, st, pl.wide);
-			case 3: return launch_direct<3>(ctx, maps, p, smem, st, pl.wide);
-			default: return launch_direct<4>(ctx, maps, p, smem, st, pl.wide);
-		}
-	}
-	if (o.kt && o.kt != 8) return launch_recover_kt(ctx, maps, p, smem, st, o);
-	const bool first_e = o.rows == LZGPU_RECOVER_ROWS_FIRST_E;
-	switch (e) {
-		case 1:
-			if (first_e) return o.kt == 8 ? launch_recover<1, 8, 0>(ctx, maps, p, smem, st, geo) : launch_recover<1, 0, 0>(ctx, maps, p, smem, st, geo);
-			return launch_recover<1, 0>(ctx, maps, p, smem, st, geo);
-		case 2:
-			if (first_e) return o.kt == 8 ? launch_recover<2, 8, 0, 1>(ctx, maps, p, smem, st, geo) : launch_recover<2, 0, 0, 1>(ctx, maps, p, smem, st, geo);
-			return launch_recover<2, 0>(ctx, maps, p, smem, st, geo);
-		case 3:
-			if (first_e) return launch_recover<3, 0, 0, 1>(ctx, maps, p, smem, st, geo);
-			return launch_recover<3, 0>(ctx, maps, p, smem, st, geo);
-		default:
-			if (first_e) return launch_recover<4, 0, 0, 1>(ctx, maps, p, smem, st, geo);
-			return launch_recover<4, 0>(ctx, maps, p, smem, st, geo);
-	}
+	lz_set_error("recover: no instantiation for k = %u, e = %u", o.kt, o.lost_data_parts);
+	return LZGPU_ERR_ARG;
 }
 
 // ---------------------------------------------------------------------------------------------------
@@ -969,91 +720,34 @@ int lz_fused_check(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, ui
 	if (total > 0x7fffffffull) return LZGPU_NOT_HANDLED;
 	p.total_units = static_cast<uint32_t>(total);
 	p.n_stages = n_stages;
-	std::memcpy(p.qmult, fs->qmult64, sizeof(p.qmult));
+	std::memcpy(p.qmult, fs->qmult, sizeof(p.qmult));
 	p.zconst = lz::crc_of_zeros(LZGPU_BLOCK_SIZE);
 	CheckTmaps maps;
-	for (uint32_t a = 0; a < NSLOT; ++a) {
-		const cuuint64_t dims[3] = {static_cast<cuuint64_t>(kRowBytes), static_cast<cuuint64_t>(pb) * 4, n_chunks};
-		const cuuint64_t strides[2] = {static_cast<cuuint64_t>(kRowBytes), part_stride};
-		const cuuint32_t box[3] = {kStepBytes, G * 4, 1};
-		const cuuint32_t estr[3] = {1, 1, 1};
-		CUresult r = fs->encode_tiled(&maps.m[a], CU_TENSOR_MAP_DATA_TYPE_UINT8, 3, const_cast<void *>(slot_ptr[a]), dims, strides, box, estr,
-		                              CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, static_cast<CUtensorMapL2promotion>(fs->promo),
-		                              CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-		if (r != CUDA_SUCCESS) return LZGPU_NOT_HANDLED;
-	}
-	const size_t smem = o.smem_bytes;
-	const int grid = persistent_grid(ctx, p.total_units, 1, launch_geo(E > 0 ? LZGPU_KERNEL_CHECK_DEGRADED : LZGPU_KERNEL_CHECK, o.threads, G,
-	                                                                   n_stages, 0, smem));
+	for (uint32_t a = 0; a < NSLOT; ++a)
+		if (make_tensor_map(fs, &maps.m[a], slot_ptr[a], static_cast<uint64_t>(pb) * 4, n_chunks, part_stride, G * 4) != CUDA_SUCCESS) return LZGPU_NOT_HANDLED;
+	const lzgpu_launch_geometry geo = launch_geo(E > 0 ? LZGPU_KERNEL_CHECK_DEGRADED : LZGPU_KERNEL_CHECK, o.threads, G, n_stages, 0, o.smem_bytes);
 	uint32_t *d_map = static_cast<uint32_t *>(d_verdict);
 	const bool consecutive = o.consecutive != 0;
-	// E lost data parts, R given parity rows: E < R <= 4, and rows other than 0 .. R-1 only with m <= 4, so R <= 3 (m >= 5 is Cauchy)
-	if (d_failed && E > 0) switch (10 * E + (consecutive ? R : R + 4)) {
-		case 12: fused_check_repair_degraded_kernel<1, 2, true><<<grid, kCheckThreads, smem, st>>>(maps, p, d_map, lost, d_failed); break;
-		case 13: fused_check_repair_degraded_kernel<1, 3, true><<<grid, kCheckThreads, smem, st>>>(maps, p, d_map, lost, d_failed); break;
-		case 14: fused_check_repair_degraded_kernel<1, 4, true><<<grid, kCheckThreads, smem, st>>>(maps, p, d_map, lost, d_failed); break;
-		case 23: fused_check_repair_degraded_kernel<2, 3, true><<<grid, kCheckThreads, smem, st>>>(maps, p, d_map, lost, d_failed); break;
-		case 24: fused_check_repair_degraded_kernel<2, 4, true><<<grid, kCheckThreads, smem, st>>>(maps, p, d_map, lost, d_failed); break;
-		case 34: fused_check_repair_degraded_kernel<3, 4, true><<<grid, kCheckThreads, smem, st>>>(maps, p, d_map, lost, d_failed); break;
-		case 16: fused_check_repair_degraded_kernel<1, 2, false><<<grid, kCheckThreads, smem, st>>>(maps, p, d_map, lost, d_failed); break;
-		case 17: fused_check_repair_degraded_kernel<1, 3, false><<<grid, kCheckThreads, smem, st>>>(maps, p, d_map, lost, d_failed); break;
-		default: fused_check_repair_degraded_kernel<2, 3, false><<<grid, kCheckThreads, smem, st>>>(maps, p, d_map, lost, d_failed); break;
+	if (E > 0) {
+		for (const CheckDegradedKernels &k : kDegradedCheckers)
+			if (k.e == E && k.r == R && k.consecutive == consecutive)
+				return d_failed ? launch(ctx, k.repair, geo, 1, p.total_units, st, maps, p, d_map, lost, d_failed)
+				                : launch(ctx, k.map, geo, 1, p.total_units, st, maps, p, d_map, lost);
+	} else {
+		for (const CheckKernels &k : kCheckers)
+			if (k.r == R && k.consecutive == consecutive)
+				return d_failed ? launch(ctx, k.repair, geo, 1, p.total_units, st, maps, p, d_map, d_failed)
+				       : map    ? launch(ctx, k.map, geo, 1, p.total_units, st, maps, p, d_map)
+				                : launch(ctx, k.check, geo, 1, p.total_units, st, maps, p);
 	}
-	else if (d_failed) switch (consecutive ? R : R + 4) {
-		case 1: fused_check_repair_kernel<1, true><<<grid, kCheckThreads, smem, st>>>(maps, p, d_map, d_failed); break;
-		case 2: fused_check_repair_kernel<2, true><<<grid, kCheckThreads, smem, st>>>(maps, p, d_map, d_failed); break;
-		case 3: fused_check_repair_kernel<3, true><<<grid, kCheckThreads, smem, st>>>(maps, p, d_map, d_failed); break;
-		case 4: fused_check_repair_kernel<4, true><<<grid, kCheckThreads, smem, st>>>(maps, p, d_map, d_failed); break;
-		case 5: fused_check_repair_kernel<1, false><<<grid, kCheckThreads, smem, st>>>(maps, p, d_map, d_failed); break;
-		case 6: fused_check_repair_kernel<2, false><<<grid, kCheckThreads, smem, st>>>(maps, p, d_map, d_failed); break;
-		default: fused_check_repair_kernel<3, false><<<grid, kCheckThreads, smem, st>>>(maps, p, d_map, d_failed); break;
-	}
-	else if (E > 0) switch (10 * E + (consecutive ? R : R + 4)) {
-		case 12: fused_check_degraded_kernel<1, 2, true><<<grid, kCheckThreads, smem, st>>>(maps, p, d_map, lost); break;
-		case 13: fused_check_degraded_kernel<1, 3, true><<<grid, kCheckThreads, smem, st>>>(maps, p, d_map, lost); break;
-		case 14: fused_check_degraded_kernel<1, 4, true><<<grid, kCheckThreads, smem, st>>>(maps, p, d_map, lost); break;
-		case 23: fused_check_degraded_kernel<2, 3, true><<<grid, kCheckThreads, smem, st>>>(maps, p, d_map, lost); break;
-		case 24: fused_check_degraded_kernel<2, 4, true><<<grid, kCheckThreads, smem, st>>>(maps, p, d_map, lost); break;
-		case 34: fused_check_degraded_kernel<3, 4, true><<<grid, kCheckThreads, smem, st>>>(maps, p, d_map, lost); break;
-		case 16: fused_check_degraded_kernel<1, 2, false><<<grid, kCheckThreads, smem, st>>>(maps, p, d_map, lost); break;
-		case 17: fused_check_degraded_kernel<1, 3, false><<<grid, kCheckThreads, smem, st>>>(maps, p, d_map, lost); break;
-		default: fused_check_degraded_kernel<2, 3, false><<<grid, kCheckThreads, smem, st>>>(maps, p, d_map, lost); break;
-	}
-	else if (map) switch (consecutive ? R : R + 4) {
-		case 1: fused_check_map_kernel<1, true><<<grid, kCheckThreads, smem, st>>>(maps, p, d_map); break;
-		case 2: fused_check_map_kernel<2, true><<<grid, kCheckThreads, smem, st>>>(maps, p, d_map); break;
-		case 3: fused_check_map_kernel<3, true><<<grid, kCheckThreads, smem, st>>>(maps, p, d_map); break;
-		case 4: fused_check_map_kernel<4, true><<<grid, kCheckThreads, smem, st>>>(maps, p, d_map); break;
-		case 5: fused_check_map_kernel<1, false><<<grid, kCheckThreads, smem, st>>>(maps, p, d_map); break;
-		case 6: fused_check_map_kernel<2, false><<<grid, kCheckThreads, smem, st>>>(maps, p, d_map); break;
-		default: fused_check_map_kernel<3, false><<<grid, kCheckThreads, smem, st>>>(maps, p, d_map); break;
-	}
-	else switch (consecutive ? R : R + 4) {
-		case 1: fused_check_kernel<1, true><<<grid, kCheckThreads, smem, st>>>(maps, p); break;
-		case 2: fused_check_kernel<2, true><<<grid, kCheckThreads, smem, st>>>(maps, p); break;
-		case 3: fused_check_kernel<3, true><<<grid, kCheckThreads, smem, st>>>(maps, p); break;
-		case 4: fused_check_kernel<4, true><<<grid, kCheckThreads, smem, st>>>(maps, p); break;
-		case 5: fused_check_kernel<1, false><<<grid, kCheckThreads, smem, st>>>(maps, p); break;
-		case 6: fused_check_kernel<2, false><<<grid, kCheckThreads, smem, st>>>(maps, p); break;
-		default: fused_check_kernel<3, false><<<grid, kCheckThreads, smem, st>>>(maps, p); break;
-	}
-	CUDA_TRY(cudaGetLastError());
-	ctx->stats.kernel_launches++;
-	return LZGPU_OK;
+	// (cannot happen: check_plan only gives the (E, R, rows) the lists hold, see kCheckers)
+	lz_set_error("check: no instantiation for e = %u, r = %u, consecutive = %d", E, R, consecutive ? 1 : 0);
+	return LZGPU_ERR_ARG;
 }
 
 // ---------------------------------------------------------------------------------------------------
 // fused slice conversion (convert_kernel.cuh)
 // ---------------------------------------------------------------------------------------------------
-template <int M, int E>
-static int launch_convert(lzgpu_ctx *ctx, const TmapArray &maps, const ConvertParams &p, size_t smem, cudaStream_t st, uint32_t rebuild_warps) {
-	const int grid = persistent_grid(ctx, p.total_units, 2, launch_geo(LZGPU_KERNEL_CONVERT, kConvertThreads, p.G, p.n_stages, rebuild_warps, smem));
-	if (M <= 2 && p.Kd == 3) fused_convert_kernel<(M <= 2 ? M : 1), E, 3><<<grid, kConvertThreads, smem, st>>>(maps, p);   // xor3 / ec(3,2) destinations
-	else fused_convert_kernel<M, E><<<grid, kConvertThreads, smem, st>>>(maps, p);
-	CUDA_TRY(cudaGetLastError());
-	ctx->stats.kernel_launches++;
-	return LZGPU_OK;
-}
 
 // Source slice `src` (k of its parts available in d_parts, at most two data parts lost, the parity parts in use being its rows
 // 0 .. e-1) -> every wanted part of the destination slice `dst` in d_out (nullptr = not wanted) + the destination slice's block
@@ -1082,7 +776,6 @@ int lz_fused_convert(lzgpu_ctx *ctx, const lzgpu_goal *src, const lzgpu_goal *ds
 	p.erased_idx[0] = pl.erased[0];
 	p.erased_idx[1] = pl.erased[1];
 	const uint32_t G = pl.G, T = pl.T, RR = pl.region_rows, n_stages = pl.n_stages;
-	const size_t smem = pl.smem;
 	const uint32_t pbs = (nb + Ks - 1) / Ks, pbd = (nb + Kd - 1) / Kd;
 	const uint32_t R = G * Kd;
 	p.Kd = Kd; p.G = G; p.pbd = pbd; p.Ks = Ks; p.T = T; p.pbs = pbs; p.region_rows = RR;
@@ -1098,7 +791,7 @@ int lz_fused_convert(lzgpu_ctx *ctx, const lzgpu_goal *src, const lzgpu_goal *ds
 	p.crc_stride = crc_stride;
 	p.tables = ctx->d_crc_tables;
 	p.first_bad = d_first_bad;
-	std::memcpy(p.qmult, fs->qmult64, sizeof(p.qmult));
+	std::memcpy(p.qmult, fs->qmult, sizeof(p.qmult));
 	p.zconst = lz::crc_of_zeros(LZGPU_BLOCK_SIZE);
 	TmapArray maps;
 	uint32_t n_par_seen = 0;
@@ -1109,15 +802,8 @@ int lz_fused_convert(lzgpu_ctx *ctx, const lzgpu_goal *src, const lzgpu_goal *ds
 		p.part_id[slot] = static_cast<uint8_t>(idx);
 		p.stored[slot] = d_part_crc ? static_cast<const uint32_t *>(d_part_crc[idx]) : nullptr;
 		if (p.stored[slot]) verifying = true;
-		const cuuint64_t dims[3] = {static_cast<cuuint64_t>(kRowBytes), static_cast<cuuint64_t>(pbs) * 4, n_chunks};
-		const cuuint64_t strides[2] = {static_cast<cuuint64_t>(kRowBytes), part_stride};
-		const cuuint32_t box[3] = {kStepBytes, T * 4, 1};
-		const cuuint32_t estr[3] = {1, 1, 1};
 		if (reinterpret_cast<uintptr_t>(d_parts[idx]) % 16) return LZGPU_NOT_HANDLED;
-		CUresult r = fs->encode_tiled(&maps.m[a], CU_TENSOR_MAP_DATA_TYPE_UINT8, 3, const_cast<void *>(d_parts[idx]), dims, strides, box, estr,
-		                              CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, static_cast<CUtensorMapL2promotion>(fs->promo),
-		                              CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-		if (r != CUDA_SUCCESS) return LZGPU_NOT_HANDLED;
+		if (make_tensor_map(fs, &maps.m[a], d_parts[idx], static_cast<uint64_t>(pbs) * 4, n_chunks, part_stride, T * 4) != CUDA_SUCCESS) return LZGPU_NOT_HANDLED;
 	}
 	p.n_loaded = static_cast<uint32_t>(Ks);
 	for (uint32_t bl = 0; bl < R; ++bl) {
@@ -1126,24 +812,12 @@ int lz_fused_convert(lzgpu_ctx *ctx, const lzgpu_goal *src, const lzgpu_goal *ds
 	}
 	for (uint32_t x = 0; x < e; ++x) p.part_id[Ks + x] = static_cast<uint8_t>(Ks + x);
 	if (verifying && !d_first_bad) return LZGPU_NOT_HANDLED;
-	if (e == 2) {
-		uint8_t gx0 = 1, gx1 = 1;
-		for (int t = 0; t < p.erased_idx[0]; ++t) gx0 = lz::gf_mul_host(gx0, 2);
-		for (int t = 0; t < p.erased_idx[1]; ++t) gx1 = lz::gf_mul_host(gx1, 2);
-		coef_planes_set(p.w[0], gx0);
-		coef_planes_set(p.w[1], lz::gf_inv_host(gx0 ^ gx1));
-	}
+	if (e == 2) set_raid6_pair(p.w, p.erased_idx[0], p.erased_idx[1]);
 	p.dbl0 = (e == 2 && p.erased_idx[0] <= 4) ? p.erased_idx[0] : 0xffu;
 	const uint32_t rebuild_warps = kConvertThreads / 32 - pl.n_workers;   // (0 without lost parts: every warp is a worker)
-#define LZ_CONVERT_CASE(MM) \
-	case MM: \
-		return e == 0 ? launch_convert<MM, 0>(ctx, maps, p, smem, st, rebuild_warps) : e == 1 ? launch_convert<MM, 1>(ctx, maps, p, smem, st, rebuild_warps) \
-		              : launch_convert<MM, 2>(ctx, maps, p, smem, st, rebuild_warps);
-	switch (Md) {
-		LZ_CONVERT_CASE(1)
-		LZ_CONVERT_CASE(2)
-		LZ_CONVERT_CASE(3)
-	}
-#undef LZ_CONVERT_CASE
-	return LZGPU_NOT_HANDLED;
+	ConvertKernel fn = nullptr;   // the compile-time destination k where the list holds it, else the runtime-k kernel
+	for (const auto &k : kConverters)
+		if (k.m == Md && k.e == e && (k.kd == Kd || (k.kd == 0 && !fn))) fn = k.fn;
+	if (!fn) return LZGPU_NOT_HANDLED;
+	return launch(ctx, fn, launch_geo(LZGPU_KERNEL_CONVERT, kConvertThreads, G, n_stages, rebuild_warps, pl.smem), 2, p.total_units, st, maps, p);
 }

@@ -159,9 +159,8 @@ __device__ __forceinline__ void tma_load_3d(uint32_t smem_dst, const CUtensorMap
 }
 
 // ---- sparse-fold CRC stream ------------------------------------------------------------------------
-// Two sparse multiples of the CRC-32 polynomial P (found by meet-in-the-middle search, lowest weight for the window):
+// A sparse multiple of the CRC-32 polynomial P (found by meet-in-the-middle search, lowest weight for the window):
 //   FW = 64 : g(x) = x^53+x^38+x^36+x^33+x^30+x^27+x^25+x^7+x^3+1      9 pulls (5 LOP3) per word, 64-word window
-//   FW = 128: g(x) = x^123+x^120+x^80+x^74+x^53+x^45+1                 6 pulls (3 LOP3) per word, 128-word window
 // g(x^32) = g(x)^32 is a multiple of P too, so with y = one 32-bit word:  W'[u] = W[u] ^ XOR_lag W'[u - lag],
 // lag = deg - exponent.  The window lives in registers; slot of word u is u & (FW-1), all indices are static.
 template <int FW>
@@ -170,11 +169,6 @@ template <>
 struct FoldSpec<64> {
 	static constexpr int deg = 53, nlag = 9;
 	__host__ __device__ static constexpr int lag(int t) { return t == 0 ? 15 : t == 1 ? 17 : t == 2 ? 20 : t == 3 ? 23 : t == 4 ? 26 : t == 5 ? 28 : t == 6 ? 46 : t == 7 ? 50 : 53; }
-};
-template <>
-struct FoldSpec<128> {
-	static constexpr int deg = 123, nlag = 6;
-	__host__ __device__ static constexpr int lag(int t) { return t == 0 ? 3 : t == 1 ? 43 : t == 2 ? 49 : t == 3 ? 70 : t == 4 ? 78 : 123; }
 };
 
 __device__ __forceinline__ uint4 lds128(uint32_t addr) {

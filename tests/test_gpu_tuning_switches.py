@@ -185,7 +185,7 @@ ENCODE = [
     ("ec(11,3)", 60, 4, "chunk", dict(LZGPU_BS_STAGES=7), (BS, 512, 4, 7, 2, 174776)),  # runtime k, three rows
     ("ec(11,3)", 60, 4, "chunk", dict(LZGPU_BS_STAGES=16), (BS, 512, 4, 8, 2, 197320)),
     ("ec(5,3)", 61, 4, "chunk", dict(LZGPU_BS_STAGES=16, LZGPU_BITSLICE=7), (BS, 512, 8, 8, 4, 197320)),
-    # the folded instantiations (LZ_BS_FOLDED_LIST) with deeper rings
+    # the folded instantiations (the bit-sliced entries of kEncoders, csrc/fused.cu) with deeper rings
     ("ec(12,4)", 70, 4, "chunk", dict(LZGPU_BS_STAGES=16), (BS, 512, 5, 5, 3, 187032)),
     ("ec(10,4)", 71, 4, "chunk", dict(LZGPU_BS_STAGES=16), (BS, 512, 6, 5, 3, 191128)),
     ("ec(6,4)", 61, 4, "chunk", dict(LZGPU_BS_STAGES=16), (BS, 512, 8, 6, 4, 197288)),
