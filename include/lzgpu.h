@@ -188,6 +188,30 @@ int lzgpu_plan_check(const lzgpu_goal *goal, const uint8_t *given, lzgpu_check_p
  * are given, as the calls do. */
 int lzgpu_plan_check_degraded(const lzgpu_goal *goal, const uint8_t *given, lzgpu_check_plan *out);
 
+/* How lzgpu_encode_slices* will encode a batch for several slices at once (pure host logic, no GPU needed): one launch of
+ * fused_slices_kernel, or the per-slice route (lzgpu_encode_chunks' kernels once per xor/ec slice) for the reason in refusal.
+ * nb: blocks per chunk.  Returns LZGPU_ERR_ARG for the arguments the calls refuse.  A context with LZGPU_DISABLE_FUSED=1 always
+ * takes the per-slice route, and so does a call whose strides or alignment the kernel cannot address; neither is part of the plan. */
+enum {   /* lzgpu_slices_plan.refusal */
+	LZGPU_SLICES_FUSED = 0,                /* not refused: one pass */
+	LZGPU_SLICES_REFUSED_SINGLE = 1,       /* one xor/ec slice: the plain encoder, its data CRCs copied to a standard slice's array */
+	LZGPU_SLICES_REFUSED_CAUCHY = 2,       /* a slice with a Cauchy generator (m >= 5, or m = 4 with k > 20) */
+	LZGPU_SLICES_REFUSED_WIDE = 3,         /* the combined stripe L = lcm(k) is longer than 64 blocks */
+	LZGPU_SLICES_REFUSED_NO_GEOMETRY = 4   /* no unit of one or more combined stripes fits the CTA */
+};
+typedef struct lzgpu_slices_plan {
+	int fused;            /* 1: one fused_slices_kernel launch; 0: the per-slice route */
+	int refusal;          /* LZGPU_SLICES_FUSED / LZGPU_SLICES_REFUSED_* */
+	uint32_t L;           /* blocks per combined stripe: lcm of the xor/ec slices' k (also when refused) */
+	uint32_t G;           /* combined stripes per work unit (fused only, as every field below) */
+	uint32_t threads;     /* threads per CTA */
+	uint32_t stages;      /* depth of the data stage ring */
+	uint32_t crc_rows;    /* CRC streams per unit: 4 G L data rows + the staged parity rows 1 .. m-1 of every stripe of every slice */
+	uint32_t smem_bytes;  /* dynamic shared memory per CTA */
+	uint32_t units;       /* work units of the batch */
+} lzgpu_slices_plan;
+int lzgpu_plan_encode_slices(const lzgpu_goal *goals, uint32_t n_slices, uint32_t n_chunks, uint32_t nb, lzgpu_slices_plan *out);
+
 /* Diagnostics (pure host logic, no GPU needed): the host build of the bit-plane arithmetic the four-parity-row encoder runs per
  * item (csrc/bitslice.cuh).  data = k columns of 32 bytes (column j = 32 bytes of data part j, k <= 32); parity receives the
  * 4 x 32 bytes of the Vandermonde parity rows 0..3 (coefficient of column j in row r: (2^r)^j, galois_field_isal.cc:53-69). */
@@ -267,7 +291,8 @@ enum {
 	LZGPU_KERNEL_RECOVER_BS3 = 7,      /* bs_recover3_kernel: three lost data parts on bit planes */
 	LZGPU_KERNEL_CONVERT = 8,          /* fused_convert_kernel: one-pass slice conversion */
 	LZGPU_KERNEL_CHECK = 9,            /* fused_check_kernel: stripe check (lzgpu_check_stripes), one 16-warp CTA per SM */
-	LZGPU_KERNEL_CHECK_DEGRADED = 10   /* fused_check_degraded_kernel: stripe map with lost data parts (lzgpu_check_stripe_map_degraded) */
+	LZGPU_KERNEL_CHECK_DEGRADED = 10,  /* fused_check_degraded_kernel: stripe map with lost data parts (lzgpu_check_stripe_map_degraded) */
+	LZGPU_KERNEL_ENCODE_SLICES = 11    /* fused_slices_kernel: one-pass encode for several slices (lzgpu_encode_slices); G = combined stripes */
 };
 typedef struct lzgpu_launch_geometry {
 	int kernel;
@@ -334,6 +359,26 @@ int lzgpu_pool_encode_chunks(lzgpu_pool *pool, const lzgpu_goal *goal, uint32_t 
                              const uint8_t *data, size_t chunk_stride,
                              uint8_t *parity, size_t parity_stride,
                              uint32_t *crc, size_t crc_stride);
+
+/* Encode a batch for every slice of a goal in one pass over the data (a goal such as "std + xor2 + xor3", goal.h:67-91; the mount
+ * writes every slice of a chunk in one operation over combined stripes of lcm(k_i) blocks, chunk_writer.cc:150-156, 494-545).
+ *   goals[i]   (i < n_slices, 1 <= n_slices <= 4) xor/ec goals or the standard slice {LZGPU_KIND_STD, 1, 0}; at least one xor/ec.
+ *              Four is the size of the kernel parameter block's per-slice arrays.
+ *   xor/ec slice i: parity[i] and crc[i] receive byte for byte what lzgpu_encode_chunks(ctx, &goals[i], n_chunks, chunk_len, data,
+ *              chunk_stride, parity[i], parity_stride[i], crc[i], crc_stride[i]) writes (layout, zero-extended trailing block,
+ *              alignment, the CRC-disabled mode, and for the _dev form the zero-fill of the partial block in the caller's buffer).
+ *   standard slice i: parity[i] may be NULL; crc[i] (chunk c at + c * crc_stride[i]) receives the nb data-block CRCs.
+ * Any other argument returns LZGPU_ERR_ARG before anything is enqueued.  chunks_encoded counts each chunk once per call.  The route
+ * is lzgpu_plan_encode_slices; both routes write the same bytes.  lzgpu_pool_encode_slices cuts the batch as lzgpu_pool_encode_chunks. */
+int lzgpu_encode_slices(lzgpu_ctx *ctx, const lzgpu_goal *goals, uint32_t n_slices, uint32_t n_chunks, uint32_t chunk_len,
+                        const uint8_t *data, size_t chunk_stride,
+                        uint8_t *const *parity, const size_t *parity_stride, uint32_t *const *crc, const size_t *crc_stride);
+int lzgpu_encode_slices_dev(lzgpu_ctx *ctx, const lzgpu_goal *goals, uint32_t n_slices, uint32_t n_chunks, uint32_t chunk_len,
+                            const void *d_data, size_t chunk_stride,
+                            void *const *d_parity, const size_t *parity_stride, void *const *d_crc, const size_t *crc_stride, void *stream);
+int lzgpu_pool_encode_slices(lzgpu_pool *pool, const lzgpu_goal *goals, uint32_t n_slices, uint32_t n_chunks, uint32_t chunk_len,
+                             const uint8_t *data, size_t chunk_stride,
+                             uint8_t *const *parity, const size_t *parity_stride, uint32_t *const *crc, const size_t *crc_stride);
 
 /* Degraded read / rebuild of n_chunks chunks.
  *   parts[i]    (i < k+m) part-major buffer of part i for all chunks: chunk c at + c*part_stride,

@@ -39,6 +39,15 @@ class LzConvertPlan(C.Structure):
                 ("stages", C.c_uint32), ("worker_warps", C.c_uint32), ("rebuild_warps", C.c_uint32), ("smem_bytes", C.c_uint32)]
 
 
+class LzSlicesPlan(C.Structure):
+    _fields_ = [("fused", C.c_int), ("refusal", C.c_int), ("L", C.c_uint32), ("G", C.c_uint32), ("threads", C.c_uint32),
+                ("stages", C.c_uint32), ("crc_rows", C.c_uint32), ("smem_bytes", C.c_uint32), ("units", C.c_uint32)]
+
+
+# lzgpu_slices_plan.refusal
+SLICES_FUSED, SLICES_REFUSED_SINGLE, SLICES_REFUSED_CAUCHY, SLICES_REFUSED_WIDE, SLICES_REFUSED_NO_GEOMETRY = range(5)
+
+
 class LzRecoverSwitches(C.Structure):
     _fields_ = [("recover_geo", C.c_int), ("recover_two", C.c_int), ("recover_k3", C.c_int), ("bs_recover", C.c_int),
                 ("bs_recover_gf_warps", C.c_int), ("direct_wide", C.c_int)]
@@ -72,7 +81,7 @@ class LzLaunchGeometry(C.Structure):
 
 # lzgpu_launch_geometry.kernel
 KERNEL_NONE, KERNEL_ENCODE, KERNEL_ENCODE_BITSLICE, KERNEL_RECOVER_GEO0, KERNEL_RECOVER_GEO1, KERNEL_RECOVER_GEO2, \
-    KERNEL_RECOVER_DIRECT, KERNEL_RECOVER_BS3, KERNEL_CONVERT, KERNEL_CHECK, KERNEL_CHECK_DEGRADED = range(11)
+    KERNEL_RECOVER_DIRECT, KERNEL_RECOVER_BS3, KERNEL_CONVERT, KERNEL_CHECK, KERNEL_CHECK_DEGRADED, KERNEL_ENCODE_SLICES = range(12)
 
 
 class LzStripeVerdict(C.Structure):
@@ -119,6 +128,7 @@ SIGNATURES = {
     "lzgpu_plan_recover": (_int, [_goalp, _vp, _vp, _int, _int, C.POINTER(LzRecoverSwitches), C.POINTER(LzRecoverPlan)]),
     "lzgpu_plan_check": (_int, [_goalp, _vp, C.POINTER(LzCheckPlan)]),
     "lzgpu_plan_check_degraded": (_int, [_goalp, _vp, C.POINTER(LzCheckPlan)]),
+    "lzgpu_plan_encode_slices": (_int, [_goalp, _u32, _u32, _u32, C.POINTER(LzSlicesPlan)]),
     "lzgpu_debug_bitslice_rows": (_int, [_int, _vp, _vp]),
     "lzgpu_debug_bitslice_recover3": (_int, [_int, _vp, _vp, _int, _vp]),
     "lzgpu_debug_repair_rows": (_int, [_int, _int, _vp, _vp, _int, _vp]),
@@ -142,6 +152,8 @@ SIGNATURES = {
     "lzgpu_debug_status_slots": (_int, [_vp, C.POINTER(_u32), C.POINTER(_u32)]),
     "lzgpu_encode_chunks": (_int, [_vp, _goalp, _u32, _u32, _vp, _sz, _vp, _sz, _vp, _sz]),
     "lzgpu_encode_chunks_dev": (_int, [_vp, _goalp, _u32, _u32, _vp, _sz, _vp, _sz, _vp, _sz, _vp]),
+    "lzgpu_encode_slices": (_int, [_vp, _goalp, _u32, _u32, _u32, _vp, _sz, _vp, _vp, _vp, _vp]),
+    "lzgpu_encode_slices_dev": (_int, [_vp, _goalp, _u32, _u32, _u32, _vp, _sz, _vp, _vp, _vp, _vp, _vp]),
     "lzgpu_recover_chunks": (_int, [_vp, _goalp, _u32, _u32, _vp, _sz, _vp, _vp, _vp, _vp, _sz, _vp]),
     "lzgpu_recover_chunks_dev": (_int, [_vp, _goalp, _u32, _u32, _vp, _sz, _vp, _vp, _vp, _vp, _sz, _vp, _vp]),
     "lzgpu_check_stripes": (_int, [_vp, _goalp, _u32, _u32, _vp, _sz, _vp, _vp, _vp]),
@@ -220,6 +232,7 @@ SIGNATURES = {
     "lzgpu_pool_share": (None, [_u32, _int, _int, C.POINTER(_u32), C.POINTER(_u32)]),
     "lzgpu_pool_get_stats": (None, [_vp, C.POINTER(LzStats)]),
     "lzgpu_pool_encode_chunks": (_int, [_vp, _goalp, _u32, _u32, _vp, _sz, _vp, _sz, _vp, _sz]),
+    "lzgpu_pool_encode_slices": (_int, [_vp, _goalp, _u32, _u32, _u32, _vp, _sz, _vp, _vp, _vp, _vp]),
     "lzgpu_pool_recover_chunks": (_int, [_vp, _goalp, _u32, _u32, _vp, _sz, _vp, _vp, _vp, _vp, _sz, _vp]),
     "lzgpu_pool_convert_chunks": (_int, [_vp, _goalp, _goalp, _u32, _u32, _vp, _sz, _vp, _vp, _vp, _sz, _vp, _vp]),
     "lzgpu_pool_crc_blocks": (_int, [_vp, _vp, _sz, _u32, _sz, _vp]),

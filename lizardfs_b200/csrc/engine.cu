@@ -18,6 +18,7 @@
 #include "engine_internal.h"
 #include "host_math.h"
 #include "correct_kernel.cuh"
+#include "fused_plan.h"
 #include "kernels_generic.cuh"
 #include "lzgpu.h"
 
@@ -827,6 +828,163 @@ extern "C" int lzgpu_encode_chunks(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint3
 		CUDA_TRY(cudaMemcpy2DAsync(crc + c0 * crc_stride, crc_stride * 4, d_c[s], d_crc_stride * 4, n_crc * 4, n, cudaMemcpyDeviceToHost, st));
 		ctx->stats.bytes_h2d += static_cast<uint64_t>(n) * chunk_len;
 		ctx->stats.bytes_d2h += static_cast<uint64_t>(n) * (par_bytes + n_crc * 4);
+		return LZGPU_OK;
+	});
+}
+
+// ------------------------------------------------------------------------------------------------
+// batched encode for several slices in one pass
+// ------------------------------------------------------------------------------------------------
+// SURVEY.md §8(d) over every slice, the data read once: read S, write each xor/ec slice's m*pb*B parity, write every slice's CRC array
+static uint64_t slices_alg_bytes(const lzgpu_goal *goals, uint32_t n_slices, uint32_t n_chunks, uint32_t chunk_len) {
+	const uint64_t B = LZGPU_BLOCK_SIZE, nb = (chunk_len + B - 1) / B;
+	uint64_t per_chunk = chunk_len;
+	for (uint32_t i = 0; i < n_slices; ++i) {
+		const uint64_t m = goal_is_std(&goals[i]) ? 0 : goals[i].m, pb = (nb + goals[i].k - 1) / goals[i].k;
+		per_chunk += m * pb * B + 4 * (nb + m * pb);
+	}
+	return n_chunks * per_chunk;
+}
+
+// The arguments of lzgpu_encode_slices* (dev: the device form's strides and 16-byte alignment, as encode_enqueue checks them; else
+// the host form's, as lzgpu_encode_chunks checks them).  Checked before anything is enqueued.
+static int check_slices(const lzgpu_ctx *ctx, const lzgpu_goal *goals, uint32_t n_slices, uint32_t chunk_len, const void *data, size_t chunk_stride,
+                        const void *const *parity, const size_t *parity_stride, const void *const *crc, const size_t *crc_stride, bool dev) {
+	if (!ctx || !goals || !data || !parity || !parity_stride || !crc || !crc_stride) return LZGPU_ERR_ARG;
+	if (n_slices < 1 || n_slices > static_cast<uint32_t>(kSlicesMax)) { lz_set_error("encode_slices: n_slices must be 1..%d", kSlicesMax); return LZGPU_ERR_ARG; }
+	if (chunk_len == 0 || chunk_len > LZGPU_CHUNK_SIZE) { lz_set_error("chunk_len out of range"); return LZGPU_ERR_ARG; }
+	const uint32_t B = LZGPU_BLOCK_SIZE, nb = (chunk_len + B - 1) / B;
+	uint32_t n_striped = 0;
+	for (uint32_t i = 0; i < n_slices; ++i) {
+		const lzgpu_goal *g = &goals[i];
+		const bool std_slice = goal_is_std(g);
+		if (!std_slice && !lzgpu_goal_valid(g)) { lz_set_error("encode_slices: goal %u is neither an xor/ec goal nor the standard slice", i); return LZGPU_ERR_ARG; }
+		const size_t m = std_slice ? 0 : g->m, pb = (nb + g->k - 1) / g->k;
+		if (!crc[i] || (!std_slice && !parity[i])) { lz_set_error("encode_slices: slice %u has no output buffer", i); return LZGPU_ERR_ARG; }
+		if (crc_stride[i] < nb + m * pb || (!std_slice && parity_stride[i] < m * pb * B) ||
+		    (dev && !std_slice && ((parity_stride[i] & 15) || (reinterpret_cast<uintptr_t>(parity[i]) & 15)))) {
+			lz_set_error("encode_slices: strides of slice %u too small or its parity buffer not 16-byte aligned", i);
+			return LZGPU_ERR_ARG;
+		}
+		n_striped += std_slice ? 0 : 1;
+	}
+	if (n_striped == 0) { lz_set_error("encode_slices: no xor/ec slice"); return LZGPU_ERR_ARG; }
+	if (dev ? (chunk_stride < static_cast<size_t>(nb) * B || (chunk_stride & 15) || (reinterpret_cast<uintptr_t>(data) & 15)) : chunk_stride < chunk_len) {
+		lz_set_error("encode_slices: chunk stride too small or data not 16-byte aligned");
+		return LZGPU_ERR_ARG;
+	}
+	return LZGPU_OK;
+}
+
+// One pass (lz_fused_encode_slices), else encode_enqueue once per xor/ec slice with the standard slice's CRCs copied from the first
+// one's data CRCs (the same bytes).  Arguments checked by check_slices.
+static int slices_enqueue(lzgpu_ctx *ctx, const lzgpu_goal *goals, uint32_t n_slices, uint32_t n_chunks, uint32_t chunk_len, const void *d_data,
+                          size_t chunk_stride, void *const *d_parity, const size_t *parity_stride, void *const *d_crc, const size_t *crc_stride,
+                          cudaStream_t st) {
+	if (n_chunks == 0) return LZGPU_OK;
+	const uint32_t B = LZGPU_BLOCK_SIZE, nb = (chunk_len + B - 1) / B;
+	if (chunk_len % B) {
+		CUDA_TRY(cudaMemset2DAsync(const_cast<uint8_t *>(static_cast<const uint8_t *>(d_data)) + chunk_len, chunk_stride, 0,
+		                           static_cast<size_t>(nb) * B - chunk_len, n_chunks, st));
+	}
+	int rc = lz_fused_encode_slices(ctx, goals, n_slices, n_chunks, nb, d_data, chunk_stride, d_parity, parity_stride, d_crc, crc_stride, st);
+	if (rc == LZGPU_OK) {
+		ctx->stats.chunks_encoded += n_chunks;
+		if (!lzgpu_crc_enabled())
+			for (uint32_t i = 0; i < n_slices && !rc; ++i) {
+				const size_t m = goal_is_std(&goals[i]) ? 0 : goals[i].m, pb = (nb + goals[i].k - 1) / goals[i].k;
+				rc = fill_crc(ctx, d_crc[i], crc_stride[i], nb + m * pb, n_chunks, st);
+			}
+		return rc;
+	}
+	if (rc != LZGPU_NOT_HANDLED) return rc;
+	int first = -1;
+	uint64_t passes = 0;
+	for (uint32_t i = 0; i < n_slices; ++i) {
+		if (goal_is_std(&goals[i])) continue;
+		if ((rc = encode_enqueue(ctx, &goals[i], n_chunks, chunk_len, d_data, chunk_stride, d_parity[i], parity_stride[i], d_crc[i], crc_stride[i], st)))
+			return rc;
+		if (first < 0) first = static_cast<int>(i);
+		++passes;
+	}
+	ctx->stats.chunks_encoded -= (passes - 1) * n_chunks;   // one count per chunk and call
+	for (uint32_t i = 0; i < n_slices; ++i)
+		if (goal_is_std(&goals[i]))
+			CUDA_TRY(cudaMemcpy2DAsync(d_crc[i], crc_stride[i] * 4, d_crc[first], crc_stride[first] * 4, static_cast<size_t>(nb) * 4, n_chunks,
+			                           cudaMemcpyDeviceToDevice, st));
+	return LZGPU_OK;
+}
+
+extern "C" int lzgpu_encode_slices_dev(lzgpu_ctx *ctx, const lzgpu_goal *goals, uint32_t n_slices, uint32_t n_chunks, uint32_t chunk_len,
+                                        const void *d_data, size_t chunk_stride, void *const *d_parity, const size_t *parity_stride,
+                                        void *const *d_crc, const size_t *crc_stride, void *stream) {
+	NvtxScope nvtx_scope("lzgpu::encode_slices_dev");
+	int rc = check_slices(ctx, goals, n_slices, chunk_len, d_data, chunk_stride, d_parity, parity_stride, d_crc, crc_stride, true);
+	if (rc) return rc;
+	if (n_chunks == 0) return LZGPU_OK;
+	DeviceGuard g(ctx->device);
+	cudaStream_t st = stream ? static_cast<cudaStream_t>(stream) : ctx->stream;
+	BatchTimer timer(ctx, st, slices_alg_bytes(goals, n_slices, n_chunks, chunk_len));
+	return slices_enqueue(ctx, goals, n_slices, n_chunks, chunk_len, d_data, chunk_stride, d_parity, parity_stride, d_crc, crc_stride, st);
+}
+
+extern "C" int lzgpu_encode_slices(lzgpu_ctx *ctx, const lzgpu_goal *goals, uint32_t n_slices, uint32_t n_chunks, uint32_t chunk_len,
+                                    const uint8_t *data, size_t chunk_stride, uint8_t *const *parity, const size_t *parity_stride,
+                                    uint32_t *const *crc, const size_t *crc_stride) {
+	NvtxScope nvtx_scope("lzgpu::encode_slices");
+	int rc = check_slices(ctx, goals, n_slices, chunk_len, data, chunk_stride, reinterpret_cast<const void *const *>(parity), parity_stride,
+	                      reinterpret_cast<const void *const *>(crc), crc_stride, false);
+	if (rc) return rc;
+	if (n_chunks == 0) return LZGPU_OK;
+	const uint32_t B = LZGPU_BLOCK_SIZE, nb = (chunk_len + B - 1) / B;
+	// device layout of a tile: the data dense; slice i's parity and CRCs dense too, at par_off[i] / crc_off[i] per chunk of the tile
+	size_t par_bytes[kSlicesMax] = {0}, n_crc[kSlicesMax] = {0}, d_crc_stride[kSlicesMax] = {0}, par_off[kSlicesMax] = {0}, crc_off[kSlicesMax] = {0};
+	size_t par_total = 0, crc_total = 0;
+	for (uint32_t i = 0; i < n_slices; ++i) {
+		const size_t m = goal_is_std(&goals[i]) ? 0 : goals[i].m, pb = (nb + goals[i].k - 1) / goals[i].k;
+		par_bytes[i] = m * pb * B;
+		n_crc[i] = nb + m * pb;
+		d_crc_stride[i] = (n_crc[i] + 3) & ~size_t(3);
+		par_off[i] = par_total;
+		crc_off[i] = crc_total;
+		par_total += par_bytes[i];
+		crc_total += d_crc_stride[i];
+	}
+	std::lock_guard<std::mutex> lk(ctx->mu);
+	DeviceGuard g(ctx->device);
+	AutoPin pin(ctx);
+	pin.add(data, static_cast<size_t>(n_chunks - 1) * chunk_stride + chunk_len);
+	for (uint32_t i = 0; i < n_slices; ++i) {
+		if (par_bytes[i]) pin.add(parity[i], static_cast<size_t>(n_chunks - 1) * parity_stride[i] + par_bytes[i]);
+		pin.add(crc[i], (static_cast<size_t>(n_chunks - 1) * crc_stride[i] + n_crc[i]) * 4);
+	}
+	const size_t d_chunk_stride = static_cast<size_t>(nb) * B;
+	const uint32_t tile = std::max<uint32_t>(1, std::min<uint32_t>(n_chunks, kHostTileBytes / LZGPU_CHUNK_SIZE));
+	void *d_in[kHostSlots], *d_par[kHostSlots], *d_c[kHostSlots];
+	for (int s = 0; s < kHostSlots; ++s) {
+		if ((rc = lz_scratch(ctx, kScratchIn0 + s, tile * d_chunk_stride, &d_in[s]))) return rc;
+		if ((rc = lz_scratch(ctx, kScratchPar0 + s, tile * par_total, &d_par[s]))) return rc;
+		if ((rc = lz_scratch(ctx, kScratchCrc0 + s, tile * crc_total * 4, &d_c[s]))) return rc;
+	}
+	return run_tiles(ctx, n_chunks, tile, kHostSlots, nullptr, [&](int s, size_t c0, size_t n, cudaStream_t st, VerifyTicket *) -> int {
+		void *dp[kSlicesMax], *dc[kSlicesMax];
+		for (uint32_t i = 0; i < n_slices; ++i) {
+			dp[i] = static_cast<uint8_t *>(d_par[s]) + tile * par_off[i];
+			dc[i] = static_cast<uint32_t *>(d_c[s]) + tile * crc_off[i];
+		}
+		CUDA_TRY(cudaMemcpy2DAsync(d_in[s], d_chunk_stride, data + c0 * chunk_stride, chunk_stride, chunk_len, n, cudaMemcpyHostToDevice, st));
+		int rc = lzgpu_encode_slices_dev(ctx, goals, n_slices, static_cast<uint32_t>(n), chunk_len, d_in[s], d_chunk_stride, dp, par_bytes, dc,
+		                                 d_crc_stride, st);
+		if (rc) return rc;
+		uint64_t d2h = 0;
+		for (uint32_t i = 0; i < n_slices; ++i) {
+			if (par_bytes[i])
+				CUDA_TRY(cudaMemcpy2DAsync(parity[i] + c0 * parity_stride[i], parity_stride[i], dp[i], par_bytes[i], par_bytes[i], n, cudaMemcpyDeviceToHost, st));
+			CUDA_TRY(cudaMemcpy2DAsync(crc[i] + c0 * crc_stride[i], crc_stride[i] * 4, dc[i], d_crc_stride[i] * 4, n_crc[i] * 4, n, cudaMemcpyDeviceToHost, st));
+			d2h += par_bytes[i] + n_crc[i] * 4;
+		}
+		ctx->stats.bytes_h2d += static_cast<uint64_t>(n) * chunk_len;
+		ctx->stats.bytes_d2h += static_cast<uint64_t>(n) * d2h;
 		return LZGPU_OK;
 	});
 }

@@ -201,6 +201,11 @@ int lz_fused_convert(lzgpu_ctx *ctx, const lzgpu_goal *src, const lzgpu_goal *ds
 int lz_fused_check(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, uint32_t nb, const void *const *d_parts, size_t part_stride,
                    const void *const *d_part_crc, void *d_verdict, cudaStream_t st, unsigned long long *d_first_bad, bool map,
                    const uint8_t *elim, unsigned long long *d_failed = nullptr);
+// One-pass encode for several slices (slices_kernel.cuh): parity of xor/ec slice i to d_parity[i], CRC arrays as lz_fused_encode
+// writes them (the standard slice: nb data CRCs) to d_crc[i].  LZGPU_NOT_HANDLED = take the per-slice route.
+int lz_fused_encode_slices(lzgpu_ctx *ctx, const lzgpu_goal *goals, uint32_t n_slices, uint32_t n_chunks, uint32_t nb, const void *d_data,
+                           size_t chunk_stride, void *const *d_parity, const size_t *parity_stride, void *const *d_crc, const size_t *crc_stride,
+                           cudaStream_t st);
 // CRC of 64 KiB blocks: block (c, b) at base + c*chunk_stride + b*65536, out[c*out_chunk_stride + b]
 int lz_fused_crc(lzgpu_ctx *ctx, const void *base, unsigned long long n_blocks, unsigned long long blocks_per_chunk,
                  unsigned long long chunk_stride, void *out, unsigned long long out_chunk_stride, cudaStream_t st);

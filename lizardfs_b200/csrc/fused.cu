@@ -16,6 +16,7 @@
 #include "convert_kernel.cuh"
 #include "bs_recover_kernel.cuh"
 #include "check_kernel.cuh"
+#include "slices_kernel.cuh"
 #include "host_math.h"
 
 using namespace lzd;
@@ -298,6 +299,13 @@ static const struct {
 	{2, 0, 3, fused_convert_kernel<2, 0, 3>}, {2, 1, 3, fused_convert_kernel<2, 1, 3>}, {2, 2, 3, fused_convert_kernel<2, 2, 3>},
 };
 
+// One-pass encode for several slices (fused_slices_kernel), keyed by the largest m of the slices
+using SlicesKernel = void (*)(CUtensorMap, SlicesParams);
+static const struct {
+	uint32_t m;
+	SlicesKernel fn;
+} kSlicers[] = {{1, fused_slices_kernel<1>}, {2, fused_slices_kernel<2>}, {3, fused_slices_kernel<3>}, {4, fused_slices_kernel<4>}};
+
 // function attributes are per device: set once per context
 static int set_all_smem_attrs(const FusedState *fs) {
 	int rc;
@@ -316,6 +324,8 @@ static int set_all_smem_attrs(const FusedState *fs) {
 		if ((rc = set_smem(k.map, kRecoverSmemCapBig)) || (rc = set_smem(k.repair, kRecoverSmemCapBig))) return rc;
 	for (const auto &k : kConverters)
 		if ((rc = set_smem(k.fn, kSmemCap))) return rc;
+	for (const auto &k : kSlicers)
+		if ((rc = set_smem(k.fn, kSlicesSmemCap))) return rc;
 	return LZGPU_OK;
 }
 
@@ -820,4 +830,70 @@ int lz_fused_convert(lzgpu_ctx *ctx, const lzgpu_goal *src, const lzgpu_goal *ds
 		if (k.m == Md && k.e == e && (k.kd == Kd || (k.kd == 0 && !fn))) fn = k.fn;
 	if (!fn) return LZGPU_NOT_HANDLED;
 	return launch(ctx, fn, launch_geo(LZGPU_KERNEL_CONVERT, kConvertThreads, G, n_stages, rebuild_warps, pl.smem), 2, p.total_units, st, maps, p);
+}
+
+// ---------------------------------------------------------------------------------------------------
+// one-pass encode for several slices (slices_kernel.cuh)
+// ---------------------------------------------------------------------------------------------------
+
+// Every slice of `goals` (xor/ec goals and at most the standard slice; the caller has checked the arguments) in one pass over the
+// data: parity of slice i to d_parity[i], CRC arrays as lz_fused_encode writes them (standard slice: the nb data CRCs) to d_crc[i].
+// LZGPU_NOT_HANDLED = the plan refuses the set, or the strides / alignment are not the kernel's: take the per-slice route.
+int lz_fused_encode_slices(lzgpu_ctx *ctx, const lzgpu_goal *goals, uint32_t n_slices, uint32_t n_chunks, uint32_t nb, const void *d_data,
+                           size_t chunk_stride, void *const *d_parity, const size_t *parity_stride, void *const *d_crc, const size_t *crc_stride,
+                           cudaStream_t st) {
+	FusedState *fs = ctx->fused;
+	if (!fs || fs->disabled || n_chunks == 0 || nb == 0) return LZGPU_NOT_HANDLED;
+	if ((chunk_stride % 16) || (reinterpret_cast<uintptr_t>(d_data) % 16)) return LZGPU_NOT_HANDLED;
+	bool cauchy[kSlicesMax] = {false};
+	for (uint32_t i = 0; i < n_slices; ++i) {
+		if (slice_is_std(goals[i])) continue;
+		cauchy[i] = lz::uses_cauchy(goals[i].k, goals[i].m);
+		if ((parity_stride[i] % 16) || (reinterpret_cast<uintptr_t>(d_parity[i]) % 16)) return LZGPU_NOT_HANDLED;
+	}
+	const SlicesPlan pl = slices_plan(goals, cauchy, n_slices, n_chunks, nb);
+	const lzgpu_slices_plan &o = pl.out;
+	if (!o.fused) return LZGPU_NOT_HANDLED;
+	SlicesParams p{};
+	uint32_t gs = 0, prow4 = 0;
+	for (uint32_t i = 0; i < n_slices; ++i) {
+		const bool std_slice = slice_is_std(goals[i]);
+		p.parity[i] = std_slice ? nullptr : static_cast<uint8_t *>(d_parity[i]);
+		p.crc[i] = static_cast<uint32_t *>(d_crc[i]);
+		p.parity_stride[i] = std_slice ? 0 : parity_stride[i];
+		p.crc_stride[i] = crc_stride[i];
+		p.k[i] = static_cast<uint32_t>(goals[i].k);
+		p.m[i] = std_slice ? 0 : static_cast<uint32_t>(goals[i].m);
+		p.pb[i] = std_slice ? 0 : (nb + p.k[i] - 1) / p.k[i];
+		p.S[i] = pl.S[i];
+		p.prow4[i] = prow4;
+		if (p.m[i] > 1) prow4 += p.S[i] * (p.m[i] - 1);
+		for (uint32_t s = 0; s < p.S[i]; ++s, ++gs) {
+			p.gs_slice[gs] = static_cast<uint8_t>(i);
+			p.gs_stripe[gs] = static_cast<uint8_t>(s);
+		}
+	}
+	p.tables = ctx->d_crc_tables;
+	p.n_slices = n_slices;
+	p.n_stripes = gs;
+	p.n_chunks = n_chunks;
+	p.nb = nb;
+	p.R = pl.R;
+	p.prows = pl.prows;
+	p.units_per_chunk = (nb + pl.R - 1) / pl.R;
+	p.total_units = o.units;
+	p.n_stages = o.stages;
+	std::memcpy(p.qmult, fs->qmult, sizeof(p.qmult));
+	p.zconst = lz::crc_of_zeros(LZGPU_BLOCK_SIZE);
+	CUtensorMap map;
+	const CUresult r = make_tensor_map(fs, &map, d_data, static_cast<uint64_t>(nb) * 4, n_chunks, chunk_stride, 4 * pl.R);
+	if (r != CUDA_SUCCESS) {
+		lz_set_error("cuTensorMapEncodeTiled failed with CUresult %d (rows/chunk %u, chunks %u, stride %zu, box rows %u)", static_cast<int>(r), nb * 4,
+		             n_chunks, chunk_stride, 4 * pl.R);
+		return LZGPU_ERR_CUDA;
+	}
+	for (const auto &k : kSlicers)
+		if (k.m == pl.m)
+			return launch(ctx, k.fn, launch_geo(LZGPU_KERNEL_ENCODE_SLICES, o.threads, o.G, o.stages, 0, o.smem_bytes), 1, p.total_units, st, map, p);
+	return LZGPU_NOT_HANDLED;   // (cannot happen: the plan refuses m > 4, which only Cauchy goals have)
 }

@@ -1,7 +1,8 @@
 // fused_plan.h — geometry of the fused encode kernel as pure functions (no CUDA calls): which unit mode a batch gets, how many
 // stripes a unit holds, how many units there are; the same for the one-pass slice conversion (convert_plan), the router of the
-// degraded read (recover_plan) and the stripe check (check_plan).  Shared by the launchers (fused.cu) and the diagnostics entry
-// points lzgpu_plan_encode, lzgpu_plan_convert, lzgpu_plan_recover and lzgpu_plan_check (host_math.cc), so the decisions are
+// degraded read (recover_plan), the stripe check (check_plan) and the one-pass multi-slice encode (slices_plan).  Shared by the
+// launchers (fused.cu) and the diagnostics entry points lzgpu_plan_encode, lzgpu_plan_convert, lzgpu_plan_recover, lzgpu_plan_check
+// and lzgpu_plan_encode_slices (host_math.cc), so the decisions are
 // unit-tested on a machine without a GPU (tests/test_host_math.py, tests/test_gpu_convert_geometry.py,
 // tests/test_gpu_recover_geometry.py, tests/test_gpu_check_geometry.py).
 #pragma once
@@ -262,6 +263,89 @@ inline ConvertPlan convert_plan(int Ks, int Ms, bool src_cauchy, int Kd, int Md,
 			pl.smem = ns * stage + 24 * ns + fixed;
 		}
 	}
+	return pl;
+}
+
+// ---------------------------------------------------------------------------------------------------
+// One-pass encode of every slice of a goal (slices_kernel.cuh): geometry as a pure function, shared by lz_fused_encode_slices and
+// lzgpu_plan_encode_slices.  A unit is G combined stripes of one chunk, R = G*L consecutive chunk blocks (L = lcm of the striped
+// slices' k), one TMA box of 4R quarter-rows per step (4R <= 256).  One 16-warp CTA per SM: thread t < 4R owns data row t, the
+// next rows are the staged parity rows 1 .. m_i - 1 of every stripe of every slice; every thread takes GF items.
+// G: the largest whose CRC rows fit the CTA and whose stages fit the shared memory, capped by ceil(nb / L) so that a batch of
+// short chunks gets no units it cannot fill; then as many stages as fit, at most four.
+// ---------------------------------------------------------------------------------------------------
+constexpr int kSlicesThreads = 512;
+constexpr int kSlicesNPST = 4;                 // parity staging ring
+constexpr int kSlicesMaxStages = 4;
+constexpr int kSlicesSmemCap = 200 * 1024;
+constexpr int kSlicesMax = 4;                  // slices per call: the size of the parameter block's per-slice arrays
+constexpr int kSlicesMaxStripes = 128;         // stripes of all slices per unit: at most 4 x 64 / 2
+LZ_HD constexpr int slices_item_words(int m) { return m >= 3 ? 2 : 4; }   // 8-byte items for three or four rows (16 accumulators next to the CRC window spill)
+
+inline size_t slices_smem_bytes(uint32_t R, uint32_t prows, uint32_t nst) {
+	const size_t stage = (static_cast<size_t>(R) * 4 * kStepBytes + 1023) & ~size_t(1023);
+	const size_t pstage = (static_cast<size_t>(prows) * kStepBytes + 1023) & ~size_t(1023);
+	return nst * stage + kSlicesNPST * pstage + 520 + 8 * (2 * nst + 2 * kSlicesNPST);
+}
+
+inline bool slice_is_std(const lzgpu_goal &g) { return g.kind == LZGPU_KIND_STD && g.k == 1 && g.m == 0; }
+
+struct SlicesPlan {
+	lzgpu_slices_plan out{};
+	uint32_t m = 0;                 // the instantiation: the largest m of the striped slices
+	uint32_t R = 0, prows = 0;      // chunk blocks per unit, staged parity rows
+	uint32_t S[kSlicesMax] = {0};   // stripes of slice i per unit (0: standard slice)
+};
+
+// goals: valid xor/ec goals or the standard slice, at least one striped (the caller checks); cauchy[i]: slice i has a Cauchy generator
+inline SlicesPlan slices_plan(const lzgpu_goal *goals, const bool *cauchy, uint32_t n_slices, uint32_t n_chunks, uint32_t nb) {
+	SlicesPlan pl;
+	lzgpu_slices_plan &o = pl.out;
+	uint32_t n_striped = 0, L = 1;
+	bool any_cauchy = false;
+	for (uint32_t i = 0; i < n_slices; ++i) {
+		if (slice_is_std(goals[i])) continue;
+		++n_striped;
+		any_cauchy |= cauchy[i];
+		const uint32_t k = static_cast<uint32_t>(goals[i].k);
+		uint32_t a = L, b = k;
+		while (b) { const uint32_t t = a % b; a = b; b = t; }
+		L = L / a * k;                     // k <= 32 and at most four slices: no overflow
+		pl.m = pl.m > static_cast<uint32_t>(goals[i].m) ? pl.m : static_cast<uint32_t>(goals[i].m);
+	}
+	o.L = L;
+	if (n_striped < 2) { o.refusal = LZGPU_SLICES_REFUSED_SINGLE; return pl; }
+	if (any_cauchy) { o.refusal = LZGPU_SLICES_REFUSED_CAUCHY; return pl; }
+	if (L > 64) { o.refusal = LZGPU_SLICES_REFUSED_WIDE; return pl; }
+	auto prows_of = [&](uint32_t R) {
+		uint32_t rows = 0;
+		for (uint32_t i = 0; i < n_slices; ++i)
+			if (!slice_is_std(goals[i])) rows += R / static_cast<uint32_t>(goals[i].k) * static_cast<uint32_t>(goals[i].m - 1) * 4;
+		return rows;
+	};
+	uint32_t G = 0;
+	for (uint32_t g = 1; g * L <= 64; ++g) {
+		const uint32_t R = g * L, prows = prows_of(R);
+		if (4 * R + prows > static_cast<uint32_t>(kSlicesThreads) || slices_smem_bytes(R, prows, 2) > static_cast<size_t>(kSlicesSmemCap)) break;
+		G = g;
+	}
+	if (G == 0) { o.refusal = LZGPU_SLICES_REFUSED_NO_GEOMETRY; return pl; }
+	const uint32_t per_chunk = (nb + L - 1) / L;
+	if (G > per_chunk) G = per_chunk;
+	pl.R = G * L;
+	pl.prows = prows_of(pl.R);
+	uint32_t nst = 2;
+	while (nst < static_cast<uint32_t>(kSlicesMaxStages) && slices_smem_bytes(pl.R, pl.prows, nst + 1) <= static_cast<size_t>(kSlicesSmemCap)) ++nst;
+	const uint64_t units = static_cast<uint64_t>((nb + pl.R - 1) / pl.R) * n_chunks;
+	if (units > 0x7fffffffull) { o.refusal = LZGPU_SLICES_REFUSED_NO_GEOMETRY; return pl; }
+	for (uint32_t i = 0; i < n_slices; ++i) pl.S[i] = slice_is_std(goals[i]) ? 0 : pl.R / static_cast<uint32_t>(goals[i].k);
+	o.fused = 1;
+	o.G = G;
+	o.threads = kSlicesThreads;
+	o.stages = nst;
+	o.crc_rows = 4 * pl.R + pl.prows;
+	o.smem_bytes = static_cast<uint32_t>(slices_smem_bytes(pl.R, pl.prows, nst));
+	o.units = static_cast<uint32_t>(units);
 	return pl;
 }
 

@@ -590,6 +590,22 @@ int lzgpu_plan_check_degraded(const lzgpu_goal *goal, const uint8_t *given, lzgp
 	return LZGPU_OK;
 }
 
+int lzgpu_plan_encode_slices(const lzgpu_goal *goals, uint32_t n_slices, uint32_t n_chunks, uint32_t nb, lzgpu_slices_plan *out) {
+	if (!out || !goals || n_slices < 1 || n_slices > static_cast<uint32_t>(lzd::kSlicesMax) || nb == 0 || nb > LZGPU_BLOCKS_IN_CHUNK)
+		return LZGPU_ERR_ARG;
+	*out = lzgpu_slices_plan{};
+	bool cauchy[lzd::kSlicesMax] = {false}, any_striped = false;
+	for (uint32_t i = 0; i < n_slices; ++i) {
+		if (lzd::slice_is_std(goals[i])) continue;
+		if (!lzgpu_goal_valid(&goals[i])) return LZGPU_ERR_ARG;
+		cauchy[i] = lz::uses_cauchy(goals[i].k, goals[i].m);
+		any_striped = true;
+	}
+	if (!any_striped) return LZGPU_ERR_ARG;
+	*out = lzd::slices_plan(goals, cauchy, n_slices, n_chunks, nb).out;
+	return LZGPU_OK;
+}
+
 const char *lzgpu_version(void) { return "lizardfs_b200 0.1 (sm_90a)"; }
 
 }  // extern "C"

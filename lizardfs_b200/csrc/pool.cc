@@ -187,6 +187,24 @@ extern "C" int lzgpu_pool_encode_chunks(lzgpu_pool *pool, const lzgpu_goal *goal
 	}, &errs);
 }
 
+extern "C" int lzgpu_pool_encode_slices(lzgpu_pool *pool, const lzgpu_goal *goals, uint32_t n_slices, uint32_t n_chunks, uint32_t chunk_len,
+                                         const uint8_t *data, size_t chunk_stride, uint8_t *const *parity, const size_t *parity_stride,
+                                         uint32_t *const *crc, const size_t *crc_stride) {
+	if (!pool || !goals || !data || !parity || !parity_stride || !crc || !crc_stride || n_slices < 1 || n_slices > 4) return LZGPU_ERR_ARG;
+	if (n_chunks == 0) return LZGPU_OK;
+	std::vector<std::string> errs;
+	return pool_run(pool, n_chunks, [&](int i, uint32_t first, uint32_t count) {
+		uint8_t *p[4] = {nullptr, nullptr, nullptr, nullptr};
+		uint32_t *c[4] = {nullptr, nullptr, nullptr, nullptr};
+		for (uint32_t s = 0; s < n_slices; ++s) {
+			if (parity[s]) p[s] = parity[s] + static_cast<size_t>(first) * parity_stride[s];
+			if (crc[s]) c[s] = crc[s] + static_cast<size_t>(first) * crc_stride[s];
+		}
+		return lzgpu_encode_slices(pool->workers[i]->ctx, goals, n_slices, count, chunk_len, data + static_cast<size_t>(first) * chunk_stride, chunk_stride,
+		                           p, parity_stride, c, crc_stride);
+	}, &errs);
+}
+
 extern "C" int lzgpu_pool_recover_chunks(lzgpu_pool *pool, const lzgpu_goal *goal, uint32_t n_chunks, uint32_t nb, const uint8_t *const *parts,
                                           size_t part_stride, const uint32_t *const *part_crc, const uint8_t *want, uint8_t *const *out,
                                           uint8_t *chunk_out, size_t chunk_out_stride, int64_t *bad) {

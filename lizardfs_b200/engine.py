@@ -119,6 +119,35 @@ def _encode_chunks(fn, h, goal, data, chunk_len, parity=None, crc=None):
     return parity, crc
 
 
+def _goal_array(goals):
+    arr = (LzGoal * len(goals))()
+    for i, g in enumerate(goals):
+        arr[i] = g.c
+    return arr
+
+
+def _encode_slices(fn, h, goals, data, chunk_len):
+    """one (parity or None, crc) per slice: parity [n, m, pb * 64 KiB] and crc [n, nb + m * pb] as _encode_chunks returns them for
+    an xor/ec slice, parity None and crc [n, nb] for the standard slice"""
+    data = _u8(data)
+    if data.ndim == 1:
+        data = data.reshape(1, -1)
+    n, stride = data.shape
+    if chunk_len is None:
+        chunk_len = stride
+    out = []
+    for g in goals:
+        nb, pb = Engine.geometry(g, chunk_len)
+        m = 0 if g.is_std else g.m
+        out.append((None if g.is_std else np.empty((n, m, pb * BLOCK_SIZE), dtype=np.uint8), np.empty((n, nb + m * pb), dtype=np.uint32)))
+    ns = len(goals)
+    par_stride = (C.c_size_t * ns)(*[0 if p is None else p.shape[1] * p.shape[2] for p, _ in out])
+    crc_stride = (C.c_size_t * ns)(*[c.shape[1] for _, c in out])
+    _check(fn(h, _goal_array(goals), ns, n, chunk_len, _p(data), stride, _ptr_array([p for p, _ in out]), par_stride,
+              _ptr_array([c for _, c in out]), crc_stride), _name(fn))
+    return out
+
+
 def _recover_chunks(fn, h, goal, nb, parts, part_crc, want, chunk_image):
     n_parts = goal.k + goal.m
     assert len(parts) == n_parts
@@ -341,6 +370,10 @@ class Pool:
     def encode_chunks(self, goal, data, chunk_len=None, parity=None, crc=None):
         return _encode_chunks(self.lib.lzgpu_pool_encode_chunks, self.h, goal, data, chunk_len, parity, crc)
 
+    def encode_slices(self, goals, data, chunk_len=None):
+        """Engine.encode_slices over every device of the pool (lzgpu_pool_encode_slices)"""
+        return _encode_slices(self.lib.lzgpu_pool_encode_slices, self.h, goals, data, chunk_len)
+
     def recover_chunks(self, goal, nb, parts, part_crc=None, want=None, chunk_image=False):
         return _recover_chunks(self.lib.lzgpu_pool_recover_chunks, self.h, goal, nb, parts, part_crc, want, chunk_image)
 
@@ -482,6 +515,28 @@ class Engine:
     def encode_chunks(self, goal, data, chunk_len=None):
         """data: uint8 array [n_chunks, stride] (chunk order). Returns (parity [n, m, pb*64K], crc [n, nb+m*pb])."""
         return _encode_chunks(self.lib.lzgpu_encode_chunks, self.h, goal, data, chunk_len)
+
+    def encode_slices(self, goals, data, chunk_len=None):
+        """Encode the batch for every slice of a goal in one pass (lzgpu_encode_slices): goals = up to four SliceTypes, the standard
+        slice among them at most once in practice.  Returns one (parity, crc) per slice, each as encode_chunks returns it for an xor/ec
+        slice; (None, the nb data-block CRCs per chunk) for the standard slice."""
+        return _encode_slices(self.lib.lzgpu_encode_slices, self.h, goals, data, chunk_len)
+
+    def encode_slices_dev(self, goals, n_chunks, chunk_len, d_data, chunk_stride, d_parity, parity_stride, d_crc, crc_stride, stream=None):
+        """lzgpu_encode_slices_dev: d_parity / d_crc / parity_stride / crc_stride are lists, one entry per slice (device pointers as
+        ints; 0 or None for the standard slice's parity)"""
+        ns = len(goals)
+        _check(self.lib.lzgpu_encode_slices_dev(self.h, _goal_array(goals), ns, n_chunks, chunk_len, d_data, chunk_stride, _dev_ptrs(d_parity, ns),
+                                                (C.c_size_t * ns)(*parity_stride), _dev_ptrs(d_crc, ns), (C.c_size_t * ns)(*crc_stride), stream),
+               "encode_slices_dev")
+
+    @staticmethod
+    def plan_encode_slices(goals, n_chunks, nb):
+        """how encode_slices would run the batch (pure host logic, csrc/fused_plan.h slices_plan; no GPU needed): dict with fused,
+        refusal (SLICES_* in _lib), L, G, threads, stages, crc_rows, smem_bytes, units"""
+        out = _lib.LzSlicesPlan()
+        _check(_lib.load().lzgpu_plan_encode_slices(_goal_array(goals), len(goals), n_chunks, nb, C.byref(out)), "plan_encode_slices")
+        return {f: getattr(out, f) for f, _ in _lib.LzSlicesPlan._fields_}
 
     def encode_chunks_dev(self, goal, n_chunks, chunk_len, d_data, chunk_stride, d_parity, parity_stride, d_crc, crc_stride, stream=None):
         _check(self.lib.lzgpu_encode_chunks_dev(self.h, C.byref(goal.c), n_chunks, chunk_len, d_data, chunk_stride, d_parity,
