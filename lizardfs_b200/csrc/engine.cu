@@ -672,12 +672,10 @@ static int check_goal(const lzgpu_goal *g) {
 	return LZGPU_OK;
 }
 
-static bool goal_is_std(const lzgpu_goal *g) { return g && g->kind == LZGPU_KIND_STD && g->k == 1 && g->m == 0; }
-
 // the context, goal and nb of a batched call (std_ok: the standard slice is a goal too, as in a conversion)
 static int check_batch(const lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t nb, bool std_ok = false) {
 	if (!ctx) return LZGPU_ERR_ARG;
-	int rc = std_ok && goal_is_std(goal) ? LZGPU_OK : check_goal(goal);
+	int rc = std_ok && slice_is_std(*goal) ? LZGPU_OK : check_goal(goal);
 	if (rc) return rc;
 	if (nb == 0 || nb > LZGPU_BLOCKS_IN_CHUNK) { lz_set_error("nb out of range"); return LZGPU_ERR_ARG; }
 	return LZGPU_OK;
@@ -704,212 +702,123 @@ static void goal_parity_rows(const lzgpu_goal *g, uint8_t *rows /* m*k */) {
 }
 
 // ------------------------------------------------------------------------------------------------
-// batched encode
+// batched encode: a chunk for one slice of its goal (lzgpu_encode_chunks*) or for several in one pass over the data
+// (lzgpu_encode_slices*).  The one-goal calls are the one-slice case of the several-slice calls.
 // ------------------------------------------------------------------------------------------------
-static int encode_enqueue(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, uint32_t chunk_len, const void *d_data, size_t chunk_stride,
-                          void *d_parity, size_t parity_stride, void *d_crc, size_t crc_stride, cudaStream_t st);
+// What slice g (a valid xor/ec goal, or the standard slice) holds of a chunk of nb blocks beside the data: m parity parts of pb
+// blocks, none for the standard slice; so par_bytes of parity and n_crc block CRCs (nb data blocks, then m x pb parity blocks).
+struct SliceShape {
+	size_t m, pb, par_bytes, n_crc;
+	SliceShape(const lzgpu_goal &g, size_t nb)
+	    : m(slice_is_std(g) ? 0 : g.m), pb((nb + g.k - 1) / g.k), par_bytes(m * pb * LZGPU_BLOCK_SIZE), n_crc(nb + m * pb) {}
+};
 
-static uint64_t encode_alg_bytes(const lzgpu_goal *goal, uint32_t n_chunks, uint32_t chunk_len) {
-	// SURVEY.md §8(d): read S, write m*pb*B parity, write 4*(nb + m*pb) CRC bytes
-	const uint64_t B = LZGPU_BLOCK_SIZE, nb = (chunk_len + B - 1) / B, pb = (nb + goal->k - 1) / goal->k;
-	return n_chunks * (static_cast<uint64_t>(chunk_len) + goal->m * pb * B + 4 * (nb + goal->m * pb));
-}
-
-extern "C" int lzgpu_encode_chunks_dev(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, uint32_t chunk_len,
-                                        const void *d_data, size_t chunk_stride, void *d_parity, size_t parity_stride,
-                                        void *d_crc, size_t crc_stride, void *stream) {
-	NvtxScope nvtx_scope("lzgpu::encode_chunks_dev");
-	if (!ctx || !d_data || !d_parity || !d_crc) return LZGPU_ERR_ARG;
-	int rc = check_goal(goal);
-	if (rc) return rc;
-	DeviceGuard g(ctx->device);
-	cudaStream_t st = stream ? static_cast<cudaStream_t>(stream) : ctx->stream;
-	BatchTimer timer(ctx, st, n_chunks ? encode_alg_bytes(goal, n_chunks, chunk_len) : 0);
-	return encode_enqueue(ctx, goal, n_chunks, chunk_len, d_data, chunk_stride, d_parity, parity_stride, d_crc, crc_stride, st);
-}
-
-static int encode_enqueue(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, uint32_t chunk_len, const void *d_data, size_t chunk_stride,
-                          void *d_parity, size_t parity_stride, void *d_crc, size_t crc_stride, cudaStream_t st) {
-	if (!ctx || !d_data || !d_parity || !d_crc) return LZGPU_ERR_ARG;
-	int rc = check_goal(goal);
-	if (rc) return rc;
-	if (chunk_len == 0 || chunk_len > LZGPU_CHUNK_SIZE) { lz_set_error("chunk_len out of range"); return LZGPU_ERR_ARG; }
-	if (n_chunks == 0) return LZGPU_OK;
-	const uint32_t B = LZGPU_BLOCK_SIZE;
-	const uint32_t nb = (chunk_len + B - 1) / B;
-	const uint32_t pb = (nb + goal->k - 1) / goal->k;
-	if (chunk_stride < static_cast<size_t>(nb) * B || parity_stride < static_cast<size_t>(goal->m) * pb * B ||
-	    crc_stride < nb + static_cast<size_t>(goal->m) * pb || (chunk_stride & 15) || (parity_stride & 15) ||
-	    (reinterpret_cast<uintptr_t>(d_data) & 15) || (reinterpret_cast<uintptr_t>(d_parity) & 15)) {
-		lz_set_error("encode: strides too small or buffers not 16-byte aligned");
-		return LZGPU_ERR_ARG;
-	}
-	// a trailing partial block is zero-extended to a whole block (the pad belongs to the stride)
-	if (chunk_len % B) {
-		CUDA_TRY(cudaMemset2DAsync(const_cast<uint8_t *>(static_cast<const uint8_t *>(d_data)) + chunk_len, chunk_stride, 0,
-		                           static_cast<size_t>(nb) * B - chunk_len, n_chunks, st));
-	}
-	rc = lz_fused_encode(ctx, goal, n_chunks, nb, d_data, chunk_stride, d_parity, parity_stride, d_crc, crc_stride, st);
-	if (rc != LZGPU_NOT_HANDLED) {
-		if (rc == LZGPU_OK) ctx->stats.chunks_encoded += n_chunks;
-		if (rc == LZGPU_OK && !lzgpu_crc_enabled()) rc = fill_crc(ctx, d_crc, crc_stride, nb + static_cast<size_t>(goal->m) * pb, n_chunks, st);
-		return rc;
-	}
-	// generic route: GF dot product over the chunk-order layout, then CRC of data and parity blocks
-	uint8_t rows[LZGPU_MAX_PARITY * LZGPU_MAX_DATA];
-	goal_parity_rows(goal, rows);
-	DotDesc d{};
-	for (int j = 0; j < goal->k; ++j) d.src[j] = static_cast<const uint8_t *>(d_data) + static_cast<size_t>(j) * B;
-	std::vector<uint8_t *> dst(goal->m);
-	for (int r = 0; r < goal->m; ++r) dst[r] = static_cast<uint8_t *>(d_parity) + static_cast<size_t>(r) * pb * B;
-	d.dst = dst.data();
-	d.n_src = goal->k;
-	d.n_dst = goal->m;
-	d.total_units = static_cast<unsigned long long>(n_chunks) * pb * (B / 16);
-	d.src_chunk_stride = chunk_stride;
-	d.src_block_stride = static_cast<unsigned long long>(goal->k) * B;
-	d.dst_chunk_stride = parity_stride;
-	d.dst_block_stride = B;
-	d.units_per_block = B / 16;
-	d.blocks_per_chunk = pb;
-	d.valid_k = goal->k;
-	d.valid_nb = nb;
-	rc = lz_gf_dot(ctx, d, rows, st);
-	if (rc) return rc;
-	rc = lz_crc_blocks(ctx, d_data, static_cast<unsigned long long>(n_chunks) * nb, nb, chunk_stride, B, B, d_crc, crc_stride, st);
-	if (rc) return rc;
-	rc = lz_crc_blocks(ctx, d_parity, static_cast<unsigned long long>(n_chunks) * goal->m * pb, static_cast<unsigned long long>(goal->m) * pb,
-	                   parity_stride, B, B, static_cast<uint32_t *>(d_crc) + nb, crc_stride, st);
-	if (rc) return rc;
-	ctx->stats.chunks_encoded += n_chunks;
-	if (!lzgpu_crc_enabled()) return fill_crc(ctx, d_crc, crc_stride, nb + static_cast<size_t>(goal->m) * pb, n_chunks, st);
-	return LZGPU_OK;
-}
-
-extern "C" int lzgpu_encode_chunks(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, uint32_t chunk_len,
-                                    const uint8_t *data, size_t chunk_stride, uint8_t *parity, size_t parity_stride,
-                                    uint32_t *crc, size_t crc_stride) {
-	NvtxScope nvtx_scope("lzgpu::encode_chunks");
-	if (!ctx || !data || !parity || !crc) return LZGPU_ERR_ARG;
-	int rc = check_goal(goal);
-	if (rc) return rc;
-	if (chunk_len == 0 || chunk_len > LZGPU_CHUNK_SIZE) { lz_set_error("chunk_len out of range"); return LZGPU_ERR_ARG; }
-	if (n_chunks == 0) return LZGPU_OK;
-	const uint32_t B = LZGPU_BLOCK_SIZE;
-	const uint32_t nb = (chunk_len + B - 1) / B;
-	const uint32_t pb = (nb + goal->k - 1) / goal->k;
-	const size_t par_bytes = static_cast<size_t>(goal->m) * pb * B;
-	const size_t n_crc = nb + static_cast<size_t>(goal->m) * pb;
-	if (chunk_stride < chunk_len || parity_stride < par_bytes || crc_stride < n_crc) {
-		lz_set_error("encode: strides smaller than the payload");
-		return LZGPU_ERR_ARG;
-	}
-	std::lock_guard<std::mutex> lk(ctx->mu);
-	DeviceGuard g(ctx->device);
-	AutoPin pin(ctx);
-	pin.add(data, static_cast<size_t>(n_chunks - 1) * chunk_stride + chunk_len);
-	pin.add(parity, static_cast<size_t>(n_chunks - 1) * parity_stride + par_bytes);
-	pin.add(crc, (static_cast<size_t>(n_chunks - 1) * crc_stride + n_crc) * 4);
-	const size_t d_chunk_stride = static_cast<size_t>(nb) * B;
-	const size_t d_crc_stride = (n_crc + 3) & ~size_t(3);
-	const uint32_t tile = std::max<uint32_t>(1, std::min<uint32_t>(n_chunks, kHostTileBytes / LZGPU_CHUNK_SIZE));
-	void *d_in[kHostSlots], *d_par[kHostSlots], *d_c[kHostSlots];
-	for (int s = 0; s < kHostSlots; ++s) {
-		if ((rc = lz_scratch(ctx, kScratchIn0 + s, tile * d_chunk_stride, &d_in[s]))) return rc;
-		if ((rc = lz_scratch(ctx, kScratchPar0 + s, tile * par_bytes, &d_par[s]))) return rc;
-		if ((rc = lz_scratch(ctx, kScratchCrc0 + s, tile * d_crc_stride * 4, &d_c[s]))) return rc;
-	}
-	return run_tiles(ctx, n_chunks, tile, kHostSlots, nullptr, [&](int s, size_t c0, size_t n, cudaStream_t st, VerifyTicket *) -> int {
-		CUDA_TRY(cudaMemcpy2DAsync(d_in[s], d_chunk_stride, data + c0 * chunk_stride, chunk_stride, chunk_len, n, cudaMemcpyHostToDevice, st));
-		int rc = lzgpu_encode_chunks_dev(ctx, goal, static_cast<uint32_t>(n), chunk_len, d_in[s], d_chunk_stride, d_par[s], par_bytes, d_c[s],
-		                                 d_crc_stride, st);
-		if (rc) return rc;
-		CUDA_TRY(cudaMemcpy2DAsync(parity + c0 * parity_stride, parity_stride, d_par[s], par_bytes, par_bytes, n, cudaMemcpyDeviceToHost, st));
-		CUDA_TRY(cudaMemcpy2DAsync(crc + c0 * crc_stride, crc_stride * 4, d_c[s], d_crc_stride * 4, n_crc * 4, n, cudaMemcpyDeviceToHost, st));
-		ctx->stats.bytes_h2d += static_cast<uint64_t>(n) * chunk_len;
-		ctx->stats.bytes_d2h += static_cast<uint64_t>(n) * (par_bytes + n_crc * 4);
-		return LZGPU_OK;
-	});
-}
-
-// ------------------------------------------------------------------------------------------------
-// batched encode for several slices in one pass
-// ------------------------------------------------------------------------------------------------
 // SURVEY.md §8(d) over every slice, the data read once: read S, write each xor/ec slice's m*pb*B parity, write every slice's CRC array
 static uint64_t slices_alg_bytes(const lzgpu_goal *goals, uint32_t n_slices, uint32_t n_chunks, uint32_t chunk_len) {
 	const uint64_t B = LZGPU_BLOCK_SIZE, nb = (chunk_len + B - 1) / B;
 	uint64_t per_chunk = chunk_len;
 	for (uint32_t i = 0; i < n_slices; ++i) {
-		const uint64_t m = goal_is_std(&goals[i]) ? 0 : goals[i].m, pb = (nb + goals[i].k - 1) / goals[i].k;
-		per_chunk += m * pb * B + 4 * (nb + m * pb);
+		const SliceShape s(goals[i], nb);
+		per_chunk += s.par_bytes + 4 * s.n_crc;
 	}
 	return n_chunks * per_chunk;
 }
 
-// The arguments of lzgpu_encode_slices* (dev: the device form's strides and 16-byte alignment, as encode_enqueue checks them; else
-// the host form's, as lzgpu_encode_chunks checks them).  Checked before anything is enqueued.
+// The arguments of every encode call, checked before anything is enqueued and whatever n_chunks is.  dev: the device forms' rules (a
+// chunk stride that holds whole blocks, since a trailing partial block is zero-extended in place; strides and buffers 16-byte
+// aligned, because the kernels load and store 16 bytes at a time); else the host forms' (strides that hold the payload).
 static int check_slices(const lzgpu_ctx *ctx, const lzgpu_goal *goals, uint32_t n_slices, uint32_t chunk_len, const void *data, size_t chunk_stride,
                         const void *const *parity, const size_t *parity_stride, const void *const *crc, const size_t *crc_stride, bool dev) {
 	if (!ctx || !goals || !data || !parity || !parity_stride || !crc || !crc_stride) return LZGPU_ERR_ARG;
-	if (n_slices < 1 || n_slices > static_cast<uint32_t>(kSlicesMax)) { lz_set_error("encode_slices: n_slices must be 1..%d", kSlicesMax); return LZGPU_ERR_ARG; }
+	if (n_slices < 1 || n_slices > static_cast<uint32_t>(kSlicesMax)) { lz_set_error("encode: n_slices must be 1..%d", kSlicesMax); return LZGPU_ERR_ARG; }
 	if (chunk_len == 0 || chunk_len > LZGPU_CHUNK_SIZE) { lz_set_error("chunk_len out of range"); return LZGPU_ERR_ARG; }
 	const uint32_t B = LZGPU_BLOCK_SIZE, nb = (chunk_len + B - 1) / B;
 	uint32_t n_striped = 0;
 	for (uint32_t i = 0; i < n_slices; ++i) {
-		const lzgpu_goal *g = &goals[i];
-		const bool std_slice = goal_is_std(g);
-		if (!std_slice && !lzgpu_goal_valid(g)) { lz_set_error("encode_slices: goal %u is neither an xor/ec goal nor the standard slice", i); return LZGPU_ERR_ARG; }
-		const size_t m = std_slice ? 0 : g->m, pb = (nb + g->k - 1) / g->k;
-		if (!crc[i] || (!std_slice && !parity[i])) { lz_set_error("encode_slices: slice %u has no output buffer", i); return LZGPU_ERR_ARG; }
-		if (crc_stride[i] < nb + m * pb || (!std_slice && parity_stride[i] < m * pb * B) ||
+		const bool std_slice = slice_is_std(goals[i]);
+		if (!std_slice && !lzgpu_goal_valid(&goals[i])) { lz_set_error("encode: goal %u is neither an xor/ec goal nor the standard slice", i); return LZGPU_ERR_ARG; }
+		const SliceShape s(goals[i], nb);
+		if (!crc[i] || (!std_slice && !parity[i])) { lz_set_error("encode: slice %u has no output buffer", i); return LZGPU_ERR_ARG; }
+		if (crc_stride[i] < s.n_crc || (!std_slice && parity_stride[i] < s.par_bytes) ||
 		    (dev && !std_slice && ((parity_stride[i] & 15) || (reinterpret_cast<uintptr_t>(parity[i]) & 15)))) {
-			lz_set_error("encode_slices: strides of slice %u too small or its parity buffer not 16-byte aligned", i);
+			lz_set_error("encode: strides of slice %u too small or its parity buffer not 16-byte aligned", i);
 			return LZGPU_ERR_ARG;
 		}
 		n_striped += std_slice ? 0 : 1;
 	}
-	if (n_striped == 0) { lz_set_error("encode_slices: no xor/ec slice"); return LZGPU_ERR_ARG; }
+	if (n_striped == 0) { lz_set_error("encode: no xor/ec slice"); return LZGPU_ERR_ARG; }
 	if (dev ? (chunk_stride < static_cast<size_t>(nb) * B || (chunk_stride & 15) || (reinterpret_cast<uintptr_t>(data) & 15)) : chunk_stride < chunk_len) {
-		lz_set_error("encode_slices: chunk stride too small or data not 16-byte aligned");
+		lz_set_error("encode: chunk stride too small or data not 16-byte aligned");
 		return LZGPU_ERR_ARG;
 	}
 	return LZGPU_OK;
 }
 
-// One pass (lz_fused_encode_slices), else encode_enqueue once per xor/ec slice with the standard slice's CRCs copied from the first
-// one's data CRCs (the same bytes).  Arguments checked by check_slices.
+// One xor/ec slice of chunks of nb whole blocks: the fused route, else the generic one.  Nothing is checked, counted or filled here.
+// slices_enqueue comes with the arguments check_slices took; convert_enqueue with a goal convert_check_args took, a chunk image whose
+// stride and alignment it checked itself (or its own temporary) and parity / CRC temporaries it sized for this goal.
+static int encode_enqueue(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, uint32_t nb, const void *d_data, size_t chunk_stride,
+                          void *d_parity, size_t parity_stride, void *d_crc, size_t crc_stride, cudaStream_t st) {
+	int rc = lz_fused_encode(ctx, goal, n_chunks, nb, d_data, chunk_stride, d_parity, parity_stride, d_crc, crc_stride, st);
+	if (rc != LZGPU_NOT_HANDLED) return rc;
+	// generic route: GF dot product over the chunk-order layout, then CRC of data and parity blocks
+	const uint32_t B = LZGPU_BLOCK_SIZE;
+	const SliceShape s(*goal, nb);
+	uint8_t rows[LZGPU_MAX_PARITY * LZGPU_MAX_DATA];
+	goal_parity_rows(goal, rows);
+	DotDesc d{};
+	for (int j = 0; j < goal->k; ++j) d.src[j] = static_cast<const uint8_t *>(d_data) + static_cast<size_t>(j) * B;
+	std::vector<uint8_t *> dst(goal->m);
+	for (int r = 0; r < goal->m; ++r) dst[r] = static_cast<uint8_t *>(d_parity) + r * s.pb * B;
+	d.dst = dst.data();
+	d.n_src = goal->k;
+	d.n_dst = goal->m;
+	d.total_units = static_cast<unsigned long long>(n_chunks) * s.pb * (B / 16);
+	d.src_chunk_stride = chunk_stride;
+	d.src_block_stride = static_cast<unsigned long long>(goal->k) * B;
+	d.dst_chunk_stride = parity_stride;
+	d.dst_block_stride = B;
+	d.units_per_block = B / 16;
+	d.blocks_per_chunk = static_cast<unsigned>(s.pb);
+	d.valid_k = goal->k;
+	d.valid_nb = nb;
+	if ((rc = lz_gf_dot(ctx, d, rows, st))) return rc;
+	if ((rc = lz_crc_blocks(ctx, d_data, static_cast<unsigned long long>(n_chunks) * nb, nb, chunk_stride, B, B, d_crc, crc_stride, st))) return rc;
+	return lz_crc_blocks(ctx, d_parity, n_chunks * s.m * s.pb, s.m * s.pb, parity_stride, B, B, static_cast<uint32_t *>(d_crc) + nb, crc_stride, st);
+}
+
+// One batch, once per call: the trailing partial block of every chunk zero-extended, then one pass over the data
+// (lz_fused_encode_slices) or, where the plan refuses the set (a single xor/ec slice among the reasons), encode_enqueue per xor/ec
+// slice.  Arguments checked by check_slices.
 static int slices_enqueue(lzgpu_ctx *ctx, const lzgpu_goal *goals, uint32_t n_slices, uint32_t n_chunks, uint32_t chunk_len, const void *d_data,
                           size_t chunk_stride, void *const *d_parity, const size_t *parity_stride, void *const *d_crc, const size_t *crc_stride,
                           cudaStream_t st) {
-	if (n_chunks == 0) return LZGPU_OK;
 	const uint32_t B = LZGPU_BLOCK_SIZE, nb = (chunk_len + B - 1) / B;
+	// a trailing partial block is zero-extended to a whole block (the pad belongs to the stride)
 	if (chunk_len % B) {
 		CUDA_TRY(cudaMemset2DAsync(const_cast<uint8_t *>(static_cast<const uint8_t *>(d_data)) + chunk_len, chunk_stride, 0,
 		                           static_cast<size_t>(nb) * B - chunk_len, n_chunks, st));
 	}
 	int rc = lz_fused_encode_slices(ctx, goals, n_slices, n_chunks, nb, d_data, chunk_stride, d_parity, parity_stride, d_crc, crc_stride, st);
-	if (rc == LZGPU_OK) {
-		ctx->stats.chunks_encoded += n_chunks;
-		if (!lzgpu_crc_enabled())
-			for (uint32_t i = 0; i < n_slices && !rc; ++i) {
-				const size_t m = goal_is_std(&goals[i]) ? 0 : goals[i].m, pb = (nb + goals[i].k - 1) / goals[i].k;
-				rc = fill_crc(ctx, d_crc[i], crc_stride[i], nb + m * pb, n_chunks, st);
-			}
-		return rc;
-	}
-	if (rc != LZGPU_NOT_HANDLED) return rc;
-	int first = -1;
-	uint64_t passes = 0;
-	for (uint32_t i = 0; i < n_slices; ++i) {
-		if (goal_is_std(&goals[i])) continue;
-		if ((rc = encode_enqueue(ctx, &goals[i], n_chunks, chunk_len, d_data, chunk_stride, d_parity[i], parity_stride[i], d_crc[i], crc_stride[i], st)))
-			return rc;
-		if (first < 0) first = static_cast<int>(i);
-		++passes;
-	}
-	ctx->stats.chunks_encoded -= (passes - 1) * n_chunks;   // one count per chunk and call
-	for (uint32_t i = 0; i < n_slices; ++i)
-		if (goal_is_std(&goals[i]))
+	int first = -1;   // the per-slice route ran: its first xor/ec slice (check_slices saw one)
+	if (rc == LZGPU_NOT_HANDLED)
+		for (uint32_t i = 0; i < n_slices; ++i) {
+			if (slice_is_std(goals[i])) continue;
+			if ((rc = encode_enqueue(ctx, &goals[i], n_chunks, nb, d_data, chunk_stride, d_parity[i], parity_stride[i], d_crc[i], crc_stride[i], st))) return rc;
+			if (first < 0) first = static_cast<int>(i);
+		}
+	if (rc) return rc;
+	ctx->stats.chunks_encoded += n_chunks;   // one count per chunk and call
+	// The per-slice route computes nothing for a standard slice: its array is a copy of the first xor/ec slice's data CRCs (the same
+	// bytes), or of the constant that stands there when CRCs are disabled.
+	const bool per_slice = first >= 0;
+	if (!lzgpu_crc_enabled())
+		for (uint32_t i = 0; i < n_slices; ++i) {
+			if (per_slice && slice_is_std(goals[i])) continue;
+			if ((rc = fill_crc(ctx, d_crc[i], crc_stride[i], SliceShape(goals[i], nb).n_crc, n_chunks, st))) return rc;
+		}
+	for (uint32_t i = 0; per_slice && i < n_slices; ++i)
+		if (slice_is_std(goals[i]))
 			CUDA_TRY(cudaMemcpy2DAsync(d_crc[i], crc_stride[i] * 4, d_crc[first], crc_stride[first] * 4, static_cast<size_t>(nb) * 4, n_chunks,
 			                           cudaMemcpyDeviceToDevice, st));
 	return LZGPU_OK;
@@ -920,12 +829,19 @@ extern "C" int lzgpu_encode_slices_dev(lzgpu_ctx *ctx, const lzgpu_goal *goals, 
                                         void *const *d_crc, const size_t *crc_stride, void *stream) {
 	NvtxScope nvtx_scope("lzgpu::encode_slices_dev");
 	int rc = check_slices(ctx, goals, n_slices, chunk_len, d_data, chunk_stride, d_parity, parity_stride, d_crc, crc_stride, true);
-	if (rc) return rc;
-	if (n_chunks == 0) return LZGPU_OK;
+	if (rc || n_chunks == 0) return rc;
 	DeviceGuard g(ctx->device);
 	cudaStream_t st = stream ? static_cast<cudaStream_t>(stream) : ctx->stream;
 	BatchTimer timer(ctx, st, slices_alg_bytes(goals, n_slices, n_chunks, chunk_len));
 	return slices_enqueue(ctx, goals, n_slices, n_chunks, chunk_len, d_data, chunk_stride, d_parity, parity_stride, d_crc, crc_stride, st);
+}
+
+// The one-slice case: the plan refuses a single slice, so encode_enqueue runs for it.  A standard goal has no xor/ec slice and is refused.
+extern "C" int lzgpu_encode_chunks_dev(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, uint32_t chunk_len,
+                                        const void *d_data, size_t chunk_stride, void *d_parity, size_t parity_stride,
+                                        void *d_crc, size_t crc_stride, void *stream) {
+	NvtxScope nvtx_scope("lzgpu::encode_chunks_dev");
+	return lzgpu_encode_slices_dev(ctx, goal, 1, n_chunks, chunk_len, d_data, chunk_stride, &d_parity, &parity_stride, &d_crc, &crc_stride, stream);
 }
 
 extern "C" int lzgpu_encode_slices(lzgpu_ctx *ctx, const lzgpu_goal *goals, uint32_t n_slices, uint32_t n_chunks, uint32_t chunk_len,
@@ -934,16 +850,16 @@ extern "C" int lzgpu_encode_slices(lzgpu_ctx *ctx, const lzgpu_goal *goals, uint
 	NvtxScope nvtx_scope("lzgpu::encode_slices");
 	int rc = check_slices(ctx, goals, n_slices, chunk_len, data, chunk_stride, reinterpret_cast<const void *const *>(parity), parity_stride,
 	                      reinterpret_cast<const void *const *>(crc), crc_stride, false);
-	if (rc) return rc;
-	if (n_chunks == 0) return LZGPU_OK;
+	if (rc || n_chunks == 0) return rc;
 	const uint32_t B = LZGPU_BLOCK_SIZE, nb = (chunk_len + B - 1) / B;
-	// device layout of a tile: the data dense; slice i's parity and CRCs dense too, at par_off[i] / crc_off[i] per chunk of the tile
+	// device layout of a tile: the data dense; slice i's parity and CRCs dense too (the CRC stride rounded up to four words), at
+	// par_off[i] / crc_off[i] per chunk of the tile
 	size_t par_bytes[kSlicesMax] = {0}, n_crc[kSlicesMax] = {0}, d_crc_stride[kSlicesMax] = {0}, par_off[kSlicesMax] = {0}, crc_off[kSlicesMax] = {0};
 	size_t par_total = 0, crc_total = 0;
 	for (uint32_t i = 0; i < n_slices; ++i) {
-		const size_t m = goal_is_std(&goals[i]) ? 0 : goals[i].m, pb = (nb + goals[i].k - 1) / goals[i].k;
-		par_bytes[i] = m * pb * B;
-		n_crc[i] = nb + m * pb;
+		const SliceShape s(goals[i], nb);
+		par_bytes[i] = s.par_bytes;
+		n_crc[i] = s.n_crc;
 		d_crc_stride[i] = (n_crc[i] + 3) & ~size_t(3);
 		par_off[i] = par_total;
 		crc_off[i] = crc_total;
@@ -987,6 +903,13 @@ extern "C" int lzgpu_encode_slices(lzgpu_ctx *ctx, const lzgpu_goal *goals, uint
 		ctx->stats.bytes_d2h += static_cast<uint64_t>(n) * d2h;
 		return LZGPU_OK;
 	});
+}
+
+extern "C" int lzgpu_encode_chunks(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, uint32_t chunk_len,
+                                    const uint8_t *data, size_t chunk_stride, uint8_t *parity, size_t parity_stride,
+                                    uint32_t *crc, size_t crc_stride) {
+	NvtxScope nvtx_scope("lzgpu::encode_chunks");
+	return lzgpu_encode_slices(ctx, goal, 1, n_chunks, chunk_len, data, chunk_stride, &parity, &parity_stride, &crc, &crc_stride);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -1937,7 +1860,7 @@ static bool same_goal(const lzgpu_goal *a, const lzgpu_goal *b) { return a->kind
 static int convert_check_args(lzgpu_ctx *ctx, const lzgpu_goal *src, const lzgpu_goal *dst, uint32_t nb, const void *parts, const uint8_t *want,
                               const void *out) {
 	if (!ctx || !src || !dst || !parts || !want || !out) return LZGPU_ERR_ARG;
-	if (!goal_is_std(dst) && check_goal(dst)) return LZGPU_ERR_ARG;  // both goals before nb
+	if (!slice_is_std(*dst) && check_goal(dst)) return LZGPU_ERR_ARG;  // both goals before nb
 	return check_batch(ctx, src, nb, true);
 }
 
@@ -2006,7 +1929,7 @@ static int convert_enqueue(lzgpu_ctx *ctx, const lzgpu_goal *src, const lzgpu_go
 	void *d_encode_crc = nullptr;  // CRC array of the destination-slice encode, when that ran
 	size_t encode_crc_stride = 0;
 
-	if (same_goal(src, dst) && !goal_is_std(src)) {
+	if (same_goal(src, dst) && !slice_is_std(*src)) {
 		// kReadDataPart (slice_recovery_planner.h:98-101): the part is read, or rebuilt from k parts of the same slice
 		uint8_t need[LZGPU_MAX_PARTS] = {0};
 		bool any = false;
@@ -2029,8 +1952,8 @@ static int convert_enqueue(lzgpu_ctx *ctx, const lzgpu_goal *src, const lzgpu_go
 		const uint8_t *image = nullptr;
 		size_t image_stride = 0;
 		bool converted = false;   // the one-pass route produced every wanted destination part
-		void *direct_image = (goal_is_std(dst) && want[0]) ? d_out[0] : nullptr;  // a standard destination IS the chunk image
-		if (goal_is_std(src)) {
+		void *direct_image = (slice_is_std(*dst) && want[0]) ? d_out[0] : nullptr;  // a standard destination IS the chunk image
+		if (slice_is_std(*src)) {
 			if (!d_parts[0]) { lz_set_error("convert: the standard chunk is not available"); return LZGPU_ERR_TOO_FEW_PARTS; }
 			image = static_cast<const uint8_t *>(d_parts[0]);
 			image_stride = part_stride;
@@ -2040,7 +1963,7 @@ static int convert_enqueue(lzgpu_ctx *ctx, const lzgpu_goal *src, const lzgpu_go
 				CUDA_TRY(cudaMemcpy2DAsync(direct_image, out_stride, image, image_stride, static_cast<size_t>(nb) * B, n_chunks, cudaMemcpyDeviceToDevice, st));
 		} else {
 			// One pass (convert_kernel.cuh): source parts -> destination parts + their CRCs, no chunk image
-			if (!goal_is_std(dst)) {
+			if (!slice_is_std(*dst)) {
 				rc = try_fused_convert(ctx, src, dst, n_chunks, nb, d_parts, part_stride, d_part_crc, want, d_out, out_stride, st, tk, &t_crc, &encode_crc_stride);
 				if (rc == LZGPU_OK) {
 					converted = true;
@@ -2050,7 +1973,7 @@ static int convert_enqueue(lzgpu_ctx *ctx, const lzgpu_goal *src, const lzgpu_go
 				}
 			}
 		}
-		if (!goal_is_std(src) && !converted) {
+		if (!slice_is_std(*src) && !converted) {
 			void *d_img = direct_image;
 			image_stride = direct_image ? out_stride : static_cast<size_t>(nb) * B;
 			if (!d_img) {
@@ -2062,7 +1985,7 @@ static int convert_enqueue(lzgpu_ctx *ctx, const lzgpu_goal *src, const lzgpu_go
 				return rc;
 			image = static_cast<const uint8_t *>(d_img);
 		}
-		if (!goal_is_std(dst) && !converted) {
+		if (!slice_is_std(*dst) && !converted) {
 			bool data_wanted = false, parity_wanted = false;
 			void *dp[LZGPU_MAX_DATA] = {nullptr};
 			for (int i = 0; i < nd; ++i) {
@@ -2095,7 +2018,8 @@ static int convert_enqueue(lzgpu_ctx *ctx, const lzgpu_goal *src, const lzgpu_go
 				if (parity_wanted) {
 					const size_t par_stride = static_cast<size_t>(dst->m) * pbd * B, crc_stride = (nb + static_cast<size_t>(dst->m) * pbd + 3) & ~size_t(3);
 					if ((rc = t_par.alloc(n_chunks * par_stride)) || (!t_crc.p && (rc = t_crc.alloc(n_chunks * crc_stride * 4)))) return rc;
-					if ((rc = encode_enqueue(ctx, dst, n_chunks, nb * B, image, image_stride, t_par.p, par_stride, t_crc.p, crc_stride, st))) return rc;
+					if ((rc = encode_enqueue(ctx, dst, n_chunks, nb, image, image_stride, t_par.p, par_stride, t_crc.p, crc_stride, st))) return rc;
+					ctx->stats.chunks_encoded += n_chunks;
 					d_encode_crc = t_crc.p;
 					encode_crc_stride = crc_stride;
 					for (int r = 0; r < dst->m; ++r)

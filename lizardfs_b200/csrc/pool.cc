@@ -177,14 +177,8 @@ static int pool_run(lzgpu_pool *pool, uint32_t n_chunks, const std::function<int
 
 extern "C" int lzgpu_pool_encode_chunks(lzgpu_pool *pool, const lzgpu_goal *goal, uint32_t n_chunks, uint32_t chunk_len, const uint8_t *data,
                                          size_t chunk_stride, uint8_t *parity, size_t parity_stride, uint32_t *crc, size_t crc_stride) {
-	if (!pool || !goal || !data || !parity || !crc) return LZGPU_ERR_ARG;
-	if (n_chunks == 0) return LZGPU_OK;
-	std::vector<std::string> errs;
-	return pool_run(pool, n_chunks, [&](int i, uint32_t first, uint32_t count) {
-		return lzgpu_encode_chunks(pool->workers[i]->ctx, goal, count, chunk_len, data + static_cast<size_t>(first) * chunk_stride, chunk_stride,
-		                           parity + static_cast<size_t>(first) * parity_stride, parity_stride, crc + static_cast<size_t>(first) * crc_stride,
-		                           crc_stride);
-	}, &errs);
+	if (!parity || !crc) return LZGPU_ERR_ARG;   // (refused for an empty batch too, which no context would see)
+	return lzgpu_pool_encode_slices(pool, goal, 1, n_chunks, chunk_len, data, chunk_stride, &parity, &parity_stride, &crc, &crc_stride);
 }
 
 extern "C" int lzgpu_pool_encode_slices(lzgpu_pool *pool, const lzgpu_goal *goals, uint32_t n_slices, uint32_t n_chunks, uint32_t chunk_len,

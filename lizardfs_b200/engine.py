@@ -103,22 +103,6 @@ def _name(fn):
 
 
 # the bodies of the batch calls that Engine and Pool share, `fn` the C function (the context or the pool as its first argument)
-def _encode_chunks(fn, h, goal, data, chunk_len, parity=None, crc=None):
-    data = _u8(data)
-    if data.ndim == 1:
-        data = data.reshape(1, -1)
-    n, stride = data.shape
-    if chunk_len is None:
-        chunk_len = stride
-    nb, pb = Engine.geometry(goal, chunk_len)
-    if parity is None:
-        parity = np.empty((n, goal.m, pb * BLOCK_SIZE), dtype=np.uint8)
-    if crc is None:
-        crc = np.empty((n, nb + goal.m * pb), dtype=np.uint32)
-    _check(fn(h, C.byref(goal.c), n, chunk_len, _p(data), stride, _p(parity), goal.m * pb * BLOCK_SIZE, _p(crc), nb + goal.m * pb), _name(fn))
-    return parity, crc
-
-
 def _goal_array(goals):
     arr = (LzGoal * len(goals))()
     for i, g in enumerate(goals):
@@ -126,26 +110,39 @@ def _goal_array(goals):
     return arr
 
 
-def _encode_slices(fn, h, goals, data, chunk_len):
-    """one (parity or None, crc) per slice: parity [n, m, pb * 64 KiB] and crc [n, nb + m * pb] as _encode_chunks returns them for
-    an xor/ec slice, parity None and crc [n, nb] for the standard slice"""
+def _encode_slices(fn, h, goals, data, chunk_len, out=None):
+    """one (parity or None, crc) per slice: parity [n, m, pb * 64 KiB] and crc [n, nb + m * pb] for an xor/ec slice, parity None and
+    crc [n, nb] for the standard slice.  out: the caller's (parity, crc) per slice, C-contiguous arrays of those shapes that the
+    call writes into; a None among them is allocated here."""
     data = _u8(data)
     if data.ndim == 1:
         data = data.reshape(1, -1)
     n, stride = data.shape
     if chunk_len is None:
         chunk_len = stride
-    out = []
-    for g in goals:
+    ns = len(goals)
+    par_stride, crc_stride = (C.c_size_t * ns)(), (C.c_size_t * ns)()
+    res = []
+    for i, (g, (parity, crc)) in enumerate(zip(goals, out or [(None, None)] * ns)):
         nb, pb = Engine.geometry(g, chunk_len)
         m = 0 if g.is_std else g.m
-        out.append((None if g.is_std else np.empty((n, m, pb * BLOCK_SIZE), dtype=np.uint8), np.empty((n, nb + m * pb), dtype=np.uint32)))
-    ns = len(goals)
-    par_stride = (C.c_size_t * ns)(*[0 if p is None else p.shape[1] * p.shape[2] for p, _ in out])
-    crc_stride = (C.c_size_t * ns)(*[c.shape[1] for _, c in out])
-    _check(fn(h, _goal_array(goals), ns, n, chunk_len, _p(data), stride, _ptr_array([p for p, _ in out]), par_stride,
-              _ptr_array([c for _, c in out]), crc_stride), _name(fn))
-    return out
+        par_stride[i], crc_stride[i] = m * pb * BLOCK_SIZE, nb + m * pb
+        if parity is None and m:
+            parity = np.empty((n, m, pb * BLOCK_SIZE), dtype=np.uint8)
+        if crc is None:
+            crc = np.empty((n, nb + m * pb), dtype=np.uint32)
+        res.append((parity, crc))
+    _check(fn(h, _goal_array(goals), ns, n, chunk_len, _p(data), stride, _ptr_array([p for p, _ in res]), par_stride,
+              _ptr_array([c for _, c in res]), crc_stride), _name(fn))
+    return res
+
+
+def _encode_chunks(fn, h, goal, data, chunk_len, parity=None, crc=None):
+    """_encode_slices for one xor/ec slice through the one-goal C call: scalars where that takes one-entry arrays"""
+    def one(h, goals, ns, n, chunk_len, data, stride, parity, par_stride, crc, crc_stride):
+        return fn(h, goals, n, chunk_len, data, stride, parity[0], par_stride[0], crc[0], crc_stride[0])
+    one.__name__ = fn.__name__
+    return _encode_slices(one, h, [goal], data, chunk_len, [(parity, crc)])[0]
 
 
 def _recover_chunks(fn, h, goal, nb, parts, part_crc, want, chunk_image):

@@ -260,6 +260,8 @@ def test_argument_refusals_launch_nothing():
             eng.encode_slices_dev(goals, 1, 8 * BLOCK, data_ptr, stride, args["par"], ps, args["crc"], args["cs"])
     with pytest.raises(LzGpuError):
         eng.encode_slices_dev(goals, 1, 8 * BLOCK, d.data_ptr(), 8 * BLOCK, [p.data_ptr(), 0], args["ps"], args["crc"], args["cs"])
+    with pytest.raises(LzGpuError):                                                  # an empty batch is checked like any other, by the one-goal call too
+        eng.encode_chunks_dev(goals[0], 0, 8 * BLOCK, d.data_ptr(), 8 * BLOCK - 16, p.data_ptr(), 4 * BLOCK, c.data_ptr(), 12)
     torch.cuda.synchronize()
     assert eng.stats()["kernel_launches"] == before
 
