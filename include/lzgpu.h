@@ -312,7 +312,8 @@ int lzgpu_debug_status_slots(lzgpu_ctx *ctx, uint32_t *allocated, uint32_t *in_u
  * share through that device's own H2D | kernel | D2H pipeline concurrently and returns when all are done.  Pool calls may be
  * issued from any number of threads; the shares of concurrent calls queue per device.  Arguments as in the per-context calls.
  * device_mask: bit d = CUDA device d, 0 = every visible device.  lzgpu_pool_create_list takes explicit device numbers (a
- * device may be listed twice: two contexts, two pipelines on one GPU).
+ * device may be listed twice: two contexts, two pipelines on one GPU).  The pool forms of the stripe check, correction, repair and
+ * decode and of the block scrub, with their rule for merging the shares' results, follow lzgpu_verify_moosefs below.
  * ------------------------------------------------------------------------------------------- */
 typedef struct lzgpu_pool lzgpu_pool;
 int lzgpu_pool_create(uint64_t device_mask, lzgpu_pool **out);
@@ -716,6 +717,46 @@ int lzgpu_verify_interleaved(lzgpu_ctx *ctx, const uint8_t *records, size_t n_bl
  * No sparse rule on this format (hddspacemgr.cc:1746-1764). */
 size_t lzgpu_moosefs_header_size(int data_parts);
 int lzgpu_verify_moosefs(lzgpu_ctx *ctx, int data_parts, const uint8_t *file_image, size_t n_blocks, int64_t *first_bad);
+
+/* The chunkserver's stripe consistency job and block scrub over every device of a pool (see "Device pool" above).  Each call takes
+ * the arguments of the per-context host-pointer call of the same name, with the pool in place of the context, and returns for any
+ * input exactly what that call returns on one context for the whole batch.  Share [first, first + count) of device slot i
+ * (lzgpu_pool_share) runs that per-context call with the part pointers moved by first * part_stride, the stored-CRC arrays by
+ * first * pb (pb = ceil(nb / k)), verdict by first, map / fix by first * pb entries; the scrub calls take blocks (records) in shares,
+ * stored_crc moved by first.
+ *   - Every share runs to the end, so every correction, repair and decode the rule allows is made, also when the call returns
+ *     LZGPU_ERR_CRC.  Shares write into disjoint ranges of the parts and results, in place and at the same time.
+ *   - A hard error (anything other than LZGPU_OK, LZGPU_ERR_CRC, LZGPU_ERR_INCONSISTENT) wins, the lowest device slot's first.
+ *     Otherwise LZGPU_ERR_CRC if any share returned it (also when an inconsistent chunk lies in an earlier share), else
+ *     LZGPU_ERR_INCONSISTENT if any share returned it, else LZGPU_OK.  lzgpu_last_error is the returning slot's text.
+ *   - bad[0..2] and *first_bad come from the lowest share that reported one, at the chunk's (block's) index in the whole batch.
+ *   - An empty batch runs on slot 0 with a count of 0, so the per-context call's argument refusals (LZGPU_ERR_TOO_FEW_PARTS, missing
+ *     stored CRCs, CRCs disabled for the repair and the decode, ...) are the pool's; with a non-empty batch every share refuses alike
+ *     and nothing is written.
+ *   - The scrub calls take host memory only: LZGPU_ERR_ARG, before any share runs, when cudaPointerGetAttributes reports device memory
+ *     (one device's memory cannot go to another device's context). */
+int lzgpu_pool_check_stripes(lzgpu_pool *pool, const lzgpu_goal *goal, uint32_t n_chunks, uint32_t nb,
+                             const uint8_t *const *parts, size_t part_stride, const uint32_t *const *part_crc,
+                             lzgpu_stripe_verdict *verdict, int64_t *bad);
+int lzgpu_pool_check_stripe_map(lzgpu_pool *pool, const lzgpu_goal *goal, uint32_t n_chunks, uint32_t nb,
+                                const uint8_t *const *parts, size_t part_stride, const uint32_t *const *part_crc,
+                                lzgpu_stripe_state *map, int64_t *bad);
+int lzgpu_pool_correct_stripes(lzgpu_pool *pool, const lzgpu_goal *goal, uint32_t n_chunks, uint32_t nb,
+                               uint8_t *const *parts, size_t part_stride, const uint32_t *const *part_crc,
+                               lzgpu_stripe_fix *fix, int64_t *bad);
+int lzgpu_pool_check_stripe_map_degraded(lzgpu_pool *pool, const lzgpu_goal *goal, uint32_t n_chunks, uint32_t nb,
+                                         const uint8_t *const *parts, size_t part_stride, const uint32_t *const *part_crc,
+                                         lzgpu_stripe_state *map, int64_t *bad);
+int lzgpu_pool_correct_stripes_degraded(lzgpu_pool *pool, const lzgpu_goal *goal, uint32_t n_chunks, uint32_t nb,
+                                        uint8_t *const *parts, size_t part_stride, const uint32_t *const *part_crc,
+                                        lzgpu_stripe_fix *fix, int64_t *bad);
+int lzgpu_pool_repair_stripes(lzgpu_pool *pool, const lzgpu_goal *goal, uint32_t n_chunks, uint32_t nb,
+                              uint8_t *const *parts, size_t part_stride, const uint32_t *const *part_crc, lzgpu_stripe_repair *fix);
+int lzgpu_pool_decode_stripes(lzgpu_pool *pool, const lzgpu_goal *goal, uint32_t n_chunks, uint32_t nb,
+                              uint8_t *const *parts, size_t part_stride, const uint32_t *const *part_crc, lzgpu_stripe_decode *fix);
+int lzgpu_pool_verify_blocks(lzgpu_pool *pool, const uint8_t *data, size_t n_blocks, uint32_t block_len,
+                             size_t block_stride, const uint32_t *stored_crc, int sparse_rule, int64_t *first_bad);
+int lzgpu_pool_verify_interleaved(lzgpu_pool *pool, const uint8_t *records, size_t n_blocks, int64_t *first_bad);
 
 /* Chunkserver block writes, batched (SURVEY.md §8 f3; hdd_write, src/chunkserver/hddspacemgr.cc:1898-2008).
  * Per request, exactly the reference's checks and CRC arithmetic: the payload must match the CRC of its packet

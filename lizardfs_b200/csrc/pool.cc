@@ -145,33 +145,46 @@ extern "C" void lzgpu_pool_share(uint32_t n_chunks, int n_devices, int i, uint32
 	if (count) *count = std::min<uint32_t>(per, n_chunks - f);
 }
 
-// run fn(worker index, first chunk, chunk count) on every device that gets a share; first error by device order wins
-static int pool_run(lzgpu_pool *pool, uint32_t n_chunks, const std::function<int(int, uint32_t, uint32_t)> &fn, std::vector<std::string> *errs) {
+// the codes and error texts of the shares of one pool call, by device slot
+struct Shares {
+	std::vector<int> rc;
+	std::vector<std::string> err;
+	int report(int i) const {  // slot i's code, with its text as the calling thread's lzgpu_last_error
+		lz_set_error("device slot %d: %s", i, err[i].c_str());
+		return rc[i];
+	}
+};
+
+// run fn(worker index, first chunk, chunk count) on every device that gets a share and wait for all of them; an empty batch goes to
+// slot 0 with a count of 0 (the calls that return early for one never get here)
+static Shares pool_each(lzgpu_pool *pool, uint32_t n_chunks, const std::function<int(int, uint32_t, uint32_t)> &fn) {
 	const int G = static_cast<int>(pool->workers.size());
-	std::vector<int> rcs(G, LZGPU_OK);
-	errs->assign(G, std::string());
+	Shares sh{std::vector<int>(G, LZGPU_OK), std::vector<std::string>(G)};
 	Latch latch;
 	for (int i = 0; i < G; ++i) {
 		uint32_t first, count;
 		lzgpu_pool_share(n_chunks, G, i, &first, &count);
-		if (count) latch.pending++;
+		if (count || (n_chunks == 0 && i == 0)) latch.pending++;
 	}
 	for (int i = 0; i < G; ++i) {
 		uint32_t first, count;
 		lzgpu_pool_share(n_chunks, G, i, &first, &count);
-		if (!count) continue;
+		if (!count && !(n_chunks == 0 && i == 0)) continue;
 		pool->workers[i]->post([&, i, first, count] {
-			rcs[i] = fn(i, first, count);
-			if (rcs[i] != LZGPU_OK) (*errs)[i] = lzgpu_last_error();  // thread-local text of the worker
+			sh.rc[i] = fn(i, first, count);
+			if (sh.rc[i] != LZGPU_OK) sh.err[i] = lzgpu_last_error();  // thread-local text of the worker
 			latch.done();
 		});
 	}
 	latch.wait();
-	for (int i = 0; i < G; ++i)
-		if (rcs[i] != LZGPU_OK) {
-			lz_set_error("device slot %d: %s", i, (*errs)[i].c_str());
-			return rcs[i];
-		}
+	return sh;
+}
+
+// pool_each, and the first error by device order wins
+static int pool_run(lzgpu_pool *pool, uint32_t n_chunks, const std::function<int(int, uint32_t, uint32_t)> &fn) {
+	const Shares sh = pool_each(pool, n_chunks, fn);
+	for (size_t i = 0; i < sh.rc.size(); ++i)
+		if (sh.rc[i] != LZGPU_OK) return sh.report(static_cast<int>(i));
 	return LZGPU_OK;
 }
 
@@ -186,7 +199,6 @@ extern "C" int lzgpu_pool_encode_slices(lzgpu_pool *pool, const lzgpu_goal *goal
                                          uint32_t *const *crc, const size_t *crc_stride) {
 	if (!pool || !goals || !data || !parity || !parity_stride || !crc || !crc_stride || n_slices < 1 || n_slices > 4) return LZGPU_ERR_ARG;
 	if (n_chunks == 0) return LZGPU_OK;
-	std::vector<std::string> errs;
 	return pool_run(pool, n_chunks, [&](int i, uint32_t first, uint32_t count) {
 		uint8_t *p[4] = {nullptr, nullptr, nullptr, nullptr};
 		uint32_t *c[4] = {nullptr, nullptr, nullptr, nullptr};
@@ -196,7 +208,7 @@ extern "C" int lzgpu_pool_encode_slices(lzgpu_pool *pool, const lzgpu_goal *goal
 		}
 		return lzgpu_encode_slices(pool->workers[i]->ctx, goals, n_slices, count, chunk_len, data + static_cast<size_t>(first) * chunk_stride, chunk_stride,
 		                           p, parity_stride, c, crc_stride);
-	}, &errs);
+	});
 }
 
 extern "C" int lzgpu_pool_recover_chunks(lzgpu_pool *pool, const lzgpu_goal *goal, uint32_t n_chunks, uint32_t nb, const uint8_t *const *parts,
@@ -208,7 +220,6 @@ extern "C" int lzgpu_pool_recover_chunks(lzgpu_pool *pool, const lzgpu_goal *goa
 	const int G = static_cast<int>(pool->workers.size()), n = goal->k + goal->m;
 	const uint32_t pb = (nb + goal->k - 1) / goal->k;
 	std::vector<int64_t> bads(static_cast<size_t>(G) * 3, -1);
-	std::vector<std::string> errs;
 	int rc = pool_run(pool, n_chunks, [&](int i, uint32_t first, uint32_t count) {
 		std::vector<const uint8_t *> p(n, nullptr);
 		std::vector<const uint32_t *> pc(n, nullptr);
@@ -223,7 +234,7 @@ extern "C" int lzgpu_pool_recover_chunks(lzgpu_pool *pool, const lzgpu_goal *goa
 		                             chunk_out_stride, &bads[static_cast<size_t>(i) * 3]);
 		if (r == LZGPU_ERR_CRC && bads[static_cast<size_t>(i) * 3] >= 0) bads[static_cast<size_t>(i) * 3] += first;
 		return r;
-	}, &errs);
+	});
 	if (rc == LZGPU_ERR_CRC && bad) {
 		// lowest chunk index over the devices that reported a mismatch (shares are ascending runs of chunks)
 		for (int i = 0; i < G; ++i)
@@ -248,7 +259,6 @@ extern "C" int lzgpu_pool_convert_chunks(lzgpu_pool *pool, const lzgpu_goal *src
 	// blocks per chunk of a source / destination part (a standard slice has the single part 0 = the chunk itself)
 	const uint32_t pbs = src->kind == LZGPU_KIND_STD ? nb : (nb + src->k - 1) / src->k, pbd = dst->kind == LZGPU_KIND_STD ? nb : (nb + dst->k - 1) / dst->k;
 	std::vector<int64_t> bads(static_cast<size_t>(G) * 3, -1);
-	std::vector<std::string> errs;
 	int rc = pool_run(pool, n_chunks, [&](int i, uint32_t first, uint32_t count) {
 		std::vector<const uint8_t *> p(ns, nullptr);
 		std::vector<const uint32_t *> pc(ns, nullptr);
@@ -266,7 +276,7 @@ extern "C" int lzgpu_pool_convert_chunks(lzgpu_pool *pool, const lzgpu_goal *src
 		                             out_stride, out_crc ? oc.data() : nullptr, &bads[static_cast<size_t>(i) * 3]);
 		if (r == LZGPU_ERR_CRC && bads[static_cast<size_t>(i) * 3] >= 0) bads[static_cast<size_t>(i) * 3] += first;
 		return r;
-	}, &errs);
+	});
 	if (rc == LZGPU_ERR_CRC && bad) {
 		for (int i = 0; i < G; ++i)
 			if (bads[static_cast<size_t>(i) * 3] >= 0) {
@@ -282,10 +292,164 @@ extern "C" int lzgpu_pool_crc_blocks(lzgpu_pool *pool, const uint8_t *data, size
 	if (!pool || !data || !crc_out) return LZGPU_ERR_ARG;
 	if (n_blocks == 0) return LZGPU_OK;
 	if (n_blocks > 0xffffffffull) return LZGPU_ERR_ARG;
-	std::vector<std::string> errs;
 	return pool_run(pool, static_cast<uint32_t>(n_blocks), [&](int i, uint32_t first, uint32_t count) {
 		return lzgpu_crc_blocks(pool->workers[i]->ctx, data + static_cast<size_t>(first) * block_stride, count, block_len, block_stride, crc_out + first);
-	}, &errs);
+	});
+}
+
+// ------------------------------------------------------------------------------------------------
+// the chunkserver's stripe check, repair and decode and its block scrub over the pool (include/lzgpu.h "device pool")
+// ------------------------------------------------------------------------------------------------
+constexpr int64_t kUnset = INT64_MIN;  // a share's bad[0] before its call: the call wrote nothing there
+
+// Run call(ctx, first, count, local_bad) on every share, every one to the end, and merge: a hard error (anything but LZGPU_OK,
+// LZGPU_ERR_CRC and LZGPU_ERR_INCONSISTENT) wins by device slot, else LZGPU_ERR_CRC if any share returned it, else
+// LZGPU_ERR_INCONSISTENT if any did, else LZGPU_OK: the precedence of the per-context calls.  bad[0 .. width-1] comes from the lowest
+// slot that reported a position, with its first chunk (block) added to bad[0]: shares are ascending runs, so that is the position
+// one context reports for the whole batch.  With none, the -1 a share wrote, or nothing when no share wrote (a refusal).
+template <class Call>
+static int pool_merged(lzgpu_pool *pool, uint32_t n_chunks, int64_t *bad, int width, Call &&call) {
+	const int G = static_cast<int>(pool->workers.size());
+	std::vector<int64_t> bads(static_cast<size_t>(G) * width, kUnset);
+	const Shares sh = pool_each(pool, n_chunks, [&](int i, uint32_t first, uint32_t count) {
+		return call(pool->workers[i]->ctx, first, count, bad ? &bads[static_cast<size_t>(i) * width] : nullptr);
+	});
+	if (bad) {
+		auto at = [&](int i) { return bads[static_cast<size_t>(i) * width]; };
+		int from = -1;
+		for (int i = G - 1; i >= 0; --i)
+			if (at(i) != kUnset) from = i;  // the lowest slot that wrote
+		for (int i = G - 1; i >= 0; --i)
+			if (at(i) >= 0) from = i;       // the lowest slot that reported a position
+		if (from >= 0) {
+			uint32_t first;
+			lzgpu_pool_share(n_chunks, G, from, &first, nullptr);
+			std::memcpy(bad, &bads[static_cast<size_t>(from) * width], width * sizeof(int64_t));
+			if (bad[0] >= 0) bad[0] += first;
+		}
+	}
+	for (int i = 0; i < G; ++i)
+		if (sh.rc[i] != LZGPU_OK && sh.rc[i] != LZGPU_ERR_CRC && sh.rc[i] != LZGPU_ERR_INCONSISTENT) return sh.report(i);
+	for (int code : {LZGPU_ERR_CRC, LZGPU_ERR_INCONSISTENT})
+		for (int i = 0; i < G; ++i)
+			if (sh.rc[i] == code) return sh.report(i);
+	return LZGPU_OK;
+}
+
+// The part-batch calls: each share gets the part pointers moved by first * part_stride, the stored-CRC arrays by first * pb and `out`
+// by first entries (per_stripe: first * pb).  Without parts, or with a goal or nb the per-context call refuses, the caller's arrays go
+// through unmoved and every share refuses identically.
+template <class P, class Out, class Call>
+static int pool_part_batch(lzgpu_pool *pool, const lzgpu_goal *goal, uint32_t n_chunks, uint32_t nb, P *const *parts, size_t part_stride,
+                           const uint32_t *const *part_crc, Out *out, bool per_stripe, int64_t *bad, Call &&call) {
+	if (!pool) return LZGPU_ERR_ARG;
+	const bool shaped = parts && lzgpu_goal_valid(goal) && nb >= 1 && nb <= LZGPU_BLOCKS_IN_CHUNK;
+	const int n = shaped ? goal->k + goal->m : 0;
+	const size_t pb = shaped ? (nb + goal->k - 1) / goal->k : 0;
+	return pool_merged(pool, n_chunks, bad, 3, [&](lzgpu_ctx *ctx, uint32_t first, uint32_t count, int64_t *b) {
+		P *p[LZGPU_MAX_PARTS];
+		const uint32_t *c[LZGPU_MAX_PARTS];
+		for (int j = 0; j < n; ++j) {
+			p[j] = parts[j] ? parts[j] + first * part_stride : nullptr;
+			c[j] = part_crc && part_crc[j] ? part_crc[j] + first * pb : nullptr;
+		}
+		return call(ctx, count, shaped ? p : parts, shaped && part_crc ? c : part_crc, out ? out + first * (per_stripe ? pb : 1) : nullptr, b);
+	});
+}
+
+extern "C" int lzgpu_pool_check_stripes(lzgpu_pool *pool, const lzgpu_goal *goal, uint32_t n_chunks, uint32_t nb, const uint8_t *const *parts,
+                                         size_t part_stride, const uint32_t *const *part_crc, lzgpu_stripe_verdict *verdict, int64_t *bad) {
+	return pool_part_batch(pool, goal, n_chunks, nb, parts, part_stride, part_crc, verdict, false, bad,
+	                       [&](lzgpu_ctx *ctx, uint32_t count, const uint8_t *const *p, const uint32_t *const *c, lzgpu_stripe_verdict *o, int64_t *b) {
+		return lzgpu_check_stripes(ctx, goal, count, nb, p, part_stride, c, o, b);
+	});
+}
+
+extern "C" int lzgpu_pool_check_stripe_map(lzgpu_pool *pool, const lzgpu_goal *goal, uint32_t n_chunks, uint32_t nb, const uint8_t *const *parts,
+                                            size_t part_stride, const uint32_t *const *part_crc, lzgpu_stripe_state *map, int64_t *bad) {
+	return pool_part_batch(pool, goal, n_chunks, nb, parts, part_stride, part_crc, map, true, bad,
+	                       [&](lzgpu_ctx *ctx, uint32_t count, const uint8_t *const *p, const uint32_t *const *c, lzgpu_stripe_state *o, int64_t *b) {
+		return lzgpu_check_stripe_map(ctx, goal, count, nb, p, part_stride, c, o, b);
+	});
+}
+
+extern "C" int lzgpu_pool_correct_stripes(lzgpu_pool *pool, const lzgpu_goal *goal, uint32_t n_chunks, uint32_t nb, uint8_t *const *parts,
+                                           size_t part_stride, const uint32_t *const *part_crc, lzgpu_stripe_fix *fix, int64_t *bad) {
+	return pool_part_batch(pool, goal, n_chunks, nb, parts, part_stride, part_crc, fix, true, bad,
+	                       [&](lzgpu_ctx *ctx, uint32_t count, uint8_t *const *p, const uint32_t *const *c, lzgpu_stripe_fix *o, int64_t *b) {
+		return lzgpu_correct_stripes(ctx, goal, count, nb, p, part_stride, c, o, b);
+	});
+}
+
+extern "C" int lzgpu_pool_check_stripe_map_degraded(lzgpu_pool *pool, const lzgpu_goal *goal, uint32_t n_chunks, uint32_t nb,
+                                                     const uint8_t *const *parts, size_t part_stride, const uint32_t *const *part_crc,
+                                                     lzgpu_stripe_state *map, int64_t *bad) {
+	return pool_part_batch(pool, goal, n_chunks, nb, parts, part_stride, part_crc, map, true, bad,
+	                       [&](lzgpu_ctx *ctx, uint32_t count, const uint8_t *const *p, const uint32_t *const *c, lzgpu_stripe_state *o, int64_t *b) {
+		return lzgpu_check_stripe_map_degraded(ctx, goal, count, nb, p, part_stride, c, o, b);
+	});
+}
+
+extern "C" int lzgpu_pool_correct_stripes_degraded(lzgpu_pool *pool, const lzgpu_goal *goal, uint32_t n_chunks, uint32_t nb, uint8_t *const *parts,
+                                                    size_t part_stride, const uint32_t *const *part_crc, lzgpu_stripe_fix *fix, int64_t *bad) {
+	return pool_part_batch(pool, goal, n_chunks, nb, parts, part_stride, part_crc, fix, true, bad,
+	                       [&](lzgpu_ctx *ctx, uint32_t count, uint8_t *const *p, const uint32_t *const *c, lzgpu_stripe_fix *o, int64_t *b) {
+		return lzgpu_correct_stripes_degraded(ctx, goal, count, nb, p, part_stride, c, o, b);
+	});
+}
+
+extern "C" int lzgpu_pool_repair_stripes(lzgpu_pool *pool, const lzgpu_goal *goal, uint32_t n_chunks, uint32_t nb, uint8_t *const *parts,
+                                          size_t part_stride, const uint32_t *const *part_crc, lzgpu_stripe_repair *fix) {
+	return pool_part_batch(pool, goal, n_chunks, nb, parts, part_stride, part_crc, fix, true, nullptr,
+	                       [&](lzgpu_ctx *ctx, uint32_t count, uint8_t *const *p, const uint32_t *const *c, lzgpu_stripe_repair *o, int64_t *) {
+		return lzgpu_repair_stripes(ctx, goal, count, nb, p, part_stride, c, o);
+	});
+}
+
+extern "C" int lzgpu_pool_decode_stripes(lzgpu_pool *pool, const lzgpu_goal *goal, uint32_t n_chunks, uint32_t nb, uint8_t *const *parts,
+                                          size_t part_stride, const uint32_t *const *part_crc, lzgpu_stripe_decode *fix) {
+	return pool_part_batch(pool, goal, n_chunks, nb, parts, part_stride, part_crc, fix, true, nullptr,
+	                       [&](lzgpu_ctx *ctx, uint32_t count, uint8_t *const *p, const uint32_t *const *c, lzgpu_stripe_decode *o, int64_t *) {
+		return lzgpu_decode_stripes(ctx, goal, count, nb, p, part_stride, c, o);
+	});
+}
+
+// The scrub calls of a context also take device memory of its device; one device's memory cannot go to another device's context,
+// so the pool refuses it before any share runs.  Asked on slot 0's device, so that no other device gets a context.
+static int host_memory_only(lzgpu_pool *pool, const char *name, const void *a, const void *b) {
+	int prev = 0;
+	cudaGetDevice(&prev);
+	cudaSetDevice(pool->workers[0]->ctx->device);
+	bool device = false;
+	for (const void *p : {a, b}) {
+		cudaPointerAttributes attr;
+		if (p && cudaPointerGetAttributes(&attr, p) == cudaSuccess) device |= attr.type == cudaMemoryTypeDevice;
+	}
+	cudaGetLastError();
+	cudaSetDevice(prev);
+	if (!device) return LZGPU_OK;
+	lz_set_error("%s: device memory given; a pool scrubs host memory only", name);
+	return LZGPU_ERR_ARG;
+}
+
+extern "C" int lzgpu_pool_verify_blocks(lzgpu_pool *pool, const uint8_t *data, size_t n_blocks, uint32_t block_len, size_t block_stride,
+                                         const uint32_t *stored_crc, int sparse_rule, int64_t *first_bad) {
+	if (!pool || n_blocks > 0xffffffffull) return LZGPU_ERR_ARG;
+	const int rc = host_memory_only(pool, "pool_verify_blocks", data, stored_crc);
+	if (rc) return rc;
+	return pool_merged(pool, static_cast<uint32_t>(n_blocks), first_bad, 1, [&](lzgpu_ctx *ctx, uint32_t first, uint32_t count, int64_t *b) {
+		return lzgpu_verify_blocks(ctx, data ? data + first * block_stride : nullptr, count, block_len, block_stride,
+		                           stored_crc ? stored_crc + first : nullptr, sparse_rule, b);
+	});
+}
+
+extern "C" int lzgpu_pool_verify_interleaved(lzgpu_pool *pool, const uint8_t *records, size_t n_blocks, int64_t *first_bad) {
+	if (!pool || n_blocks > 0xffffffffull) return LZGPU_ERR_ARG;
+	const int rc = host_memory_only(pool, "pool_verify_interleaved", records, nullptr);
+	if (rc) return rc;
+	return pool_merged(pool, static_cast<uint32_t>(n_blocks), first_bad, 1, [&](lzgpu_ctx *ctx, uint32_t first, uint32_t count, int64_t *b) {
+		return lzgpu_verify_interleaved(ctx, records ? records + first * (4 + size_t(LZGPU_BLOCK_SIZE)) : nullptr, count, b);
+	});
 }
 
 extern "C" void lzgpu_pool_get_stats(lzgpu_pool *pool, lzgpu_stats *out) {

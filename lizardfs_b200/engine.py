@@ -176,6 +176,47 @@ def _convert_chunks(fn, h, src, dst, nb, parts, want, part_crc, with_crc):
     return out, ocrc
 
 
+def _part_batch(fn, h, goal, nb, parts, part_crc, result, attr, in_place=False):
+    # the host-pointer check, map and correction: result(n_chunks, pb) makes the array the call fills, which is returned, and
+    # attached to a ChunkCrcError as `attr`
+    assert len(parts) == goal.k + goal.m
+    pb = (nb + goal.k - 1) // goal.k
+    parts, n, crcs = _host_parts(parts, part_crc, pb, in_place=in_place)
+    out = result(n, pb)
+    bad = (C.c_int64 * 3)(-1, -1, -1)
+    rc = fn(h, C.byref(goal.c), n, nb, _ptr_array(parts), pb * BLOCK_SIZE, crcs, _p(out), bad)
+    _check_crc(rc, _name(fn), bad, **{attr: out})
+    return out
+
+
+def _stripe_fix(fn, h, goal, nb, parts, part_crc, dtype):
+    # the host-pointer repair and decode: the parts are rewritten in place, the entries of `dtype` [n_chunks, pb] are returned
+    # and attached to a ChunkCrcError as .fix
+    assert len(parts) == goal.k + goal.m
+    pb = (nb + goal.k - 1) // goal.k
+    parts, n, crcs = _host_parts(parts, part_crc, pb, in_place=True)
+    out = np.empty((n, pb), dtype=dtype)
+    rc = fn(h, C.byref(goal.c), n, nb, _ptr_array(parts), pb * BLOCK_SIZE, crcs, _p(out))
+    _check_crc(rc, _name(fn), (-1, -1, -1), fix=out)
+    return out
+
+
+def _verify_blocks(fn, h, data, stored_crc, block_len, sparse_rule):
+    data = _u8(data).reshape(-1)
+    stored = np.ascontiguousarray(stored_crc, dtype=np.uint32)
+    bad = C.c_int64(-1)
+    rc = fn(h, _p(data), stored.size, block_len, block_len, _p(stored), int(sparse_rule), C.byref(bad))
+    _check_crc(rc, _name(fn), (bad.value,))
+
+
+def _verify_interleaved(fn, h, records):
+    records = _u8(records).reshape(-1)
+    n = records.size // (4 + BLOCK_SIZE)
+    bad = C.c_int64(-1)
+    rc = fn(h, _p(records), n, C.byref(bad))
+    _check_crc(rc, _name(fn), (bad.value,))
+
+
 # ------------------------------------------------------------------------------------------------
 # goals / slice types
 # ------------------------------------------------------------------------------------------------
@@ -384,6 +425,41 @@ class Pool:
         _check(self.lib.lzgpu_pool_crc_blocks(self.h, _p(data), data.shape[0], block_len, block_len, _p(out)), "pool_crc_blocks")
         return out
 
+    # the chunkserver's stripe consistency job and block scrub: the Engine methods of the same names over every device of the pool,
+    # the same arguments, results and errors for the whole batch (lzgpu_pool_check_stripes ... in include/lzgpu.h)
+    def check_stripes(self, goal, nb, parts, part_crc=None):
+        return _part_batch(self.lib.lzgpu_pool_check_stripes, self.h, goal, nb, parts, part_crc,
+                           lambda n, pb: np.empty(n, dtype=Engine.VERDICT_DTYPE), "verdict")
+
+    def check_stripe_map(self, goal, nb, parts, part_crc=None):
+        return _part_batch(self.lib.lzgpu_pool_check_stripe_map, self.h, goal, nb, parts, part_crc,
+                           lambda n, pb: np.empty((n, pb), dtype=Engine.STRIPE_STATE_DTYPE), "map")
+
+    def correct_stripes(self, goal, nb, parts, part_crc=None):
+        return _part_batch(self.lib.lzgpu_pool_correct_stripes, self.h, goal, nb, parts, part_crc,
+                           lambda n, pb: np.empty((n, pb), dtype=Engine.STRIPE_FIX_DTYPE), "fix", in_place=True)
+
+    def check_stripe_map_degraded(self, goal, nb, parts, part_crc=None):
+        return _part_batch(self.lib.lzgpu_pool_check_stripe_map_degraded, self.h, goal, nb, parts, part_crc,
+                           lambda n, pb: np.empty((n, pb), dtype=Engine.STRIPE_STATE_DTYPE), "map")
+
+    def correct_stripes_degraded(self, goal, nb, parts, part_crc=None):
+        return _part_batch(self.lib.lzgpu_pool_correct_stripes_degraded, self.h, goal, nb, parts, part_crc,
+                           lambda n, pb: np.empty((n, pb), dtype=Engine.STRIPE_FIX_DTYPE), "fix", in_place=True)
+
+    def repair_stripes(self, goal, nb, parts, part_crc):
+        return _stripe_fix(self.lib.lzgpu_pool_repair_stripes, self.h, goal, nb, parts, part_crc, Engine.STRIPE_REPAIR_DTYPE)
+
+    def decode_stripes(self, goal, nb, parts, part_crc):
+        return _stripe_fix(self.lib.lzgpu_pool_decode_stripes, self.h, goal, nb, parts, part_crc, Engine.STRIPE_DECODE_DTYPE)
+
+    def verify_blocks(self, data, stored_crc, block_len=BLOCK_SIZE, sparse_rule=False):
+        """host memory only: the pool refuses device pointers (ERR_ARG)"""
+        _verify_blocks(self.lib.lzgpu_pool_verify_blocks, self.h, data, stored_crc, block_len, sparse_rule)
+
+    def verify_interleaved(self, records):
+        _verify_interleaved(self.lib.lzgpu_pool_verify_interleaved, self.h, records)
+
 
 class ReedSolomon:
     """Mirror of ReedSolomon<32,32> (src/common/reed_solomon.h:41-155)."""
@@ -570,35 +646,12 @@ class Engine:
                 bad, stream)
         _check_crc(rc, _name(fn), bad)
 
-    def _part_batch(self, fn, goal, nb, parts, part_crc, result, attr, in_place=False):
-        # the host-pointer check, map and correction: result(n_chunks, pb) makes the array the call fills, which is returned, and
-        # attached to a ChunkCrcError as `attr`
-        assert len(parts) == goal.k + goal.m
-        pb = (nb + goal.k - 1) // goal.k
-        parts, n, crcs = _host_parts(parts, part_crc, pb, in_place=in_place)
-        out = result(n, pb)
-        bad = (C.c_int64 * 3)(-1, -1, -1)
-        rc = fn(self.h, C.byref(goal.c), n, nb, _ptr_array(parts), pb * BLOCK_SIZE, crcs, _p(out), bad)
-        _check_crc(rc, _name(fn), bad, **{attr: out})
-        return out
-
     def _stripe_fix_dev(self, fn, goal, n_chunks, nb, d_parts, part_stride, d_part_crc, d_fix, stream):
         # the device-pointer repair and decode: the check's arguments without `bad`, as the call only enqueues
         n_parts = goal.k + goal.m
         rc = fn(self.h, C.byref(goal.c), n_chunks, nb, _dev_ptrs(d_parts, n_parts), part_stride, _dev_ptrs(d_part_crc, n_parts), d_fix,
                 stream)
         _check(rc, _name(fn))
-
-    def _stripe_fix(self, fn, goal, nb, parts, part_crc, dtype):
-        # the host-pointer repair and decode: the parts are rewritten in place, the entries of `dtype` [n_chunks, pb] are returned
-        # and attached to a ChunkCrcError as .fix
-        assert len(parts) == goal.k + goal.m
-        pb = (nb + goal.k - 1) // goal.k
-        parts, n, crcs = _host_parts(parts, part_crc, pb, in_place=True)
-        out = np.empty((n, pb), dtype=dtype)
-        rc = fn(self.h, C.byref(goal.c), n, nb, _ptr_array(parts), pb * BLOCK_SIZE, crcs, _p(out))
-        _check_crc(rc, _name(fn), (-1, -1, -1), fix=out)
-        return out
 
     # ---- stripe check ------------------------------------------------------------------------
     VERDICT_DTYPE = np.dtype([("first_bad_stripe", np.int32), ("bad_rows", np.uint32), ("suspect_part", np.int32)])
@@ -609,8 +662,8 @@ class Engine:
         Returns the verdicts, a structured array [n_chunks] of VERDICT_DTYPE (first_bad_stripe, bad_rows, suspect_part; -1 = none),
         whether or not any chunk is inconsistent; raises ChunkCrcError on a stored-CRC mismatch (its .verdict holds the verdicts,
         which are written for every chunk all the same)."""
-        return self._part_batch(self.lib.lzgpu_check_stripes, goal, nb, parts, part_crc,
-                                lambda n, pb: np.empty(n, dtype=self.VERDICT_DTYPE), "verdict")
+        return _part_batch(self.lib.lzgpu_check_stripes, self.h, goal, nb, parts, part_crc,
+                           lambda n, pb: np.empty(n, dtype=self.VERDICT_DTYPE), "verdict")
 
     def check_stripes_dev(self, goal, n_chunks, nb, d_parts, part_stride, d_part_crc, d_verdict, stream=None):
         """Device-pointer stripe check: the verdicts go to d_verdict (n_chunks x 12 bytes, device memory).  With d_part_crc the
@@ -624,8 +677,8 @@ class Engine:
         structured array [n_chunks, pb] of STRIPE_STATE_DTYPE (bad_rows, 0 = a codeword; suspect_part, -1 = none), whether or not
         any stripe is bad; raises ChunkCrcError on a stored-CRC mismatch (its .map holds the map, written in full all the same).
         For each chunk the lowest bad stripe and its entry equal check_stripes' verdict."""
-        return self._part_batch(self.lib.lzgpu_check_stripe_map, goal, nb, parts, part_crc,
-                                lambda n, pb: np.empty((n, pb), dtype=self.STRIPE_STATE_DTYPE), "map")
+        return _part_batch(self.lib.lzgpu_check_stripe_map, self.h, goal, nb, parts, part_crc,
+                           lambda n, pb: np.empty((n, pb), dtype=self.STRIPE_STATE_DTYPE), "map")
 
     def check_stripe_map_dev(self, goal, n_chunks, nb, d_parts, part_stride, d_part_crc, d_map, stream=None):
         """Device-pointer stripe map: n_chunks * pb entries of 8 bytes go to d_map (device memory).  With d_part_crc the call waits
@@ -641,8 +694,8 @@ class Engine:
         pb] of STRIPE_FIX_DTYPE (bad_rows and suspect_part as the map had them before the call; status = _lib.FIX_*; crc of the
         corrected block), whether or not a stripe is left bad; raises ChunkCrcError on a stored-CRC mismatch (its .fix holds the
         entries, written in full all the same, and the corrections the rule allowed are made)."""
-        return self._part_batch(self.lib.lzgpu_correct_stripes, goal, nb, parts, part_crc,
-                                lambda n, pb: np.empty((n, pb), dtype=self.STRIPE_FIX_DTYPE), "fix", in_place=True)
+        return _part_batch(self.lib.lzgpu_correct_stripes, self.h, goal, nb, parts, part_crc,
+                           lambda n, pb: np.empty((n, pb), dtype=self.STRIPE_FIX_DTYPE), "fix", in_place=True)
 
     def correct_stripes_dev(self, goal, n_chunks, nb, d_parts, part_stride, d_part_crc, d_fix, stream=None):
         """Device-pointer stripe correction: the corrected blocks are written into d_parts, n_chunks * pb entries of 16 bytes go to
@@ -655,8 +708,8 @@ class Engine:
         parts and part_crc as in check_stripe_map, but any part may be None as long as k + 1 are given: the first k given parts are
         the inputs, the others (parity parts) are checked against their re-encoding from the inputs, and bad_rows bit r is spare part
         k + r.  With every data part given the result is check_stripe_map's."""
-        return self._part_batch(self.lib.lzgpu_check_stripe_map_degraded, goal, nb, parts, part_crc,
-                                lambda n, pb: np.empty((n, pb), dtype=self.STRIPE_STATE_DTYPE), "map")
+        return _part_batch(self.lib.lzgpu_check_stripe_map_degraded, self.h, goal, nb, parts, part_crc,
+                           lambda n, pb: np.empty((n, pb), dtype=self.STRIPE_STATE_DTYPE), "map")
 
     def check_stripe_map_degraded_dev(self, goal, n_chunks, nb, d_parts, part_stride, d_part_crc, d_map, stream=None):
         """Device-pointer form of check_stripe_map_degraded, as check_stripe_map_dev"""
@@ -666,8 +719,8 @@ class Engine:
     def correct_stripes_degraded(self, goal, nb, parts, part_crc=None):
         """correct_stripes on the map of check_stripe_map_degraded (lzgpu_correct_stripes_degraded): every stripe that names a
         suspect has its block rewritten in place from the first k given parts other than it; a missing part is never written"""
-        return self._part_batch(self.lib.lzgpu_correct_stripes_degraded, goal, nb, parts, part_crc,
-                                lambda n, pb: np.empty((n, pb), dtype=self.STRIPE_FIX_DTYPE), "fix", in_place=True)
+        return _part_batch(self.lib.lzgpu_correct_stripes_degraded, self.h, goal, nb, parts, part_crc,
+                           lambda n, pb: np.empty((n, pb), dtype=self.STRIPE_FIX_DTYPE), "fix", in_place=True)
 
     def correct_stripes_degraded_dev(self, goal, n_chunks, nb, d_parts, part_stride, d_part_crc, d_fix, stream=None):
         """Device-pointer form of correct_stripes_degraded, as correct_stripes_dev"""
@@ -683,7 +736,7 @@ class Engine:
         of STRIPE_REPAIR_DTYPE (crc_failed: bit p = the block of part p failed its stored CRC before the call; status = _lib.FIX_*,
         REBUILT and CRC_ONLY included), whether or not a stripe is left bad; raises ChunkCrcError when a block still fails its stored
         CRC after the call (its .fix holds the entries, and every repair the rule allowed is made)."""
-        return self._stripe_fix(self.lib.lzgpu_repair_stripes, goal, nb, parts, part_crc, self.STRIPE_REPAIR_DTYPE)
+        return _stripe_fix(self.lib.lzgpu_repair_stripes, self.h, goal, nb, parts, part_crc, self.STRIPE_REPAIR_DTYPE)
 
     def repair_stripes_dev(self, goal, n_chunks, nb, d_parts, part_stride, d_part_crc, d_fix, stream=None):
         """Device-pointer form of repair_stripes: the rewritten blocks go into d_parts, n_chunks * pb entries of 24 bytes to d_fix
@@ -699,7 +752,7 @@ class Engine:
         Returns a structured array [n_chunks, pb] of STRIPE_DECODE_DTYPE (the first five fields as repair_stripes returns them unless
         status == _lib.FIX_DECODED; located: bit p = part p's block was located and rewritten; located_crc: their new CRCs,
         ascending part); raises ChunkCrcError when a block still fails its stored CRC after the call (its .fix holds the entries)."""
-        return self._stripe_fix(self.lib.lzgpu_decode_stripes, goal, nb, parts, part_crc, self.STRIPE_DECODE_DTYPE)
+        return _stripe_fix(self.lib.lzgpu_decode_stripes, self.h, goal, nb, parts, part_crc, self.STRIPE_DECODE_DTYPE)
 
     def decode_stripes_dev(self, goal, n_chunks, nb, d_parts, part_stride, d_part_crc, d_fix, stream=None):
         """Device-pointer form of decode_stripes: the rewritten blocks go into d_parts, n_chunks * pb entries of 40 bytes to d_fix
@@ -835,19 +888,11 @@ class Engine:
         _check(self.lib.lzgpu_crc_blocks_dev(self.h, d_data, n_blocks, block_len, block_stride, d_out, stream), "crc_blocks_dev")
 
     def verify_blocks(self, data, stored_crc, block_len=BLOCK_SIZE, sparse_rule=False):
-        data = _u8(data).reshape(-1)
-        stored = np.ascontiguousarray(stored_crc, dtype=np.uint32)
-        bad = C.c_int64(-1)
-        rc = self.lib.lzgpu_verify_blocks(self.h, _p(data), stored.size, block_len, block_len, _p(stored), int(sparse_rule), C.byref(bad))
-        _check_crc(rc, "verify_blocks", (bad.value,))
+        _verify_blocks(self.lib.lzgpu_verify_blocks, self.h, data, stored_crc, block_len, sparse_rule)
 
     def verify_interleaved(self, records):
         """records: on-disk layout, n x (4-byte big-endian CRC + 65536 data bytes) (chunk.h:40)."""
-        records = _u8(records).reshape(-1)
-        n = records.size // (4 + BLOCK_SIZE)
-        bad = C.c_int64(-1)
-        rc = self.lib.lzgpu_verify_interleaved(self.h, _p(records), n, C.byref(bad))
-        _check_crc(rc, "verify_interleaved", (bad.value,))
+        _verify_interleaved(self.lib.lzgpu_verify_interleaved, self.h, records)
 
     def verify_interleaved_ptr(self, ptr, n_blocks):
         """same, `ptr` = raw address of the records: host memory or a device buffer of this engine's device"""
