@@ -292,7 +292,8 @@ enum {
 	LZGPU_KERNEL_CONVERT = 8,          /* fused_convert_kernel: one-pass slice conversion */
 	LZGPU_KERNEL_CHECK = 9,            /* fused_check_kernel: stripe check (lzgpu_check_stripes), one 16-warp CTA per SM */
 	LZGPU_KERNEL_CHECK_DEGRADED = 10,  /* fused_check_degraded_kernel: stripe map with lost data parts (lzgpu_check_stripe_map_degraded) */
-	LZGPU_KERNEL_ENCODE_SLICES = 11    /* fused_slices_kernel: one-pass encode for several slices (lzgpu_encode_slices); G = combined stripes */
+	LZGPU_KERNEL_ENCODE_SLICES = 11,   /* fused_slices_kernel: one-pass encode for several slices (lzgpu_encode_slices); G = combined stripes */
+	LZGPU_KERNEL_RECOVER_SLICES = 12   /* recover_slices_kernel: recovery from the parts of every slice (lzgpu_recover_slices); G = combined stripes */
 };
 typedef struct lzgpu_launch_geometry {
 	int kernel;
@@ -380,6 +381,63 @@ int lzgpu_encode_slices_dev(lzgpu_ctx *ctx, const lzgpu_goal *goals, uint32_t n_
 int lzgpu_pool_encode_slices(lzgpu_pool *pool, const lzgpu_goal *goals, uint32_t n_slices, uint32_t n_chunks, uint32_t chunk_len,
                              const uint8_t *data, size_t chunk_stride,
                              uint8_t *const *parity, const size_t *parity_stride, uint32_t *const *crc, const size_t *crc_stride);
+
+/* Recover a chunk of a multi-slice goal from the surviving parts of ALL its slices together, and rebuild every lost part of every
+ * slice in the same pass.  The reference scores each slice on its own (ChunkCopiesCalculator::evalRedundancyLevel,
+ * chunk_copies_calculator.cc:224-246): a chunk is lost once every slice holds fewer than k distinct parts.  But every slice stores the
+ * same chunk bytes: a data block missing from one slice may be held by a data part of another, or pinned down by the parity equations
+ * of several slices together.  With xor2 + xor3, for example, xor2 parts 0, 1 and xor3 parts 0, 2 determine every block.
+ *   goals, n_slices   1..4 xor/ec goals or the standard slice {LZGPU_KIND_STD,1,0}, at least one xor/ec, as in lzgpu_encode_slices;
+ *                     L = lcm of their k.  A repeated slice type, L > 64 or more than 64 parts in all: LZGPU_ERR_ARG.
+ *   flat parts        slice i's parts follow those of slices 0 .. i-1: k_i + m_i per slice (data first), one for a standard slice.
+ *                     parts, part_crc, want, out and out_crc are indexed by this flat number g.
+ *   parts[g]          part-major buffer of part g, chunk c at + c * part_stride[slice of g], pb_i = ceil(nb / k_i) blocks (short parts
+ *                     zero-padded; a standard part holds the nb blocks in chunk order); NULL = lost.  part_stride / out_stride: one
+ *                     entry per slice.  Layout, zero padding, alignment (_dev: 16-byte buffers and strides, 4-byte CRC arrays) and the
+ *                     CRC-disabled mode as in lzgpu_recover_chunks.
+ *   part_crc[g]       stored CRCs of a given part (chunk c at + c * pb_i), or NULL / part_crc == NULL: not verified.  Every block of
+ *                     every given part with stored CRCs is verified in the same pass; a mismatch returns LZGPU_ERR_CRC with bad[0..3] =
+ *                     the smallest (chunk, slice, part in the slice, block), and the outputs are then undefined.  In deferred mode
+ *                     lzgpu_last_bad reports (chunk, flat part, block).
+ *   want[g]           any part that is not given (LZGPU_ERR_ARG for a given one): out[g] (chunk c at + c * out_stride[slice]) receives
+ *                     what lzgpu_encode_slices / lzgpu_split_chunks write for the original chunk, out_crc[g] (optional, chunk c at
+ *                     + c * pb_i) its block CRCs (the CRC of zeros for a padding block).
+ *   chunk_out         optional chunk-order image of nb blocks, chunk c at + c * chunk_out_stride.
+ * If a block the call must write is not determined by the given parts (lzgpu_plan_recover_slices; a wanted parity part needs every data
+ * block of its stripes), the call returns LZGPU_ERR_TOO_FEW_PARTS before anything is enqueued.  When one slice alone has k given parts
+ * the bytes equal what lzgpu_convert_chunks writes from that slice.  Stale inputs (valid CRC, wrong bytes) are not detected: the stripe
+ * calls are the tool for that.  There is one route, recover_slices_kernel (LZGPU_DISABLE_FUSED does not apply; LZGPU_GRID_CAP does),
+ * reported by lzgpu_debug_last_geometry as LZGPU_KERNEL_RECOVER_SLICES; a goal set whose largest request does not fit the kernel's
+ * shared memory (more than 192 blocks or 64 parity blocks per combined stripe) returns LZGPU_ERR_ARG, as the plan says (ok = 0). */
+typedef struct lzgpu_slices_recover_plan {
+	uint64_t known;            /* bit q: combined-stripe position q is held by a given data part of some slice */
+	uint64_t determined;       /* known, plus the positions solved from the given parity blocks */
+	uint64_t tail_determined;  /* the same for the chunk's last, partial combined stripe (positions at or past nb are known zeros and
+	                              set); equal to determined when L divides nb */
+	uint32_t L;                /* blocks per combined stripe */
+	uint32_t tail_blocks;      /* chunk blocks in the last combined stripe when L does not divide nb, else 0 */
+	uint32_t unknowns, equations;            /* full stripe: positions not known; independent equations the solve uses (<= unknowns) */
+	uint32_t tail_unknowns, tail_equations;  /* the same for the tail stripe (0 without one) */
+	int ok;                    /* 1: the kernel takes this goal set with these given parts */
+	uint32_t G, threads, stages, smem_bytes; /* launch geometry, as lzgpu_debug_last_geometry reports it */
+} lzgpu_slices_recover_plan;
+int lzgpu_plan_recover_slices(const lzgpu_goal *goals, uint32_t n_slices, uint32_t nb, const uint8_t *given, lzgpu_slices_recover_plan *out);
+int lzgpu_recover_slices(lzgpu_ctx *ctx, const lzgpu_goal *goals, uint32_t n_slices, uint32_t n_chunks, uint32_t nb,
+                         const uint8_t *const *parts, const size_t *part_stride, const uint32_t *const *part_crc,
+                         const uint8_t *want, uint8_t *const *out, const size_t *out_stride, uint32_t *const *out_crc,
+                         uint8_t *chunk_out, size_t chunk_out_stride, int64_t *bad /* [4] */);
+int lzgpu_recover_slices_dev(lzgpu_ctx *ctx, const lzgpu_goal *goals, uint32_t n_slices, uint32_t n_chunks, uint32_t nb,
+                             const void *const *d_parts, const size_t *part_stride, const void *const *d_part_crc,
+                             const uint8_t *want, void *const *d_out, const size_t *out_stride, void *const *d_out_crc,
+                             void *d_chunk_out, size_t chunk_out_stride, int64_t *bad /* host, [4] */, void *stream);
+/* The host build of the solve (csrc/slices_solve.h) for one stripe shape: positions < valid are chunk blocks, the rest known zeros
+ * (valid = L: a full combined stripe).  unk_pos[x] (x < *n_unknowns): the unknown positions, ascending; equation e (e < *n_equations):
+ * parity row eq_row[e] of slice eq_slice[e], over that slice's stripe eq_stripe[e] of the combined stripe; rows[64 x + e]: the
+ * coefficient of equation e's syndrome (the given parity block minus the known positions' share) in unknown x, all zero when x is not
+ * determined; *determined as in lzgpu_slices_recover_plan.  Arrays of 64 entries (rows: 64 x 64).  LZGPU_ERR_ARG for bad arguments. */
+int lzgpu_debug_recover_slices_rows(const lzgpu_goal *goals, uint32_t n_slices, const uint8_t *given, uint32_t valid, uint32_t *n_unknowns,
+                                    uint32_t *n_equations, uint8_t *unk_pos, uint8_t *eq_slice, uint8_t *eq_row, uint8_t *eq_stripe,
+                                    uint8_t *rows, uint64_t *determined);
 
 /* Degraded read / rebuild of n_chunks chunks.
  *   parts[i]    (i < k+m) part-major buffer of part i for all chunks: chunk c at + c*part_stride,

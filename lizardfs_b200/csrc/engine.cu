@@ -19,6 +19,7 @@
 #include "host_math.h"
 #include "correct_kernel.cuh"
 #include "fused_plan.h"
+#include "slices_solve.h"
 #include "kernels_generic.cuh"
 #include "lzgpu.h"
 
@@ -2140,6 +2141,236 @@ extern "C" int lzgpu_convert_chunks(lzgpu_ctx *ctx, const lzgpu_goal *src, const
 		}
 		return LZGPU_OK;
 	});
+}
+
+// ------------------------------------------------------------------------------------------------
+// recovery from the parts of every slice of a goal together (lzgpu_recover_slices*)
+// ------------------------------------------------------------------------------------------------
+// What the argument check derives for the enqueue: the flat part layout, the solve of both stripe shapes and the launch geometry
+struct RecoverSlicesCall {
+	lzd::SliceLayout lay;
+	lzd::SliceSolve shapes[2];   // a full combined stripe, the chunk's last one when L does not divide nb
+	lzd::RsGeometry geo;
+	uint32_t pb[kSlicesMax] = {0};
+};
+
+// The arguments of both forms, checked before anything is enqueued and whatever n_chunks is.  dev: the device form's alignment rules
+// (16-byte buffers and strides, 4-byte CRC arrays).  LZGPU_ERR_TOO_FEW_PARTS when a block the call must write is not determined.
+static int recover_slices_args(const lzgpu_ctx *ctx, const lzgpu_goal *goals, uint32_t n_slices, uint32_t nb, const void *const *parts,
+                               const size_t *part_stride, const void *const *part_crc, const uint8_t *want, const void *const *out,
+                               const size_t *out_stride, const void *const *out_crc, const void *chunk_out, size_t chunk_out_stride, bool dev,
+                               RecoverSlicesCall &c) {
+	if (!ctx || !parts || !part_stride || !want) return LZGPU_ERR_ARG;
+	const char *why = nullptr;
+	if (lzd::slice_layout(goals, n_slices, c.lay, &why)) { lz_set_error("recover_slices: %s", why); return LZGPU_ERR_ARG; }
+	if (nb == 0 || nb > LZGPU_BLOCKS_IN_CHUNK) { lz_set_error("nb out of range"); return LZGPU_ERR_ARG; }
+	const lzd::SliceLayout &lay = c.lay;
+	const size_t B = LZGPU_BLOCK_SIZE;
+	uint8_t given[LZGPU_MAX_PARTS] = {0};
+	for (uint32_t i = 0; i < lay.n_slices; ++i) {
+		c.pb[i] = (nb + lay.k[i] - 1) / lay.k[i];
+		const size_t bytes = static_cast<size_t>(c.pb[i]) * B;
+		for (uint32_t g = lay.base[i]; g < lay.base[i] + lay.k[i] + lay.m[i]; ++g) {
+			given[g] = parts[g] != nullptr;
+			if (given[g] && (part_stride[i] < bytes || (dev && (part_stride[i] & 15)))) {
+				lz_set_error("recover_slices: part_stride[%u] too small or not a multiple of 16", i);
+				return LZGPU_ERR_ARG;
+			}
+			if (!want[g]) continue;
+			if (given[g]) { lz_set_error("recover_slices: part %u is given and wanted", g); return LZGPU_ERR_ARG; }
+			if (!out || !out[g] || !out_stride) { lz_set_error("recover_slices: wanted part %u has no output buffer", g); return LZGPU_ERR_ARG; }
+			if (out_stride[i] < bytes || (dev && (out_stride[i] & 15))) {
+				lz_set_error("recover_slices: out_stride[%u] too small or not a multiple of 16", i);
+				return LZGPU_ERR_ARG;
+			}
+		}
+	}
+	if (chunk_out && (chunk_out_stride < static_cast<size_t>(nb) * B || (dev && (chunk_out_stride & 15)))) {
+		lz_set_error("recover_slices: chunk_out_stride must cover nb blocks (and be a multiple of 16)");
+		return LZGPU_ERR_ARG;
+	}
+	if (dev) {
+		const int n = static_cast<int>(lay.n_parts);
+		int rc;
+		if ((rc = check_part_ptrs("recover_slices", "parts", parts, n, 16)) || (rc = check_part_ptrs("recover_slices", "out", out, n, 16)) ||
+		    (rc = check_part_ptrs("recover_slices", "part_crc", part_crc, n, 4)) || (rc = check_part_ptrs("recover_slices", "out_crc", out_crc, n, 4)))
+			return rc;
+		if (reinterpret_cast<uintptr_t>(chunk_out) & 15) { lz_set_error("recover_slices: chunk_out is not 16-byte aligned"); return LZGPU_ERR_ARG; }
+	}
+	const uint32_t tail = nb % lay.L;
+	lzd::slice_solve(lay, given, lay.L, c.shapes[0]);
+	if (tail) lzd::slice_solve(lay, given, tail, c.shapes[1]);
+	for (int t = 0; t < 2; ++t) {
+		if (t == 0 ? nb < lay.L : tail == 0) continue;   // a shape no chunk of the call has
+		const lzd::SliceSolve &sv = c.shapes[t];
+		const uint64_t lost = lzd::slice_needed(lay, want, chunk_out != nullptr, sv.valid) & ~sv.determined;
+		if (lost) {
+			lz_set_error("recover_slices: positions %#llx of the %s combined stripe are not determined by the given parts",
+			             static_cast<unsigned long long>(lost), t ? "last" : "full");
+			return LZGPU_ERR_TOO_FEW_PARTS;
+		}
+	}
+	const lzd::SliceSolve used[2] = {nb >= lay.L ? c.shapes[0] : c.shapes[1], tail ? c.shapes[1] : c.shapes[0]};
+	c.geo = lzd::rs_geometry(lay, given, used, 2);
+	if (!c.geo.ok) {
+		lz_set_error("recover_slices: a combined stripe has more blocks than the kernel stages (%u slots, %u CRC streams)", c.geo.slots, c.geo.states);
+		return LZGPU_ERR_ARG;
+	}
+	return LZGPU_OK;
+}
+
+// DESIGN.md §4.8: read the given parts (+ their stored CRCs), write the wanted parts (+ their CRCs) and the image
+static uint64_t recover_slices_alg_bytes(const RecoverSlicesCall &c, uint32_t n_chunks, uint32_t nb, const void *const *parts, bool crcs,
+                                         const uint8_t *want, bool out_crcs, bool image) {
+	const uint64_t B = LZGPU_BLOCK_SIZE;
+	uint64_t per_chunk = image ? static_cast<uint64_t>(nb) * B : 0;
+	for (uint32_t i = 0; i < c.lay.n_slices; ++i)
+		for (uint32_t g = c.lay.base[i]; g < c.lay.base[i] + c.lay.k[i] + c.lay.m[i]; ++g) {
+			if (parts[g]) per_chunk += c.pb[i] * (B + (crcs ? 4 : 0));
+			if (want[g]) per_chunk += c.pb[i] * (B + (out_crcs ? 4 : 0));
+		}
+	return n_chunks * per_chunk;
+}
+
+// bad[0..3] = chunk, slice, part of the slice, block from the ticket's chunk, flat part, block
+static void recover_slices_bad(const lzd::SliceLayout &lay, const int64_t *b3, int64_t *bad) {
+	if (!bad || b3[1] < 0) return;
+	const int i = lay.slice_of(static_cast<uint32_t>(b3[1]));
+	bad[0] = b3[0];
+	bad[1] = i;
+	bad[2] = b3[1] - lay.base[i];
+	bad[3] = b3[2];
+}
+
+// one launch; *tk is armed when a given part has stored CRCs (the kernel compares them with the constant while CRCs are disabled)
+static int recover_slices_enqueue(lzgpu_ctx *ctx, const RecoverSlicesCall &c, uint32_t n_chunks, uint32_t nb, const void *const *d_parts,
+                                  const size_t *part_stride, const void *const *d_part_crc, const uint8_t *want, void *const *d_out,
+                                  const size_t *out_stride, void *const *d_out_crc, void *d_chunk_out, size_t chunk_out_stride, cudaStream_t st,
+                                  VerifyTicket *tk) {
+	bool verifying = false;
+	for (uint32_t g = 0; g < c.lay.n_parts; ++g) verifying |= d_parts[g] && d_part_crc && d_part_crc[g];
+	int rc;
+	if (verifying && (rc = tk->arm(ctx, st))) return rc;
+	if ((rc = lz_recover_slices(ctx, c.lay, c.shapes, c.geo, n_chunks, nb, d_parts, part_stride, verifying ? d_part_crc : nullptr, want, d_out,
+	                            out_stride, d_out_crc, d_chunk_out, chunk_out_stride, st, verifying ? tk->word(0) : nullptr)))
+		return rc;
+	ctx->stats.chunks_recovered += n_chunks;
+	return verifying ? tk->publish_fused() : LZGPU_OK;
+}
+
+extern "C" int lzgpu_recover_slices_dev(lzgpu_ctx *ctx, const lzgpu_goal *goals, uint32_t n_slices, uint32_t n_chunks, uint32_t nb,
+                                         const void *const *d_parts, const size_t *part_stride, const void *const *d_part_crc,
+                                         const uint8_t *want, void *const *d_out, const size_t *out_stride, void *const *d_out_crc,
+                                         void *d_chunk_out, size_t chunk_out_stride, int64_t *bad, void *stream) {
+	NvtxScope nvtx_scope("lzgpu::recover_slices_dev");
+	auto c = std::make_unique<RecoverSlicesCall>();
+	int rc = recover_slices_args(ctx, goals, n_slices, nb, d_parts, part_stride, d_part_crc, want, d_out, out_stride, d_out_crc, d_chunk_out,
+	                             chunk_out_stride, true, *c);
+	if (rc || n_chunks == 0) return rc;
+	if (bad) bad[0] = bad[1] = bad[2] = bad[3] = -1;
+	int64_t b3[3] = {-1, -1, -1};
+	rc = dev_call(ctx, stream, recover_slices_alg_bytes(*c, n_chunks, nb, d_parts, d_part_crc != nullptr, want, d_out_crc != nullptr, d_chunk_out != nullptr),
+	              b3, [&](cudaStream_t st, VerifyTicket *tk) {
+		              return recover_slices_enqueue(ctx, *c, n_chunks, nb, d_parts, part_stride, d_part_crc, want, d_out, out_stride, d_out_crc, d_chunk_out,
+		                                            chunk_out_stride, st, tk);
+	              });
+	if (rc == LZGPU_ERR_CRC) recover_slices_bad(c->lay, b3, bad);
+	return rc;
+}
+
+extern "C" int lzgpu_recover_slices(lzgpu_ctx *ctx, const lzgpu_goal *goals, uint32_t n_slices, uint32_t n_chunks, uint32_t nb,
+                                     const uint8_t *const *parts, const size_t *part_stride, const uint32_t *const *part_crc, const uint8_t *want,
+                                     uint8_t *const *out, const size_t *out_stride, uint32_t *const *out_crc, uint8_t *chunk_out,
+                                     size_t chunk_out_stride, int64_t *bad) {
+	NvtxScope nvtx_scope("lzgpu::recover_slices");
+	auto c = std::make_unique<RecoverSlicesCall>();
+	int rc = recover_slices_args(ctx, goals, n_slices, nb, reinterpret_cast<const void *const *>(parts), part_stride,
+	                             reinterpret_cast<const void *const *>(part_crc), want, reinterpret_cast<const void *const *>(out), out_stride,
+	                             reinterpret_cast<const void *const *>(out_crc), chunk_out, chunk_out_stride, false, *c);
+	if (rc || n_chunks == 0) return rc;
+	if (bad) bad[0] = bad[1] = bad[2] = bad[3] = -1;
+	const lzd::SliceLayout &lay = c->lay;
+	const uint32_t n = lay.n_parts;
+	const size_t B = LZGPU_BLOCK_SIZE;
+	// device layout of a tile: every given part, then every wanted part, then the image, each dense (tile chunks of pb_i blocks); the
+	// stored and the computed CRCs likewise
+	size_t off[LZGPU_MAX_PARTS] = {0}, crc_off[LZGPU_MAX_PARTS] = {0}, bytes[LZGPU_MAX_PARTS] = {0}, per_chunk = 0, crc_words = 0;
+	size_t dstride[kSlicesMax] = {0};
+	for (uint32_t g = 0; g < n; ++g) {
+		const int i = lay.slice_of(g);
+		dstride[i] = static_cast<size_t>(c->pb[i]) * B;
+		if (!parts[g] && !want[g]) continue;
+		bytes[g] = dstride[i];
+		off[g] = per_chunk;
+		per_chunk += bytes[g];
+		if ((parts[g] && part_crc && part_crc[g]) || (want[g] && out_crc && out_crc[g])) {
+			crc_off[g] = crc_words;
+			crc_words += c->pb[i];
+		}
+	}
+	const size_t img_off = per_chunk, img_bytes = chunk_out ? static_cast<size_t>(nb) * B : 0;
+	per_chunk += img_bytes;
+	std::lock_guard<std::mutex> lk(ctx->mu);
+	DeviceGuard dg(ctx->device);
+	AutoPin pin(ctx);
+	for (uint32_t g = 0; g < n; ++g) {
+		const int i = lay.slice_of(g);
+		if (parts[g]) pin.add(parts[g], static_cast<size_t>(n_chunks - 1) * part_stride[i] + bytes[g]);
+		if (want[g]) pin.add(out[g], static_cast<size_t>(n_chunks - 1) * out_stride[i] + bytes[g]);
+	}
+	if (chunk_out) pin.add(chunk_out, static_cast<size_t>(n_chunks - 1) * chunk_out_stride + img_bytes);
+	const uint32_t tile = static_cast<uint32_t>(std::max<size_t>(1, std::min<size_t>(n_chunks, (2 * kHostTileBytes) / std::max<size_t>(per_chunk, 1))));
+	const int n_slots = n_chunks > tile ? kHostSlots : 1;
+	void *d_in[kHostSlots], *d_crc[kHostSlots];
+	for (int s = 0; s < n_slots; ++s)
+		if ((rc = lz_scratch(ctx, kScratchIn0 + s, tile * per_chunk, &d_in[s])) ||
+		    (rc = lz_scratch(ctx, kScratchCrc0 + s, tile * std::max<size_t>(crc_words, 1) * 4, &d_crc[s])))
+			return rc;
+	int64_t b3[3] = {-1, -1, -1};
+	rc = run_tiles(ctx, n_chunks, tile, n_slots, b3, [&](int s, size_t c0, size_t nc, cudaStream_t st, VerifyTicket *tk) -> int {
+		void *dp[LZGPU_MAX_PARTS] = {nullptr}, *dpc[LZGPU_MAX_PARTS] = {nullptr}, *dout[LZGPU_MAX_PARTS] = {nullptr}, *docrc[LZGPU_MAX_PARTS] = {nullptr};
+		bool any_crc = false;
+		for (uint32_t g = 0; g < n; ++g) {
+			const int i = lay.slice_of(g);
+			uint8_t *buf = static_cast<uint8_t *>(d_in[s]) + tile * off[g];
+			uint32_t *cbuf = static_cast<uint32_t *>(d_crc[s]) + tile * crc_off[g];
+			if (parts[g]) {
+				CUDA_TRY(cudaMemcpy2DAsync(buf, bytes[g], parts[g] + c0 * part_stride[i], part_stride[i], bytes[g], nc, cudaMemcpyHostToDevice, st));
+				ctx->stats.bytes_h2d += nc * bytes[g];
+				dp[g] = buf;
+				if (part_crc && part_crc[g]) {
+					CUDA_TRY(cudaMemcpyAsync(cbuf, part_crc[g] + c0 * c->pb[i], nc * c->pb[i] * 4, cudaMemcpyHostToDevice, st));
+					dpc[g] = cbuf;
+					any_crc = true;
+				}
+			} else if (want[g]) {
+				dout[g] = buf;
+				if (out_crc && out_crc[g]) docrc[g] = cbuf;
+			}
+		}
+		void *dimg = chunk_out ? static_cast<uint8_t *>(d_in[s]) + tile * img_off : nullptr;
+		int rc;
+		{
+			BatchTimer timer(ctx, st, recover_slices_alg_bytes(*c, static_cast<uint32_t>(nc), nb, dp, any_crc, want, out_crc != nullptr, chunk_out != nullptr));
+			rc = recover_slices_enqueue(ctx, *c, static_cast<uint32_t>(nc), nb, dp, dstride, any_crc ? dpc : nullptr, want, dout, dstride,
+			                            out_crc ? docrc : nullptr, dimg, img_bytes, st, tk);
+		}
+		if (rc) return rc;
+		for (uint32_t g = 0; g < n; ++g) {
+			if (!want[g]) continue;
+			const int i = lay.slice_of(g);
+			CUDA_TRY(cudaMemcpy2DAsync(out[g] + c0 * out_stride[i], out_stride[i], dout[g], bytes[g], bytes[g], nc, cudaMemcpyDeviceToHost, st));
+			ctx->stats.bytes_d2h += nc * bytes[g];
+			if (docrc[g]) CUDA_TRY(cudaMemcpyAsync(out_crc[g] + c0 * c->pb[i], docrc[g], nc * c->pb[i] * 4, cudaMemcpyDeviceToHost, st));
+		}
+		if (chunk_out) {
+			CUDA_TRY(cudaMemcpy2DAsync(chunk_out + c0 * chunk_out_stride, chunk_out_stride, dimg, img_bytes, img_bytes, nc, cudaMemcpyDeviceToHost, st));
+			ctx->stats.bytes_d2h += nc * img_bytes;
+		}
+		return LZGPU_OK;
+	});
+	if (rc == LZGPU_ERR_CRC) recover_slices_bad(lay, b3, bad);
+	return rc;
 }
 
 // ------------------------------------------------------------------------------------------------

@@ -206,6 +206,18 @@ int lz_fused_check(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, ui
 int lz_fused_encode_slices(lzgpu_ctx *ctx, const lzgpu_goal *goals, uint32_t n_slices, uint32_t n_chunks, uint32_t nb, const void *d_data,
                            size_t chunk_stride, void *const *d_parity, const size_t *parity_stride, void *const *d_crc, const size_t *crc_stride,
                            cudaStream_t st);
+// Recovery from the parts of every slice together (recover_slices_kernel.cuh): the one launch of lzgpu_recover_slices*, whose arguments,
+// solve (shapes[0] a full combined stripe, shapes[1] the tail) and geometry the caller has checked.  d_first_bad: the armed result word
+// whenever d_part_crc is given.
+namespace lzd {
+struct SliceLayout;
+struct SliceSolve;
+struct RsGeometry;
+}  // namespace lzd
+int lz_recover_slices(lzgpu_ctx *ctx, const lzd::SliceLayout &lay, const lzd::SliceSolve *shapes, const lzd::RsGeometry &geo, uint32_t n_chunks,
+                      uint32_t nb, const void *const *d_parts, const size_t *part_stride, const void *const *d_part_crc, const uint8_t *want,
+                      void *const *d_out, const size_t *out_stride, void *const *d_out_crc, void *d_image, size_t image_stride, cudaStream_t st,
+                      unsigned long long *d_first_bad);
 // CRC of 64 KiB blocks: block (c, b) at base + c*chunk_stride + b*65536, out[c*out_chunk_stride + b]
 int lz_fused_crc(lzgpu_ctx *ctx, const void *base, unsigned long long n_blocks, unsigned long long blocks_per_chunk,
                  unsigned long long chunk_stride, void *out, unsigned long long out_chunk_stride, cudaStream_t st);

@@ -9,6 +9,7 @@
 #include <numeric>
 #include <cstdlib>
 #include <cstring>
+#include <memory>
 #include <mutex>
 
 #include "engine_internal.h"
@@ -17,6 +18,7 @@
 #include "bs_recover_kernel.cuh"
 #include "check_kernel.cuh"
 #include "slices_kernel.cuh"
+#include "recover_slices_kernel.cuh"
 #include "host_math.h"
 
 using namespace lzd;
@@ -306,6 +308,10 @@ static const struct {
 	SlicesKernel fn;
 } kSlicers[] = {{1, fused_slices_kernel<1>}, {2, fused_slices_kernel<2>}, {3, fused_slices_kernel<3>}, {4, fused_slices_kernel<4>}};
 
+// Recovery from the parts of every slice together (recover_slices_kernel): one instantiation, any goal set
+using RecoverSlicesKernel = void (*)(RecoverSlicesParams);
+static const RecoverSlicesKernel kRecoverSlicers[] = {recover_slices_kernel};
+
 // function attributes are per device: set once per context
 static int set_all_smem_attrs(const FusedState *fs) {
 	int rc;
@@ -326,6 +332,8 @@ static int set_all_smem_attrs(const FusedState *fs) {
 		if ((rc = set_smem(k.fn, kSmemCap))) return rc;
 	for (const auto &k : kSlicers)
 		if ((rc = set_smem(k.fn, kSlicesSmemCap))) return rc;
+	for (const RecoverSlicesKernel k : kRecoverSlicers)
+		if ((rc = set_smem(k, static_cast<int>(kRsSmemCap)))) return rc;
 	return LZGPU_OK;
 }
 
@@ -896,4 +904,116 @@ int lz_fused_encode_slices(lzgpu_ctx *ctx, const lzgpu_goal *goals, uint32_t n_s
 		if (k.m == pl.m)
 			return launch(ctx, k.fn, launch_geo(LZGPU_KERNEL_ENCODE_SLICES, o.threads, o.G, o.stages, 0, o.smem_bytes), 1, p.total_units, st, map, p);
 	return LZGPU_NOT_HANDLED;   // (cannot happen: the plan refuses m > 4, which only Cauchy goals have)
+}
+
+// ---------------------------------------------------------------------------------------------------
+// recovery from the parts of every slice together (recover_slices_kernel.cuh)
+// ---------------------------------------------------------------------------------------------------
+
+// The kernel's tables for one stripe shape: what is read and staged, what is written, the CRC streams, the solve
+static void rs_fill_shape(RsShape &o, const SliceLayout &lay, const SliceSolve &sv, const void *const *d_parts, const void *const *d_stored,
+                          const uint8_t *want, void *const *d_out_crc, bool image) {
+	const uint32_t L = lay.L, E = sv.n_eq;
+	std::memset(&o, 0, sizeof(o));
+	uint64_t staged = 0;
+	auto add_state = [&](uint8_t part, uint8_t s, uint8_t written) -> uint8_t {
+		o.state[o.n_state] = RsEntry{part, s, written, 0};
+		return static_cast<uint8_t>(o.n_state++);
+	};
+	for (uint32_t i = 0; i < lay.n_slices; ++i)
+		for (uint32_t p = 0; p < lay.k[i] + lay.m[i]; ++p) {
+			const uint32_t g = lay.base[i] + p;
+			if (!d_parts[g]) continue;
+			for (uint32_t s = 0; s < L / lay.k[i]; ++s) {
+				if (!stripe_exists(lay, i, s, sv.valid)) continue;
+				uint8_t slot = kRsNone;
+				if (p < lay.k[i]) {
+					const uint32_t q = s * lay.k[i] + p;
+					if (q < sv.valid && !((staged >> q) & 1ull)) { slot = static_cast<uint8_t>(q); staged |= 1ull << q; }
+				} else {
+					for (uint32_t e = 0; e < E; ++e)
+						if (sv.eq_slice[e] == i && sv.eq_row[e] == p - lay.k[i] && sv.eq_stripe[e] == s) slot = static_cast<uint8_t>(L + e);
+				}
+				const bool verify = d_stored && d_stored[g];
+				if (slot == kRsNone && !verify) continue;   // neither used nor verified: not read
+				o.read[o.n_read++] = RsEntry{static_cast<uint8_t>(g), static_cast<uint8_t>(s), slot, verify ? add_state(static_cast<uint8_t>(g), static_cast<uint8_t>(s), 0) : kRsNone};
+			}
+		}
+	for (uint32_t q = 0; q < L; ++q)
+		if (!((staged >> q) & 1ull)) o.zero[o.n_zero++] = static_cast<uint8_t>(q);
+	o.n_unknown = static_cast<uint16_t>(sv.n_unknown);
+	o.n_eq = static_cast<uint16_t>(E);
+	std::memcpy(o.unk_pos, sv.unk_pos, sizeof(o.unk_pos));
+	std::memcpy(o.eq_slice, sv.eq_slice, sizeof(o.eq_slice));
+	std::memcpy(o.eq_row, sv.eq_row, sizeof(o.eq_row));
+	std::memcpy(o.eq_stripe, sv.eq_stripe, sizeof(o.eq_stripe));
+	std::memcpy(o.rows, sv.rows, sizeof(o.rows));
+	for (uint32_t i = 0; i < lay.n_slices; ++i)
+		for (uint32_t p = 0; p < lay.k[i] + lay.m[i]; ++p) {
+			const uint32_t g = lay.base[i] + p;
+			if (!want[g]) continue;
+			for (uint32_t s = 0; s < L / lay.k[i]; ++s) {
+				if (!stripe_exists(lay, i, s, sv.valid)) continue;
+				uint8_t slot;
+				if (p < lay.k[i]) {
+					slot = static_cast<uint8_t>(s * lay.k[i] + p);
+				} else {
+					o.out_slice[o.n_out] = static_cast<uint8_t>(i);
+					o.out_row[o.n_out] = static_cast<uint8_t>(p - lay.k[i]);
+					o.out_stripe[o.n_out] = static_cast<uint8_t>(s);
+					slot = static_cast<uint8_t>(L + E + o.n_out++);
+				}
+				const uint8_t st = d_out_crc && d_out_crc[g] ? add_state(static_cast<uint8_t>(g), static_cast<uint8_t>(s), 1) : kRsNone;
+				o.write[o.n_write++] = RsEntry{static_cast<uint8_t>(g), static_cast<uint8_t>(s), slot, st};
+			}
+		}
+	if (image)
+		for (uint32_t q = 0; q < sv.valid; ++q) o.write[o.n_write++] = RsEntry{kRsNone, static_cast<uint8_t>(q), static_cast<uint8_t>(q), kRsNone};
+}
+
+int lz_recover_slices(lzgpu_ctx *ctx, const SliceLayout &lay, const SliceSolve *shapes, const RsGeometry &geo, uint32_t n_chunks, uint32_t nb,
+                      const void *const *d_parts, const size_t *part_stride, const void *const *d_part_crc, const uint8_t *want, void *const *d_out,
+                      const size_t *out_stride, void *const *d_out_crc, void *d_image, size_t image_stride, cudaStream_t st,
+                      unsigned long long *d_first_bad) {
+	auto p = std::make_unique<RecoverSlicesParams>();
+	std::memset(p.get(), 0, sizeof(RecoverSlicesParams));
+	const bool crc_on = lzgpu_crc_enabled() != 0;
+	for (uint32_t i = 0; i < lay.n_slices; ++i) {
+		p->part_stride[i] = part_stride ? part_stride[i] : 0;
+		p->out_stride[i] = out_stride ? out_stride[i] : 0;
+		p->k[i] = lay.k[i];
+		p->spc[i] = lay.L / lay.k[i];
+		p->pb[i] = (nb + lay.k[i] - 1) / lay.k[i];
+		for (uint32_t g = lay.base[i]; g < lay.base[i] + lay.k[i] + lay.m[i]; ++g) {
+			p->part_slice[g] = static_cast<uint8_t>(i);
+			p->parts[g] = static_cast<const uint8_t *>(d_parts[g]);
+			p->stored[g] = d_part_crc ? static_cast<const uint32_t *>(d_part_crc[g]) : nullptr;
+			p->out[g] = want[g] ? static_cast<uint8_t *>(d_out[g]) : nullptr;
+			p->out_crc[g] = want[g] && d_out_crc ? static_cast<uint32_t *>(d_out_crc[g]) : nullptr;
+		}
+	}
+	std::memcpy(p->gen, lay.gen, sizeof(p->gen));
+	p->image = static_cast<uint8_t *>(d_image);
+	p->image_stride = image_stride;
+	p->tables = ctx->d_crc_tables;
+	p->first_bad = d_first_bad;
+	p->L = lay.L;
+	p->G = geo.G;
+	p->nb = nb;
+	p->n_cs = (nb + lay.L - 1) / lay.L;
+	p->tail = nb % lay.L ? 1u : 0u;
+	p->units_per_chunk = (p->n_cs + geo.G - 1) / geo.G;
+	p->total_units = p->units_per_chunk * n_chunks;
+	p->n_slots = geo.slots;
+	p->n_states_max = geo.states;
+	p->crc_off = crc_on ? 0u : 1u;
+	p->zconst = lz::crc_of_zeros(LZGPU_BLOCK_SIZE);
+	for (int i = 0; i < 5; ++i) p->tree_mult[i] = lz::crc_xpow_bytes(2048ull << i);
+	const bool verifying = d_part_crc != nullptr;
+	if (verifying && !d_first_bad) return LZGPU_ERR_ARG;  // (cannot happen: the caller arms a ticket whenever it passes stored CRCs)
+	for (int t = 0; t < 2; ++t)
+		if (t == 0 ? nb >= lay.L : p->tail != 0)
+			rs_fill_shape(p->shape[t], lay, shapes[t], d_parts, d_part_crc, want, d_out_crc, d_image != nullptr);
+	const lzgpu_launch_geometry g = launch_geo(LZGPU_KERNEL_RECOVER_SLICES, geo.threads, geo.G, geo.stages, 0, geo.smem);
+	return launch(ctx, kRecoverSlicers[0], g, 1, p->total_units, st, *p);
 }

@@ -9,11 +9,13 @@
 #include "fused_plan.h"
 #include "repair_rows.h"
 #include "decode_locate.h"
+#include "slices_solve.h"
 
 #include <cctype>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <memory>
 
 namespace lz {
 
@@ -603,6 +605,56 @@ int lzgpu_plan_encode_slices(const lzgpu_goal *goals, uint32_t n_slices, uint32_
 	}
 	if (!any_striped) return LZGPU_ERR_ARG;
 	*out = lzd::slices_plan(goals, cauchy, n_slices, n_chunks, nb).out;
+	return LZGPU_OK;
+}
+
+int lzgpu_plan_recover_slices(const lzgpu_goal *goals, uint32_t n_slices, uint32_t nb, const uint8_t *given, lzgpu_slices_recover_plan *out) {
+	if (!out || !given || nb == 0 || nb > LZGPU_BLOCKS_IN_CHUNK) return LZGPU_ERR_ARG;
+	*out = lzgpu_slices_recover_plan{};
+	lzd::SliceLayout lay;
+	const char *why = nullptr;
+	if (lzd::slice_layout(goals, n_slices, lay, &why) != LZGPU_OK) return LZGPU_ERR_ARG;
+	lzd::SliceSolve sv[2];
+	lzd::slice_solve(lay, given, lay.L, sv[0]);
+	const uint32_t tail = nb % lay.L;
+	if (tail) lzd::slice_solve(lay, given, tail, sv[1]);
+	out->L = lay.L;
+	out->known = sv[0].known;
+	out->determined = sv[0].determined;
+	out->tail_determined = tail ? sv[1].determined : sv[0].determined;
+	out->tail_blocks = tail;
+	out->unknowns = sv[0].n_unknown;
+	out->equations = sv[0].n_eq;
+	out->tail_unknowns = tail ? sv[1].n_unknown : 0;
+	out->tail_equations = tail ? sv[1].n_eq : 0;
+	// the shapes the call's chunks have: full stripes when nb >= L, the tail when L does not divide nb
+	const lzd::SliceSolve used[2] = {nb >= lay.L ? sv[0] : sv[1], tail ? sv[1] : sv[0]};
+	const lzd::RsGeometry g = lzd::rs_geometry(lay, given, used, 2);
+	out->ok = g.ok ? 1 : 0;
+	out->G = g.G;
+	out->threads = g.threads;
+	out->stages = g.stages;
+	out->smem_bytes = static_cast<uint32_t>(g.smem);
+	return LZGPU_OK;
+}
+
+int lzgpu_debug_recover_slices_rows(const lzgpu_goal *goals, uint32_t n_slices, const uint8_t *given, uint32_t valid, uint32_t *n_unknowns,
+                                    uint32_t *n_equations, uint8_t *unk_pos, uint8_t *eq_slice, uint8_t *eq_row, uint8_t *eq_stripe,
+                                    uint8_t *rows, uint64_t *determined) {
+	if (!given || !n_unknowns || !n_equations || !unk_pos || !eq_slice || !eq_row || !eq_stripe || !rows || !determined) return LZGPU_ERR_ARG;
+	lzd::SliceLayout lay;
+	const char *why = nullptr;
+	if (lzd::slice_layout(goals, n_slices, lay, &why) != LZGPU_OK || valid == 0 || valid > lay.L) return LZGPU_ERR_ARG;
+	auto sv = std::make_unique<lzd::SliceSolve>();
+	lzd::slice_solve(lay, given, valid, *sv);
+	*n_unknowns = sv->n_unknown;
+	*n_equations = sv->n_eq;
+	std::memcpy(unk_pos, sv->unk_pos, lzd::kRsMaxL);
+	std::memcpy(eq_slice, sv->eq_slice, lzd::kRsMaxL);
+	std::memcpy(eq_row, sv->eq_row, lzd::kRsMaxL);
+	std::memcpy(eq_stripe, sv->eq_stripe, lzd::kRsMaxL);
+	std::memcpy(rows, sv->rows, sizeof(sv->rows));
+	*determined = sv->determined;
 	return LZGPU_OK;
 }
 

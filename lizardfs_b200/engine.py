@@ -623,6 +623,55 @@ class Engine:
         Returns (out_list, chunk_out or None); raises ChunkCrcError on a stored-CRC mismatch."""
         return _recover_chunks(self.lib.lzgpu_recover_chunks, self.h, goal, nb, parts, part_crc, want, chunk_image)
 
+    def recover_slices(self, goals, nb, parts, part_crc=None, want=None, chunk_image=False, with_crc=True):
+        """Recover a chunk of a multi-slice goal from the given parts of every slice together (lzgpu_recover_slices).  goals: up to
+        four SliceTypes; parts: one entry per flat part (slice i's k + m parts after those of the slices before it, one for the
+        standard slice), an array [n_chunks, pb_i * 64K] or None (lost); part_crc: None, or one [n_chunks, pb_i] uint32 array or None
+        per flat part.  want: flags per flat part (default: every lost part).  Returns (out, out_crc, image): out[g] / out_crc[g] for
+        every wanted part (else None), image [n_chunks, nb * 64K] or None.  Raises LzGpuError(ERR_TOO_FEW_PARTS) when a block it must
+        write is not determined, ChunkCrcError (.where = chunk, slice, part, block) on a stored-CRC mismatch."""
+        ns = len(goals)
+        pbs = [-(-nb // g.k) for g in goals]
+        slice_of = [i for i, g in enumerate(goals) for _ in range(1 if g.is_std else g.k + g.m)]
+        assert len(parts) == len(slice_of)
+        arrs = [None if p is None else _u8(p).reshape(-1, pbs[slice_of[j]] * BLOCK_SIZE) for j, p in enumerate(parts)]
+        n = next(a.shape[0] for a in arrs if a is not None)
+        crcs = None if part_crc is None else _ptr_array([None if c is None else np.ascontiguousarray(c, dtype=np.uint32) for c in part_crc])
+        if want is None:
+            want = [1 if a is None else 0 for a in arrs]
+        w = np.asarray(want, dtype=np.uint8)
+        out = [np.zeros((n, pbs[slice_of[j]] * BLOCK_SIZE), dtype=np.uint8) if w[j] else None for j in range(len(arrs))]
+        ocrc = [np.zeros((n, pbs[slice_of[j]]), dtype=np.uint32) if (w[j] and with_crc) else None for j in range(len(arrs))]
+        img = np.zeros((n, nb * BLOCK_SIZE), dtype=np.uint8) if chunk_image else None
+        strides = (C.c_size_t * ns)(*[pb * BLOCK_SIZE for pb in pbs])
+        bad = (C.c_int64 * 4)(-1, -1, -1, -1)
+        rc = self.lib.lzgpu_recover_slices(self.h, _goal_array(goals), ns, n, nb, _ptr_array(arrs), strides, crcs, _p(w), _ptr_array(out),
+                                           strides, _ptr_array(ocrc) if with_crc else None, _p(img), nb * BLOCK_SIZE, bad)
+        _check_crc(rc, "recover_slices", bad)
+        return out, ocrc, img
+
+    def recover_slices_dev(self, goals, n_chunks, nb, d_parts, part_stride, d_part_crc, want, d_out, out_stride, d_out_crc=None,
+                           d_chunk_out=None, chunk_out_stride=0, stream=None):
+        """lzgpu_recover_slices_dev: d_parts / d_part_crc / d_out / d_out_crc are lists over the flat parts (device pointers as ints,
+        0 or None = absent), part_stride / out_stride one entry per slice.  Raises ChunkCrcError (.where = chunk, slice, part, block)."""
+        ns, n = len(goals), len(want)
+        w = np.asarray(want, dtype=np.uint8)
+        bad = (C.c_int64 * 4)(-1, -1, -1, -1)
+        rc = self.lib.lzgpu_recover_slices_dev(self.h, _goal_array(goals), ns, n_chunks, nb, _dev_ptrs(d_parts, n), (C.c_size_t * ns)(*part_stride),
+                                               _dev_ptrs(d_part_crc, n), _p(w), _dev_ptrs(d_out, n), (C.c_size_t * ns)(*out_stride),
+                                               _dev_ptrs(d_out_crc, n), d_chunk_out, chunk_out_stride, bad, stream)
+        _check_crc(rc, "recover_slices_dev", bad)
+
+    @staticmethod
+    def plan_recover_slices(goals, nb, given):
+        """what recover_slices can rebuild from the given flat parts (pure host logic, csrc/slices_solve.h; no GPU needed): dict with
+        known, determined, tail_determined (bit q: combined-stripe position q), L, tail_blocks, unknowns, equations, tail_unknowns,
+        tail_equations, ok and the launch geometry G, threads, stages, smem_bytes"""
+        out = _lib.LzSlicesRecoverPlan()
+        g = np.asarray(given, dtype=np.uint8)
+        _check(_lib.load().lzgpu_plan_recover_slices(_goal_array(goals), len(goals), nb, _p(g), C.byref(out)), "plan_recover_slices")
+        return {f: getattr(out, f) for f, _ in _lib.LzSlicesRecoverPlan._fields_}
+
     def recover_chunks_dev(self, goal, n_chunks, nb, d_parts, part_stride, d_part_crc, want, d_out, d_chunk_out=None,
                            chunk_out_stride=None, stream=None):
         """Device-pointer degraded read.  With d_part_crc the call waits for its stream and raises ChunkCrcError on a
