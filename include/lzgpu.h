@@ -745,6 +745,13 @@ int lzgpu_pool_convert_chunks(lzgpu_pool *pool, const lzgpu_goal *src, const lzg
                               const uint8_t *const *parts, size_t part_stride, const uint32_t *const *part_crc,
                               const uint8_t *want, uint8_t *const *out, size_t out_stride, uint32_t *const *out_crc,
                               int64_t *bad); /* the same over every device of a pool: chunks dealt in contiguous runs */
+int lzgpu_pool_recover_slices(lzgpu_pool *pool, const lzgpu_goal *goals, uint32_t n_slices, uint32_t n_chunks, uint32_t nb,
+                              const uint8_t *const *parts, const size_t *part_stride, const uint32_t *const *part_crc,
+                              const uint8_t *want, uint8_t *const *out, const size_t *out_stride, uint32_t *const *out_crc,
+                              uint8_t *chunk_out, size_t chunk_out_stride, int64_t *bad /* [4] */);
+                             /* lzgpu_recover_slices over every device of a pool, host memory only: for any input the code, bytes, CRCs,
+                              * image and bad[0..3] lzgpu_recover_slices returns on one context for the whole batch (shares and merge as
+                              * for the pool's stripe calls below) */
 int lzgpu_convert_chunks_dev(lzgpu_ctx *ctx, const lzgpu_goal *src, const lzgpu_goal *dst, uint32_t n_chunks, uint32_t nb,
                              const void *const *d_parts, size_t part_stride, const void *const *d_part_crc,
                              const uint8_t *want, void *const *d_out, size_t out_stride, void *const *d_out_crc,

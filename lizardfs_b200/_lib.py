@@ -247,6 +247,7 @@ SIGNATURES = {
     "lzgpu_pool_encode_slices": (_int, [_vp, _goalp, _u32, _u32, _u32, _vp, _sz, _vp, _vp, _vp, _vp]),
     "lzgpu_pool_recover_chunks": (_int, [_vp, _goalp, _u32, _u32, _vp, _sz, _vp, _vp, _vp, _vp, _sz, _vp]),
     "lzgpu_pool_convert_chunks": (_int, [_vp, _goalp, _goalp, _u32, _u32, _vp, _sz, _vp, _vp, _vp, _sz, _vp, _vp]),
+    "lzgpu_pool_recover_slices": (_int, [_vp, _goalp, _u32, _u32, _u32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
     "lzgpu_pool_crc_blocks": (_int, [_vp, _vp, _sz, _u32, _sz, _vp]),
     "lzgpu_pool_check_stripes": (_int, [_vp, _goalp, _u32, _u32, _vp, _sz, _vp, _vp, _vp]),
     "lzgpu_pool_check_stripe_map": (_int, [_vp, _goalp, _u32, _u32, _vp, _sz, _vp, _vp, _vp]),

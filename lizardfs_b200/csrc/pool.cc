@@ -21,6 +21,7 @@
 
 #include "engine_internal.h"
 #include "lzgpu.h"
+#include "slices_solve.h"
 
 namespace {
 
@@ -411,6 +412,38 @@ extern "C" int lzgpu_pool_decode_stripes(lzgpu_pool *pool, const lzgpu_goal *goa
 	return pool_part_batch(pool, goal, n_chunks, nb, parts, part_stride, part_crc, fix, true, nullptr,
 	                       [&](lzgpu_ctx *ctx, uint32_t count, uint8_t *const *p, const uint32_t *const *c, lzgpu_stripe_decode *o, int64_t *) {
 		return lzgpu_decode_stripes(ctx, goal, count, nb, p, part_stride, c, o);
+	});
+}
+
+// Recovery from the parts of every slice (lzgpu_recover_slices) over the pool: slice i's part and out pointers moved by first *
+// part_stride[i] and first * out_stride[i], its stored and computed CRC arrays by first * pb_i (the layout of the per-context call,
+// lzd::slice_layout), the image by first * chunk_out_stride; the codes and bad[0..3] merged by pool_merged.  With goals, nb or pointer
+// arrays the per-context call refuses, the caller's arrays go through unmoved and every share refuses alike.
+extern "C" int lzgpu_pool_recover_slices(lzgpu_pool *pool, const lzgpu_goal *goals, uint32_t n_slices, uint32_t n_chunks, uint32_t nb,
+                                          const uint8_t *const *parts, const size_t *part_stride, const uint32_t *const *part_crc,
+                                          const uint8_t *want, uint8_t *const *out, const size_t *out_stride, uint32_t *const *out_crc,
+                                          uint8_t *chunk_out, size_t chunk_out_stride, int64_t *bad) {
+	if (!pool) return LZGPU_ERR_ARG;
+	lzd::SliceLayout lay;
+	const char *why = nullptr;
+	const bool shaped = parts && part_stride && nb >= 1 && nb <= LZGPU_BLOCKS_IN_CHUNK && lzd::slice_layout(goals, n_slices, lay, &why) == LZGPU_OK;
+	return pool_merged(pool, n_chunks, bad, 4, [&](lzgpu_ctx *ctx, uint32_t first, uint32_t count, int64_t *b) {
+		const uint8_t *p[LZGPU_MAX_PARTS];
+		const uint32_t *c[LZGPU_MAX_PARTS];
+		uint8_t *o[LZGPU_MAX_PARTS];
+		uint32_t *oc[LZGPU_MAX_PARTS];
+		for (uint32_t g = 0; shaped && g < lay.n_parts; ++g) {
+			const int i = lay.slice_of(g);
+			const size_t pb = (nb + lay.k[i] - 1) / lay.k[i];
+			p[g] = parts[g] ? parts[g] + first * part_stride[i] : nullptr;
+			c[g] = part_crc && part_crc[g] ? part_crc[g] + first * pb : nullptr;
+			// without out_stride a wanted part is refused by every share, and an unwanted one is not touched
+			o[g] = out && out[g] ? out[g] + (out_stride ? first * out_stride[i] : 0) : nullptr;
+			oc[g] = out_crc && out_crc[g] ? out_crc[g] + first * pb : nullptr;
+		}
+		return lzgpu_recover_slices(ctx, goals, n_slices, count, nb, shaped ? p : parts, part_stride, shaped && part_crc ? c : part_crc, want,
+		                            shaped && out ? o : out, out_stride, shaped && out_crc ? oc : out_crc,
+		                            chunk_out ? chunk_out + first * chunk_out_stride : nullptr, chunk_out_stride, b);
 	});
 }
 

@@ -176,6 +176,28 @@ def _convert_chunks(fn, h, src, dst, nb, parts, want, part_crc, with_crc):
     return out, ocrc
 
 
+def _recover_slices(fn, h, goals, nb, parts, part_crc, want, chunk_image, with_crc):
+    ns = len(goals)
+    pbs = [-(-nb // g.k) for g in goals]
+    slice_of = [i for i, g in enumerate(goals) for _ in range(1 if g.is_std else g.k + g.m)]
+    assert len(parts) == len(slice_of)
+    arrs = [None if p is None else _u8(p).reshape(-1, pbs[slice_of[j]] * BLOCK_SIZE) for j, p in enumerate(parts)]
+    n = next(a.shape[0] for a in arrs if a is not None)
+    crcs = None if part_crc is None else _ptr_array([None if c is None else np.ascontiguousarray(c, dtype=np.uint32) for c in part_crc])
+    if want is None:
+        want = [1 if a is None else 0 for a in arrs]
+    w = np.asarray(want, dtype=np.uint8)
+    out = [np.zeros((n, pbs[slice_of[j]] * BLOCK_SIZE), dtype=np.uint8) if w[j] else None for j in range(len(arrs))]
+    ocrc = [np.zeros((n, pbs[slice_of[j]]), dtype=np.uint32) if (w[j] and with_crc) else None for j in range(len(arrs))]
+    img = np.zeros((n, nb * BLOCK_SIZE), dtype=np.uint8) if chunk_image else None
+    strides = (C.c_size_t * ns)(*[pb * BLOCK_SIZE for pb in pbs])
+    bad = (C.c_int64 * 4)(-1, -1, -1, -1)
+    rc = fn(h, _goal_array(goals), ns, n, nb, _ptr_array(arrs), strides, crcs, _p(w), _ptr_array(out), strides,
+            _ptr_array(ocrc) if with_crc else None, _p(img), nb * BLOCK_SIZE, bad)
+    _check_crc(rc, _name(fn), bad)
+    return out, ocrc, img
+
+
 def _part_batch(fn, h, goal, nb, parts, part_crc, result, attr, in_place=False):
     # the host-pointer check, map and correction: result(n_chunks, pb) makes the array the call fills, which is returned, and
     # attached to a ChunkCrcError as `attr`
@@ -419,6 +441,11 @@ class Pool:
         """Engine.convert_chunks over every device of the pool (lzgpu_pool_convert_chunks)"""
         return _convert_chunks(self.lib.lzgpu_pool_convert_chunks, self.h, src, dst, nb, parts, want, part_crc, with_crc)
 
+    def recover_slices(self, goals, nb, parts, part_crc=None, want=None, chunk_image=False, with_crc=True):
+        """Engine.recover_slices over every device of the pool (lzgpu_pool_recover_slices): the same arguments, results and errors for
+        the whole batch; ChunkCrcError.where = (chunk in the batch, slice, part, block)"""
+        return _recover_slices(self.lib.lzgpu_pool_recover_slices, self.h, goals, nb, parts, part_crc, want, chunk_image, with_crc)
+
     def crc_blocks(self, data, block_len=BLOCK_SIZE):
         data = _u8(data).reshape(-1, block_len)
         out = np.empty(data.shape[0], dtype=np.uint32)
@@ -630,25 +657,7 @@ class Engine:
         per flat part.  want: flags per flat part (default: every lost part).  Returns (out, out_crc, image): out[g] / out_crc[g] for
         every wanted part (else None), image [n_chunks, nb * 64K] or None.  Raises LzGpuError(ERR_TOO_FEW_PARTS) when a block it must
         write is not determined, ChunkCrcError (.where = chunk, slice, part, block) on a stored-CRC mismatch."""
-        ns = len(goals)
-        pbs = [-(-nb // g.k) for g in goals]
-        slice_of = [i for i, g in enumerate(goals) for _ in range(1 if g.is_std else g.k + g.m)]
-        assert len(parts) == len(slice_of)
-        arrs = [None if p is None else _u8(p).reshape(-1, pbs[slice_of[j]] * BLOCK_SIZE) for j, p in enumerate(parts)]
-        n = next(a.shape[0] for a in arrs if a is not None)
-        crcs = None if part_crc is None else _ptr_array([None if c is None else np.ascontiguousarray(c, dtype=np.uint32) for c in part_crc])
-        if want is None:
-            want = [1 if a is None else 0 for a in arrs]
-        w = np.asarray(want, dtype=np.uint8)
-        out = [np.zeros((n, pbs[slice_of[j]] * BLOCK_SIZE), dtype=np.uint8) if w[j] else None for j in range(len(arrs))]
-        ocrc = [np.zeros((n, pbs[slice_of[j]]), dtype=np.uint32) if (w[j] and with_crc) else None for j in range(len(arrs))]
-        img = np.zeros((n, nb * BLOCK_SIZE), dtype=np.uint8) if chunk_image else None
-        strides = (C.c_size_t * ns)(*[pb * BLOCK_SIZE for pb in pbs])
-        bad = (C.c_int64 * 4)(-1, -1, -1, -1)
-        rc = self.lib.lzgpu_recover_slices(self.h, _goal_array(goals), ns, n, nb, _ptr_array(arrs), strides, crcs, _p(w), _ptr_array(out),
-                                           strides, _ptr_array(ocrc) if with_crc else None, _p(img), nb * BLOCK_SIZE, bad)
-        _check_crc(rc, "recover_slices", bad)
-        return out, ocrc, img
+        return _recover_slices(self.lib.lzgpu_recover_slices, self.h, goals, nb, parts, part_crc, want, chunk_image, with_crc)
 
     def recover_slices_dev(self, goals, n_chunks, nb, d_parts, part_stride, d_part_crc, want, d_out, out_stride, d_out_crc=None,
                            d_chunk_out=None, chunk_out_stride=0, stream=None):
