@@ -302,6 +302,22 @@ typedef struct lzgpu_launch_geometry {
 	uint32_t smem_bytes;
 } lzgpu_launch_geometry;
 int lzgpu_debug_last_geometry(lzgpu_ctx *ctx, lzgpu_launch_geometry *out);
+/* Diagnostics: which fused_stream_kernel instantiation a launch of the encoder family (LZGPU_KERNEL_ENCODE / _ENCODE_BITSLICE: the
+ * encode, its passes of four Cauchy rows, the CRC-only form and the conversion's SPLIT form) ran.  lzgpu_debug_encoder_kernels lists
+ * every compiled instantiation, in the launcher's table order, the 4-byte-item twin of a generic-coefficient entry right after it;
+ * pure host logic, returns the count (out may be NULL; at most `capacity` entries are written). */
+typedef struct lzgpu_encoder_kernel {
+	int m;                /* parity rows of the instantiation; 0 = the CRC-only form */
+	int generic;          /* coefficients read per launch (Cauchy rows; Vandermonde rows on the nine-warp CTA) */
+	int bitsliced, striped, split;
+	uint32_t kt, gt;      /* compile-time k and G; 0 = read at run time */
+	uint32_t item_bytes;  /* bytes per GF item: 16 / 8 packed, 4 for the narrow generic twin, 32 bit-sliced */
+} lzgpu_encoder_kernel;
+int lzgpu_debug_encoder_kernels(lzgpu_encoder_kernel *out, uint32_t capacity);
+/* The instantiation (index into that list) and unit mode (0 per-chunk, 1 flat, 2 striped) of the context's latest persistent launch,
+ * taken in the same snapshot as lzgpu_debug_last_geometry; *index = -1, *mode = 0 when that launch was not an encoder kernel (or
+ * before the first launch).  A multi-pass Cauchy encode reports its last pass. */
+int lzgpu_debug_last_encoder(lzgpu_ctx *ctx, int32_t *index, uint32_t *mode);
 /* Diagnostics: verification result slots of the context — how many exist and how many a call holds right now (0 when no call runs). */
 int lzgpu_debug_status_slots(lzgpu_ctx *ctx, uint32_t *allocated, uint32_t *in_use);
 

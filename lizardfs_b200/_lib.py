@@ -79,6 +79,11 @@ class LzLaunchGeometry(C.Structure):
                 ("stages", C.c_uint32), ("gf_warps", C.c_uint32), ("smem_bytes", C.c_uint32)]
 
 
+class LzEncoderKernel(C.Structure):
+    _fields_ = [("m", C.c_int), ("generic", C.c_int), ("bitsliced", C.c_int), ("striped", C.c_int), ("split", C.c_int), ("kt", C.c_uint32),
+                ("gt", C.c_uint32), ("item_bytes", C.c_uint32)]
+
+
 # lzgpu_launch_geometry.kernel
 KERNEL_NONE, KERNEL_ENCODE, KERNEL_ENCODE_BITSLICE, KERNEL_RECOVER_GEO0, KERNEL_RECOVER_GEO1, KERNEL_RECOVER_GEO2, \
     KERNEL_RECOVER_DIRECT, KERNEL_RECOVER_BS3, KERNEL_CONVERT, KERNEL_CHECK, KERNEL_CHECK_DEGRADED, KERNEL_ENCODE_SLICES, \
@@ -159,6 +164,8 @@ SIGNATURES = {
     "lzgpu_reset_stats": (None, [_vp]),
     "lzgpu_debug_last_launch": (_int, [_vp, C.POINTER(_u32), C.POINTER(_u32)]),
     "lzgpu_debug_last_geometry": (_int, [_vp, C.POINTER(LzLaunchGeometry)]),
+    "lzgpu_debug_encoder_kernels": (_int, [C.POINTER(LzEncoderKernel), _u32]),
+    "lzgpu_debug_last_encoder": (_int, [_vp, C.POINTER(C.c_int32), C.POINTER(_u32)]),
     "lzgpu_debug_status_slots": (_int, [_vp, C.POINTER(_u32), C.POINTER(_u32)]),
     "lzgpu_encode_chunks": (_int, [_vp, _goalp, _u32, _u32, _vp, _sz, _vp, _sz, _vp, _sz]),
     "lzgpu_encode_chunks_dev": (_int, [_vp, _goalp, _u32, _u32, _vp, _sz, _vp, _sz, _vp, _sz, _vp]),

@@ -47,8 +47,10 @@ struct FusedState {
 	int bitslice = LZ_BITSLICE_DEFAULT;  // LZGPU_BITSLICE: Vandermonde parity rows on bit planes (W = 8 items, bitslice.cuh) — bit 0: four rows, bit 1: three rows with k >= 7, bit 2: three rows with any k; 0 = packed-byte Horner
 	int promo = 3;  // CU_TENSOR_MAP_L2_PROMOTION_L2_256B: measured faster streaming than 128B/none
 	uint32_t grid_cap = 0;  // LZGPU_GRID_CAP (testing): at most this many CTAs per persistent launch, so that every CTA walks several units; 0 = no cap
-	std::mutex last_mu;                     // guards last_geo: grid, units and the rest are recorded and read as one snapshot
+	std::mutex last_mu;                     // guards the three below: they are recorded and read as one snapshot
 	lzgpu_launch_geometry last_geo{};       // the latest persistent launch (lzgpu_debug_last_launch, lzgpu_debug_last_geometry)
+	int32_t last_encoder = -1;              // its encoder instantiation and unit mode (lzgpu_debug_last_encoder); -1: not an encoder
+	uint32_t last_mode = 0;
 };
 
 // what a launch site knows of its kernel's geometry before the grid is chosen (persistent_grid adds grid and units)
@@ -63,16 +65,28 @@ static lzgpu_launch_geometry launch_geo(int kernel, uint32_t threads, uint32_t G
 	return g;
 }
 
+// What a launch records as the context's latest: its geometry, and for an encoder kernel (fused_run) the kernel's position in the
+// list lzgpu_debug_encoder_kernels reports and the unit mode; every other launch records encoder -1
+struct LaunchRecord {
+	lzgpu_launch_geometry geo;
+	int32_t encoder;
+	uint32_t mode;
+	LaunchRecord(const lzgpu_launch_geometry &g, int32_t e = -1, uint32_t m = 0) : geo(g), encoder(e), mode(m) {}
+};
+
 // CTAs of a persistent launch (each CTA starts at unit blockIdx.x and steps by gridDim.x): one per unit, at most `per_sm` per SM,
 // and at most LZGPU_GRID_CAP when that is set.  Records the launch (geo, completed with grid and units) as the context's latest.
-static int persistent_grid(lzgpu_ctx *ctx, uint64_t total_units, int per_sm, lzgpu_launch_geometry geo) {
+static int persistent_grid(lzgpu_ctx *ctx, uint64_t total_units, int per_sm, const LaunchRecord &rec) {
 	FusedState *fs = ctx->fused;
 	uint64_t grid = std::min<uint64_t>(total_units, static_cast<uint64_t>(ctx->sm_count) * per_sm);
 	if (fs->grid_cap) grid = std::min<uint64_t>(grid, fs->grid_cap);
+	lzgpu_launch_geometry geo = rec.geo;
 	geo.grid = static_cast<uint32_t>(grid);
 	geo.units = static_cast<uint32_t>(total_units);
 	std::lock_guard<std::mutex> lock(fs->last_mu);
 	fs->last_geo = geo;
+	fs->last_encoder = rec.encoder;
+	fs->last_mode = rec.mode;
 	return static_cast<int>(grid);
 }
 
@@ -117,10 +131,10 @@ static void elim3_constants(int x0, int x1, int x2, uint8_t c[6]) {
 
 // One persistent launch: geo.threads threads and geo.smem_bytes bytes of shared memory per CTA, the grid from persistent_grid
 template <class... P, class... A>
-static int launch(lzgpu_ctx *ctx, void (*kernel)(P...), const lzgpu_launch_geometry &geo, int per_sm, uint64_t units, cudaStream_t st,
+static int launch(lzgpu_ctx *ctx, void (*kernel)(P...), const LaunchRecord &rec, int per_sm, uint64_t units, cudaStream_t st,
                   const A &...args) {
-	const int grid = persistent_grid(ctx, units, per_sm, geo);
-	kernel<<<grid, geo.threads, geo.smem_bytes, st>>>(args...);
+	const int grid = persistent_grid(ctx, units, per_sm, rec);
+	kernel<<<grid, rec.geo.threads, rec.geo.smem_bytes, st>>>(args...);
 	CUDA_TRY(cudaGetLastError());
 	ctx->stats.kernel_launches++;
 	return LZGPU_OK;
@@ -202,6 +216,13 @@ static const EncodeKernelEntry *find_encoder(int M, bool generic, uint32_t K, ui
 		if (k.k == 0) runtime_k = &k;
 	}
 	return runtime_k;
+}
+
+// position of entry k's kernel (narrow: its 4-byte-item twin, right after it) in the list lzgpu_debug_encoder_kernels reports
+static int32_t encoder_index(const EncodeKernelEntry *k, bool narrow) {
+	int32_t i = 0;
+	for (const EncodeKernelEntry *e = kEncoders; e != k; ++e) i += e->narrow ? 2 : 1;
+	return i + (narrow ? 1 : 0);
 }
 
 // Degraded read (fused_recover_kernel), keyed by the plan's kernel, lost data parts, compile-time k (0: runtime) and parity rows:
@@ -395,6 +416,32 @@ extern "C" int lzgpu_debug_last_geometry(lzgpu_ctx *ctx, lzgpu_launch_geometry *
 	return LZGPU_OK;
 }
 
+extern "C" int lzgpu_debug_last_encoder(lzgpu_ctx *ctx, int32_t *index, uint32_t *mode) {
+	if (!ctx || !ctx->fused || !index || !mode) return LZGPU_ERR_ARG;
+	std::lock_guard<std::mutex> lock(ctx->fused->last_mu);
+	*index = ctx->fused->last_encoder;
+	*mode = ctx->fused->last_mode;
+	return LZGPU_OK;
+}
+
+extern "C" int lzgpu_debug_encoder_kernels(lzgpu_encoder_kernel *out, uint32_t capacity) {
+	uint32_t n = 0;
+	for (const EncodeKernelEntry &k : kEncoders)
+		for (int narrow = 0; narrow <= (k.narrow ? 1 : 0); ++narrow, ++n) {
+			if (!out || n >= capacity) continue;
+			lzgpu_encoder_kernel &o = out[n];
+			o.m = k.m;
+			o.generic = k.generic;
+			o.bitsliced = k.bs;
+			o.striped = k.striped;
+			o.split = k.split;
+			o.kt = k.k;
+			o.gt = k.g;
+			o.item_bytes = k.bs ? 32u : narrow ? 4u : 4u * static_cast<uint32_t>(fused_item_words(k.m, k.generic));  // (the W of each instantiation)
+		}
+	return static_cast<int>(n);
+}
+
 // rows_per_chunk rows of kRowBytes per chunk, chunk c at base + c * chunk_stride (0: contiguous), boxes of box_rows rows
 static CUresult make_tensor_map(const FusedState *fs, CUtensorMap *map, const void *base, uint64_t rows_per_chunk, uint64_t n_chunks,
                                 uint64_t chunk_stride, uint32_t box_rows) {
@@ -472,8 +519,9 @@ static int fused_run(lzgpu_ctx *ctx, int M, bool generic, const uint8_t *coef_ro
 	if (!k) return LZGPU_NOT_HANDLED;
 	const lzgpu_launch_geometry geo = launch_geo(pl.bs ? LZGPU_KERNEL_ENCODE_BITSLICE : LZGPU_KERNEL_ENCODE, pl.threads, G, pl.n_stages,
 	                                             pl.bs ? (16 * G + 31) / 32 : 0, pl.smem);
-	const EncodeKernel fn = k->narrow && fused_generic_item_words(G) == 1 ? k->narrow : k->fn;
-	return launch(ctx, fn, geo, fused_ctas_per_sm(M, generic, 64, pl.bs), p.total_units, st, map, p);
+	const bool narrow = k->narrow && fused_generic_item_words(G) == 1;
+	return launch(ctx, narrow ? k->narrow : k->fn, LaunchRecord(geo, encoder_index(k, narrow), pl.mode), fused_ctas_per_sm(M, generic, 64, pl.bs),
+	              p.total_units, st, map, p);
 }
 
 int lz_fused_encode(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, uint32_t nb, const void *d_data, size_t chunk_stride,

@@ -542,6 +542,16 @@ class ReedSolomon:
 # ------------------------------------------------------------------------------------------------
 # batched engine
 # ------------------------------------------------------------------------------------------------
+def encoder_kernels():
+    """every compiled fused_stream_kernel instantiation (lzgpu_debug_encoder_kernels; pure host logic, no GPU needed), in the order
+    Engine.last_encoder() indexes: a list of dicts of m, generic, bitsliced, striped, split, kt, gt (0: read at run time), item_bytes"""
+    lib = _lib.load()
+    n = lib.lzgpu_debug_encoder_kernels(None, 0)
+    out = (_lib.LzEncoderKernel * n)()
+    _check(0 if lib.lzgpu_debug_encoder_kernels(out, n) == n else _lib.ERR_ARG, "debug_encoder_kernels")
+    return [{f: getattr(e, f) for f, _ in _lib.LzEncoderKernel._fields_} for e in out]
+
+
 class Engine:
     """One context on one GPU.  Host arrays in, host arrays out; the *_dev methods take raw device
     pointers (ints, e.g. torch.Tensor.data_ptr()) and are asynchronous on the given stream."""
@@ -584,6 +594,13 @@ class Engine:
         g = _lib.LzLaunchGeometry()
         _check(self.lib.lzgpu_debug_last_geometry(self.h, C.byref(g)), "debug_last_geometry")
         return {f: getattr(g, f) for f, _ in _lib.LzLaunchGeometry._fields_}
+
+    def last_encoder(self):
+        """(index, mode) of the same launch as last_geometry() (lzgpu_debug_last_encoder): its position in encoder_kernels() and its
+        unit mode (0 per-chunk, 1 flat, 2 striped); (-1, 0) when that launch was not a fused_stream_kernel instantiation"""
+        index, mode = C.c_int32(), C.c_uint32()
+        _check(self.lib.lzgpu_debug_last_encoder(self.h, C.byref(index), C.byref(mode)), "debug_last_encoder")
+        return index.value, mode.value
 
     def status_slots(self):
         """(allocated, in_use) verification result slots of this context (lzgpu_debug_status_slots)"""

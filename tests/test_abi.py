@@ -66,7 +66,8 @@ def test_struct_layouts_match_the_header(tmp_path):
     from lizardfs_b200 import _lib
     structs = {"lzgpu_goal": _lib.LzGoal, "lzgpu_stats": _lib.LzStats, "lzgpu_block_write": _lib.LzBlockWrite, "lzgpu_encode_plan": _lib.LzEncodePlan,
                "lzgpu_launch_geometry": _lib.LzLaunchGeometry, "lzgpu_recover_switches": _lib.LzRecoverSwitches,
-               "lzgpu_recover_plan": _lib.LzRecoverPlan, "lzgpu_check_plan": _lib.LzCheckPlan}
+               "lzgpu_recover_plan": _lib.LzRecoverPlan, "lzgpu_check_plan": _lib.LzCheckPlan,
+               "lzgpu_encoder_kernel": _lib.LzEncoderKernel}
     lines = ['#include <stdio.h>', '#include <stddef.h>', '#include "lzgpu.h"', 'int main(void) {']
     for name, cls in structs.items():
         lines.append(f'printf("{name} %zu", sizeof({name}));')

@@ -136,42 +136,43 @@ def sliced(oracle, text, nb, n, seed):
 # ---- encode --------------------------------------------------------------------------------------------------------------------
 
 ENCODE = [
-    # goal, blocks per chunk, chunks, chunk stride in blocks, switches — ragged shapes (nb % k != 0) where the unit mode allows them
-    ("ec(8,2)", 61, 14, 61, dict(LZGPU_STRIPED=0)),            # per-chunk units, folded (k, G) = (8, 7): two units per chunk, one of them ragged
-    ("ec(8,2)", 61, 14, 61, dict(LZGPU_STRIPED=1)),            # striped units, folded
-    ("ec(8,2)", 61, 14, 64, {}),                               # automatic (striped: per-chunk units would waste slots), padded stride
-    ("ec(8,2)", 16, 56, 16, {}),                               # flat units across chunk boundaries
-    ("xor2", 65, 8, 65, dict(LZGPU_STRIPED=0)),                # folded (2, 32)
-    ("xor3", 62, 8, 62, dict(LZGPU_STRIPED=0)),                # folded (3, 20)
-    ("ec(3,2)", 50, 8, 50, dict(LZGPU_STRIPED=0)),             # folded (3, 16)
-    ("ec(3,2)", 50, N, 50, dict(LZGPU_STRIPED=1)),             # striped, folded
-    ("ec(5,3)", 43, 8, 43, dict(LZGPU_STRIPED=0)),             # folded (5, 8), packed-byte three rows
-    ("ec(5,3)", 43, 16, 43, dict(LZGPU_STRIPED=1)),            # striped, folded
-    ("ec(8,4)", 67, 8, 67, dict(LZGPU_STRIPED=0, LZGPU_BITSLICE=0)),   # folded (8, 8) on the packed-byte route
-    ("ec(7,2)", 31, N, 31, dict(LZGPU_STRIPED=0)),             # runtime k
-    ("ec(11,3)", 40, N, 40, dict(LZGPU_STRIPED=0, LZGPU_BITSLICE=0)),  # runtime k, packed-byte three rows
-    ("ec(8,3)", 37, N, 37, dict(LZGPU_STRIPED=0)),             # bit-sliced, three rows, folded
-    ("ec(11,3)", 40, N, 40, dict(LZGPU_STRIPED=0)),            # bit-sliced, three rows, runtime k
-    ("ec(8,3)", 37, 2 * N, 37, dict(LZGPU_STRIPED=1)),         # bit-sliced striped, three rows
-    ("ec(8,4)", 67, 8, 67, dict(LZGPU_STRIPED=0)),             # bit-sliced, four rows, folded
-    ("ec(7,4)", 30, N, 30, dict(LZGPU_STRIPED=0)),             # bit-sliced, four rows, runtime k
-    ("ec(8,4)", 67, N, 67, dict(LZGPU_STRIPED=1)),             # bit-sliced striped instantiation, folded (8, 8)
-    ("ec(21,4)", 50, 8, 50, dict(LZGPU_STRIPED=0)),            # Cauchy rows on the generic-coefficient kernel
-    ("ec(21,4)", 50, N, 50, {}),                               # the same, automatic unit mode
-    ("ec(8,6)", 37, N, 37, {}),                                # m > 4: two passes (four rows, then two)
-    ("ec(31,3)", 70, 8, 70, dict(LZGPU_BITSLICE=0)),           # Vandermonde rows that fit only the generic-coefficient CTA
+    # goal, blocks per chunk, chunks, chunk stride in blocks, switches, the encoder instantiation (lzgpu_debug_encoder_kernels index;
+    # the last pass for m > 4) — ragged shapes (nb % k != 0) where the unit mode allows them
+    ("ec(8,2)", 61, 14, 61, dict(LZGPU_STRIPED=0), 25),         # per-chunk units, folded (k, G) = (8, 7): two units per chunk, one of them ragged
+    ("ec(8,2)", 61, 14, 61, dict(LZGPU_STRIPED=1), 43),         # striped units, folded
+    ("ec(8,2)", 61, 14, 64, {}, 43),                            # automatic (striped: per-chunk units would waste slots), padded stride
+    ("ec(8,2)", 16, 56, 16, {}, 25),                            # flat units across chunk boundaries
+    ("xor2", 65, 8, 65, dict(LZGPU_STRIPED=0), 26),             # folded (2, 32)
+    ("xor3", 62, 8, 62, dict(LZGPU_STRIPED=0), 27),             # folded (3, 20)
+    ("ec(3,2)", 50, 8, 50, dict(LZGPU_STRIPED=0), 28),          # folded (3, 16)
+    ("ec(3,2)", 50, N, 50, dict(LZGPU_STRIPED=1), 46),          # striped, folded
+    ("ec(5,3)", 43, 8, 43, dict(LZGPU_STRIPED=0), 31),          # folded (5, 8), packed-byte three rows
+    ("ec(5,3)", 43, 16, 43, dict(LZGPU_STRIPED=1), 47),         # striped, folded
+    ("ec(8,4)", 67, 8, 67, dict(LZGPU_STRIPED=0, LZGPU_BITSLICE=0), 33),  # folded (8, 8) on the packed-byte route
+    ("ec(7,2)", 31, N, 31, dict(LZGPU_STRIPED=0), 2),           # runtime k
+    ("ec(11,3)", 40, N, 40, dict(LZGPU_STRIPED=0, LZGPU_BITSLICE=0), 3),  # runtime k, packed-byte three rows
+    ("ec(8,3)", 37, N, 37, dict(LZGPU_STRIPED=0), 58),          # bit-sliced, three rows, folded
+    ("ec(11,3)", 40, N, 40, dict(LZGPU_STRIPED=0), 49),         # bit-sliced, three rows, runtime k
+    ("ec(8,3)", 37, 2 * N, 37, dict(LZGPU_STRIPED=1), 51),      # bit-sliced striped, three rows
+    ("ec(8,4)", 67, 8, 67, dict(LZGPU_STRIPED=0), 53),          # bit-sliced, four rows, folded
+    ("ec(7,4)", 30, N, 30, dict(LZGPU_STRIPED=0), 50),          # bit-sliced, four rows, runtime k
+    ("ec(8,4)", 67, N, 67, dict(LZGPU_STRIPED=1), 62),          # bit-sliced striped instantiation, folded (8, 8)
+    ("ec(21,4)", 50, 8, 50, dict(LZGPU_STRIPED=0), 12),         # Cauchy rows on the generic-coefficient kernel
+    ("ec(21,4)", 50, N, 50, {}, 24),                            # the same, automatic unit mode
+    ("ec(8,6)", 37, N, 37, {}, 7),                              # m > 4: two passes (four rows, then two)
+    ("ec(31,3)", 70, 8, 70, dict(LZGPU_BITSLICE=0), 10),        # Vandermonde rows that fit only the generic-coefficient CTA
 ]
 
 
 def _id(case):
-    env = ",".join(f"{k[6:]}={v}" for k, v in sorted(case[-1].items()))
-    return "-".join(str(x) for x in case[:-1]) + (f"-{env}" if env else "")
+    env = ",".join(f"{k[6:]}={v}" for k, v in sorted(case[4].items()))
+    return "-".join(str(x) for x in case[:4]) + (f"-{env}" if env else "")
 
 
 @pytest.mark.parametrize("cap", CAPS)
 @pytest.mark.parametrize("case", ENCODE, ids=[_id(c) for c in ENCODE])
 def test_encode_with_several_units_per_cta(oracle, case, cap):
-    text, nb, n, stride, env = case
+    text, nb, n, stride, env, kernel = case
     goal = L.SliceType(text)
     m, pb = goal.m, -(-nb // goal.k)
     n_crc = nb + m * pb
@@ -184,6 +185,7 @@ def test_encode_with_several_units_per_cta(oracle, case, cap):
     mark_launch(e)
     e.encode_chunks_dev(goal, n, nb * BLOCK, ptr(d_data), stride * BLOCK, ptr(d_par), m * pb * BLOCK, ptr(d_crc), n_crc)
     assert_walks(e, cap)
+    assert e.last_encoder()[0] == kernel, (e.last_encoder(), L.encoder_kernels()[kernel])
     e.sync()
     parity = host(d_par).reshape(n, m, pb * BLOCK)
     crc = host(d_crc, np.uint32)
