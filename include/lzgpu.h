@@ -928,7 +928,12 @@ int lzgpu_dev_sync(lzgpu_ctx *ctx);
 /* Deferred verification: a *_dev call that is given stored CRCs normally waits for its stream to report the verdict.  While
  * deferred mode is on it only enqueues (back-to-back calls keep the GPU busy), and the verdicts are collected by the next
  * lzgpu_dev_sync(ctx): LZGPU_ERR_CRC if any deferred call found a mismatch — the first one in call order, whose chunk / part /
- * block (relative to that call) lzgpu_last_bad returns.  Nothing is ever dropped: results must not be used before the sync. */
+ * block (relative to that call) lzgpu_last_bad returns.  Nothing is ever dropped: results must not be used before the sync.
+ * Calls from other threads: lzgpu_dev_sync collects every deferred call that returned before lzgpu_dev_sync was called, and also
+ * those that other threads make while it waits for the device; a call made later is left for the next sync.  A verdict is read
+ * only once the result copy of its own call has completed on that call's stream, however late the call was enqueued, so each
+ * mismatch is reported by exactly one sync and a slot is never reused before its call has finished with it.  The streams of
+ * deferred calls may be destroyed before the sync. */
 int lzgpu_ctx_set_deferred_verify(lzgpu_ctx *ctx, int enabled);
 int lzgpu_last_bad(lzgpu_ctx *ctx, int64_t *bad /* [3] */);
 /* page-locked host memory for staging buffers that feed the host-pointer entry points (H2D/D2H at full PCIe rate) */

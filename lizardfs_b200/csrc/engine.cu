@@ -116,6 +116,7 @@ static int ctx_init_resources(lzgpu_ctx *ctx) {
 		StatusSlot sl;
 		CUDA_TRY(cudaMalloc(&sl.d, sizeof(unsigned long long) * LZGPU_MAX_PARTS));
 		CUDA_TRY(cudaMallocHost(&sl.h, sizeof(unsigned long long) * LZGPU_MAX_PARTS));
+		CUDA_TRY(cudaEventCreateWithFlags(&sl.copied, cudaEventDisableTiming));
 		sl.index = i;
 		ctx->status_all.push_back(sl);
 		ctx->status_free.push_back(i);
@@ -176,6 +177,7 @@ extern "C" void lzgpu_ctx_destroy(lzgpu_ctx *ctx) {
 	for (auto &sl : ctx->status_all) {
 		if (sl.d) cudaFree(sl.d);
 		if (sl.h) cudaFreeHost(sl.h);
+		if (sl.copied) cudaEventDestroy(sl.copied);
 	}
 	for (auto &t : ctx->timing) {
 		if (t.e0) cudaEventDestroy(t.e0);
@@ -313,6 +315,7 @@ static int lz_status_acquire(lzgpu_ctx *ctx, StatusSlot *out) {
 		StatusSlot sl;
 		CUDA_TRY(cudaMalloc(&sl.d, sizeof(unsigned long long) * LZGPU_MAX_PARTS));
 		CUDA_TRY(cudaMallocHost(&sl.h, sizeof(unsigned long long) * LZGPU_MAX_PARTS));
+		CUDA_TRY(cudaEventCreateWithFlags(&sl.copied, cudaEventDisableTiming));
 		sl.index = static_cast<int>(ctx->status_all.size());
 		ctx->status_all.push_back(sl);
 		ctx->status_free.push_back(sl.index);
@@ -360,6 +363,7 @@ int VerifyTicket::publish(bool fused, int n_words, uint32_t blocks) {
 	n_words_ = n_words;
 	blocks_ = blocks;
 	CUDA_TRY(cudaMemcpyAsync(slot_.h, slot_.d, sizeof(unsigned long long) * n_words, cudaMemcpyDeviceToHost, st_));
+	CUDA_TRY(cudaEventRecord(slot_.copied, st_));
 	return LZGPU_OK;
 }
 
@@ -392,6 +396,17 @@ int VerifyTicket::take(int64_t *bad) {
 int VerifyTicket::wait_take(int64_t *bad) {
 	if (!armed()) return LZGPU_OK;
 	cudaError_t e = cudaStreamSynchronize(st_);
+	if (e != cudaSuccess) {
+		cudaGetLastError();
+		lz_set_error("CUDA error %s while waiting for the verification result", cudaGetErrorName(e));
+		return LZGPU_ERR_CUDA;  // the slot goes back when the owner is destroyed
+	}
+	return take(bad);
+}
+
+int VerifyTicket::wait_copied_take(int64_t *bad) {
+	if (!armed()) return LZGPU_OK;
+	cudaError_t e = cudaEventSynchronize(slot_.copied);
 	if (e != cudaSuccess) {
 		cudaGetLastError();
 		lz_set_error("CUDA error %s while waiting for the verification result", cudaGetErrorName(e));
@@ -2973,17 +2988,28 @@ extern "C" int lzgpu_dev_sync(lzgpu_ctx *ctx) {
 	if (!ctx) return LZGPU_ERR_ARG;
 	DeviceGuard g(ctx->device);
 	CUDA_TRY(cudaDeviceSynchronize());
-	// deferred verdicts, in call order: the first mismatch is the one reported, every slot is returned
-	std::lock_guard<std::mutex> lk(ctx->pending_mu);
+	// Deferred verdicts, in call order: the first mismatch is the one reported, every slot is returned.  Another thread may have
+	// enqueued a deferred call and pushed its ticket after the device synchronisation began, so an idle device says nothing about
+	// that call: each verdict is read only once its own result copy has completed.
+	std::vector<VerifyTicket> mine;
+	{
+		std::lock_guard<std::mutex> lk(ctx->pending_mu);
+		mine.swap(ctx->pending);
+	}
 	int rc = LZGPU_OK;
-	for (VerifyTicket &tk : ctx->pending) {
+	int64_t first[3] = {-1, -1, -1};
+	for (VerifyTicket &tk : mine) {
 		int64_t bad[3] = {-1, -1, -1};
-		const int r = tk.take(bad);
+		const int r = tk.wait_copied_take(bad);
 		if (r != LZGPU_OK && rc == LZGPU_OK) {
 			rc = r;
-			ctx->last_bad[0] = bad[0]; ctx->last_bad[1] = bad[1]; ctx->last_bad[2] = bad[2];
+			first[0] = bad[0]; first[1] = bad[1]; first[2] = bad[2];
 		}
 	}
-	ctx->pending.clear();
+	mine.clear();  // a ticket a CUDA error left armed waits for its stream here and returns its slot
+	if (rc != LZGPU_OK) {
+		std::lock_guard<std::mutex> lk(ctx->pending_mu);
+		ctx->last_bad[0] = first[0]; ctx->last_bad[1] = first[1]; ctx->last_bad[2] = first[2];
+	}
 	return rc;
 }

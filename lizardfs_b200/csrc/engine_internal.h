@@ -54,6 +54,7 @@ struct LzCounters {
 // never share a result word.
 struct StatusSlot {
 	unsigned long long *d = nullptr, *h = nullptr;
+	cudaEvent_t copied = nullptr;  // recorded on the call's stream right after the copy of the words to h
 	int index = -1;
 };
 
@@ -80,6 +81,9 @@ public:
 	int take(int64_t *bad);
 	// waits for the stream, then take(); LZGPU_OK at once when nothing is armed
 	int wait_take(int64_t *bad);
+	// waits for the copy of the words (the slot's event), then take(): lzgpu_dev_sync collects a deferred verdict this way, since
+	// the call that owns it may have been enqueued on another thread after the sync began, on a stream that may be gone by now
+	int wait_copied_take(int64_t *bad);
 
 private:
 	int publish(bool fused, int n_words, uint32_t blocks);
