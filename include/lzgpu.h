@@ -293,7 +293,8 @@ enum {
 	LZGPU_KERNEL_CHECK = 9,            /* fused_check_kernel: stripe check (lzgpu_check_stripes), one 16-warp CTA per SM */
 	LZGPU_KERNEL_CHECK_DEGRADED = 10,  /* fused_check_degraded_kernel: stripe map with lost data parts (lzgpu_check_stripe_map_degraded) */
 	LZGPU_KERNEL_ENCODE_SLICES = 11,   /* fused_slices_kernel: one-pass encode for several slices (lzgpu_encode_slices); G = combined stripes */
-	LZGPU_KERNEL_RECOVER_SLICES = 12   /* recover_slices_kernel: recovery from the parts of every slice (lzgpu_recover_slices); G = combined stripes */
+	LZGPU_KERNEL_RECOVER_SLICES = 12,  /* recover_slices_kernel: recovery from the parts of every slice (lzgpu_recover_slices); G = combined stripes */
+	LZGPU_KERNEL_SALVAGE_SLICES = 13   /* recover_slices_kernel, SALVAGE form: the determined blocks of a chunk (lzgpu_salvage_slices) */
 };
 typedef struct lzgpu_launch_geometry {
 	int kernel;
@@ -454,6 +455,55 @@ int lzgpu_recover_slices_dev(lzgpu_ctx *ctx, const lzgpu_goal *goals, uint32_t n
 int lzgpu_debug_recover_slices_rows(const lzgpu_goal *goals, uint32_t n_slices, const uint8_t *given, uint32_t valid, uint32_t *n_unknowns,
                                     uint32_t *n_equations, uint8_t *unk_pos, uint8_t *eq_slice, uint8_t *eq_row, uint8_t *eq_stripe,
                                     uint8_t *rows, uint64_t *determined);
+
+/* Salvage the blocks of lost chunks of a multi-slice goal that the surviving parts of all slices still determine, with a status byte per
+ * block.  lzgpu_recover_slices refuses a chunk whose given parts do not determine every block it must write (LZGPU_ERR_TOO_FEW_PARTS);
+ * this call takes such a chunk and writes what is still known: the blocks a given data part of some slice holds, and those the given
+ * parity blocks of several slices pin down.  For the operator's repair path: a salvaged image is never written back as if it were the
+ * chunk, since its holes are zeros, not data.
+ *   goals, n_slices, nb, parts, part_stride, part_crc   as in lzgpu_recover_slices: flat part numbering, layout, alignment, stored-CRC
+ *                     verification and the CRC-disabled mode.  Every chunk of a call has the same given parts.  Nothing is wanted.
+ *   image             chunk-order image of nb blocks, chunk c at + c * image_stride (image_stride covers nb blocks; _dev: a multiple of
+ *                     16): every block the given parts determine, zeros elsewhere.
+ *   image_crc         optional, block b of chunk c at [c * nb + b]: mycrc32 of every image block as written (the CRC of zeros for a HOLE
+ *                     or WITHHELD block); LZGPU_FAKE_CRC with CRCs disabled.
+ *   map               block b of chunk c at [c * nb + b]: LZGPU_SALVAGE_* below.  For each stripe shape KNOWN, SOLVED and HOLE are
+ *                     exactly the plan's masks (lzgpu_plan_salvage_slices; determined is lzgpu_plan_recover_slices' mask).
+ * A block that fails its stored CRC is never used: with F the given blocks of one combined stripe that fail, a position whose value
+ * depends on a block of F is WITHHELD (zeros).  A KNOWN position depends on its staged copy; a SOLVED one on every equation e whose
+ * coefficient in its solve row is not zero (lzgpu_debug_recover_slices_rows), that is on e's parity block and on the staged copies of
+ * the known positions of e's slice stripe.  The call does not solve again around F: run it again with the failing part set to NULL and
+ * merge the two maps (a block KNOWN or SOLVED in either is good).
+ * Refused before anything is enqueued: no part given (LZGPU_ERR_TOO_FEW_PARTS); arguments lzgpu_recover_slices refuses, no image or
+ * map, or a goal set whose salvage does not fit the kernel's tables (plan ok = 0) (LZGPU_ERR_ARG).  Holes are not an error.
+ * Returns LZGPU_ERR_CRC when a given block fails its stored CRC, with bad[0..3] the smallest (chunk, slice, part in the slice, block) as
+ * in lzgpu_recover_slices; unlike there, the image, image_crc and map are then still complete and valid.  Otherwise LZGPU_OK.  The _dev
+ * form follows lzgpu_recover_slices_dev: it waits only when stored CRCs are given, and deferred mode moves the wait to lzgpu_dev_sync
+ * (lzgpu_last_bad: chunk, flat part, block).  When every block is determined and no CRC fails, the image is byte for byte
+ * lzgpu_recover_slices' chunk_out.  One route, the SALVAGE instantiation of recover_slices_kernel, reported by
+ * lzgpu_debug_last_geometry as LZGPU_KERNEL_SALVAGE_SLICES (LZGPU_GRID_CAP applies).  lzgpu_pool_salvage_slices cuts the batch as
+ * lzgpu_pool_recover_slices: parts and part_crc move by slice, image by first * image_stride, image_crc and map by first * nb. */
+enum {
+	LZGPU_SALVAGE_HOLE = 0,     /* not determined by the given parts: zeros */
+	LZGPU_SALVAGE_KNOWN = 1,    /* copied from a given data part (the first given part in flat order that holds it) */
+	LZGPU_SALVAGE_SOLVED = 2,   /* solved from given parity blocks (csrc/slices_solve.h) */
+	LZGPU_SALVAGE_WITHHELD = 3  /* determined, but computed from a given block that fails its stored CRC: zeros */
+};
+typedef struct lzgpu_slices_salvage_plan {
+	uint64_t known, determined;            /* full combined stripe, as lzgpu_slices_recover_plan (bit q: position q) */
+	uint64_t tail_known, tail_determined;  /* the chunk's last, partial combined stripe (positions at or past nb: not in tail_known,
+	                                          set in tail_determined); equal to the above when L divides nb */
+	uint32_t L, tail_blocks;               /* as lzgpu_slices_recover_plan */
+	int ok;                                /* 1: the kernel takes this goal set with these given parts */
+	uint32_t G, threads, stages, smem_bytes; /* launch geometry, as lzgpu_debug_last_geometry reports it */
+} lzgpu_slices_salvage_plan;
+int lzgpu_plan_salvage_slices(const lzgpu_goal *goals, uint32_t n_slices, uint32_t nb, const uint8_t *given, lzgpu_slices_salvage_plan *out);
+int lzgpu_salvage_slices(lzgpu_ctx *ctx, const lzgpu_goal *goals, uint32_t n_slices, uint32_t n_chunks, uint32_t nb,
+                         const uint8_t *const *parts, const size_t *part_stride, const uint32_t *const *part_crc,
+                         uint8_t *image, size_t image_stride, uint32_t *image_crc, uint8_t *map, int64_t *bad /* [4] */);
+int lzgpu_salvage_slices_dev(lzgpu_ctx *ctx, const lzgpu_goal *goals, uint32_t n_slices, uint32_t n_chunks, uint32_t nb,
+                             const void *const *d_parts, const size_t *part_stride, const void *const *d_part_crc,
+                             void *d_image, size_t image_stride, void *d_image_crc, void *d_map, int64_t *bad /* host, [4] */, void *stream);
 
 /* Degraded read / rebuild of n_chunks chunks.
  *   parts[i]    (i < k+m) part-major buffer of part i for all chunks: chunk c at + c*part_stride,
@@ -768,6 +818,11 @@ int lzgpu_pool_recover_slices(lzgpu_pool *pool, const lzgpu_goal *goals, uint32_
                              /* lzgpu_recover_slices over every device of a pool, host memory only: for any input the code, bytes, CRCs,
                               * image and bad[0..3] lzgpu_recover_slices returns on one context for the whole batch (shares and merge as
                               * for the pool's stripe calls below) */
+int lzgpu_pool_salvage_slices(lzgpu_pool *pool, const lzgpu_goal *goals, uint32_t n_slices, uint32_t n_chunks, uint32_t nb,
+                              const uint8_t *const *parts, const size_t *part_stride, const uint32_t *const *part_crc,
+                              uint8_t *image, size_t image_stride, uint32_t *image_crc, uint8_t *map, int64_t *bad);
+                             /* lzgpu_salvage_slices over every device of a pool, host memory only: for any input the code, image,
+                              * image CRCs, map and bad[0..3] lzgpu_salvage_slices returns on one context for the whole batch */
 int lzgpu_convert_chunks_dev(lzgpu_ctx *ctx, const lzgpu_goal *src, const lzgpu_goal *dst, uint32_t n_chunks, uint32_t nb,
                              const void *const *d_parts, size_t part_stride, const void *const *d_part_crc,
                              const uint8_t *want, void *const *d_out, size_t out_stride, void *const *d_out_crc,

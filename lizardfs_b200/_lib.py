@@ -87,7 +87,7 @@ class LzEncoderKernel(C.Structure):
 # lzgpu_launch_geometry.kernel
 KERNEL_NONE, KERNEL_ENCODE, KERNEL_ENCODE_BITSLICE, KERNEL_RECOVER_GEO0, KERNEL_RECOVER_GEO1, KERNEL_RECOVER_GEO2, \
     KERNEL_RECOVER_DIRECT, KERNEL_RECOVER_BS3, KERNEL_CONVERT, KERNEL_CHECK, KERNEL_CHECK_DEGRADED, KERNEL_ENCODE_SLICES, \
-    KERNEL_RECOVER_SLICES = range(13)
+    KERNEL_RECOVER_SLICES, KERNEL_SALVAGE_SLICES = range(14)
 
 
 class LzSlicesRecoverPlan(C.Structure):
@@ -95,6 +95,16 @@ class LzSlicesRecoverPlan(C.Structure):
                 ("tail_blocks", C.c_uint32), ("unknowns", C.c_uint32), ("equations", C.c_uint32), ("tail_unknowns", C.c_uint32),
                 ("tail_equations", C.c_uint32), ("ok", C.c_int), ("G", C.c_uint32), ("threads", C.c_uint32), ("stages", C.c_uint32),
                 ("smem_bytes", C.c_uint32)]
+
+
+class LzSlicesSalvagePlan(C.Structure):
+    _fields_ = [("known", C.c_uint64), ("determined", C.c_uint64), ("tail_known", C.c_uint64), ("tail_determined", C.c_uint64),
+                ("L", C.c_uint32), ("tail_blocks", C.c_uint32), ("ok", C.c_int), ("G", C.c_uint32), ("threads", C.c_uint32),
+                ("stages", C.c_uint32), ("smem_bytes", C.c_uint32)]
+
+
+# lzgpu_salvage_slices' map bytes
+SALVAGE_HOLE, SALVAGE_KNOWN, SALVAGE_SOLVED, SALVAGE_WITHHELD = range(4)
 
 
 class LzStripeVerdict(C.Structure):
@@ -147,6 +157,7 @@ SIGNATURES = {
     "lzgpu_debug_repair_rows": (_int, [_int, _int, _vp, _vp, _int, _vp]),
     "lzgpu_plan_recover_slices": (_int, [_goalp, _u32, _u32, _vp, C.POINTER(LzSlicesRecoverPlan)]),
     "lzgpu_debug_recover_slices_rows": (_int, [_goalp, _u32, _vp, _u32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "lzgpu_plan_salvage_slices": (_int, [_goalp, _u32, _u32, _vp, C.POINTER(LzSlicesSalvagePlan)]),
     "lzgpu_debug_locate_errors": (_int, [_int, _int, _vp, _vp, _vp, _u32, _vp]),
     "lzgpu_goal_slice_type": (_int, [_goalp]),
     "lzgpu_goal_from_slice_type": (_int, [_int, _goalp]),
@@ -173,6 +184,8 @@ SIGNATURES = {
     "lzgpu_encode_slices_dev": (_int, [_vp, _goalp, _u32, _u32, _u32, _vp, _sz, _vp, _vp, _vp, _vp, _vp]),
     "lzgpu_recover_slices": (_int, [_vp, _goalp, _u32, _u32, _u32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
     "lzgpu_recover_slices_dev": (_int, [_vp, _goalp, _u32, _u32, _u32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _sz, _vp, _vp]),
+    "lzgpu_salvage_slices": (_int, [_vp, _goalp, _u32, _u32, _u32, _vp, _vp, _vp, _vp, _sz, _vp, _vp, _vp]),
+    "lzgpu_salvage_slices_dev": (_int, [_vp, _goalp, _u32, _u32, _u32, _vp, _vp, _vp, _vp, _sz, _vp, _vp, _vp, _vp]),
     "lzgpu_recover_chunks": (_int, [_vp, _goalp, _u32, _u32, _vp, _sz, _vp, _vp, _vp, _vp, _sz, _vp]),
     "lzgpu_recover_chunks_dev": (_int, [_vp, _goalp, _u32, _u32, _vp, _sz, _vp, _vp, _vp, _vp, _sz, _vp, _vp]),
     "lzgpu_check_stripes": (_int, [_vp, _goalp, _u32, _u32, _vp, _sz, _vp, _vp, _vp]),
@@ -255,6 +268,7 @@ SIGNATURES = {
     "lzgpu_pool_recover_chunks": (_int, [_vp, _goalp, _u32, _u32, _vp, _sz, _vp, _vp, _vp, _vp, _sz, _vp]),
     "lzgpu_pool_convert_chunks": (_int, [_vp, _goalp, _goalp, _u32, _u32, _vp, _sz, _vp, _vp, _vp, _sz, _vp, _vp]),
     "lzgpu_pool_recover_slices": (_int, [_vp, _goalp, _u32, _u32, _u32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
+    "lzgpu_pool_salvage_slices": (_int, [_vp, _goalp, _u32, _u32, _u32, _vp, _vp, _vp, _vp, _sz, _vp, _vp, _vp]),
     "lzgpu_pool_crc_blocks": (_int, [_vp, _vp, _sz, _u32, _sz, _vp]),
     "lzgpu_pool_check_stripes": (_int, [_vp, _goalp, _u32, _u32, _vp, _sz, _vp, _vp, _vp]),
     "lzgpu_pool_check_stripe_map": (_int, [_vp, _goalp, _u32, _u32, _vp, _sz, _vp, _vp, _vp]),

@@ -2161,23 +2161,31 @@ extern "C" int lzgpu_convert_chunks(lzgpu_ctx *ctx, const lzgpu_goal *src, const
 // ------------------------------------------------------------------------------------------------
 // recovery from the parts of every slice of a goal together (lzgpu_recover_slices*)
 // ------------------------------------------------------------------------------------------------
-// What the argument check derives for the enqueue: the flat part layout, the solve of both stripe shapes and the launch geometry
+// What the argument check derives for the enqueue: the flat part layout, the solve of both stripe shapes and the launch geometry.
+// salvage: the call is lzgpu_salvage_slices* (set by the caller before the check)
 struct RecoverSlicesCall {
 	lzd::SliceLayout lay;
 	lzd::SliceSolve shapes[2];   // a full combined stripe, the chunk's last one when L does not divide nb
 	lzd::RsGeometry geo;
 	uint32_t pb[kSlicesMax] = {0};
+	bool salvage = false;
 };
 
+// lzgpu_salvage_slices* want no part
+static const uint8_t kWantNone[LZGPU_MAX_PARTS] = {0};
+
 // The arguments of both forms, checked before anything is enqueued and whatever n_chunks is.  dev: the device form's alignment rules
-// (16-byte buffers and strides, 4-byte CRC arrays).  LZGPU_ERR_TOO_FEW_PARTS when a block the call must write is not determined.
+// (16-byte buffers and strides, 4-byte CRC arrays).  LZGPU_ERR_TOO_FEW_PARTS when a block the call must write is not determined; in the
+// salvage form (c.salvage; want = kWantNone, chunk_out the image) when no part is given, and the image and the map are required.
 static int recover_slices_args(const lzgpu_ctx *ctx, const lzgpu_goal *goals, uint32_t n_slices, uint32_t nb, const void *const *parts,
                                const size_t *part_stride, const void *const *part_crc, const uint8_t *want, const void *const *out,
                                const size_t *out_stride, const void *const *out_crc, const void *chunk_out, size_t chunk_out_stride, bool dev,
-                               RecoverSlicesCall &c) {
+                               RecoverSlicesCall &c, const void *image_crc = nullptr, const void *map = nullptr) {
 	if (!ctx || !parts || !part_stride || !want) return LZGPU_ERR_ARG;
+	const char *fn = c.salvage ? "salvage_slices" : "recover_slices";
+	if (c.salvage && (!chunk_out || !map)) { lz_set_error("salvage_slices: the image and the map are required"); return LZGPU_ERR_ARG; }
 	const char *why = nullptr;
-	if (lzd::slice_layout(goals, n_slices, c.lay, &why)) { lz_set_error("recover_slices: %s", why); return LZGPU_ERR_ARG; }
+	if (lzd::slice_layout(goals, n_slices, c.lay, &why)) { lz_set_error("%s: %s", fn, why); return LZGPU_ERR_ARG; }
 	if (nb == 0 || nb > LZGPU_BLOCKS_IN_CHUNK) { lz_set_error("nb out of range"); return LZGPU_ERR_ARG; }
 	const lzd::SliceLayout &lay = c.lay;
 	const size_t B = LZGPU_BLOCK_SIZE;
@@ -2188,7 +2196,7 @@ static int recover_slices_args(const lzgpu_ctx *ctx, const lzgpu_goal *goals, ui
 		for (uint32_t g = lay.base[i]; g < lay.base[i] + lay.k[i] + lay.m[i]; ++g) {
 			given[g] = parts[g] != nullptr;
 			if (given[g] && (part_stride[i] < bytes || (dev && (part_stride[i] & 15)))) {
-				lz_set_error("recover_slices: part_stride[%u] too small or not a multiple of 16", i);
+				lz_set_error("%s: part_stride[%u] too small or not a multiple of 16", fn, i);
 				return LZGPU_ERR_ARG;
 			}
 			if (!want[g]) continue;
@@ -2201,21 +2209,28 @@ static int recover_slices_args(const lzgpu_ctx *ctx, const lzgpu_goal *goals, ui
 		}
 	}
 	if (chunk_out && (chunk_out_stride < static_cast<size_t>(nb) * B || (dev && (chunk_out_stride & 15)))) {
-		lz_set_error("recover_slices: chunk_out_stride must cover nb blocks (and be a multiple of 16)");
+		lz_set_error(c.salvage ? "salvage_slices: image_stride must cover nb blocks (and be a multiple of 16)"
+		                       : "recover_slices: chunk_out_stride must cover nb blocks (and be a multiple of 16)");
 		return LZGPU_ERR_ARG;
 	}
 	if (dev) {
 		const int n = static_cast<int>(lay.n_parts);
 		int rc;
-		if ((rc = check_part_ptrs("recover_slices", "parts", parts, n, 16)) || (rc = check_part_ptrs("recover_slices", "out", out, n, 16)) ||
-		    (rc = check_part_ptrs("recover_slices", "part_crc", part_crc, n, 4)) || (rc = check_part_ptrs("recover_slices", "out_crc", out_crc, n, 4)))
+		if ((rc = check_part_ptrs(fn, "parts", parts, n, 16)) || (rc = check_part_ptrs(fn, "out", out, n, 16)) ||
+		    (rc = check_part_ptrs(fn, "part_crc", part_crc, n, 4)) || (rc = check_part_ptrs(fn, "out_crc", out_crc, n, 4)))
 			return rc;
-		if (reinterpret_cast<uintptr_t>(chunk_out) & 15) { lz_set_error("recover_slices: chunk_out is not 16-byte aligned"); return LZGPU_ERR_ARG; }
+		if (reinterpret_cast<uintptr_t>(chunk_out) & 15) { lz_set_error("%s: %s is not 16-byte aligned", fn, c.salvage ? "image" : "chunk_out"); return LZGPU_ERR_ARG; }
+		if (reinterpret_cast<uintptr_t>(image_crc) & 3) { lz_set_error("salvage_slices: image_crc is not 4-byte aligned"); return LZGPU_ERR_ARG; }
+	}
+	if (c.salvage) {
+		bool any = false;
+		for (uint32_t g = 0; g < lay.n_parts; ++g) any |= parts[g] != nullptr;
+		if (!any) { lz_set_error("salvage_slices: no part is given"); return LZGPU_ERR_TOO_FEW_PARTS; }
 	}
 	const uint32_t tail = nb % lay.L;
 	lzd::slice_solve(lay, given, lay.L, c.shapes[0]);
 	if (tail) lzd::slice_solve(lay, given, tail, c.shapes[1]);
-	for (int t = 0; t < 2; ++t) {
+	for (int t = 0; t < 2 && !c.salvage; ++t) {   // salvage writes what is determined, holes are not refused
 		if (t == 0 ? nb < lay.L : tail == 0) continue;   // a shape no chunk of the call has
 		const lzd::SliceSolve &sv = c.shapes[t];
 		const uint64_t lost = lzd::slice_needed(lay, want, chunk_out != nullptr, sv.valid) & ~sv.determined;
@@ -2226,19 +2241,21 @@ static int recover_slices_args(const lzgpu_ctx *ctx, const lzgpu_goal *goals, ui
 		}
 	}
 	const lzd::SliceSolve used[2] = {nb >= lay.L ? c.shapes[0] : c.shapes[1], tail ? c.shapes[1] : c.shapes[0]};
-	c.geo = lzd::rs_geometry(lay, given, used, 2);
+	c.geo = lzd::rs_geometry(lay, given, used, 2, c.salvage);
 	if (!c.geo.ok) {
-		lz_set_error("recover_slices: a combined stripe has more blocks than the kernel stages (%u slots, %u CRC streams)", c.geo.slots, c.geo.states);
+		lz_set_error("%s: a combined stripe has more blocks than the kernel stages (%u slots, %u CRC streams)", fn, c.geo.slots, c.geo.states);
 		return LZGPU_ERR_ARG;
 	}
 	return LZGPU_OK;
 }
 
-// DESIGN.md §4.8: read the given parts (+ their stored CRCs), write the wanted parts (+ their CRCs) and the image
+// DESIGN.md §4.8: read the given parts (+ their stored CRCs), write the wanted parts (+ their CRCs) and the image (+ the salvage form's
+// image CRCs and map)
 static uint64_t recover_slices_alg_bytes(const RecoverSlicesCall &c, uint32_t n_chunks, uint32_t nb, const void *const *parts, bool crcs,
-                                         const uint8_t *want, bool out_crcs, bool image) {
+                                         const uint8_t *want, bool out_crcs, bool image, bool image_crcs = false) {
 	const uint64_t B = LZGPU_BLOCK_SIZE;
 	uint64_t per_chunk = image ? static_cast<uint64_t>(nb) * B : 0;
+	if (c.salvage) per_chunk += static_cast<uint64_t>(nb) * (image_crcs ? 5 : 1);
 	for (uint32_t i = 0; i < c.lay.n_slices; ++i)
 		for (uint32_t g = c.lay.base[i]; g < c.lay.base[i] + c.lay.k[i] + c.lay.m[i]; ++g) {
 			if (parts[g]) per_chunk += c.pb[i] * (B + (crcs ? 4 : 0));
@@ -2261,16 +2278,33 @@ static void recover_slices_bad(const lzd::SliceLayout &lay, const int64_t *b3, i
 static int recover_slices_enqueue(lzgpu_ctx *ctx, const RecoverSlicesCall &c, uint32_t n_chunks, uint32_t nb, const void *const *d_parts,
                                   const size_t *part_stride, const void *const *d_part_crc, const uint8_t *want, void *const *d_out,
                                   const size_t *out_stride, void *const *d_out_crc, void *d_chunk_out, size_t chunk_out_stride, cudaStream_t st,
-                                  VerifyTicket *tk) {
+                                  VerifyTicket *tk, void *d_image_crc = nullptr, void *d_map = nullptr) {
 	bool verifying = false;
 	for (uint32_t g = 0; g < c.lay.n_parts; ++g) verifying |= d_parts[g] && d_part_crc && d_part_crc[g];
 	int rc;
 	if (verifying && (rc = tk->arm(ctx, st))) return rc;
 	if ((rc = lz_recover_slices(ctx, c.lay, c.shapes, c.geo, n_chunks, nb, d_parts, part_stride, verifying ? d_part_crc : nullptr, want, d_out,
-	                            out_stride, d_out_crc, d_chunk_out, chunk_out_stride, st, verifying ? tk->word(0) : nullptr)))
+	                            out_stride, d_out_crc, d_chunk_out, chunk_out_stride, d_image_crc, d_map, st, verifying ? tk->word(0) : nullptr)))
 		return rc;
 	ctx->stats.chunks_recovered += n_chunks;
 	return verifying ? tk->publish_fused() : LZGPU_OK;
+}
+
+// The device form of both calls, after their argument check
+static int recover_slices_dev_call(lzgpu_ctx *ctx, const RecoverSlicesCall &c, uint32_t n_chunks, uint32_t nb, const void *const *d_parts,
+                                   const size_t *part_stride, const void *const *d_part_crc, const uint8_t *want, void *const *d_out,
+                                   const size_t *out_stride, void *const *d_out_crc, void *d_chunk_out, size_t chunk_out_stride,
+                                   void *d_image_crc, void *d_map, int64_t *bad, void *stream) {
+	if (bad) bad[0] = bad[1] = bad[2] = bad[3] = -1;
+	int64_t b3[3] = {-1, -1, -1};
+	const int rc = dev_call(ctx, stream, recover_slices_alg_bytes(c, n_chunks, nb, d_parts, d_part_crc != nullptr, want, d_out_crc != nullptr,
+	                                                              d_chunk_out != nullptr, d_image_crc != nullptr),
+	                        b3, [&](cudaStream_t st, VerifyTicket *tk) {
+		                        return recover_slices_enqueue(ctx, c, n_chunks, nb, d_parts, part_stride, d_part_crc, want, d_out, out_stride, d_out_crc,
+		                                                      d_chunk_out, chunk_out_stride, st, tk, d_image_crc, d_map);
+	                        });
+	if (rc == LZGPU_ERR_CRC) recover_slices_bad(c.lay, b3, bad);
+	return rc;
 }
 
 extern "C" int lzgpu_recover_slices_dev(lzgpu_ctx *ctx, const lzgpu_goal *goals, uint32_t n_slices, uint32_t n_chunks, uint32_t nb,
@@ -2282,49 +2316,56 @@ extern "C" int lzgpu_recover_slices_dev(lzgpu_ctx *ctx, const lzgpu_goal *goals,
 	int rc = recover_slices_args(ctx, goals, n_slices, nb, d_parts, part_stride, d_part_crc, want, d_out, out_stride, d_out_crc, d_chunk_out,
 	                             chunk_out_stride, true, *c);
 	if (rc || n_chunks == 0) return rc;
-	if (bad) bad[0] = bad[1] = bad[2] = bad[3] = -1;
-	int64_t b3[3] = {-1, -1, -1};
-	rc = dev_call(ctx, stream, recover_slices_alg_bytes(*c, n_chunks, nb, d_parts, d_part_crc != nullptr, want, d_out_crc != nullptr, d_chunk_out != nullptr),
-	              b3, [&](cudaStream_t st, VerifyTicket *tk) {
-		              return recover_slices_enqueue(ctx, *c, n_chunks, nb, d_parts, part_stride, d_part_crc, want, d_out, out_stride, d_out_crc, d_chunk_out,
-		                                            chunk_out_stride, st, tk);
-	              });
-	if (rc == LZGPU_ERR_CRC) recover_slices_bad(c->lay, b3, bad);
-	return rc;
+	return recover_slices_dev_call(ctx, *c, n_chunks, nb, d_parts, part_stride, d_part_crc, want, d_out, out_stride, d_out_crc, d_chunk_out,
+	                               chunk_out_stride, nullptr, nullptr, bad, stream);
 }
 
-extern "C" int lzgpu_recover_slices(lzgpu_ctx *ctx, const lzgpu_goal *goals, uint32_t n_slices, uint32_t n_chunks, uint32_t nb,
-                                     const uint8_t *const *parts, const size_t *part_stride, const uint32_t *const *part_crc, const uint8_t *want,
-                                     uint8_t *const *out, const size_t *out_stride, uint32_t *const *out_crc, uint8_t *chunk_out,
-                                     size_t chunk_out_stride, int64_t *bad) {
-	NvtxScope nvtx_scope("lzgpu::recover_slices");
+extern "C" int lzgpu_salvage_slices_dev(lzgpu_ctx *ctx, const lzgpu_goal *goals, uint32_t n_slices, uint32_t n_chunks, uint32_t nb,
+                                         const void *const *d_parts, const size_t *part_stride, const void *const *d_part_crc, void *d_image,
+                                         size_t image_stride, void *d_image_crc, void *d_map, int64_t *bad, void *stream) {
+	NvtxScope nvtx_scope("lzgpu::salvage_slices_dev");
 	auto c = std::make_unique<RecoverSlicesCall>();
-	int rc = recover_slices_args(ctx, goals, n_slices, nb, reinterpret_cast<const void *const *>(parts), part_stride,
-	                             reinterpret_cast<const void *const *>(part_crc), want, reinterpret_cast<const void *const *>(out), out_stride,
-	                             reinterpret_cast<const void *const *>(out_crc), chunk_out, chunk_out_stride, false, *c);
+	c->salvage = true;
+	int rc = recover_slices_args(ctx, goals, n_slices, nb, d_parts, part_stride, d_part_crc, kWantNone, nullptr, nullptr, nullptr, d_image,
+	                             image_stride, true, *c, d_image_crc, d_map);
 	if (rc || n_chunks == 0) return rc;
+	return recover_slices_dev_call(ctx, *c, n_chunks, nb, d_parts, part_stride, d_part_crc, kWantNone, nullptr, nullptr, nullptr, d_image,
+	                               image_stride, d_image_crc, d_map, bad, stream);
+}
+
+// The host form of both calls, after their argument check: the given parts (+ stored CRCs) staged tile by tile, the wanted parts
+// (+ CRCs), the image and the salvage form's image CRCs and map copied back.  The salvage form runs every tile past a CRC mismatch, so
+// that its outputs are complete.
+static int recover_slices_host(lzgpu_ctx *ctx, const RecoverSlicesCall &c, uint32_t n_chunks, uint32_t nb, const uint8_t *const *parts,
+                               const size_t *part_stride, const uint32_t *const *part_crc, const uint8_t *want, uint8_t *const *out,
+                               const size_t *out_stride, uint32_t *const *out_crc, uint8_t *chunk_out, size_t chunk_out_stride,
+                               uint32_t *image_crc, uint8_t *map, int64_t *bad) {
+	int rc;
 	if (bad) bad[0] = bad[1] = bad[2] = bad[3] = -1;
-	const lzd::SliceLayout &lay = c->lay;
+	const lzd::SliceLayout &lay = c.lay;
 	const uint32_t n = lay.n_parts;
 	const size_t B = LZGPU_BLOCK_SIZE;
-	// device layout of a tile: every given part, then every wanted part, then the image, each dense (tile chunks of pb_i blocks); the
-	// stored and the computed CRCs likewise
+	// device layout of a tile: every given part, then every wanted part, then the image and the map, each dense (tile chunks of pb_i
+	// blocks, nb blocks, nb bytes); the stored and the computed CRCs likewise, the image CRCs last
 	size_t off[LZGPU_MAX_PARTS] = {0}, crc_off[LZGPU_MAX_PARTS] = {0}, bytes[LZGPU_MAX_PARTS] = {0}, per_chunk = 0, crc_words = 0;
 	size_t dstride[kSlicesMax] = {0};
 	for (uint32_t g = 0; g < n; ++g) {
 		const int i = lay.slice_of(g);
-		dstride[i] = static_cast<size_t>(c->pb[i]) * B;
+		dstride[i] = static_cast<size_t>(c.pb[i]) * B;
 		if (!parts[g] && !want[g]) continue;
 		bytes[g] = dstride[i];
 		off[g] = per_chunk;
 		per_chunk += bytes[g];
 		if ((parts[g] && part_crc && part_crc[g]) || (want[g] && out_crc && out_crc[g])) {
 			crc_off[g] = crc_words;
-			crc_words += c->pb[i];
+			crc_words += c.pb[i];
 		}
 	}
 	const size_t img_off = per_chunk, img_bytes = chunk_out ? static_cast<size_t>(nb) * B : 0;
 	per_chunk += img_bytes;
+	const size_t map_off = per_chunk, map_bytes = map ? nb : 0, img_crc_off = crc_words;
+	per_chunk += map_bytes;
+	if (image_crc) crc_words += nb;
 	std::lock_guard<std::mutex> lk(ctx->mu);
 	DeviceGuard dg(ctx->device);
 	AutoPin pin(ctx);
@@ -2334,6 +2375,8 @@ extern "C" int lzgpu_recover_slices(lzgpu_ctx *ctx, const lzgpu_goal *goals, uin
 		if (want[g]) pin.add(out[g], static_cast<size_t>(n_chunks - 1) * out_stride[i] + bytes[g]);
 	}
 	if (chunk_out) pin.add(chunk_out, static_cast<size_t>(n_chunks - 1) * chunk_out_stride + img_bytes);
+	if (image_crc) pin.add(image_crc, static_cast<size_t>(n_chunks) * nb * 4);
+	if (map) pin.add(map, static_cast<size_t>(n_chunks) * nb);
 	const uint32_t tile = static_cast<uint32_t>(std::max<size_t>(1, std::min<size_t>(n_chunks, (2 * kHostTileBytes) / std::max<size_t>(per_chunk, 1))));
 	const int n_slots = n_chunks > tile ? kHostSlots : 1;
 	void *d_in[kHostSlots], *d_crc[kHostSlots];
@@ -2354,7 +2397,7 @@ extern "C" int lzgpu_recover_slices(lzgpu_ctx *ctx, const lzgpu_goal *goals, uin
 				ctx->stats.bytes_h2d += nc * bytes[g];
 				dp[g] = buf;
 				if (part_crc && part_crc[g]) {
-					CUDA_TRY(cudaMemcpyAsync(cbuf, part_crc[g] + c0 * c->pb[i], nc * c->pb[i] * 4, cudaMemcpyHostToDevice, st));
+					CUDA_TRY(cudaMemcpyAsync(cbuf, part_crc[g] + c0 * c.pb[i], nc * c.pb[i] * 4, cudaMemcpyHostToDevice, st));
 					dpc[g] = cbuf;
 					any_crc = true;
 				}
@@ -2364,11 +2407,14 @@ extern "C" int lzgpu_recover_slices(lzgpu_ctx *ctx, const lzgpu_goal *goals, uin
 			}
 		}
 		void *dimg = chunk_out ? static_cast<uint8_t *>(d_in[s]) + tile * img_off : nullptr;
+		uint8_t *dmap = map ? static_cast<uint8_t *>(d_in[s]) + tile * map_off : nullptr;
+		uint32_t *dimg_crc = image_crc ? static_cast<uint32_t *>(d_crc[s]) + tile * img_crc_off : nullptr;
 		int rc;
 		{
-			BatchTimer timer(ctx, st, recover_slices_alg_bytes(*c, static_cast<uint32_t>(nc), nb, dp, any_crc, want, out_crc != nullptr, chunk_out != nullptr));
-			rc = recover_slices_enqueue(ctx, *c, static_cast<uint32_t>(nc), nb, dp, dstride, any_crc ? dpc : nullptr, want, dout, dstride,
-			                            out_crc ? docrc : nullptr, dimg, img_bytes, st, tk);
+			BatchTimer timer(ctx, st, recover_slices_alg_bytes(c, static_cast<uint32_t>(nc), nb, dp, any_crc, want, out_crc != nullptr, chunk_out != nullptr,
+			                                                   image_crc != nullptr));
+			rc = recover_slices_enqueue(ctx, c, static_cast<uint32_t>(nc), nb, dp, dstride, any_crc ? dpc : nullptr, want, dout, dstride,
+			                            out_crc ? docrc : nullptr, dimg, img_bytes, st, tk, dimg_crc, dmap);
 		}
 		if (rc) return rc;
 		for (uint32_t g = 0; g < n; ++g) {
@@ -2376,16 +2422,49 @@ extern "C" int lzgpu_recover_slices(lzgpu_ctx *ctx, const lzgpu_goal *goals, uin
 			const int i = lay.slice_of(g);
 			CUDA_TRY(cudaMemcpy2DAsync(out[g] + c0 * out_stride[i], out_stride[i], dout[g], bytes[g], bytes[g], nc, cudaMemcpyDeviceToHost, st));
 			ctx->stats.bytes_d2h += nc * bytes[g];
-			if (docrc[g]) CUDA_TRY(cudaMemcpyAsync(out_crc[g] + c0 * c->pb[i], docrc[g], nc * c->pb[i] * 4, cudaMemcpyDeviceToHost, st));
+			if (docrc[g]) CUDA_TRY(cudaMemcpyAsync(out_crc[g] + c0 * c.pb[i], docrc[g], nc * c.pb[i] * 4, cudaMemcpyDeviceToHost, st));
 		}
 		if (chunk_out) {
 			CUDA_TRY(cudaMemcpy2DAsync(chunk_out + c0 * chunk_out_stride, chunk_out_stride, dimg, img_bytes, img_bytes, nc, cudaMemcpyDeviceToHost, st));
 			ctx->stats.bytes_d2h += nc * img_bytes;
 		}
+		if (map) {
+			CUDA_TRY(cudaMemcpyAsync(map + c0 * nb, dmap, nc * nb, cudaMemcpyDeviceToHost, st));
+			ctx->stats.bytes_d2h += nc * nb;
+		}
+		if (image_crc) CUDA_TRY(cudaMemcpyAsync(image_crc + c0 * nb, dimg_crc, nc * nb * 4, cudaMemcpyDeviceToHost, st));
 		return LZGPU_OK;
-	});
+	}, c.salvage);
 	if (rc == LZGPU_ERR_CRC) recover_slices_bad(lay, b3, bad);
 	return rc;
+}
+
+extern "C" int lzgpu_recover_slices(lzgpu_ctx *ctx, const lzgpu_goal *goals, uint32_t n_slices, uint32_t n_chunks, uint32_t nb,
+                                     const uint8_t *const *parts, const size_t *part_stride, const uint32_t *const *part_crc, const uint8_t *want,
+                                     uint8_t *const *out, const size_t *out_stride, uint32_t *const *out_crc, uint8_t *chunk_out,
+                                     size_t chunk_out_stride, int64_t *bad) {
+	NvtxScope nvtx_scope("lzgpu::recover_slices");
+	auto c = std::make_unique<RecoverSlicesCall>();
+	int rc = recover_slices_args(ctx, goals, n_slices, nb, reinterpret_cast<const void *const *>(parts), part_stride,
+	                             reinterpret_cast<const void *const *>(part_crc), want, reinterpret_cast<const void *const *>(out), out_stride,
+	                             reinterpret_cast<const void *const *>(out_crc), chunk_out, chunk_out_stride, false, *c);
+	if (rc || n_chunks == 0) return rc;
+	return recover_slices_host(ctx, *c, n_chunks, nb, parts, part_stride, part_crc, want, out, out_stride, out_crc, chunk_out, chunk_out_stride,
+	                           nullptr, nullptr, bad);
+}
+
+extern "C" int lzgpu_salvage_slices(lzgpu_ctx *ctx, const lzgpu_goal *goals, uint32_t n_slices, uint32_t n_chunks, uint32_t nb,
+                                     const uint8_t *const *parts, const size_t *part_stride, const uint32_t *const *part_crc, uint8_t *image,
+                                     size_t image_stride, uint32_t *image_crc, uint8_t *map, int64_t *bad) {
+	NvtxScope nvtx_scope("lzgpu::salvage_slices");
+	auto c = std::make_unique<RecoverSlicesCall>();
+	c->salvage = true;
+	int rc = recover_slices_args(ctx, goals, n_slices, nb, reinterpret_cast<const void *const *>(parts), part_stride,
+	                             reinterpret_cast<const void *const *>(part_crc), kWantNone, nullptr, nullptr, nullptr, image, image_stride, false,
+	                             *c, image_crc, map);
+	if (rc || n_chunks == 0) return rc;
+	return recover_slices_host(ctx, *c, n_chunks, nb, parts, part_stride, part_crc, kWantNone, nullptr, nullptr, nullptr, image, image_stride,
+	                           image_crc, map, bad);
 }
 
 // ------------------------------------------------------------------------------------------------

@@ -329,9 +329,9 @@ static const struct {
 	SlicesKernel fn;
 } kSlicers[] = {{1, fused_slices_kernel<1>}, {2, fused_slices_kernel<2>}, {3, fused_slices_kernel<3>}, {4, fused_slices_kernel<4>}};
 
-// Recovery from the parts of every slice together (recover_slices_kernel): one instantiation, any goal set
+// Recovery from the parts of every slice together (recover_slices_kernel): one instantiation for any goal set, and its SALVAGE twin
 using RecoverSlicesKernel = void (*)(RecoverSlicesParams);
-static const RecoverSlicesKernel kRecoverSlicers[] = {recover_slices_kernel};
+static const RecoverSlicesKernel kRecoverSlicers[] = {recover_slices_kernel<false>, recover_slices_kernel<true>};
 
 // function attributes are per device: set once per context
 static int set_all_smem_attrs(const FusedState *fs) {
@@ -958,14 +958,15 @@ int lz_fused_encode_slices(lzgpu_ctx *ctx, const lzgpu_goal *goals, uint32_t n_s
 // recovery from the parts of every slice together (recover_slices_kernel.cuh)
 // ---------------------------------------------------------------------------------------------------
 
-// The kernel's tables for one stripe shape: what is read and staged, what is written, the CRC streams, the solve
+// The kernel's tables for one stripe shape: what is read and staged, what is written, the CRC streams, the solve.  image_crc: the
+// image blocks get CRC streams (the salvage form)
 static void rs_fill_shape(RsShape &o, const SliceLayout &lay, const SliceSolve &sv, const void *const *d_parts, const void *const *d_stored,
-                          const uint8_t *want, void *const *d_out_crc, bool image) {
+                          const uint8_t *want, void *const *d_out_crc, bool image, bool image_crc) {
 	const uint32_t L = lay.L, E = sv.n_eq;
 	std::memset(&o, 0, sizeof(o));
 	uint64_t staged = 0;
 	auto add_state = [&](uint8_t part, uint8_t s, uint8_t written) -> uint8_t {
-		o.state[o.n_state] = RsEntry{part, s, written, 0};
+		o.state[o.n_state] = RsEntry{part, s, written, static_cast<uint8_t>(written ? 0 : o.n_read)};   // a read block's: its read entry
 		return static_cast<uint8_t>(o.n_state++);
 	};
 	for (uint32_t i = 0; i < lay.n_slices; ++i)
@@ -984,7 +985,8 @@ static void rs_fill_shape(RsShape &o, const SliceLayout &lay, const SliceSolve &
 				}
 				const bool verify = d_stored && d_stored[g];
 				if (slot == kRsNone && !verify) continue;   // neither used nor verified: not read
-				o.read[o.n_read++] = RsEntry{static_cast<uint8_t>(g), static_cast<uint8_t>(s), slot, verify ? add_state(static_cast<uint8_t>(g), static_cast<uint8_t>(s), 0) : kRsNone};
+				const uint8_t st = verify ? add_state(static_cast<uint8_t>(g), static_cast<uint8_t>(s), 0) : kRsNone;   // names read entry n_read
+				o.read[o.n_read++] = RsEntry{static_cast<uint8_t>(g), static_cast<uint8_t>(s), slot, st};
 			}
 		}
 	for (uint32_t q = 0; q < L; ++q)
@@ -1016,13 +1018,48 @@ static void rs_fill_shape(RsShape &o, const SliceLayout &lay, const SliceSolve &
 			}
 		}
 	if (image)
-		for (uint32_t q = 0; q < sv.valid; ++q) o.write[o.n_write++] = RsEntry{kRsNone, static_cast<uint8_t>(q), static_cast<uint8_t>(q), kRsNone};
+		for (uint32_t q = 0; q < sv.valid; ++q)
+			o.write[o.n_write++] = RsEntry{kRsNone, static_cast<uint8_t>(q), static_cast<uint8_t>(q), image_crc ? add_state(kRsNone, static_cast<uint8_t>(q), 1) : kRsNone};
+}
+
+// The salvage form's masks for one stripe shape, from the tables rs_fill_shape made of it: a known position depends on the read entry
+// that staged it; a solved one on every equation its row uses (rows[x][e] != 0), i.e. on that equation's parity block and on the
+// staged known positions of its slice stripe.  Status from the solve's masks.
+static void rs_fill_salvage(RsSalvage &o, const RsShape &sh, const SliceLayout &lay, const SliceSolve &sv) {
+	const uint32_t L = lay.L, E = sv.n_eq;
+	std::memset(&o, 0, sizeof(o));
+	int stager[kRsMaxL], eq_read[kRsMaxL];
+	for (uint32_t q = 0; q < L; ++q) stager[q] = eq_read[q] = -1;
+	for (uint32_t r = 0; r < sh.n_read; ++r) {
+		const uint32_t slot = sh.read[r].slot;
+		if (slot == kRsNone) continue;
+		if (slot < L) stager[slot] = static_cast<int>(r);
+		else eq_read[slot - L] = static_cast<int>(r);
+	}
+	auto depend = [&](uint32_t q, int r) {
+		if (r >= 0) o.dep[q][r >> 5] |= 1u << (r & 31);
+	};
+	for (uint32_t q = 0; q < sv.valid; ++q) {
+		const bool known = (sv.known >> q) & 1ull, determined = (sv.determined >> q) & 1ull;
+		o.status[q] = known ? LZGPU_SALVAGE_KNOWN : determined ? LZGPU_SALVAGE_SOLVED : LZGPU_SALVAGE_HOLE;
+		if (known) depend(q, stager[q]);
+	}
+	for (uint32_t x = 0; x < sv.n_unknown; ++x) {
+		const uint32_t q = sv.unk_pos[x];
+		for (uint32_t e = 0; e < E; ++e) {
+			if (!sv.rows[x][e]) continue;
+			const uint32_t i = sv.eq_slice[e], s = sv.eq_stripe[e];
+			depend(q, eq_read[e]);
+			for (uint32_t j = 0; j < lay.k[i]; ++j)
+				if (s * lay.k[i] + j < sv.valid && ((sv.known >> (s * lay.k[i] + j)) & 1ull)) depend(q, stager[s * lay.k[i] + j]);
+		}
+	}
 }
 
 int lz_recover_slices(lzgpu_ctx *ctx, const SliceLayout &lay, const SliceSolve *shapes, const RsGeometry &geo, uint32_t n_chunks, uint32_t nb,
                       const void *const *d_parts, const size_t *part_stride, const void *const *d_part_crc, const uint8_t *want, void *const *d_out,
-                      const size_t *out_stride, void *const *d_out_crc, void *d_image, size_t image_stride, cudaStream_t st,
-                      unsigned long long *d_first_bad) {
+                      const size_t *out_stride, void *const *d_out_crc, void *d_image, size_t image_stride, void *d_image_crc, void *d_map,
+                      cudaStream_t st, unsigned long long *d_first_bad) {
 	auto p = std::make_unique<RecoverSlicesParams>();
 	std::memset(p.get(), 0, sizeof(RecoverSlicesParams));
 	const bool crc_on = lzgpu_crc_enabled() != 0;
@@ -1059,9 +1096,14 @@ int lz_recover_slices(lzgpu_ctx *ctx, const SliceLayout &lay, const SliceSolve *
 	for (int i = 0; i < 5; ++i) p->tree_mult[i] = lz::crc_xpow_bytes(2048ull << i);
 	const bool verifying = d_part_crc != nullptr;
 	if (verifying && !d_first_bad) return LZGPU_ERR_ARG;  // (cannot happen: the caller arms a ticket whenever it passes stored CRCs)
+	const bool salvage = d_map != nullptr;
+	p->image_crc = static_cast<uint32_t *>(d_image_crc);
+	p->map = static_cast<uint8_t *>(d_map);
 	for (int t = 0; t < 2; ++t)
-		if (t == 0 ? nb >= lay.L : p->tail != 0)
-			rs_fill_shape(p->shape[t], lay, shapes[t], d_parts, d_part_crc, want, d_out_crc, d_image != nullptr);
-	const lzgpu_launch_geometry g = launch_geo(LZGPU_KERNEL_RECOVER_SLICES, geo.threads, geo.G, geo.stages, 0, geo.smem);
-	return launch(ctx, kRecoverSlicers[0], g, 1, p->total_units, st, *p);
+		if (t == 0 ? nb >= lay.L : p->tail != 0) {
+			rs_fill_shape(p->shape[t], lay, shapes[t], d_parts, d_part_crc, want, d_out_crc, d_image != nullptr, d_image_crc != nullptr);
+			if (salvage) rs_fill_salvage(p->salvage[t], p->shape[t], lay, shapes[t]);
+		}
+	const lzgpu_launch_geometry g = launch_geo(salvage ? LZGPU_KERNEL_SALVAGE_SLICES : LZGPU_KERNEL_RECOVER_SLICES, geo.threads, geo.G, geo.stages, 0, geo.smem);
+	return launch(ctx, kRecoverSlicers[salvage ? 1 : 0], g, 1, p->total_units, st, *p);
 }

@@ -638,6 +638,32 @@ int lzgpu_plan_recover_slices(const lzgpu_goal *goals, uint32_t n_slices, uint32
 	return LZGPU_OK;
 }
 
+int lzgpu_plan_salvage_slices(const lzgpu_goal *goals, uint32_t n_slices, uint32_t nb, const uint8_t *given, lzgpu_slices_salvage_plan *out) {
+	if (!out || !given || nb == 0 || nb > LZGPU_BLOCKS_IN_CHUNK) return LZGPU_ERR_ARG;
+	*out = lzgpu_slices_salvage_plan{};
+	lzd::SliceLayout lay;
+	const char *why = nullptr;
+	if (lzd::slice_layout(goals, n_slices, lay, &why) != LZGPU_OK) return LZGPU_ERR_ARG;
+	lzd::SliceSolve sv[2];
+	lzd::slice_solve(lay, given, lay.L, sv[0]);
+	const uint32_t tail = nb % lay.L;
+	if (tail) lzd::slice_solve(lay, given, tail, sv[1]);
+	out->L = lay.L;
+	out->tail_blocks = tail;
+	out->known = sv[0].known;
+	out->determined = sv[0].determined;
+	out->tail_known = tail ? sv[1].known : sv[0].known;
+	out->tail_determined = tail ? sv[1].determined : sv[0].determined;
+	const lzd::SliceSolve used[2] = {nb >= lay.L ? sv[0] : sv[1], tail ? sv[1] : sv[0]};
+	const lzd::RsGeometry g = lzd::rs_geometry(lay, given, used, 2, true);
+	out->ok = g.ok ? 1 : 0;
+	out->G = g.G;
+	out->threads = g.threads;
+	out->stages = g.stages;
+	out->smem_bytes = static_cast<uint32_t>(g.smem);
+	return LZGPU_OK;
+}
+
 int lzgpu_debug_recover_slices_rows(const lzgpu_goal *goals, uint32_t n_slices, const uint8_t *given, uint32_t valid, uint32_t *n_unknowns,
                                     uint32_t *n_equations, uint8_t *unk_pos, uint8_t *eq_slice, uint8_t *eq_row, uint8_t *eq_stripe,
                                     uint8_t *rows, uint64_t *determined) {

@@ -17,6 +17,12 @@
 //   store   warp w takes write entries: the wanted data and parity blocks (CRC folded when out_crc is given) and the image
 // At the end of a combined stripe every CRC stream is merged; a read block is compared with its stored CRC (the smallest mismatch,
 // (chunk * 64 + flat part) * 1024 + block, lowers the result word), a written block's CRC is stored.
+//
+// The SALVAGE instantiation (lzgpu_salvage_slices) writes the image only, with a CRC stream per image block, whatever the given parts
+// determine: an undetermined unknown has an all-zero solve row, so it comes out as zeros.  A read block that fails its stored CRC also
+// sets its read entry's bit in a shared mask; after the merge every position whose value depends on a failing read entry (the host's
+// dependency mask, RsSalvage) is withheld: the CTA zeroes its image block, which it stored earlier in the stripe, and gives it the CRC
+// of zeros.  Then the stripe's status bytes are written to the map.
 #pragma once
 #include <cstdint>
 
@@ -35,7 +41,7 @@ struct RsEntry {
 	uint8_t part;   // flat part (read / written); kRsNone: the image
 	uint8_t s;      // stripe of the part's slice in the combined stripe; the image: the position
 	uint8_t slot;   // staged slab slot: position q < L, L + e (equation e), L + E + w (wanted parity block w); kRsNone: not staged
-	uint8_t state;  // CRC stream; kRsNone: none
+	uint8_t state;  // CRC stream; kRsNone: none.  In a stream entry of a read block: that block's read entry
 };
 
 struct RsShape {
@@ -47,6 +53,14 @@ struct RsShape {
 	uint8_t eq_slice[kRsMaxL], eq_row[kRsMaxL], eq_stripe[kRsMaxL];
 	uint8_t out_slice[kRsMaxOut], out_row[kRsMaxOut], out_stripe[kRsMaxOut];
 	uint8_t rows[kRsMaxL][kRsMaxL];
+};
+
+// lzgpu_salvage_slices, per stripe shape: bit r of dep[q] = the value of position q depends on read entry r (its staged copy, or a
+// chosen equation's parity block or known position that its solve row uses); status[q] = LZGPU_SALVAGE_KNOWN / _SOLVED / _HOLE
+constexpr uint32_t kRsMaskWords = kRsMaxEntries / 32;
+struct RsSalvage {
+	uint32_t dep[kRsMaxL][kRsMaskWords];
+	uint8_t status[kRsMaxL];
 };
 
 struct RecoverSlicesParams {
@@ -64,7 +78,18 @@ struct RecoverSlicesParams {
 	uint32_t L, G, nb, n_cs, units_per_chunk, total_units, tail, n_slots, n_states_max, crc_off, zconst;
 	uint32_t tree_mult[5];
 	RsShape shape[2];   // 0: a full combined stripe, 1: the chunk's last one when L does not divide nb
+	// the SALVAGE instantiation only: the image's block CRCs (nullptr: none) and status bytes, block c * nb + b, and the shapes' masks
+	uint32_t *image_crc;
+	uint8_t *map;
+	RsSalvage salvage[2];
 };
+static_assert(sizeof(RecoverSlicesParams) <= 32764, "recover_slices_kernel's parameter block must fit the 32764-byte kernel parameter limit");
+
+// The per-stripe shared words of the SALVAGE instantiation: the failing read entries, then the withheld positions
+__device__ __forceinline__ uint32_t *rs_salvage_smem() {
+	__shared__ uint32_t words[kRsMaskWords + 2];
+	return words;
+}
 
 // c * v for the four bytes of v; c is uniform across the CTA
 __device__ __forceinline__ uint32_t rs_gf_mul(uint32_t v, uint32_t c) {
@@ -78,6 +103,7 @@ __device__ __forceinline__ uint32_t rs_gf_mul(uint32_t v, uint32_t c) {
 	return r;
 }
 
+template <bool SALVAGE>
 __global__ void __launch_bounds__(kRsThreads, 1) recover_slices_kernel(const __grid_constant__ RecoverSlicesParams p) {
 	extern __shared__ __align__(1024) uint8_t smem[];
 	uint32_t *s_tab = reinterpret_cast<uint32_t *>(smem);
@@ -97,6 +123,8 @@ __global__ void __launch_bounds__(kRsThreads, 1) recover_slices_kernel(const __g
 			const uint32_t E = sh.n_eq;
 			__syncthreads();   // the previous stripe's streams are merged
 			for (uint32_t i = tid; i < sh.n_state * 32u; i += kRsThreads) s_crc[i] = 0;
+			if constexpr (SALVAGE)
+				if (tid < kRsMaskWords + 2) rs_salvage_smem()[tid] = 0;
 			__syncthreads();
 			for (uint32_t slab = 0; slab < 64; ++slab) {
 				const uint32_t off = lane * 2048 + slab * 32;
@@ -178,6 +206,12 @@ __global__ void __launch_bounds__(kRsThreads, 1) recover_slices_kernel(const __g
 				}
 				if (lane != 0) continue;
 				const RsEntry en = sh.state[z];
+				if constexpr (SALVAGE) {
+					if (en.part == kRsNone) {   // an image block; a withheld one is given the CRC of zeros below
+						p.image_crc[static_cast<unsigned long long>(c) * p.nb + cs * L + en.s] = p.crc_off ? LZGPU_FAKE_CRC : (st ^ p.zconst);
+						continue;
+					}
+				}
 				const uint32_t i = p.part_slice[en.part];
 				const unsigned long long blk = static_cast<unsigned long long>(cs) * p.spc[i] + en.s;
 				const unsigned long long at = static_cast<unsigned long long>(c) * p.pb[i] + blk;
@@ -186,6 +220,31 @@ __global__ void __launch_bounds__(kRsThreads, 1) recover_slices_kernel(const __g
 					p.out_crc[en.part][at] = crc;
 				} else if (p.stored[en.part][at] != crc) {
 					atomicMin(p.first_bad, (static_cast<unsigned long long>(c) * 64ull + en.part) * 1024ull + blk);
+					if constexpr (SALVAGE) atomicOr(&rs_salvage_smem()[en.state >> 5], 1u << (en.state & 31));
+				}
+			}
+			if constexpr (SALVAGE) {
+				// ---------------- withhold what depends on a failing block, then the stripe's map bytes ----------------
+				__syncthreads();
+				uint32_t *fail = rs_salvage_smem(), *withheld = fail + kRsMaskWords;
+				const RsSalvage &sv = p.salvage[(p.tail && cs == p.n_cs - 1) ? 1 : 0];
+				const uint32_t valid = min(L, p.nb - cs * L);
+				const unsigned long long b0 = static_cast<unsigned long long>(c) * p.nb + cs * L;
+				if (tid < valid) {
+					bool w = false;
+#pragma unroll
+					for (uint32_t i = 0; i < kRsMaskWords; ++i) w |= (fail[i] & sv.dep[tid][i]) != 0;
+					p.map[b0 + tid] = w ? LZGPU_SALVAGE_WITHHELD : sv.status[tid];
+					if (w) {
+						if (p.image_crc) p.image_crc[b0 + tid] = p.crc_off ? LZGPU_FAKE_CRC : p.zconst;
+						atomicOr(&withheld[tid >> 5], 1u << (tid & 31));
+					}
+				}
+				__syncthreads();
+				for (uint32_t q = 0; q < valid; ++q) {
+					if (!((withheld[q >> 5] >> (q & 31)) & 1u)) continue;
+					uint4 *dst = reinterpret_cast<uint4 *>(p.image + c * p.image_stride + (static_cast<unsigned long long>(cs * L + q) << 16));
+					for (uint32_t i = tid; i < 65536u / 16u; i += kRsThreads) dst[i] = make_uint4(0, 0, 0, 0);
 				}
 			}
 		}

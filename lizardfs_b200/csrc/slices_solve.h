@@ -195,7 +195,8 @@ inline uint64_t slice_needed(const SliceLayout &lay, const uint8_t *want, bool i
 
 // Launch geometry of recover_slices_kernel (recover_slices_kernel.cuh), sized for the largest request the given parts allow (every
 // part that is not given wanted, with its CRCs, and the image), so that it does not depend on `want`: one 256-thread CTA per SM, a
-// unit of G combined stripes, shared memory = the CRC tables + one 1 KiB slab per staged block + 128 bytes per CRC stream.
+// unit of G combined stripes, shared memory = the CRC tables + one 1 KiB slab per staged block + 128 bytes per CRC stream.  salvage:
+// the largest salvage request instead (lzgpu_salvage_slices: nothing wanted, every given part verified, the image with its CRCs).
 constexpr uint32_t kRsThreadsPerCta = 256, kRsEntryCap = 192, kRsOutCap = 64;
 constexpr size_t kRsSmemCap = 220 * 1024;
 struct RsGeometry {
@@ -204,7 +205,7 @@ struct RsGeometry {
 	size_t smem = 0;
 };
 
-inline RsGeometry rs_geometry(const SliceLayout &lay, const uint8_t *given, const SliceSolve *shapes, int n_shapes) {
+inline RsGeometry rs_geometry(const SliceLayout &lay, const uint8_t *given, const SliceSolve *shapes, int n_shapes, bool salvage = false) {
 	RsGeometry g;
 	g.G = lay.L >= 8 ? 1 : 8 / lay.L;
 	g.threads = kRsThreadsPerCta;
@@ -217,10 +218,10 @@ inline RsGeometry rs_geometry(const SliceLayout &lay, const uint8_t *given, cons
 				if (!stripe_exists(lay, i, s, sv.valid)) continue;
 				for (uint32_t p = 0; p < lay.k[i] + lay.m[i]; ++p) {
 					if (given[lay.base[i] + p]) ++reads;
-					else { ++writes; outs += p >= lay.k[i] ? 1 : 0; }
+					else if (!salvage) { ++writes; outs += p >= lay.k[i] ? 1 : 0; }
 				}
 			}
-		const uint32_t states = reads + writes - sv.valid;
+		const uint32_t states = salvage ? reads + sv.valid : reads + writes - sv.valid;
 		fits = fits && reads <= kRsEntryCap && writes <= kRsEntryCap && states <= kRsEntryCap && outs <= kRsOutCap;
 		g.slots = std::max(g.slots, lay.L + sv.n_eq + outs);
 		g.states = std::max(g.states, states);

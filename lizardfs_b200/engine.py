@@ -198,6 +198,23 @@ def _recover_slices(fn, h, goals, nb, parts, part_crc, want, chunk_image, with_c
     return out, ocrc, img
 
 
+def _salvage_slices(fn, h, goals, nb, parts, part_crc, with_crc):
+    pbs = [-(-nb // g.k) for g in goals]
+    slice_of = [i for i, g in enumerate(goals) for _ in range(1 if g.is_std else g.k + g.m)]
+    assert len(parts) == len(slice_of)
+    arrs = [None if p is None else _u8(p).reshape(-1, pbs[slice_of[j]] * BLOCK_SIZE) for j, p in enumerate(parts)]
+    n = next((a.shape[0] for a in arrs if a is not None), 0)
+    crcs = None if part_crc is None else _ptr_array([None if c is None else np.ascontiguousarray(c, dtype=np.uint32) for c in part_crc])
+    img = np.zeros((n, nb * BLOCK_SIZE), dtype=np.uint8)
+    icrc = np.zeros((n, nb), dtype=np.uint32) if with_crc else None
+    smap = np.zeros((n, nb), dtype=np.uint8)
+    strides = (C.c_size_t * len(goals))(*[pb * BLOCK_SIZE for pb in pbs])
+    bad = (C.c_int64 * 4)(-1, -1, -1, -1)
+    rc = fn(h, _goal_array(goals), len(goals), n, nb, _ptr_array(arrs), strides, crcs, _p(img), nb * BLOCK_SIZE, _p(icrc), _p(smap), bad)
+    _check_crc(rc, _name(fn), bad, image=img, image_crc=icrc, map=smap)
+    return img, icrc, smap
+
+
 def _part_batch(fn, h, goal, nb, parts, part_crc, result, attr, in_place=False):
     # the host-pointer check, map and correction: result(n_chunks, pb) makes the array the call fills, which is returned, and
     # attached to a ChunkCrcError as `attr`
@@ -446,6 +463,11 @@ class Pool:
         the whole batch; ChunkCrcError.where = (chunk in the batch, slice, part, block)"""
         return _recover_slices(self.lib.lzgpu_pool_recover_slices, self.h, goals, nb, parts, part_crc, want, chunk_image, with_crc)
 
+    def salvage_slices(self, goals, nb, parts, part_crc=None, with_crc=True):
+        """Engine.salvage_slices over every device of the pool (lzgpu_pool_salvage_slices): the same arguments, results and errors for
+        the whole batch; ChunkCrcError.where = (chunk in the batch, slice, part, block)"""
+        return _salvage_slices(self.lib.lzgpu_pool_salvage_slices, self.h, goals, nb, parts, part_crc, with_crc)
+
     def crc_blocks(self, data, block_len=BLOCK_SIZE):
         data = _u8(data).reshape(-1, block_len)
         out = np.empty(data.shape[0], dtype=np.uint32)
@@ -687,6 +709,35 @@ class Engine:
                                                _dev_ptrs(d_part_crc, n), _p(w), _dev_ptrs(d_out, n), (C.c_size_t * ns)(*out_stride),
                                                _dev_ptrs(d_out_crc, n), d_chunk_out, chunk_out_stride, bad, stream)
         _check_crc(rc, "recover_slices_dev", bad)
+
+    def salvage_slices(self, goals, nb, parts, part_crc=None, with_crc=True):
+        """Salvage the blocks of lost chunks of a multi-slice goal that the given parts of every slice still determine
+        (lzgpu_salvage_slices).  goals, parts, part_crc as in recover_slices.  Returns (image, image_crc, map): image [n_chunks, nb * 64K]
+        with every determined block and zeros elsewhere, image_crc [n_chunks, nb] uint32 (None without with_crc), map [n_chunks, nb]
+        of _lib.SALVAGE_* per block.  Raises LzGpuError(ERR_TOO_FEW_PARTS) when no part is given; on a stored-CRC mismatch
+        ChunkCrcError (.where = chunk, slice, part, block) with the still complete results as .image, .image_crc and .map."""
+        return _salvage_slices(self.lib.lzgpu_salvage_slices, self.h, goals, nb, parts, part_crc, with_crc)
+
+    def salvage_slices_dev(self, goals, n_chunks, nb, d_parts, part_stride, d_part_crc, d_image, image_stride, d_image_crc, d_map,
+                           stream=None):
+        """lzgpu_salvage_slices_dev: d_parts / d_part_crc are lists over the flat parts (device pointers as ints, 0 or None = absent),
+        part_stride one entry per slice; d_image_crc may be None.  Raises ChunkCrcError (.where = chunk, slice, part, block); the device
+        results are then still complete."""
+        ns, n = len(goals), sum(1 if g.is_std else g.k + g.m for g in goals)
+        bad = (C.c_int64 * 4)(-1, -1, -1, -1)
+        rc = self.lib.lzgpu_salvage_slices_dev(self.h, _goal_array(goals), ns, n_chunks, nb, _dev_ptrs(d_parts, n), (C.c_size_t * ns)(*part_stride),
+                                               _dev_ptrs(d_part_crc, n), d_image, image_stride, d_image_crc, d_map, bad, stream)
+        _check_crc(rc, "salvage_slices_dev", bad)
+
+    @staticmethod
+    def plan_salvage_slices(goals, nb, given):
+        """what salvage_slices writes from the given flat parts (pure host logic, csrc/slices_solve.h; no GPU needed): dict with known,
+        determined, tail_known, tail_determined (bit q: combined-stripe position q), L, tail_blocks, ok and the launch geometry G,
+        threads, stages, smem_bytes"""
+        out = _lib.LzSlicesSalvagePlan()
+        g = np.asarray(given, dtype=np.uint8)
+        _check(_lib.load().lzgpu_plan_salvage_slices(_goal_array(goals), len(goals), nb, _p(g), C.byref(out)), "plan_salvage_slices")
+        return {f: getattr(out, f) for f, _ in _lib.LzSlicesSalvagePlan._fields_}
 
     @staticmethod
     def plan_recover_slices(goals, nb, given):

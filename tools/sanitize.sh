@@ -129,6 +129,29 @@ for c in range(5):
     p_ref, c_ref = o.encode_chunk(g.kind, g.k, g.m, data[c])
     assert (par[c] == p_ref).all() and (crc[c] == c_ref).all()
 pool.close()
+# the salvage of a multi-slice chunk (recover_slices_kernel, SALVAGE form): xor2 + xor3 with xor2's parity and xor3's data part 0
+# given (positions 1, 2 solved, 4, 5 holes), a tail stripe, and one corrupt byte in xor3 part 0 so that its dependents are withheld
+goals = [L.SliceType("xor2"), L.SliceType("xor3")]
+nblk = 14
+data = np.stack([O.fill_chunk(o, nblk * 65536, 31, c) for c in range(2)])
+enc = eng.encode_slices(goals, data)
+sparts = []
+for g, (par, crc) in zip(goals, enc):
+    pb = -(-nblk // g.k)
+    padded = np.zeros((2, pb * g.k * 65536), dtype=np.uint8)
+    padded[:, :nblk * 65536] = data
+    sparts += [np.ascontiguousarray(padded.reshape(2, pb, g.k, 65536)[:, :, j]).reshape(2, -1) for j in range(g.k)] + [par[:, 0]]
+given = [0, 0, 1, 1, 0, 0, 0]
+img, icrc, smap = eng.salvage_slices(goals, nblk, [p if x else None for p, x in zip(sparts, given)])
+assert (smap == 2).any() and (smap == 0).any()
+rot = sparts[3].copy()
+rot[1, 70000] ^= 1
+scrc = [eng.crc_blocks(p.reshape(-1)).reshape(2, -1) if x else None for p, x in zip(sparts, given)]
+try:
+    eng.salvage_slices(goals, nblk, [rot if g == 3 else (p if x else None) for g, (p, x) in enumerate(zip(sparts, given))], scrc)
+    raise AssertionError("the corrupt block passed")
+except L.ChunkCrcError as e:
+    assert (e.map == 3).any()
 print("sanitizer case OK")
 PY
 for tool in ${TOOLS:-memcheck racecheck synccheck}; do
