@@ -294,7 +294,8 @@ enum {
 	LZGPU_KERNEL_CHECK_DEGRADED = 10,  /* fused_check_degraded_kernel: stripe map with lost data parts (lzgpu_check_stripe_map_degraded) */
 	LZGPU_KERNEL_ENCODE_SLICES = 11,   /* fused_slices_kernel: one-pass encode for several slices (lzgpu_encode_slices); G = combined stripes */
 	LZGPU_KERNEL_RECOVER_SLICES = 12,  /* recover_slices_kernel: recovery from the parts of every slice (lzgpu_recover_slices); G = combined stripes */
-	LZGPU_KERNEL_SALVAGE_SLICES = 13   /* recover_slices_kernel, SALVAGE form: the determined blocks of a chunk (lzgpu_salvage_slices) */
+	LZGPU_KERNEL_SALVAGE_SLICES = 13,  /* recover_slices_kernel, SALVAGE form: the determined blocks of a chunk (lzgpu_salvage_slices) */
+	LZGPU_KERNEL_CHECK_SLICES = 14     /* recover_slices_kernel, CHECK form: the consistency map of several slices (lzgpu_check_slices) */
 };
 typedef struct lzgpu_launch_geometry {
 	int kernel;
@@ -422,8 +423,8 @@ int lzgpu_pool_encode_slices(lzgpu_pool *pool, const lzgpu_goal *goals, uint32_t
  *   chunk_out         optional chunk-order image of nb blocks, chunk c at + c * chunk_out_stride.
  * If a block the call must write is not determined by the given parts (lzgpu_plan_recover_slices; a wanted parity part needs every data
  * block of its stripes), the call returns LZGPU_ERR_TOO_FEW_PARTS before anything is enqueued.  When one slice alone has k given parts
- * the bytes equal what lzgpu_convert_chunks writes from that slice.  Stale inputs (valid CRC, wrong bytes) are not detected: the stripe
- * calls are the tool for that.  There is one route, recover_slices_kernel (LZGPU_DISABLE_FUSED does not apply; LZGPU_GRID_CAP does),
+ * the bytes equal what lzgpu_convert_chunks writes from that slice.  Stale inputs (valid CRC, wrong bytes) are not detected: run
+ * lzgpu_check_slices on the same given parts first.  There is one route, recover_slices_kernel (LZGPU_DISABLE_FUSED does not apply; LZGPU_GRID_CAP does),
  * reported by lzgpu_debug_last_geometry as LZGPU_KERNEL_RECOVER_SLICES; a goal set whose largest request does not fit the kernel's
  * shared memory (more than 192 blocks or 64 parity blocks per combined stripe) returns LZGPU_ERR_ARG, as the plan says (ok = 0). */
 typedef struct lzgpu_slices_recover_plan {
@@ -504,6 +505,72 @@ int lzgpu_salvage_slices(lzgpu_ctx *ctx, const lzgpu_goal *goals, uint32_t n_sli
 int lzgpu_salvage_slices_dev(lzgpu_ctx *ctx, const lzgpu_goal *goals, uint32_t n_slices, uint32_t n_chunks, uint32_t nb,
                              const void *const *d_parts, const size_t *part_stride, const void *const *d_part_crc,
                              void *d_image, size_t image_stride, void *d_image_crc, void *d_map, int64_t *bad /* host, [4] */, void *stream);
+
+/* Consistency map of the slices of a multi-slice goal: for every combined stripe, do the given parts of all slices describe one chunk,
+ * and which part is stale?  Each slice can be self-consistent and pass its CRCs while the slices disagree (the standard copy and an
+ * xor2 slice holding different versions of a block: a read returns different bytes depending on the slice that serves it), and
+ * lzgpu_recover_slices solves lost blocks from the parts of several slices at once, so one stale given block makes every block solved
+ * from it wrong, with fresh CRCs.  Run this first: it uses the redundancy the given parts still carry.
+ *   goals, n_slices, nb, parts, part_stride, part_crc, bad   as in lzgpu_recover_slices, with nothing wanted: flat part numbering,
+ *                     layout and zero padding, alignment, every given block verified against its stored CRCs in the same pass,
+ *                     bad[0..3] the smallest (chunk, slice, part in the slice, block), deferred mode (lzgpu_last_bad: chunk, flat part,
+ *                     block), the CRC-disabled mode.  Every chunk of a call has the same given parts.
+ *   map[c * n_cs + cs]  (n_cs = ceil(nb / L); every entry written, also when a stored CRC failed; _dev: 8-byte aligned): combined
+ *                     stripe cs of chunk c, that is part blocks cs * L / k_i .. (cs + 1) * L / k_i - 1 of slice i.
+ * Checks (csrc/slices_check.h).  A shape (a full combined stripe, or the chunk's last, with positions at or past nb known zeros) has as
+ * given blocks every block of a given parity part in a slice stripe that exists and every block of a given data part at a position
+ * < nb (a data block past the chunk's end is padding: verified, never a check).  The basis is what lzgpu_recover_slices solves from:
+ * the first given copy, in flat order, of each known position and the independent parity equations it chooses.  Every other given
+ * block defines one check, that block XOR what the basis predicts for it: the first copy for another copy of a known position, the
+ * re-encoding of its slice stripe for a parity block (the unknowns from a particular solution, free unknowns 0).  Checks are numbered
+ * in flat order of their defining block (part, then stripe); there are given blocks - rank of them (lzgpu_debug_check_slices_rows).
+ *   bad_checks        bit h: check h has a non-zero syndrome somewhere in the combined stripe; 0: consistent
+ *   suspect_part      the one given part g such that at every byte where the syndrome vector S is not zero, S lies in the span of the
+ *                     columns of g's blocks (the given parts other than g satisfy every check of the code punctured at g); -1 when no
+ *                     part or more than one does, and when consistent.  A stale part with several blocks in the stripe is one suspect.
+ *                     With one goal (n_slices = 1) and at least k + 1 given parts, bad_checks != 0 exactly when
+ *                     lzgpu_check_stripe_map_degraded reports bad_rows != 0 for that stripe, with the same suspect_part, except
+ *                     in the chunk's last stripe when a lost data part's block there lies past the chunk's end: this call knows that
+ *                     block is zero, which the degraded map solves for, so it has one more check and may name a part there that the
+ *                     degraded map leaves at -1.
+ * The plan (lzgpu_plan_check_slices) says what a clean map means: a part outside `checked` can change a block undetected, and only a
+ * part in `locatable` is always named when it alone is stale.
+ * Refused before anything is enqueued: no part given, or no shape of the batch has a check (LZGPU_ERR_TOO_FEW_PARTS); what
+ * lzgpu_recover_slices refuses, no map, more than 64 checks in a shape, or tables that do not fit the kernel (plan ok = 0)
+ * (LZGPU_ERR_ARG).  lzgpu_check_slices returns LZGPU_ERR_CRC when a stored CRC failed, else LZGPU_ERR_INCONSISTENT when any entry is
+ * bad, else LZGPU_OK.  lzgpu_check_slices_dev writes the map to d_map on `stream` and returns LZGPU_OK or LZGPU_ERR_CRC; it waits for
+ * the stream only when stored CRCs are given, as lzgpu_recover_slices_dev.  The route: the CHECK instantiation of
+ * recover_slices_kernel (lzgpu_debug_last_geometry: LZGPU_KERNEL_CHECK_SLICES; LZGPU_GRID_CAP applies), then a locate pass over the
+ * bad entries.  lzgpu_pool_check_slices cuts the batch as lzgpu_pool_salvage_slices: parts and part_crc move by slice, the map by
+ * first * n_cs. */
+typedef struct lzgpu_slices_check {
+	uint64_t bad_checks;    /* bit h: check h of this stripe's shape has a non-zero syndrome somewhere in the combined stripe; 0 = consistent */
+	int32_t suspect_part;   /* flat part whose corruption alone explains every syndrome byte of the combined stripe, else -1 (also when consistent) */
+	uint32_t zero;          /* written 0 */
+} lzgpu_slices_check;       /* 16 bytes, 8-byte aligned */
+typedef struct lzgpu_slices_check_plan {
+	uint32_t L, tail_blocks;            /* as lzgpu_slices_recover_plan */
+	uint32_t n_checks, tail_n_checks;   /* checks of a full combined stripe and of the chunk's last one (equal when L divides nb) */
+	uint64_t checked, tail_checked;     /* bit g: part g is given, and each of its blocks in the shape has a non-zero coefficient in some
+	                                       check, so a change confined to any one of its blocks is detected */
+	uint64_t locatable, tail_locatable; /* bit g: part g is given, its columns have full rank and their span meets the span of every other
+	                                       given part's columns only in 0: every change confined to g's blocks is detected and named g */
+	int ok;                             /* 1: at most 64 checks per shape and the kernel takes the tables */
+	uint32_t G, threads, stages, smem_bytes; /* launch geometry, as lzgpu_debug_last_geometry reports it */
+} lzgpu_slices_check_plan;
+int lzgpu_plan_check_slices(const lzgpu_goal *goals, uint32_t n_slices, uint32_t nb, const uint8_t *given, lzgpu_slices_check_plan *out);
+/* The checks of one shape (positions < valid are chunk blocks, valid = L: a full combined stripe): *n_checks, and for check h < 64 its
+ * defining block (check_part[h], check_stripe[h]) and its coefficients coef[(h * 64 + g) * 64 + s] over given block s of flat part g
+ * (s: the stripe of g's slice within the combined stripe; a standard part has one per position), zero elsewhere.  LZGPU_ERR_ARG for bad
+ * arguments or more than 64 checks (*n_checks is still set). */
+int lzgpu_debug_check_slices_rows(const lzgpu_goal *goals, uint32_t n_slices, const uint8_t *given, uint32_t valid, uint32_t *n_checks,
+                                  uint8_t *check_part, uint8_t *check_stripe, uint8_t *coef /* [64][64][64] */);
+int lzgpu_check_slices(lzgpu_ctx *ctx, const lzgpu_goal *goals, uint32_t n_slices, uint32_t n_chunks, uint32_t nb,
+                       const uint8_t *const *parts, const size_t *part_stride, const uint32_t *const *part_crc,
+                       lzgpu_slices_check *map, int64_t *bad /* [4] */);
+int lzgpu_check_slices_dev(lzgpu_ctx *ctx, const lzgpu_goal *goals, uint32_t n_slices, uint32_t n_chunks, uint32_t nb,
+                           const void *const *d_parts, const size_t *part_stride, const void *const *d_part_crc,
+                           void *d_map, int64_t *bad /* host, [4] */, void *stream);
 
 /* Degraded read / rebuild of n_chunks chunks.
  *   parts[i]    (i < k+m) part-major buffer of part i for all chunks: chunk c at + c*part_stride,
@@ -823,6 +890,11 @@ int lzgpu_pool_salvage_slices(lzgpu_pool *pool, const lzgpu_goal *goals, uint32_
                               uint8_t *image, size_t image_stride, uint32_t *image_crc, uint8_t *map, int64_t *bad);
                              /* lzgpu_salvage_slices over every device of a pool, host memory only: for any input the code, image,
                               * image CRCs, map and bad[0..3] lzgpu_salvage_slices returns on one context for the whole batch */
+int lzgpu_pool_check_slices(lzgpu_pool *pool, const lzgpu_goal *goals, uint32_t n_slices, uint32_t n_chunks, uint32_t nb,
+                            const uint8_t *const *parts, const size_t *part_stride, const uint32_t *const *part_crc,
+                            lzgpu_slices_check *map, int64_t *bad);
+                             /* lzgpu_check_slices over every device of a pool, host memory only: for any input the code, map and
+                              * bad[0..3] lzgpu_check_slices returns on one context for the whole batch (an empty batch runs on slot 0) */
 int lzgpu_convert_chunks_dev(lzgpu_ctx *ctx, const lzgpu_goal *src, const lzgpu_goal *dst, uint32_t n_chunks, uint32_t nb,
                              const void *const *d_parts, size_t part_stride, const void *const *d_part_crc,
                              const uint8_t *want, void *const *d_out, size_t out_stride, void *const *d_out_crc,

@@ -87,7 +87,7 @@ class LzEncoderKernel(C.Structure):
 # lzgpu_launch_geometry.kernel
 KERNEL_NONE, KERNEL_ENCODE, KERNEL_ENCODE_BITSLICE, KERNEL_RECOVER_GEO0, KERNEL_RECOVER_GEO1, KERNEL_RECOVER_GEO2, \
     KERNEL_RECOVER_DIRECT, KERNEL_RECOVER_BS3, KERNEL_CONVERT, KERNEL_CHECK, KERNEL_CHECK_DEGRADED, KERNEL_ENCODE_SLICES, \
-    KERNEL_RECOVER_SLICES, KERNEL_SALVAGE_SLICES = range(14)
+    KERNEL_RECOVER_SLICES, KERNEL_SALVAGE_SLICES, KERNEL_CHECK_SLICES = range(15)
 
 
 class LzSlicesRecoverPlan(C.Structure):
@@ -101,6 +101,12 @@ class LzSlicesSalvagePlan(C.Structure):
     _fields_ = [("known", C.c_uint64), ("determined", C.c_uint64), ("tail_known", C.c_uint64), ("tail_determined", C.c_uint64),
                 ("L", C.c_uint32), ("tail_blocks", C.c_uint32), ("ok", C.c_int), ("G", C.c_uint32), ("threads", C.c_uint32),
                 ("stages", C.c_uint32), ("smem_bytes", C.c_uint32)]
+
+
+class LzSlicesCheckPlan(C.Structure):
+    _fields_ = [("L", C.c_uint32), ("tail_blocks", C.c_uint32), ("n_checks", C.c_uint32), ("tail_n_checks", C.c_uint32),
+                ("checked", C.c_uint64), ("tail_checked", C.c_uint64), ("locatable", C.c_uint64), ("tail_locatable", C.c_uint64),
+                ("ok", C.c_int), ("G", C.c_uint32), ("threads", C.c_uint32), ("stages", C.c_uint32), ("smem_bytes", C.c_uint32)]
 
 
 # lzgpu_salvage_slices' map bytes
@@ -158,6 +164,8 @@ SIGNATURES = {
     "lzgpu_plan_recover_slices": (_int, [_goalp, _u32, _u32, _vp, C.POINTER(LzSlicesRecoverPlan)]),
     "lzgpu_debug_recover_slices_rows": (_int, [_goalp, _u32, _vp, _u32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "lzgpu_plan_salvage_slices": (_int, [_goalp, _u32, _u32, _vp, C.POINTER(LzSlicesSalvagePlan)]),
+    "lzgpu_plan_check_slices": (_int, [_goalp, _u32, _u32, _vp, C.POINTER(LzSlicesCheckPlan)]),
+    "lzgpu_debug_check_slices_rows": (_int, [_goalp, _u32, _vp, _u32, _vp, _vp, _vp, _vp]),
     "lzgpu_debug_locate_errors": (_int, [_int, _int, _vp, _vp, _vp, _u32, _vp]),
     "lzgpu_goal_slice_type": (_int, [_goalp]),
     "lzgpu_goal_from_slice_type": (_int, [_int, _goalp]),
@@ -186,6 +194,8 @@ SIGNATURES = {
     "lzgpu_recover_slices_dev": (_int, [_vp, _goalp, _u32, _u32, _u32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _sz, _vp, _vp]),
     "lzgpu_salvage_slices": (_int, [_vp, _goalp, _u32, _u32, _u32, _vp, _vp, _vp, _vp, _sz, _vp, _vp, _vp]),
     "lzgpu_salvage_slices_dev": (_int, [_vp, _goalp, _u32, _u32, _u32, _vp, _vp, _vp, _vp, _sz, _vp, _vp, _vp, _vp]),
+    "lzgpu_check_slices": (_int, [_vp, _goalp, _u32, _u32, _u32, _vp, _vp, _vp, _vp, _vp]),
+    "lzgpu_check_slices_dev": (_int, [_vp, _goalp, _u32, _u32, _u32, _vp, _vp, _vp, _vp, _vp, _vp]),
     "lzgpu_recover_chunks": (_int, [_vp, _goalp, _u32, _u32, _vp, _sz, _vp, _vp, _vp, _vp, _sz, _vp]),
     "lzgpu_recover_chunks_dev": (_int, [_vp, _goalp, _u32, _u32, _vp, _sz, _vp, _vp, _vp, _vp, _sz, _vp, _vp]),
     "lzgpu_check_stripes": (_int, [_vp, _goalp, _u32, _u32, _vp, _sz, _vp, _vp, _vp]),
@@ -269,6 +279,7 @@ SIGNATURES = {
     "lzgpu_pool_convert_chunks": (_int, [_vp, _goalp, _goalp, _u32, _u32, _vp, _sz, _vp, _vp, _vp, _sz, _vp, _vp]),
     "lzgpu_pool_recover_slices": (_int, [_vp, _goalp, _u32, _u32, _u32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
     "lzgpu_pool_salvage_slices": (_int, [_vp, _goalp, _u32, _u32, _u32, _vp, _vp, _vp, _vp, _sz, _vp, _vp, _vp]),
+    "lzgpu_pool_check_slices": (_int, [_vp, _goalp, _u32, _u32, _u32, _vp, _vp, _vp, _vp, _vp]),
     "lzgpu_pool_crc_blocks": (_int, [_vp, _vp, _sz, _u32, _sz, _vp]),
     "lzgpu_pool_check_stripes": (_int, [_vp, _goalp, _u32, _u32, _vp, _sz, _vp, _vp, _vp]),
     "lzgpu_pool_check_stripe_map": (_int, [_vp, _goalp, _u32, _u32, _vp, _sz, _vp, _vp, _vp]),

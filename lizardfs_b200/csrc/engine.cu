@@ -19,7 +19,7 @@
 #include "host_math.h"
 #include "correct_kernel.cuh"
 #include "fused_plan.h"
-#include "slices_solve.h"
+#include "slices_check.h"
 #include "kernels_generic.cuh"
 #include "lzgpu.h"
 
@@ -2162,28 +2162,34 @@ extern "C" int lzgpu_convert_chunks(lzgpu_ctx *ctx, const lzgpu_goal *src, const
 // recovery from the parts of every slice of a goal together (lzgpu_recover_slices*)
 // ------------------------------------------------------------------------------------------------
 // What the argument check derives for the enqueue: the flat part layout, the solve of both stripe shapes and the launch geometry.
-// salvage: the call is lzgpu_salvage_slices* (set by the caller before the check)
+// salvage: the call is lzgpu_salvage_slices*; check: lzgpu_check_slices*, with the checks of both shapes (set by the caller before
+// the check)
 struct RecoverSlicesCall {
 	lzd::SliceLayout lay;
 	lzd::SliceSolve shapes[2];   // a full combined stripe, the chunk's last one when L does not divide nb
+	lzd::SliceChecks checks[2];
 	lzd::RsGeometry geo;
 	uint32_t pb[kSlicesMax] = {0};
-	bool salvage = false;
+	bool salvage = false, check = false;
+	lzd::RsMode mode() const { return check ? lzd::RsMode::CHECK : salvage ? lzd::RsMode::SALVAGE : lzd::RsMode::RECOVER; }
 };
 
-// lzgpu_salvage_slices* want no part
+// lzgpu_salvage_slices* and lzgpu_check_slices* want no part
 static const uint8_t kWantNone[LZGPU_MAX_PARTS] = {0};
 
 // The arguments of both forms, checked before anything is enqueued and whatever n_chunks is.  dev: the device form's alignment rules
 // (16-byte buffers and strides, 4-byte CRC arrays).  LZGPU_ERR_TOO_FEW_PARTS when a block the call must write is not determined; in the
-// salvage form (c.salvage; want = kWantNone, chunk_out the image) when no part is given, and the image and the map are required.
+// salvage form (c.salvage; want = kWantNone, chunk_out the image) when no part is given, and the image and the map are required.  In
+// the check form (c.check; want = kWantNone, no image, map required) when no part is given or no shape of the batch has a check; more
+// than 64 checks in a shape is LZGPU_ERR_ARG.
 static int recover_slices_args(const lzgpu_ctx *ctx, const lzgpu_goal *goals, uint32_t n_slices, uint32_t nb, const void *const *parts,
                                const size_t *part_stride, const void *const *part_crc, const uint8_t *want, const void *const *out,
                                const size_t *out_stride, const void *const *out_crc, const void *chunk_out, size_t chunk_out_stride, bool dev,
                                RecoverSlicesCall &c, const void *image_crc = nullptr, const void *map = nullptr) {
 	if (!ctx || !parts || !part_stride || !want) return LZGPU_ERR_ARG;
-	const char *fn = c.salvage ? "salvage_slices" : "recover_slices";
+	const char *fn = c.check ? "check_slices" : c.salvage ? "salvage_slices" : "recover_slices";
 	if (c.salvage && (!chunk_out || !map)) { lz_set_error("salvage_slices: the image and the map are required"); return LZGPU_ERR_ARG; }
+	if (c.check && !map) { lz_set_error("check_slices: the map is required"); return LZGPU_ERR_ARG; }
 	const char *why = nullptr;
 	if (lzd::slice_layout(goals, n_slices, c.lay, &why)) { lz_set_error("%s: %s", fn, why); return LZGPU_ERR_ARG; }
 	if (nb == 0 || nb > LZGPU_BLOCKS_IN_CHUNK) { lz_set_error("nb out of range"); return LZGPU_ERR_ARG; }
@@ -2222,15 +2228,27 @@ static int recover_slices_args(const lzgpu_ctx *ctx, const lzgpu_goal *goals, ui
 		if (reinterpret_cast<uintptr_t>(chunk_out) & 15) { lz_set_error("%s: %s is not 16-byte aligned", fn, c.salvage ? "image" : "chunk_out"); return LZGPU_ERR_ARG; }
 		if (reinterpret_cast<uintptr_t>(image_crc) & 3) { lz_set_error("salvage_slices: image_crc is not 4-byte aligned"); return LZGPU_ERR_ARG; }
 	}
-	if (c.salvage) {
+	if (c.salvage || c.check) {
 		bool any = false;
 		for (uint32_t g = 0; g < lay.n_parts; ++g) any |= parts[g] != nullptr;
-		if (!any) { lz_set_error("salvage_slices: no part is given"); return LZGPU_ERR_TOO_FEW_PARTS; }
+		if (!any) { lz_set_error("%s: no part is given", fn); return LZGPU_ERR_TOO_FEW_PARTS; }
 	}
 	const uint32_t tail = nb % lay.L;
 	lzd::slice_solve(lay, given, lay.L, c.shapes[0]);
 	if (tail) lzd::slice_solve(lay, given, tail, c.shapes[1]);
-	for (int t = 0; t < 2 && !c.salvage; ++t) {   // salvage writes what is determined, holes are not refused
+	for (int t = 0; t < 2 && c.check; ++t) {
+		if (t == 0 ? nb < lay.L : tail == 0) continue;
+		lzd::slice_checks(lay, given, c.shapes[t], c.checks[t]);
+		if (c.checks[t].n_checks > lzd::kScMaxChecks) {
+			lz_set_error("check_slices: the %s combined stripe has %u checks, more than 64", t ? "last" : "full", c.checks[t].n_checks);
+			return LZGPU_ERR_ARG;
+		}
+	}
+	if (c.check && (nb < lay.L || !c.checks[0].n_checks) && (!tail || !c.checks[1].n_checks)) {
+		lz_set_error("check_slices: no combined stripe of the batch has a check");
+		return LZGPU_ERR_TOO_FEW_PARTS;
+	}
+	for (int t = 0; t < 2 && !c.salvage && !c.check; ++t) {   // salvage writes what is determined, holes are not refused
 		if (t == 0 ? nb < lay.L : tail == 0) continue;   // a shape no chunk of the call has
 		const lzd::SliceSolve &sv = c.shapes[t];
 		const uint64_t lost = lzd::slice_needed(lay, want, chunk_out != nullptr, sv.valid) & ~sv.determined;
@@ -2241,7 +2259,7 @@ static int recover_slices_args(const lzgpu_ctx *ctx, const lzgpu_goal *goals, ui
 		}
 	}
 	const lzd::SliceSolve used[2] = {nb >= lay.L ? c.shapes[0] : c.shapes[1], tail ? c.shapes[1] : c.shapes[0]};
-	c.geo = lzd::rs_geometry(lay, given, used, 2, c.salvage);
+	c.geo = lzd::rs_geometry(lay, given, used, 2, c.mode());
 	if (!c.geo.ok) {
 		lz_set_error("%s: a combined stripe has more blocks than the kernel stages (%u slots, %u CRC streams)", fn, c.geo.slots, c.geo.states);
 		return LZGPU_ERR_ARG;
@@ -2256,6 +2274,7 @@ static uint64_t recover_slices_alg_bytes(const RecoverSlicesCall &c, uint32_t n_
 	const uint64_t B = LZGPU_BLOCK_SIZE;
 	uint64_t per_chunk = image ? static_cast<uint64_t>(nb) * B : 0;
 	if (c.salvage) per_chunk += static_cast<uint64_t>(nb) * (image_crcs ? 5 : 1);
+	if (c.check) per_chunk += (nb + c.lay.L - 1) / c.lay.L * sizeof(lzgpu_slices_check);
 	for (uint32_t i = 0; i < c.lay.n_slices; ++i)
 		for (uint32_t g = c.lay.base[i]; g < c.lay.base[i] + c.lay.k[i] + c.lay.m[i]; ++g) {
 			if (parts[g]) per_chunk += c.pb[i] * (B + (crcs ? 4 : 0));
@@ -2284,9 +2303,10 @@ static int recover_slices_enqueue(lzgpu_ctx *ctx, const RecoverSlicesCall &c, ui
 	int rc;
 	if (verifying && (rc = tk->arm(ctx, st))) return rc;
 	if ((rc = lz_recover_slices(ctx, c.lay, c.shapes, c.geo, n_chunks, nb, d_parts, part_stride, verifying ? d_part_crc : nullptr, want, d_out,
-	                            out_stride, d_out_crc, d_chunk_out, chunk_out_stride, d_image_crc, d_map, st, verifying ? tk->word(0) : nullptr)))
+	                            out_stride, d_out_crc, d_chunk_out, chunk_out_stride, d_image_crc, d_map, c.check ? c.checks : nullptr, st,
+	                            verifying ? tk->word(0) : nullptr)))
 		return rc;
-	ctx->stats.chunks_recovered += n_chunks;
+	if (!c.check) ctx->stats.chunks_recovered += n_chunks;
 	return verifying ? tk->publish_fused() : LZGPU_OK;
 }
 
@@ -2333,9 +2353,24 @@ extern "C" int lzgpu_salvage_slices_dev(lzgpu_ctx *ctx, const lzgpu_goal *goals,
 	                               image_stride, d_image_crc, d_map, bad, stream);
 }
 
-// The host form of both calls, after their argument check: the given parts (+ stored CRCs) staged tile by tile, the wanted parts
-// (+ CRCs), the image and the salvage form's image CRCs and map copied back.  The salvage form runs every tile past a CRC mismatch, so
-// that its outputs are complete.
+extern "C" int lzgpu_check_slices_dev(lzgpu_ctx *ctx, const lzgpu_goal *goals, uint32_t n_slices, uint32_t n_chunks, uint32_t nb,
+                                       const void *const *d_parts, const size_t *part_stride, const void *const *d_part_crc, void *d_map,
+                                       int64_t *bad, void *stream) {
+	NvtxScope nvtx_scope("lzgpu::check_slices_dev");
+	auto c = std::make_unique<RecoverSlicesCall>();
+	c->check = true;
+	int rc = recover_slices_args(ctx, goals, n_slices, nb, d_parts, part_stride, d_part_crc, kWantNone, nullptr, nullptr, nullptr, nullptr, 0,
+	                             true, *c, nullptr, d_map);
+	if (rc) return rc;
+	if (reinterpret_cast<uintptr_t>(d_map) & 7) { lz_set_error("check_slices: map is not 8-byte aligned"); return LZGPU_ERR_ARG; }
+	if (n_chunks == 0) return LZGPU_OK;
+	return recover_slices_dev_call(ctx, *c, n_chunks, nb, d_parts, part_stride, d_part_crc, kWantNone, nullptr, nullptr, nullptr, nullptr, 0,
+	                               nullptr, d_map, bad, stream);
+}
+
+// The host form of the three calls, after their argument check: the given parts (+ stored CRCs) staged tile by tile, the wanted
+// parts (+ CRCs), the image and the salvage form's image CRCs and map (or the check form's map) copied back.  The salvage and check
+// forms run every tile past a CRC mismatch, so that their outputs are complete.
 static int recover_slices_host(lzgpu_ctx *ctx, const RecoverSlicesCall &c, uint32_t n_chunks, uint32_t nb, const uint8_t *const *parts,
                                const size_t *part_stride, const uint32_t *const *part_crc, const uint8_t *want, uint8_t *const *out,
                                const size_t *out_stride, uint32_t *const *out_crc, uint8_t *chunk_out, size_t chunk_out_stride,
@@ -2363,7 +2398,8 @@ static int recover_slices_host(lzgpu_ctx *ctx, const RecoverSlicesCall &c, uint3
 	}
 	const size_t img_off = per_chunk, img_bytes = chunk_out ? static_cast<size_t>(nb) * B : 0;
 	per_chunk += img_bytes;
-	const size_t map_off = per_chunk, map_bytes = map ? nb : 0, img_crc_off = crc_words;
+	const size_t map_off = per_chunk, img_crc_off = crc_words;
+	const size_t map_bytes = !map ? 0 : c.check ? (nb + lay.L - 1) / lay.L * sizeof(lzgpu_slices_check) : nb;
 	per_chunk += map_bytes;
 	if (image_crc) crc_words += nb;
 	std::lock_guard<std::mutex> lk(ctx->mu);
@@ -2376,7 +2412,7 @@ static int recover_slices_host(lzgpu_ctx *ctx, const RecoverSlicesCall &c, uint3
 	}
 	if (chunk_out) pin.add(chunk_out, static_cast<size_t>(n_chunks - 1) * chunk_out_stride + img_bytes);
 	if (image_crc) pin.add(image_crc, static_cast<size_t>(n_chunks) * nb * 4);
-	if (map) pin.add(map, static_cast<size_t>(n_chunks) * nb);
+	if (map) pin.add(map, static_cast<size_t>(n_chunks) * map_bytes);
 	const uint32_t tile = static_cast<uint32_t>(std::max<size_t>(1, std::min<size_t>(n_chunks, (2 * kHostTileBytes) / std::max<size_t>(per_chunk, 1))));
 	const int n_slots = n_chunks > tile ? kHostSlots : 1;
 	void *d_in[kHostSlots], *d_crc[kHostSlots];
@@ -2429,12 +2465,12 @@ static int recover_slices_host(lzgpu_ctx *ctx, const RecoverSlicesCall &c, uint3
 			ctx->stats.bytes_d2h += nc * img_bytes;
 		}
 		if (map) {
-			CUDA_TRY(cudaMemcpyAsync(map + c0 * nb, dmap, nc * nb, cudaMemcpyDeviceToHost, st));
-			ctx->stats.bytes_d2h += nc * nb;
+			CUDA_TRY(cudaMemcpyAsync(map + c0 * map_bytes, dmap, nc * map_bytes, cudaMemcpyDeviceToHost, st));
+			ctx->stats.bytes_d2h += nc * map_bytes;
 		}
 		if (image_crc) CUDA_TRY(cudaMemcpyAsync(image_crc + c0 * nb, dimg_crc, nc * nb * 4, cudaMemcpyDeviceToHost, st));
 		return LZGPU_OK;
-	}, c.salvage);
+	}, c.salvage || c.check);
 	if (rc == LZGPU_ERR_CRC) recover_slices_bad(lay, b3, bad);
 	return rc;
 }
@@ -2465,6 +2501,25 @@ extern "C" int lzgpu_salvage_slices(lzgpu_ctx *ctx, const lzgpu_goal *goals, uin
 	if (rc || n_chunks == 0) return rc;
 	return recover_slices_host(ctx, *c, n_chunks, nb, parts, part_stride, part_crc, kWantNone, nullptr, nullptr, nullptr, image, image_stride,
 	                           image_crc, map, bad);
+}
+
+extern "C" int lzgpu_check_slices(lzgpu_ctx *ctx, const lzgpu_goal *goals, uint32_t n_slices, uint32_t n_chunks, uint32_t nb,
+                                   const uint8_t *const *parts, const size_t *part_stride, const uint32_t *const *part_crc,
+                                   lzgpu_slices_check *map, int64_t *bad) {
+	NvtxScope nvtx_scope("lzgpu::check_slices");
+	auto c = std::make_unique<RecoverSlicesCall>();
+	c->check = true;
+	int rc = recover_slices_args(ctx, goals, n_slices, nb, reinterpret_cast<const void *const *>(parts), part_stride,
+	                             reinterpret_cast<const void *const *>(part_crc), kWantNone, nullptr, nullptr, nullptr, nullptr, 0, false, *c,
+	                             nullptr, map);
+	if (rc || n_chunks == 0) return rc;
+	rc = recover_slices_host(ctx, *c, n_chunks, nb, parts, part_stride, part_crc, kWantNone, nullptr, nullptr, nullptr, nullptr, 0, nullptr,
+	                         reinterpret_cast<uint8_t *>(map), bad);
+	if (rc) return rc;
+	const size_t n = static_cast<size_t>(n_chunks) * ((nb + c->lay.L - 1) / c->lay.L);
+	for (size_t e = 0; e < n; ++e)
+		if (map[e].bad_checks) return LZGPU_ERR_INCONSISTENT;
+	return LZGPU_OK;
 }
 
 // ------------------------------------------------------------------------------------------------

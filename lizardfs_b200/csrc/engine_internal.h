@@ -213,16 +213,19 @@ int lz_fused_encode_slices(lzgpu_ctx *ctx, const lzgpu_goal *goals, uint32_t n_s
 // Recovery from the parts of every slice together (recover_slices_kernel.cuh): the one launch of lzgpu_recover_slices*, whose arguments,
 // solve (shapes[0] a full combined stripe, shapes[1] the tail) and geometry the caller has checked.  d_first_bad: the armed result word
 // whenever d_part_crc is given.  d_map != nullptr: the salvage form (lzgpu_salvage_slices*: nothing wanted, the image, its optional
-// block CRCs d_image_crc and the status bytes d_map), on the SALVAGE instantiation.
+// block CRCs d_image_crc and the status bytes d_map), on the SALVAGE instantiation.  checks != nullptr: the check form
+// (lzgpu_check_slices*: nothing wanted, no image, checks[0..1] of both shapes, the entries d_map), on the CHECK instantiation and then
+// the locate pass.
 namespace lzd {
 struct SliceLayout;
 struct SliceSolve;
+struct SliceChecks;
 struct RsGeometry;
 }  // namespace lzd
 int lz_recover_slices(lzgpu_ctx *ctx, const lzd::SliceLayout &lay, const lzd::SliceSolve *shapes, const lzd::RsGeometry &geo, uint32_t n_chunks,
                       uint32_t nb, const void *const *d_parts, const size_t *part_stride, const void *const *d_part_crc, const uint8_t *want,
                       void *const *d_out, const size_t *out_stride, void *const *d_out_crc, void *d_image, size_t image_stride, void *d_image_crc,
-                      void *d_map, cudaStream_t st, unsigned long long *d_first_bad);
+                      void *d_map, const lzd::SliceChecks *checks, cudaStream_t st, unsigned long long *d_first_bad);
 // CRC of 64 KiB blocks: block (c, b) at base + c*chunk_stride + b*65536, out[c*out_chunk_stride + b]
 int lz_fused_crc(lzgpu_ctx *ctx, const void *base, unsigned long long n_blocks, unsigned long long blocks_per_chunk,
                  unsigned long long chunk_stride, void *out, unsigned long long out_chunk_stride, cudaStream_t st);

@@ -19,6 +19,7 @@
 #include "check_kernel.cuh"
 #include "slices_kernel.cuh"
 #include "recover_slices_kernel.cuh"
+#include "slices_check.h"
 #include "host_math.h"
 
 using namespace lzd;
@@ -329,9 +330,11 @@ static const struct {
 	SlicesKernel fn;
 } kSlicers[] = {{1, fused_slices_kernel<1>}, {2, fused_slices_kernel<2>}, {3, fused_slices_kernel<3>}, {4, fused_slices_kernel<4>}};
 
-// Recovery from the parts of every slice together (recover_slices_kernel): one instantiation for any goal set, and its SALVAGE twin
+// Recovery from the parts of every slice together (recover_slices_kernel): one instantiation for any goal set, and its SALVAGE and
+// CHECK twins, indexed by RsMode
 using RecoverSlicesKernel = void (*)(RecoverSlicesParams);
-static const RecoverSlicesKernel kRecoverSlicers[] = {recover_slices_kernel<false>, recover_slices_kernel<true>};
+static const RecoverSlicesKernel kRecoverSlicers[] = {recover_slices_kernel<RsMode::RECOVER>, recover_slices_kernel<RsMode::SALVAGE>,
+                                                      recover_slices_kernel<RsMode::CHECK>};
 
 // function attributes are per device: set once per context
 static int set_all_smem_attrs(const FusedState *fs) {
@@ -959,9 +962,11 @@ int lz_fused_encode_slices(lzgpu_ctx *ctx, const lzgpu_goal *goals, uint32_t n_s
 // ---------------------------------------------------------------------------------------------------
 
 // The kernel's tables for one stripe shape: what is read and staged, what is written, the CRC streams, the solve.  image_crc: the
-// image blocks get CRC streams (the salvage form)
+// image blocks get CRC streams (the salvage form).  chk: the check form's checks of this shape (slices_check.h): each defining block
+// staged at L + E + h, its prediction as the wanted-parity entry h (a further copy of position q: row kRsNone, stripe q), and the
+// particular-solution rows instead of the solve's
 static void rs_fill_shape(RsShape &o, const SliceLayout &lay, const SliceSolve &sv, const void *const *d_parts, const void *const *d_stored,
-                          const uint8_t *want, void *const *d_out_crc, bool image, bool image_crc) {
+                          const uint8_t *want, void *const *d_out_crc, bool image, bool image_crc, const SliceChecks *chk = nullptr) {
 	const uint32_t L = lay.L, E = sv.n_eq;
 	std::memset(&o, 0, sizeof(o));
 	uint64_t staged = 0;
@@ -983,6 +988,13 @@ static void rs_fill_shape(RsShape &o, const SliceLayout &lay, const SliceSolve &
 					for (uint32_t e = 0; e < E; ++e)
 						if (sv.eq_slice[e] == i && sv.eq_row[e] == p - lay.k[i] && sv.eq_stripe[e] == s) slot = static_cast<uint8_t>(L + e);
 				}
+				if (chk && chk->check_of[g][s] >= 0) {
+					const uint32_t h = static_cast<uint32_t>(chk->check_of[g][s]);
+					slot = static_cast<uint8_t>(L + E + h);
+					o.out_slice[h] = static_cast<uint8_t>(i);
+					o.out_row[h] = p < lay.k[i] ? kRsNone : static_cast<uint8_t>(p - lay.k[i]);
+					o.out_stripe[h] = static_cast<uint8_t>(p < lay.k[i] ? s * lay.k[i] + p : s);
+				}
 				const bool verify = d_stored && d_stored[g];
 				if (slot == kRsNone && !verify) continue;   // neither used nor verified: not read
 				const uint8_t st = verify ? add_state(static_cast<uint8_t>(g), static_cast<uint8_t>(s), 0) : kRsNone;   // names read entry n_read
@@ -997,7 +1009,8 @@ static void rs_fill_shape(RsShape &o, const SliceLayout &lay, const SliceSolve &
 	std::memcpy(o.eq_slice, sv.eq_slice, sizeof(o.eq_slice));
 	std::memcpy(o.eq_row, sv.eq_row, sizeof(o.eq_row));
 	std::memcpy(o.eq_stripe, sv.eq_stripe, sizeof(o.eq_stripe));
-	std::memcpy(o.rows, sv.rows, sizeof(o.rows));
+	std::memcpy(o.rows, chk ? chk->prow : sv.rows, sizeof(o.rows));
+	if (chk) o.n_out = static_cast<uint16_t>(chk->n_checks);
 	for (uint32_t i = 0; i < lay.n_slices; ++i)
 		for (uint32_t p = 0; p < lay.k[i] + lay.m[i]; ++p) {
 			const uint32_t g = lay.base[i] + p;
@@ -1056,10 +1069,68 @@ static void rs_fill_salvage(RsSalvage &o, const RsShape &sh, const SliceLayout &
 	}
 }
 
+// lzgpu_check_slices' locate pass, after the CHECK launch has written every entry: the tables of both shapes in a stream-ordered
+// temporary, and one CTA per bad entry
+static int rs_locate(lzgpu_ctx *ctx, const SliceLayout &lay, const SliceChecks *checks, uint32_t n_chunks, uint32_t nb,
+                     const void *const *d_parts, const size_t *part_stride, RsCheckEntry *d_map, cudaStream_t st) {
+	const uint32_t n_cs = (nb + lay.L - 1) / lay.L, tail = nb % lay.L ? 1u : 0u;
+	const size_t rows = checks[0].ann.size() / kScMaxChecks + (tail ? checks[1].ann.size() / kScMaxChecks : 0);
+	std::vector<uint8_t> host(sizeof(RsLocate) + rows * kRsMaxOut, 0);
+	RsLocate *loc = reinterpret_cast<RsLocate *>(host.data());
+	uint8_t *ann = host.data() + sizeof(RsLocate);
+	uint32_t row0 = 0;
+	for (int t = 0; t < 2; ++t) {
+		if (t == 0 ? nb < lay.L : !tail) continue;
+		const SliceChecks &ck = checks[t];
+		RsLocateShape &o = loc->shape[t];
+		o.n_blocks = ck.n_blocks;
+		o.n_checks = ck.n_checks;
+		o.ann0 = row0;
+		for (uint32_t b = 0; b < ck.n_blocks; ++b) {
+			o.blk_part[b] = ck.blk_part[b];
+			o.blk_s[b] = ck.blk_s[b];
+			for (uint32_t h = 0; h < ck.n_checks; ++h) o.H[h][b] = ck.H[h * ck.n_blocks + b];
+		}
+		for (uint32_t g = 0; g < LZGPU_MAX_PARTS; ++g) {
+			if (!((ck.parts >> g) & 1ull)) continue;
+			o.cand_part[o.n_cand] = static_cast<uint8_t>(g);
+			o.cand_first[o.n_cand] = static_cast<uint16_t>(ck.ann_first[g]);
+			o.cand_first[++o.n_cand] = static_cast<uint16_t>(ck.ann_first[g + 1]);
+		}
+		std::memcpy(ann + static_cast<size_t>(row0) * kRsMaxOut, ck.ann.data(), ck.ann.size());
+		row0 += static_cast<uint32_t>(ck.ann.size() / kScMaxChecks);
+	}
+	TmpBuf d_loc(ctx, st);
+	int rc;
+	if ((rc = d_loc.alloc(host.size()))) return rc;
+	CUDA_TRY(cudaMemcpyAsync(d_loc.p, host.data(), host.size(), cudaMemcpyHostToDevice, st));
+	auto p = std::make_unique<LocateSlicesParams>();
+	std::memset(p.get(), 0, sizeof(LocateSlicesParams));
+	for (uint32_t i = 0; i < lay.n_slices; ++i) {
+		p->part_stride[i] = part_stride[i];
+		p->spc[i] = lay.L / lay.k[i];
+		for (uint32_t g = lay.base[i]; g < lay.base[i] + lay.k[i] + lay.m[i]; ++g) {
+			p->part_slice[g] = static_cast<uint8_t>(i);
+			p->parts[g] = static_cast<const uint8_t *>(d_parts[g]);
+		}
+	}
+	p->map = d_map;
+	p->loc = static_cast<const RsLocate *>(d_loc.p);
+	p->n_entries = static_cast<unsigned long long>(n_chunks) * n_cs;
+	p->n_cs = n_cs;
+	p->tail = tail;
+	uint64_t grid = std::min<uint64_t>(p->n_entries, static_cast<uint64_t>(ctx->sm_count) * 8);
+	if (ctx->fused->grid_cap) grid = std::min<uint64_t>(grid, ctx->fused->grid_cap);
+	locate_slices_kernel<<<static_cast<unsigned>(grid), kRslThreads, 0, st>>>(*p);
+	CUDA_TRY(cudaGetLastError());
+	ctx->stats.kernel_launches++;
+	return LZGPU_OK;
+}
+
 int lz_recover_slices(lzgpu_ctx *ctx, const SliceLayout &lay, const SliceSolve *shapes, const RsGeometry &geo, uint32_t n_chunks, uint32_t nb,
                       const void *const *d_parts, const size_t *part_stride, const void *const *d_part_crc, const uint8_t *want, void *const *d_out,
                       const size_t *out_stride, void *const *d_out_crc, void *d_image, size_t image_stride, void *d_image_crc, void *d_map,
-                      cudaStream_t st, unsigned long long *d_first_bad) {
+                      const SliceChecks *checks, cudaStream_t st, unsigned long long *d_first_bad) {
 	auto p = std::make_unique<RecoverSlicesParams>();
 	std::memset(p.get(), 0, sizeof(RecoverSlicesParams));
 	const bool crc_on = lzgpu_crc_enabled() != 0;
@@ -1096,14 +1167,18 @@ int lz_recover_slices(lzgpu_ctx *ctx, const SliceLayout &lay, const SliceSolve *
 	for (int i = 0; i < 5; ++i) p->tree_mult[i] = lz::crc_xpow_bytes(2048ull << i);
 	const bool verifying = d_part_crc != nullptr;
 	if (verifying && !d_first_bad) return LZGPU_ERR_ARG;  // (cannot happen: the caller arms a ticket whenever it passes stored CRCs)
-	const bool salvage = d_map != nullptr;
+	const RsMode mode = checks ? RsMode::CHECK : d_map ? RsMode::SALVAGE : RsMode::RECOVER;
 	p->image_crc = static_cast<uint32_t *>(d_image_crc);
 	p->map = static_cast<uint8_t *>(d_map);
 	for (int t = 0; t < 2; ++t)
 		if (t == 0 ? nb >= lay.L : p->tail != 0) {
-			rs_fill_shape(p->shape[t], lay, shapes[t], d_parts, d_part_crc, want, d_out_crc, d_image != nullptr, d_image_crc != nullptr);
-			if (salvage) rs_fill_salvage(p->salvage[t], p->shape[t], lay, shapes[t]);
+			rs_fill_shape(p->shape[t], lay, shapes[t], d_parts, d_part_crc, want, d_out_crc, d_image != nullptr, d_image_crc != nullptr,
+			              checks ? &checks[t] : nullptr);
+			if (mode == RsMode::SALVAGE) rs_fill_salvage(p->salvage[t], p->shape[t], lay, shapes[t]);
 		}
-	const lzgpu_launch_geometry g = launch_geo(salvage ? LZGPU_KERNEL_SALVAGE_SLICES : LZGPU_KERNEL_RECOVER_SLICES, geo.threads, geo.G, geo.stages, 0, geo.smem);
-	return launch(ctx, kRecoverSlicers[salvage ? 1 : 0], g, 1, p->total_units, st, *p);
+	static const int kKernelOf[] = {LZGPU_KERNEL_RECOVER_SLICES, LZGPU_KERNEL_SALVAGE_SLICES, LZGPU_KERNEL_CHECK_SLICES};
+	const lzgpu_launch_geometry g = launch_geo(kKernelOf[static_cast<int>(mode)], geo.threads, geo.G, geo.stages, 0, geo.smem);
+	int rc = launch(ctx, kRecoverSlicers[static_cast<int>(mode)], g, 1, p->total_units, st, *p);
+	if (rc || mode != RsMode::CHECK) return rc;
+	return rs_locate(ctx, lay, checks, n_chunks, nb, d_parts, part_stride, static_cast<RsCheckEntry *>(d_map), st);
 }

@@ -9,7 +9,7 @@
 #include "fused_plan.h"
 #include "repair_rows.h"
 #include "decode_locate.h"
-#include "slices_solve.h"
+#include "slices_check.h"
 
 #include <cctype>
 #include <cstdio>
@@ -655,12 +655,69 @@ int lzgpu_plan_salvage_slices(const lzgpu_goal *goals, uint32_t n_slices, uint32
 	out->tail_known = tail ? sv[1].known : sv[0].known;
 	out->tail_determined = tail ? sv[1].determined : sv[0].determined;
 	const lzd::SliceSolve used[2] = {nb >= lay.L ? sv[0] : sv[1], tail ? sv[1] : sv[0]};
-	const lzd::RsGeometry g = lzd::rs_geometry(lay, given, used, 2, true);
+	const lzd::RsGeometry g = lzd::rs_geometry(lay, given, used, 2, lzd::RsMode::SALVAGE);
 	out->ok = g.ok ? 1 : 0;
 	out->G = g.G;
 	out->threads = g.threads;
 	out->stages = g.stages;
 	out->smem_bytes = static_cast<uint32_t>(g.smem);
+	return LZGPU_OK;
+}
+
+int lzgpu_plan_check_slices(const lzgpu_goal *goals, uint32_t n_slices, uint32_t nb, const uint8_t *given, lzgpu_slices_check_plan *out) {
+	if (!out || !given || nb == 0 || nb > LZGPU_BLOCKS_IN_CHUNK) return LZGPU_ERR_ARG;
+	*out = lzgpu_slices_check_plan{};
+	lzd::SliceLayout lay;
+	const char *why = nullptr;
+	if (lzd::slice_layout(goals, n_slices, lay, &why) != LZGPU_OK) return LZGPU_ERR_ARG;
+	lzd::SliceSolve sv[2];
+	auto ck = std::make_unique<lzd::SliceChecks[]>(2);
+	const uint32_t tail = nb % lay.L;
+	lzd::slice_solve(lay, given, lay.L, sv[0]);
+	lzd::slice_checks(lay, given, sv[0], ck[0], true);
+	if (tail) {
+		lzd::slice_solve(lay, given, tail, sv[1]);
+		lzd::slice_checks(lay, given, sv[1], ck[1], true);
+	}
+	const lzd::SliceChecks &t = tail ? ck[1] : ck[0];
+	out->L = lay.L;
+	out->tail_blocks = tail;
+	out->n_checks = ck[0].n_checks;
+	out->tail_n_checks = t.n_checks;
+	out->checked = ck[0].checked;
+	out->tail_checked = t.checked;
+	out->locatable = ck[0].locatable;
+	out->tail_locatable = t.locatable;
+	const lzd::SliceSolve used[2] = {nb >= lay.L ? sv[0] : sv[1], tail ? sv[1] : sv[0]};
+	const lzd::RsGeometry g = lzd::rs_geometry(lay, given, used, 2, lzd::RsMode::CHECK);
+	out->ok = g.ok ? 1 : 0;
+	out->G = g.G;
+	out->threads = g.threads;
+	out->stages = g.stages;
+	out->smem_bytes = static_cast<uint32_t>(g.smem);
+	return LZGPU_OK;
+}
+
+int lzgpu_debug_check_slices_rows(const lzgpu_goal *goals, uint32_t n_slices, const uint8_t *given, uint32_t valid, uint32_t *n_checks,
+                                  uint8_t *check_part, uint8_t *check_stripe, uint8_t *coef) {
+	if (!given || !n_checks || !check_part || !check_stripe || !coef) return LZGPU_ERR_ARG;
+	lzd::SliceLayout lay;
+	const char *why = nullptr;
+	if (lzd::slice_layout(goals, n_slices, lay, &why) != LZGPU_OK || valid == 0 || valid > lay.L) return LZGPU_ERR_ARG;
+	auto sv = std::make_unique<lzd::SliceSolve>();
+	auto ck = std::make_unique<lzd::SliceChecks>();
+	lzd::slice_solve(lay, given, valid, *sv);
+	lzd::slice_checks(lay, given, *sv, *ck);
+	*n_checks = ck->n_checks;
+	if (ck->n_checks > lzd::kScMaxChecks) return LZGPU_ERR_ARG;
+	std::memset(check_part, 0, 64);
+	std::memset(check_stripe, 0, 64);
+	std::memset(coef, 0, 64 * 64 * 64);
+	for (uint32_t h = 0; h < ck->n_checks; ++h) {
+		check_part[h] = ck->blk_part[ck->def[h]];
+		check_stripe[h] = ck->blk_s[ck->def[h]];
+		for (uint32_t b = 0; b < ck->n_blocks; ++b) coef[(h * 64 + ck->blk_part[b]) * 64 + ck->blk_s[b]] = ck->H[h * ck->n_blocks + b];
+	}
 	return LZGPU_OK;
 }
 

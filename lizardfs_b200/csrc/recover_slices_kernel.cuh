@@ -23,6 +23,13 @@
 // sets its read entry's bit in a shared mask; after the merge every position whose value depends on a failing read entry (the host's
 // dependency mask, RsSalvage) is withheld: the CTA zeroes its image block, which it stored earlier in the stripe, and gives it the CRC
 // of zeros.  Then the stripe's status bytes are written to the map.
+//
+// The CHECK instantiation (lzgpu_check_slices) writes nothing but one map entry per combined stripe.  It stages the basis of
+// slices_check.h (the first copy of each known position, the chosen equations' parity blocks) and every check's defining block (slot
+// L + E + h), solves the unknowns by the particular-solution rows, and in the wanted-parity step re-encodes each check's prediction (a
+// further copy of a known position: that position) and compares it with the defining block word by word.  Each thread ORs bit h into
+// a 64-bit mask where they differ; the warps OR theirs into a shared word pair, and the stripe's entry is {mask, -1, 0}.
+// locate_slices_kernel then names the suspect part of every entry whose mask is not zero.
 #pragma once
 #include <cstdint>
 
@@ -85,7 +92,15 @@ struct RecoverSlicesParams {
 };
 static_assert(sizeof(RecoverSlicesParams) <= 32764, "recover_slices_kernel's parameter block must fit the 32764-byte kernel parameter limit");
 
-// The per-stripe shared words of the SALVAGE instantiation: the failing read entries, then the withheld positions
+// lzgpu_slices_check as the kernels write it
+struct RsCheckEntry {
+	unsigned long long bad_checks;
+	int suspect_part;
+	uint32_t zero;
+};
+
+// The per-stripe shared words of the SALVAGE instantiation: the failing read entries, then the withheld positions (CHECK: words 0
+// and 1 are the stripe's bad_checks)
 __device__ __forceinline__ uint32_t *rs_salvage_smem() {
 	__shared__ uint32_t words[kRsMaskWords + 2];
 	return words;
@@ -103,8 +118,9 @@ __device__ __forceinline__ uint32_t rs_gf_mul(uint32_t v, uint32_t c) {
 	return r;
 }
 
-template <bool SALVAGE>
+template <RsMode MODE>
 __global__ void __launch_bounds__(kRsThreads, 1) recover_slices_kernel(const __grid_constant__ RecoverSlicesParams p) {
+	constexpr bool SALVAGE = MODE == RsMode::SALVAGE, CHECK = MODE == RsMode::CHECK;
 	extern __shared__ __align__(1024) uint8_t smem[];
 	uint32_t *s_tab = reinterpret_cast<uint32_t *>(smem);
 	uint8_t *s_slab = smem + 4096;
@@ -121,9 +137,10 @@ __global__ void __launch_bounds__(kRsThreads, 1) recover_slices_kernel(const __g
 			if (cs >= p.n_cs) break;
 			const RsShape &sh = p.shape[(p.tail && cs == p.n_cs - 1) ? 1 : 0];
 			const uint32_t E = sh.n_eq;
+			[[maybe_unused]] unsigned long long bad = 0;   // CHECK: the checks this thread has seen differ
 			__syncthreads();   // the previous stripe's streams are merged
 			for (uint32_t i = tid; i < sh.n_state * 32u; i += kRsThreads) s_crc[i] = 0;
-			if constexpr (SALVAGE)
+			if constexpr (SALVAGE || CHECK)
 				if (tid < kRsMaskWords + 2) rs_salvage_smem()[tid] = 0;
 			__syncthreads();
 			for (uint32_t slab = 0; slab < 64; ++slab) {
@@ -166,8 +183,11 @@ __global__ void __launch_bounds__(kRsThreads, 1) recover_slices_kernel(const __g
 				for (uint32_t w = 0; w < sh.n_out; ++w) {
 					const uint32_t i = sh.out_slice[w], r = sh.out_row[w], s = sh.out_stripe[w], k = p.k[i];
 					uint32_t v = 0;
-					for (uint32_t j = 0; j < k; ++j) v ^= rs_gf_mul(W[(s * k + j) * 256u + tid], p.gen[i][r][j]);
-					W[(L + E + w) * 256u + tid] = v;
+					if (CHECK && r == kRsNone) v = W[s * 256u + tid];   // a further copy of position s
+					else
+						for (uint32_t j = 0; j < k; ++j) v ^= rs_gf_mul(W[(s * k + j) * 256u + tid], p.gen[i][r][j]);
+					if constexpr (CHECK) bad |= static_cast<unsigned long long>(v != W[(L + E + w) * 256u + tid]) << w;
+					else W[(L + E + w) * 256u + tid] = v;
 				}
 				__syncthreads();
 				// ---------------- store ----------------
@@ -223,6 +243,22 @@ __global__ void __launch_bounds__(kRsThreads, 1) recover_slices_kernel(const __g
 					if constexpr (SALVAGE) atomicOr(&rs_salvage_smem()[en.state >> 5], 1u << (en.state & 31));
 				}
 			}
+			if constexpr (CHECK) {
+				// ---------------- the stripe's entry ----------------
+				uint32_t *mask = rs_salvage_smem();
+				const uint32_t lo = __reduce_or_sync(0xffffffffu, static_cast<uint32_t>(bad)), hi = __reduce_or_sync(0xffffffffu, static_cast<uint32_t>(bad >> 32));
+				if (lane == 0 && (lo | hi)) {
+					atomicOr(&mask[0], lo);
+					atomicOr(&mask[1], hi);
+				}
+				__syncthreads();
+				if (tid == 0) {
+					RsCheckEntry *en = reinterpret_cast<RsCheckEntry *>(p.map) + static_cast<unsigned long long>(c) * p.n_cs + cs;
+					en->bad_checks = (static_cast<unsigned long long>(mask[1]) << 32) | mask[0];
+					en->suspect_part = -1;
+					en->zero = 0;
+				}
+			}
 			if constexpr (SALVAGE) {
 				// ---------------- withhold what depends on a failing block, then the stripe's map bytes ----------------
 				__syncthreads();
@@ -248,6 +284,84 @@ __global__ void __launch_bounds__(kRsThreads, 1) recover_slices_kernel(const __g
 				}
 			}
 		}
+	}
+}
+
+// lzgpu_check_slices' locate pass, per stripe shape (a device buffer: the dense rows and the annihilators exceed the parameter block).
+// The given blocks of the shape, its check rows over them, and per candidate part (a given part with a block in the shape) its
+// annihilator rows, kScMaxChecks bytes each, at rows[ann0 + first[c] ..] after the two shapes.
+struct RsLocateShape {
+	uint32_t n_blocks, n_checks, n_cand, ann0;
+	uint8_t blk_part[kRsMaxEntries], blk_s[kRsMaxEntries];
+	uint8_t cand_part[LZGPU_MAX_PARTS];
+	uint16_t cand_first[LZGPU_MAX_PARTS + 1];
+	uint8_t H[kRsMaxOut][kRsMaxEntries];
+};
+struct RsLocate {
+	RsLocateShape shape[2];   // then the annihilator rows of both shapes
+};
+struct LocateSlicesParams {
+	const uint8_t *parts[LZGPU_MAX_PARTS];
+	unsigned long long part_stride[kSlicesMax];
+	uint32_t spc[kSlicesMax];
+	uint8_t part_slice[LZGPU_MAX_PARTS];
+	RsCheckEntry *map;
+	const RsLocate *loc;
+	unsigned long long n_entries;
+	uint32_t n_cs, tail;
+};
+constexpr int kRslThreads = 128;
+
+// One CTA per bad entry (grid-stride over the map; a clean entry is skipped, its suspect is already -1).  Thread t owns words t,
+// t + 128, ... of the stripe's blocks: it forms the syndrome words S_h = sum_b H[h][b] y_b, and where they are not all zero drops every
+// candidate an annihilator row of which does not map them to zero (a 4-byte word: the test holds for each of its bytes).  The one
+// candidate left is the suspect; none or several: -1.
+__global__ void __launch_bounds__(kRslThreads) locate_slices_kernel(const __grid_constant__ LocateSlicesParams p) {
+	__shared__ uint32_t S[kRsMaxOut][kRslThreads];
+	__shared__ unsigned long long s_alive;
+	const uint32_t tid = threadIdx.x;
+	const uint8_t *ann = reinterpret_cast<const uint8_t *>(p.loc + 1);
+	for (unsigned long long e = blockIdx.x; e < p.n_entries; e += gridDim.x) {
+		if (p.map[e].bad_checks == 0) continue;
+		const uint32_t c = static_cast<uint32_t>(e / p.n_cs), cs = static_cast<uint32_t>(e % p.n_cs);
+		const RsLocateShape &sh = p.loc->shape[(p.tail && cs == p.n_cs - 1) ? 1 : 0];
+		const uint32_t nc = sh.n_checks;
+		if (tid == 0) s_alive = sh.n_cand >= 64 ? ~0ull : (1ull << sh.n_cand) - 1ull;
+		__syncthreads();
+		unsigned long long alive = s_alive;
+		for (uint32_t w = tid; w < 65536u / 4u; w += kRslThreads) {
+			for (uint32_t h = 0; h < nc; ++h) S[h][tid] = 0;
+			for (uint32_t b = 0; b < sh.n_blocks; ++b) {
+				const uint32_t g = sh.blk_part[b], i = p.part_slice[g];
+				const unsigned long long blk = static_cast<unsigned long long>(cs) * p.spc[i] + sh.blk_s[b];
+				const uint32_t v = reinterpret_cast<const uint32_t *>(p.parts[g] + c * p.part_stride[i] + (blk << 16))[w];
+				for (uint32_t h = 0; h < nc; ++h) {
+					const uint32_t coef = sh.H[h][b];
+					if (coef) S[h][tid] ^= rs_gf_mul(v, coef);
+				}
+			}
+			uint32_t any = 0;
+			for (uint32_t h = 0; h < nc; ++h) any |= S[h][tid];
+			if (!any) continue;
+			for (unsigned long long left = alive; left; left &= left - 1) {
+				const uint32_t ci = static_cast<uint32_t>(__ffsll(static_cast<long long>(left)) - 1);
+				bool fits = true;
+				for (uint32_t r = sh.cand_first[ci]; r < sh.cand_first[ci + 1] && fits; ++r) {
+					const uint8_t *row = ann + static_cast<size_t>(sh.ann0 + r) * kRsMaxOut;
+					uint32_t acc = 0;
+					for (uint32_t h = 0; h < nc; ++h) acc ^= rs_gf_mul(S[h][tid], row[h]);
+					fits = acc == 0;
+				}
+				if (!fits) alive &= ~(1ull << ci);
+			}
+		}
+		atomicAnd(&s_alive, alive);
+		__syncthreads();
+		if (tid == 0) {
+			const unsigned long long left = s_alive;
+			p.map[e].suspect_part = left && !(left & (left - 1)) ? sh.cand_part[__ffsll(static_cast<long long>(left)) - 1] : -1;
+		}
+		__syncthreads();
 	}
 }
 

@@ -195,8 +195,10 @@ inline uint64_t slice_needed(const SliceLayout &lay, const uint8_t *want, bool i
 
 // Launch geometry of recover_slices_kernel (recover_slices_kernel.cuh), sized for the largest request the given parts allow (every
 // part that is not given wanted, with its CRCs, and the image), so that it does not depend on `want`: one 256-thread CTA per SM, a
-// unit of G combined stripes, shared memory = the CRC tables + one 1 KiB slab per staged block + 128 bytes per CRC stream.  salvage:
+// unit of G combined stripes, shared memory = the CRC tables + one 1 KiB slab per staged block + 128 bytes per CRC stream.  SALVAGE:
 // the largest salvage request instead (lzgpu_salvage_slices: nothing wanted, every given part verified, the image with its CRCs).
+// CHECK (lzgpu_check_slices): every given part verified, nothing written, a slab per check's defining block (slice_check_count).
+enum class RsMode : int { RECOVER, SALVAGE, CHECK };
 constexpr uint32_t kRsThreadsPerCta = 256, kRsEntryCap = 192, kRsOutCap = 64;
 constexpr size_t kRsSmemCap = 220 * 1024;
 struct RsGeometry {
@@ -205,7 +207,21 @@ struct RsGeometry {
 	size_t smem = 0;
 };
 
-inline RsGeometry rs_geometry(const SliceLayout &lay, const uint8_t *given, const SliceSolve *shapes, int n_shapes, bool salvage = false) {
+// The checks of a shape (lzgpu_check_slices, slices_check.h): its given blocks (a data block past the chunk's end is padding, not
+// one of them) less the rank, |known| + E
+inline uint32_t slice_check_count(const SliceLayout &lay, const uint8_t *given, const SliceSolve &sv) {
+	uint32_t n = 0;
+	for (uint32_t i = 0; i < lay.n_slices; ++i)
+		for (uint32_t p = 0; p < lay.k[i] + lay.m[i]; ++p) {
+			if (!given[lay.base[i] + p]) continue;
+			for (uint32_t s = 0; s < lay.L / lay.k[i]; ++s)
+				if (stripe_exists(lay, i, s, sv.valid) && (p >= lay.k[i] || s * lay.k[i] + p < sv.valid)) ++n;
+		}
+	return n - static_cast<uint32_t>(__builtin_popcountll(sv.known)) - sv.n_eq;
+}
+
+inline RsGeometry rs_geometry(const SliceLayout &lay, const uint8_t *given, const SliceSolve *shapes, int n_shapes, RsMode mode = RsMode::RECOVER) {
+	const bool salvage = mode == RsMode::SALVAGE, check = mode == RsMode::CHECK;
 	RsGeometry g;
 	g.G = lay.L >= 8 ? 1 : 8 / lay.L;
 	g.threads = kRsThreadsPerCta;
@@ -218,10 +234,14 @@ inline RsGeometry rs_geometry(const SliceLayout &lay, const uint8_t *given, cons
 				if (!stripe_exists(lay, i, s, sv.valid)) continue;
 				for (uint32_t p = 0; p < lay.k[i] + lay.m[i]; ++p) {
 					if (given[lay.base[i] + p]) ++reads;
-					else if (!salvage) { ++writes; outs += p >= lay.k[i] ? 1 : 0; }
+					else if (!salvage && !check) { ++writes; outs += p >= lay.k[i] ? 1 : 0; }
 				}
 			}
-		const uint32_t states = salvage ? reads + sv.valid : reads + writes - sv.valid;
+		if (check) {
+			writes = 0;
+			outs = slice_check_count(lay, given, sv);
+		}
+		const uint32_t states = salvage ? reads + sv.valid : check ? reads : reads + writes - sv.valid;
 		fits = fits && reads <= kRsEntryCap && writes <= kRsEntryCap && states <= kRsEntryCap && outs <= kRsOutCap;
 		g.slots = std::max(g.slots, lay.L + sv.n_eq + outs);
 		g.states = std::max(g.states, states);

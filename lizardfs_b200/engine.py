@@ -17,6 +17,7 @@ Everything here is a thin ctypes veneer over the C ABI (include/lzgpu.h): all ar
 bytes happens in the CUDA kernels of liblzgpu.so.  numpy is used only to own host buffers.
 """
 import ctypes as C
+import math
 
 import numpy as np
 
@@ -213,6 +214,28 @@ def _salvage_slices(fn, h, goals, nb, parts, part_crc, with_crc):
     rc = fn(h, _goal_array(goals), len(goals), n, nb, _ptr_array(arrs), strides, crcs, _p(img), nb * BLOCK_SIZE, _p(icrc), _p(smap), bad)
     _check_crc(rc, _name(fn), bad, image=img, image_crc=icrc, map=smap)
     return img, icrc, smap
+
+
+SLICES_CHECK_DTYPE = np.dtype([("bad_checks", np.uint64), ("suspect_part", np.int32), ("zero", np.uint32)])
+
+
+def _check_slices(fn, h, goals, nb, parts, part_crc):
+    pbs = [-(-nb // g.k) for g in goals]
+    slice_of = [i for i, g in enumerate(goals) for _ in range(1 if g.is_std else g.k + g.m)]
+    assert len(parts) == len(slice_of)
+    arrs = [None if p is None else _u8(p).reshape(-1, pbs[slice_of[j]] * BLOCK_SIZE) for j, p in enumerate(parts)]
+    n = next((a.shape[0] for a in arrs if a is not None), 0)
+    crcs = None if part_crc is None else _ptr_array([None if c is None else np.ascontiguousarray(c, dtype=np.uint32) for c in part_crc])
+    L = 1
+    for g in goals:
+        if not g.is_std:
+            L = L * g.k // math.gcd(L, g.k)
+    out = np.zeros((n, -(-nb // L)), dtype=SLICES_CHECK_DTYPE)
+    strides = (C.c_size_t * len(goals))(*[pb * BLOCK_SIZE for pb in pbs])
+    bad = (C.c_int64 * 4)(-1, -1, -1, -1)
+    rc = fn(h, _goal_array(goals), len(goals), n, nb, _ptr_array(arrs), strides, crcs, _p(out), bad)
+    _check_crc(rc, _name(fn), bad, map=out)
+    return out
 
 
 def _part_batch(fn, h, goal, nb, parts, part_crc, result, attr, in_place=False):
@@ -467,6 +490,11 @@ class Pool:
         """Engine.salvage_slices over every device of the pool (lzgpu_pool_salvage_slices): the same arguments, results and errors for
         the whole batch; ChunkCrcError.where = (chunk in the batch, slice, part, block)"""
         return _salvage_slices(self.lib.lzgpu_pool_salvage_slices, self.h, goals, nb, parts, part_crc, with_crc)
+
+    def check_slices(self, goals, nb, parts, part_crc=None):
+        """Engine.check_slices over every device of the pool (lzgpu_pool_check_slices): the same arguments, map and errors for the
+        whole batch; ChunkCrcError.where = (chunk in the batch, slice, part, block)"""
+        return _check_slices(self.lib.lzgpu_pool_check_slices, self.h, goals, nb, parts, part_crc)
 
     def crc_blocks(self, data, block_len=BLOCK_SIZE):
         data = _u8(data).reshape(-1, block_len)
@@ -728,6 +756,47 @@ class Engine:
         rc = self.lib.lzgpu_salvage_slices_dev(self.h, _goal_array(goals), ns, n_chunks, nb, _dev_ptrs(d_parts, n), (C.c_size_t * ns)(*part_stride),
                                                _dev_ptrs(d_part_crc, n), d_image, image_stride, d_image_crc, d_map, bad, stream)
         _check_crc(rc, "salvage_slices_dev", bad)
+
+    SLICES_CHECK_DTYPE = SLICES_CHECK_DTYPE
+
+    def check_slices(self, goals, nb, parts, part_crc=None):
+        """Do the given parts of every slice describe one chunk, combined stripe by combined stripe (lzgpu_check_slices)?  goals, parts,
+        part_crc as in recover_slices.  Returns a structured array [n_chunks, ceil(nb / L)] of SLICES_CHECK_DTYPE (bad_checks, 0 =
+        consistent; suspect_part, the flat part to blame or -1), whether or not any entry is bad; raises ChunkCrcError (.where = chunk,
+        slice, part, block) on a stored-CRC mismatch, with the map, written in full all the same, as .map."""
+        return _check_slices(self.lib.lzgpu_check_slices, self.h, goals, nb, parts, part_crc)
+
+    def check_slices_dev(self, goals, n_chunks, nb, d_parts, part_stride, d_part_crc, d_map, stream=None):
+        """lzgpu_check_slices_dev: d_parts / d_part_crc are lists over the flat parts (device pointers as ints, 0 or None = absent),
+        part_stride one entry per slice; n_chunks * ceil(nb / L) entries of 16 bytes go to d_map (8-byte aligned device memory).
+        Raises ChunkCrcError (.where = chunk, slice, part, block); the map is then still complete."""
+        ns, n = len(goals), sum(1 if g.is_std else g.k + g.m for g in goals)
+        bad = (C.c_int64 * 4)(-1, -1, -1, -1)
+        rc = self.lib.lzgpu_check_slices_dev(self.h, _goal_array(goals), ns, n_chunks, nb, _dev_ptrs(d_parts, n), (C.c_size_t * ns)(*part_stride),
+                                             _dev_ptrs(d_part_crc, n), d_map, bad, stream)
+        _check_crc(rc, "check_slices_dev", bad)
+
+    @staticmethod
+    def plan_check_slices(goals, nb, given):
+        """what check_slices checks with the given flat parts (pure host logic, csrc/slices_check.h; no GPU needed): dict with L,
+        tail_blocks, n_checks, tail_n_checks, checked, tail_checked, locatable, tail_locatable (bit g: flat part g), ok and the launch
+        geometry G, threads, stages, smem_bytes"""
+        out = _lib.LzSlicesCheckPlan()
+        g = np.asarray(given, dtype=np.uint8)
+        _check(_lib.load().lzgpu_plan_check_slices(_goal_array(goals), len(goals), nb, _p(g), C.byref(out)), "plan_check_slices")
+        return {f: getattr(out, f) for f, _ in _lib.LzSlicesCheckPlan._fields_}
+
+    @staticmethod
+    def debug_check_slices_rows(goals, given, valid):
+        """the checks of one stripe shape (csrc/slices_check.h; no GPU needed): (check_part [n], check_stripe [n], coef [n, 64, 64]),
+        coef[h, g, s] the coefficient of block s of flat part g in check h.  Raises LzGpuError(ERR_ARG) with more than 64 checks."""
+        n = C.c_uint32()
+        part, stripe = np.zeros(64, dtype=np.uint8), np.zeros(64, dtype=np.uint8)
+        coef = np.zeros((64, 64, 64), dtype=np.uint8)
+        g = np.asarray(given, dtype=np.uint8)
+        _check(_lib.load().lzgpu_debug_check_slices_rows(_goal_array(goals), len(goals), _p(g), valid, C.byref(n), _p(part), _p(stripe),
+                                                          _p(coef)), "debug_check_slices_rows")
+        return part[:n.value].copy(), stripe[:n.value].copy(), coef[:n.value].copy()
 
     @staticmethod
     def plan_salvage_slices(goals, nb, given):
