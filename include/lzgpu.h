@@ -295,7 +295,8 @@ enum {
 	LZGPU_KERNEL_ENCODE_SLICES = 11,   /* fused_slices_kernel: one-pass encode for several slices (lzgpu_encode_slices); G = combined stripes */
 	LZGPU_KERNEL_RECOVER_SLICES = 12,  /* recover_slices_kernel: recovery from the parts of every slice (lzgpu_recover_slices); G = combined stripes */
 	LZGPU_KERNEL_SALVAGE_SLICES = 13,  /* recover_slices_kernel, SALVAGE form: the determined blocks of a chunk (lzgpu_salvage_slices) */
-	LZGPU_KERNEL_CHECK_SLICES = 14     /* recover_slices_kernel, CHECK form: the consistency map of several slices (lzgpu_check_slices) */
+	LZGPU_KERNEL_CHECK_SLICES = 14,    /* recover_slices_kernel, CHECK form: the consistency map of several slices (lzgpu_check_slices) */
+	LZGPU_KERNEL_CORRECT_SLICES = 15   /* recover_slices_kernel, CORRECT form: the map and the CRC gate of lzgpu_correct_slices */
 };
 typedef struct lzgpu_launch_geometry {
 	int kernel;
@@ -571,6 +572,66 @@ int lzgpu_check_slices(lzgpu_ctx *ctx, const lzgpu_goal *goals, uint32_t n_slice
 int lzgpu_check_slices_dev(lzgpu_ctx *ctx, const lzgpu_goal *goals, uint32_t n_slices, uint32_t n_chunks, uint32_t nb,
                            const void *const *d_parts, const size_t *part_stride, const void *const *d_part_crc,
                            void *d_map, int64_t *bad /* host, [4] */, void *stream);
+
+/* Correction of several slices: the consistency map of lzgpu_check_slices, and every combined stripe it blames on one part corrected
+ * in place, with the new block CRCs, in one call.  Each combined stripe may blame a different part; rebuilding the suspect whole with
+ * lzgpu_recover_slices would spread a second stripe's fault into it (the repair rule of lzgpu_check_stripe_map).
+ *   goals, n_slices, nb, parts, part_stride, part_crc, bad   exactly as in lzgpu_check_slices: flat part numbering, layout and zero
+ *                     padding, every given block verified against its stored CRCs in the same pass, bad[0..3], deferred mode, the
+ *                     CRC-disabled mode and the refusals.  The part buffers must not overlap each other.
+ *   new_crc[g]        optional (new_crc or new_crc[g] NULL: none; _dev: 4-byte aligned), part_crc[g]'s layout: at every block the call
+ *                     writes it receives mycrc32(0, block, 65536) of the block as written (LZGPU_FAKE_CRC with CRCs disabled); nothing
+ *                     else in it is touched.  It may be part_crc[g] itself: the stored CRCs are read before any is written.
+ *   fix[c * n_cs + cs]  (n_cs = ceil(nb / L); every entry written, also when a stored CRC failed; _dev: 8-byte aligned): bad_checks and
+ *                     suspect_part equal what lzgpu_check_slices returns for the same input before the call.
+ * Rule.  Combined stripe cs of chunk c is corrected only when bad_checks != 0, suspect_part = g >= 0, g is correctable in this shape
+ * (lzgpu_plan_correct_slices) and no given block of the stripe outside g fails its stored CRC (padding blocks included).  Otherwise
+ * nothing is written and the status says why: LZGPU_FIX_CLEAN (bad_checks == 0), LZGPU_FIX_UNEXPLAINED (no suspect),
+ * LZGPU_FIX_CRC_CONFLICT (another part's block fails its CRC), LZGPU_FIX_UNDETERMINED (g is named but its blocks are not determined
+ * by the others: two of its blocks have equal columns, say).  A suspect block that fails its own CRC is corrected, as in
+ * lzgpu_correct_stripes.
+ * What is written: g's blocks in the shape (data blocks at positions < nb, the parity blocks of slice stripes that exist; padding never),
+ * each byte y ^ e with e = P_g S the one solution of H_g e = S (P_g: a left inverse of g's columns of the check matrix,
+ * lzgpu_debug_correct_slices_rows).  The result is the only value of g's blocks that satisfies every check with the other given parts;
+ * with one stale part it is the original.  Wherever lzgpu_recover_slices accepts a one-combined-stripe window with g NULL and wanted,
+ * it is byte for byte what that window rebuilds.
+ * With one goal (n_slices = 1, every data part given, padding blocks as encoded: this call never checks or writes them) suspect_part,
+ * status, the bytes written and the CRCs equal lzgpu_correct_stripes on the same input (bad_checks and bad_rows number their checks
+ * differently).
+ * lzgpu_correct_slices returns LZGPU_ERR_CRC when a stored CRC failed (the corrections the rule allows are still made), else
+ * LZGPU_ERR_INCONSISTENT when an entry is left UNEXPLAINED or UNDETERMINED, else LZGPU_OK.  The host form copies back to the caller's
+ * buffers only the rewritten blocks, their CRCs and the fix entries.  lzgpu_correct_slices_dev writes on `stream` and returns LZGPU_OK or
+ * LZGPU_ERR_CRC; it waits for the stream only when stored CRCs are given, as lzgpu_check_slices_dev.  The CRC gate is decided on the
+ * device.  Refused before anything is enqueued, beside lzgpu_check_slices' refusals: no fix, new_crc arrays that are not 4-byte aligned
+ * (LZGPU_ERR_ARG).  The route: the CORRECT instantiation of recover_slices_kernel (lzgpu_debug_last_geometry:
+ * LZGPU_KERNEL_CORRECT_SLICES; LZGPU_GRID_CAP applies), the locate pass over the bad entries, then correct_slices_kernel.
+ * lzgpu_pool_correct_slices cuts the batch as lzgpu_pool_check_slices: parts, part_crc and new_crc move by slice, fix by first * n_cs. */
+enum { LZGPU_FIX_UNDETERMINED = 7 };  /* lzgpu_slices_fix.status, beside LZGPU_FIX_CLEAN .. LZGPU_FIX_DECODED */
+typedef struct lzgpu_slices_fix {
+	uint64_t bad_checks;    /* as lzgpu_slices_check, before the correction */
+	int32_t suspect_part;   /* as lzgpu_slices_check, before the correction (flat part, -1 none) */
+	int32_t status;         /* LZGPU_FIX_CLEAN / _CORRECTED / _UNEXPLAINED / _CRC_CONFLICT / _UNDETERMINED */
+	uint64_t crc_failed;    /* bit g: a given block of flat part g in this combined stripe fails its stored CRC (padding blocks included) */
+	uint64_t changed;       /* CORRECTED: bit s = the suspect's block s in this combined stripe had bytes changed (s: the stripe of its
+	                           slice; for a standard part, the position); else 0 */
+} lzgpu_slices_fix;         /* 32 bytes, 8-byte aligned */
+typedef struct lzgpu_slices_correct_plan {
+	lzgpu_slices_check_plan check;          /* exactly what lzgpu_plan_check_slices returns */
+	uint64_t correctable, tail_correctable; /* bit g: part g is given and its columns of H have full rank, so the other given blocks
+	                                           determine its blocks, and a named g is corrected.  locatable is a subset of this. */
+} lzgpu_slices_correct_plan;
+int lzgpu_plan_correct_slices(const lzgpu_goal *goals, uint32_t n_slices, uint32_t nb, const uint8_t *given, lzgpu_slices_correct_plan *out);
+/* The left inverse P_g of one shape (as lzgpu_debug_check_slices_rows): *n_blocks blocks of flat part `part`, block j being the part's
+ * block blk_s[j] in the combined stripe, and rows[j * 64 + h] the coefficient of syndrome S_h in the error of block j.  LZGPU_ERR_ARG for
+ * bad arguments, more than 64 checks, or a part that is not correctable there. */
+int lzgpu_debug_correct_slices_rows(const lzgpu_goal *goals, uint32_t n_slices, const uint8_t *given, uint32_t valid, int part,
+                                    uint32_t *n_blocks, uint8_t *blk_s /* [64] */, uint8_t *rows /* [64][64] */);
+int lzgpu_correct_slices(lzgpu_ctx *ctx, const lzgpu_goal *goals, uint32_t n_slices, uint32_t n_chunks, uint32_t nb,
+                         uint8_t *const *parts, const size_t *part_stride, const uint32_t *const *part_crc, uint32_t *const *new_crc,
+                         lzgpu_slices_fix *fix, int64_t *bad /* [4] */);
+int lzgpu_correct_slices_dev(lzgpu_ctx *ctx, const lzgpu_goal *goals, uint32_t n_slices, uint32_t n_chunks, uint32_t nb,
+                             void *const *d_parts, const size_t *part_stride, const void *const *d_part_crc, void *const *d_new_crc,
+                             void *d_fix, int64_t *bad /* host, [4] */, void *stream);
 
 /* Degraded read / rebuild of n_chunks chunks.
  *   parts[i]    (i < k+m) part-major buffer of part i for all chunks: chunk c at + c*part_stride,
@@ -895,6 +956,11 @@ int lzgpu_pool_check_slices(lzgpu_pool *pool, const lzgpu_goal *goals, uint32_t 
                             lzgpu_slices_check *map, int64_t *bad);
                              /* lzgpu_check_slices over every device of a pool, host memory only: for any input the code, map and
                               * bad[0..3] lzgpu_check_slices returns on one context for the whole batch (an empty batch runs on slot 0) */
+int lzgpu_pool_correct_slices(lzgpu_pool *pool, const lzgpu_goal *goals, uint32_t n_slices, uint32_t n_chunks, uint32_t nb,
+                              uint8_t *const *parts, const size_t *part_stride, const uint32_t *const *part_crc,
+                              uint32_t *const *new_crc, lzgpu_slices_fix *fix, int64_t *bad);
+                             /* lzgpu_correct_slices over every device of a pool, host memory only: for any input the code, parts,
+                              * new CRCs, fix entries and bad[0..3] lzgpu_correct_slices gives on one context for the whole batch */
 int lzgpu_convert_chunks_dev(lzgpu_ctx *ctx, const lzgpu_goal *src, const lzgpu_goal *dst, uint32_t n_chunks, uint32_t nb,
                              const void *const *d_parts, size_t part_stride, const void *const *d_part_crc,
                              const uint8_t *want, void *const *d_out, size_t out_stride, void *const *d_out_crc,

@@ -87,7 +87,7 @@ class LzEncoderKernel(C.Structure):
 # lzgpu_launch_geometry.kernel
 KERNEL_NONE, KERNEL_ENCODE, KERNEL_ENCODE_BITSLICE, KERNEL_RECOVER_GEO0, KERNEL_RECOVER_GEO1, KERNEL_RECOVER_GEO2, \
     KERNEL_RECOVER_DIRECT, KERNEL_RECOVER_BS3, KERNEL_CONVERT, KERNEL_CHECK, KERNEL_CHECK_DEGRADED, KERNEL_ENCODE_SLICES, \
-    KERNEL_RECOVER_SLICES, KERNEL_SALVAGE_SLICES, KERNEL_CHECK_SLICES = range(15)
+    KERNEL_RECOVER_SLICES, KERNEL_SALVAGE_SLICES, KERNEL_CHECK_SLICES, KERNEL_CORRECT_SLICES = range(16)
 
 
 class LzSlicesRecoverPlan(C.Structure):
@@ -109,6 +109,10 @@ class LzSlicesCheckPlan(C.Structure):
                 ("ok", C.c_int), ("G", C.c_uint32), ("threads", C.c_uint32), ("stages", C.c_uint32), ("smem_bytes", C.c_uint32)]
 
 
+class LzSlicesCorrectPlan(C.Structure):
+    _fields_ = [("check", LzSlicesCheckPlan), ("correctable", C.c_uint64), ("tail_correctable", C.c_uint64)]
+
+
 # lzgpu_salvage_slices' map bytes
 SALVAGE_HOLE, SALVAGE_KNOWN, SALVAGE_SOLVED, SALVAGE_WITHHELD = range(4)
 
@@ -127,6 +131,7 @@ class LzStripeFix(C.Structure):
 
 # lzgpu_stripe_fix.status (lzgpu_stripe_repair.status: also REBUILT and CRC_ONLY; lzgpu_stripe_decode.status: also DECODED)
 FIX_CLEAN, FIX_CORRECTED, FIX_UNEXPLAINED, FIX_CRC_CONFLICT, FIX_REBUILT, FIX_CRC_ONLY, FIX_DECODED = range(7)
+FIX_UNDETERMINED = 7   # lzgpu_slices_fix.status only
 
 
 class LzStripeRepair(C.Structure):
@@ -166,6 +171,8 @@ SIGNATURES = {
     "lzgpu_plan_salvage_slices": (_int, [_goalp, _u32, _u32, _vp, C.POINTER(LzSlicesSalvagePlan)]),
     "lzgpu_plan_check_slices": (_int, [_goalp, _u32, _u32, _vp, C.POINTER(LzSlicesCheckPlan)]),
     "lzgpu_debug_check_slices_rows": (_int, [_goalp, _u32, _vp, _u32, _vp, _vp, _vp, _vp]),
+    "lzgpu_plan_correct_slices": (_int, [_goalp, _u32, _u32, _vp, C.POINTER(LzSlicesCorrectPlan)]),
+    "lzgpu_debug_correct_slices_rows": (_int, [_goalp, _u32, _vp, _u32, _int, _vp, _vp, _vp]),
     "lzgpu_debug_locate_errors": (_int, [_int, _int, _vp, _vp, _vp, _u32, _vp]),
     "lzgpu_goal_slice_type": (_int, [_goalp]),
     "lzgpu_goal_from_slice_type": (_int, [_int, _goalp]),
@@ -196,6 +203,8 @@ SIGNATURES = {
     "lzgpu_salvage_slices_dev": (_int, [_vp, _goalp, _u32, _u32, _u32, _vp, _vp, _vp, _vp, _sz, _vp, _vp, _vp, _vp]),
     "lzgpu_check_slices": (_int, [_vp, _goalp, _u32, _u32, _u32, _vp, _vp, _vp, _vp, _vp]),
     "lzgpu_check_slices_dev": (_int, [_vp, _goalp, _u32, _u32, _u32, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "lzgpu_correct_slices": (_int, [_vp, _goalp, _u32, _u32, _u32, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "lzgpu_correct_slices_dev": (_int, [_vp, _goalp, _u32, _u32, _u32, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "lzgpu_recover_chunks": (_int, [_vp, _goalp, _u32, _u32, _vp, _sz, _vp, _vp, _vp, _vp, _sz, _vp]),
     "lzgpu_recover_chunks_dev": (_int, [_vp, _goalp, _u32, _u32, _vp, _sz, _vp, _vp, _vp, _vp, _sz, _vp, _vp]),
     "lzgpu_check_stripes": (_int, [_vp, _goalp, _u32, _u32, _vp, _sz, _vp, _vp, _vp]),
@@ -280,6 +289,7 @@ SIGNATURES = {
     "lzgpu_pool_recover_slices": (_int, [_vp, _goalp, _u32, _u32, _u32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
     "lzgpu_pool_salvage_slices": (_int, [_vp, _goalp, _u32, _u32, _u32, _vp, _vp, _vp, _vp, _sz, _vp, _vp, _vp]),
     "lzgpu_pool_check_slices": (_int, [_vp, _goalp, _u32, _u32, _u32, _vp, _vp, _vp, _vp, _vp]),
+    "lzgpu_pool_correct_slices": (_int, [_vp, _goalp, _u32, _u32, _u32, _vp, _vp, _vp, _vp, _vp, _vp]),
     "lzgpu_pool_crc_blocks": (_int, [_vp, _vp, _sz, _u32, _sz, _vp]),
     "lzgpu_pool_check_stripes": (_int, [_vp, _goalp, _u32, _u32, _vp, _sz, _vp, _vp, _vp]),
     "lzgpu_pool_check_stripe_map": (_int, [_vp, _goalp, _u32, _u32, _vp, _sz, _vp, _vp, _vp]),

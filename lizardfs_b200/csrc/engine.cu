@@ -2162,16 +2162,19 @@ extern "C" int lzgpu_convert_chunks(lzgpu_ctx *ctx, const lzgpu_goal *src, const
 // recovery from the parts of every slice of a goal together (lzgpu_recover_slices*)
 // ------------------------------------------------------------------------------------------------
 // What the argument check derives for the enqueue: the flat part layout, the solve of both stripe shapes and the launch geometry.
-// salvage: the call is lzgpu_salvage_slices*; check: lzgpu_check_slices*, with the checks of both shapes (set by the caller before
-// the check)
+// salvage: the call is lzgpu_salvage_slices*; check: lzgpu_check_slices*, with the checks of both shapes; correct (with check):
+// lzgpu_correct_slices*, the map being the fix entries (set by the caller before the check)
 struct RecoverSlicesCall {
 	lzd::SliceLayout lay;
 	lzd::SliceSolve shapes[2];   // a full combined stripe, the chunk's last one when L does not divide nb
 	lzd::SliceChecks checks[2];
 	lzd::RsGeometry geo;
 	uint32_t pb[kSlicesMax] = {0};
-	bool salvage = false, check = false;
-	lzd::RsMode mode() const { return check ? lzd::RsMode::CHECK : salvage ? lzd::RsMode::SALVAGE : lzd::RsMode::RECOVER; }
+	bool salvage = false, check = false, correct = false;
+	lzd::RsMode mode() const {
+		return correct ? lzd::RsMode::CORRECT : check ? lzd::RsMode::CHECK : salvage ? lzd::RsMode::SALVAGE : lzd::RsMode::RECOVER;
+	}
+	size_t entry_bytes() const { return correct ? sizeof(lzgpu_slices_fix) : sizeof(lzgpu_slices_check); }
 };
 
 // lzgpu_salvage_slices* and lzgpu_check_slices* want no part
@@ -2181,15 +2184,15 @@ static const uint8_t kWantNone[LZGPU_MAX_PARTS] = {0};
 // (16-byte buffers and strides, 4-byte CRC arrays).  LZGPU_ERR_TOO_FEW_PARTS when a block the call must write is not determined; in the
 // salvage form (c.salvage; want = kWantNone, chunk_out the image) when no part is given, and the image and the map are required.  In
 // the check form (c.check; want = kWantNone, no image, map required) when no part is given or no shape of the batch has a check; more
-// than 64 checks in a shape is LZGPU_ERR_ARG.
+// than 64 checks in a shape is LZGPU_ERR_ARG.  The correction form (c.correct) is the check form with the fix entries as the map.
 static int recover_slices_args(const lzgpu_ctx *ctx, const lzgpu_goal *goals, uint32_t n_slices, uint32_t nb, const void *const *parts,
                                const size_t *part_stride, const void *const *part_crc, const uint8_t *want, const void *const *out,
                                const size_t *out_stride, const void *const *out_crc, const void *chunk_out, size_t chunk_out_stride, bool dev,
                                RecoverSlicesCall &c, const void *image_crc = nullptr, const void *map = nullptr) {
 	if (!ctx || !parts || !part_stride || !want) return LZGPU_ERR_ARG;
-	const char *fn = c.check ? "check_slices" : c.salvage ? "salvage_slices" : "recover_slices";
+	const char *fn = c.correct ? "correct_slices" : c.check ? "check_slices" : c.salvage ? "salvage_slices" : "recover_slices";
 	if (c.salvage && (!chunk_out || !map)) { lz_set_error("salvage_slices: the image and the map are required"); return LZGPU_ERR_ARG; }
-	if (c.check && !map) { lz_set_error("check_slices: the map is required"); return LZGPU_ERR_ARG; }
+	if (c.check && !map) { lz_set_error("%s: the %s is required", fn, c.correct ? "fix" : "map"); return LZGPU_ERR_ARG; }
 	const char *why = nullptr;
 	if (lzd::slice_layout(goals, n_slices, c.lay, &why)) { lz_set_error("%s: %s", fn, why); return LZGPU_ERR_ARG; }
 	if (nb == 0 || nb > LZGPU_BLOCKS_IN_CHUNK) { lz_set_error("nb out of range"); return LZGPU_ERR_ARG; }
@@ -2240,12 +2243,12 @@ static int recover_slices_args(const lzgpu_ctx *ctx, const lzgpu_goal *goals, ui
 		if (t == 0 ? nb < lay.L : tail == 0) continue;
 		lzd::slice_checks(lay, given, c.shapes[t], c.checks[t]);
 		if (c.checks[t].n_checks > lzd::kScMaxChecks) {
-			lz_set_error("check_slices: the %s combined stripe has %u checks, more than 64", t ? "last" : "full", c.checks[t].n_checks);
+			lz_set_error("%s: the %s combined stripe has %u checks, more than 64", fn, t ? "last" : "full", c.checks[t].n_checks);
 			return LZGPU_ERR_ARG;
 		}
 	}
 	if (c.check && (nb < lay.L || !c.checks[0].n_checks) && (!tail || !c.checks[1].n_checks)) {
-		lz_set_error("check_slices: no combined stripe of the batch has a check");
+		lz_set_error("%s: no combined stripe of the batch has a check", fn);
 		return LZGPU_ERR_TOO_FEW_PARTS;
 	}
 	for (int t = 0; t < 2 && !c.salvage && !c.check; ++t) {   // salvage writes what is determined, holes are not refused
@@ -2274,7 +2277,7 @@ static uint64_t recover_slices_alg_bytes(const RecoverSlicesCall &c, uint32_t n_
 	const uint64_t B = LZGPU_BLOCK_SIZE;
 	uint64_t per_chunk = image ? static_cast<uint64_t>(nb) * B : 0;
 	if (c.salvage) per_chunk += static_cast<uint64_t>(nb) * (image_crcs ? 5 : 1);
-	if (c.check) per_chunk += (nb + c.lay.L - 1) / c.lay.L * sizeof(lzgpu_slices_check);
+	if (c.check) per_chunk += (nb + c.lay.L - 1) / c.lay.L * c.entry_bytes();
 	for (uint32_t i = 0; i < c.lay.n_slices; ++i)
 		for (uint32_t g = c.lay.base[i]; g < c.lay.base[i] + c.lay.k[i] + c.lay.m[i]; ++g) {
 			if (parts[g]) per_chunk += c.pb[i] * (B + (crcs ? 4 : 0));
@@ -2297,14 +2300,14 @@ static void recover_slices_bad(const lzd::SliceLayout &lay, const int64_t *b3, i
 static int recover_slices_enqueue(lzgpu_ctx *ctx, const RecoverSlicesCall &c, uint32_t n_chunks, uint32_t nb, const void *const *d_parts,
                                   const size_t *part_stride, const void *const *d_part_crc, const uint8_t *want, void *const *d_out,
                                   const size_t *out_stride, void *const *d_out_crc, void *d_chunk_out, size_t chunk_out_stride, cudaStream_t st,
-                                  VerifyTicket *tk, void *d_image_crc = nullptr, void *d_map = nullptr) {
+                                  VerifyTicket *tk, void *d_image_crc = nullptr, void *d_map = nullptr, void *const *d_new_crc = nullptr) {
 	bool verifying = false;
 	for (uint32_t g = 0; g < c.lay.n_parts; ++g) verifying |= d_parts[g] && d_part_crc && d_part_crc[g];
 	int rc;
 	if (verifying && (rc = tk->arm(ctx, st))) return rc;
 	if ((rc = lz_recover_slices(ctx, c.lay, c.shapes, c.geo, n_chunks, nb, d_parts, part_stride, verifying ? d_part_crc : nullptr, want, d_out,
-	                            out_stride, d_out_crc, d_chunk_out, chunk_out_stride, d_image_crc, d_map, c.check ? c.checks : nullptr, st,
-	                            verifying ? tk->word(0) : nullptr)))
+	                            out_stride, d_out_crc, d_chunk_out, chunk_out_stride, d_image_crc, d_map, c.check ? c.checks : nullptr,
+	                            d_new_crc, c.correct, st, verifying ? tk->word(0) : nullptr)))
 		return rc;
 	if (!c.check) ctx->stats.chunks_recovered += n_chunks;
 	return verifying ? tk->publish_fused() : LZGPU_OK;
@@ -2314,14 +2317,14 @@ static int recover_slices_enqueue(lzgpu_ctx *ctx, const RecoverSlicesCall &c, ui
 static int recover_slices_dev_call(lzgpu_ctx *ctx, const RecoverSlicesCall &c, uint32_t n_chunks, uint32_t nb, const void *const *d_parts,
                                    const size_t *part_stride, const void *const *d_part_crc, const uint8_t *want, void *const *d_out,
                                    const size_t *out_stride, void *const *d_out_crc, void *d_chunk_out, size_t chunk_out_stride,
-                                   void *d_image_crc, void *d_map, int64_t *bad, void *stream) {
+                                   void *d_image_crc, void *d_map, int64_t *bad, void *stream, void *const *d_new_crc = nullptr) {
 	if (bad) bad[0] = bad[1] = bad[2] = bad[3] = -1;
 	int64_t b3[3] = {-1, -1, -1};
 	const int rc = dev_call(ctx, stream, recover_slices_alg_bytes(c, n_chunks, nb, d_parts, d_part_crc != nullptr, want, d_out_crc != nullptr,
 	                                                              d_chunk_out != nullptr, d_image_crc != nullptr),
 	                        b3, [&](cudaStream_t st, VerifyTicket *tk) {
 		                        return recover_slices_enqueue(ctx, c, n_chunks, nb, d_parts, part_stride, d_part_crc, want, d_out, out_stride, d_out_crc,
-		                                                      d_chunk_out, chunk_out_stride, st, tk, d_image_crc, d_map);
+		                                                      d_chunk_out, chunk_out_stride, st, tk, d_image_crc, d_map, d_new_crc);
 	                        });
 	if (rc == LZGPU_ERR_CRC) recover_slices_bad(c.lay, b3, bad);
 	return rc;
@@ -2368,13 +2371,30 @@ extern "C" int lzgpu_check_slices_dev(lzgpu_ctx *ctx, const lzgpu_goal *goals, u
 	                               nullptr, d_map, bad, stream);
 }
 
-// The host form of the three calls, after their argument check: the given parts (+ stored CRCs) staged tile by tile, the wanted
+extern "C" int lzgpu_correct_slices_dev(lzgpu_ctx *ctx, const lzgpu_goal *goals, uint32_t n_slices, uint32_t n_chunks, uint32_t nb,
+                                         void *const *d_parts, const size_t *part_stride, const void *const *d_part_crc, void *const *d_new_crc,
+                                         void *d_fix, int64_t *bad, void *stream) {
+	NvtxScope nvtx_scope("lzgpu::correct_slices_dev");
+	auto c = std::make_unique<RecoverSlicesCall>();
+	c->check = c->correct = true;
+	int rc = recover_slices_args(ctx, goals, n_slices, nb, d_parts, part_stride, d_part_crc, kWantNone, nullptr, nullptr, nullptr, nullptr, 0,
+	                             true, *c, nullptr, d_fix);
+	if (rc) return rc;
+	if ((rc = check_part_ptrs("correct_slices", "new_crc", d_new_crc, static_cast<int>(c->lay.n_parts), 4))) return rc;
+	if (reinterpret_cast<uintptr_t>(d_fix) & 7) { lz_set_error("correct_slices: fix is not 8-byte aligned"); return LZGPU_ERR_ARG; }
+	if (n_chunks == 0) return LZGPU_OK;
+	return recover_slices_dev_call(ctx, *c, n_chunks, nb, d_parts, part_stride, d_part_crc, kWantNone, nullptr, nullptr, nullptr, nullptr, 0,
+	                               nullptr, d_fix, bad, stream, d_new_crc);
+}
+
+// The host form of the four calls, after their argument check: the given parts (+ stored CRCs) staged tile by tile, the wanted
 // parts (+ CRCs), the image and the salvage form's image CRCs and map (or the check form's map) copied back.  The salvage and check
-// forms run every tile past a CRC mismatch, so that their outputs are complete.
+// forms run every tile past a CRC mismatch, so that their outputs are complete.  The correction form corrects the staged tile and
+// copies back its fix entries, and then, for each corrected entry, only the suspect's rewritten blocks and their new CRCs (new_crc).
 static int recover_slices_host(lzgpu_ctx *ctx, const RecoverSlicesCall &c, uint32_t n_chunks, uint32_t nb, const uint8_t *const *parts,
                                const size_t *part_stride, const uint32_t *const *part_crc, const uint8_t *want, uint8_t *const *out,
                                const size_t *out_stride, uint32_t *const *out_crc, uint8_t *chunk_out, size_t chunk_out_stride,
-                               uint32_t *image_crc, uint8_t *map, int64_t *bad) {
+                               uint32_t *image_crc, uint8_t *map, int64_t *bad, uint32_t *const *new_crc = nullptr) {
 	int rc;
 	if (bad) bad[0] = bad[1] = bad[2] = bad[3] = -1;
 	const lzd::SliceLayout &lay = c.lay;
@@ -2383,6 +2403,7 @@ static int recover_slices_host(lzgpu_ctx *ctx, const RecoverSlicesCall &c, uint3
 	// device layout of a tile: every given part, then every wanted part, then the image and the map, each dense (tile chunks of pb_i
 	// blocks, nb blocks, nb bytes); the stored and the computed CRCs likewise, the image CRCs last
 	size_t off[LZGPU_MAX_PARTS] = {0}, crc_off[LZGPU_MAX_PARTS] = {0}, bytes[LZGPU_MAX_PARTS] = {0}, per_chunk = 0, crc_words = 0;
+	size_t new_crc_off[LZGPU_MAX_PARTS] = {0};
 	size_t dstride[kSlicesMax] = {0};
 	for (uint32_t g = 0; g < n; ++g) {
 		const int i = lay.slice_of(g);
@@ -2395,11 +2416,16 @@ static int recover_slices_host(lzgpu_ctx *ctx, const RecoverSlicesCall &c, uint3
 			crc_off[g] = crc_words;
 			crc_words += c.pb[i];
 		}
+		if (parts[g] && new_crc && new_crc[g]) {
+			new_crc_off[g] = crc_words;
+			crc_words += c.pb[i];
+		}
 	}
 	const size_t img_off = per_chunk, img_bytes = chunk_out ? static_cast<size_t>(nb) * B : 0;
 	per_chunk += img_bytes;
 	const size_t map_off = per_chunk, img_crc_off = crc_words;
-	const size_t map_bytes = !map ? 0 : c.check ? (nb + lay.L - 1) / lay.L * sizeof(lzgpu_slices_check) : nb;
+	const uint32_t n_cs = (nb + lay.L - 1) / lay.L;
+	const size_t map_bytes = !map ? 0 : c.check ? n_cs * c.entry_bytes() : nb;
 	per_chunk += map_bytes;
 	if (image_crc) crc_words += nb;
 	std::lock_guard<std::mutex> lk(ctx->mu);
@@ -2423,6 +2449,7 @@ static int recover_slices_host(lzgpu_ctx *ctx, const RecoverSlicesCall &c, uint3
 	int64_t b3[3] = {-1, -1, -1};
 	rc = run_tiles(ctx, n_chunks, tile, n_slots, b3, [&](int s, size_t c0, size_t nc, cudaStream_t st, VerifyTicket *tk) -> int {
 		void *dp[LZGPU_MAX_PARTS] = {nullptr}, *dpc[LZGPU_MAX_PARTS] = {nullptr}, *dout[LZGPU_MAX_PARTS] = {nullptr}, *docrc[LZGPU_MAX_PARTS] = {nullptr};
+		void *dncrc[LZGPU_MAX_PARTS] = {nullptr};
 		bool any_crc = false;
 		for (uint32_t g = 0; g < n; ++g) {
 			const int i = lay.slice_of(g);
@@ -2437,6 +2464,7 @@ static int recover_slices_host(lzgpu_ctx *ctx, const RecoverSlicesCall &c, uint3
 					dpc[g] = cbuf;
 					any_crc = true;
 				}
+				if (new_crc && new_crc[g]) dncrc[g] = static_cast<uint32_t *>(d_crc[s]) + tile * new_crc_off[g];
 			} else if (want[g]) {
 				dout[g] = buf;
 				if (out_crc && out_crc[g]) docrc[g] = cbuf;
@@ -2450,7 +2478,7 @@ static int recover_slices_host(lzgpu_ctx *ctx, const RecoverSlicesCall &c, uint3
 			BatchTimer timer(ctx, st, recover_slices_alg_bytes(c, static_cast<uint32_t>(nc), nb, dp, any_crc, want, out_crc != nullptr, chunk_out != nullptr,
 			                                                   image_crc != nullptr));
 			rc = recover_slices_enqueue(ctx, c, static_cast<uint32_t>(nc), nb, dp, dstride, any_crc ? dpc : nullptr, want, dout, dstride,
-			                            out_crc ? docrc : nullptr, dimg, img_bytes, st, tk, dimg_crc, dmap);
+			                            out_crc ? docrc : nullptr, dimg, img_bytes, st, tk, dimg_crc, dmap, dncrc);
 		}
 		if (rc) return rc;
 		for (uint32_t g = 0; g < n; ++g) {
@@ -2469,6 +2497,31 @@ static int recover_slices_host(lzgpu_ctx *ctx, const RecoverSlicesCall &c, uint3
 			ctx->stats.bytes_d2h += nc * map_bytes;
 		}
 		if (image_crc) CUDA_TRY(cudaMemcpyAsync(image_crc + c0 * nb, dimg_crc, nc * nb * 4, cudaMemcpyDeviceToHost, st));
+		if (!c.correct) return LZGPU_OK;
+		// the corrected entries' rewritten blocks, a run of consecutive part blocks at a time, and their new CRCs
+		CUDA_TRY(cudaStreamSynchronize(st));
+		const lzgpu_slices_fix *fix = reinterpret_cast<const lzgpu_slices_fix *>(map) + c0 * n_cs;
+		for (size_t e = 0; e < nc * n_cs; ++e) {
+			if (fix[e].status != LZGPU_FIX_CORRECTED) continue;
+			const size_t cc = e / n_cs, cs = e % n_cs;
+			const lzd::SliceChecks &ck = c.checks[(nb % lay.L) && cs == n_cs - 1 ? 1 : 0];
+			const uint32_t g = static_cast<uint32_t>(fix[e].suspect_part);
+			const int i = lay.slice_of(g);
+			const size_t spc = lay.L / lay.k[i];
+			for (uint32_t b = 0; b < ck.n_blocks;) {
+				if (ck.blk_part[b] != g) { ++b; continue; }
+				uint32_t run = 1;
+				while (b + run < ck.n_blocks && ck.blk_part[b + run] == g && ck.blk_s[b + run] == ck.blk_s[b] + run) ++run;
+				const size_t blk = cs * spc + ck.blk_s[b];
+				CUDA_TRY(cudaMemcpyAsync(const_cast<uint8_t *>(parts[g]) + (c0 + cc) * part_stride[i] + blk * B,
+				                         static_cast<const uint8_t *>(dp[g]) + cc * bytes[g] + blk * B, run * B, cudaMemcpyDeviceToHost, st));
+				ctx->stats.bytes_d2h += run * B;
+				if (dncrc[g])
+					CUDA_TRY(cudaMemcpyAsync(new_crc[g] + (c0 + cc) * c.pb[i] + blk, static_cast<const uint32_t *>(dncrc[g]) + cc * c.pb[i] + blk,
+					                         run * 4, cudaMemcpyDeviceToHost, st));
+				b += run;
+			}
+		}
 		return LZGPU_OK;
 	}, c.salvage || c.check);
 	if (rc == LZGPU_ERR_CRC) recover_slices_bad(lay, b3, bad);
@@ -2519,6 +2572,28 @@ extern "C" int lzgpu_check_slices(lzgpu_ctx *ctx, const lzgpu_goal *goals, uint3
 	const size_t n = static_cast<size_t>(n_chunks) * ((nb + c->lay.L - 1) / c->lay.L);
 	for (size_t e = 0; e < n; ++e)
 		if (map[e].bad_checks) return LZGPU_ERR_INCONSISTENT;
+	return LZGPU_OK;
+}
+
+extern "C" int lzgpu_correct_slices(lzgpu_ctx *ctx, const lzgpu_goal *goals, uint32_t n_slices, uint32_t n_chunks, uint32_t nb,
+                                     uint8_t *const *parts, const size_t *part_stride, const uint32_t *const *part_crc, uint32_t *const *new_crc,
+                                     lzgpu_slices_fix *fix, int64_t *bad) {
+	NvtxScope nvtx_scope("lzgpu::correct_slices");
+	auto c = std::make_unique<RecoverSlicesCall>();
+	c->check = c->correct = true;
+	int rc = recover_slices_args(ctx, goals, n_slices, nb, reinterpret_cast<const void *const *>(parts), part_stride,
+	                             reinterpret_cast<const void *const *>(part_crc), kWantNone, nullptr, nullptr, nullptr, nullptr, 0, false, *c,
+	                             nullptr, fix);
+	if (rc) return rc;
+	if ((rc = check_part_ptrs("correct_slices", "new_crc", reinterpret_cast<const void *const *>(new_crc), static_cast<int>(c->lay.n_parts), 4)))
+		return rc;
+	if (n_chunks == 0) return LZGPU_OK;
+	rc = recover_slices_host(ctx, *c, n_chunks, nb, parts, part_stride, part_crc, kWantNone, nullptr, nullptr, nullptr, nullptr, 0, nullptr,
+	                         reinterpret_cast<uint8_t *>(fix), bad, new_crc);
+	if (rc) return rc;
+	const size_t n = static_cast<size_t>(n_chunks) * ((nb + c->lay.L - 1) / c->lay.L);
+	for (size_t e = 0; e < n; ++e)
+		if (fix[e].status == LZGPU_FIX_UNEXPLAINED || fix[e].status == LZGPU_FIX_UNDETERMINED) return LZGPU_ERR_INCONSISTENT;
 	return LZGPU_OK;
 }
 

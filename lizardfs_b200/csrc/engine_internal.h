@@ -215,7 +215,8 @@ int lz_fused_encode_slices(lzgpu_ctx *ctx, const lzgpu_goal *goals, uint32_t n_s
 // whenever d_part_crc is given.  d_map != nullptr: the salvage form (lzgpu_salvage_slices*: nothing wanted, the image, its optional
 // block CRCs d_image_crc and the status bytes d_map), on the SALVAGE instantiation.  checks != nullptr: the check form
 // (lzgpu_check_slices*: nothing wanted, no image, checks[0..1] of both shapes, the entries d_map), on the CHECK instantiation and then
-// the locate pass.
+// the locate pass.  correct: the correction form (lzgpu_correct_slices*: as the check form, d_map the fix entries, d_new_crc the optional
+// new CRC arrays per flat part), on the CORRECT instantiation, the locate pass and correct_slices_kernel.
 namespace lzd {
 struct SliceLayout;
 struct SliceSolve;
@@ -225,7 +226,8 @@ struct RsGeometry;
 int lz_recover_slices(lzgpu_ctx *ctx, const lzd::SliceLayout &lay, const lzd::SliceSolve *shapes, const lzd::RsGeometry &geo, uint32_t n_chunks,
                       uint32_t nb, const void *const *d_parts, const size_t *part_stride, const void *const *d_part_crc, const uint8_t *want,
                       void *const *d_out, const size_t *out_stride, void *const *d_out_crc, void *d_image, size_t image_stride, void *d_image_crc,
-                      void *d_map, const lzd::SliceChecks *checks, cudaStream_t st, unsigned long long *d_first_bad);
+                      void *d_map, const lzd::SliceChecks *checks, void *const *d_new_crc, bool correct, cudaStream_t st,
+                      unsigned long long *d_first_bad);
 // CRC of 64 KiB blocks: block (c, b) at base + c*chunk_stride + b*65536, out[c*out_chunk_stride + b]
 int lz_fused_crc(lzgpu_ctx *ctx, const void *base, unsigned long long n_blocks, unsigned long long blocks_per_chunk,
                  unsigned long long chunk_stride, void *out, unsigned long long out_chunk_stride, cudaStream_t st);

@@ -330,11 +330,12 @@ static const struct {
 	SlicesKernel fn;
 } kSlicers[] = {{1, fused_slices_kernel<1>}, {2, fused_slices_kernel<2>}, {3, fused_slices_kernel<3>}, {4, fused_slices_kernel<4>}};
 
-// Recovery from the parts of every slice together (recover_slices_kernel): one instantiation for any goal set, and its SALVAGE and
-// CHECK twins, indexed by RsMode
+// Recovery from the parts of every slice together (recover_slices_kernel): one instantiation for any goal set, and its SALVAGE,
+// CHECK and CORRECT twins, indexed by RsMode
 using RecoverSlicesKernel = void (*)(RecoverSlicesParams);
 static const RecoverSlicesKernel kRecoverSlicers[] = {recover_slices_kernel<RsMode::RECOVER>, recover_slices_kernel<RsMode::SALVAGE>,
-                                                      recover_slices_kernel<RsMode::CHECK>};
+                                                      recover_slices_kernel<RsMode::CHECK>, recover_slices_kernel<RsMode::CORRECT>};
+static_assert(sizeof(RsFixEntry) == sizeof(lzgpu_slices_fix) && sizeof(RsCheckEntry) == sizeof(lzgpu_slices_check), "entry layouts");
 
 // function attributes are per device: set once per context
 static int set_all_smem_attrs(const FusedState *fs) {
@@ -358,6 +359,7 @@ static int set_all_smem_attrs(const FusedState *fs) {
 		if ((rc = set_smem(k.fn, kSlicesSmemCap))) return rc;
 	for (const RecoverSlicesKernel k : kRecoverSlicers)
 		if ((rc = set_smem(k, static_cast<int>(kRsSmemCap)))) return rc;
+	if ((rc = set_smem(correct_slices_kernel, static_cast<int>(rsc_smem_bytes(kScMaxChecks, kRsMaxL))))) return rc;
 	return LZGPU_OK;
 }
 
@@ -1070,11 +1072,15 @@ static void rs_fill_salvage(RsSalvage &o, const RsShape &sh, const SliceLayout &
 }
 
 // lzgpu_check_slices' locate pass, after the CHECK launch has written every entry: the tables of both shapes in a stream-ordered
-// temporary, and one CTA per bad entry
+// temporary, and one CTA per bad entry.  d_fix: lzgpu_correct_slices, after the CORRECT launch (d_map a temporary, d_crc_failed its
+// masks): the rows of P of both shapes after the annihilators, then correct_slices_kernel over every entry.
 static int rs_locate(lzgpu_ctx *ctx, const SliceLayout &lay, const SliceChecks *checks, uint32_t n_chunks, uint32_t nb,
-                     const void *const *d_parts, const size_t *part_stride, RsCheckEntry *d_map, cudaStream_t st) {
+                     const void *const *d_parts, const size_t *part_stride, RsCheckEntry *d_map, cudaStream_t st,
+                     RsFixEntry *d_fix = nullptr, const unsigned long long *d_crc_failed = nullptr, void *const *d_new_crc = nullptr) {
 	const uint32_t n_cs = (nb + lay.L - 1) / lay.L, tail = nb % lay.L ? 1u : 0u;
-	const size_t rows = checks[0].ann.size() / kScMaxChecks + (tail ? checks[1].ann.size() / kScMaxChecks : 0);
+	size_t rows = checks[0].ann.size() / kScMaxChecks + (tail ? checks[1].ann.size() / kScMaxChecks : 0);
+	const size_t ann_rows = rows;
+	if (d_fix) rows += checks[0].n_blocks + (tail ? checks[1].n_blocks : 0);
 	std::vector<uint8_t> host(sizeof(RsLocate) + rows * kRsMaxOut, 0);
 	RsLocate *loc = reinterpret_cast<RsLocate *>(host.data());
 	uint8_t *ann = host.data() + sizeof(RsLocate);
@@ -1100,6 +1106,26 @@ static int rs_locate(lzgpu_ctx *ctx, const SliceLayout &lay, const SliceChecks *
 		std::memcpy(ann + static_cast<size_t>(row0) * kRsMaxOut, ck.ann.data(), ck.ann.size());
 		row0 += static_cast<uint32_t>(ck.ann.size() / kScMaxChecks);
 	}
+	auto cp = std::make_unique<CorrectSlicesParams>();
+	std::memset(cp.get(), 0, sizeof(CorrectSlicesParams));
+	size_t smem = 0;
+	for (uint32_t t = 0, prow = static_cast<uint32_t>(ann_rows); d_fix && t < 2; ++t) {
+		if (t == 0 ? nb < lay.L : !tail) continue;
+		const SliceChecks &ck = checks[t];
+		RsCorrectShape &o = cp->shape[t];
+		o.correctable = ck.correctable;
+		o.prow0 = prow;
+		uint32_t most = 0;
+		for (uint32_t b = 0; b < ck.n_blocks; ++b) {
+			const uint32_t g = ck.blk_part[b];
+			if (!o.blk_count[g]) o.blk_first[g] = static_cast<uint8_t>(b);
+			++o.blk_count[g];
+			if ((ck.correctable >> g) & 1ull) most = std::max<uint32_t>(most, o.blk_count[g]);
+			std::memcpy(ann + static_cast<size_t>(prow + b) * kRsMaxOut, &ck.pinv[static_cast<size_t>(b) * kScMaxChecks], kScMaxChecks);
+		}
+		prow += ck.n_blocks;
+		smem = std::max(smem, rsc_smem_bytes(ck.n_checks, most));
+	}
 	TmpBuf d_loc(ctx, st);
 	int rc;
 	if ((rc = d_loc.alloc(host.size()))) return rc;
@@ -1124,13 +1150,39 @@ static int rs_locate(lzgpu_ctx *ctx, const SliceLayout &lay, const SliceChecks *
 	locate_slices_kernel<<<static_cast<unsigned>(grid), kRslThreads, 0, st>>>(*p);
 	CUDA_TRY(cudaGetLastError());
 	ctx->stats.kernel_launches++;
+	if (!d_fix) return LZGPU_OK;
+	for (uint32_t i = 0; i < lay.n_slices; ++i) {
+		cp->part_stride[i] = part_stride[i];
+		cp->spc[i] = lay.L / lay.k[i];
+		cp->pb[i] = (nb + lay.k[i] - 1) / lay.k[i];
+		for (uint32_t g = lay.base[i]; g < lay.base[i] + lay.k[i] + lay.m[i]; ++g) {
+			cp->part_slice[g] = static_cast<uint8_t>(i);
+			cp->parts[g] = static_cast<uint8_t *>(const_cast<void *>(d_parts[g]));
+			cp->new_crc[g] = d_new_crc ? static_cast<uint32_t *>(d_new_crc[g]) : nullptr;
+		}
+	}
+	cp->map = d_map;
+	cp->crc_failed = d_crc_failed;
+	cp->fix = d_fix;
+	cp->loc = p->loc;
+	cp->tables = ctx->d_crc_tables;
+	cp->n_entries = p->n_entries;
+	cp->n_cs = n_cs;
+	cp->tail = tail;
+	cp->crc_off = lzgpu_crc_enabled() ? 0u : 1u;
+	cp->zconst = lz::crc_of_zeros(LZGPU_BLOCK_SIZE);
+	cp->run_mult = lz::crc_xpow_bytes(kRscRun);
+	for (int i = 0; i < 5; ++i) cp->tree_mult[i] = lz::crc_xpow_bytes(2048ull << i);
+	correct_slices_kernel<<<static_cast<unsigned>(grid), kRscThreads, smem, st>>>(*cp);
+	CUDA_TRY(cudaGetLastError());
+	ctx->stats.kernel_launches++;
 	return LZGPU_OK;
 }
 
 int lz_recover_slices(lzgpu_ctx *ctx, const SliceLayout &lay, const SliceSolve *shapes, const RsGeometry &geo, uint32_t n_chunks, uint32_t nb,
                       const void *const *d_parts, const size_t *part_stride, const void *const *d_part_crc, const uint8_t *want, void *const *d_out,
                       const size_t *out_stride, void *const *d_out_crc, void *d_image, size_t image_stride, void *d_image_crc, void *d_map,
-                      const SliceChecks *checks, cudaStream_t st, unsigned long long *d_first_bad) {
+                      const SliceChecks *checks, void *const *d_new_crc, bool correct, cudaStream_t st, unsigned long long *d_first_bad) {
 	auto p = std::make_unique<RecoverSlicesParams>();
 	std::memset(p.get(), 0, sizeof(RecoverSlicesParams));
 	const bool crc_on = lzgpu_crc_enabled() != 0;
@@ -1167,18 +1219,29 @@ int lz_recover_slices(lzgpu_ctx *ctx, const SliceLayout &lay, const SliceSolve *
 	for (int i = 0; i < 5; ++i) p->tree_mult[i] = lz::crc_xpow_bytes(2048ull << i);
 	const bool verifying = d_part_crc != nullptr;
 	if (verifying && !d_first_bad) return LZGPU_ERR_ARG;  // (cannot happen: the caller arms a ticket whenever it passes stored CRCs)
-	const RsMode mode = checks ? RsMode::CHECK : d_map ? RsMode::SALVAGE : RsMode::RECOVER;
+	const RsMode mode = correct ? RsMode::CORRECT : checks ? RsMode::CHECK : d_map ? RsMode::SALVAGE : RsMode::RECOVER;
 	p->image_crc = static_cast<uint32_t *>(d_image_crc);
 	p->map = static_cast<uint8_t *>(d_map);
+	TmpBuf d_tmp(ctx, st);   // CORRECT: the check's entries and the failing-part masks, before correct_slices_kernel writes d_map
+	const unsigned long long n_entries = static_cast<unsigned long long>(n_chunks) * p->n_cs;
+	if (correct) {
+		int rc;
+		if ((rc = d_tmp.alloc(n_entries * (sizeof(RsCheckEntry) + sizeof(unsigned long long))))) return rc;
+		p->map = static_cast<uint8_t *>(d_tmp.p);
+		p->crc_failed = reinterpret_cast<unsigned long long *>(p->map + n_entries * sizeof(RsCheckEntry));
+	}
 	for (int t = 0; t < 2; ++t)
 		if (t == 0 ? nb >= lay.L : p->tail != 0) {
 			rs_fill_shape(p->shape[t], lay, shapes[t], d_parts, d_part_crc, want, d_out_crc, d_image != nullptr, d_image_crc != nullptr,
 			              checks ? &checks[t] : nullptr);
 			if (mode == RsMode::SALVAGE) rs_fill_salvage(p->salvage[t], p->shape[t], lay, shapes[t]);
 		}
-	static const int kKernelOf[] = {LZGPU_KERNEL_RECOVER_SLICES, LZGPU_KERNEL_SALVAGE_SLICES, LZGPU_KERNEL_CHECK_SLICES};
+	static const int kKernelOf[] = {LZGPU_KERNEL_RECOVER_SLICES, LZGPU_KERNEL_SALVAGE_SLICES, LZGPU_KERNEL_CHECK_SLICES,
+	                                LZGPU_KERNEL_CORRECT_SLICES};
 	const lzgpu_launch_geometry g = launch_geo(kKernelOf[static_cast<int>(mode)], geo.threads, geo.G, geo.stages, 0, geo.smem);
 	int rc = launch(ctx, kRecoverSlicers[static_cast<int>(mode)], g, 1, p->total_units, st, *p);
-	if (rc || mode != RsMode::CHECK) return rc;
-	return rs_locate(ctx, lay, checks, n_chunks, nb, d_parts, part_stride, static_cast<RsCheckEntry *>(d_map), st);
+	if (rc || !checks) return rc;
+	if (!correct) return rs_locate(ctx, lay, checks, n_chunks, nb, d_parts, part_stride, static_cast<RsCheckEntry *>(d_map), st);
+	return rs_locate(ctx, lay, checks, n_chunks, nb, d_parts, part_stride, reinterpret_cast<RsCheckEntry *>(p->map), st,
+	                 static_cast<RsFixEntry *>(d_map), p->crc_failed, d_new_crc);
 }

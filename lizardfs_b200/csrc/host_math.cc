@@ -721,6 +721,51 @@ int lzgpu_debug_check_slices_rows(const lzgpu_goal *goals, uint32_t n_slices, co
 	return LZGPU_OK;
 }
 
+int lzgpu_plan_correct_slices(const lzgpu_goal *goals, uint32_t n_slices, uint32_t nb, const uint8_t *given, lzgpu_slices_correct_plan *out) {
+	if (!out) return LZGPU_ERR_ARG;
+	*out = lzgpu_slices_correct_plan{};
+	int rc = lzgpu_plan_check_slices(goals, n_slices, nb, given, &out->check);
+	if (rc) return rc;
+	lzd::SliceLayout lay;
+	const char *why = nullptr;
+	lzd::slice_layout(goals, n_slices, lay, &why);
+	auto sv = std::make_unique<lzd::SliceSolve>();
+	auto ck = std::make_unique<lzd::SliceChecks>();
+	const uint32_t tail = nb % lay.L;
+	lzd::slice_solve(lay, given, lay.L, *sv);
+	lzd::slice_checks(lay, given, *sv, *ck);
+	out->correctable = out->tail_correctable = ck->correctable;
+	if (tail) {
+		lzd::slice_solve(lay, given, tail, *sv);
+		lzd::slice_checks(lay, given, *sv, *ck);
+		out->tail_correctable = ck->correctable;
+	}
+	return LZGPU_OK;
+}
+
+int lzgpu_debug_correct_slices_rows(const lzgpu_goal *goals, uint32_t n_slices, const uint8_t *given, uint32_t valid, int part,
+                                    uint32_t *n_blocks, uint8_t *blk_s, uint8_t *rows) {
+	if (!given || !n_blocks || !blk_s || !rows || part < 0 || part >= LZGPU_MAX_PARTS) return LZGPU_ERR_ARG;
+	lzd::SliceLayout lay;
+	const char *why = nullptr;
+	if (lzd::slice_layout(goals, n_slices, lay, &why) != LZGPU_OK || valid == 0 || valid > lay.L) return LZGPU_ERR_ARG;
+	auto sv = std::make_unique<lzd::SliceSolve>();
+	auto ck = std::make_unique<lzd::SliceChecks>();
+	lzd::slice_solve(lay, given, valid, *sv);
+	lzd::slice_checks(lay, given, *sv, *ck);
+	*n_blocks = 0;
+	if (ck->n_checks > lzd::kScMaxChecks || !((ck->correctable >> part) & 1ull)) return LZGPU_ERR_ARG;
+	std::memset(blk_s, 0, 64);
+	std::memset(rows, 0, 64 * 64);
+	for (uint32_t b = 0; b < ck->n_blocks; ++b) {
+		if (ck->blk_part[b] != part) continue;
+		blk_s[*n_blocks] = ck->blk_s[b];
+		std::memcpy(rows + static_cast<size_t>(*n_blocks) * 64, &ck->pinv[static_cast<size_t>(b) * lzd::kScMaxChecks], ck->n_checks);
+		++*n_blocks;
+	}
+	return LZGPU_OK;
+}
+
 int lzgpu_debug_recover_slices_rows(const lzgpu_goal *goals, uint32_t n_slices, const uint8_t *given, uint32_t valid, uint32_t *n_unknowns,
                                     uint32_t *n_equations, uint8_t *unk_pos, uint8_t *eq_slice, uint8_t *eq_row, uint8_t *eq_stripe,
                                     uint8_t *rows, uint64_t *determined) {

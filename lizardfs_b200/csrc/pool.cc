@@ -499,6 +499,32 @@ extern "C" int lzgpu_pool_check_slices(lzgpu_pool *pool, const lzgpu_goal *goals
 	});
 }
 
+// The correction of several slices (lzgpu_correct_slices) over the pool: parts, stored and new CRCs move by slice, the fix entries by
+// first * n_cs; the codes and bad[0..3] merged by pool_merged, as lzgpu_pool_check_slices.
+extern "C" int lzgpu_pool_correct_slices(lzgpu_pool *pool, const lzgpu_goal *goals, uint32_t n_slices, uint32_t n_chunks, uint32_t nb,
+                                          uint8_t *const *parts, const size_t *part_stride, const uint32_t *const *part_crc,
+                                          uint32_t *const *new_crc, lzgpu_slices_fix *fix, int64_t *bad) {
+	if (!pool) return LZGPU_ERR_ARG;
+	lzd::SliceLayout lay;
+	const char *why = nullptr;
+	const bool shaped = parts && part_stride && nb >= 1 && nb <= LZGPU_BLOCKS_IN_CHUNK && lzd::slice_layout(goals, n_slices, lay, &why) == LZGPU_OK;
+	const size_t n_cs = shaped ? (nb + lay.L - 1) / lay.L : 0;
+	return pool_merged(pool, n_chunks, bad, 4, [&](lzgpu_ctx *ctx, uint32_t first, uint32_t count, int64_t *b) {
+		uint8_t *p[LZGPU_MAX_PARTS];
+		const uint32_t *c[LZGPU_MAX_PARTS];
+		uint32_t *nc[LZGPU_MAX_PARTS];
+		for (uint32_t g = 0; shaped && g < lay.n_parts; ++g) {
+			const int i = lay.slice_of(g);
+			const size_t pb = (nb + lay.k[i] - 1) / lay.k[i];
+			p[g] = parts[g] ? parts[g] + first * part_stride[i] : nullptr;
+			c[g] = part_crc && part_crc[g] ? part_crc[g] + first * pb : nullptr;
+			nc[g] = new_crc && new_crc[g] ? new_crc[g] + first * pb : nullptr;
+		}
+		return lzgpu_correct_slices(ctx, goals, n_slices, count, nb, shaped ? p : parts, part_stride, shaped && part_crc ? c : part_crc,
+		                            shaped && new_crc ? nc : new_crc, fix && shaped ? fix + first * n_cs : fix, b);
+	});
+}
+
 // The scrub calls of a context also take device memory of its device; one device's memory cannot go to another device's context,
 // so the pool refuses it before any share runs.  Asked on slot 0's device, so that no other device gets a context.
 static int host_memory_only(lzgpu_pool *pool, const char *name, const void *a, const void *b) {

@@ -30,6 +30,10 @@
 // further copy of a known position: that position) and compares it with the defining block word by word.  Each thread ORs bit h into
 // a 64-bit mask where they differ; the warps OR theirs into a shared word pair, and the stripe's entry is {mask, -1, 0}.
 // locate_slices_kernel then names the suspect part of every entry whose mask is not zero.
+//
+// The CORRECT instantiation (lzgpu_correct_slices) is the CHECK one, writing its entries to a temporary map, plus one 64-bit mask per
+// combined stripe: the parts with a read block that fails its stored CRC (the SALVAGE form's shared failing-read-entry mask, mapped to
+// parts).  locate_slices_kernel names the suspects, and correct_slices_kernel applies the rule and rewrites the suspect's blocks.
 #pragma once
 #include <cstdint>
 
@@ -89,6 +93,8 @@ struct RecoverSlicesParams {
 	uint32_t *image_crc;
 	uint8_t *map;
 	RsSalvage salvage[2];
+	// the CORRECT instantiation only: bit g of crc_failed[c * n_cs + cs] = a read block of part g fails its stored CRC
+	unsigned long long *crc_failed;
 };
 static_assert(sizeof(RecoverSlicesParams) <= 32764, "recover_slices_kernel's parameter block must fit the 32764-byte kernel parameter limit");
 
@@ -100,7 +106,7 @@ struct RsCheckEntry {
 };
 
 // The per-stripe shared words of the SALVAGE instantiation: the failing read entries, then the withheld positions (CHECK: words 0
-// and 1 are the stripe's bad_checks)
+// and 1 are the stripe's bad_checks; CORRECT: the failing read entries, then bad_checks)
 __device__ __forceinline__ uint32_t *rs_salvage_smem() {
 	__shared__ uint32_t words[kRsMaskWords + 2];
 	return words;
@@ -120,7 +126,7 @@ __device__ __forceinline__ uint32_t rs_gf_mul(uint32_t v, uint32_t c) {
 
 template <RsMode MODE>
 __global__ void __launch_bounds__(kRsThreads, 1) recover_slices_kernel(const __grid_constant__ RecoverSlicesParams p) {
-	constexpr bool SALVAGE = MODE == RsMode::SALVAGE, CHECK = MODE == RsMode::CHECK;
+	constexpr bool SALVAGE = MODE == RsMode::SALVAGE, CORRECT = MODE == RsMode::CORRECT, CHECK = MODE == RsMode::CHECK || CORRECT;
 	extern __shared__ __align__(1024) uint8_t smem[];
 	uint32_t *s_tab = reinterpret_cast<uint32_t *>(smem);
 	uint8_t *s_slab = smem + 4096;
@@ -137,7 +143,7 @@ __global__ void __launch_bounds__(kRsThreads, 1) recover_slices_kernel(const __g
 			if (cs >= p.n_cs) break;
 			const RsShape &sh = p.shape[(p.tail && cs == p.n_cs - 1) ? 1 : 0];
 			const uint32_t E = sh.n_eq;
-			[[maybe_unused]] unsigned long long bad = 0;   // CHECK: the checks this thread has seen differ
+			[[maybe_unused]] unsigned long long bad = 0;   // CHECK, CORRECT: the checks this thread has seen differ
 			__syncthreads();   // the previous stripe's streams are merged
 			for (uint32_t i = tid; i < sh.n_state * 32u; i += kRsThreads) s_crc[i] = 0;
 			if constexpr (SALVAGE || CHECK)
@@ -240,12 +246,12 @@ __global__ void __launch_bounds__(kRsThreads, 1) recover_slices_kernel(const __g
 					p.out_crc[en.part][at] = crc;
 				} else if (p.stored[en.part][at] != crc) {
 					atomicMin(p.first_bad, (static_cast<unsigned long long>(c) * 64ull + en.part) * 1024ull + blk);
-					if constexpr (SALVAGE) atomicOr(&rs_salvage_smem()[en.state >> 5], 1u << (en.state & 31));
+					if constexpr (SALVAGE || CORRECT) atomicOr(&rs_salvage_smem()[en.state >> 5], 1u << (en.state & 31));
 				}
 			}
 			if constexpr (CHECK) {
 				// ---------------- the stripe's entry ----------------
-				uint32_t *mask = rs_salvage_smem();
+				uint32_t *mask = rs_salvage_smem() + (CORRECT ? kRsMaskWords : 0);
 				const uint32_t lo = __reduce_or_sync(0xffffffffu, static_cast<uint32_t>(bad)), hi = __reduce_or_sync(0xffffffffu, static_cast<uint32_t>(bad >> 32));
 				if (lane == 0 && (lo | hi)) {
 					atomicOr(&mask[0], lo);
@@ -257,6 +263,17 @@ __global__ void __launch_bounds__(kRsThreads, 1) recover_slices_kernel(const __g
 					en->bad_checks = (static_cast<unsigned long long>(mask[1]) << 32) | mask[0];
 					en->suspect_part = -1;
 					en->zero = 0;
+				}
+				if constexpr (CORRECT) {
+					if (warp == 0) {   // the failing read entries, mapped to parts
+						const uint32_t *fail = rs_salvage_smem();
+						unsigned long long parts = 0;
+						for (uint32_t r = lane; r < sh.n_read; r += 32)
+							if ((fail[r >> 5] >> (r & 31)) & 1u) parts |= 1ull << sh.read[r].part;
+						const uint32_t plo = __reduce_or_sync(0xffffffffu, static_cast<uint32_t>(parts));
+						const uint32_t phi = __reduce_or_sync(0xffffffffu, static_cast<uint32_t>(parts >> 32));
+						if (lane == 0) p.crc_failed[static_cast<unsigned long long>(c) * p.n_cs + cs] = (static_cast<unsigned long long>(phi) << 32) | plo;
+					}
 				}
 			}
 			if constexpr (SALVAGE) {
@@ -312,6 +329,23 @@ struct LocateSlicesParams {
 };
 constexpr int kRslThreads = 128;
 
+// The syndrome words of word w of combined stripe cs of chunk c: S[h * stride] = sum over the shape's given blocks b of H[h][b] y_b
+__device__ __forceinline__ void rs_syndrome_word(const RsLocateShape &sh, const uint8_t *const *parts, const unsigned long long *part_stride,
+                                                 const uint32_t *spc, const uint8_t *part_slice, uint32_t c, uint32_t cs, uint32_t w,
+                                                 uint32_t *S, uint32_t stride) {
+	const uint32_t nc = sh.n_checks;
+	for (uint32_t h = 0; h < nc; ++h) S[h * stride] = 0;
+	for (uint32_t b = 0; b < sh.n_blocks; ++b) {
+		const uint32_t g = sh.blk_part[b], i = part_slice[g];
+		const unsigned long long blk = static_cast<unsigned long long>(cs) * spc[i] + sh.blk_s[b];
+		const uint32_t v = reinterpret_cast<const uint32_t *>(parts[g] + c * part_stride[i] + (blk << 16))[w];
+		for (uint32_t h = 0; h < nc; ++h) {
+			const uint32_t coef = sh.H[h][b];
+			if (coef) S[h * stride] ^= rs_gf_mul(v, coef);
+		}
+	}
+}
+
 // One CTA per bad entry (grid-stride over the map; a clean entry is skipped, its suspect is already -1).  Thread t owns words t,
 // t + 128, ... of the stripe's blocks: it forms the syndrome words S_h = sum_b H[h][b] y_b, and where they are not all zero drops every
 // candidate an annihilator row of which does not map them to zero (a 4-byte word: the test holds for each of its bytes).  The one
@@ -330,16 +364,7 @@ __global__ void __launch_bounds__(kRslThreads) locate_slices_kernel(const __grid
 		__syncthreads();
 		unsigned long long alive = s_alive;
 		for (uint32_t w = tid; w < 65536u / 4u; w += kRslThreads) {
-			for (uint32_t h = 0; h < nc; ++h) S[h][tid] = 0;
-			for (uint32_t b = 0; b < sh.n_blocks; ++b) {
-				const uint32_t g = sh.blk_part[b], i = p.part_slice[g];
-				const unsigned long long blk = static_cast<unsigned long long>(cs) * p.spc[i] + sh.blk_s[b];
-				const uint32_t v = reinterpret_cast<const uint32_t *>(p.parts[g] + c * p.part_stride[i] + (blk << 16))[w];
-				for (uint32_t h = 0; h < nc; ++h) {
-					const uint32_t coef = sh.H[h][b];
-					if (coef) S[h][tid] ^= rs_gf_mul(v, coef);
-				}
-			}
+			rs_syndrome_word(sh, p.parts, p.part_stride, p.spc, p.part_slice, c, cs, w, &S[0][tid], kRslThreads);
 			uint32_t any = 0;
 			for (uint32_t h = 0; h < nc; ++h) any |= S[h][tid];
 			if (!any) continue;
@@ -362,6 +387,121 @@ __global__ void __launch_bounds__(kRslThreads) locate_slices_kernel(const __grid
 			p.map[e].suspect_part = left && !(left & (left - 1)) ? sh.cand_part[__ffsll(static_cast<long long>(left)) - 1] : -1;
 		}
 		__syncthreads();
+	}
+}
+
+// lzgpu_slices_fix as correct_slices_kernel writes it
+struct RsFixEntry {
+	unsigned long long bad_checks;
+	int suspect_part, status;
+	unsigned long long crc_failed, changed;
+};
+
+// correct_slices_kernel's tables per stripe shape (the blocks and checks are the locate pass's RsLocateShape): the correctable parts,
+// each part's run of blocks in the shape's list, and the row of P for block b of the list at rows[prow0 + b] (rows of kRsMaxOut bytes
+// after the annihilators; zero for a part that is not correctable)
+struct RsCorrectShape {
+	unsigned long long correctable;
+	uint32_t prow0;
+	uint8_t blk_first[LZGPU_MAX_PARTS], blk_count[LZGPU_MAX_PARTS];
+};
+struct CorrectSlicesParams {
+	uint8_t *parts[LZGPU_MAX_PARTS];
+	uint32_t *new_crc[LZGPU_MAX_PARTS];   // nullptr: none
+	unsigned long long part_stride[kSlicesMax];
+	uint32_t spc[kSlicesMax], pb[kSlicesMax];
+	uint8_t part_slice[LZGPU_MAX_PARTS];
+	const RsCheckEntry *map;
+	const unsigned long long *crc_failed;
+	RsFixEntry *fix;
+	const RsLocate *loc;
+	const uint32_t *tables;
+	unsigned long long n_entries;
+	uint32_t n_cs, tail, crc_off, zconst, run_mult;   // run_mult: x^(8 * kRscRun) mod P
+	uint32_t tree_mult[5];                            // x^(8 * 2048 * 2^i) mod P, as recover_slices_kernel's
+	RsCorrectShape shape[2];
+};
+constexpr int kRscThreads = 128;
+constexpr uint32_t kRscRun = 65536u / kRscThreads;   // bytes of each block per thread, contiguous
+// dynamic shared memory: the CRC tables, the syndrome words [h][tid], the CRC streams of the suspect's blocks [j][tid]
+constexpr size_t rsc_smem_bytes(uint32_t n_checks, uint32_t n_suspect_blocks) { return 4096 + (n_checks + n_suspect_blocks) * kRscThreads * 4ull; }
+
+// One CTA per entry (grid-stride over the map), every fix entry written.  The rule: CLEAN without bad checks, UNEXPLAINED without a
+// suspect g, CRC_CONFLICT when a part other than g has a failing block, UNDETERMINED when g is not correctable, else CORRECTED.  A
+// corrected entry: thread t owns bytes [kRscRun t, kRscRun (t + 1)) of every block; per word it forms the syndromes (rs_syndrome_word),
+// e_j = sum_h P[j][h] S_h for each block j of g, XORs e_j into the block in place and folds the word as written into block j's CRC
+// stream.  The four streams of a lane's 2048 bytes are chained, then merged by the tree of crc_blocks_kernel.
+__global__ void __launch_bounds__(kRscThreads) correct_slices_kernel(const __grid_constant__ CorrectSlicesParams p) {
+	extern __shared__ __align__(16) uint32_t rsc_smem[];
+	uint32_t *s_tab = rsc_smem, *S = rsc_smem + 1024;
+	__shared__ uint32_t s_changed[2];
+	const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+	for (uint32_t i = tid; i < 1024; i += kRscThreads) s_tab[i] = p.tables[i];
+	const uint8_t *rows = reinterpret_cast<const uint8_t *>(p.loc + 1);
+	__syncthreads();
+	for (unsigned long long e = blockIdx.x; e < p.n_entries; e += gridDim.x) {
+		const RsCheckEntry en = p.map[e];
+		const unsigned long long failed = p.crc_failed[e];
+		const uint32_t c = static_cast<uint32_t>(e / p.n_cs), cs = static_cast<uint32_t>(e % p.n_cs), t = (p.tail && cs == p.n_cs - 1) ? 1 : 0;
+		const RsLocateShape &sh = p.loc->shape[t];
+		const RsCorrectShape &cor = p.shape[t];
+		const int g = en.suspect_part;
+		const int status = !en.bad_checks ? LZGPU_FIX_CLEAN
+		                   : g < 0 ? LZGPU_FIX_UNEXPLAINED
+		                   : (failed & ~(1ull << g)) ? LZGPU_FIX_CRC_CONFLICT
+		                   : !((cor.correctable >> g) & 1ull) ? LZGPU_FIX_UNDETERMINED : LZGPU_FIX_CORRECTED;
+		if (status != LZGPU_FIX_CORRECTED) {
+			if (tid == 0) p.fix[e] = RsFixEntry{en.bad_checks, g, status, failed, 0ull};
+			continue;
+		}
+		const uint32_t nc = sh.n_checks, b0 = cor.blk_first[g], nbk = cor.blk_count[g], i = p.part_slice[g];
+		uint32_t *s_crc = S + nc * kRscThreads;
+		uint8_t *base = p.parts[g] + c * p.part_stride[i] + ((static_cast<unsigned long long>(cs) * p.spc[i]) << 16);
+		if (tid < 2) s_changed[tid] = 0;
+		for (uint32_t j = 0; j < nbk; ++j) s_crc[j * kRscThreads + tid] = 0;
+		unsigned long long changed = 0;
+		for (uint32_t w = tid * (kRscRun / 4); w < (tid + 1) * (kRscRun / 4); ++w) {
+			rs_syndrome_word(sh, reinterpret_cast<const uint8_t *const *>(p.parts), p.part_stride, p.spc, p.part_slice, c, cs, w, S + tid,
+			                 kRscThreads);
+			for (uint32_t j = 0; j < nbk; ++j) {
+				const uint8_t *row = rows + static_cast<size_t>(cor.prow0 + b0 + j) * kRsMaxOut;
+				uint32_t err = 0;
+				for (uint32_t h = 0; h < nc; ++h) err ^= rs_gf_mul(S[h * kRscThreads + tid], row[h]);
+				const uint32_t s = sh.blk_s[b0 + j];
+				uint32_t *word = reinterpret_cast<uint32_t *>(base + (static_cast<unsigned long long>(s) << 16)) + w;
+				uint32_t y = *word;
+				if (err) {
+					y ^= err;
+					*word = y;
+					changed |= 1ull << s;
+				}
+				if (!p.crc_off) s_crc[j * kRscThreads + tid] = crc_step_word(s_crc[j * kRscThreads + tid], y, s_tab);
+			}
+		}
+		const uint32_t lo = __reduce_or_sync(0xffffffffu, static_cast<uint32_t>(changed)), hi = __reduce_or_sync(0xffffffffu, static_cast<uint32_t>(changed >> 32));
+		__syncthreads();   // s_changed cleared, every stream complete
+		if (lane == 0 && (lo | hi)) {
+			atomicOr(&s_changed[0], lo);
+			atomicOr(&s_changed[1], hi);
+		}
+		// ---------------- each block's CRC: lane l chains the runs of threads 4l .. 4l + 3, then the tree ----------------
+		uint32_t *out = p.new_crc[g];
+		for (uint32_t j = warp; out && j < nbk; j += kRscThreads / 32) {
+			const uint32_t *sc = s_crc + j * kRscThreads + lane * 4;
+			uint32_t st = sc[0];
+			for (int r = 1; r < 4; ++r) st = crc_mulmod(st, p.run_mult) ^ sc[r];
+#pragma unroll
+			for (int l = 0; l < 5; ++l) {
+				const uint32_t right = __shfl_down_sync(0xffffffffu, st, 1u << l);
+				st = crc_mulmod(st, p.tree_mult[l]) ^ right;
+			}
+			if (lane == 0)
+				out[static_cast<unsigned long long>(c) * p.pb[i] + static_cast<unsigned long long>(cs) * p.spc[i] + sh.blk_s[b0 + j]] =
+				    p.crc_off ? LZGPU_FAKE_CRC : (st ^ p.zconst);
+		}
+		__syncthreads();
+		if (tid == 0) p.fix[e] = RsFixEntry{en.bad_checks, g, status, failed, (static_cast<unsigned long long>(s_changed[1]) << 32) | s_changed[0]};
+		__syncthreads();   // S, the streams and s_changed are free for the next entry
 	}
 }
 

@@ -13,6 +13,10 @@
 //
 // A part g explains a syndrome vector S when S lies in the span of the columns of g's blocks in the check matrix H.  The locate pass
 // tests that with an annihilator per part: rows spanning {w : w H_g = 0}, so S is in the span exactly when every row maps it to 0.
+//
+// lzgpu_correct_slices corrects a named part g when its columns H_g have full rank (g is `correctable`): then H_g e = S has exactly one
+// solution, the error of g's blocks, and e = P_g S for any left inverse P_g (P_g H_g = I).  P_g is the top of the row operations that
+// bring H_g to [I; 0] (Gauss-Jordan of [H_g | I]); the rank test is the same elimination.
 #pragma once
 #include <cstdint>
 #include <cstring>
@@ -28,6 +32,8 @@ struct SliceChecks {
 	uint32_t valid = 0, n_blocks = 0, rank = 0, n_checks = 0;   // n_checks may exceed kScMaxChecks: then only the counts are filled
 	uint64_t parts = 0;                      // given parts with a block in this shape
 	uint64_t checked = 0, locatable = 0;     // lzgpu_slices_check_plan's masks (locatable only when asked for)
+	uint64_t correctable = 0;                // given parts with a block in the shape whose columns of H have full rank
+	std::vector<uint8_t> pinv;               // [b * kScMaxChecks + h]: block b of a correctable part, coefficient of S_h in its error
 	std::vector<uint8_t> blk_part, blk_s;    // given block b: flat part, stripe of the part's slice in the combined stripe
 	std::vector<uint32_t> def;               // check h: its defining block
 	std::vector<uint8_t> H;                  // [h * n_blocks + b]: coefficient of given block b in check h
@@ -213,6 +219,41 @@ inline void slice_checks(const SliceLayout &lay, const uint8_t *given, const Sli
 			o.ann.insert(o.ann.end(), w, w + kScMaxChecks);
 			++o.ann_first[g + 1];
 		}
+	}
+
+	// correctable, the left inverses: Gauss-Jordan of [H_g | I] (nc rows), the first c rows of the right half are P_g
+	o.pinv.assign(static_cast<size_t>(n) * kScMaxChecks, 0);
+	for (uint32_t g = 0; g < LZGPU_MAX_PARTS; ++g) {
+		if (!((o.parts >> g) & 1ull)) continue;
+		uint32_t b0 = 0;
+		while (o.blk_part[b0] != g) ++b0;
+		uint32_t c = 0;
+		while (b0 + c < n && o.blk_part[b0 + c] == g) ++c;
+		if (c > nc) continue;
+		const uint32_t W = c + nc;
+		std::vector<uint8_t> M(static_cast<size_t>(nc) * W, 0);
+		for (uint32_t h = 0; h < nc; ++h) {
+			for (uint32_t j = 0; j < c; ++j) M[h * W + j] = o.H[h * n + b0 + j];
+			M[h * W + c + h] = 1;
+		}
+		bool full = true;
+		for (uint32_t j = 0; j < c && full; ++j) {
+			uint32_t pr = j;
+			while (pr < nc && !M[pr * W + j]) ++pr;
+			if (pr == nc) { full = false; break; }
+			if (pr != j)
+				for (uint32_t x = 0; x < W; ++x) std::swap(M[pr * W + x], M[j * W + x]);
+			const uint8_t inv = lz::gf_inv_host(M[j * W + j]);
+			for (uint32_t x = 0; x < W; ++x) M[j * W + x] = lz::gf_mul_host(M[j * W + x], inv);
+			for (uint32_t h = 0; h < nc; ++h) {
+				const uint8_t f = M[h * W + j];
+				if (h == j || !f) continue;
+				for (uint32_t x = 0; x < W; ++x) M[h * W + x] ^= lz::gf_mul_host(f, M[j * W + x]);
+			}
+		}
+		if (!full) continue;
+		o.correctable |= 1ull << g;
+		for (uint32_t j = 0; j < c; ++j) std::memcpy(&o.pinv[static_cast<size_t>(b0 + j) * kScMaxChecks], &M[j * W + c], nc);
 	}
 	if (!locatable) return;
 	for (uint32_t g = 0; g < LZGPU_MAX_PARTS; ++g) {

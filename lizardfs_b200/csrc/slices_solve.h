@@ -197,8 +197,9 @@ inline uint64_t slice_needed(const SliceLayout &lay, const uint8_t *want, bool i
 // part that is not given wanted, with its CRCs, and the image), so that it does not depend on `want`: one 256-thread CTA per SM, a
 // unit of G combined stripes, shared memory = the CRC tables + one 1 KiB slab per staged block + 128 bytes per CRC stream.  SALVAGE:
 // the largest salvage request instead (lzgpu_salvage_slices: nothing wanted, every given part verified, the image with its CRCs).
-// CHECK (lzgpu_check_slices): every given part verified, nothing written, a slab per check's defining block (slice_check_count).
-enum class RsMode : int { RECOVER, SALVAGE, CHECK };
+// CHECK (lzgpu_check_slices): every given part verified, nothing written, a slab per check's defining block (slice_check_count);
+// CORRECT (lzgpu_correct_slices) stages what CHECK stages.
+enum class RsMode : int { RECOVER, SALVAGE, CHECK, CORRECT };
 constexpr uint32_t kRsThreadsPerCta = 256, kRsEntryCap = 192, kRsOutCap = 64;
 constexpr size_t kRsSmemCap = 220 * 1024;
 struct RsGeometry {
@@ -221,7 +222,7 @@ inline uint32_t slice_check_count(const SliceLayout &lay, const uint8_t *given, 
 }
 
 inline RsGeometry rs_geometry(const SliceLayout &lay, const uint8_t *given, const SliceSolve *shapes, int n_shapes, RsMode mode = RsMode::RECOVER) {
-	const bool salvage = mode == RsMode::SALVAGE, check = mode == RsMode::CHECK;
+	const bool salvage = mode == RsMode::SALVAGE, check = mode == RsMode::CHECK || mode == RsMode::CORRECT;
 	RsGeometry g;
 	g.G = lay.L >= 8 ? 1 : 8 / lay.L;
 	g.threads = kRsThreadsPerCta;

@@ -238,6 +238,34 @@ def _check_slices(fn, h, goals, nb, parts, part_crc):
     return out
 
 
+SLICES_FIX_DTYPE = np.dtype([("bad_checks", np.uint64), ("suspect_part", np.int32), ("status", np.int32), ("crc_failed", np.uint64),
+                             ("changed", np.uint64)])
+
+
+def _correct_slices(fn, h, goals, nb, parts, part_crc, with_crc):
+    pbs = [-(-nb // g.k) for g in goals]
+    slice_of = [i for i, g in enumerate(goals) for _ in range(1 if g.is_std else g.k + g.m)]
+    assert len(parts) == len(slice_of)
+    for p in parts:
+        if p is not None and not (isinstance(p, np.ndarray) and p.dtype == np.uint8 and p.flags.c_contiguous and p.flags.writeable):
+            raise ValueError("correct_slices corrects the parts in place: each must be a writeable C-contiguous uint8 array")
+    arrs = [None if p is None else p.reshape(-1, pbs[slice_of[j]] * BLOCK_SIZE) for j, p in enumerate(parts)]
+    n = next((a.shape[0] for a in arrs if a is not None), 0)
+    crcs = None if part_crc is None else _ptr_array([None if c is None else np.ascontiguousarray(c, dtype=np.uint32) for c in part_crc])
+    new_crc = [np.zeros((n, pbs[slice_of[j]]), dtype=np.uint32) if (a is not None and with_crc) else None for j, a in enumerate(arrs)]
+    L = 1
+    for g in goals:
+        if not g.is_std:
+            L = L * g.k // math.gcd(L, g.k)
+    fix = np.zeros((n, -(-nb // L)), dtype=SLICES_FIX_DTYPE)
+    strides = (C.c_size_t * len(goals))(*[pb * BLOCK_SIZE for pb in pbs])
+    bad = (C.c_int64 * 4)(-1, -1, -1, -1)
+    rc = fn(h, _goal_array(goals), len(goals), n, nb, _ptr_array(arrs), strides, crcs, _ptr_array(new_crc) if with_crc else None, _p(fix),
+            bad)
+    _check_crc(rc, _name(fn), bad, fix=fix, new_crc=new_crc if with_crc else None)
+    return fix, (new_crc if with_crc else None)
+
+
 def _part_batch(fn, h, goal, nb, parts, part_crc, result, attr, in_place=False):
     # the host-pointer check, map and correction: result(n_chunks, pb) makes the array the call fills, which is returned, and
     # attached to a ChunkCrcError as `attr`
@@ -495,6 +523,11 @@ class Pool:
         """Engine.check_slices over every device of the pool (lzgpu_pool_check_slices): the same arguments, map and errors for the
         whole batch; ChunkCrcError.where = (chunk in the batch, slice, part, block)"""
         return _check_slices(self.lib.lzgpu_pool_check_slices, self.h, goals, nb, parts, part_crc)
+
+    def correct_slices(self, goals, nb, parts, part_crc=None, with_crc=True):
+        """Engine.correct_slices over every device of the pool (lzgpu_pool_correct_slices): the same arguments, results and errors
+        as on one context."""
+        return _correct_slices(self.lib.lzgpu_pool_correct_slices, self.h, goals, nb, parts, part_crc, with_crc)
 
     def crc_blocks(self, data, block_len=BLOCK_SIZE):
         data = _u8(data).reshape(-1, block_len)
@@ -775,6 +808,53 @@ class Engine:
         rc = self.lib.lzgpu_check_slices_dev(self.h, _goal_array(goals), ns, n_chunks, nb, _dev_ptrs(d_parts, n), (C.c_size_t * ns)(*part_stride),
                                              _dev_ptrs(d_part_crc, n), d_map, bad, stream)
         _check_crc(rc, "check_slices_dev", bad)
+
+    SLICES_FIX_DTYPE = SLICES_FIX_DTYPE
+
+    def correct_slices(self, goals, nb, parts, part_crc=None, with_crc=True):
+        """Check the given parts of every slice and correct in place each combined stripe that the check blames on one part
+        (lzgpu_correct_slices).  goals, parts, part_crc as in check_slices, but every given part must be a writeable C-contiguous uint8
+        array: the suspect's blocks are rewritten in it.  Returns (fix, new_crc): fix a structured array [n_chunks, ceil(nb / L)] of
+        SLICES_FIX_DTYPE (bad_checks and suspect_part as check_slices had them before the call; status = _lib.FIX_CLEAN / _CORRECTED /
+        _UNEXPLAINED / _CRC_CONFLICT / _UNDETERMINED; crc_failed, bit g: a block of flat part g fails its stored CRC; changed, bit s:
+        the suspect's block s changed), whether or not an entry is left bad; new_crc[g] a [n_chunks, pb_g] uint32 array per given part
+        (None without with_crc) holding the new CRC at every rewritten block and 0 elsewhere.  Raises ChunkCrcError (.where = chunk,
+        slice, part, block) on a stored-CRC mismatch, with .fix and .new_crc complete and the corrections the rule allows made."""
+        return _correct_slices(self.lib.lzgpu_correct_slices, self.h, goals, nb, parts, part_crc, with_crc)
+
+    def correct_slices_dev(self, goals, n_chunks, nb, d_parts, part_stride, d_part_crc, d_new_crc, d_fix, stream=None):
+        """lzgpu_correct_slices_dev: d_parts / d_part_crc / d_new_crc are lists over the flat parts (device pointers as ints, 0 or
+        None = absent; d_new_crc may be None), part_stride one entry per slice; n_chunks * ceil(nb / L) entries of 32 bytes go to d_fix
+        (8-byte aligned device memory).  Raises ChunkCrcError (.where = chunk, slice, part, block); the entries are then still complete."""
+        ns, n = len(goals), sum(1 if g.is_std else g.k + g.m for g in goals)
+        bad = (C.c_int64 * 4)(-1, -1, -1, -1)
+        rc = self.lib.lzgpu_correct_slices_dev(self.h, _goal_array(goals), ns, n_chunks, nb, _dev_ptrs(d_parts, n),
+                                               (C.c_size_t * ns)(*part_stride), _dev_ptrs(d_part_crc, n), _dev_ptrs(d_new_crc, n), d_fix, bad,
+                                               stream)
+        _check_crc(rc, "correct_slices_dev", bad)
+
+    @staticmethod
+    def plan_correct_slices(goals, nb, given):
+        """what correct_slices corrects with the given flat parts (pure host logic, csrc/slices_check.h; no GPU needed): the dict of
+        plan_check_slices, with correctable and tail_correctable (bit g: flat part g is corrected when named)"""
+        out = _lib.LzSlicesCorrectPlan()
+        g = np.asarray(given, dtype=np.uint8)
+        _check(_lib.load().lzgpu_plan_correct_slices(_goal_array(goals), len(goals), nb, _p(g), C.byref(out)), "plan_correct_slices")
+        d = {f: getattr(out.check, f) for f, _ in _lib.LzSlicesCheckPlan._fields_}
+        d.update(correctable=out.correctable, tail_correctable=out.tail_correctable)
+        return d
+
+    @staticmethod
+    def debug_correct_slices_rows(goals, given, valid, part):
+        """the left inverse P_g of one stripe shape (csrc/slices_check.h; no GPU needed): (blk_s [n], rows [n, 64]), rows[j, h] the
+        coefficient of syndrome S_h in the error of the part's block blk_s[j].  Raises LzGpuError(ERR_ARG) when the part is not
+        correctable there."""
+        n = C.c_uint32()
+        blk_s, rows = np.zeros(64, dtype=np.uint8), np.zeros((64, 64), dtype=np.uint8)
+        g = np.asarray(given, dtype=np.uint8)
+        _check(_lib.load().lzgpu_debug_correct_slices_rows(_goal_array(goals), len(goals), _p(g), valid, part, C.byref(n), _p(blk_s),
+                                                            _p(rows)), "debug_correct_slices_rows")
+        return blk_s[:n.value].copy(), rows[:n.value].copy()
 
     @staticmethod
     def plan_check_slices(goals, nb, given):

@@ -152,6 +152,14 @@ try:
     raise AssertionError("the corrupt block passed")
 except L.ChunkCrcError as e:
     assert (e.map == 3).any()
+# the correction of several slices (recover_slices_kernel CORRECT form, locate, correct_slices_kernel): xor2 + xor3 with every part
+# given, a stale byte in xor3's parity in the tail combined stripe, corrected back with its new CRC
+full = [p.copy() for p in sparts]
+full[6][0, 4 * 65536 + 9] ^= 0x41
+fcrc = [eng.crc_blocks(p.reshape(-1)).reshape(2, -1) for p in full]
+fix, ncrc = eng.correct_slices(goals, nblk, full, fcrc)
+assert (fix["status"] == 1).sum() == 1 and all((a == b).all() for a, b in zip(full, sparts))
+assert ncrc[6][0, 4] == eng.crc_blocks(sparts[6][0, 4 * 65536:5 * 65536])[0]
 print("sanitizer case OK")
 PY
 for tool in ${TOOLS:-memcheck racecheck synccheck}; do
