@@ -2161,38 +2161,25 @@ extern "C" int lzgpu_convert_chunks(lzgpu_ctx *ctx, const lzgpu_goal *src, const
 // ------------------------------------------------------------------------------------------------
 // recovery from the parts of every slice of a goal together (lzgpu_recover_slices*)
 // ------------------------------------------------------------------------------------------------
-// What the argument check derives for the enqueue: the flat part layout, the solve of both stripe shapes and the launch geometry.
-// salvage: the call is lzgpu_salvage_slices*; check: lzgpu_check_slices*, with the checks of both shapes; correct (with check):
-// lzgpu_correct_slices*, the map being the fix entries (set by the caller before the check)
-struct RecoverSlicesCall {
-	lzd::SliceLayout lay;
-	lzd::SliceSolve shapes[2];   // a full combined stripe, the chunk's last one when L does not divide nb
-	lzd::SliceChecks checks[2];
-	lzd::RsGeometry geo;
-	uint32_t pb[kSlicesMax] = {0};
-	bool salvage = false, check = false, correct = false;
-	lzd::RsMode mode() const {
-		return correct ? lzd::RsMode::CORRECT : check ? lzd::RsMode::CHECK : salvage ? lzd::RsMode::SALVAGE : lzd::RsMode::RECOVER;
-	}
-	size_t entry_bytes() const { return correct ? sizeof(lzgpu_slices_fix) : sizeof(lzgpu_slices_check); }
-};
+static const char *const kSlicesFn[] = {"recover_slices", "salvage_slices", "check_slices", "correct_slices"};   // by lzd::RsMode
 
-// lzgpu_salvage_slices* and lzgpu_check_slices* want no part
+// the salvage, check and correction want no part
 static const uint8_t kWantNone[LZGPU_MAX_PARTS] = {0};
 
-// The arguments of both forms, checked before anything is enqueued and whatever n_chunks is.  dev: the device form's alignment rules
-// (16-byte buffers and strides, 4-byte CRC arrays).  LZGPU_ERR_TOO_FEW_PARTS when a block the call must write is not determined; in the
-// salvage form (c.salvage; want = kWantNone, chunk_out the image) when no part is given, and the image and the map are required.  In
-// the check form (c.check; want = kWantNone, no image, map required) when no part is given or no shape of the batch has a check; more
-// than 64 checks in a shape is LZGPU_ERR_ARG.  The correction form (c.correct) is the check form with the fix entries as the map.
-static int recover_slices_args(const lzgpu_ctx *ctx, const lzgpu_goal *goals, uint32_t n_slices, uint32_t nb, const void *const *parts,
-                               const size_t *part_stride, const void *const *part_crc, const uint8_t *want, const void *const *out,
-                               const size_t *out_stride, const void *const *out_crc, const void *chunk_out, size_t chunk_out_stride, bool dev,
-                               RecoverSlicesCall &c, const void *image_crc = nullptr, const void *map = nullptr) {
-	if (!ctx || !parts || !part_stride || !want) return LZGPU_ERR_ARG;
-	const char *fn = c.correct ? "correct_slices" : c.check ? "check_slices" : c.salvage ? "salvage_slices" : "recover_slices";
-	if (c.salvage && (!chunk_out || !map)) { lz_set_error("salvage_slices: the image and the map are required"); return LZGPU_ERR_ARG; }
-	if (c.check && !map) { lz_set_error("%s: the %s is required", fn, c.correct ? "fix" : "map"); return LZGPU_ERR_ARG; }
+// The arguments of the four calls (c.mode: the recovery, salvage, check or correction) in the buffers b, checked before anything is
+// enqueued and whatever n_chunks is; they fill the rest of c.  dev: the device form's alignment rules (16-byte buffers and strides,
+// 4-byte CRC arrays, an 8-byte aligned map).  LZGPU_ERR_TOO_FEW_PARTS when a block the recovery must write is not determined (the
+// salvage writes what is determined, holes are not refused), when no part is given to the other three, and when no shape of the
+// batch has a check for the check and correction.  The salvage requires the image and the map, the check the map, the correction
+// the fix entries (b.map); more than 64 checks in a shape is LZGPU_ERR_ARG.
+static int recover_slices_args(const lzgpu_ctx *ctx, const lzgpu_goal *goals, uint32_t n_slices, uint32_t nb, const SlicesBufs &b, bool dev,
+                               RecoverSlicesCall &c) {
+	if (!ctx || !b.parts || !b.part_stride || !b.want) return LZGPU_ERR_ARG;
+	const bool salvage = c.mode == lzd::RsMode::SALVAGE, correct = c.mode == lzd::RsMode::CORRECT;
+	const bool check = correct || c.mode == lzd::RsMode::CHECK;
+	const char *fn = kSlicesFn[static_cast<int>(c.mode)];
+	if (salvage && (!b.image || !b.map)) { lz_set_error("salvage_slices: the image and the map are required"); return LZGPU_ERR_ARG; }
+	if (check && !b.map) { lz_set_error("%s: the %s is required", fn, correct ? "fix" : "map"); return LZGPU_ERR_ARG; }
 	const char *why = nullptr;
 	if (lzd::slice_layout(goals, n_slices, c.lay, &why)) { lz_set_error("%s: %s", fn, why); return LZGPU_ERR_ARG; }
 	if (nb == 0 || nb > LZGPU_BLOCKS_IN_CHUNK) { lz_set_error("nb out of range"); return LZGPU_ERR_ARG; }
@@ -2203,85 +2190,82 @@ static int recover_slices_args(const lzgpu_ctx *ctx, const lzgpu_goal *goals, ui
 		c.pb[i] = (nb + lay.k[i] - 1) / lay.k[i];
 		const size_t bytes = static_cast<size_t>(c.pb[i]) * B;
 		for (uint32_t g = lay.base[i]; g < lay.base[i] + lay.k[i] + lay.m[i]; ++g) {
-			given[g] = parts[g] != nullptr;
-			if (given[g] && (part_stride[i] < bytes || (dev && (part_stride[i] & 15)))) {
+			given[g] = b.parts[g] != nullptr;
+			if (given[g] && (b.part_stride[i] < bytes || (dev && (b.part_stride[i] & 15)))) {
 				lz_set_error("%s: part_stride[%u] too small or not a multiple of 16", fn, i);
 				return LZGPU_ERR_ARG;
 			}
-			if (!want[g]) continue;
+			if (!b.want[g]) continue;
 			if (given[g]) { lz_set_error("recover_slices: part %u is given and wanted", g); return LZGPU_ERR_ARG; }
-			if (!out || !out[g] || !out_stride) { lz_set_error("recover_slices: wanted part %u has no output buffer", g); return LZGPU_ERR_ARG; }
-			if (out_stride[i] < bytes || (dev && (out_stride[i] & 15))) {
+			if (!b.out || !b.out[g] || !b.out_stride) { lz_set_error("recover_slices: wanted part %u has no output buffer", g); return LZGPU_ERR_ARG; }
+			if (b.out_stride[i] < bytes || (dev && (b.out_stride[i] & 15))) {
 				lz_set_error("recover_slices: out_stride[%u] too small or not a multiple of 16", i);
 				return LZGPU_ERR_ARG;
 			}
 		}
 	}
-	if (chunk_out && (chunk_out_stride < static_cast<size_t>(nb) * B || (dev && (chunk_out_stride & 15)))) {
-		lz_set_error(c.salvage ? "salvage_slices: image_stride must cover nb blocks (and be a multiple of 16)"
-		                       : "recover_slices: chunk_out_stride must cover nb blocks (and be a multiple of 16)");
+	if (b.image && (b.image_stride < static_cast<size_t>(nb) * B || (dev && (b.image_stride & 15)))) {
+		lz_set_error(salvage ? "salvage_slices: image_stride must cover nb blocks (and be a multiple of 16)"
+		                     : "recover_slices: chunk_out_stride must cover nb blocks (and be a multiple of 16)");
 		return LZGPU_ERR_ARG;
 	}
+	const int n = static_cast<int>(lay.n_parts);
+	int rc;
 	if (dev) {
-		const int n = static_cast<int>(lay.n_parts);
-		int rc;
-		if ((rc = check_part_ptrs(fn, "parts", parts, n, 16)) || (rc = check_part_ptrs(fn, "out", out, n, 16)) ||
-		    (rc = check_part_ptrs(fn, "part_crc", part_crc, n, 4)) || (rc = check_part_ptrs(fn, "out_crc", out_crc, n, 4)))
+		if ((rc = check_part_ptrs(fn, "parts", b.parts, n, 16)) || (rc = check_part_ptrs(fn, "out", b.out, n, 16)) ||
+		    (rc = check_part_ptrs(fn, "part_crc", b.part_crc, n, 4)) || (rc = check_part_ptrs(fn, "out_crc", b.out_crc, n, 4)))
 			return rc;
-		if (reinterpret_cast<uintptr_t>(chunk_out) & 15) { lz_set_error("%s: %s is not 16-byte aligned", fn, c.salvage ? "image" : "chunk_out"); return LZGPU_ERR_ARG; }
-		if (reinterpret_cast<uintptr_t>(image_crc) & 3) { lz_set_error("salvage_slices: image_crc is not 4-byte aligned"); return LZGPU_ERR_ARG; }
+		if (reinterpret_cast<uintptr_t>(b.image) & 15) { lz_set_error("%s: %s is not 16-byte aligned", fn, salvage ? "image" : "chunk_out"); return LZGPU_ERR_ARG; }
+		if (reinterpret_cast<uintptr_t>(b.image_crc) & 3) { lz_set_error("salvage_slices: image_crc is not 4-byte aligned"); return LZGPU_ERR_ARG; }
 	}
-	if (c.salvage || c.check) {
+	if (c.mode != lzd::RsMode::RECOVER) {
 		bool any = false;
-		for (uint32_t g = 0; g < lay.n_parts; ++g) any |= parts[g] != nullptr;
+		for (uint32_t g = 0; g < lay.n_parts; ++g) any |= b.parts[g] != nullptr;
 		if (!any) { lz_set_error("%s: no part is given", fn); return LZGPU_ERR_TOO_FEW_PARTS; }
 	}
 	const uint32_t tail = nb % lay.L;
-	lzd::slice_solve(lay, given, lay.L, c.shapes[0]);
-	if (tail) lzd::slice_solve(lay, given, tail, c.shapes[1]);
-	for (int t = 0; t < 2 && c.check; ++t) {
-		if (t == 0 ? nb < lay.L : tail == 0) continue;
-		lzd::slice_checks(lay, given, c.shapes[t], c.checks[t]);
+	lzd::slice_shapes(lay, given, nb, c.mode, c);
+	for (int t = 0; t < 2 && check; ++t) {
+		if (t == 0 ? nb < lay.L : tail == 0) continue;   // a shape no chunk of the call has
 		if (c.checks[t].n_checks > lzd::kScMaxChecks) {
 			lz_set_error("%s: the %s combined stripe has %u checks, more than 64", fn, t ? "last" : "full", c.checks[t].n_checks);
 			return LZGPU_ERR_ARG;
 		}
 	}
-	if (c.check && (nb < lay.L || !c.checks[0].n_checks) && (!tail || !c.checks[1].n_checks)) {
+	if (check && (nb < lay.L || !c.checks[0].n_checks) && (!tail || !c.checks[1].n_checks)) {
 		lz_set_error("%s: no combined stripe of the batch has a check", fn);
 		return LZGPU_ERR_TOO_FEW_PARTS;
 	}
-	for (int t = 0; t < 2 && !c.salvage && !c.check; ++t) {   // salvage writes what is determined, holes are not refused
-		if (t == 0 ? nb < lay.L : tail == 0) continue;   // a shape no chunk of the call has
+	for (int t = 0; t < 2 && c.mode == lzd::RsMode::RECOVER; ++t) {
+		if (t == 0 ? nb < lay.L : tail == 0) continue;
 		const lzd::SliceSolve &sv = c.shapes[t];
-		const uint64_t lost = lzd::slice_needed(lay, want, chunk_out != nullptr, sv.valid) & ~sv.determined;
+		const uint64_t lost = lzd::slice_needed(lay, b.want, b.image != nullptr, sv.valid) & ~sv.determined;
 		if (lost) {
 			lz_set_error("recover_slices: positions %#llx of the %s combined stripe are not determined by the given parts",
 			             static_cast<unsigned long long>(lost), t ? "last" : "full");
 			return LZGPU_ERR_TOO_FEW_PARTS;
 		}
 	}
-	const lzd::SliceSolve used[2] = {nb >= lay.L ? c.shapes[0] : c.shapes[1], tail ? c.shapes[1] : c.shapes[0]};
-	c.geo = lzd::rs_geometry(lay, given, used, 2, c.mode());
 	if (!c.geo.ok) {
 		lz_set_error("%s: a combined stripe has more blocks than the kernel stages (%u slots, %u CRC streams)", fn, c.geo.slots, c.geo.states);
 		return LZGPU_ERR_ARG;
 	}
+	if (correct && (rc = check_part_ptrs(fn, "new_crc", b.new_crc, n, 4))) return rc;
+	if (dev && check && (reinterpret_cast<uintptr_t>(b.map) & 7)) { lz_set_error("%s: %s is not 8-byte aligned", fn, correct ? "fix" : "map"); return LZGPU_ERR_ARG; }
 	return LZGPU_OK;
 }
 
-// DESIGN.md §4.8: read the given parts (+ their stored CRCs), write the wanted parts (+ their CRCs) and the image (+ the salvage form's
-// image CRCs and map)
-static uint64_t recover_slices_alg_bytes(const RecoverSlicesCall &c, uint32_t n_chunks, uint32_t nb, const void *const *parts, bool crcs,
-                                         const uint8_t *want, bool out_crcs, bool image, bool image_crcs = false) {
+// DESIGN.md §4.8: read the given parts (+ their stored CRCs), write the wanted parts (+ their CRCs) and the image (+ the salvage's
+// image CRCs and map, or the check's or correction's entries)
+static uint64_t recover_slices_alg_bytes(const RecoverSlicesCall &c, uint32_t n_chunks, uint32_t nb, const SlicesBufs &d) {
 	const uint64_t B = LZGPU_BLOCK_SIZE;
-	uint64_t per_chunk = image ? static_cast<uint64_t>(nb) * B : 0;
-	if (c.salvage) per_chunk += static_cast<uint64_t>(nb) * (image_crcs ? 5 : 1);
-	if (c.check) per_chunk += (nb + c.lay.L - 1) / c.lay.L * c.entry_bytes();
+	uint64_t per_chunk = d.image ? static_cast<uint64_t>(nb) * B : 0;
+	if (c.mode == lzd::RsMode::SALVAGE) per_chunk += static_cast<uint64_t>(nb) * (d.image_crc ? 5 : 1);
+	if (c.mode == lzd::RsMode::CHECK || c.mode == lzd::RsMode::CORRECT) per_chunk += (nb + c.lay.L - 1) / c.lay.L * c.entry_bytes();
 	for (uint32_t i = 0; i < c.lay.n_slices; ++i)
 		for (uint32_t g = c.lay.base[i]; g < c.lay.base[i] + c.lay.k[i] + c.lay.m[i]; ++g) {
-			if (parts[g]) per_chunk += c.pb[i] * (B + (crcs ? 4 : 0));
-			if (want[g]) per_chunk += c.pb[i] * (B + (out_crcs ? 4 : 0));
+			if (d.parts[g]) per_chunk += c.pb[i] * (B + (d.part_crc ? 4 : 0));
+			if (d.want[g]) per_chunk += c.pb[i] * (B + (d.out_crc ? 4 : 0));
 		}
 	return n_chunks * per_chunk;
 }
@@ -2296,37 +2280,33 @@ static void recover_slices_bad(const lzd::SliceLayout &lay, const int64_t *b3, i
 	bad[3] = b3[2];
 }
 
-// one launch; *tk is armed when a given part has stored CRCs (the kernel compares them with the constant while CRCs are disabled)
-static int recover_slices_enqueue(lzgpu_ctx *ctx, const RecoverSlicesCall &c, uint32_t n_chunks, uint32_t nb, const void *const *d_parts,
-                                  const size_t *part_stride, const void *const *d_part_crc, const uint8_t *want, void *const *d_out,
-                                  const size_t *out_stride, void *const *d_out_crc, void *d_chunk_out, size_t chunk_out_stride, cudaStream_t st,
-                                  VerifyTicket *tk, void *d_image_crc = nullptr, void *d_map = nullptr, void *const *d_new_crc = nullptr) {
+// one launch on the device buffers d; *tk is armed when a given part has stored CRCs (the kernel compares them with the constant
+// while CRCs are disabled)
+static int recover_slices_enqueue(lzgpu_ctx *ctx, const RecoverSlicesCall &c, uint32_t n_chunks, uint32_t nb, const SlicesBufs &d,
+                                  cudaStream_t st, VerifyTicket *tk) {
 	bool verifying = false;
-	for (uint32_t g = 0; g < c.lay.n_parts; ++g) verifying |= d_parts[g] && d_part_crc && d_part_crc[g];
+	for (uint32_t g = 0; g < c.lay.n_parts; ++g) verifying |= d.parts[g] && d.part_crc && d.part_crc[g];
 	int rc;
 	if (verifying && (rc = tk->arm(ctx, st))) return rc;
-	if ((rc = lz_recover_slices(ctx, c.lay, c.shapes, c.geo, n_chunks, nb, d_parts, part_stride, verifying ? d_part_crc : nullptr, want, d_out,
-	                            out_stride, d_out_crc, d_chunk_out, chunk_out_stride, d_image_crc, d_map, c.check ? c.checks : nullptr,
-	                            d_new_crc, c.correct, st, verifying ? tk->word(0) : nullptr)))
-		return rc;
-	if (!c.check) ctx->stats.chunks_recovered += n_chunks;
+	SlicesBufs k = d;
+	if (!verifying) k.part_crc = nullptr;
+	if ((rc = lz_recover_slices(ctx, c, k, n_chunks, nb, st, verifying ? tk->word(0) : nullptr))) return rc;
+	if (c.mode == lzd::RsMode::RECOVER || c.mode == lzd::RsMode::SALVAGE) ctx->stats.chunks_recovered += n_chunks;
 	return verifying ? tk->publish_fused() : LZGPU_OK;
 }
 
-// The device form of both calls, after their argument check
-static int recover_slices_dev_call(lzgpu_ctx *ctx, const RecoverSlicesCall &c, uint32_t n_chunks, uint32_t nb, const void *const *d_parts,
-                                   const size_t *part_stride, const void *const *d_part_crc, const uint8_t *want, void *const *d_out,
-                                   const size_t *out_stride, void *const *d_out_crc, void *d_chunk_out, size_t chunk_out_stride,
-                                   void *d_image_crc, void *d_map, int64_t *bad, void *stream, void *const *d_new_crc = nullptr) {
+// The device form of the four calls: the argument check, then one launch on the caller's stream
+static int recover_slices_dev(lzgpu_ctx *ctx, lzd::RsMode mode, const lzgpu_goal *goals, uint32_t n_slices, uint32_t n_chunks, uint32_t nb,
+                              const SlicesBufs &d, int64_t *bad, void *stream) {
+	auto c = std::make_unique<RecoverSlicesCall>();
+	c->mode = mode;
+	int rc = recover_slices_args(ctx, goals, n_slices, nb, d, true, *c);
+	if (rc || n_chunks == 0) return rc;
 	if (bad) bad[0] = bad[1] = bad[2] = bad[3] = -1;
 	int64_t b3[3] = {-1, -1, -1};
-	const int rc = dev_call(ctx, stream, recover_slices_alg_bytes(c, n_chunks, nb, d_parts, d_part_crc != nullptr, want, d_out_crc != nullptr,
-	                                                              d_chunk_out != nullptr, d_image_crc != nullptr),
-	                        b3, [&](cudaStream_t st, VerifyTicket *tk) {
-		                        return recover_slices_enqueue(ctx, c, n_chunks, nb, d_parts, part_stride, d_part_crc, want, d_out, out_stride, d_out_crc,
-		                                                      d_chunk_out, chunk_out_stride, st, tk, d_image_crc, d_map, d_new_crc);
-	                        });
-	if (rc == LZGPU_ERR_CRC) recover_slices_bad(c.lay, b3, bad);
+	rc = dev_call(ctx, stream, recover_slices_alg_bytes(*c, n_chunks, nb, d), b3,
+	              [&](cudaStream_t st, VerifyTicket *tk) { return recover_slices_enqueue(ctx, *c, n_chunks, nb, d, st, tk); });
+	if (rc == LZGPU_ERR_CRC) recover_slices_bad(c->lay, b3, bad);
 	return rc;
 }
 
@@ -2335,67 +2315,58 @@ extern "C" int lzgpu_recover_slices_dev(lzgpu_ctx *ctx, const lzgpu_goal *goals,
                                          const uint8_t *want, void *const *d_out, const size_t *out_stride, void *const *d_out_crc,
                                          void *d_chunk_out, size_t chunk_out_stride, int64_t *bad, void *stream) {
 	NvtxScope nvtx_scope("lzgpu::recover_slices_dev");
-	auto c = std::make_unique<RecoverSlicesCall>();
-	int rc = recover_slices_args(ctx, goals, n_slices, nb, d_parts, part_stride, d_part_crc, want, d_out, out_stride, d_out_crc, d_chunk_out,
-	                             chunk_out_stride, true, *c);
-	if (rc || n_chunks == 0) return rc;
-	return recover_slices_dev_call(ctx, *c, n_chunks, nb, d_parts, part_stride, d_part_crc, want, d_out, out_stride, d_out_crc, d_chunk_out,
-	                               chunk_out_stride, nullptr, nullptr, bad, stream);
+	return recover_slices_dev(ctx, lzd::RsMode::RECOVER, goals, n_slices, n_chunks, nb,
+	                          {d_parts, part_stride, d_part_crc, want, d_out, out_stride, d_out_crc, d_chunk_out, chunk_out_stride}, bad, stream);
 }
 
 extern "C" int lzgpu_salvage_slices_dev(lzgpu_ctx *ctx, const lzgpu_goal *goals, uint32_t n_slices, uint32_t n_chunks, uint32_t nb,
                                          const void *const *d_parts, const size_t *part_stride, const void *const *d_part_crc, void *d_image,
                                          size_t image_stride, void *d_image_crc, void *d_map, int64_t *bad, void *stream) {
 	NvtxScope nvtx_scope("lzgpu::salvage_slices_dev");
-	auto c = std::make_unique<RecoverSlicesCall>();
-	c->salvage = true;
-	int rc = recover_slices_args(ctx, goals, n_slices, nb, d_parts, part_stride, d_part_crc, kWantNone, nullptr, nullptr, nullptr, d_image,
-	                             image_stride, true, *c, d_image_crc, d_map);
-	if (rc || n_chunks == 0) return rc;
-	return recover_slices_dev_call(ctx, *c, n_chunks, nb, d_parts, part_stride, d_part_crc, kWantNone, nullptr, nullptr, nullptr, d_image,
-	                               image_stride, d_image_crc, d_map, bad, stream);
+	SlicesBufs d{d_parts, part_stride, d_part_crc, kWantNone};
+	d.image = d_image, d.image_stride = image_stride, d.image_crc = d_image_crc, d.map = d_map;
+	return recover_slices_dev(ctx, lzd::RsMode::SALVAGE, goals, n_slices, n_chunks, nb, d, bad, stream);
 }
 
 extern "C" int lzgpu_check_slices_dev(lzgpu_ctx *ctx, const lzgpu_goal *goals, uint32_t n_slices, uint32_t n_chunks, uint32_t nb,
                                        const void *const *d_parts, const size_t *part_stride, const void *const *d_part_crc, void *d_map,
                                        int64_t *bad, void *stream) {
 	NvtxScope nvtx_scope("lzgpu::check_slices_dev");
-	auto c = std::make_unique<RecoverSlicesCall>();
-	c->check = true;
-	int rc = recover_slices_args(ctx, goals, n_slices, nb, d_parts, part_stride, d_part_crc, kWantNone, nullptr, nullptr, nullptr, nullptr, 0,
-	                             true, *c, nullptr, d_map);
-	if (rc) return rc;
-	if (reinterpret_cast<uintptr_t>(d_map) & 7) { lz_set_error("check_slices: map is not 8-byte aligned"); return LZGPU_ERR_ARG; }
-	if (n_chunks == 0) return LZGPU_OK;
-	return recover_slices_dev_call(ctx, *c, n_chunks, nb, d_parts, part_stride, d_part_crc, kWantNone, nullptr, nullptr, nullptr, nullptr, 0,
-	                               nullptr, d_map, bad, stream);
+	SlicesBufs d{d_parts, part_stride, d_part_crc, kWantNone};
+	d.map = d_map;
+	return recover_slices_dev(ctx, lzd::RsMode::CHECK, goals, n_slices, n_chunks, nb, d, bad, stream);
 }
 
 extern "C" int lzgpu_correct_slices_dev(lzgpu_ctx *ctx, const lzgpu_goal *goals, uint32_t n_slices, uint32_t n_chunks, uint32_t nb,
                                          void *const *d_parts, const size_t *part_stride, const void *const *d_part_crc, void *const *d_new_crc,
                                          void *d_fix, int64_t *bad, void *stream) {
 	NvtxScope nvtx_scope("lzgpu::correct_slices_dev");
-	auto c = std::make_unique<RecoverSlicesCall>();
-	c->check = c->correct = true;
-	int rc = recover_slices_args(ctx, goals, n_slices, nb, d_parts, part_stride, d_part_crc, kWantNone, nullptr, nullptr, nullptr, nullptr, 0,
-	                             true, *c, nullptr, d_fix);
-	if (rc) return rc;
-	if ((rc = check_part_ptrs("correct_slices", "new_crc", d_new_crc, static_cast<int>(c->lay.n_parts), 4))) return rc;
-	if (reinterpret_cast<uintptr_t>(d_fix) & 7) { lz_set_error("correct_slices: fix is not 8-byte aligned"); return LZGPU_ERR_ARG; }
-	if (n_chunks == 0) return LZGPU_OK;
-	return recover_slices_dev_call(ctx, *c, n_chunks, nb, d_parts, part_stride, d_part_crc, kWantNone, nullptr, nullptr, nullptr, nullptr, 0,
-	                               nullptr, d_fix, bad, stream, d_new_crc);
+	SlicesBufs d{d_parts, part_stride, d_part_crc, kWantNone};
+	d.map = d_fix, d.new_crc = d_new_crc;
+	return recover_slices_dev(ctx, lzd::RsMode::CORRECT, goals, n_slices, n_chunks, nb, d, bad, stream);
 }
 
-// The host form of the four calls, after their argument check: the given parts (+ stored CRCs) staged tile by tile, the wanted
-// parts (+ CRCs), the image and the salvage form's image CRCs and map (or the check form's map) copied back.  The salvage and check
-// forms run every tile past a CRC mismatch, so that their outputs are complete.  The correction form corrects the staged tile and
-// copies back its fix entries, and then, for each corrected entry, only the suspect's rewritten blocks and their new CRCs (new_crc).
-static int recover_slices_host(lzgpu_ctx *ctx, const RecoverSlicesCall &c, uint32_t n_chunks, uint32_t nb, const uint8_t *const *parts,
-                               const size_t *part_stride, const uint32_t *const *part_crc, const uint8_t *want, uint8_t *const *out,
-                               const size_t *out_stride, uint32_t *const *out_crc, uint8_t *chunk_out, size_t chunk_out_stride,
-                               uint32_t *image_crc, uint8_t *map, int64_t *bad, uint32_t *const *new_crc = nullptr) {
-	int rc;
+// The host form of the four calls: the argument check, then the given parts (+ stored CRCs) staged tile by tile, the wanted parts
+// (+ CRCs), the image and the salvage's image CRCs and map (or the check's entries) copied back.  The salvage, check and correction
+// run every tile past a CRC mismatch, so that their outputs are complete.  The correction corrects the staged tile and copies back its
+// fix entries, and then, for each corrected entry, only the suspect's rewritten blocks and their new CRCs (new_crc).  The check and
+// correction return LZGPU_ERR_INCONSISTENT when an entry is left bad.
+static int recover_slices_host(lzgpu_ctx *ctx, lzd::RsMode mode, const lzgpu_goal *goals, uint32_t n_slices, uint32_t n_chunks, uint32_t nb,
+                               const SlicesBufs &h, int64_t *bad) {
+	auto cp = std::make_unique<RecoverSlicesCall>();
+	cp->mode = mode;
+	int rc = recover_slices_args(ctx, goals, n_slices, nb, h, false, *cp);
+	if (rc || n_chunks == 0) return rc;
+	const RecoverSlicesCall &c = *cp;
+	const bool check = mode == lzd::RsMode::CHECK || mode == lzd::RsMode::CORRECT;
+	const auto parts = reinterpret_cast<const uint8_t *const *>(h.parts);
+	const auto part_crc = reinterpret_cast<const uint32_t *const *>(h.part_crc);
+	const auto out = reinterpret_cast<uint8_t *const *>(h.out);
+	const auto out_crc = reinterpret_cast<uint32_t *const *>(h.out_crc);
+	const auto new_crc = reinterpret_cast<uint32_t *const *>(h.new_crc);
+	const auto chunk_out = static_cast<uint8_t *>(h.image), map = static_cast<uint8_t *>(h.map);
+	const auto image_crc = static_cast<uint32_t *>(h.image_crc);
+	const uint8_t *want = h.want;
 	if (bad) bad[0] = bad[1] = bad[2] = bad[3] = -1;
 	const lzd::SliceLayout &lay = c.lay;
 	const uint32_t n = lay.n_parts;
@@ -2425,7 +2396,7 @@ static int recover_slices_host(lzgpu_ctx *ctx, const RecoverSlicesCall &c, uint3
 	per_chunk += img_bytes;
 	const size_t map_off = per_chunk, img_crc_off = crc_words;
 	const uint32_t n_cs = (nb + lay.L - 1) / lay.L;
-	const size_t map_bytes = !map ? 0 : c.check ? n_cs * c.entry_bytes() : nb;
+	const size_t map_bytes = !map ? 0 : check ? n_cs * c.entry_bytes() : nb;
 	per_chunk += map_bytes;
 	if (image_crc) crc_words += nb;
 	std::lock_guard<std::mutex> lk(ctx->mu);
@@ -2433,10 +2404,10 @@ static int recover_slices_host(lzgpu_ctx *ctx, const RecoverSlicesCall &c, uint3
 	AutoPin pin(ctx);
 	for (uint32_t g = 0; g < n; ++g) {
 		const int i = lay.slice_of(g);
-		if (parts[g]) pin.add(parts[g], static_cast<size_t>(n_chunks - 1) * part_stride[i] + bytes[g]);
-		if (want[g]) pin.add(out[g], static_cast<size_t>(n_chunks - 1) * out_stride[i] + bytes[g]);
+		if (parts[g]) pin.add(parts[g], static_cast<size_t>(n_chunks - 1) * h.part_stride[i] + bytes[g]);
+		if (want[g]) pin.add(out[g], static_cast<size_t>(n_chunks - 1) * h.out_stride[i] + bytes[g]);
 	}
-	if (chunk_out) pin.add(chunk_out, static_cast<size_t>(n_chunks - 1) * chunk_out_stride + img_bytes);
+	if (chunk_out) pin.add(chunk_out, static_cast<size_t>(n_chunks - 1) * h.image_stride + img_bytes);
 	if (image_crc) pin.add(image_crc, static_cast<size_t>(n_chunks) * nb * 4);
 	if (map) pin.add(map, static_cast<size_t>(n_chunks) * map_bytes);
 	const uint32_t tile = static_cast<uint32_t>(std::max<size_t>(1, std::min<size_t>(n_chunks, (2 * kHostTileBytes) / std::max<size_t>(per_chunk, 1))));
@@ -2456,7 +2427,7 @@ static int recover_slices_host(lzgpu_ctx *ctx, const RecoverSlicesCall &c, uint3
 			uint8_t *buf = static_cast<uint8_t *>(d_in[s]) + tile * off[g];
 			uint32_t *cbuf = static_cast<uint32_t *>(d_crc[s]) + tile * crc_off[g];
 			if (parts[g]) {
-				CUDA_TRY(cudaMemcpy2DAsync(buf, bytes[g], parts[g] + c0 * part_stride[i], part_stride[i], bytes[g], nc, cudaMemcpyHostToDevice, st));
+				CUDA_TRY(cudaMemcpy2DAsync(buf, bytes[g], parts[g] + c0 * h.part_stride[i], h.part_stride[i], bytes[g], nc, cudaMemcpyHostToDevice, st));
 				ctx->stats.bytes_h2d += nc * bytes[g];
 				dp[g] = buf;
 				if (part_crc && part_crc[g]) {
@@ -2470,34 +2441,33 @@ static int recover_slices_host(lzgpu_ctx *ctx, const RecoverSlicesCall &c, uint3
 				if (out_crc && out_crc[g]) docrc[g] = cbuf;
 			}
 		}
-		void *dimg = chunk_out ? static_cast<uint8_t *>(d_in[s]) + tile * img_off : nullptr;
-		uint8_t *dmap = map ? static_cast<uint8_t *>(d_in[s]) + tile * map_off : nullptr;
-		uint32_t *dimg_crc = image_crc ? static_cast<uint32_t *>(d_crc[s]) + tile * img_crc_off : nullptr;
+		const SlicesBufs d{dp, dstride, any_crc ? dpc : nullptr, want, dout, dstride, out_crc ? docrc : nullptr,
+		                   chunk_out ? static_cast<uint8_t *>(d_in[s]) + tile * img_off : nullptr, img_bytes,
+		                   image_crc ? static_cast<uint32_t *>(d_crc[s]) + tile * img_crc_off : nullptr,
+		                   map ? static_cast<uint8_t *>(d_in[s]) + tile * map_off : nullptr, dncrc};
 		int rc;
 		{
-			BatchTimer timer(ctx, st, recover_slices_alg_bytes(c, static_cast<uint32_t>(nc), nb, dp, any_crc, want, out_crc != nullptr, chunk_out != nullptr,
-			                                                   image_crc != nullptr));
-			rc = recover_slices_enqueue(ctx, c, static_cast<uint32_t>(nc), nb, dp, dstride, any_crc ? dpc : nullptr, want, dout, dstride,
-			                            out_crc ? docrc : nullptr, dimg, img_bytes, st, tk, dimg_crc, dmap, dncrc);
+			BatchTimer timer(ctx, st, recover_slices_alg_bytes(c, static_cast<uint32_t>(nc), nb, d));
+			rc = recover_slices_enqueue(ctx, c, static_cast<uint32_t>(nc), nb, d, st, tk);
 		}
 		if (rc) return rc;
 		for (uint32_t g = 0; g < n; ++g) {
 			if (!want[g]) continue;
 			const int i = lay.slice_of(g);
-			CUDA_TRY(cudaMemcpy2DAsync(out[g] + c0 * out_stride[i], out_stride[i], dout[g], bytes[g], bytes[g], nc, cudaMemcpyDeviceToHost, st));
+			CUDA_TRY(cudaMemcpy2DAsync(out[g] + c0 * h.out_stride[i], h.out_stride[i], dout[g], bytes[g], bytes[g], nc, cudaMemcpyDeviceToHost, st));
 			ctx->stats.bytes_d2h += nc * bytes[g];
 			if (docrc[g]) CUDA_TRY(cudaMemcpyAsync(out_crc[g] + c0 * c.pb[i], docrc[g], nc * c.pb[i] * 4, cudaMemcpyDeviceToHost, st));
 		}
 		if (chunk_out) {
-			CUDA_TRY(cudaMemcpy2DAsync(chunk_out + c0 * chunk_out_stride, chunk_out_stride, dimg, img_bytes, img_bytes, nc, cudaMemcpyDeviceToHost, st));
+			CUDA_TRY(cudaMemcpy2DAsync(chunk_out + c0 * h.image_stride, h.image_stride, d.image, img_bytes, img_bytes, nc, cudaMemcpyDeviceToHost, st));
 			ctx->stats.bytes_d2h += nc * img_bytes;
 		}
 		if (map) {
-			CUDA_TRY(cudaMemcpyAsync(map + c0 * map_bytes, dmap, nc * map_bytes, cudaMemcpyDeviceToHost, st));
+			CUDA_TRY(cudaMemcpyAsync(map + c0 * map_bytes, d.map, nc * map_bytes, cudaMemcpyDeviceToHost, st));
 			ctx->stats.bytes_d2h += nc * map_bytes;
 		}
-		if (image_crc) CUDA_TRY(cudaMemcpyAsync(image_crc + c0 * nb, dimg_crc, nc * nb * 4, cudaMemcpyDeviceToHost, st));
-		if (!c.correct) return LZGPU_OK;
+		if (image_crc) CUDA_TRY(cudaMemcpyAsync(image_crc + c0 * nb, d.image_crc, nc * nb * 4, cudaMemcpyDeviceToHost, st));
+		if (mode != lzd::RsMode::CORRECT) return LZGPU_OK;
 		// the corrected entries' rewritten blocks, a run of consecutive part blocks at a time, and their new CRCs
 		CUDA_TRY(cudaStreamSynchronize(st));
 		const lzgpu_slices_fix *fix = reinterpret_cast<const lzgpu_slices_fix *>(map) + c0 * n_cs;
@@ -2513,7 +2483,7 @@ static int recover_slices_host(lzgpu_ctx *ctx, const RecoverSlicesCall &c, uint3
 				uint32_t run = 1;
 				while (b + run < ck.n_blocks && ck.blk_part[b + run] == g && ck.blk_s[b + run] == ck.blk_s[b] + run) ++run;
 				const size_t blk = cs * spc + ck.blk_s[b];
-				CUDA_TRY(cudaMemcpyAsync(const_cast<uint8_t *>(parts[g]) + (c0 + cc) * part_stride[i] + blk * B,
+				CUDA_TRY(cudaMemcpyAsync(const_cast<uint8_t *>(parts[g]) + (c0 + cc) * h.part_stride[i] + blk * B,
 				                         static_cast<const uint8_t *>(dp[g]) + cc * bytes[g] + blk * B, run * B, cudaMemcpyDeviceToHost, st));
 				ctx->stats.bytes_d2h += run * B;
 				if (dncrc[g])
@@ -2523,9 +2493,16 @@ static int recover_slices_host(lzgpu_ctx *ctx, const RecoverSlicesCall &c, uint3
 			}
 		}
 		return LZGPU_OK;
-	}, c.salvage || c.check);
+	}, mode != lzd::RsMode::RECOVER);
 	if (rc == LZGPU_ERR_CRC) recover_slices_bad(lay, b3, bad);
-	return rc;
+	if (rc || !check) return rc;
+	const auto *entries = reinterpret_cast<const lzgpu_slices_check *>(map);
+	const auto *fix = reinterpret_cast<const lzgpu_slices_fix *>(map);
+	for (size_t e = 0; e < static_cast<size_t>(n_chunks) * n_cs; ++e)
+		if (mode == lzd::RsMode::CHECK ? entries[e].bad_checks != 0
+		                               : fix[e].status == LZGPU_FIX_UNEXPLAINED || fix[e].status == LZGPU_FIX_UNDETERMINED)
+			return LZGPU_ERR_INCONSISTENT;
+	return LZGPU_OK;
 }
 
 extern "C" int lzgpu_recover_slices(lzgpu_ctx *ctx, const lzgpu_goal *goals, uint32_t n_slices, uint32_t n_chunks, uint32_t nb,
@@ -2533,68 +2510,37 @@ extern "C" int lzgpu_recover_slices(lzgpu_ctx *ctx, const lzgpu_goal *goals, uin
                                      uint8_t *const *out, const size_t *out_stride, uint32_t *const *out_crc, uint8_t *chunk_out,
                                      size_t chunk_out_stride, int64_t *bad) {
 	NvtxScope nvtx_scope("lzgpu::recover_slices");
-	auto c = std::make_unique<RecoverSlicesCall>();
-	int rc = recover_slices_args(ctx, goals, n_slices, nb, reinterpret_cast<const void *const *>(parts), part_stride,
-	                             reinterpret_cast<const void *const *>(part_crc), want, reinterpret_cast<const void *const *>(out), out_stride,
-	                             reinterpret_cast<const void *const *>(out_crc), chunk_out, chunk_out_stride, false, *c);
-	if (rc || n_chunks == 0) return rc;
-	return recover_slices_host(ctx, *c, n_chunks, nb, parts, part_stride, part_crc, want, out, out_stride, out_crc, chunk_out, chunk_out_stride,
-	                           nullptr, nullptr, bad);
+	return recover_slices_host(ctx, lzd::RsMode::RECOVER, goals, n_slices, n_chunks, nb,
+	                           {reinterpret_cast<const void *const *>(parts), part_stride, reinterpret_cast<const void *const *>(part_crc), want,
+	                            reinterpret_cast<void *const *>(out), out_stride, reinterpret_cast<void *const *>(out_crc), chunk_out, chunk_out_stride},
+	                           bad);
 }
 
 extern "C" int lzgpu_salvage_slices(lzgpu_ctx *ctx, const lzgpu_goal *goals, uint32_t n_slices, uint32_t n_chunks, uint32_t nb,
                                      const uint8_t *const *parts, const size_t *part_stride, const uint32_t *const *part_crc, uint8_t *image,
                                      size_t image_stride, uint32_t *image_crc, uint8_t *map, int64_t *bad) {
 	NvtxScope nvtx_scope("lzgpu::salvage_slices");
-	auto c = std::make_unique<RecoverSlicesCall>();
-	c->salvage = true;
-	int rc = recover_slices_args(ctx, goals, n_slices, nb, reinterpret_cast<const void *const *>(parts), part_stride,
-	                             reinterpret_cast<const void *const *>(part_crc), kWantNone, nullptr, nullptr, nullptr, image, image_stride, false,
-	                             *c, image_crc, map);
-	if (rc || n_chunks == 0) return rc;
-	return recover_slices_host(ctx, *c, n_chunks, nb, parts, part_stride, part_crc, kWantNone, nullptr, nullptr, nullptr, image, image_stride,
-	                           image_crc, map, bad);
+	SlicesBufs h{reinterpret_cast<const void *const *>(parts), part_stride, reinterpret_cast<const void *const *>(part_crc), kWantNone};
+	h.image = image, h.image_stride = image_stride, h.image_crc = image_crc, h.map = map;
+	return recover_slices_host(ctx, lzd::RsMode::SALVAGE, goals, n_slices, n_chunks, nb, h, bad);
 }
 
 extern "C" int lzgpu_check_slices(lzgpu_ctx *ctx, const lzgpu_goal *goals, uint32_t n_slices, uint32_t n_chunks, uint32_t nb,
                                    const uint8_t *const *parts, const size_t *part_stride, const uint32_t *const *part_crc,
                                    lzgpu_slices_check *map, int64_t *bad) {
 	NvtxScope nvtx_scope("lzgpu::check_slices");
-	auto c = std::make_unique<RecoverSlicesCall>();
-	c->check = true;
-	int rc = recover_slices_args(ctx, goals, n_slices, nb, reinterpret_cast<const void *const *>(parts), part_stride,
-	                             reinterpret_cast<const void *const *>(part_crc), kWantNone, nullptr, nullptr, nullptr, nullptr, 0, false, *c,
-	                             nullptr, map);
-	if (rc || n_chunks == 0) return rc;
-	rc = recover_slices_host(ctx, *c, n_chunks, nb, parts, part_stride, part_crc, kWantNone, nullptr, nullptr, nullptr, nullptr, 0, nullptr,
-	                         reinterpret_cast<uint8_t *>(map), bad);
-	if (rc) return rc;
-	const size_t n = static_cast<size_t>(n_chunks) * ((nb + c->lay.L - 1) / c->lay.L);
-	for (size_t e = 0; e < n; ++e)
-		if (map[e].bad_checks) return LZGPU_ERR_INCONSISTENT;
-	return LZGPU_OK;
+	SlicesBufs h{reinterpret_cast<const void *const *>(parts), part_stride, reinterpret_cast<const void *const *>(part_crc), kWantNone};
+	h.map = map;
+	return recover_slices_host(ctx, lzd::RsMode::CHECK, goals, n_slices, n_chunks, nb, h, bad);
 }
 
 extern "C" int lzgpu_correct_slices(lzgpu_ctx *ctx, const lzgpu_goal *goals, uint32_t n_slices, uint32_t n_chunks, uint32_t nb,
                                      uint8_t *const *parts, const size_t *part_stride, const uint32_t *const *part_crc, uint32_t *const *new_crc,
                                      lzgpu_slices_fix *fix, int64_t *bad) {
 	NvtxScope nvtx_scope("lzgpu::correct_slices");
-	auto c = std::make_unique<RecoverSlicesCall>();
-	c->check = c->correct = true;
-	int rc = recover_slices_args(ctx, goals, n_slices, nb, reinterpret_cast<const void *const *>(parts), part_stride,
-	                             reinterpret_cast<const void *const *>(part_crc), kWantNone, nullptr, nullptr, nullptr, nullptr, 0, false, *c,
-	                             nullptr, fix);
-	if (rc) return rc;
-	if ((rc = check_part_ptrs("correct_slices", "new_crc", reinterpret_cast<const void *const *>(new_crc), static_cast<int>(c->lay.n_parts), 4)))
-		return rc;
-	if (n_chunks == 0) return LZGPU_OK;
-	rc = recover_slices_host(ctx, *c, n_chunks, nb, parts, part_stride, part_crc, kWantNone, nullptr, nullptr, nullptr, nullptr, 0, nullptr,
-	                         reinterpret_cast<uint8_t *>(fix), bad, new_crc);
-	if (rc) return rc;
-	const size_t n = static_cast<size_t>(n_chunks) * ((nb + c->lay.L - 1) / c->lay.L);
-	for (size_t e = 0; e < n; ++e)
-		if (fix[e].status == LZGPU_FIX_UNEXPLAINED || fix[e].status == LZGPU_FIX_UNDETERMINED) return LZGPU_ERR_INCONSISTENT;
-	return LZGPU_OK;
+	SlicesBufs h{reinterpret_cast<const void *const *>(parts), part_stride, reinterpret_cast<const void *const *>(part_crc), kWantNone};
+	h.map = fix, h.new_crc = reinterpret_cast<void *const *>(new_crc);
+	return recover_slices_host(ctx, lzd::RsMode::CORRECT, goals, n_slices, n_chunks, nb, h, bad);
 }
 
 // ------------------------------------------------------------------------------------------------

@@ -10,6 +10,7 @@
 #include <vector>
 
 #include "lzgpu.h"
+#include "slices_check.h"
 
 #define LZGPU_NOT_HANDLED 1  // internal: the fused path does not specialise this shape, use the generic kernels
 
@@ -210,23 +211,38 @@ int lz_fused_check(lzgpu_ctx *ctx, const lzgpu_goal *goal, uint32_t n_chunks, ui
 int lz_fused_encode_slices(lzgpu_ctx *ctx, const lzgpu_goal *goals, uint32_t n_slices, uint32_t n_chunks, uint32_t nb, const void *d_data,
                            size_t chunk_stride, void *const *d_parity, const size_t *parity_stride, void *const *d_crc, const size_t *crc_stride,
                            cudaStream_t st);
-// Recovery from the parts of every slice together (recover_slices_kernel.cuh): the one launch of lzgpu_recover_slices*, whose arguments,
-// solve (shapes[0] a full combined stripe, shapes[1] the tail) and geometry the caller has checked.  d_first_bad: the armed result word
-// whenever d_part_crc is given.  d_map != nullptr: the salvage form (lzgpu_salvage_slices*: nothing wanted, the image, its optional
-// block CRCs d_image_crc and the status bytes d_map), on the SALVAGE instantiation.  checks != nullptr: the check form
-// (lzgpu_check_slices*: nothing wanted, no image, checks[0..1] of both shapes, the entries d_map), on the CHECK instantiation and then
-// the locate pass.  correct: the correction form (lzgpu_correct_slices*: as the check form, d_map the fix entries, d_new_crc the optional
-// new CRC arrays per flat part), on the CORRECT instantiation, the locate pass and correct_slices_kernel.
-namespace lzd {
-struct SliceLayout;
-struct SliceSolve;
-struct SliceChecks;
-struct RsGeometry;
-}  // namespace lzd
-int lz_recover_slices(lzgpu_ctx *ctx, const lzd::SliceLayout &lay, const lzd::SliceSolve *shapes, const lzd::RsGeometry &geo, uint32_t n_chunks,
-                      uint32_t nb, const void *const *d_parts, const size_t *part_stride, const void *const *d_part_crc, const uint8_t *want,
-                      void *const *d_out, const size_t *out_stride, void *const *d_out_crc, void *d_image, size_t image_stride, void *d_image_crc,
-                      void *d_map, const lzd::SliceChecks *checks, void *const *d_new_crc, bool correct, cudaStream_t st,
+// The buffers of one call of the multi-slice recovery family (lzgpu_recover_slices*, _salvage_, _check_, _correct_): the caller's,
+// host or device, or one staged tile's.  Per flat part: parts (NULL = not given), part_crc, want, out and out_crc (the wanted parts),
+// new_crc (the correction's new CRCs); per slice: part_stride, out_stride.  The image with image_stride and image_crc; map: the
+// salvage's status bytes, the check's entries or the correction's fix entries.
+struct SlicesBufs {
+	const void *const *parts = nullptr;
+	const size_t *part_stride = nullptr;
+	const void *const *part_crc = nullptr;
+	const uint8_t *want = nullptr;
+	void *const *out = nullptr;
+	const size_t *out_stride = nullptr;
+	void *const *out_crc = nullptr;
+	void *image = nullptr;
+	size_t image_stride = 0;
+	void *image_crc = nullptr;
+	void *map = nullptr;
+	void *const *new_crc = nullptr;
+};
+
+// What the argument check derives from a call of that family: which call it is (mode), the flat part layout, blocks per part of each
+// slice (pb), and the shape plan (the solve of both stripe shapes, their checks for CHECK and CORRECT, the launch geometry)
+struct RecoverSlicesCall : lzd::SliceShapes {
+	lzd::RsMode mode = lzd::RsMode::RECOVER;
+	lzd::SliceLayout lay;
+	uint32_t pb[lzd::kSlicesMax] = {0};
+	size_t entry_bytes() const { return mode == lzd::RsMode::CORRECT ? sizeof(lzgpu_slices_fix) : sizeof(lzgpu_slices_check); }
+};
+
+// The one launch of a checked call of that family on the device buffers d (recover_slices_kernel.cuh), on the kernel instantiation of
+// c.mode; CHECK then runs the locate pass, CORRECT the locate pass and correct_slices_kernel.  d_first_bad: the armed result word
+// whenever d.part_crc is given.
+int lz_recover_slices(lzgpu_ctx *ctx, const RecoverSlicesCall &c, const SlicesBufs &d, uint32_t n_chunks, uint32_t nb, cudaStream_t st,
                       unsigned long long *d_first_bad);
 // CRC of 64 KiB blocks: block (c, b) at base + c*chunk_stride + b*65536, out[c*out_chunk_stride + b]
 int lz_fused_crc(lzgpu_ctx *ctx, const void *base, unsigned long long n_blocks, unsigned long long blocks_per_chunk,

@@ -1071,12 +1071,27 @@ static void rs_fill_salvage(RsSalvage &o, const RsShape &sh, const SliceLayout &
 	}
 }
 
-// lzgpu_check_slices' locate pass, after the CHECK launch has written every entry: the tables of both shapes in a stream-ordered
-// temporary, and one CTA per bad entry.  d_fix: lzgpu_correct_slices, after the CORRECT launch (d_map a temporary, d_crc_failed its
-// masks): the rows of P of both shapes after the annihilators, then correct_slices_kernel over every entry.
-static int rs_locate(lzgpu_ctx *ctx, const SliceLayout &lay, const SliceChecks *checks, uint32_t n_chunks, uint32_t nb,
-                     const void *const *d_parts, const size_t *part_stride, RsCheckEntry *d_map, cudaStream_t st,
-                     RsFixEntry *d_fix = nullptr, const unsigned long long *d_crc_failed = nullptr, void *const *d_new_crc = nullptr) {
+// part_stride, spc and every flat part's slice and pointer, alike in the parameters of the recovery, locate and correct kernels
+template <class Params>
+static void rs_fill_parts(Params &o, const SliceLayout &lay, const void *const *d_parts, const size_t *part_stride) {
+	for (uint32_t i = 0; i < lay.n_slices; ++i) {
+		o.part_stride[i] = part_stride[i];
+		o.spc[i] = lay.L / lay.k[i];
+		for (uint32_t g = lay.base[i]; g < lay.base[i] + lay.k[i] + lay.m[i]; ++g) {
+			o.part_slice[g] = static_cast<uint8_t>(i);
+			o.parts[g] = static_cast<uint8_t *>(const_cast<void *>(d_parts[g]));
+		}
+	}
+}
+
+// lzgpu_check_slices' locate pass, after the CHECK launch has written every entry to d_map: the tables of both shapes in a
+// stream-ordered temporary, and one CTA per bad entry.  lzgpu_correct_slices, after the CORRECT launch (d_map a temporary, d_crc_failed
+// its masks): the rows of P of both shapes after the annihilators, then correct_slices_kernel over every entry, into d.map's fix entries.
+static int rs_locate(lzgpu_ctx *ctx, const RecoverSlicesCall &c, const SlicesBufs &d, uint32_t n_chunks, uint32_t nb, RsCheckEntry *d_map,
+                     const unsigned long long *d_crc_failed, cudaStream_t st) {
+	const SliceLayout &lay = c.lay;
+	const SliceChecks *checks = c.checks;
+	RsFixEntry *d_fix = c.mode == RsMode::CORRECT ? static_cast<RsFixEntry *>(d.map) : nullptr;
 	const uint32_t n_cs = (nb + lay.L - 1) / lay.L, tail = nb % lay.L ? 1u : 0u;
 	size_t rows = checks[0].ann.size() / kScMaxChecks + (tail ? checks[1].ann.size() / kScMaxChecks : 0);
 	const size_t ann_rows = rows;
@@ -1132,14 +1147,7 @@ static int rs_locate(lzgpu_ctx *ctx, const SliceLayout &lay, const SliceChecks *
 	CUDA_TRY(cudaMemcpyAsync(d_loc.p, host.data(), host.size(), cudaMemcpyHostToDevice, st));
 	auto p = std::make_unique<LocateSlicesParams>();
 	std::memset(p.get(), 0, sizeof(LocateSlicesParams));
-	for (uint32_t i = 0; i < lay.n_slices; ++i) {
-		p->part_stride[i] = part_stride[i];
-		p->spc[i] = lay.L / lay.k[i];
-		for (uint32_t g = lay.base[i]; g < lay.base[i] + lay.k[i] + lay.m[i]; ++g) {
-			p->part_slice[g] = static_cast<uint8_t>(i);
-			p->parts[g] = static_cast<const uint8_t *>(d_parts[g]);
-		}
-	}
+	rs_fill_parts(*p, lay, d.parts, d.part_stride);
 	p->map = d_map;
 	p->loc = static_cast<const RsLocate *>(d_loc.p);
 	p->n_entries = static_cast<unsigned long long>(n_chunks) * n_cs;
@@ -1151,16 +1159,9 @@ static int rs_locate(lzgpu_ctx *ctx, const SliceLayout &lay, const SliceChecks *
 	CUDA_TRY(cudaGetLastError());
 	ctx->stats.kernel_launches++;
 	if (!d_fix) return LZGPU_OK;
-	for (uint32_t i = 0; i < lay.n_slices; ++i) {
-		cp->part_stride[i] = part_stride[i];
-		cp->spc[i] = lay.L / lay.k[i];
-		cp->pb[i] = (nb + lay.k[i] - 1) / lay.k[i];
-		for (uint32_t g = lay.base[i]; g < lay.base[i] + lay.k[i] + lay.m[i]; ++g) {
-			cp->part_slice[g] = static_cast<uint8_t>(i);
-			cp->parts[g] = static_cast<uint8_t *>(const_cast<void *>(d_parts[g]));
-			cp->new_crc[g] = d_new_crc ? static_cast<uint32_t *>(d_new_crc[g]) : nullptr;
-		}
-	}
+	rs_fill_parts(*cp, lay, d.parts, d.part_stride);
+	std::memcpy(cp->pb, c.pb, sizeof(cp->pb));
+	for (uint32_t g = 0; g < lay.n_parts; ++g) cp->new_crc[g] = d.new_crc ? static_cast<uint32_t *>(d.new_crc[g]) : nullptr;
 	cp->map = d_map;
 	cp->crc_failed = d_crc_failed;
 	cp->fix = d_fix;
@@ -1179,30 +1180,27 @@ static int rs_locate(lzgpu_ctx *ctx, const SliceLayout &lay, const SliceChecks *
 	return LZGPU_OK;
 }
 
-int lz_recover_slices(lzgpu_ctx *ctx, const SliceLayout &lay, const SliceSolve *shapes, const RsGeometry &geo, uint32_t n_chunks, uint32_t nb,
-                      const void *const *d_parts, const size_t *part_stride, const void *const *d_part_crc, const uint8_t *want, void *const *d_out,
-                      const size_t *out_stride, void *const *d_out_crc, void *d_image, size_t image_stride, void *d_image_crc, void *d_map,
-                      const SliceChecks *checks, void *const *d_new_crc, bool correct, cudaStream_t st, unsigned long long *d_first_bad) {
+int lz_recover_slices(lzgpu_ctx *ctx, const RecoverSlicesCall &c, const SlicesBufs &d, uint32_t n_chunks, uint32_t nb, cudaStream_t st,
+                      unsigned long long *d_first_bad) {
+	const SliceLayout &lay = c.lay;
+	const RsGeometry &geo = c.geo;
+	const RsMode mode = c.mode;
+	const bool checks = mode == RsMode::CHECK || mode == RsMode::CORRECT;
 	auto p = std::make_unique<RecoverSlicesParams>();
 	std::memset(p.get(), 0, sizeof(RecoverSlicesParams));
 	const bool crc_on = lzgpu_crc_enabled() != 0;
-	for (uint32_t i = 0; i < lay.n_slices; ++i) {
-		p->part_stride[i] = part_stride ? part_stride[i] : 0;
-		p->out_stride[i] = out_stride ? out_stride[i] : 0;
-		p->k[i] = lay.k[i];
-		p->spc[i] = lay.L / lay.k[i];
-		p->pb[i] = (nb + lay.k[i] - 1) / lay.k[i];
-		for (uint32_t g = lay.base[i]; g < lay.base[i] + lay.k[i] + lay.m[i]; ++g) {
-			p->part_slice[g] = static_cast<uint8_t>(i);
-			p->parts[g] = static_cast<const uint8_t *>(d_parts[g]);
-			p->stored[g] = d_part_crc ? static_cast<const uint32_t *>(d_part_crc[g]) : nullptr;
-			p->out[g] = want[g] ? static_cast<uint8_t *>(d_out[g]) : nullptr;
-			p->out_crc[g] = want[g] && d_out_crc ? static_cast<uint32_t *>(d_out_crc[g]) : nullptr;
-		}
+	rs_fill_parts(*p, lay, d.parts, d.part_stride);
+	for (uint32_t i = 0; i < lay.n_slices; ++i) p->out_stride[i] = d.out_stride ? d.out_stride[i] : 0;
+	for (uint32_t g = 0; g < lay.n_parts; ++g) {
+		p->stored[g] = d.part_crc ? static_cast<const uint32_t *>(d.part_crc[g]) : nullptr;
+		p->out[g] = d.want[g] ? static_cast<uint8_t *>(d.out[g]) : nullptr;
+		p->out_crc[g] = d.want[g] && d.out_crc ? static_cast<uint32_t *>(d.out_crc[g]) : nullptr;
 	}
+	std::memcpy(p->k, lay.k, sizeof(p->k));
+	std::memcpy(p->pb, c.pb, sizeof(p->pb));
 	std::memcpy(p->gen, lay.gen, sizeof(p->gen));
-	p->image = static_cast<uint8_t *>(d_image);
-	p->image_stride = image_stride;
+	p->image = static_cast<uint8_t *>(d.image);
+	p->image_stride = d.image_stride;
 	p->tables = ctx->d_crc_tables;
 	p->first_bad = d_first_bad;
 	p->L = lay.L;
@@ -1217,14 +1215,13 @@ int lz_recover_slices(lzgpu_ctx *ctx, const SliceLayout &lay, const SliceSolve *
 	p->crc_off = crc_on ? 0u : 1u;
 	p->zconst = lz::crc_of_zeros(LZGPU_BLOCK_SIZE);
 	for (int i = 0; i < 5; ++i) p->tree_mult[i] = lz::crc_xpow_bytes(2048ull << i);
-	const bool verifying = d_part_crc != nullptr;
+	const bool verifying = d.part_crc != nullptr;
 	if (verifying && !d_first_bad) return LZGPU_ERR_ARG;  // (cannot happen: the caller arms a ticket whenever it passes stored CRCs)
-	const RsMode mode = correct ? RsMode::CORRECT : checks ? RsMode::CHECK : d_map ? RsMode::SALVAGE : RsMode::RECOVER;
-	p->image_crc = static_cast<uint32_t *>(d_image_crc);
-	p->map = static_cast<uint8_t *>(d_map);
-	TmpBuf d_tmp(ctx, st);   // CORRECT: the check's entries and the failing-part masks, before correct_slices_kernel writes d_map
+	p->image_crc = static_cast<uint32_t *>(d.image_crc);
+	p->map = static_cast<uint8_t *>(d.map);
+	TmpBuf d_tmp(ctx, st);   // CORRECT: the check's entries and the failing-part masks, before correct_slices_kernel writes d.map
 	const unsigned long long n_entries = static_cast<unsigned long long>(n_chunks) * p->n_cs;
-	if (correct) {
+	if (mode == RsMode::CORRECT) {
 		int rc;
 		if ((rc = d_tmp.alloc(n_entries * (sizeof(RsCheckEntry) + sizeof(unsigned long long))))) return rc;
 		p->map = static_cast<uint8_t *>(d_tmp.p);
@@ -1232,16 +1229,14 @@ int lz_recover_slices(lzgpu_ctx *ctx, const SliceLayout &lay, const SliceSolve *
 	}
 	for (int t = 0; t < 2; ++t)
 		if (t == 0 ? nb >= lay.L : p->tail != 0) {
-			rs_fill_shape(p->shape[t], lay, shapes[t], d_parts, d_part_crc, want, d_out_crc, d_image != nullptr, d_image_crc != nullptr,
-			              checks ? &checks[t] : nullptr);
-			if (mode == RsMode::SALVAGE) rs_fill_salvage(p->salvage[t], p->shape[t], lay, shapes[t]);
+			rs_fill_shape(p->shape[t], lay, c.shapes[t], d.parts, d.part_crc, d.want, d.out_crc, d.image != nullptr, d.image_crc != nullptr,
+			              checks ? &c.checks[t] : nullptr);
+			if (mode == RsMode::SALVAGE) rs_fill_salvage(p->salvage[t], p->shape[t], lay, c.shapes[t]);
 		}
 	static const int kKernelOf[] = {LZGPU_KERNEL_RECOVER_SLICES, LZGPU_KERNEL_SALVAGE_SLICES, LZGPU_KERNEL_CHECK_SLICES,
 	                                LZGPU_KERNEL_CORRECT_SLICES};
 	const lzgpu_launch_geometry g = launch_geo(kKernelOf[static_cast<int>(mode)], geo.threads, geo.G, geo.stages, 0, geo.smem);
 	int rc = launch(ctx, kRecoverSlicers[static_cast<int>(mode)], g, 1, p->total_units, st, *p);
 	if (rc || !checks) return rc;
-	if (!correct) return rs_locate(ctx, lay, checks, n_chunks, nb, d_parts, part_stride, static_cast<RsCheckEntry *>(d_map), st);
-	return rs_locate(ctx, lay, checks, n_chunks, nb, d_parts, part_stride, reinterpret_cast<RsCheckEntry *>(p->map), st,
-	                 static_cast<RsFixEntry *>(d_map), p->crc_failed, d_new_crc);
+	return rs_locate(ctx, c, d, n_chunks, nb, reinterpret_cast<RsCheckEntry *>(p->map), p->crc_failed, st);
 }

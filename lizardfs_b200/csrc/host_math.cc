@@ -608,94 +608,76 @@ int lzgpu_plan_encode_slices(const lzgpu_goal *goals, uint32_t n_slices, uint32_
 	return LZGPU_OK;
 }
 
-int lzgpu_plan_recover_slices(const lzgpu_goal *goals, uint32_t n_slices, uint32_t nb, const uint8_t *given, lzgpu_slices_recover_plan *out) {
+}  // extern "C"
+
+// The plans' common part: the arguments, the layout, the shape plan with all a plan reports (lzd::slice_shapes), L, tail_blocks and
+// the launch geometry
+template <class Plan>
+static int slices_plan(const lzgpu_goal *goals, uint32_t n_slices, uint32_t nb, const uint8_t *given, lzd::RsMode mode, Plan *out,
+                       lzd::SliceShapes &sh) {
 	if (!out || !given || nb == 0 || nb > LZGPU_BLOCKS_IN_CHUNK) return LZGPU_ERR_ARG;
-	*out = lzgpu_slices_recover_plan{};
+	*out = Plan{};
 	lzd::SliceLayout lay;
 	const char *why = nullptr;
 	if (lzd::slice_layout(goals, n_slices, lay, &why) != LZGPU_OK) return LZGPU_ERR_ARG;
-	lzd::SliceSolve sv[2];
-	lzd::slice_solve(lay, given, lay.L, sv[0]);
-	const uint32_t tail = nb % lay.L;
-	if (tail) lzd::slice_solve(lay, given, tail, sv[1]);
+	lzd::slice_shapes(lay, given, nb, mode, sh, true);
 	out->L = lay.L;
-	out->known = sv[0].known;
-	out->determined = sv[0].determined;
-	out->tail_determined = tail ? sv[1].determined : sv[0].determined;
-	out->tail_blocks = tail;
-	out->unknowns = sv[0].n_unknown;
-	out->equations = sv[0].n_eq;
-	out->tail_unknowns = tail ? sv[1].n_unknown : 0;
-	out->tail_equations = tail ? sv[1].n_eq : 0;
-	// the shapes the call's chunks have: full stripes when nb >= L, the tail when L does not divide nb
-	const lzd::SliceSolve used[2] = {nb >= lay.L ? sv[0] : sv[1], tail ? sv[1] : sv[0]};
-	const lzd::RsGeometry g = lzd::rs_geometry(lay, given, used, 2);
-	out->ok = g.ok ? 1 : 0;
-	out->G = g.G;
-	out->threads = g.threads;
-	out->stages = g.stages;
-	out->smem_bytes = static_cast<uint32_t>(g.smem);
+	out->tail_blocks = nb % lay.L;
+	out->ok = sh.geo.ok ? 1 : 0;
+	out->G = sh.geo.G;
+	out->threads = sh.geo.threads;
+	out->stages = sh.geo.stages;
+	out->smem_bytes = static_cast<uint32_t>(sh.geo.smem);
+	return LZGPU_OK;
+}
+
+extern "C" {
+
+int lzgpu_plan_recover_slices(const lzgpu_goal *goals, uint32_t n_slices, uint32_t nb, const uint8_t *given, lzgpu_slices_recover_plan *out) {
+	auto sh = std::make_unique<lzd::SliceShapes>();
+	const int rc = slices_plan(goals, n_slices, nb, given, lzd::RsMode::RECOVER, out, *sh);
+	if (rc) return rc;
+	const lzd::SliceSolve &full = sh->shapes[0], &last = out->tail_blocks ? sh->shapes[1] : full;
+	out->known = full.known;
+	out->determined = full.determined;
+	out->tail_determined = last.determined;
+	out->unknowns = full.n_unknown;
+	out->equations = full.n_eq;
+	out->tail_unknowns = out->tail_blocks ? last.n_unknown : 0;
+	out->tail_equations = out->tail_blocks ? last.n_eq : 0;
 	return LZGPU_OK;
 }
 
 int lzgpu_plan_salvage_slices(const lzgpu_goal *goals, uint32_t n_slices, uint32_t nb, const uint8_t *given, lzgpu_slices_salvage_plan *out) {
-	if (!out || !given || nb == 0 || nb > LZGPU_BLOCKS_IN_CHUNK) return LZGPU_ERR_ARG;
-	*out = lzgpu_slices_salvage_plan{};
-	lzd::SliceLayout lay;
-	const char *why = nullptr;
-	if (lzd::slice_layout(goals, n_slices, lay, &why) != LZGPU_OK) return LZGPU_ERR_ARG;
-	lzd::SliceSolve sv[2];
-	lzd::slice_solve(lay, given, lay.L, sv[0]);
-	const uint32_t tail = nb % lay.L;
-	if (tail) lzd::slice_solve(lay, given, tail, sv[1]);
-	out->L = lay.L;
-	out->tail_blocks = tail;
-	out->known = sv[0].known;
-	out->determined = sv[0].determined;
-	out->tail_known = tail ? sv[1].known : sv[0].known;
-	out->tail_determined = tail ? sv[1].determined : sv[0].determined;
-	const lzd::SliceSolve used[2] = {nb >= lay.L ? sv[0] : sv[1], tail ? sv[1] : sv[0]};
-	const lzd::RsGeometry g = lzd::rs_geometry(lay, given, used, 2, lzd::RsMode::SALVAGE);
-	out->ok = g.ok ? 1 : 0;
-	out->G = g.G;
-	out->threads = g.threads;
-	out->stages = g.stages;
-	out->smem_bytes = static_cast<uint32_t>(g.smem);
+	auto sh = std::make_unique<lzd::SliceShapes>();
+	const int rc = slices_plan(goals, n_slices, nb, given, lzd::RsMode::SALVAGE, out, *sh);
+	if (rc) return rc;
+	const lzd::SliceSolve &full = sh->shapes[0], &last = out->tail_blocks ? sh->shapes[1] : full;
+	out->known = full.known;
+	out->determined = full.determined;
+	out->tail_known = last.known;
+	out->tail_determined = last.determined;
+	return LZGPU_OK;
+}
+
+// lzgpu_plan_check_slices, and the check plan of lzgpu_plan_correct_slices with the checks it reads correctable from
+static int check_plan(const lzgpu_goal *goals, uint32_t n_slices, uint32_t nb, const uint8_t *given, lzgpu_slices_check_plan *out,
+                      lzd::SliceShapes &sh) {
+	const int rc = slices_plan(goals, n_slices, nb, given, lzd::RsMode::CHECK, out, sh);
+	if (rc) return rc;
+	const lzd::SliceChecks &full = sh.checks[0], &last = out->tail_blocks ? sh.checks[1] : full;
+	out->n_checks = full.n_checks;
+	out->tail_n_checks = last.n_checks;
+	out->checked = full.checked;
+	out->tail_checked = last.checked;
+	out->locatable = full.locatable;
+	out->tail_locatable = last.locatable;
 	return LZGPU_OK;
 }
 
 int lzgpu_plan_check_slices(const lzgpu_goal *goals, uint32_t n_slices, uint32_t nb, const uint8_t *given, lzgpu_slices_check_plan *out) {
-	if (!out || !given || nb == 0 || nb > LZGPU_BLOCKS_IN_CHUNK) return LZGPU_ERR_ARG;
-	*out = lzgpu_slices_check_plan{};
-	lzd::SliceLayout lay;
-	const char *why = nullptr;
-	if (lzd::slice_layout(goals, n_slices, lay, &why) != LZGPU_OK) return LZGPU_ERR_ARG;
-	lzd::SliceSolve sv[2];
-	auto ck = std::make_unique<lzd::SliceChecks[]>(2);
-	const uint32_t tail = nb % lay.L;
-	lzd::slice_solve(lay, given, lay.L, sv[0]);
-	lzd::slice_checks(lay, given, sv[0], ck[0], true);
-	if (tail) {
-		lzd::slice_solve(lay, given, tail, sv[1]);
-		lzd::slice_checks(lay, given, sv[1], ck[1], true);
-	}
-	const lzd::SliceChecks &t = tail ? ck[1] : ck[0];
-	out->L = lay.L;
-	out->tail_blocks = tail;
-	out->n_checks = ck[0].n_checks;
-	out->tail_n_checks = t.n_checks;
-	out->checked = ck[0].checked;
-	out->tail_checked = t.checked;
-	out->locatable = ck[0].locatable;
-	out->tail_locatable = t.locatable;
-	const lzd::SliceSolve used[2] = {nb >= lay.L ? sv[0] : sv[1], tail ? sv[1] : sv[0]};
-	const lzd::RsGeometry g = lzd::rs_geometry(lay, given, used, 2, lzd::RsMode::CHECK);
-	out->ok = g.ok ? 1 : 0;
-	out->G = g.G;
-	out->threads = g.threads;
-	out->stages = g.stages;
-	out->smem_bytes = static_cast<uint32_t>(g.smem);
-	return LZGPU_OK;
+	auto sh = std::make_unique<lzd::SliceShapes>();
+	return check_plan(goals, n_slices, nb, given, out, *sh);
 }
 
 int lzgpu_debug_check_slices_rows(const lzgpu_goal *goals, uint32_t n_slices, const uint8_t *given, uint32_t valid, uint32_t *n_checks,
@@ -724,22 +706,11 @@ int lzgpu_debug_check_slices_rows(const lzgpu_goal *goals, uint32_t n_slices, co
 int lzgpu_plan_correct_slices(const lzgpu_goal *goals, uint32_t n_slices, uint32_t nb, const uint8_t *given, lzgpu_slices_correct_plan *out) {
 	if (!out) return LZGPU_ERR_ARG;
 	*out = lzgpu_slices_correct_plan{};
-	int rc = lzgpu_plan_check_slices(goals, n_slices, nb, given, &out->check);
+	auto sh = std::make_unique<lzd::SliceShapes>();
+	const int rc = check_plan(goals, n_slices, nb, given, &out->check, *sh);
 	if (rc) return rc;
-	lzd::SliceLayout lay;
-	const char *why = nullptr;
-	lzd::slice_layout(goals, n_slices, lay, &why);
-	auto sv = std::make_unique<lzd::SliceSolve>();
-	auto ck = std::make_unique<lzd::SliceChecks>();
-	const uint32_t tail = nb % lay.L;
-	lzd::slice_solve(lay, given, lay.L, *sv);
-	lzd::slice_checks(lay, given, *sv, *ck);
-	out->correctable = out->tail_correctable = ck->correctable;
-	if (tail) {
-		lzd::slice_solve(lay, given, tail, *sv);
-		lzd::slice_checks(lay, given, *sv, *ck);
-		out->tail_correctable = ck->correctable;
-	}
+	out->correctable = sh->checks[0].correctable;
+	out->tail_correctable = sh->checks[out->check.tail_blocks ? 1 : 0].correctable;
 	return LZGPU_OK;
 }
 

@@ -415,113 +415,92 @@ extern "C" int lzgpu_pool_decode_stripes(lzgpu_pool *pool, const lzgpu_goal *goa
 	});
 }
 
-// Recovery from the parts of every slice (lzgpu_recover_slices) over the pool: slice i's part and out pointers moved by first *
-// part_stride[i] and first * out_stride[i], its stored and computed CRC arrays by first * pb_i (the layout of the per-context call,
-// lzd::slice_layout), the image by first * chunk_out_stride; the codes and bad[0..3] merged by pool_merged.  With goals, nb or pointer
-// arrays the per-context call refuses, the caller's arrays go through unmoved and every share refuses alike.
+// One share of a multi-slice call: its first chunk, and shift(a, buf, step), the per-flat-part array a with part g moved by first *
+// step[i] for its slice i (step NULL: not moved) in buf, or a itself when a is NULL or the per-context call refuses (not shaped)
+struct SlicesShare {
+	const lzd::SliceLayout &lay;
+	bool shaped;
+	uint32_t first;
+	const size_t *pb;   // blocks per part of each slice
+	size_t n_cs;        // combined stripes per chunk
+	template <class T>
+	T *const *shift(T *const *a, T **buf, const size_t *step) const {
+		if (!shaped || !a) return a;
+		for (uint32_t g = 0; g < lay.n_parts; ++g) buf[g] = a[g] ? a[g] + (step ? first * step[lay.slice_of(g)] : 0) : nullptr;
+		return buf;
+	}
+};
+
+// The multi-slice calls (lzgpu_recover_slices, _salvage_, _check_, _correct_) over the pool: each share gets slice i's part pointers
+// moved by first * part_stride[i] and its stored-CRC arrays by first * pb_i (the flat layout of lzd::slice_layout); call(ctx, share,
+// count, parts, part_crc, bad) moves the call's own arrays.  The codes and bad[0..3] are merged by pool_merged (a hard error, then
+// LZGPU_ERR_CRC, then LZGPU_ERR_INCONSISTENT; bad from the lowest share).  With goals, nb or pointer arrays the per-context call
+// refuses, the caller's arrays go through unmoved and every share refuses alike.
+template <class P, class Call>
+static int pool_slices(lzgpu_pool *pool, const lzgpu_goal *goals, uint32_t n_slices, uint32_t n_chunks, uint32_t nb, P *const *parts,
+                       const size_t *part_stride, const uint32_t *const *part_crc, int64_t *bad, Call &&call) {
+	if (!pool) return LZGPU_ERR_ARG;
+	lzd::SliceLayout lay;
+	const char *why = nullptr;
+	const bool shaped = parts && part_stride && nb >= 1 && nb <= LZGPU_BLOCKS_IN_CHUNK && lzd::slice_layout(goals, n_slices, lay, &why) == LZGPU_OK;
+	size_t pb[lzd::kSlicesMax] = {0};
+	for (uint32_t i = 0; shaped && i < lay.n_slices; ++i) pb[i] = (nb + lay.k[i] - 1) / lay.k[i];
+	const size_t n_cs = shaped ? (nb + lay.L - 1) / lay.L : 0;
+	return pool_merged(pool, n_chunks, bad, 4, [&](lzgpu_ctx *ctx, uint32_t first, uint32_t count, int64_t *b) {
+		const SlicesShare sh{lay, shaped, first, pb, n_cs};
+		P *p[LZGPU_MAX_PARTS];
+		const uint32_t *c[LZGPU_MAX_PARTS];
+		return call(ctx, sh, count, sh.shift(parts, p, part_stride), sh.shift(part_crc, c, pb), b);
+	});
+}
+
+// the image moves by first * chunk_out_stride, the wanted parts by first * out_stride[i] and their CRCs by first * pb_i
 extern "C" int lzgpu_pool_recover_slices(lzgpu_pool *pool, const lzgpu_goal *goals, uint32_t n_slices, uint32_t n_chunks, uint32_t nb,
                                           const uint8_t *const *parts, const size_t *part_stride, const uint32_t *const *part_crc,
                                           const uint8_t *want, uint8_t *const *out, const size_t *out_stride, uint32_t *const *out_crc,
                                           uint8_t *chunk_out, size_t chunk_out_stride, int64_t *bad) {
-	if (!pool) return LZGPU_ERR_ARG;
-	lzd::SliceLayout lay;
-	const char *why = nullptr;
-	const bool shaped = parts && part_stride && nb >= 1 && nb <= LZGPU_BLOCKS_IN_CHUNK && lzd::slice_layout(goals, n_slices, lay, &why) == LZGPU_OK;
-	return pool_merged(pool, n_chunks, bad, 4, [&](lzgpu_ctx *ctx, uint32_t first, uint32_t count, int64_t *b) {
-		const uint8_t *p[LZGPU_MAX_PARTS];
-		const uint32_t *c[LZGPU_MAX_PARTS];
+	return pool_slices(pool, goals, n_slices, n_chunks, nb, parts, part_stride, part_crc, bad,
+	                   [&](lzgpu_ctx *ctx, const SlicesShare &sh, uint32_t count, const uint8_t *const *p, const uint32_t *const *c, int64_t *b) {
 		uint8_t *o[LZGPU_MAX_PARTS];
 		uint32_t *oc[LZGPU_MAX_PARTS];
-		for (uint32_t g = 0; shaped && g < lay.n_parts; ++g) {
-			const int i = lay.slice_of(g);
-			const size_t pb = (nb + lay.k[i] - 1) / lay.k[i];
-			p[g] = parts[g] ? parts[g] + first * part_stride[i] : nullptr;
-			c[g] = part_crc && part_crc[g] ? part_crc[g] + first * pb : nullptr;
-			// without out_stride a wanted part is refused by every share, and an unwanted one is not touched
-			o[g] = out && out[g] ? out[g] + (out_stride ? first * out_stride[i] : 0) : nullptr;
-			oc[g] = out_crc && out_crc[g] ? out_crc[g] + first * pb : nullptr;
-		}
-		return lzgpu_recover_slices(ctx, goals, n_slices, count, nb, shaped ? p : parts, part_stride, shaped && part_crc ? c : part_crc, want,
-		                            shaped && out ? o : out, out_stride, shaped && out_crc ? oc : out_crc,
-		                            chunk_out ? chunk_out + first * chunk_out_stride : nullptr, chunk_out_stride, b);
+		// without out_stride a wanted part is refused by every share, and an unwanted one is not touched
+		return lzgpu_recover_slices(ctx, goals, n_slices, count, nb, p, part_stride, c, want, sh.shift(out, o, out_stride), out_stride,
+		                            sh.shift(out_crc, oc, sh.pb), chunk_out ? chunk_out + sh.first * chunk_out_stride : nullptr,
+		                            chunk_out_stride, b);
 	});
 }
 
-// The salvage of the determined blocks (lzgpu_salvage_slices) over the pool: parts and stored CRCs move as in lzgpu_pool_recover_slices,
-// the image by first * image_stride, its CRCs and the map by first * nb; the codes and bad[0..3] merged by pool_merged.  With goals, nb
-// or pointer arrays the per-context call refuses, the caller's arrays go through unmoved and every share refuses alike.
+// the image moves by first * image_stride, its CRCs and the map by first * nb
 extern "C" int lzgpu_pool_salvage_slices(lzgpu_pool *pool, const lzgpu_goal *goals, uint32_t n_slices, uint32_t n_chunks, uint32_t nb,
                                           const uint8_t *const *parts, const size_t *part_stride, const uint32_t *const *part_crc,
                                           uint8_t *image, size_t image_stride, uint32_t *image_crc, uint8_t *map, int64_t *bad) {
-	if (!pool) return LZGPU_ERR_ARG;
-	lzd::SliceLayout lay;
-	const char *why = nullptr;
-	const bool shaped = parts && part_stride && nb >= 1 && nb <= LZGPU_BLOCKS_IN_CHUNK && lzd::slice_layout(goals, n_slices, lay, &why) == LZGPU_OK;
-	return pool_merged(pool, n_chunks, bad, 4, [&](lzgpu_ctx *ctx, uint32_t first, uint32_t count, int64_t *b) {
-		const uint8_t *p[LZGPU_MAX_PARTS];
-		const uint32_t *c[LZGPU_MAX_PARTS];
-		for (uint32_t g = 0; shaped && g < lay.n_parts; ++g) {
-			const int i = lay.slice_of(g);
-			const size_t pb = (nb + lay.k[i] - 1) / lay.k[i];
-			p[g] = parts[g] ? parts[g] + first * part_stride[i] : nullptr;
-			c[g] = part_crc && part_crc[g] ? part_crc[g] + first * pb : nullptr;
-		}
-		const size_t at = static_cast<size_t>(first) * nb;
-		return lzgpu_salvage_slices(ctx, goals, n_slices, count, nb, shaped ? p : parts, part_stride, shaped && part_crc ? c : part_crc,
-		                            image ? image + first * image_stride : nullptr, image_stride, image_crc ? image_crc + at : nullptr,
-		                            map ? map + at : nullptr, b);
+	return pool_slices(pool, goals, n_slices, n_chunks, nb, parts, part_stride, part_crc, bad,
+	                   [&](lzgpu_ctx *ctx, const SlicesShare &sh, uint32_t count, const uint8_t *const *p, const uint32_t *const *c, int64_t *b) {
+		const size_t at = static_cast<size_t>(sh.first) * nb;
+		return lzgpu_salvage_slices(ctx, goals, n_slices, count, nb, p, part_stride, c, image ? image + sh.first * image_stride : nullptr,
+		                            image_stride, image_crc ? image_crc + at : nullptr, map ? map + at : nullptr, b);
 	});
 }
 
-// The consistency map of several slices (lzgpu_check_slices) over the pool: parts and stored CRCs move as in
-// lzgpu_pool_salvage_slices, the map by first * n_cs; the codes and bad[0..3] merged by pool_merged (a hard error, then LZGPU_ERR_CRC,
-// then LZGPU_ERR_INCONSISTENT; bad from the lowest share).  With goals, nb or pointer arrays the per-context call refuses, the
-// caller's arrays go through unmoved and every share refuses alike.
+// the map moves by first * n_cs
 extern "C" int lzgpu_pool_check_slices(lzgpu_pool *pool, const lzgpu_goal *goals, uint32_t n_slices, uint32_t n_chunks, uint32_t nb,
                                         const uint8_t *const *parts, const size_t *part_stride, const uint32_t *const *part_crc,
                                         lzgpu_slices_check *map, int64_t *bad) {
-	if (!pool) return LZGPU_ERR_ARG;
-	lzd::SliceLayout lay;
-	const char *why = nullptr;
-	const bool shaped = parts && part_stride && nb >= 1 && nb <= LZGPU_BLOCKS_IN_CHUNK && lzd::slice_layout(goals, n_slices, lay, &why) == LZGPU_OK;
-	const size_t n_cs = shaped ? (nb + lay.L - 1) / lay.L : 0;
-	return pool_merged(pool, n_chunks, bad, 4, [&](lzgpu_ctx *ctx, uint32_t first, uint32_t count, int64_t *b) {
-		const uint8_t *p[LZGPU_MAX_PARTS];
-		const uint32_t *c[LZGPU_MAX_PARTS];
-		for (uint32_t g = 0; shaped && g < lay.n_parts; ++g) {
-			const int i = lay.slice_of(g);
-			const size_t pb = (nb + lay.k[i] - 1) / lay.k[i];
-			p[g] = parts[g] ? parts[g] + first * part_stride[i] : nullptr;
-			c[g] = part_crc && part_crc[g] ? part_crc[g] + first * pb : nullptr;
-		}
-		return lzgpu_check_slices(ctx, goals, n_slices, count, nb, shaped ? p : parts, part_stride, shaped && part_crc ? c : part_crc,
-		                          map && shaped ? map + first * n_cs : map, b);
+	return pool_slices(pool, goals, n_slices, n_chunks, nb, parts, part_stride, part_crc, bad,
+	                   [&](lzgpu_ctx *ctx, const SlicesShare &sh, uint32_t count, const uint8_t *const *p, const uint32_t *const *c, int64_t *b) {
+		return lzgpu_check_slices(ctx, goals, n_slices, count, nb, p, part_stride, c, map && sh.shaped ? map + sh.first * sh.n_cs : map, b);
 	});
 }
 
-// The correction of several slices (lzgpu_correct_slices) over the pool: parts, stored and new CRCs move by slice, the fix entries by
-// first * n_cs; the codes and bad[0..3] merged by pool_merged, as lzgpu_pool_check_slices.
+// the new CRCs move by first * pb_i, the fix entries by first * n_cs
 extern "C" int lzgpu_pool_correct_slices(lzgpu_pool *pool, const lzgpu_goal *goals, uint32_t n_slices, uint32_t n_chunks, uint32_t nb,
                                           uint8_t *const *parts, const size_t *part_stride, const uint32_t *const *part_crc,
                                           uint32_t *const *new_crc, lzgpu_slices_fix *fix, int64_t *bad) {
-	if (!pool) return LZGPU_ERR_ARG;
-	lzd::SliceLayout lay;
-	const char *why = nullptr;
-	const bool shaped = parts && part_stride && nb >= 1 && nb <= LZGPU_BLOCKS_IN_CHUNK && lzd::slice_layout(goals, n_slices, lay, &why) == LZGPU_OK;
-	const size_t n_cs = shaped ? (nb + lay.L - 1) / lay.L : 0;
-	return pool_merged(pool, n_chunks, bad, 4, [&](lzgpu_ctx *ctx, uint32_t first, uint32_t count, int64_t *b) {
-		uint8_t *p[LZGPU_MAX_PARTS];
-		const uint32_t *c[LZGPU_MAX_PARTS];
+	return pool_slices(pool, goals, n_slices, n_chunks, nb, parts, part_stride, part_crc, bad,
+	                   [&](lzgpu_ctx *ctx, const SlicesShare &sh, uint32_t count, uint8_t *const *p, const uint32_t *const *c, int64_t *b) {
 		uint32_t *nc[LZGPU_MAX_PARTS];
-		for (uint32_t g = 0; shaped && g < lay.n_parts; ++g) {
-			const int i = lay.slice_of(g);
-			const size_t pb = (nb + lay.k[i] - 1) / lay.k[i];
-			p[g] = parts[g] ? parts[g] + first * part_stride[i] : nullptr;
-			c[g] = part_crc && part_crc[g] ? part_crc[g] + first * pb : nullptr;
-			nc[g] = new_crc && new_crc[g] ? new_crc[g] + first * pb : nullptr;
-		}
-		return lzgpu_correct_slices(ctx, goals, n_slices, count, nb, shaped ? p : parts, part_stride, shaped && part_crc ? c : part_crc,
-		                            shaped && new_crc ? nc : new_crc, fix && shaped ? fix + first * n_cs : fix, b);
+		return lzgpu_correct_slices(ctx, goals, n_slices, count, nb, p, part_stride, c, sh.shift(new_crc, nc, sh.pb),
+		                            fix && sh.shaped ? fix + sh.first * sh.n_cs : fix, b);
 	});
 }
 

@@ -272,4 +272,24 @@ inline void slice_checks(const SliceLayout &lay, const uint8_t *given, const Sli
 	}
 }
 
+// The stripe shapes of a batch of nb blocks per chunk, for a call of `mode` and for its plan: the solve of a full combined stripe
+// (shapes[0]) and of the chunk's last one when L does not divide nb (shapes[1]); for CHECK and CORRECT the checks of each shape a chunk
+// has; and the launch geometry of those shapes.  plan: what the lzgpu_plan_*_slices report beyond what the call needs: the full shape's
+// checks even when nb < L, and the locatable masks.
+struct SliceShapes {
+	SliceSolve shapes[2];
+	SliceChecks checks[2];
+	RsGeometry geo;
+};
+
+inline void slice_shapes(const SliceLayout &lay, const uint8_t *given, uint32_t nb, RsMode mode, SliceShapes &o, bool plan = false) {
+	const uint32_t tail = nb % lay.L;
+	slice_solve(lay, given, lay.L, o.shapes[0]);
+	if (tail) slice_solve(lay, given, tail, o.shapes[1]);
+	for (int t = 0; t < 2 && (mode == RsMode::CHECK || mode == RsMode::CORRECT); ++t)
+		if (t == 0 ? plan || nb >= lay.L : tail != 0) slice_checks(lay, given, o.shapes[t], o.checks[t], plan);
+	const SliceSolve used[2] = {nb >= lay.L ? o.shapes[0] : o.shapes[1], tail ? o.shapes[1] : o.shapes[0]};
+	o.geo = rs_geometry(lay, given, used, 2, mode);
+}
+
 }  // namespace lzd

@@ -177,39 +177,50 @@ def _convert_chunks(fn, h, src, dst, nb, parts, want, part_crc, with_crc):
     return out, ocrc
 
 
-def _recover_slices(fn, h, goals, nb, parts, part_crc, want, chunk_image, with_crc):
-    ns = len(goals)
+def _n_flat(goals):
+    """the flat parts of a multi-slice goal: slice i's k + m parts after those of the slices before it, one for the standard slice"""
+    return sum(1 if g.is_std else g.k + g.m for g in goals)
+
+
+def _slices_host(goals, nb, parts, part_crc, in_place=False):
+    """The shared preamble of the multi-slice host-pointer calls.  parts: one entry per flat part, each None or [n_chunks, pb_i *
+    64 KiB] uint8 (in_place: the call corrects them, so each must already be a writeable C-contiguous uint8 array).  Returns (parts,
+    n_chunks, C array of the stored-CRC pointers or None, C array of the part strides per slice, pb per flat part, L); n_chunks is 0
+    when no part is given, for the library to refuse the call."""
     pbs = [-(-nb // g.k) for g in goals]
-    slice_of = [i for i, g in enumerate(goals) for _ in range(1 if g.is_std else g.k + g.m)]
-    assert len(parts) == len(slice_of)
-    arrs = [None if p is None else _u8(p).reshape(-1, pbs[slice_of[j]] * BLOCK_SIZE) for j, p in enumerate(parts)]
-    n = next(a.shape[0] for a in arrs if a is not None)
+    pb = [pbs[i] for i, g in enumerate(goals) for _ in range(1 if g.is_std else g.k + g.m)]
+    assert len(parts) == len(pb)
+    if in_place:
+        for p in parts:
+            if p is not None and not (isinstance(p, np.ndarray) and p.dtype == np.uint8 and p.flags.c_contiguous and p.flags.writeable):
+                raise ValueError("correct_slices corrects the parts in place: each must be a writeable C-contiguous uint8 array")
+    arrs = [None if p is None else (p if in_place else _u8(p)).reshape(-1, pb[j] * BLOCK_SIZE) for j, p in enumerate(parts)]
+    n = next((a.shape[0] for a in arrs if a is not None), 0)
     crcs = None if part_crc is None else _ptr_array([None if c is None else np.ascontiguousarray(c, dtype=np.uint32) for c in part_crc])
+    strides = (C.c_size_t * len(goals))(*[p * BLOCK_SIZE for p in pbs])
+    return arrs, n, crcs, strides, pb, math.lcm(*[g.k for g in goals if not g.is_std])
+
+
+def _recover_slices(fn, h, goals, nb, parts, part_crc, want, chunk_image, with_crc):
+    arrs, n, crcs, strides, pb, _ = _slices_host(goals, nb, parts, part_crc)
     if want is None:
         want = [1 if a is None else 0 for a in arrs]
     w = np.asarray(want, dtype=np.uint8)
-    out = [np.zeros((n, pbs[slice_of[j]] * BLOCK_SIZE), dtype=np.uint8) if w[j] else None for j in range(len(arrs))]
-    ocrc = [np.zeros((n, pbs[slice_of[j]]), dtype=np.uint32) if (w[j] and with_crc) else None for j in range(len(arrs))]
+    out = [np.zeros((n, pb[j] * BLOCK_SIZE), dtype=np.uint8) if w[j] else None for j in range(len(arrs))]
+    ocrc = [np.zeros((n, pb[j]), dtype=np.uint32) if (w[j] and with_crc) else None for j in range(len(arrs))]
     img = np.zeros((n, nb * BLOCK_SIZE), dtype=np.uint8) if chunk_image else None
-    strides = (C.c_size_t * ns)(*[pb * BLOCK_SIZE for pb in pbs])
     bad = (C.c_int64 * 4)(-1, -1, -1, -1)
-    rc = fn(h, _goal_array(goals), ns, n, nb, _ptr_array(arrs), strides, crcs, _p(w), _ptr_array(out), strides,
+    rc = fn(h, _goal_array(goals), len(goals), n, nb, _ptr_array(arrs), strides, crcs, _p(w), _ptr_array(out), strides,
             _ptr_array(ocrc) if with_crc else None, _p(img), nb * BLOCK_SIZE, bad)
     _check_crc(rc, _name(fn), bad)
     return out, ocrc, img
 
 
 def _salvage_slices(fn, h, goals, nb, parts, part_crc, with_crc):
-    pbs = [-(-nb // g.k) for g in goals]
-    slice_of = [i for i, g in enumerate(goals) for _ in range(1 if g.is_std else g.k + g.m)]
-    assert len(parts) == len(slice_of)
-    arrs = [None if p is None else _u8(p).reshape(-1, pbs[slice_of[j]] * BLOCK_SIZE) for j, p in enumerate(parts)]
-    n = next((a.shape[0] for a in arrs if a is not None), 0)
-    crcs = None if part_crc is None else _ptr_array([None if c is None else np.ascontiguousarray(c, dtype=np.uint32) for c in part_crc])
+    arrs, n, crcs, strides, _, _ = _slices_host(goals, nb, parts, part_crc)
     img = np.zeros((n, nb * BLOCK_SIZE), dtype=np.uint8)
     icrc = np.zeros((n, nb), dtype=np.uint32) if with_crc else None
     smap = np.zeros((n, nb), dtype=np.uint8)
-    strides = (C.c_size_t * len(goals))(*[pb * BLOCK_SIZE for pb in pbs])
     bad = (C.c_int64 * 4)(-1, -1, -1, -1)
     rc = fn(h, _goal_array(goals), len(goals), n, nb, _ptr_array(arrs), strides, crcs, _p(img), nb * BLOCK_SIZE, _p(icrc), _p(smap), bad)
     _check_crc(rc, _name(fn), bad, image=img, image_crc=icrc, map=smap)
@@ -220,18 +231,8 @@ SLICES_CHECK_DTYPE = np.dtype([("bad_checks", np.uint64), ("suspect_part", np.in
 
 
 def _check_slices(fn, h, goals, nb, parts, part_crc):
-    pbs = [-(-nb // g.k) for g in goals]
-    slice_of = [i for i, g in enumerate(goals) for _ in range(1 if g.is_std else g.k + g.m)]
-    assert len(parts) == len(slice_of)
-    arrs = [None if p is None else _u8(p).reshape(-1, pbs[slice_of[j]] * BLOCK_SIZE) for j, p in enumerate(parts)]
-    n = next((a.shape[0] for a in arrs if a is not None), 0)
-    crcs = None if part_crc is None else _ptr_array([None if c is None else np.ascontiguousarray(c, dtype=np.uint32) for c in part_crc])
-    L = 1
-    for g in goals:
-        if not g.is_std:
-            L = L * g.k // math.gcd(L, g.k)
+    arrs, n, crcs, strides, _, L = _slices_host(goals, nb, parts, part_crc)
     out = np.zeros((n, -(-nb // L)), dtype=SLICES_CHECK_DTYPE)
-    strides = (C.c_size_t * len(goals))(*[pb * BLOCK_SIZE for pb in pbs])
     bad = (C.c_int64 * 4)(-1, -1, -1, -1)
     rc = fn(h, _goal_array(goals), len(goals), n, nb, _ptr_array(arrs), strides, crcs, _p(out), bad)
     _check_crc(rc, _name(fn), bad, map=out)
@@ -243,22 +244,9 @@ SLICES_FIX_DTYPE = np.dtype([("bad_checks", np.uint64), ("suspect_part", np.int3
 
 
 def _correct_slices(fn, h, goals, nb, parts, part_crc, with_crc):
-    pbs = [-(-nb // g.k) for g in goals]
-    slice_of = [i for i, g in enumerate(goals) for _ in range(1 if g.is_std else g.k + g.m)]
-    assert len(parts) == len(slice_of)
-    for p in parts:
-        if p is not None and not (isinstance(p, np.ndarray) and p.dtype == np.uint8 and p.flags.c_contiguous and p.flags.writeable):
-            raise ValueError("correct_slices corrects the parts in place: each must be a writeable C-contiguous uint8 array")
-    arrs = [None if p is None else p.reshape(-1, pbs[slice_of[j]] * BLOCK_SIZE) for j, p in enumerate(parts)]
-    n = next((a.shape[0] for a in arrs if a is not None), 0)
-    crcs = None if part_crc is None else _ptr_array([None if c is None else np.ascontiguousarray(c, dtype=np.uint32) for c in part_crc])
-    new_crc = [np.zeros((n, pbs[slice_of[j]]), dtype=np.uint32) if (a is not None and with_crc) else None for j, a in enumerate(arrs)]
-    L = 1
-    for g in goals:
-        if not g.is_std:
-            L = L * g.k // math.gcd(L, g.k)
+    arrs, n, crcs, strides, pb, L = _slices_host(goals, nb, parts, part_crc, in_place=True)
+    new_crc = [np.zeros((n, pb[j]), dtype=np.uint32) if (a is not None and with_crc) else None for j, a in enumerate(arrs)]
     fix = np.zeros((n, -(-nb // L)), dtype=SLICES_FIX_DTYPE)
-    strides = (C.c_size_t * len(goals))(*[pb * BLOCK_SIZE for pb in pbs])
     bad = (C.c_int64 * 4)(-1, -1, -1, -1)
     rc = fn(h, _goal_array(goals), len(goals), n, nb, _ptr_array(arrs), strides, crcs, _ptr_array(new_crc) if with_crc else None, _p(fix),
             bad)
@@ -759,17 +747,22 @@ class Engine:
         write is not determined, ChunkCrcError (.where = chunk, slice, part, block) on a stored-CRC mismatch."""
         return _recover_slices(self.lib.lzgpu_recover_slices, self.h, goals, nb, parts, part_crc, want, chunk_image, with_crc)
 
+    def _slices_dev(self, fn, goals, n_chunks, nb, d_parts, part_stride, d_part_crc, stream, *own):
+        # the multi-slice device-pointer calls: goals, the flat parts with their stored CRCs and part_stride per slice, then the
+        # call's own arguments
+        ns, n = len(goals), _n_flat(goals)
+        bad = (C.c_int64 * 4)(-1, -1, -1, -1)
+        rc = fn(self.h, _goal_array(goals), ns, n_chunks, nb, _dev_ptrs(d_parts, n), (C.c_size_t * ns)(*part_stride), _dev_ptrs(d_part_crc, n),
+                *own, bad, stream)
+        _check_crc(rc, _name(fn), bad)
+
     def recover_slices_dev(self, goals, n_chunks, nb, d_parts, part_stride, d_part_crc, want, d_out, out_stride, d_out_crc=None,
                            d_chunk_out=None, chunk_out_stride=0, stream=None):
         """lzgpu_recover_slices_dev: d_parts / d_part_crc / d_out / d_out_crc are lists over the flat parts (device pointers as ints,
         0 or None = absent), part_stride / out_stride one entry per slice.  Raises ChunkCrcError (.where = chunk, slice, part, block)."""
-        ns, n = len(goals), len(want)
-        w = np.asarray(want, dtype=np.uint8)
-        bad = (C.c_int64 * 4)(-1, -1, -1, -1)
-        rc = self.lib.lzgpu_recover_slices_dev(self.h, _goal_array(goals), ns, n_chunks, nb, _dev_ptrs(d_parts, n), (C.c_size_t * ns)(*part_stride),
-                                               _dev_ptrs(d_part_crc, n), _p(w), _dev_ptrs(d_out, n), (C.c_size_t * ns)(*out_stride),
-                                               _dev_ptrs(d_out_crc, n), d_chunk_out, chunk_out_stride, bad, stream)
-        _check_crc(rc, "recover_slices_dev", bad)
+        n, w = _n_flat(goals), np.asarray(want, dtype=np.uint8)
+        self._slices_dev(self.lib.lzgpu_recover_slices_dev, goals, n_chunks, nb, d_parts, part_stride, d_part_crc, stream, _p(w),
+                         _dev_ptrs(d_out, n), (C.c_size_t * len(goals))(*out_stride), _dev_ptrs(d_out_crc, n), d_chunk_out, chunk_out_stride)
 
     def salvage_slices(self, goals, nb, parts, part_crc=None, with_crc=True):
         """Salvage the blocks of lost chunks of a multi-slice goal that the given parts of every slice still determine
@@ -784,11 +777,8 @@ class Engine:
         """lzgpu_salvage_slices_dev: d_parts / d_part_crc are lists over the flat parts (device pointers as ints, 0 or None = absent),
         part_stride one entry per slice; d_image_crc may be None.  Raises ChunkCrcError (.where = chunk, slice, part, block); the device
         results are then still complete."""
-        ns, n = len(goals), sum(1 if g.is_std else g.k + g.m for g in goals)
-        bad = (C.c_int64 * 4)(-1, -1, -1, -1)
-        rc = self.lib.lzgpu_salvage_slices_dev(self.h, _goal_array(goals), ns, n_chunks, nb, _dev_ptrs(d_parts, n), (C.c_size_t * ns)(*part_stride),
-                                               _dev_ptrs(d_part_crc, n), d_image, image_stride, d_image_crc, d_map, bad, stream)
-        _check_crc(rc, "salvage_slices_dev", bad)
+        self._slices_dev(self.lib.lzgpu_salvage_slices_dev, goals, n_chunks, nb, d_parts, part_stride, d_part_crc, stream, d_image,
+                         image_stride, d_image_crc, d_map)
 
     SLICES_CHECK_DTYPE = SLICES_CHECK_DTYPE
 
@@ -803,11 +793,7 @@ class Engine:
         """lzgpu_check_slices_dev: d_parts / d_part_crc are lists over the flat parts (device pointers as ints, 0 or None = absent),
         part_stride one entry per slice; n_chunks * ceil(nb / L) entries of 16 bytes go to d_map (8-byte aligned device memory).
         Raises ChunkCrcError (.where = chunk, slice, part, block); the map is then still complete."""
-        ns, n = len(goals), sum(1 if g.is_std else g.k + g.m for g in goals)
-        bad = (C.c_int64 * 4)(-1, -1, -1, -1)
-        rc = self.lib.lzgpu_check_slices_dev(self.h, _goal_array(goals), ns, n_chunks, nb, _dev_ptrs(d_parts, n), (C.c_size_t * ns)(*part_stride),
-                                             _dev_ptrs(d_part_crc, n), d_map, bad, stream)
-        _check_crc(rc, "check_slices_dev", bad)
+        self._slices_dev(self.lib.lzgpu_check_slices_dev, goals, n_chunks, nb, d_parts, part_stride, d_part_crc, stream, d_map)
 
     SLICES_FIX_DTYPE = SLICES_FIX_DTYPE
 
@@ -826,12 +812,8 @@ class Engine:
         """lzgpu_correct_slices_dev: d_parts / d_part_crc / d_new_crc are lists over the flat parts (device pointers as ints, 0 or
         None = absent; d_new_crc may be None), part_stride one entry per slice; n_chunks * ceil(nb / L) entries of 32 bytes go to d_fix
         (8-byte aligned device memory).  Raises ChunkCrcError (.where = chunk, slice, part, block); the entries are then still complete."""
-        ns, n = len(goals), sum(1 if g.is_std else g.k + g.m for g in goals)
-        bad = (C.c_int64 * 4)(-1, -1, -1, -1)
-        rc = self.lib.lzgpu_correct_slices_dev(self.h, _goal_array(goals), ns, n_chunks, nb, _dev_ptrs(d_parts, n),
-                                               (C.c_size_t * ns)(*part_stride), _dev_ptrs(d_part_crc, n), _dev_ptrs(d_new_crc, n), d_fix, bad,
-                                               stream)
-        _check_crc(rc, "correct_slices_dev", bad)
+        self._slices_dev(self.lib.lzgpu_correct_slices_dev, goals, n_chunks, nb, d_parts, part_stride, d_part_crc, stream,
+                         _dev_ptrs(d_new_crc, _n_flat(goals)), d_fix)
 
     @staticmethod
     def plan_correct_slices(goals, nb, given):

@@ -271,6 +271,10 @@ def test_refusals_write_nothing(eng, pools, kind, n):
         assert rc == code and bad == [-7] * 4, (rc, bad)
         assert all((o == SENT).all() for o in outs if o is not None) and (img == SENT).all()
         assert all((c == SENT_CRC).all() for c in ocrc if c is not None)
+        if kind == "too_few_parts":
+            with pytest.raises(L.LzGpuError) as ex:   # no part given at all: every share refuses it
+                pool.recover_slices(b.goals, nb, [None] * len(given))
+            assert ex.value.status == _lib.ERR_TOO_FEW_PARTS
 
 
 @gpu

@@ -227,6 +227,9 @@ def test_undetermined_patterns_refuse_and_write_nothing(names):
     with pytest.raises(LzGpuError) as ex:
         e.recover_slices(goals, nb, [p if given[g] else None for g, p in enumerate(parts)])
     assert ex.value.status == _lib.ERR_TOO_FEW_PARTS
+    with pytest.raises(LzGpuError) as ex:   # no part given at all: the library refuses it
+        e.recover_slices(goals, nb, [None] * n)
+    assert ex.value.status == _lib.ERR_TOO_FEW_PARTS
 
 
 @pytest.mark.parametrize("ctx", ["default", "cap2"])
