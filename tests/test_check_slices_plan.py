@@ -70,8 +70,8 @@ def shapes(goals):
     return [(full, L, L), (full - 1, L, (full - 1) % L)] if L > 1 else [(full, L, L)]
 
 
-def masks_model(goals, given, valid):
-    """(checked, locatable) from the codewords supported on sets of blocks"""
+def masks_model(goals, given, valid, rank=rank):
+    """(checked, locatable) from the codewords supported on sets of blocks (rank: the GF(2^8) rank used, the plain one by default)"""
     blocks = given_blocks(goals, given, valid)
     L = lcm_of(goals)
     A = [r for _, _, r in blocks]

@@ -160,6 +160,35 @@ fcrc = [eng.crc_blocks(p.reshape(-1)).reshape(2, -1) for p in full]
 fix, ncrc = eng.correct_slices(goals, nblk, full, fcrc)
 assert (fix["status"] == 1).sum() == 1 and all((a == b).all() for a, b in zip(full, sparts))
 assert ncrc[6][0, 4] == eng.crc_blocks(sparts[6][0, 4 * 65536:5 * 65536])[0]
+# the same at the limits of the tables (tests/test_slices_check_edges.py): A, ec(8,8) + ec(16,32) with all 64 parts, 64 checks, a
+# stale flat part 63 in combined stripe 1; C, std + ec(31,1) + ec(2,1) with ec(2,1) lost, L = 62, the whole std copy of stripe 1
+# stale: a 62-block correction in correct_slices_kernel's largest shared memory
+for names, given, nblk, stale in [(("ec(8,8)", "ec(16,32)"), [1] * 64, 32, (63, [1])),
+                                  (("std", "ec(31,1)", "ec(2,1)"), [1] * 33 + [0] * 3, 124, (0, list(range(62, 124))))]:
+    goals = [L.SliceType(2, 1, 0) if x == "std" else L.SliceType(x) for x in names]
+    data = np.stack([O.fill_chunk(o, nblk * 65536, 37, 0)])
+    enc = eng.encode_slices(goals, data)
+    eparts = []
+    for g, (par, crc) in zip(goals, enc):
+        if g.is_std:
+            eparts.append(data.copy())
+            continue
+        pb = -(-nblk // g.k)
+        padded = np.zeros((1, pb * g.k * 65536), dtype=np.uint8)
+        padded[:, :nblk * 65536] = data
+        eparts += [np.ascontiguousarray(padded.reshape(1, pb, g.k, 65536)[:, :, j]).reshape(1, -1) for j in range(g.k)]
+        eparts += [np.ascontiguousarray(par[:, r]) for r in range(g.m)]
+    part, blks = stale
+    bad = [p.copy() for p in eparts]
+    for b in blks:
+        bad[part][0, b * 65536 + 77] ^= 0x3C
+    inp = [p if x else None for p, x in zip(bad, given)]
+    bcrc = [eng.crc_blocks(p.reshape(-1)).reshape(1, -1) if x else None for p, x in zip(bad, given)]
+    m = eng.check_slices(goals, nblk, inp, bcrc)
+    assert m[0, 1]["suspect_part"] == part and m[0, 1]["bad_checks"] != 0
+    fix, _ = eng.correct_slices(goals, nblk, inp, bcrc)
+    assert fix[0, 1]["status"] == 1 and bin(int(fix[0, 1]["changed"])).count("1") == len(blks)
+    assert all(a is None or (a == b).all() for a, b in zip(inp, eparts))
 print("sanitizer case OK")
 PY
 for tool in ${TOOLS:-memcheck racecheck synccheck}; do
