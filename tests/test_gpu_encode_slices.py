@@ -148,6 +148,7 @@ def test_every_planned_geometry(entry, ctx):
         par_stride.append(0 if g.is_std else par.shape[1])
         crc_ptr.append(crc.data_ptr())
         crc_stride.append(crc.shape[1])
+    torch.cuda.synchronize()        # the fills and copies above run on torch's stream; the call runs on the context's own stream
     eng.encode_slices_dev(goals, n, nb * BLOCK, d_data.data_ptr(), nb * BLOCK, par_ptr, par_stride, crc_ptr, crc_stride)
     torch.cuda.synchronize()
     geo = eng.last_geometry()
@@ -186,6 +187,7 @@ def test_dev_form_at_padded_strides_with_guard_bytes():
         par_stride.append(ps)
         crc_ptr.append(cbuf.data_ptr() + OFF)
         crc_stride.append(cs)
+    torch.cuda.synchronize()
     eng.encode_slices_dev(goals, n, chunk_len, dbuf.data_ptr() + OFF, dstride, par_ptr, par_stride, crc_ptr, crc_stride)
     torch.cuda.synchronize()
     want = per_slice(eng, goals, data, chunk_len)

@@ -189,6 +189,17 @@ for names, given, nblk, stale in [(("ec(8,8)", "ec(16,32)"), [1] * 64, 32, (63, 
     fix, _ = eng.correct_slices(goals, nblk, inp, bcrc)
     assert fix[0, 1]["status"] == 1 and bin(int(fix[0, 1]["changed"])).count("1") == len(blks)
     assert all(a is None or (a == b).all() for a, b in zip(inp, eparts))
+# the one-pass encode of several slices at the limits of its tables (tests/test_encode_slices_edges.py): A, xor2 x 3 + ec(2,3) with
+# 128 stripes per unit, 16 GF items per thread and 512 CRC streams; F, ec(2,4) + ec(21,3) with the shared memory 392 bytes under the
+# cap; two chunks each, the last unit partial and the last block short
+for names, nblk in [(("xor2", "xor2", "xor2", "ec(2,3)"), 67), (("ec(2,4)", "ec(21,3)"), 43)]:
+    goals = [L.SliceType(x) for x in names]
+    data = np.stack([O.fill_chunk(o, nblk * 65536 - 999, 41, c) for c in range(2)])
+    enc = eng.encode_slices(goals, data)
+    for g, (par, crc) in zip(goals, enc):
+        for c in range(2):
+            p_ref, c_ref = o.encode_chunk(g.kind, g.k, g.m, data[c])
+            assert (par[c] == p_ref).all() and (crc[c] == c_ref).all(), names
 print("sanitizer case OK")
 PY
 for tool in ${TOOLS:-memcheck racecheck synccheck}; do
